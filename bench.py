@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- keyframe-window optimize() throughput (BASELINE.json metric) on N B200s.
+"""bench.py -- keyframe-window optimize() throughput (BASELINE.json metric) on N H100s.
 
 A "step" = one pass of the hot path over one batch: Estimator::optimize(10 iterations) on every
 resident 10-keyframe / 2000-landmark stereo window (BASELINE.json configs[1]; synthetic, seeded).
@@ -11,6 +11,7 @@ resident 10-keyframe / 2000-landmark stereo window (BASELINE.json configs[1]; sy
 `--impl reference` times the CPU oracle (the restated okvis_ceres path; the real reference cannot be
 built here) on the box's host cores on the same workload.
 Windows shard across ranks with no data-path collective (independent windows): weak scaling.
+`--dump-outputs DIR` writes what the last timed step computed (summaries and downloaded estimates) as .npy files.
 """
 import argparse
 import json
@@ -27,14 +28,32 @@ sys.path.insert(0, ROOT)
 
 METRIC = "keyframe-window optimize() iters/sec (10KF/2k-lm stereo)"
 ITERS = 10
+DUMP_LIMIT_BYTES = 64 << 20        # --dump-outputs writes at most this much
 
 
-def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return float(d["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+# NVIDIA data-sheet peaks of the H100 variants (checked in this order against the device name): HBM GB/s and FP64
+# GFLOP/s without tensor cores (DFMA -- k_linearize, k_lmblock and k_schur issue no DMMA).  Not measured.
+DATA_SHEET_PEAKS = (("H100 NVL", "H100 NVL", 3900.0, 30000.0), ("H100 PCIe", "H100 PCIe", 2000.0, 26000.0),
+                    ("H100", "H100 SXM", 3350.0, 34000.0))
+
+
+def data_sheet_peaks(device_name):
+    """(HBM GB/s, FP64 DFMA GFLOP/s, source) for the card; (None, None, reason) for a card the table does not list."""
+    for key, variant, hbm, fp64 in DATA_SHEET_PEAKS:
+        if key in device_name:
+            return hbm, fp64, "NVIDIA %s data sheet" % variant
+    return None, None, "no data-sheet peak listed for %s" % device_name
+
+
+def gpu_identity(gpu_index):
+    """Name and power limit of the GPU the numbers were measured on (nvidia-smi, read only)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(gpu_index), "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=10).stdout.strip()
+        name, power, sm_max = [x.strip() for x in out.split(",")]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(sm_max)}
+    except Exception:
+        return None
 
 
 class ClockSampler(threading.Thread):
@@ -71,18 +90,11 @@ class ClockSampler(threading.Thread):
         return {"sm_mhz": float(np.median(self.sm)), "sm_max_mhz": float(max(self.sm_max)), "reasons": sorted(self.reasons)}
 
 
-def fp64_roofline(achieved_gflops):
-    """The Jacobian / J^T J / Schur group against the FP64 peak (the bound that really applies: ~50 FLOP per byte).  The
-    driver's MEASURED_PEAKS.json has no FP64 figure; the peak is this project's own measurement (tools/fp64_peak.cu,
-    DFMA and DMMA both 37 TFLOP/s on this B200), committed under profiles/."""
-    path = os.path.join(ROOT, "profiles", "r01_fp64_peak.json")
-    try:
-        pk = json.load(open(path))
-        peak = 1e3 * float(max(pk["fp64_fma_tflops"], pk["fp64_dmma_tflops"]))
-        src = "profiles/r01_fp64_peak.json (tools/fp64_peak.cu)"
-    except Exception:
-        peak, src = 37000.0, "fallback 37 TFLOP/s"
-    return {"bound": "fp64", "achieved": achieved_gflops, "peak": peak, "unit": "GFLOP/s", "frac": achieved_gflops / peak,
+def fp64_roofline(achieved_gflops, peak, src):
+    """The Jacobian / J^T J / Schur group against the FP64 peak (~50 FLOP per byte: FP64 bounds it before HBM does).
+    The peak is the data sheet's FP64 rate without tensor cores, because these kernels issue DFMA only."""
+    return {"bound": "fp64", "achieved": achieved_gflops, "peak": peak, "unit": "GFLOP/s",
+            "frac": achieved_gflops / peak if peak else None,
             "flops": "SURVEY 8d model: 1500 N_obs + 324 sum f_l^2 + d^3/3 + 14000 (K-1) per window-iteration", "peak_source": src}
 
 
@@ -377,6 +389,25 @@ def cfg5_leg(torch, dist, dev, rank, world, local_rank, reps=5):
         c5.close()
 
 
+def dump_outputs(out_dir, ctx, B, summaries):
+    """What the last timed step handed its caller: the okb_optimize summaries and the estimates okb_window_download_batch
+    returns (poses, speed/bias, landmarks, landmark quality), stacked over the windows, float64.  Above 64 MB a fixed,
+    seeded sample of windows is written (window_index says which)."""
+    outs = ctx.download_batch(0, B)
+    per_window = sum(v.nbytes for v in outs[0].values()) + 8 * 8
+    idx = np.arange(B)
+    if B * per_window > DUMP_LIMIT_BYTES:
+        idx = np.sort(np.random.default_rng(0).choice(B, DUMP_LIMIT_BYTES // per_window, replace=False))
+    arrays = {"window_index": idx.astype(np.float64)}
+    for k in ("initial_cost", "final_cost", "iterations", "num_successful_steps", "termination", "imu_redo_count", "final_radius"):
+        arrays[k] = np.array([summaries[i][k] for i in idx], np.float64)
+    for k in ("poses", "speed_bias", "landmarks", "quality"):
+        arrays[k] = np.stack([outs[i][k] for i in idx]).astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
+
+
 def run_b200(args):
     import torch
     from okvis_b200 import capi
@@ -423,9 +454,12 @@ def run_b200(args):
     with torch.cuda.stream(stream):
         ev0.record(stream)
         for _ in range(args.steps):
-            iters += sum(s["iterations"] for s in step())
+            last = step()
+            iters += sum(s["iterations"] for s in last)
         ev1.record(stream)
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ctx, B, last)
     elapsed_ms = ev0.elapsed_time(ev1)
     prof = ctx.profile_read()
     ctx.profile_enable(False)
@@ -439,7 +473,7 @@ def run_b200(args):
     # (poses, speed/bias, landmarks, quality).  Each step therefore solves the same graph as the resident leg from the
     # same initial estimates.  Two slot ranges alternate so that the host-side command packing, the H2D copy, the
     # device-side graph compile and the D2H copy of one range overlap the solve of the other (transfer stream).
-    e2e_steps = max(12, 2 * args.steps)     # the two-range pipeline needs a fill and a drain step: amortised like in a long stream
+    e2e_steps = args.steps
     range_windows = [windows[i % len(windows)] for i in range(Be)]
     descs = ctx.make_descs(range_windows)              # descriptors only point at the host arrays
     for base in (0, Be):
@@ -514,7 +548,7 @@ def run_b200(args):
     if isinstance(frontend, dict):
         frontend["images_per_s_all_gpus"] = ips_all
     if rank == 0:
-        peak, peak_kind = load_peaks()
+        peak, fp64_peak, peak_kind = data_sheet_peaks(torch.cuda.get_device_name(dev))
         w = windows[0]
         bytes_iter = float(np.mean([x.algorithmic_bytes_per_iteration() for x in windows]))
         flops_iter = float(np.mean([x.algorithmic_flops_per_iteration() for x in windows]))
@@ -523,18 +557,6 @@ def run_b200(args):
         sv_ms = prof["solve_ms"] / max(prof["solve_launches"], 1)
         achieved = B * bytes_iter / (lm_ms * 1e-3) / 1e9
         total_k = prof["landmarks_ms"] + prof["solve_ms"] + prof["quality_ms"]
-        # DRAM bytes per launch of the group from the committed ncu --set full captures (profiles/), scaled to B
-        traffic, traffic_src = None, None
-        import glob
-        tpaths = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_traffic.json")))
-        tpath = tpaths[-1] if tpaths else ""
-        if tpath:
-            tj = json.load(open(tpath))
-            ks = tj.get("kernels", {})
-            if all(k in ks for k in ("k_linearize", "k_lmblock", "k_schur")):
-                traffic = sum(ks[k]["dram_read_bytes"] + ks[k]["dram_write_bytes"] for k in ("k_linearize", "k_lmblock", "k_schur"))
-                traffic = traffic * B / float(tj.get("windows", B))
-                traffic_src = "profiles/%s (ncu dram__bytes_read+write.sum of the three kernels at %d windows)" % (os.path.basename(tpath), tj.get("windows", B))
         # CPU baseline: bounded sample of the same workload on this box's host cores -- one oracle thread per
         # window; as many windows in flight as there are usable CPUs (cgroup quota) or twice that, whichever is faster
         cores = host_cpus()
@@ -558,16 +580,16 @@ def run_b200(args):
                     "full_window_upload_bytes": int(full_upload_bytes) * world,
                     "note": "resident windows: per step reset (device) + re-add of the newest frame with its IMU term and observations (H2D) "
                             "+ optimize(10) + download of all estimates (D2H); two slot ranges alternate so transfers overlap the solve"},
+            "gpu": gpu_identity(local_rank),
             "gpu_launches": launches_all,
             "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": "k_linearize + k_lmblock + k_schur (residuals, Jacobian factors, J^T J, Schur complement)",
-                         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                         "traffic_source": traffic_src,
+                         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak if peak else None,
                          "peak_source": peak_kind, "avg_launch_ms": lm_ms, "algorithmic_bytes_per_window_iteration": bytes_iter,
                          "fp64_gflops": B * flops_iter / (lm_ms * 1e-3) / 1e9,
                          "share_of_kernel_time": prof["landmarks_ms"] / max(total_k, 1e-9),
                          "k_solve_avg_launch_ms": sv_ms, "k_solve_share": prof["solve_ms"] / max(total_k, 1e-9)},
-            "roofline_fp64": fp64_roofline(B * flops_iter / (lm_ms * 1e-3) / 1e9),
+            "roofline_fp64": fp64_roofline(B * flops_iter / (lm_ms * 1e-3) / 1e9, fp64_peak, peak_kind + ", FP64 without tensor cores"),
             "cpu_baseline": {"value": cpu_iters / cpu_dt, "unit": "iterations/s", "cores": cores, "kind": "port",
                              "sample": "%d windows x optimize(%d) + quality pass, one oracle thread per window, %d threads" % (n_cpu, ITERS, cores)},
             "latency": lat,
@@ -587,12 +609,17 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--batch", type=int, default=592, help="resident windows per GPU (4 per SM)")
-    ap.add_argument("--e2e-batch", type=int, default=592, help="windows per step of the e2e leg (two slot ranges of this size alternate)")
+    ap.add_argument("--batch", type=int, default=528, help="resident windows per GPU (4 per SM of a 132-SM H100)")
+    ap.add_argument("--e2e-batch", type=int, default=528, help="windows per step of the e2e leg (two slot ranges of this size alternate)")
     ap.add_argument("--skip-cpu", action="store_true", help="tuning runs only: shrink the cpu_baseline sample to one window")
     ap.add_argument("--host-threads", type=int, default=12, help="host threads packing/uploading windows in the e2e leg")
     ap.add_argument("--distinct", type=int, default=8, help="distinct synthetic windows per rank (replicated to fill the batch)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs is supported for --impl b200 only")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":
         run_reference(args)

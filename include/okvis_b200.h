@@ -1,5 +1,5 @@
 /*
- * okvis_b200.h -- C-ABI of libokvis_b200.so, the B200-native hot path of OKVIS.
+ * okvis_b200.h -- C-ABI of libokvis_b200.so, the H100-native (sm_90a) hot path of OKVIS.
  *
  * Every entry point is extern "C", takes plain pointers / sizes / POD structs and
  * returns an int status (0 = OKB_OK, <0 = error, see okb_status).  Host buffers are

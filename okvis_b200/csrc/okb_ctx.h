@@ -46,7 +46,7 @@ struct okb_frontend_state;
 struct okb_ctx {
   int device = 0;
   int max_windows = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int smem_optin = 0;
   int smem_per_sm = 0;
   int chunk_cap = 1;

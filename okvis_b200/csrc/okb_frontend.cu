@@ -1,4 +1,4 @@
-// Frontend path of libokvis_b200.so (sm_100a): Harris detect -> uniformity -> gravity-aligned
+// Frontend path of libokvis_b200.so (sm_90a): Harris detect -> uniformity -> gravity-aligned
 // 48/64-byte binary descriptor, and the DenseMatcher Hamming brute force.
 //   okb_detect_describe   <- Frontend::detectAndDescribe (okvis_frontend/src/Frontend.cpp:92-114)
 //   okb_hamming_match     <- DenseMatcher::match          (okvis_matcher/include/okvis/implementation/DenseMatcher.hpp:48-225,

@@ -1,4 +1,4 @@
-// Device-resident window graph (sm_100a): the "master" copy of a keyframe window in the caller's index space,
+// Device-resident window graph (sm_90a): the "master" copy of a keyframe window in the caller's index space,
 // edited by a command interpreter and compiled into the solver's working layout on the device.
 //
 //   host (okb_window_upload / okb_window_add_frame / ... in okb_estimator.cu) only appends COMMANDS + payload to a

@@ -1,4 +1,4 @@
-// IMU preintegration / propagation / residual for the B200 estimator path, written ONCE against a
+// IMU preintegration / propagation / residual for the CUDA estimator path, written ONCE against a
 // tiny "cooperative context" so the same code runs (a) warp-cooperatively inside kernels (32 lanes
 // share the 15x15 products through shared memory, small 3x3 algebra is replicated per lane) and
 // (b) sequentially on the host for the GPU-less host check (tests/hostcheck).

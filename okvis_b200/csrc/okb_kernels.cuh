@@ -1,4 +1,4 @@
-// Kernels of the batched dogleg/Schur solver (sm_100a).  One solver round is
+// Kernels of the batched dogleg/Schur solver (sm_90a).  One solver round is
 //   k_imu (side stream) || k_linearize -> k_lmblock -> k_schur -> k_reduce_partials   (okb_kernels_lm.cuh), then
 //   k_solve ("S"): one CTA of 256 threads per window, two CTAs per SM.  IMU / prior / marginalisation terms
 //       assembled directly in the shared-memory system buffer (packed lower triangle), step acceptance

@@ -1,4 +1,4 @@
-// Landmark-side kernels of the solver round (sm_100a):
+// Landmark-side kernels of the solver round (sm_90a):
 //   k_linearize ("A1"): one thread per (landmark, frame).  Reprojection residuals + Jacobian factors of
 //       the frame's cameras, Cauchy weighting, per-frame M_f = sum rho' A^T A and m_f = sum rho' A^T r
 //       (stored tile-major, see lm_M_index), plus the pose-block contributions H_pp,f = G^T M_f G and

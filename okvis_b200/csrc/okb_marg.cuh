@@ -1,4 +1,4 @@
-// Device-side marginalisation (sm_100a): the numeric work of okvis::ceres::MarginalizationError that
+// Device-side marginalisation (sm_90a): the numeric work of okvis::ceres::MarginalizationError that
 // Estimator::applyMarginalizationStrategy (okvis_ceres/src/Estimator.cpp:434-773) drives once per frame --
 //   addResidualBlock       okvis_ceres/src/MarginalizationError.cpp:127-435  (linearise residual blocks at the
 //                          first-estimate linearisation points, Cauchy correction :313-365, H += J^T J, b0 -= J^T r)

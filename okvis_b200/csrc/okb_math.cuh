@@ -1,4 +1,4 @@
-// Per-thread math of the B200 estimator path: kinematics, camera models, single-residual functors.
+// Per-thread math of the CUDA estimator path: kinematics, camera models, single-residual functors.
 // Everything here is OKB_HD (host + device) so tests can also compile it for the host and compare it
 // with the oracle without a GPU (tests/hostcheck); the product only ever calls it from kernels.
 //

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def _cuda_device_present():
@@ -29,7 +29,7 @@ def pytest_collection_modifyitems(config, items):
     gpu_items = [it for it in items if it.get_closest_marker("gpu")]
     if not gpu_items or _cuda_device_present():
         return
-    skip = pytest.mark.skip(reason="no CUDA device (run with -m gpu on the B200 box)")
+    skip = pytest.mark.skip(reason="no CUDA device (run with -m gpu on an H100)")
     for it in gpu_items:
         it.add_marker(skip)
 

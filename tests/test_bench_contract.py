@@ -1,4 +1,4 @@
-"""bench.py's reference arm runs without a GPU: check the JSON contract of the line it prints (the B200 arm prints
+"""bench.py's reference arm runs without a GPU: check the JSON contract of the line it prints (the GPU arm prints
 the same keys plus roofline / clocks / gpu_launches and is exercised on the GPU box)."""
 import json
 import os

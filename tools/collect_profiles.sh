@@ -4,7 +4,7 @@
 # into the tracked files under profiles/.
 set -u
 R=${1:-r01}
-B=${2:-592}
+B=${2:-528}
 mkdir -p gpurun_out
 ncu --metrics gpu__time_duration.sum --clock-control none -c 700 --csv --log-file gpurun_out/${R}_launches_bench.csv \
     python bench.py --steps 2 --warmup 3 --skip-cpu > gpurun_out/${R}_bench_under_ncu.log 2>&1

@@ -4,7 +4,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 from okvis_b200 import capi, synthetic
-Be = int(sys.argv[1]) if len(sys.argv) > 1 else 148
+Be = int(sys.argv[1]) if len(sys.argv) > 1 else 132
 ctx = capi.Context(0, 2 * Be)
 ws = [synthetic.make_window(2, i) for i in range(8)]
 rw = [ws[i % 8] for i in range(Be)]

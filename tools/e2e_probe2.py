@@ -1,10 +1,10 @@
-"""Where does the e2e leg lose time?  Variants of the streaming loop on 592-window ranges."""
+"""Where does the e2e leg lose time?  Variants of the streaming loop on 528-window ranges."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
 from okvis_b200 import capi, synthetic
-B = int(sys.argv[1]) if len(sys.argv) > 1 else 592
+B = int(sys.argv[1]) if len(sys.argv) > 1 else 528
 ctx = capi.Context(0, 2 * B)
 ws = [synthetic.make_window(2, i) for i in range(8)]
 rw = [ws[i % 8] for i in range(B)]

@@ -1,5 +1,5 @@
 // FP64 peak micro-benchmarks on the bench GPU: vector DFMA and tensor DMMA (mma.sync.m8n8k4.f64).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_peak fp64_peak.cu ; prints JSON.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_peak fp64_peak.cu ; prints JSON.
 #include <cstdio>
 #include <cuda_runtime.h>
 

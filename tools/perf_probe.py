@@ -8,7 +8,7 @@ out = open(os.path.join(ROOT, "gpurun_out", "perf_probe.txt"), "w")
 def P(*a):
     s = " ".join(str(x) for x in a); print(s); out.write(s + "\n"); out.flush()
 ws = [synthetic.make_window(2, i) for i in range(4)]
-for B in (1, 148, 592):
+for B in (1, 132, 528):
     ctx = capi.Context(0, B)
     for i in range(B):
         ctx.upload(i, ws[i % 4])

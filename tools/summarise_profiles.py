@@ -4,7 +4,7 @@ solver kernel from its --set full capture."""
 import csv, json, os, shutil, sys
 from collections import defaultdict
 R = sys.argv[1] if len(sys.argv) > 1 else "r01"
-B = int(sys.argv[2]) if len(sys.argv) > 2 else 592
+B = int(sys.argv[2]) if len(sys.argv) > 2 else 528
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G, P = os.path.join(ROOT, "gpurun_out"), os.path.join(ROOT, "profiles")
 
@@ -62,7 +62,7 @@ json.dump({"windows": B, "note": "one ncu --set full capture per kernel, tools/p
            "kernels": kern}, open(os.path.join(P, f"{R}_traffic.json"), "w"), indent=1)
 
 with open(os.path.join(P, f"{R}_summary.md"), "w") as f_:
-    f_.write(f"# {R}: ncu summary of the solver kernels (B200, cfg-2 windows)\n\n")
+    f_.write(f"# {R}: ncu summary of the solver kernels (H100, cfg-2 windows)\n\n")
     f_.write(f"## Launch list of `bench.py --steps 2 --warmup 3` (first 700 launches; `{R}_launches_bench.csv`)\n\n")
     f_.write("per-launch times under ncu are cold-cache and serialised: read the SHARE, not the absolute\n\n")
     f_.write("| kernel | launches | total us | mean us | share |\n|---|---|---|---|---|\n")
