@@ -101,6 +101,9 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
   cudaFuncSetAttribute(k_solve<512>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(k_schur, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(k_quality, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
+  cudaFuncSetAttribute(k_landmarks<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemL_bytes(2));
+  cudaFuncSetAttribute(k_landmarks<2, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_landmarks<4, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemL_bytes(4));
   *out = c;
   return OKB_OK;
 }
@@ -226,7 +229,7 @@ int plan_arena(okb_ctx* c, int win, const WinCaps& q) {
   const size_t o_pose_c = P.take(8 * 7 * Kc), o_sb_c = P.take(8 * 9 * Kc), o_lm_c = P.take(8 * 4 * (size_t)Lpc);
   size_t o_lmg[2], o_lmE[2], o_gd[2], o_Ed[2];
   for (int b = 0; b < 2; ++b) { o_lmg[b] = P.take(8 * 3 * (size_t)Lc); o_lmE[b] = P.take(8 * 3 * (size_t)Lc); }
-  const size_t o_Rinv = P.take(8 * 6 * (size_t)Lc), o_slotctx = P.take(sizeof(SlotCtx) * NSPc), o_mf = P.take(8 * 3 * (size_t)Lpc * Kc);
+  const size_t o_Rinv = P.take(8 * 6 * (size_t)Lc), o_slotctx = P.take(sizeof(SlotCtx) * NSPc);
   const size_t o_gn = P.take(8 * 3 * (size_t)Lc), o_Li = P.take(8 * 9 * (size_t)Lpc), o_scale = P.take(8 * 3 * (size_t)Lc);
   const int n_cx = (Lc + L1_THREADS - 1) / L1_THREADS;
   const size_t o_partH = P.take(8 * (size_t)n_cx * Kc * kPartH), o_part = P.take(8 * (size_t)dcpc * dcpc * c->chunk_cap);
@@ -281,7 +284,7 @@ int plan_arena(okb_ctx* c, int win, const WinCaps& q) {
   W.lm = dp(o_lm); W.pose_init = dp(o_pose_i); W.sb_init = dp(o_sb_i);
   W.pose_c = dp(o_pose_c); W.sb_c = dp(o_sb_c); W.lm_c = dp(o_lm_c);
   for (int b = 0; b < 2; ++b) { W.lm_g[b] = dp(o_lmg[b]); W.lm_E[b] = dp(o_lmE[b]); W.gd[b] = dp(o_gd[b]); W.Ed[b] = dp(o_Ed[b]); }
-  W.lm_Rinv = dp(o_Rinv); W.slot_ctx = reinterpret_cast<SlotCtx*>(A + o_slotctx); W.lm_mf = dp(o_mf); W.lm_gn = dp(o_gn);
+  W.lm_Rinv = dp(o_Rinv); W.slot_ctx = reinterpret_cast<SlotCtx*>(A + o_slotctx); W.lm_gn = dp(o_gn);
   W.lm_Li = dp(o_Li); W.lm_scale = dp(o_scale); W.partH = dp(o_partH); W.partA = dp(o_part);
   W.Hd = dp(o_Hd); W.ud = dp(o_ud); W.scale_d = dp(o_scd); W.chol = dp(o_chol);
   W.obs_z = reinterpret_cast<double2*>(A + o_obsz); W.obs_w = dp(o_obsw); W.lm_M = dp(o_M); W.quality = dp(o_quality);
@@ -1087,7 +1090,7 @@ extern "C" int okb_window_reset(okb_ctx* c, int first, int count) {
 // Launch geometry of one optimize of windows [first, first+count): everything a captured CUDA graph depends on
 // besides the kernel arguments.
 struct RoundPlan {
-  int max_chunks = 1, max_imu = 0, max_cx = 1, max_K = 1, acc_copies = 1, chol_smem = 1, solve_threads = S_THREADS, gxQ = 1, shard = 0, push_gx = 1;
+  int max_chunks = 1, max_imu = 0, max_cx = 1, lm_wide = 0, acc_copies = 1, chol_smem = 1, solve_threads = S_THREADS, gxQ = 1, shard = 0, push_gx = 1;
   size_t smA = 0, smS = 0, smQ = 0;
 };
 static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
@@ -1108,7 +1111,6 @@ static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
     P.max_imu = std::max(P.max_imu, W.n_imu);
     P.smA = std::max(P.smA, smemA2_bytes(W.K, W.dcp, acc_copies));
     P.max_cx = std::max(P.max_cx, (W.L + L1_THREADS - 1) / L1_THREADS);
-    P.max_K = std::max(P.max_K, W.K);
     {      // the roomiest mode this window fits; the range runs in the most modest one (1 > 2 > 0)
       const int wm = smemS_bytes(W.d, W.dc, W.K, W.marg_n, W.n_imu, 1) <= (size_t)c->smem_optin ? 1
                    : smemS_bytes(W.d, W.dc, W.K, W.marg_n, W.n_imu, 2) <= (size_t)c->smem_optin ? 2 : 0;
@@ -1136,6 +1138,9 @@ static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
     }
   }
   P.acc_copies = acc_copies; P.chol_smem = chol_smem;
+  // k_landmarks: launches whose landmark tiles would fill less than half the SMs (few windows, the cfg-5 window) split
+  // every tile's frame walk over a cluster of two 512-thread CTAs; the sums keep their order in either shape
+  P.lm_wide = (2 * count * P.max_cx <= c->sm_count) ? 1 : 0;
   P.solve_threads = (2 * count <= c->sm_count) ? 512 : S_THREADS;      // few windows: one wide CTA per SM (all ranks of a sharded window choose alike)
   P.gxQ = std::max(1, std::min((maxL + 127) / 128, (4 * c->sm_count + count - 1) / count));
   P.shard = c->shard_world > 1 ? 1 : 0;
@@ -1158,15 +1163,24 @@ static int launch_rounds(okb_ctx* c, int first, int count, const okb_solve_optio
       c->launches += 1;
     }
     prof_begin(c, 0);
-    k_linearize<<<dim3(P.max_cx, P.max_K, count), L1_THREADS, 0, c->stream>>>(c->d_wins, first);
-    k_lmblock<<<dim3(P.max_cx, count), 128, 0, c->stream>>>(c->d_wins, first);
+    if (P.lm_wide) {     // one cluster of two CTAs per landmark tile
+      cudaLaunchConfig_t cfg = {};
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeClusterDimension;
+      attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+      cfg.gridDim = dim3(2 * P.max_cx, count); cfg.blockDim = dim3(4 * L1_THREADS); cfg.dynamicSmemBytes = smemL_bytes(4);
+      cfg.stream = c->stream; cfg.attrs = attr; cfg.numAttrs = 1;
+      cudaLaunchKernelEx(&cfg, k_landmarks<4, 2>, (const WinDev*)c->d_wins, first);
+    } else {
+      k_landmarks<2, 1><<<dim3(P.max_cx, count), 2 * L1_THREADS, smemL_bytes(2), c->stream>>>(c->d_wins, first);
+    }
     k_schur<<<gridA, A2_THREADS, P.smA, c->stream>>>(c->d_wins, first, P.acc_copies, opt.max_iterations);
     if (P.shard) {    // chunk reduction fused with the push half of the all-reduce over peer memory
       k_shard_push<<<dim3(P.push_gx, count), 256, 0, c->stream>>>(c->d_wins, first);
       c->launches += 1;
     } else if (P.max_chunks > 1) { k_reduce_partials<<<dim3(8, count), 256, 0, c->stream>>>(c->d_wins, first); c->launches += 1; }
     prof_end(c);
-    c->launches += 3;
+    c->launches += 2;
     if (P.max_imu > 0 && !imu_serial) cudaStreamWaitEvent(c->stream, c->ev_imu, 0);
     prof_begin(c, 1);
     if (P.solve_threads == 512) k_solve<512><<<count, 512, P.smS, c->stream>>>(c->d_wins, first, opt, P.chol_smem);

@@ -85,10 +85,9 @@ __host__ __device__ inline size_t shard_win_bytes(int world, size_t box_cap) {
 
 // Everything kernels need to know about one window.  All pointers are device pointers into the
 // window's arena.
-// lm_M / lm_mf are tile-major: [tile of 32 landmarks][frame][element][32] -- a warp's accesses are 256-byte rows and
+// lm_M is tile-major: [tile of 32 landmarks][frame][element][32] -- a warp's accesses are 256-byte rows and
 // the frames [a, b] of one tile are ONE contiguous block (a single TMA bulk copy in k_schur).
 __host__ __device__ inline size_t lm_M_index(int l, int f, int K) { return ((size_t)(l >> 5) * K + f) * 192 + (l & 31); }   // + 32 * element (0..5)
-__host__ __device__ inline size_t lm_mf_index(int l, int f, int K) { return ((size_t)(l >> 5) * K + f) * 96 + (l & 31); }    // + 32 * element (0..2)
 
 // packed download block: pose [K][7] | speed/bias [NSB][9] | pad to 4 doubles | landmarks [L][4] | quality [L]
 // (the landmark part is written with 32-byte vector stores)
@@ -114,7 +113,7 @@ struct WinDev {
   int dirty;                                   // 1 = the graph changed: compile before the next optimize
   int full;                                    // 1 = the pending commit is a full upload: snapshot the initial state
   int K, NSB, NE, L, NC;
-  int Lp;              // L rounded up to whole tiles of 32: leading dimension of lm_M / lm_mf, rows of lm_Li / lm_c (bulk copies stay aligned)
+  int Lp;              // L rounded up to whole tiles of 32: leading dimension of lm_M, rows of lm_Li / lm_c (bulk copies stay aligned)
   int CP;              // cameras per frame padded to a power of two
   int NS;              // slots = K * CP  (slot = frame * CP + cam)
   int NG;              // slot groups of 32 lanes
@@ -137,7 +136,7 @@ struct WinDev {
   int n_obs;                                   // host's upper bound of the list length (launch sizing); exact: st->g.n_obs
   // Landmarks are stored sorted by (first, last) observing frame (okb_window_upload): tracks are runs of
   // consecutive frames, so neighbouring landmarks see nearly the same frames -> warp-coherent visibility
-  // in k_linearize and block-sparse Schur tiles in k_schur.
+  // in k_landmarks and block-sparse Schur tiles in k_schur.
   unsigned char* zero_ptr[3];                  // regions cleared by k_zero at every compile: observation grid (z, w), M blocks
   size_t zero_bytes[3];
   uint32_t* lm_inv;                            // [L] caller's landmark index -> internal (sorted) index
@@ -147,7 +146,6 @@ struct WinDev {
   double* lm_E[2];                             // [L][3] metric (Ceres diagonal^2 / scale^2)
   double* lm_Rinv;                             // [L][6] (H_ll + mu E)^-1, symmetric packed
   double* lm_M;                                // [Lp/32][K][6][32] per-frame sum of rho' A^T A (lm_M_index)
-  double* lm_mf;                               // [Lp/32][K][3][32] per-frame sum of rho' A^T r (lm_mf_index)
   SlotCtx* slot_ctx;                           // [NS] built by k_reset / k_solve whenever the candidate poses change
   double* lm_Li;                               // [L][9] L^-1 of (H_ll + mu E) (6) and z = L^-1 g_l (3)
   double* lm_gn;                               // [L][3] Gauss-Newton step of the current linearisation
@@ -156,7 +154,7 @@ struct WinDev {
   // kernel A -> kernel S partial sums, one record per chunk
   double* partA;                               // [n_chunks][dcp*dcp] Schur accumulator per chunk (k_schur)
   int partA_stride;                            // dcp*dcp
-  double* partH;                               // [ceil(L/128)][K][32] pose-block sums, cost, step norm (k_linearize)
+  double* partH;                               // [ceil(L/128)][K][32] pose-block sums, cost, step norm (k_landmarks)
   // dense part
   double* Hd;                                  // [d][d] J^T J restricted to dense blocks (speculative)
   double* gd[2];                               // [d]

@@ -1,5 +1,5 @@
 // Kernels of the batched dogleg/Schur solver (sm_90a).  One solver round is
-//   k_imu (side stream) || k_linearize -> k_lmblock -> k_schur -> k_reduce_partials   (okb_kernels_lm.cuh), then
+//   k_imu (side stream) || k_landmarks -> k_schur -> k_reduce_partials   (okb_kernels_lm.cuh), then
 //   k_solve ("S"): one CTA of 256 threads per window, two CTAs per SM.  IMU / prior / marginalisation terms
 //       assembled directly in the shared-memory system buffer (packed lower triangle), step acceptance
 //       (Ceres 1.9 trust-region logic), blocked Cholesky with the right-hand side as an appended row,

@@ -1,20 +1,20 @@
 // Landmark-side kernels of the solver round (sm_90a):
-//   k_linearize ("A1"): one thread per (landmark, frame).  Reprojection residuals + Jacobian factors of
-//       the frame's cameras, Cauchy weighting, per-frame M_f = sum rho' A^T A and m_f = sum rho' A^T r
-//       (stored tile-major, see lm_M_index), plus the pose-block contributions H_pp,f = G^T M_f G and
-//       g_p,f = G^T m_f reduced per CTA.  All global loads are issued up front; CTAs whose landmarks
-//       do not see the frame exit immediately (landmarks are sorted by observing-frame range).
-//   k_lmblock ("A1b"): one thread per landmark: H_ll = sum_f M_f, (H_ll + mu E)^-1 by 3x3 Cholesky.
+//   k_landmarks ("A1"): one CTA per 128 landmarks.  Candidate landmark, reprojection residuals + Jacobian factors of
+//       the cameras of every frame its tiles see, Cauchy weighting, per-frame M_f = sum rho' A^T A (stored tile-major,
+//       see lm_M_index) and m_f = sum rho' A^T r, the pose-block contributions H_pp,f = G^T M_f G and g_p,f = G^T m_f
+//       reduced per (CTA, frame), then H_ll = sum_f M_f, g_l = -sum_f m_f and (H_ll + mu E)^-1 by 3x3 Cholesky.
 //   k_schur ("A2"): one CTA per (landmark chunk, window), tiles of 32 landmarks staged by TMA bulk copies:
 //       Y_f = W_f L^-T into a shared-memory tile, then the Schur complement as a block-sparse SYRK
 //       S += Y Y^T with one lane per 6x6 frame-block pair (details at the kernel).
 //   k_quality: post-solve landmark quality (Estimator.cpp:880-894), one thread per landmark.
 #pragma once
+#include <cooperative_groups.h>
+
 #include "okb_estimator.cuh"
 
 namespace okb {
 
-constexpr int L1_THREADS = 128;          // k_linearize block = landmarks per CTA (x one frame)
+constexpr int L1_THREADS = 128;          // landmarks per k_landmarks CTA: one partH record per (CTA, frame)
 constexpr int A2_THREADS = 192;          // k_schur block (6 warps at 168 registers: two CTAs per SM)
 constexpr int A2_TILE = 32;              // landmarks per Y tile
 constexpr int kPartH = 32;               // doubles per (cx, frame) record: 27 H_pp/g_p + cost + stepnorm2 + pad
@@ -28,7 +28,7 @@ struct SlotCtx {
 static_assert(sizeof(SlotCtx) % 8 == 0, "SlotCtx is copied as doubles");
 
 // (frame, camera) contexts at the candidate poses: computed once per round by the kernel that writes the
-// candidate (k_reset / k_solve) instead of by every k_linearize CTA.
+// candidate (k_reset / k_solve) instead of by every k_landmarks CTA.
 __device__ inline void build_slot_ctx(const WinDev& W, int tid, int nthr) {
   for (int s = tid; s < W.NS; s += nthr) {
     const SlotInfo si = W.slots[s];
@@ -41,94 +41,140 @@ __device__ inline void build_slot_ctx(const WinDev& W, int tid, int nthr) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// A1
+// A1: CS CTAs (one cluster) per (128 sorted landmarks, window), FG groups of 128 threads each; thread (g, t) owns
+// landmark t.  Walk lane p = crank * FG + g (crank = rank in the cluster), P = CS * FG lanes.
+//   1. per landmark (group 0): candidate X = lm + a g/E + b GN; CTA 0 also stores lm_c and the step-norm partial;
+//   2. frame walk in rounds: in round k lane p takes the walked frame of rank k P + p (the frames seen by the 4
+//      tiles, ascending), so P frames are in flight.  Per (landmark, frame): <= CP projections, M_f / m_f, the lm_M
+//      store, the 27 pose-block values and the cost, reduced over the 128 landmarks into the (cx, f) record in fixed
+//      order.  M_f / m_f are staged in shared memory (double-buffered by round); after the round's barrier group 0 of
+//      CTA 0 adds them to H_ll / g_l in frame order (the other CTA's through distributed shared memory);
+//   3. group 0 of CTA 0 runs the landmark-block epilogue: metric E, R = H_ll + mu E, 3x3 Cholesky, R^-1, L^-1 | z.
+// H_ll and g_l are summed frame by frame in ascending order whatever P is, so a window gives the same bits alone or in
+// a batch of any size.  The running sums live in shared memory (registers would spill at the 128 that two CTAs per
+// SM allow).
+// Every (cx, f < K) record is written (zeros for frames no tile of the CTA sees); slot 28 of frame 0's record
+// holds the CTA's step norm.  Per record the sums have the same order as a one-frame-per-CTA reduction.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(L1_THREADS) k_linearize(const WinDev* __restrict__ wins, int win_first) {
-  const WinDev& W = wins[win_first + blockIdx.z];
-  const SolverState* st = W.st;
-  if (st->done) return;
-  const int f = blockIdx.y;
-  const int cx = blockIdx.x;
-  if (f >= W.K || cx * L1_THREADS >= W.L) return;
-  const int tid = threadIdx.x;
-  const int L = W.L, CP = W.CP;
+constexpr int kLmRows = 28;     // values reduced per (landmark, frame): 27 H_pp / g_p + cost
 
-  __shared__ SlotCtx slots[32];                 // the frame's cameras (CP <= 32)
-  __shared__ double sred[kPartH][L1_THREADS + 1];
-  __shared__ double s_tw[3];
+// dynamic shared memory of k_landmarks<FG>: per group [kLmRows][129] reduction rows, the step-norm row, X [4][128],
+// the running H_ll | g_l [9][128], staged M_f | m_f [2 rounds][FG][9][128]
+__host__ __device__ inline size_t smemL_bytes(int groups) {
+  return ((size_t)groups * kLmRows * (L1_THREADS + 1) + L1_THREADS + 4 * L1_THREADS + 9 * L1_THREADS + (size_t)2 * groups * 9 * L1_THREADS) *
+         sizeof(double);
+}
 
-  // Landmarks are sorted by observing-frame range: a CTA whose 4 tiles are not seen by frame f has nothing
-  // to do except publishing zeros (frame 0 also carries the candidate landmark update).
-  if (f != 0) {
-    bool any = false;
-#pragma unroll
-    for (int t = 0; t < L1_THREADS / 32; ++t) {
-      const int tile = cx * (L1_THREADS / 32) + t;
-      if (tile * 32 < L) {
-        const uint32_t tr = W.tile_range[tile];
-        any = any || ((int)(tr & 0xffu) <= f && f <= (int)(tr >> 8));
-      }
-    }
-    if (!any) {
-      if (tid < 29) W.partH[((size_t)cx * W.K + f) * kPartH + tid] = 0.0;
-      return;
-    }
-  }
-  // All global loads of this thread are issued before anything waits on them (one memory round trip instead
-  // of a chain visibility -> landmark -> observations): the visibility mask, the landmark, the observations of
-  // the first two cameras and, in STEP mode, the stored step.  Speculative for unobserved pairs; with
-  // sorted landmarks those are few inside a CTA that is not skipped.
+__device__ __forceinline__ void group_sync(int g) {      // barrier of the 128 threads of group g (id 0 is __syncthreads)
+  asm volatile("bar.sync %0, %1;" ::"r"(g + 1), "r"(L1_THREADS) : "memory");
+}
+
+// <FG = 2, CS = 1>: 256 threads, two CTAs (16 warps) per SM at <= 128 registers.  <4, 2> (launches whose tiles would
+// fill less than half the SMs): clusters of two 512-thread CTAs, one CTA per SM, 8 frames in flight per tile.
+template <int FG, int CS>
+__global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 2 : 1) k_landmarks(const WinDev* __restrict__ wins, int win_first) {
+  const WinDev& W = wins[win_first + blockIdx.y];
+  SolverState* st = W.st;
+  if (st->done) return;                // (uniform over a cluster: same window, same landmark tile)
+  const int cx = blockIdx.x / CS, crank = blockIdx.x % CS;
+  const int L = W.L, K = W.K, CP = W.CP;
+  if (cx * L1_THREADS >= L) return;
+  const int tid = threadIdx.x, g = tid / L1_THREADS, t = tid % L1_THREADS;
+  constexpr int P = CS * FG;
+  const int lane = crank * FG + g;
+  const int l = cx * L1_THREADS + t;
   const int mode = st->mode, cur = st->cur;
   const bool cauchy = W.use_cauchy != 0;
-  const int l = cx * L1_THREADS + tid;
-  const int lc = min(l, L - 1);
-  const uint32_t vmask = W.lm_vis[lc];
-  const double4 x4 = *reinterpret_cast<const double4*>(W.lm + 4 * (size_t)lc);
-  const size_t gi0 = (size_t)(f * CP) * L + lc;
-  double w0 = W.obs_w[gi0], w1 = 0.0;
-  double2 z0 = W.obs_z[gi0], z1 = make_double2(0, 0);
-  if (CP > 1) { w1 = W.obs_w[gi0 + L]; z1 = W.obs_z[gi0 + L]; }
-  double sg[3] = {0, 0, 0}, sE[3] = {1, 1, 1}, sgn[3] = {0, 0, 0};
-  if (mode == MODE_STEP) {
-    const double* g = W.lm_g[cur] + 3 * (size_t)lc;
-    const double* E = W.lm_E[cur] + 3 * (size_t)lc;
-    const double* gn = W.lm_gn + 3 * (size_t)lc;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) { sg[c] = g[c]; sE[c] = E[c]; sgn[c] = gn[c]; }
-  }
-  {
-    const double* src = reinterpret_cast<const double*>(W.slot_ctx + f * CP);
-    double* dst = reinterpret_cast<double*>(slots);
-    const int n = CP * (int)(sizeof(SlotCtx) / sizeof(double));
-    for (int i = tid; i < n; i += L1_THREADS) dst[i] = src[i];
-  }
-  if (tid < 3) s_tw[tid] = W.pose_c[7 * f + tid];
-#pragma unroll
-  for (int i = 0; i < 29; ++i) sred[i][tid] = 0.0;   // contributions go straight to shared memory (no live registers)
-  __syncthreads();
+  double* rec = W.partH + (size_t)cx * K * kPartH;        // this CTA's records [K][kPartH]
 
-  if (l < L) {
-    const bool vis = (vmask >> f) & 1u;
-    if (vis || f == 0) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  double(*sred_all)[L1_THREADS + 1] = reinterpret_cast<double(*)[L1_THREADS + 1]>(smem_raw);
+  double(*sred)[L1_THREADS + 1] = sred_all + g * kLmRows;               // this group's rows
+  double* sdn = &sred_all[FG * kLmRows][0];                              // step norm per landmark
+  double* sX = sdn + L1_THREADS;                                         // [4][128] candidate landmarks
+  double* sHg = sX + 4 * L1_THREADS;                                     // [9][128] running H_ll (6) | g_l (3)
+  double* sstage = sHg + 9 * L1_THREADS;                                 // [2][FG][9][128] M_f (6) | m_f (3) per lane
+  const bool owner = crank == 0 && g == 0;                               // adds the staged blocks, runs the epilogue
+  if (owner) {
+#pragma unroll
+    for (int k = 0; k < 9; ++k) sHg[k * L1_THREADS + t] = 0.0;
+  }
+
+  // frames seen by the CTA's 4 tiles (landmarks are sorted by observing-frame range)
+  uint32_t fmask = 0;
+#pragma unroll
+  for (int q = 0; q < L1_THREADS / 32; ++q) {
+    const int tile = cx * (L1_THREADS / 32) + q;
+    if (tile * 32 < L) {
+      const uint32_t tr = W.tile_range[tile];
+      const uint32_t fa = tr & 0xffu, fb = tr >> 8;
+      if (fa <= fb) fmask |= ((2u << fb) - 1u) & ~((1u << fa) - 1u);
+    }
+  }
+  const uint32_t vmask = (l < L) ? W.lm_vis[l] : 0u;
+
+  // ---- 1. per-landmark work (group 0)
+  if (g == 0) {
+    double dn = 0.0;
+    if (l < L) {
+      const double4 x4 = *reinterpret_cast<const double4*>(W.lm + 4 * (size_t)l);
       double X[4] = {x4.x, x4.y, x4.z, x4.w};
       if (mode == MODE_STEP) {
         const double a = st->a, b = st->b;
-        double dn = 0;
+        const double* gp = W.lm_g[cur] + 3 * (size_t)l;
+        const double* Ep = W.lm_E[cur] + 3 * (size_t)l;
+        const double* gn = W.lm_gn + 3 * (size_t)l;
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-          const double dlt = a * sg[c] / sE[c] + b * sgn[c];
+          const double dlt = a * gp[c] / Ep[c] + b * gn[c];
           X[c] += dlt;
           dn += dlt * dlt;
         }
-        if (f == 0) sred[28][tid] = dn;
       }
-      if (f == 0) *reinterpret_cast<double4*>(W.lm_c + 4 * (size_t)l) = make_double4(X[0], X[1], X[2], X[3]);
-      if (vis) {
+      if (crank == 0) *reinterpret_cast<double4*>(W.lm_c + 4 * (size_t)l) = make_double4(X[0], X[1], X[2], X[3]);
+#pragma unroll
+      for (int c = 0; c < 4; ++c) sX[c * L1_THREADS + t] = X[c];
+    }
+    sdn[t] = dn;
+  }
+  // records of frames no tile sees, and slot 28 (step norm) of frames other than 0
+  for (int i = tid; crank == 0 && i < K * 29; i += FG * L1_THREADS) {
+    const int f = i / 29, e = i % 29;
+    if (e == 28 ? f != 0 : !((fmask >> f) & 1u)) rec[(size_t)f * kPartH + e] = 0.0;
+  }
+  __syncthreads();
+  if (crank == 0 && tid < 4) {      // step norm into slot 28 of frame 0's record: 4 lanes x 32 columns, then two shuffle steps
+    const int q = tid;
+    double s = 0.0;
+#pragma unroll 8
+    for (int i = 0; i < 32; ++i) s += sdn[q * 32 + ((i + 4 * q) & 31)];
+    s += __shfl_xor_sync(0xfu, s, 1);
+    s += __shfl_xor_sync(0xfu, s, 2);
+    if (q == 0) rec[28] = s;
+  }
+
+  // ---- 2. frame walk in rounds of P frames
+  const int nf = __popc(fmask);
+  uint32_t rest = fmask;
+  for (int i = 0; i < lane && rest; ++i) rest &= rest - 1;
+  for (int r0 = 0; r0 < nf; r0 += P) {
+    const int buf = (r0 / P) & 1;
+    double* stg = sstage + (size_t)((buf * FG + g) * 9) * L1_THREADS + t;     // element k at stg[k * L1_THREADS]
+    if (r0 + lane < nf) {      // (uniform over the group)
+      const int f = __ffs(rest) - 1;
+#pragma unroll
+      for (int i = 0; i < P; ++i) rest &= rest - 1;
+      if ((vmask >> f) & 1u) {
+        const double X[4] = {sX[t], sX[L1_THREADS + t], sX[2 * L1_THREADS + t], sX[3 * L1_THREADS + t]};
+        const size_t gi0 = (size_t)(f * CP) * L + l;
+        const SlotCtx* sc = W.slot_ctx + f * CP;
         double M0 = 0, M1 = 0, M2 = 0, M3 = 0, M4 = 0, M5 = 0, m0 = 0, m1 = 0, m2 = 0, cost = 0, lprod = 1.0;
-        auto add_obs = [&](const SlotCtx& sc, double wobs, double2 z) {
-          if (wobs > 0.0 && sc.valid) {
+        for (int c = 0; c < CP; ++c) {
+          const double wobs = W.obs_w[gi0 + (size_t)c * L];
+          if (wobs > 0.0 && sc[c].valid) {
+            const double2 z = W.obs_z[gi0 + (size_t)c * L];
             double r[2], A[6];
-            reproj_slot<true>(sc.xf, sc.cam, X, z.x, z.y, wobs, r, A);
+            reproj_slot<true>(sc[c].xf, sc[c].cam, X, z.x, z.y, wobs, r, A);
             const double sq = r[0] * r[0] + r[1] * r[1];
             double rho1 = 1.0;
             if (cauchy) {          // 0.5 log(1 + s) per block: the logs of a frame's cameras are taken as one log of the product
@@ -146,82 +192,85 @@ __global__ void __launch_bounds__(L1_THREADS) k_linearize(const WinDev* __restri
             m1 += rho1 * (A[1] * r[0] + A[4] * r[1]);
             m2 += rho1 * (A[2] * r[0] + A[5] * r[1]);
           }
-        };
-        add_obs(slots[0], w0, z0);
-        if (CP > 1) add_obs(slots[1], w1, z1);
-        for (int c = 2; c < CP; ++c) {
-          const size_t gi = gi0 + (size_t)c * L;
-          add_obs(slots[c], W.obs_w[gi], W.obs_z[gi]);
         }
         if (cauchy) cost += 0.5 * log(lprod);
-        double* Mo = W.lm_M + lm_M_index(l, f, W.K);          // tile-major: a warp stores 256-byte rows
+        double* Mo = W.lm_M + lm_M_index(l, f, K);          // tile-major: a warp stores 256-byte rows
         Mo[0] = M0; Mo[32] = M1; Mo[64] = M2; Mo[96] = M3; Mo[128] = M4; Mo[160] = M5;
-        double* mo = W.lm_mf + lm_mf_index(l, f, W.K);
-        mo[0] = m0; mo[32] = m1; mo[64] = m2;
+        stg[0] = M0; stg[L1_THREADS] = M1; stg[2 * L1_THREADS] = M2; stg[3 * L1_THREADS] = M3; stg[4 * L1_THREADS] = M4;
+        stg[5 * L1_THREADS] = M5; stg[6 * L1_THREADS] = m0; stg[7 * L1_THREADS] = m1; stg[8 * L1_THREADS] = m2;
         // pose-block contributions: G = [w I, -[p]x], p = X - t_WS w
+        const double* tw = W.pose_c + 7 * f;
         const double w = X[3];
-        const double p0 = X[0] - s_tw[0] * w, p1 = X[1] - s_tw[1] * w, p2 = X[2] - s_tw[2] * w;
+        const double p0 = X[0] - tw[0] * w, p1 = X[1] - tw[1] * w, p2 = X[2] - tw[2] * w;
         const double Q00 = M1 * p2 - M2 * p1, Q01 = -M0 * p2 + M2 * p0, Q02 = M0 * p1 - M1 * p0;
         const double Q10 = M3 * p2 - M4 * p1, Q11 = -M1 * p2 + M4 * p0, Q12 = M1 * p1 - M3 * p0;
         const double Q20 = M4 * p2 - M5 * p1, Q21 = -M2 * p2 + M5 * p0, Q22 = M2 * p1 - M4 * p0;
         const double w2 = w * w;
-        sred[0][tid] = w2 * M0; sred[1][tid] = w2 * M1; sred[2][tid] = w2 * M2; sred[3][tid] = w2 * M3; sred[4][tid] = w2 * M4; sred[5][tid] = w2 * M5;
-        sred[6][tid] = -w * Q00; sred[7][tid] = -w * Q01; sred[8][tid] = -w * Q02;
-        sred[9][tid] = -w * Q10; sred[10][tid] = -w * Q11; sred[11][tid] = -w * Q12;
-        sred[12][tid] = -w * Q20; sred[13][tid] = -w * Q21; sred[14][tid] = -w * Q22;
-        sred[15][tid] = p2 * Q10 - p1 * Q20; sred[16][tid] = p2 * Q11 - p1 * Q21; sred[17][tid] = p2 * Q12 - p1 * Q22;
-        sred[18][tid] = -p2 * Q01 + p0 * Q21; sred[19][tid] = -p2 * Q02 + p0 * Q22;
-        sred[20][tid] = p1 * Q02 - p0 * Q12;
-        sred[21][tid] = w * m0; sred[22][tid] = w * m1; sred[23][tid] = w * m2;
-        sred[24][tid] = p1 * m2 - p2 * m1; sred[25][tid] = p2 * m0 - p0 * m2; sred[26][tid] = p0 * m1 - p1 * m0;
-        sred[27][tid] = cost;
-      }
-    }
-  }
-  // ---- CTA reduction of the 29 used values (fixed order -> deterministic): 4 threads per value, each sums
-  // 32 of the 128 columns serially (no shuffles), then two shuffle steps combine the four partials
-  __syncthreads();
-  {
-    const int e = tid >> 2, q = tid & 3;
-    double s = 0.0;
-    if (e < 29) {
-      const double* row = &sred[e][q * 32];
-#pragma unroll 8
-      for (int i = 0; i < 32; ++i) s += row[(i + 4 * q) & 31];     // rotated start: the four partial sums hit different banks
-    }
-    s += __shfl_xor_sync(0xffffffffu, s, 1);
-    s += __shfl_xor_sync(0xffffffffu, s, 2);
-    if (e < 29 && q == 0) W.partH[((size_t)cx * W.K + f) * kPartH + e] = s;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Landmark blocks: one thread per landmark.  H_ll = sum_f M_f, g_l = -sum_f m_f, the metric E_l,
-// R = H_ll + mu E and its Cholesky factor: stores R^-1 (back-substitution), L^-1 (Schur tile),
-// g_l, E_l and z = L^-1 g_l.  [f][l] layouts make every load/store coalesced.
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_lmblock(const WinDev* __restrict__ wins, int win_first) {
-  const WinDev& W = wins[win_first + blockIdx.y];
-  SolverState* st = W.st;
-  if (st->done) return;
-  const int l = blockIdx.x * blockDim.x + threadIdx.x;
-  const int L = W.L, K = W.K;
-  if (l >= L) return;
-  const int mode = st->mode, cur = st->cur;
-  const double mu = (mode == MODE_STEP) ? fmax(kMinMu, 2.0 * st->mu / kMuIncrease) : st->mu;
-  double H[6] = {0, 0, 0, 0, 0, 0}, gl[3] = {0, 0, 0};
-  uint32_t vis = W.lm_vis[l];
-  for (int f = 0; f < K; ++f) {
-    if ((vis >> f) & 1u) {
-      const double* Mo = W.lm_M + lm_M_index(l, f, K);
-      const double* mo = W.lm_mf + lm_mf_index(l, f, K);
+        sred[0][t] = w2 * M0; sred[1][t] = w2 * M1; sred[2][t] = w2 * M2; sred[3][t] = w2 * M3; sred[4][t] = w2 * M4; sred[5][t] = w2 * M5;
+        sred[6][t] = -w * Q00; sred[7][t] = -w * Q01; sred[8][t] = -w * Q02;
+        sred[9][t] = -w * Q10; sred[10][t] = -w * Q11; sred[11][t] = -w * Q12;
+        sred[12][t] = -w * Q20; sred[13][t] = -w * Q21; sred[14][t] = -w * Q22;
+        sred[15][t] = p2 * Q10 - p1 * Q20; sred[16][t] = p2 * Q11 - p1 * Q21; sred[17][t] = p2 * Q12 - p1 * Q22;
+        sred[18][t] = -p2 * Q01 + p0 * Q21; sred[19][t] = -p2 * Q02 + p0 * Q22;
+        sred[20][t] = p1 * Q02 - p0 * Q12;
+        sred[21][t] = w * m0; sred[22][t] = w * m1; sred[23][t] = w * m2;
+        sred[24][t] = p1 * m2 - p2 * m1; sred[25][t] = p2 * m0 - p0 * m2; sred[26][t] = p0 * m1 - p1 * m0;
+        sred[27][t] = cost;
+      } else {
 #pragma unroll
-      for (int i = 0; i < 6; ++i) H[i] += Mo[32 * i];
-      gl[0] -= mo[0]; gl[1] -= mo[32]; gl[2] -= mo[64];
+        for (int e = 0; e < kLmRows; ++e) sred[e][t] = 0.0;
+#pragma unroll
+        for (int k = 0; k < 9; ++k) stg[k * L1_THREADS] = 0.0;
+      }
+      // group reduction of the 28 values (fixed order -> deterministic): 4 threads per value, each sums 32 of the 128
+      // columns serially, then two shuffle steps combine the four partials
+      group_sync(g);
+      {
+        const int e = t >> 2, q = t & 3;
+        double s = 0.0;
+        if (e < kLmRows) {
+          const double* row = &sred[e][q * 32];
+#pragma unroll 8
+          for (int i = 0; i < 32; ++i) s += row[(i + 4 * q) & 31];     // rotated start: the four partial sums hit different banks
+        }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        if (e < kLmRows && q == 0) rec[(size_t)f * kPartH + e] = s;
+      }
+      group_sync(g);
+    }
+    // the round's blocks are staged: add them in frame order (buffer buf is rewritten two rounds later, after the
+    // next round's barrier, which the owner reaches only when these reads are done)
+    if constexpr (CS > 1) cooperative_groups::this_cluster().sync();
+    else __syncthreads();
+    if (owner) {
+      double v[9];
+#pragma unroll
+      for (int k = 0; k < 9; ++k) v[k] = sHg[k * L1_THREADS + t];
+      for (int q = 0; q < P && r0 + q < nf; ++q) {
+        const double* src = sstage + (size_t)((buf * FG + q % FG) * 9) * L1_THREADS + t;
+        if constexpr (CS > 1) src = cooperative_groups::this_cluster().map_shared_rank(src, q / FG);
+#pragma unroll
+        for (int k = 0; k < 6; ++k) v[k] += src[k * L1_THREADS];
+#pragma unroll
+        for (int k = 6; k < 9; ++k) v[k] -= src[k * L1_THREADS];
+      }
+#pragma unroll
+      for (int k = 0; k < 9; ++k) sHg[k * L1_THREADS + t] = v[k];
     }
   }
+  if constexpr (CS > 1) cooperative_groups::this_cluster().sync();     // the peers' staging stays until it is read
+
+  // ---- 3. landmark-block epilogue (group 0 of CTA 0)
+  if (!owner || l >= L) return;
+  double v[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) v[k] = sHg[k * L1_THREADS + t];
+  const double H0 = v[0], H1 = v[1], H2 = v[2], H3 = v[3], H4 = v[4], H5 = v[5], gl0 = v[6], gl1 = v[7], gl2 = v[8];
+  const double mu = (mode == MODE_STEP) ? fmax(kMinMu, 2.0 * st->mu / kMuIncrease) : st->mu;
+  const double gl[3] = {gl0, gl1, gl2};
   double sc3[3], E[3];
-  const double hd[3] = {H[0], H[3], H[5]};
+  const double hd[3] = {H0, H3, H5};
   if (mode == MODE_INIT) {
 #pragma unroll
     for (int c = 0; c < 3; ++c) { sc3[c] = 1.0 / (1.0 + sqrt(hd[c])); W.lm_scale[3 * (size_t)l + c] = sc3[c]; }
@@ -234,7 +283,7 @@ __global__ void __launch_bounds__(128) k_lmblock(const WinDev* __restrict__ wins
     const double s2 = sc3[c] * sc3[c];
     E[c] = fmin(fmax(s2 * hd[c], kMinDiag), kMaxDiag) / s2;
   }
-  const double R[6] = {H[0] + mu * E[0], H[1], H[2], H[3] + mu * E[1], H[4], H[5] + mu * E[2]};
+  const double R[6] = {H0 + mu * E[0], H1, H2, H3 + mu * E[1], H4, H5 + mu * E[2]};
   double Lc[6], Li[6];
   if (chol3(R, Lc)) linv3(Lc, Li);
   else {

@@ -8,7 +8,7 @@ B=${2:-528}
 mkdir -p gpurun_out
 ncu --metrics gpu__time_duration.sum --clock-control none -c 700 --csv --log-file gpurun_out/${R}_launches_bench.csv \
     python bench.py --steps 2 --warmup 3 --skip-cpu > gpurun_out/${R}_bench_under_ncu.log 2>&1
-for k in k_linearize k_lmblock k_schur k_solve k_imu k_quality; do
+for k in k_landmarks k_schur k_solve k_imu k_quality; do
   skip=6; [ $k = k_quality ] && skip=1
   ncu --set full --clock-control none --import-source on -k regex:"^$k" -s $skip -c 1 -f -o gpurun_out/${R}_$k \
       python tools/prof_small.py $B 4 > /dev/null 2>&1

@@ -31,7 +31,7 @@ shutil.copy(os.path.join(G, f"{R}_launches_bench.csv"), os.path.join(P, f"{R}_la
 
 # ---- per-kernel full captures
 kern = {}
-for k in ("k_linearize", "k_lmblock", "k_schur", "k_solve", "k_imu", "k_quality"):
+for k in ("k_landmarks", "k_schur", "k_solve", "k_imu", "k_quality"):
     raw = os.path.join(G, f"{R}_{k}_raw.csv")
     det = os.path.join(G, f"{R}_{k}_details.csv")
     if not os.path.exists(raw):
