@@ -1434,16 +1434,16 @@ __global__ void k_hook_reproj(int n, okb_camera cam, const double* pose, const d
 // one warp
 __global__ void k_hook_imu(okb_imu_params prm, const okb_imu_sample* s, int n, int64_t t0, int64_t t1, const double* in /*32*/,
                            const double* sb_ref, int have_ref, ImuCache* cache, double* out /* r15 | SF 450 | sqrt 225 | redo */) {
-  __shared__ double buf[3 * 225 + 450 + 450 + 16 + 32 * kImuPre];
+  __shared__ double buf[kImuScratch];
   WarpCtx cx;
-  ImuWork wk{buf, buf + 225, buf + 450, buf + 1125, buf + 1591};
-  double* F01 = buf + 675; double* SF = buf + 1125; double* r15 = buf + 1575;
+  const ImuScratch sc = imu_scratch(buf);
+  double* SF = sc.SF; double* r15 = sc.r15;
   if (threadIdx.x == 0) { cache->valid = 0; cache->redo_count = 0; for (int k = 0; k < 9; ++k) cache->sb_ref[k] = 0; }
   __syncwarp();
-  if (have_ref) imu_preintegrate(cx, s, n, prm, t0, t1, sb_ref, cache, wk);
+  if (have_ref) imu_preintegrate(cx, s, n, prm, t0, t1, sb_ref, cache, sc.wk);
   const int before = cache->redo_count;
   __syncwarp();
-  imu_evaluate(cx, s, n, prm, t0, t1, in, in + 7, in + 16, in + 23, cache, wk, F01, (double*)nullptr, r15, SF);
+  imu_evaluate(cx, s, n, prm, t0, t1, in, in + 7, in + 16, in + 23, cache, sc.wk, sc.F01, (double*)nullptr, r15, SF);
   for (int e = threadIdx.x; e < 15; e += 32) out[e] = r15[e];
   for (int e = threadIdx.x; e < 450; e += 32) out[15 + e] = SF[e];
   for (int e = threadIdx.x; e < 225; e += 32) out[465 + e] = cache->sqrt_info[e];
@@ -1451,10 +1451,10 @@ __global__ void k_hook_imu(okb_imu_params prm, const okb_imu_sample* s, int n, i
 }
 __global__ void k_hook_propagate(okb_imu_params prm, const okb_imu_sample* s, int n, int64_t t0, int64_t t1, double* io /*16*/,
                                  double* cov, double* jac, int want_cov, int want_jac, int* n_used) {
-  __shared__ double buf[4 * 225 + 32 * kImuPre];
+  __shared__ double buf[kImuScratch];
   WarpCtx cx;
-  ImuWork wk{buf, buf + 225, buf + 450, buf + 675, buf + 900};
-  const int steps = imu_propagate(cx, s, n, prm, t0, t1, io, io + 7, want_cov ? cov : nullptr, want_jac ? jac : nullptr, wk);
+  const int steps = imu_propagate(cx, s, n, prm, t0, t1, io, io + 7, want_cov ? cov : nullptr, want_jac ? jac : nullptr,
+                                  imu_scratch(buf).wk);
   if (threadIdx.x == 0) *n_used = steps;
 }
 __global__ void k_hook_pose(const double* in /* meas7 S36 pose7 */, double* out /* r6 J36 */) {

@@ -63,16 +63,39 @@ OKB_HD double ns_to_sec(int64_t ns) {
   return (double)sec + 1e-9 * (double)nsec;
 }
 
-constexpr int kImuPre = 30;   // doubles per precomputed sample: valid, dt, sigma_g, sigma_a, ac(3), dq(4), Jr(9), R(dq^-1)(9), last
+// imu_integrate works through the samples in batches of kImuBatch.  Each sample has a record of kImuRec doubles:
+// first its precompute (kImuPre doubles: valid, dt, sigma_g, sigma_a, ac(3), dq(4), Jr(9), R(dq^-1)(9), last), then,
+// written over it by the state step, what the covariance step needs: flag (0 skip, 1 integrate, 2 integrate and
+// stop), dt, sigma_g, sigma_a, add(3), 0.5 CCa dt(3), F09, F012, C1, sumA, CC (3x3 each).
+constexpr int kImuPre = 30;
+constexpr int kImuRec = 55;
+constexpr int kImuBatch = 8;
+constexpr int kImuState = (int)(sizeof(ImuInt) / sizeof(double));
 
-// Workspace for the cooperative 15x15 products: 3 matrices of 225 doubles (shared memory on the device).
+// Workspace of one term (shared memory on the device).
 struct ImuWork {
-  double* P;    // covariance (result)
-  double* F;    // scratch (rows of N; later general 15x15 scratch)
-  double* T;    // scratch (U = N P; later general 15x15 scratch)
-  double* P2;   // second covariance buffer for the ping-pong update
-  double* S;    // per-sample precompute buffer: 32 x kImuPre doubles
+  double* P;    // covariance (result), 15x15
+  double* F;    // 15x15 scratch
+  double* T;    // 15x15 scratch
+  double* St;   // the running ImuInt of imu_integrate (kImuState doubles), read by every lane afterwards
+  double* S;    // kImuBatch x kImuRec per-sample records; only imu_integrate uses them, so they may overlay F and T
+  OKB_HD ImuInt& state() const { return *reinterpret_cast<ImuInt*>(St); }
 };
+
+// One term's shared scratch of kImuScratch doubles: P | F | T with the records over F | T and the state behind T.  Once
+// the preintegration has stored sqrt_info all of that is dead, and the evaluation's [F0|F1] (450), sqrt_info [F0|F1]
+// (450) and r15 (15 + 1 pad) reuse the space.
+constexpr int kImuScratch = 450 + 450 + 16;
+static_assert(kImuBatch * kImuRec <= 450 && 675 + kImuState <= kImuScratch, "IMU scratch layout");
+struct ImuScratch {
+  ImuWork wk;
+  double* F01;
+  double* SF;
+  double* r15;
+};
+OKB_HD ImuScratch imu_scratch(double* buf) {
+  return ImuScratch{ImuWork{buf, buf + 225, buf + 450, buf + 675, buf + 225}, buf, buf + 450, buf + 900};
+}
 
 // y = F x for the 15-vector x with F = I + N (N as listed in imu_integrate): rows 0..8 only.
 OKB_HD void imu_apply_F(const double* x, double* y, double dt, const double* X03, const double* F09,
@@ -101,34 +124,40 @@ OKB_HD void imu_apply_F(const double* x, double* y, double dt, const double* X03
 
 // Integrates the samples over [t0,t1].  PREINT selects the redoPreintegration variant
 // (dalpha_db_g uses the right Jacobian; sigma2_v = dt*sigma_a_c^2), otherwise the propagation variant.
-// Returns the number of steps (-1 if the samples do not reach t1).  With WANT_COV the covariance is
-// accumulated in wk.P (must be provided).
+// Returns the number of steps (-1 if the samples do not reach t1).  The final state is left in wk.state(); with
+// WANT_COV the covariance is accumulated in wk.P.
 template <bool PREINT, bool WANT_COV, class Ctx>
 OKB_HD int imu_integrate(const Ctx& cx, const okb_imu_sample* s, int n, const okb_imu_params& prm, int64_t t0,
-                         int64_t t1, const double* sb, ImuInt& st, ImuWork wk) {
+                         int64_t t1, const double* sb, ImuWork wk) {
   if (!(s[n - 1].t_ns >= t1)) return -1;
-  st.Delta_q[0] = st.Delta_q[1] = st.Delta_q[2] = 0; st.Delta_q[3] = 1;
-  for (int k = 0; k < 9; ++k) {
-    st.C_integral[k] = st.C_doubleintegral[k] = st.cross[k] = 0;
-    st.dalpha_db_g[k] = st.dv_db_g[k] = st.dp_db_g[k] = 0;
+  ImuInt& st = wk.state();
+  if (cx.lane() == 0) {
+    st.Delta_q[0] = st.Delta_q[1] = st.Delta_q[2] = 0; st.Delta_q[3] = 1;
+    for (int k = 0; k < 9; ++k) {
+      st.C_integral[k] = st.C_doubleintegral[k] = st.cross[k] = 0;
+      st.dalpha_db_g[k] = st.dv_db_g[k] = st.dp_db_g[k] = 0;
+    }
+    for (int k = 0; k < 3; ++k) st.acc_integral[k] = st.acc_doubleintegral[k] = 0;
+    st.Delta_t = 0;
   }
-  for (int k = 0; k < 3; ++k) st.acc_integral[k] = st.acc_doubleintegral[k] = 0;
-  st.Delta_t = 0;
-  double* Pc = wk.P;   // covariance, updated in place (wk.T holds the intermediate F P)
-  if (WANT_COV) {
+  double* Pc = wk.P;   // covariance, updated in place
+  if (WANT_COV)
     for (int e = cx.lane(); e < 225; e += cx.lanes()) wk.P[e] = 0.0;
-    cx.sync();
-  }
-  // The per-sample quantities that do not depend on the running state (interpolated rates, dt, the
-  // rotation increment dq with its sinc/cos, the right Jacobian, R(dq^-1), saturation flags) are computed
-  // for 32 samples at a time with one sample per lane; the sequential recursion below then only chains
-  // small matrix products.  Same formulas, same order of operations per sample as the reference loop.
+  cx.sync();
+  // Three passes per batch of samples, with the same formulas and the same order of operations per sample as the
+  // reference loop:
+  //  1. the quantities that do not depend on the running state (interpolated rates, dt, the rotation increment dq
+  //     with its sinc/cos, the right Jacobian, R(dq^-1), saturation flags), one sample per lane;
+  //  2. the state recursion (3x3 algebra) on lane 0, which leaves in each sample's record the blocks of N;
+  //  3. the covariance recursion, which reads those blocks as broadcast loads.
+  // The state does not depend on the covariance, so 2 can run ahead of 3; keeping them apart keeps the running state
+  // out of the registers of the 15-wide covariance products.
   int i = 0;
   bool finished = false;
-  for (int base = 0; base < n && !finished; base += 32) {
-    for (int j = cx.lane(); j < 32; j += cx.lanes()) {
+  for (int base = 0; base < n && !finished; base += kImuBatch) {
+    for (int j = cx.lane(); j < kImuBatch; j += cx.lanes()) {
       const int it = base + j;
-      double* o = wk.S + j * kImuPre;
+      double* o = wk.S + j * kImuRec;
       o[0] = 0.0;
       if (it >= n) continue;
       const bool last = (it + 1 == n);
@@ -178,14 +207,15 @@ OKB_HD int imu_integrate(const Ctx& cx, const okb_imu_sample* s, int n, const ok
       o[0] = 1.0;
     }
     cx.sync();
-    for (int j = 0; j < 32 && base + j < n; ++j) {
-      const double* o = wk.S + j * kImuPre;
+    for (int j = 0; cx.lane() == 0 && j < kImuBatch && base + j < n; ++j) {   // the state recursion: lane 0 only
+      double* o = wk.S + j * kImuRec;
       if (o[0] == 0.0) continue;
-      const double dt = o[1], sigma_g_c = o[2], sigma_a_c = o[3];
+      const double dt = o[1];
       const double ac[3] = {o[4], o[5], o[6]};
       const double dq[4] = {o[7], o[8], o[9], o[10]};
       const double* Jr = o + 11;
       const double* Rdqi = o + 20;
+      const bool last = (o[29] != 0.0);
       st.Delta_t += dt;
       double q1[4];
       qmul(st.Delta_q, dq, q1);
@@ -227,35 +257,51 @@ OKB_HD int imu_integrate(const Ctx& cx, const okb_imu_sample* s, int n, const ok
         F09[k] = dt * st.dv_db_g[k] + 0.25 * dt * dt * sumA[k];
         st.dp_db_g[k] += F09[k];
       }
+      for (int k = 0; k < 4; ++k) st.Delta_q[k] = q1[k];
+      for (int k = 0; k < 9; ++k) { st.C_integral[k] = Ci1[k]; st.cross[k] = cross1[k]; st.dv_db_g[k] = dv1[k]; }
+      for (int k = 0; k < 3; ++k) st.acc_integral[k] = ai1[k];
+      // the record of the covariance step, over the precompute (read completely above)
+      if (WANT_COV) {
+        for (int k = 0; k < 3; ++k) { o[4 + k] = add[k]; o[7 + k] = 0.5 * CCa[k] * dt; }
+        for (int k = 0; k < 9; ++k) { o[10 + k] = F09[k]; o[19 + k] = F012[k]; o[28 + k] = C1[k]; o[37 + k] = sumA[k]; o[46 + k] = CC[k]; }
+      }
+      o[0] = last ? 2.0 : 1.0;
+      if (last) break;
+    }
+    cx.sync();
+    for (int j = 0; j < kImuBatch && base + j < n; ++j) {
+      const double* o = wk.S + j * kImuRec;
+      if (o[0] == 0.0) continue;
       if (WANT_COV) {
         // P <- F P F^T + Q with F = I + N, N nonzero only in rows 0..8:
         //   N = {(0,3):-[add]x, (0,6): dt I, (0,9): F09, (0,12): F012, (3,9): -dt C1,
         //        (6,3): -[0.5 CCa dt]x, (6,9): 0.5 dt sumA, (6,12): -0.5 CC dt}
-        // One lane per column: T(:,c) = F P(:,c), then one lane per row: P'(l,:) = F T(l,:)^T.  The blocks of
-        // N stay in registers (constant indexing), each lane does 2 x 66 multiply-adds per sample.
+        // One lane per column: P(:,c) <- F P(:,c), then one lane per row: P(l,:) <- F P(l,:)^T + Q(l,:).  Each lane
+        // reads its whole column (row) before it writes it back, so P is updated in place.  Each lane does
+        // 2 x 66 multiply-adds per sample.
+        const double dt = o[1], sigma_g_c = o[2], sigma_a_c = o[3];
         double X03[9], X63[9];
-        crossMx(add, X03);
-        const double v63[3] = {0.5 * CCa[0] * dt, 0.5 * CCa[1] * dt, 0.5 * CCa[2] * dt};
-        crossMx(v63, X63);
+        crossMx(o + 4, X03);
+        crossMx(o + 7, X63);
+        const double *F09 = o + 10, *F012 = o + 19, *C1 = o + 28, *sumA = o + 37, *CC = o + 46;
         const double s2_dalpha = dt * sigma_g_c * sigma_g_c;
         const double s2_v = PREINT ? dt * sigma_a_c * sigma_a_c : dt * sigma_a_c * prm.sigma_a_c;
         const double s2_p = 0.5 * dt * dt * s2_v;
         const double s2_bg = dt * prm.sigma_gw_c * prm.sigma_gw_c;
         const double s2_ba = dt * prm.sigma_aw_c * prm.sigma_aw_c;
-        double* Tm = wk.T;
         for (int c = cx.lane(); c < 15; c += cx.lanes()) {
           double x[15], y[15];
 #pragma unroll
           for (int k = 0; k < 15; ++k) x[k] = Pc[k * 15 + c];
           imu_apply_F(x, y, dt, X03, F09, F012, C1, X63, sumA, CC);
 #pragma unroll
-          for (int k = 0; k < 15; ++k) Tm[k * 15 + c] = y[k];
+          for (int k = 0; k < 15; ++k) Pc[k * 15 + c] = y[k];
         }
         cx.sync();
         for (int l = cx.lane(); l < 15; l += cx.lanes()) {
           double x[15], y[15];
 #pragma unroll
-          for (int k = 0; k < 15; ++k) x[k] = Tm[l * 15 + k];
+          for (int k = 0; k < 15; ++k) x[k] = Pc[l * 15 + k];
           imu_apply_F(x, y, dt, X03, F09, F012, C1, X63, sumA, CC);
           const int bq = l / 3;
           const double qd = (bq == 0) ? s2_p : (bq == 1) ? s2_dalpha : (bq == 2) ? s2_v : (bq == 3) ? s2_bg : s2_ba;
@@ -264,13 +310,10 @@ OKB_HD int imu_integrate(const Ctx& cx, const okb_imu_sample* s, int n, const ok
         }
         cx.sync();
       }
-      for (int k = 0; k < 4; ++k) st.Delta_q[k] = q1[k];
-      for (int k = 0; k < 9; ++k) { st.C_integral[k] = Ci1[k]; st.cross[k] = cross1[k]; st.dv_db_g[k] = dv1[k]; }
-      for (int k = 0; k < 3; ++k) st.acc_integral[k] = ai1[k];
       ++i;
-      if (o[29] != 0.0) { finished = true; break; }
+      if (o[0] == 2.0) { finished = true; break; }
     }
-    cx.sync();   // the per-sample buffer is rewritten by the next batch
+    cx.sync();   // the records are rewritten by the next batch
   }
   return i;
 }
@@ -302,9 +345,9 @@ OKB_HD bool chol15(const Ctx& cx, double* M) {
 template <class Ctx>
 OKB_HD int imu_preintegrate(const Ctx& cx, const okb_imu_sample* s, int n, const okb_imu_params& prm, int64_t t0,
                             int64_t t1, const double* sb, ImuCache* cache, ImuWork wk) {
-  ImuInt st;
-  const int steps = imu_integrate<true, true>(cx, s, n, prm, t0, t1, sb, st, wk);
+  const int steps = imu_integrate<true, true>(cx, s, n, prm, t0, t1, sb, wk);
   if (steps < 0) return steps;
+  const ImuInt& st = wk.state();
   // symmetrise P into F (workspace)
   for (int e = cx.lane(); e < 225; e += cx.lanes()) {
     const int rr = e / 15, cc = e % 15;
@@ -361,7 +404,7 @@ OKB_HD int imu_preintegrate(const Ctx& cx, const okb_imu_sample* s, int n, const
 //   e15   : unweighted error (15)                 r15: sqrt_info * e
 //   SF    : [15][30] = sqrt_info * [F0 | F1]  (the four minimal Jacobians side by side:
 //           cols 0-5 pose0, 6-14 sb0, 15-20 pose1, 21-29 sb1)
-// wk needs 3x225 doubles; F01 needs 450 doubles (F0|F1 unweighted, [15][30]).
+// F01 needs 450 doubles (F0|F1 unweighted, [15][30]); it and SF may overlay wk (see imu_scratch).
 template <class Ctx>
 OKB_HD void imu_evaluate(const Ctx& cx, const okb_imu_sample* s, int n, const okb_imu_params& prm, int64_t t0, int64_t t1,
                          const double* pose0, const double* sb0, const double* pose1, const double* sb1, ImuCache* cache,
@@ -419,37 +462,52 @@ OKB_HD void imu_evaluate(const Ctx& cx, const okb_imu_sample* s, int n, const ok
   }
   mat3mul(T39, cache->dalpha_db_g, B39);
   for (int k = 0; k < 9; ++k) B39[k] = -B39[k];
-  // assemble [F0 | F1] (15 x 30) cooperatively
+  // assemble [F0 | F1] (15 x 30) cooperatively: the lanes write the identity, the zeros and the blocks read from the
+  // cache; lane 0 writes the blocks computed above, with constant indices so that they stay in registers
   for (int e = cx.lane(); e < 450; e += cx.lanes()) {
     const int rr = e / 30, c30 = e % 30;
     const int which = c30 / 15, cc = c30 % 15;
     const int br = rr / 3, bc = cc / 3, a = rr % 3, b = cc % 3;
     double v;
+    bool lane0 = false;
     if (which == 0) {
       v = (rr == cc) ? 1.0 : 0.0;
       if (br == 0) {
-        if (bc == 0) v = C_S0W[a * 3 + b];
-        else if (bc == 1) v = B03[a * 3 + b];
-        else if (bc == 2) v = C_S0W[a * 3 + b] * Delta_t;
+        if (bc <= 2) lane0 = true;
         else if (bc == 3) v = cache->dp_db_g[a * 3 + b];
         else v = -cache->C_doubleintegral[a * 3 + b];
       } else if (br == 1) {
-        if (bc == 1) v = B33[a * 3 + b];
-        else if (bc == 3) v = B39[a * 3 + b];
+        lane0 = (bc == 1 || bc == 3);
       } else if (br == 2) {
-        if (bc == 1) v = B63[a * 3 + b];
-        else if (bc == 2) v = C_S0W[a * 3 + b];
+        if (bc == 1 || bc == 2) lane0 = true;
         else if (bc == 3) v = cache->dv_db_g[a * 3 + b];
         else if (bc == 4) v = -cache->C_integral[a * 3 + b];
         else v = 0.0;
       }
     } else {
       v = (rr == cc) ? -1.0 : 0.0;
-      if (br == 0 && bc == 0) v = -C_S0W[a * 3 + b];
-      else if (br == 1 && bc == 1) v = B133[a * 3 + b];
-      else if (br == 2 && bc == 2) v = -C_S0W[a * 3 + b];
+      lane0 = (br == bc && br < 3);
     }
-    F01[e] = v;
+    if (!lane0) F01[e] = v;
+  }
+  if (cx.lane() == 0) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+#pragma unroll
+      for (int b = 0; b < 3; ++b) {
+        const int k = a * 3 + b;
+        F01[a * 30 + b] = C_S0W[k];                      // F0 (0,0)
+        F01[a * 30 + 3 + b] = B03[k];                    // F0 (0,1)
+        F01[a * 30 + 6 + b] = C_S0W[k] * Delta_t;        // F0 (0,2)
+        F01[(3 + a) * 30 + 3 + b] = B33[k];              // F0 (1,1)
+        F01[(3 + a) * 30 + 9 + b] = B39[k];              // F0 (1,3)
+        F01[(6 + a) * 30 + 3 + b] = B63[k];              // F0 (2,1)
+        F01[(6 + a) * 30 + 6 + b] = C_S0W[k];            // F0 (2,2)
+        F01[a * 30 + 15 + b] = -C_S0W[k];                // F1 (0,0)
+        F01[(3 + a) * 30 + 18 + b] = B133[k];            // F1 (1,1)
+        F01[(6 + a) * 30 + 21 + b] = -C_S0W[k];          // F1 (2,2)
+      }
+    }
   }
   cx.sync();
   // error vector (replicated), uses F0 rows 0..2 / 6..8, cols 9..14
@@ -475,7 +533,9 @@ OKB_HD void imu_evaluate(const Ctx& cx, const okb_imu_sample* s, int n, const ok
   if (r15) {
     for (int e = cx.lane(); e < 15; e += cx.lanes()) {
       double sacc = 0;
-      for (int k = e; k < 15; ++k) sacc += cache->sqrt_info[e * 15 + k] * err[k];
+#pragma unroll
+      for (int k = 0; k < 15; ++k)
+        if (k >= e) sacc += cache->sqrt_info[e * 15 + k] * err[k];   // constant index: err stays in registers
       r15[e] = sacc;
     }
   }
@@ -494,11 +554,11 @@ OKB_HD void imu_evaluate(const Ctx& cx, const okb_imu_sample* s, int n, const ok
 template <class Ctx>
 OKB_HD int imu_propagate(const Ctx& cx, const okb_imu_sample* s, int n, const okb_imu_params& prm, int64_t t0, int64_t t1,
                          double* pose, double* sb, double* covariance, double* jacobian, ImuWork wk) {
-  ImuInt st;
   int steps;
-  if (covariance) steps = imu_integrate<false, true>(cx, s, n, prm, t0, t1, sb, st, wk);
-  else steps = imu_integrate<false, false>(cx, s, n, prm, t0, t1, sb, st, wk);
+  if (covariance) steps = imu_integrate<false, true>(cx, s, n, prm, t0, t1, sb, wk);
+  else steps = imu_integrate<false, false>(cx, s, n, prm, t0, t1, sb, wk);
   if (steps < 0) return steps;
+  const ImuInt& st = wk.state();
   double q0[4] = {pose[3], pose[4], pose[5], pose[6]};
   qnormalize(q0);
   double C0[9];

@@ -5,7 +5,7 @@
 //       (Ceres 1.9 trust-region logic), blocked Cholesky with the right-hand side as an appended row,
 //       backward substitution, landmark back-substitution, traditional dogleg step, candidate state and
 //       the (frame, camera) contexts of the next linearisation.
-// plus k_imu (one warp per IMU term), k_zero / k_prepare (upload epilogue on the transfer stream), k_reset.
+// plus k_imu (IMU_G lanes per IMU term), k_zero / k_prepare (upload epilogue on the transfer stream), k_reset.
 #pragma once
 #include "okb_chol.cuh"
 #include "okb_estimator.cuh"
@@ -15,7 +15,6 @@ namespace okb {
 
 constexpr int S_THREADS = 256;    // two k_solve CTAs per SM (packed system: ~112 KB of shared memory each)
 constexpr int S_WARPS = S_THREADS / 32;
-constexpr int kImuScratch = 3 * 225 + 450 + 450 + 16 + 32 * kImuPre;   // doubles of shared scratch per IMU warp
 constexpr int kImuOut = 932;     // doubles per IMU term produced by k_imu: H30 | g30 | cost | pad
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
@@ -57,28 +56,28 @@ __device__ __forceinline__ double block_max(double v, double* red) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Kernel I: IMU_G lanes per IMU term (255 registers available, no spills): residual, the four minimal
-// Jacobians, and the term's contribution  [J0 J1 J2 J3]^T [J0 J1 J2 J3] (30x30), J^T r (30), cost.
-// Re-preintegrates exactly when the reference's Evaluate() would.
+// Kernel I: IMU_G lanes per IMU term: residual, the four minimal Jacobians, and the term's contribution
+// [J0 J1 J2 J3]^T [J0 J1 J2 J3] (30x30), J^T r (30), cost.  Re-preintegrates exactly when the reference's Evaluate()
+// would.  A term's shared scratch is kImuScratch doubles (7.3 KB) and the kernel is held to 168 registers, so that
+// 12 CTAs (24 terms) fit on an SM.
 // ------------------------------------------------------------------------------------------------
 constexpr int IMU_G = 16;      // lanes per IMU term: 32 / IMU_G terms per warp
 __host__ __device__ inline size_t smemI_bytes() { return (size_t)(32 / IMU_G) * kImuScratch * sizeof(double); }
-__global__ void __launch_bounds__(32) k_imu(const WinDev* __restrict__ wins, int win_first) {
+__global__ void __launch_bounds__(32, 12) k_imu(const WinDev* __restrict__ wins, int win_first) {
   const WinDev& W = wins[win_first + blockIdx.y];
   if (W.st->done) return;
   const int grp = (threadIdx.x & 31) / IMU_G;
   const int t = blockIdx.x * (32 / IMU_G) + grp;
   if (t >= W.n_imu) return;
   extern __shared__ __align__(16) double imu_buf[];
-  double* buf = imu_buf + (size_t)grp * kImuScratch;
   GroupCtx<IMU_G> cx;
-  ImuWork wk{buf, buf + 225, buf + 450, buf + 675 + 450, buf + 675 + 900 + 16};   // P2 aliases the SF buffer (unused while preintegrating)
-  double* F01 = buf + 675;
-  double* SF = buf + 675 + 450;
-  double* r15 = buf + 675 + 900;
+  const ImuScratch sc = imu_scratch(imu_buf + (size_t)grp * kImuScratch);
+  double* SF = sc.SF;
+  double* r15 = sc.r15;
   const okb_imu_term& T = W.imu_terms[t];
   imu_evaluate(cx, W.samples + T.sample_offset, (int)T.sample_count, W.imu_params, T.t0_ns, T.t1_ns, W.pose_c + 7 * T.pose0,
-               W.sb_c + 9 * T.sb0, W.pose_c + 7 * T.pose1, W.sb_c + 9 * T.sb1, W.imu_cache + t, wk, F01, (double*)nullptr, r15, SF);
+               W.sb_c + 9 * T.sb0, W.pose_c + 7 * T.pose1, W.sb_c + 9 * T.sb1, W.imu_cache + t, sc.wk, sc.F01, (double*)nullptr,
+               r15, SF);
   double* out = W.imu_out + (size_t)t * kImuOut;
   const int lane = cx.lane();
   for (int e = lane; e < 900; e += IMU_G) {

@@ -257,14 +257,13 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
     const okb_imu_term& T = W.imu_terms[t];
     const int blks[4] = {s_pose_blk[T.pose0], s_sb_blk[T.sb0], s_pose_blk[T.pose1], s_sb_blk[T.sb1]};
     if (blks[0] < 0 || blks[1] < 0 || blks[2] < 0 || blks[3] < 0) { if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); } return; }
-    double* F01 = s_imu + 675;
-    double* SF = s_imu + 675 + 450;
-    double* r15 = s_imu + 675 + 900;
+    const ImuScratch isc = imu_scratch(s_imu);
+    double* SF = isc.SF;
+    double* r15 = isc.r15;
     if (warp == 0) {
       WarpCtx cx;
-      ImuWork wk{s_imu, s_imu + 225, s_imu + 450, s_imu + 675 + 450, s_imu + 675 + 900 + 16};
       imu_evaluate(cx, W.samples + T.sample_offset, (int)T.sample_count, W.imu_params, T.t0_ns, T.t1_ns, sc.xlin + 9 * blks[0], sc.xlin + 9 * blks[1],
-                   sc.xlin + 9 * blks[2], sc.xlin + 9 * blks[3], W.imu_cache + t, wk, F01, (double*)nullptr, r15, SF);
+                   sc.xlin + 9 * blks[2], sc.xlin + 9 * blks[3], W.imu_cache + t, isc.wk, isc.F01, (double*)nullptr, r15, SF);
     }
     __syncthreads();
     const int offs[4] = {s_col[blks[0]], s_col[blks[1]], s_col[blks[2]], s_col[blks[3]]};
