@@ -26,6 +26,7 @@ struct WinStore {
   bool committed = false;
   int obs_bound = 0;                  // upper bound of the device-side observation list length
   int K_init = 0, NSB_init = 0, L_init = 0;   // shape at the last full upload (okb_window_reset)
+  int cam_model = okb::kDistAny;      // distortion model shared by all cameras of the last full upload, else kDistAny
   std::vector<okb_imu_term> terms;    // host mirror of the IMU terms / prior indices (dimension bookkeeping of remove_frame)
   std::vector<uint32_t> pp_idx, sbp_idx;
   size_t h2d_bytes = 0;

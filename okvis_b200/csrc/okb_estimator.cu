@@ -35,6 +35,13 @@ static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; 
 // ---------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------
+template <int MODEL>
+static void set_landmarks_attributes() {
+  cudaFuncSetAttribute(k_landmarks<2, 1, MODEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemL_bytes(2));
+  cudaFuncSetAttribute(k_landmarks<2, 1, MODEL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_landmarks<4, 2, MODEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemL_bytes(4));
+}
+
 // The transfer stream gets the highest priority: its small kernels (k_zero / k_prepare) are scheduled as soon
 // as CTA slots free up instead of waiting behind the solver kernels of other slots.
 static cudaError_t create_transfer_stream(cudaStream_t* s) {
@@ -101,9 +108,11 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
   cudaFuncSetAttribute(k_solve<512>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(k_schur, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(k_quality, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
-  cudaFuncSetAttribute(k_landmarks<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemL_bytes(2));
-  cudaFuncSetAttribute(k_landmarks<2, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(k_landmarks<4, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemL_bytes(4));
+  set_landmarks_attributes<OKB_DIST_NONE>();
+  set_landmarks_attributes<OKB_DIST_RADTAN>();
+  set_landmarks_attributes<OKB_DIST_EQUIDISTANT>();
+  set_landmarks_attributes<OKB_DIST_RADTAN8>();
+  set_landmarks_attributes<kDistAny>();
   *out = c;
   return OKB_OK;
 }
@@ -514,6 +523,10 @@ static int upload_pack(okb_ctx* c, int win, const okb_window_desc* D) {
   S.obs_bound = D->n_obs;
   S.full_pending = true;
   S.K_init = K; S.NSB_init = NSB; S.L_init = L;
+  S.cam_model = D->cameras[0].model;      // cameras enter a window only here (CMD_RESET_GRAPH)
+  for (int i = 1; i < NC; ++i)
+    if (D->cameras[i].model != S.cam_model) S.cam_model = kDistAny;
+  if (S.cam_model < OKB_DIST_NONE || S.cam_model > OKB_DIST_RADTAN8) S.cam_model = kDistAny;
   S.uploaded = true;
   return OKB_OK;
 }
@@ -1091,6 +1104,7 @@ extern "C" int okb_window_reset(okb_ctx* c, int first, int count) {
 // besides the kernel arguments.
 struct RoundPlan {
   int max_chunks = 1, max_imu = 0, max_cx = 1, lm_wide = 0, acc_copies = 1, chol_smem = 1, solve_threads = S_THREADS, gxQ = 1, shard = 0, push_gx = 1;
+  int lm_model = kDistAny, _pad = 0;      // (no padding bytes: the plan is compared bytewise as a graph key)
   size_t smA = 0, smS = 0, smQ = 0;
 };
 static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
@@ -1141,11 +1155,30 @@ static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
   // k_landmarks: launches whose landmark tiles would fill less than half the SMs (few windows, the cfg-5 window) split
   // every tile's frame walk over a cluster of two 512-thread CTAs; the sums keep their order in either shape
   P.lm_wide = (2 * count * P.max_cx <= c->sm_count) ? 1 : 0;
+  // k_landmarks is instantiated per distortion model: the one every camera of the launch shares, else the run-time switch
+  P.lm_model = c->wins[first].cam_model;
+  for (int i = first + 1; i < first + count; ++i)
+    if (c->wins[i].cam_model != P.lm_model) P.lm_model = kDistAny;
   P.solve_threads = (2 * count <= c->sm_count) ? 512 : S_THREADS;      // few windows: one wide CTA per SM (all ranks of a sharded window choose alike)
   P.gxQ = std::max(1, std::min((maxL + 127) / 128, (4 * c->sm_count + count - 1) / count));
   P.shard = c->shard_world > 1 ? 1 : 0;
   P.push_gx = std::max(1, std::min(16, c->sm_count / std::max(1, count)));
   return OKB_OK;
+}
+
+template <int MODEL>
+static void launch_landmarks(okb_ctx* c, int first, int count, const RoundPlan& P) {
+  if (P.lm_wide) {     // one cluster of two CTAs per landmark tile
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3(2 * P.max_cx, count); cfg.blockDim = dim3(4 * L1_THREADS); cfg.dynamicSmemBytes = smemL_bytes(4);
+    cfg.stream = c->stream; cfg.attrs = attr; cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, k_landmarks<4, 2, MODEL>, (const WinDev*)c->d_wins, first);
+  } else {
+    k_landmarks<2, 1, MODEL><<<dim3(P.max_cx, count), 2 * L1_THREADS, smemL_bytes(2), c->stream>>>(c->d_wins, first);
+  }
 }
 
 static int launch_rounds(okb_ctx* c, int first, int count, const okb_solve_options& opt, int rounds, const RoundPlan& P) {
@@ -1163,16 +1196,12 @@ static int launch_rounds(okb_ctx* c, int first, int count, const okb_solve_optio
       c->launches += 1;
     }
     prof_begin(c, 0);
-    if (P.lm_wide) {     // one cluster of two CTAs per landmark tile
-      cudaLaunchConfig_t cfg = {};
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      cfg.gridDim = dim3(2 * P.max_cx, count); cfg.blockDim = dim3(4 * L1_THREADS); cfg.dynamicSmemBytes = smemL_bytes(4);
-      cfg.stream = c->stream; cfg.attrs = attr; cfg.numAttrs = 1;
-      cudaLaunchKernelEx(&cfg, k_landmarks<4, 2>, (const WinDev*)c->d_wins, first);
-    } else {
-      k_landmarks<2, 1><<<dim3(P.max_cx, count), 2 * L1_THREADS, smemL_bytes(2), c->stream>>>(c->d_wins, first);
+    switch (P.lm_model) {
+      case OKB_DIST_NONE: launch_landmarks<OKB_DIST_NONE>(c, first, count, P); break;
+      case OKB_DIST_RADTAN: launch_landmarks<OKB_DIST_RADTAN>(c, first, count, P); break;
+      case OKB_DIST_EQUIDISTANT: launch_landmarks<OKB_DIST_EQUIDISTANT>(c, first, count, P); break;
+      case OKB_DIST_RADTAN8: launch_landmarks<OKB_DIST_RADTAN8>(c, first, count, P); break;
+      default: launch_landmarks<kDistAny>(c, first, count, P); break;
     }
     k_schur<<<gridA, A2_THREADS, P.smA, c->stream>>>(c->d_wins, first, P.acc_copies, opt.max_iterations);
     if (P.shard) {    // chunk reduction fused with the push half of the all-reduce over peer memory

@@ -46,33 +46,52 @@ __device__ inline void build_slot_ctx(const WinDev& W, int tid, int nthr) {
 //   1. per landmark (group 0): candidate X = lm + a g/E + b GN; CTA 0 also stores lm_c and the step-norm partial;
 //   2. frame walk in rounds: in round k lane p takes the walked frame of rank k P + p (the frames seen by the 4
 //      tiles, ascending), so P frames are in flight.  Per (landmark, frame): <= CP projections, M_f / m_f, the lm_M
-//      store, the 27 pose-block values and the cost, reduced over the 128 landmarks into the (cx, f) record in fixed
-//      order.  M_f / m_f are staged in shared memory (double-buffered by round); after the round's barrier group 0 of
-//      CTA 0 adds them to H_ll / g_l in frame order (the other CTA's through distributed shared memory);
+//      store, the 27 pose-block values and the cost.  Each warp reduces its 32 landmarks' 28 values with a
+//      reduce-scatter butterfly (lane e ends with value e) and stores them as the warp's partial; after the round's
+//      barrier warp 0 of the group adds the four partials in warp order into the (cx, f) record.  M_f / m_f are staged
+//      in shared memory; group 0 of CTA 0 adds them to H_ll / g_l in frame order after the same barrier (the other
+//      CTA's through distributed shared memory).  Partials and staging are double-buffered by round;
 //   3. group 0 of CTA 0 runs the landmark-block epilogue: metric E, R = H_ll + mu E, 3x3 Cholesky, R^-1, L^-1 | z.
-// H_ll and g_l are summed frame by frame in ascending order whatever P is, so a window gives the same bits alone or in
-// a batch of any size.  The running sums live in shared memory (registers would spill at the 128 that two CTAs per
-// SM allow).
+// H_ll and g_l are summed frame by frame in ascending order whatever P is, and a record's sum order depends only on
+// the landmark's position in the tile, so a window gives the same bits alone or in a batch of any size.  The running
+// sums live in shared memory.
 // Every (cx, f < K) record is written (zeros for frames no tile of the CTA sees); slot 28 of frame 0's record
-// holds the CTA's step norm.  Per record the sums have the same order as a one-frame-per-CTA reduction.
+// holds the CTA's step norm.
+// MODEL is the distortion model of every camera in the launch (OKB_DIST_*), or kDistAny to switch per camera.
 // ------------------------------------------------------------------------------------------------
 constexpr int kLmRows = 28;     // values reduced per (landmark, frame): 27 H_pp / g_p + cost
 
-// dynamic shared memory of k_landmarks<FG>: per group [kLmRows][129] reduction rows, the step-norm row, X [4][128],
-// the running H_ll | g_l [9][128], staged M_f | m_f [2 rounds][FG][9][128]
+// dynamic shared memory of k_landmarks<FG>: the step-norm row, X [4][128], the running H_ll | g_l [9][128], staged
+// M_f | m_f [2 rounds][FG][9][128], warp partials [2 rounds][FG][4 warps][32]
 __host__ __device__ inline size_t smemL_bytes(int groups) {
-  return ((size_t)groups * kLmRows * (L1_THREADS + 1) + L1_THREADS + 4 * L1_THREADS + 9 * L1_THREADS + (size_t)2 * groups * 9 * L1_THREADS) *
+  return ((size_t)L1_THREADS + 4 * L1_THREADS + 9 * L1_THREADS + (size_t)2 * groups * 9 * L1_THREADS + (size_t)2 * groups * L1_THREADS) *
          sizeof(double);
 }
 
-__device__ __forceinline__ void group_sync(int g) {      // barrier of the 128 threads of group g (id 0 is __syncthreads)
-  asm volatile("bar.sync %0, %1;" ::"r"(g + 1), "r"(L1_THREADS) : "memory");
+// Reduce-scatter of 32 values over a warp: on return lane e holds the sum over the warp's lanes of value e.  A fixed
+// butterfly (xor 16, 8, 4, 2, 1), 31 shuffles, so the summation order is the same on every launch.
+template <int O>
+__device__ __forceinline__ void reduce_scatter_step(double (&v)[32]) {     // v[0, 2 O) -> v[0, O): this lane's half
+  const bool hi = (threadIdx.x & O) != 0;
+#pragma unroll
+  for (int i = 0; i < O; ++i) {
+    const double keep = hi ? v[i + O] : v[i], send = hi ? v[i] : v[i + O];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, O);
+  }
+}
+__device__ __forceinline__ double warp_reduce_scatter32(double (&v)[32]) {
+  reduce_scatter_step<16>(v);
+  reduce_scatter_step<8>(v);
+  reduce_scatter_step<4>(v);
+  reduce_scatter_step<2>(v);
+  reduce_scatter_step<1>(v);
+  return v[0];
 }
 
-// <FG = 2, CS = 1>: 256 threads, two CTAs (16 warps) per SM at <= 128 registers.  <4, 2> (launches whose tiles would
-// fill less than half the SMs): clusters of two 512-thread CTAs, one CTA per SM, 8 frames in flight per tile.
-template <int FG, int CS>
-__global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 2 : 1) k_landmarks(const WinDev* __restrict__ wins, int win_first) {
+// <FG = 2, CS = 1>: 256 threads, three CTAs (24 warps) per SM at <= 80 registers.  <4, 2> (launches whose tiles
+// would fill less than half the SMs): clusters of two 512-thread CTAs, one CTA per SM, 8 frames in flight per tile.
+template <int FG, int CS, int MODEL>
+__global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 3 : 1) k_landmarks(const WinDev* __restrict__ wins, int win_first) {
   const WinDev& W = wins[win_first + blockIdx.y];
   SolverState* st = W.st;
   if (st->done) return;                // (uniform over a cluster: same window, same landmark tile)
@@ -88,12 +107,11 @@ __global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 2 : 1) k_landmarks(
   double* rec = W.partH + (size_t)cx * K * kPartH;        // this CTA's records [K][kPartH]
 
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  double(*sred_all)[L1_THREADS + 1] = reinterpret_cast<double(*)[L1_THREADS + 1]>(smem_raw);
-  double(*sred)[L1_THREADS + 1] = sred_all + g * kLmRows;               // this group's rows
-  double* sdn = &sred_all[FG * kLmRows][0];                              // step norm per landmark
+  double* sdn = reinterpret_cast<double*>(smem_raw);                     // step norm per landmark
   double* sX = sdn + L1_THREADS;                                         // [4][128] candidate landmarks
   double* sHg = sX + 4 * L1_THREADS;                                     // [9][128] running H_ll (6) | g_l (3)
   double* sstage = sHg + 9 * L1_THREADS;                                 // [2][FG][9][128] M_f (6) | m_f (3) per lane
+  double* spart = sstage + 2 * FG * 9 * L1_THREADS;                      // [2][FG][4][32] warp partials of the 28 values
   const bool owner = crank == 0 && g == 0;                               // adds the staged blocks, runs the epilogue
   if (owner) {
 #pragma unroll
@@ -160,21 +178,28 @@ __global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 2 : 1) k_landmarks(
   for (int r0 = 0; r0 < nf; r0 += P) {
     const int buf = (r0 / P) & 1;
     double* stg = sstage + (size_t)((buf * FG + g) * 9) * L1_THREADS + t;     // element k at stg[k * L1_THREADS]
-    if (r0 + lane < nf) {      // (uniform over the group)
-      const int f = __ffs(rest) - 1;
+    double* part = spart + (size_t)(buf * FG + g) * L1_THREADS;              // [4 warps][32]
+    const bool walks = r0 + lane < nf;     // (uniform over the group)
+    const int f = __ffs(rest) - 1;
+    if (walks) {
 #pragma unroll
       for (int i = 0; i < P; ++i) rest &= rest - 1;
+      double v[32];
       if ((vmask >> f) & 1u) {
-        const double X[4] = {sX[t], sX[L1_THREADS + t], sX[2 * L1_THREADS + t], sX[3 * L1_THREADS + t]};
         const size_t gi0 = (size_t)(f * CP) * L + l;
         const SlotCtx* sc = W.slot_ctx + f * CP;
-        double M0 = 0, M1 = 0, M2 = 0, M3 = 0, M4 = 0, M5 = 0, m0 = 0, m1 = 0, m2 = 0, cost = 0, lprod = 1.0;
+        // M_f | m_f are accumulated in this lane's staging slot, not in registers: with one distortion model the
+        // observation loop then fits in the 80 registers of three CTAs per SM without spilling
+#pragma unroll
+        for (int k = 0; k < 9; ++k) stg[k * L1_THREADS] = 0.0;
+        double cost = 0, lprod = 1.0;
         for (int c = 0; c < CP; ++c) {
           const double wobs = W.obs_w[gi0 + (size_t)c * L];
           if (wobs > 0.0 && sc[c].valid) {
             const double2 z = W.obs_z[gi0 + (size_t)c * L];
+            const double X[4] = {sX[t], sX[L1_THREADS + t], sX[2 * L1_THREADS + t], sX[3 * L1_THREADS + t]};
             double r[2], A[6];
-            reproj_slot<true>(sc[c].xf, sc[c].cam, X, z.x, z.y, wobs, r, A);
+            reproj_slot<true, MODEL>(sc[c].xf, sc[c].cam, X, z.x, z.y, wobs, r, A);
             const double sq = r[0] * r[0] + r[1] * r[1];
             double rho1 = 1.0;
             if (cauchy) {          // 0.5 log(1 + s) per block: the logs of a frame's cameras are taken as one log of the product
@@ -182,67 +207,57 @@ __global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 2 : 1) k_landmarks(
               lprod *= 1.0 + sq;
               if (lprod > 1e250) { cost += 0.5 * log(lprod); lprod = 1.0; }
             } else cost += 0.5 * sq;
-            M0 += rho1 * (A[0] * A[0] + A[3] * A[3]);
-            M1 += rho1 * (A[0] * A[1] + A[3] * A[4]);
-            M2 += rho1 * (A[0] * A[2] + A[3] * A[5]);
-            M3 += rho1 * (A[1] * A[1] + A[4] * A[4]);
-            M4 += rho1 * (A[1] * A[2] + A[4] * A[5]);
-            M5 += rho1 * (A[2] * A[2] + A[5] * A[5]);
-            m0 += rho1 * (A[0] * r[0] + A[3] * r[1]);
-            m1 += rho1 * (A[1] * r[0] + A[4] * r[1]);
-            m2 += rho1 * (A[2] * r[0] + A[5] * r[1]);
+            stg[0] += rho1 * (A[0] * A[0] + A[3] * A[3]);
+            stg[L1_THREADS] += rho1 * (A[0] * A[1] + A[3] * A[4]);
+            stg[2 * L1_THREADS] += rho1 * (A[0] * A[2] + A[3] * A[5]);
+            stg[3 * L1_THREADS] += rho1 * (A[1] * A[1] + A[4] * A[4]);
+            stg[4 * L1_THREADS] += rho1 * (A[1] * A[2] + A[4] * A[5]);
+            stg[5 * L1_THREADS] += rho1 * (A[2] * A[2] + A[5] * A[5]);
+            stg[6 * L1_THREADS] += rho1 * (A[0] * r[0] + A[3] * r[1]);
+            stg[7 * L1_THREADS] += rho1 * (A[1] * r[0] + A[4] * r[1]);
+            stg[8 * L1_THREADS] += rho1 * (A[2] * r[0] + A[5] * r[1]);
           }
         }
         if (cauchy) cost += 0.5 * log(lprod);
+        const double M0 = stg[0], M1 = stg[L1_THREADS], M2 = stg[2 * L1_THREADS], M3 = stg[3 * L1_THREADS], M4 = stg[4 * L1_THREADS];
+        const double M5 = stg[5 * L1_THREADS], m0 = stg[6 * L1_THREADS], m1 = stg[7 * L1_THREADS], m2 = stg[8 * L1_THREADS];
         double* Mo = W.lm_M + lm_M_index(l, f, K);          // tile-major: a warp stores 256-byte rows
         Mo[0] = M0; Mo[32] = M1; Mo[64] = M2; Mo[96] = M3; Mo[128] = M4; Mo[160] = M5;
-        stg[0] = M0; stg[L1_THREADS] = M1; stg[2 * L1_THREADS] = M2; stg[3 * L1_THREADS] = M3; stg[4 * L1_THREADS] = M4;
-        stg[5 * L1_THREADS] = M5; stg[6 * L1_THREADS] = m0; stg[7 * L1_THREADS] = m1; stg[8 * L1_THREADS] = m2;
         // pose-block contributions: G = [w I, -[p]x], p = X - t_WS w
         const double* tw = W.pose_c + 7 * f;
-        const double w = X[3];
-        const double p0 = X[0] - tw[0] * w, p1 = X[1] - tw[1] * w, p2 = X[2] - tw[2] * w;
+        const double w = sX[3 * L1_THREADS + t];
+        const double p0 = sX[t] - tw[0] * w, p1 = sX[L1_THREADS + t] - tw[1] * w, p2 = sX[2 * L1_THREADS + t] - tw[2] * w;
         const double Q00 = M1 * p2 - M2 * p1, Q01 = -M0 * p2 + M2 * p0, Q02 = M0 * p1 - M1 * p0;
         const double Q10 = M3 * p2 - M4 * p1, Q11 = -M1 * p2 + M4 * p0, Q12 = M1 * p1 - M3 * p0;
         const double Q20 = M4 * p2 - M5 * p1, Q21 = -M2 * p2 + M5 * p0, Q22 = M2 * p1 - M4 * p0;
         const double w2 = w * w;
-        sred[0][t] = w2 * M0; sred[1][t] = w2 * M1; sred[2][t] = w2 * M2; sred[3][t] = w2 * M3; sred[4][t] = w2 * M4; sred[5][t] = w2 * M5;
-        sred[6][t] = -w * Q00; sred[7][t] = -w * Q01; sred[8][t] = -w * Q02;
-        sred[9][t] = -w * Q10; sred[10][t] = -w * Q11; sred[11][t] = -w * Q12;
-        sred[12][t] = -w * Q20; sred[13][t] = -w * Q21; sred[14][t] = -w * Q22;
-        sred[15][t] = p2 * Q10 - p1 * Q20; sred[16][t] = p2 * Q11 - p1 * Q21; sred[17][t] = p2 * Q12 - p1 * Q22;
-        sred[18][t] = -p2 * Q01 + p0 * Q21; sred[19][t] = -p2 * Q02 + p0 * Q22;
-        sred[20][t] = p1 * Q02 - p0 * Q12;
-        sred[21][t] = w * m0; sred[22][t] = w * m1; sred[23][t] = w * m2;
-        sred[24][t] = p1 * m2 - p2 * m1; sred[25][t] = p2 * m0 - p0 * m2; sred[26][t] = p0 * m1 - p1 * m0;
-        sred[27][t] = cost;
+        v[0] = w2 * M0; v[1] = w2 * M1; v[2] = w2 * M2; v[3] = w2 * M3; v[4] = w2 * M4; v[5] = w2 * M5;
+        v[6] = -w * Q00; v[7] = -w * Q01; v[8] = -w * Q02;
+        v[9] = -w * Q10; v[10] = -w * Q11; v[11] = -w * Q12;
+        v[12] = -w * Q20; v[13] = -w * Q21; v[14] = -w * Q22;
+        v[15] = p2 * Q10 - p1 * Q20; v[16] = p2 * Q11 - p1 * Q21; v[17] = p2 * Q12 - p1 * Q22;
+        v[18] = -p2 * Q01 + p0 * Q21; v[19] = -p2 * Q02 + p0 * Q22;
+        v[20] = p1 * Q02 - p0 * Q12;
+        v[21] = w * m0; v[22] = w * m1; v[23] = w * m2;
+        v[24] = p1 * m2 - p2 * m1; v[25] = p2 * m0 - p0 * m2; v[26] = p0 * m1 - p1 * m0;
+        v[27] = cost;
       } else {
 #pragma unroll
-        for (int e = 0; e < kLmRows; ++e) sred[e][t] = 0.0;
+        for (int e = 0; e < kLmRows; ++e) v[e] = 0.0;
 #pragma unroll
         for (int k = 0; k < 9; ++k) stg[k * L1_THREADS] = 0.0;
       }
-      // group reduction of the 28 values (fixed order -> deterministic): 4 threads per value, each sums 32 of the 128
-      // columns serially, then two shuffle steps combine the four partials
-      group_sync(g);
-      {
-        const int e = t >> 2, q = t & 3;
-        double s = 0.0;
-        if (e < kLmRows) {
-          const double* row = &sred[e][q * 32];
-#pragma unroll 8
-          for (int i = 0; i < 32; ++i) s += row[(i + 4 * q) & 31];     // rotated start: the four partial sums hit different banks
-        }
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        if (e < kLmRows && q == 0) rec[(size_t)f * kPartH + e] = s;
-      }
-      group_sync(g);
+#pragma unroll
+      for (int e = kLmRows; e < 32; ++e) v[e] = 0.0;
+      part[t] = warp_reduce_scatter32(v);      // part[32 w + e]: warp w's sum of value e
     }
-    // the round's blocks are staged: add them in frame order (buffer buf is rewritten two rounds later, after the
-    // next round's barrier, which the owner reaches only when these reads are done)
+    // the round's blocks and partials are staged (buffer buf is rewritten two rounds later, after the next round's
+    // barrier, which their readers reach only when these reads are done)
     if constexpr (CS > 1) cooperative_groups::this_cluster().sync();
     else __syncthreads();
+    if (walks && t < kLmRows) {      // warp 0 of the group: the four warps' partials in warp order
+      rec[(size_t)f * kPartH + t] = ((part[t] + part[32 + t]) + part[64 + t]) + part[96 + t];
+    }
     if (owner) {
       double v[9];
 #pragma unroll

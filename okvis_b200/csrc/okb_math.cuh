@@ -212,87 +212,96 @@ OKB_HD void cam_load(const okb_camera& c, CamIntr& o) {
   for (int i = 0; i < 8; ++i) o.k[i] = c.dist[i];
 }
 
+// Distortion model of a projection: one of OKB_DIST_* fixes it at compile time, kDistAny switches on CamIntr::model
+// at run time (unknown models project as OKB_DIST_NONE).  Kernels whose launch has one model across all cameras
+// instantiate that model and carry no registers for the others.
+constexpr int kDistAny = -1;
+
 // distortion of the normalised point u -> d and (optionally) its 2x2 Jacobian Jd (row-major).
 // Returns false where the reference's distort() fails (radtan8, rho > 9); outputs are then zero.
-template <bool WANT_J>
+template <bool WANT_J, int MODEL = kDistAny>
 OKB_HD bool distort(const CamIntr& c, double u0, double u1, double* d, double* Jd) {
-  switch (c.model) {
-    case OKB_DIST_RADTAN: {
-      const double k1 = c.k[0], k2 = c.k[1], p1 = c.k[2], p2 = c.k[3];
-      const double mx = u0 * u0, my = u1 * u1, mxy = u0 * u1, rho = mx + my;
-      const double rad = k1 * rho + k2 * rho * rho;
-      d[0] = u0 + u0 * rad + 2.0 * p1 * mxy + p2 * (rho + 2.0 * mx);
-      d[1] = u1 + u1 * rad + 2.0 * p2 * mxy + p1 * (rho + 2.0 * my);
-      if (WANT_J) {
-        Jd[0] = 1 + rad + k1 * 2.0 * mx + k2 * rho * 4 * mx + 2.0 * p1 * u1 + 6 * p2 * u0;
-        Jd[2] = k1 * 2.0 * u0 * u1 + k2 * 4 * rho * u0 * u1 + p1 * 2.0 * u0 + 2.0 * p2 * u1;
-        Jd[1] = Jd[2];
-        Jd[3] = 1 + rad + k1 * 2.0 * my + k2 * rho * 4 * my + 6 * p1 * u1 + 2.0 * p2 * u0;
-      }
-      return true;
+  if constexpr (MODEL == kDistAny) {
+    switch (c.model) {
+      case OKB_DIST_RADTAN: return distort<WANT_J, OKB_DIST_RADTAN>(c, u0, u1, d, Jd);
+      case OKB_DIST_EQUIDISTANT: return distort<WANT_J, OKB_DIST_EQUIDISTANT>(c, u0, u1, d, Jd);
+      case OKB_DIST_RADTAN8: return distort<WANT_J, OKB_DIST_RADTAN8>(c, u0, u1, d, Jd);
+      default: return distort<WANT_J, OKB_DIST_NONE>(c, u0, u1, d, Jd);
     }
-    case OKB_DIST_EQUIDISTANT: {
-      const double k1 = c.k[0], k2 = c.k[1], k3 = c.k[2], k4 = c.k[3];
-      const double r2 = u0 * u0 + u1 * u1;
-      const double r = sqrt(r2);
-      const double th = atan(r);
-      const double th2 = th * th, th4 = th2 * th2, th6 = th4 * th2, th8 = th4 * th4;
-      const double poly = 1 + k1 * th2 + k2 * th4 + k3 * th6 + k4 * th8;
-      const double thd = th * poly;
-      const bool big = r > 1e-8;
-      const double scaling = big ? thd / r : 1.0;
-      d[0] = scaling * u0; d[1] = scaling * u1;
-      if (WANT_J) {
-        if (big) {
-          // d = s(r) u, s = thd/r:  J = s I + (s'/r) u u^T,  s' = (dthd/dr * r - thd)/r^2,
-          // dthd/dr = (poly + th*dpoly/dth) / (1+r^2)   (same function the reference differentiates symbolically)
-          const double dpoly = 2 * k1 * th + 4 * k2 * th2 * th + 6 * k3 * th4 * th + 8 * k4 * th6 * th;
-          const double dthd = (poly + th * dpoly) / (1.0 + r2);
-          const double sp_over_r = (dthd * r - thd) / (r2 * r);
-          Jd[0] = scaling + sp_over_r * u0 * u0;
-          Jd[1] = sp_over_r * u0 * u1;
-          Jd[2] = Jd[1];
-          Jd[3] = scaling + sp_over_r * u1 * u1;
-        } else {
-          Jd[0] = 1; Jd[1] = 0; Jd[2] = 0; Jd[3] = 1;
-        }
-      }
-      return true;
+  } else if constexpr (MODEL == OKB_DIST_RADTAN) {
+    const double k1 = c.k[0], k2 = c.k[1], p1 = c.k[2], p2 = c.k[3];
+    const double mx = u0 * u0, my = u1 * u1, mxy = u0 * u1, rho = mx + my;
+    const double rad = k1 * rho + k2 * rho * rho;
+    d[0] = u0 + u0 * rad + 2.0 * p1 * mxy + p2 * (rho + 2.0 * mx);
+    d[1] = u1 + u1 * rad + 2.0 * p2 * mxy + p1 * (rho + 2.0 * my);
+    if (WANT_J) {
+      Jd[0] = 1 + rad + k1 * 2.0 * mx + k2 * rho * 4 * mx + 2.0 * p1 * u1 + 6 * p2 * u0;
+      Jd[2] = k1 * 2.0 * u0 * u1 + k2 * 4 * rho * u0 * u1 + p1 * 2.0 * u0 + 2.0 * p2 * u1;
+      Jd[1] = Jd[2];
+      Jd[3] = 1 + rad + k1 * 2.0 * my + k2 * rho * 4 * my + 6 * p1 * u1 + 2.0 * p2 * u0;
     }
-    case OKB_DIST_RADTAN8: {
-      const double k1 = c.k[0], k2 = c.k[1], p1 = c.k[2], p2 = c.k[3], k3 = c.k[4], k4 = c.k[5], k5 = c.k[6], k6 = c.k[7];
-      const double mx = u0 * u0, my = u1 * u1, mxy = u0 * u1, rho = mx + my;
-      if (rho > 9.0) {
-        d[0] = d[1] = 0.0;
-        if (WANT_J) { Jd[0] = Jd[1] = Jd[2] = Jd[3] = 0.0; }
-        return false;
-      }
-      const double num = 1.0 + ((k3 * rho + k2) * rho + k1) * rho;
-      const double den = 1.0 + ((k6 * rho + k5) * rho + k4) * rho;
-      const double rad = num / den;
-      d[0] = u0 * rad + 2.0 * p1 * mxy + p2 * (rho + 2.0 * mx);
-      d[1] = u1 * rad + 2.0 * p2 * mxy + p1 * (rho + 2.0 * my);
-      if (WANT_J) {
-        // d(rad)/d(rho) = (num' den - num den') / den^2 ; d(rho)/du = 2u
-        const double dnum = (3 * k3 * rho + 2 * k2) * rho + k1;
-        const double dden = (3 * k6 * rho + 2 * k5) * rho + k4;
-        const double drad = (dnum * den - num * dden) / (den * den);
-        Jd[0] = rad + 2 * u0 * u0 * drad + 2.0 * p1 * u1 + 6.0 * p2 * u0;
-        Jd[1] = 2 * u0 * u1 * drad + 2.0 * p1 * u0 + 2.0 * p2 * u1;
+    return true;
+  } else if constexpr (MODEL == OKB_DIST_EQUIDISTANT) {
+    const double k1 = c.k[0], k2 = c.k[1], k3 = c.k[2], k4 = c.k[3];
+    const double r2 = u0 * u0 + u1 * u1;
+    const double r = sqrt(r2);
+    const double th = atan(r);
+    const double th2 = th * th, th4 = th2 * th2, th6 = th4 * th2, th8 = th4 * th4;
+    const double poly = 1 + k1 * th2 + k2 * th4 + k3 * th6 + k4 * th8;
+    const double thd = th * poly;
+    const bool big = r > 1e-8;
+    const double scaling = big ? thd / r : 1.0;
+    d[0] = scaling * u0; d[1] = scaling * u1;
+    if (WANT_J) {
+      if (big) {
+        // d = s(r) u, s = thd/r:  J = s I + (s'/r) u u^T,  s' = (dthd/dr * r - thd)/r^2,
+        // dthd/dr = (poly + th*dpoly/dth) / (1+r^2)   (same function the reference differentiates symbolically)
+        const double dpoly = 2 * k1 * th + 4 * k2 * th2 * th + 6 * k3 * th4 * th + 8 * k4 * th6 * th;
+        const double dthd = (poly + th * dpoly) / (1.0 + r2);
+        const double sp_over_r = (dthd * r - thd) / (r2 * r);
+        Jd[0] = scaling + sp_over_r * u0 * u0;
+        Jd[1] = sp_over_r * u0 * u1;
         Jd[2] = Jd[1];
-        Jd[3] = rad + 2 * u1 * u1 * drad + 6.0 * p1 * u1 + 2.0 * p2 * u0;
+        Jd[3] = scaling + sp_over_r * u1 * u1;
+      } else {
+        Jd[0] = 1; Jd[1] = 0; Jd[2] = 0; Jd[3] = 1;
       }
-      return true;
     }
-    default:
-      d[0] = u0; d[1] = u1;
-      if (WANT_J) { Jd[0] = 1; Jd[1] = 0; Jd[2] = 0; Jd[3] = 1; }
-      return true;
+    return true;
+  } else if constexpr (MODEL == OKB_DIST_RADTAN8) {
+    const double k1 = c.k[0], k2 = c.k[1], p1 = c.k[2], p2 = c.k[3], k3 = c.k[4], k4 = c.k[5], k5 = c.k[6], k6 = c.k[7];
+    const double mx = u0 * u0, my = u1 * u1, mxy = u0 * u1, rho = mx + my;
+    if (rho > 9.0) {
+      d[0] = d[1] = 0.0;
+      if (WANT_J) { Jd[0] = Jd[1] = Jd[2] = Jd[3] = 0.0; }
+      return false;
+    }
+    const double num = 1.0 + ((k3 * rho + k2) * rho + k1) * rho;
+    const double den = 1.0 + ((k6 * rho + k5) * rho + k4) * rho;
+    const double rad = num / den;
+    d[0] = u0 * rad + 2.0 * p1 * mxy + p2 * (rho + 2.0 * mx);
+    d[1] = u1 * rad + 2.0 * p2 * mxy + p1 * (rho + 2.0 * my);
+    if (WANT_J) {
+      // d(rad)/d(rho) = (num' den - num den') / den^2 ; d(rho)/du = 2u
+      const double dnum = (3 * k3 * rho + 2 * k2) * rho + k1;
+      const double dden = (3 * k6 * rho + 2 * k5) * rho + k4;
+      const double drad = (dnum * den - num * dden) / (den * den);
+      Jd[0] = rad + 2 * u0 * u0 * drad + 2.0 * p1 * u1 + 6.0 * p2 * u0;
+      Jd[1] = 2 * u0 * u1 * drad + 2.0 * p1 * u0 + 2.0 * p2 * u1;
+      Jd[2] = Jd[1];
+      Jd[3] = rad + 2 * u1 * u1 * drad + 6.0 * p1 * u1 + 2.0 * p2 * u0;
+    }
+    return true;
+  } else {
+    static_assert(MODEL == OKB_DIST_NONE, "unknown distortion model");
+    d[0] = u0; d[1] = u1;
+    if (WANT_J) { Jd[0] = 1; Jd[1] = 0; Jd[2] = 0; Jd[3] = 1; }
+    return true;
   }
 }
 
 // PinholeCamera::project (+ point Jacobian 2x3 row-major).  Singular depth -> zeros, false.
-template <bool WANT_J>
+template <bool WANT_J, int MODEL = kDistAny>
 OKB_HD bool project(const CamIntr& c, const double* pt, double* ip, double* J) {
   if (fabs(pt[2]) < 1.0e-12) {
     ip[0] = ip[1] = 0.0;
@@ -302,7 +311,7 @@ OKB_HD bool project(const CamIntr& c, const double* pt, double* ip, double* J) {
   const double rz = 1.0 / pt[2];
   const double u0 = pt[0] * rz, u1 = pt[1] * rz;
   double d[2], Jd[4];
-  const bool ok = distort<WANT_J>(c, u0, u1, d, Jd);
+  const bool ok = distort<WANT_J, MODEL>(c, u0, u1, d, Jd);
   if (WANT_J) {
     const double rz2 = rz * rz;
     J[0] = c.fu * Jd[0] * rz;
@@ -341,7 +350,7 @@ OKB_HD void make_slot_xf(const double* pose, const double* ext, SlotXf& o) {
 // One observation.  Outputs the raw (sqrt-information weighted, NOT robustified) residual r and
 // A = sqrtInfo * dproj * C_CW (2x3 row-major; zero if the point is "invalid" exactly as the
 // reference zeroes its Jacobians).  Returns hp_C.w (needed by nobody else) via *w_out if non-null.
-template <bool WANT_J>
+template <bool WANT_J, int MODEL = kDistAny>
 OKB_HD void reproj_slot(const SlotXf& xf, const CamIntr& cam, const double* X /*hom. landmark*/, double z0, double z1,
                         double sqrt_info, double* r, double* A) {
   const double w = X[3];
@@ -357,7 +366,10 @@ OKB_HD void reproj_slot(const SlotXf& xf, const CamIntr& cam, const double* X /*
   double pt[3] = {pc[0], pc[1], pc[2]};
   if (w < 0) { pt[0] = -pt[0]; pt[1] = -pt[1]; pt[2] = -pt[2]; }
   double ip[2], Jp[6];
-  project<WANT_J>(cam, pt, ip, Jp);
+  project<WANT_J, MODEL>(cam, pt, ip, Jp);
+#ifdef __CUDA_ARCH__
+  asm volatile("" ::: "memory");      // R is read again below rather than held in registers across the projection
+#endif
   r[0] = sqrt_info * (z0 - ip[0]);
   r[1] = sqrt_info * (z1 - ip[1]);
   if (WANT_J) {
