@@ -409,6 +409,28 @@ int okb_detect_describe(okb_ctx* ctx, int cam_slot, const uint8_t* img, int widt
                         const okb_camera* cam, const double R_CW[9], const okb_detect_params* params,
                         okb_keypoint* out_kp, uint8_t* out_desc, int max_out, int* n_out);
 
+/* One camera image of a batch (Frontend::detectAndDescribe for one camera of one session). */
+typedef struct okb_image_desc {
+  const uint8_t* img;              /* host, row stride `stride` bytes */
+  int32_t width, height, stride, _pad;
+  okb_camera cam;                  /* geometry for the orientation (Frame::describe) */
+  double R_CW[9];                  /* as okb_detect_describe */
+} okb_image_desc;
+
+/* n_images images (n_images <= 65535), one parameter set.  out_kp [n_images][max_out],
+ * out_desc [n_images][max_out][desc_bytes], n_out [n_images].  Per image the result is bit-identical to
+ * okb_detect_describe on that image.  Images may differ in size, stride, camera and R_CW.  An image with more NMS
+ * candidates than the detector holds gets n_out = -1 and the call returns OKB_ERR_CAPACITY; every other image's
+ * outputs are still written.  Arguments are checked per image before any device work (OKB_ERR_INVALID_ARG);
+ * n_images == 0 is a no-op.  The batch runs on a stream of its own (not the solver's), blocks until done, and is
+ * serialised with other batch calls on the context; it may run beside okb_detect_describe on the camera slots.
+ * Device and pinned buffers grow to the largest batch seen and are kept; a call that has to grow them frees the old
+ * ones, which waits for all work on the device (an okb_optimize_async in flight included).  Issue one batch of the
+ * largest size first to size them.
+ * host_threads: host packing threads (<= 0: library default), as okb_window_upload_batch. */
+int okb_detect_describe_batch(okb_ctx* ctx, int n_images, const okb_image_desc* images, const okb_detect_params* params,
+                              okb_keypoint* out_kp, uint8_t* out_desc, int max_out, int32_t* n_out, int host_threads);
+
 typedef struct okb_pair {          /* DenseMatcher::Pairing */
   int32_t index_a;                 /* -1 = B element unmatched */
   float distance;
@@ -455,6 +477,22 @@ typedef struct okb_match_gate {
 int okb_hamming_match_gated(okb_ctx* ctx, const uint8_t* A, int nA, const uint8_t* B, int nB, int desc_bytes,
                             const uint8_t* skipA, const uint8_t* skipB, float threshold, int num_best, int use_ratio,
                             float ratio_threshold, const okb_match_gate* gate, okb_pair* out_topk, okb_pair* out_pairs);
+
+/* One DenseMatcher::match of a batch.  gate == NULL: plain Hamming (okb_hamming_match); else as
+ * okb_hamming_match_gated.  use_ratio as there (the ratio test itself stays with the caller). */
+typedef struct okb_match_job {
+  const uint8_t *A, *B, *skipA, *skipB;   /* skip* may be NULL */
+  int32_t nA, nB;
+  float threshold;
+  int32_t num_best, use_ratio, _pad;
+  const okb_match_gate* gate;
+  okb_pair* out_topk;                     /* [nA][num_best] or NULL */
+  okb_pair* out_pairs;                    /* [nB] */
+} okb_match_job;
+/* n_jobs matches with one descriptor length.  Per job the outputs equal the single call's; plain, 3D-2D and 2D-2D
+ * jobs may share a call, and jobs with nA == 0 or nB == 0 are answered on the host.  Arguments are checked per job
+ * before any device work.  Runs on the batch stream (see okb_detect_describe_batch), blocking. */
+int okb_hamming_match_batch(okb_ctx* ctx, int n_jobs, const okb_match_job* jobs, int desc_bytes);
 
 /* Candidate-list mode for the production (geometry-gated) matching algorithm: for every A, every B
  * with Hamming distance < threshold in ascending B order, CSR layout.  row_ptr [nA+1];

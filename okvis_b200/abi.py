@@ -100,6 +100,17 @@ def make_match_gate(mode, kp_b, kp_size_b, proj_into_b=None, proj_uncertainty=No
     return g
 
 
+class ImageDesc(C.Structure):
+    _fields_ = [("img", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("stride", C.c_int32), ("_pad", C.c_int32),
+                ("cam", Camera), ("R_CW", C.c_double * 9)]
+
+
+class MatchJob(C.Structure):
+    _fields_ = [("A", C.c_void_p), ("B", C.c_void_p), ("skipA", C.c_void_p), ("skipB", C.c_void_p), ("nA", C.c_int32),
+                ("nB", C.c_int32), ("threshold", C.c_float), ("num_best", C.c_int32), ("use_ratio", C.c_int32), ("_pad", C.c_int32),
+                ("gate", C.POINTER(MatchGate)), ("out_topk", C.c_void_p), ("out_pairs", C.c_void_p)]
+
+
 class WindowDesc(C.Structure):
     _fields_ = [("n_poses", C.c_int32), ("n_speed_bias", C.c_int32), ("n_extrinsics", C.c_int32),
                 ("n_landmarks", C.c_int32), ("n_cameras", C.c_int32), ("n_obs", C.c_int32),

@@ -406,6 +406,70 @@ class Context:
                                               C.byref(prm), _p(kps), _p(desc), max_keypoints, C.byref(n)))
         return kps[:n.value].copy(), desc[:n.value].copy()
 
+    def detect_describe_batch(self, imgs, cams, R_CWs, uniformity_radius=40.0, absolute_threshold=800.0, max_keypoints=400,
+                              desc_bytes=48, rotation_invariance=True, host_threads=0, return_status=False):
+        """okb_detect_describe_batch: one (keypoints, descriptors) per image, each equal to detect_describe on it.
+        `imgs` are 2-D uint8 arrays (rows may be strided).  With return_status the call returns (results, status) instead
+        of raising OKB_ERR_CAPACITY; an image over the candidate capacity then gives None."""
+        n = len(imgs)
+        prm = abi.DetectParams()
+        prm.uniformity_radius, prm.absolute_threshold = uniformity_radius, absolute_threshold
+        prm.max_keypoints, prm.desc_bytes, prm.rotation_invariance = max_keypoints, desc_bytes, int(rotation_invariance)
+        descs = (abi.ImageDesc * max(n, 1))()
+        keep = []
+        for i, (img, cam, R) in enumerate(zip(imgs, cams, R_CWs)):
+            img = np.asarray(img, dtype=np.uint8)
+            if img.strides[1] != 1:
+                img = np.ascontiguousarray(img)
+            keep.append(img)
+            d = descs[i]
+            d.img = img.ctypes.data
+            d.height, d.width = img.shape
+            d.stride = img.strides[0]
+            C.memmove(C.addressof(d.cam), np.array([cam], abi.camera_dtype).ctypes.data, C.sizeof(abi.Camera))
+            for k, v in enumerate(np.asarray(R, dtype=np.float64).reshape(9)):
+                d.R_CW[k] = float(v)
+        kps = np.zeros((n, max_keypoints), abi.keypoint_dtype)
+        desc = np.zeros((n, max_keypoints, desc_bytes), np.uint8)
+        n_out = np.zeros(n, np.int32)
+        rc = lib().okb_detect_describe_batch(self._h, n, descs, C.byref(prm), _p(kps), _p(desc), max_keypoints, _p(n_out),
+                                             int(host_threads))
+        if rc != 0 and not (return_status and rc == abi.OKB_ERR_CAPACITY):
+            self._check(rc)
+        out = [(kps[i, :m].copy(), desc[i, :m].copy()) if m >= 0 else None for i, m in enumerate(n_out.tolist())]
+        return (out, rc) if return_status else out
+
+    @staticmethod
+    def make_match_job(A, B, skipA=None, skipB=None, threshold=60.0, num_best=4, use_ratio=False, gate=None, want_topk=True):
+        """One okb_match_job over numpy arrays; its output arrays are job.topk (or None) and job.pairs."""
+        A = np.ascontiguousarray(A, dtype=np.uint8)
+        B = np.ascontiguousarray(B, dtype=np.uint8)
+        sa = np.ascontiguousarray(skipA, dtype=np.uint8) if skipA is not None else None
+        sb = np.ascontiguousarray(skipB, dtype=np.uint8) if skipB is not None else None
+        j = abi.MatchJob()
+        j.A, j.B = A.ctypes.data, B.ctypes.data
+        j.skipA = sa.ctypes.data if sa is not None else None
+        j.skipB = sb.ctypes.data if sb is not None else None
+        j.nA, j.nB, j.threshold, j.num_best, j.use_ratio = A.shape[0], B.shape[0], threshold, num_best, int(use_ratio)
+        if gate is not None:
+            j.gate = C.pointer(gate)
+        j.topk = np.zeros((A.shape[0], num_best), abi.pair_dtype) if want_topk else None
+        j.pairs = np.zeros(B.shape[0], abi.pair_dtype)
+        j.out_topk = j.topk.ctypes.data if want_topk else None
+        j.out_pairs = j.pairs.ctypes.data
+        j._keep = (A, B, sa, sb, gate)
+        return j
+
+    def hamming_match_batch(self, jobs, desc_bytes):
+        """okb_hamming_match_batch over `jobs`: make_match_job results, or dicts of its keyword arguments.  Returns one
+        dict(topk, pairs) per job, like hamming_match / hamming_match_gated."""
+        jobs = [j if isinstance(j, abi.MatchJob) else self.make_match_job(**j) for j in jobs]
+        arr = (abi.MatchJob * max(len(jobs), 1))()
+        for i, j in enumerate(jobs):
+            arr[i] = j
+        self._check(lib().okb_hamming_match_batch(self._h, len(jobs), arr, int(desc_bytes)))
+        return [dict(topk=j.topk, pairs=j.pairs) for j in jobs]
+
 
 def matches_from_pairs(pairs, topk, threshold, use_ratio=False, ratio_threshold=3.0):
     """The serial epilogue of DenseMatcher::matchBody (DenseMatcher.hpp(impl):97-122): turns the per-B

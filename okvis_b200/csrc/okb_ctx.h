@@ -99,3 +99,4 @@ struct okb_ctx {
 };
 
 void okb_frontend_release(okb_ctx* c);
+int64_t okb_frontend_launches(const okb_ctx* c);   // kernel launches of the frontend calls (counted atomically)

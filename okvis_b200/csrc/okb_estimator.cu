@@ -151,7 +151,7 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
 }
 
 extern "C" const char* okb_last_error(const okb_ctx* c) { return c ? c->error.c_str() : g_create_error.c_str(); }
-extern "C" int64_t okb_kernel_launches(const okb_ctx* c) { return c ? c->launches : 0; }
+extern "C" int64_t okb_kernel_launches(const okb_ctx* c) { return c ? c->launches + okb_frontend_launches(c) : 0; }
 extern "C" void* okb_stream(const okb_ctx* c) { return c ? (void*)c->stream : nullptr; }
 
 // ---------------------------------------------------------------------------------------------

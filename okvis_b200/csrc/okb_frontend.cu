@@ -10,10 +10,13 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <atomic>
 #include <mutex>
+#include <thread>
 #include <vector>
 
 #include "okb_ctx.h"
@@ -85,36 +88,74 @@ Pattern make_pattern(int desc_bytes) {
   return P;
 }
 
-struct SlotBuffers {
-  cudaStream_t stream = nullptr;
-  int W = 0, H = 0;
-  uint8_t* d_img = nullptr;
+// One image of a detect launch (device table, one entry per image): its geometry, its gravity direction and where
+// its data lie in the launch's buffers.
+struct FeImage {
+  okb_camera cam;
+  double gC[3];                 // gravity direction in the camera frame: R_CW * (0,0,-1)
+  unsigned long long img;       // byte offset of the packed image (row stride W) in the input buffer
+  unsigned long long px;        // element offset of its score plane (cumulative W * H)
+  unsigned long long ii;        // element offset of its integral image (cumulative (W + 1) * (H + 1))
+  unsigned long long uni;       // word offset of its global-memory uniformity scratch (sized by its own cell grid)
+  int W, H, max_cells;
+};
+
+// Buffers of a detect launch over n images; they grow with the launch and are kept across calls.  A camera slot owns
+// one set (n = 1), the batch call another.
+struct DetectBuffers {
+  uint8_t* h_in = nullptr;         // pinned: [FeImage table | packed images], one H2D copy
+  uint8_t* d_in = nullptr;
+  size_t h_in_cap = 0, d_in_cap = 0;
   int32_t* d_score = nullptr;
   uint32_t* d_integral = nullptr;
-  unsigned long long* d_keys = nullptr;
-  int* d_count = nullptr;          // [0] candidates, [1] accepted
-  uint32_t *d_cell_start = nullptr, *d_cell_cur = nullptr, *d_order = nullptr, *d_acc = nullptr;   // uniformity scratch
-  uint32_t* d_rounds = nullptr;      // [4][kMaxCand]: blocker | alive list 0 | alive list 1 | pending
-  uint8_t* d_state = nullptr;
-  int max_cells = 0;
-  okb_keypoint* d_kp = nullptr;
-  uint8_t* d_desc = nullptr;
-  int kp_cap = 0, desc_cap = 0;
-  uint8_t* h_img = nullptr;        // pinned
-  okb_keypoint* h_kp = nullptr;    // pinned
-  uint8_t* h_desc = nullptr;       // pinned
-  int* h_count = nullptr;          // pinned
+  unsigned long long* d_keys = nullptr;    // [n][kMaxCand]
+  uint32_t* d_uni = nullptr;       // [n][uni_stride]: global-memory uniformity scratch (UniScratch)
+  uint8_t* d_state = nullptr;      // [n][kMaxCand]
+  size_t cap_score = 0, cap_integral = 0, cap_keys = 0, cap_uni = 0, cap_state = 0;
+  uint8_t* d_out = nullptr;        // [counts n x 4 | keypoints n x maxk | descriptors n x maxk x desc_bytes], one D2H copy
+  uint8_t* h_out = nullptr;        // pinned mirror
+  size_t d_out_cap = 0, h_out_cap = 0;
+  void release() {
+    if (h_in) cudaFreeHost(h_in);
+    if (h_out) cudaFreeHost(h_out);
+    cudaFree(d_in); cudaFree(d_score); cudaFree(d_integral); cudaFree(d_keys); cudaFree(d_uni); cudaFree(d_state); cudaFree(d_out);
+  }
+};
+
+struct DevPattern {
+  int* half = nullptr;
+  uint8_t *pi = nullptr, *pj = nullptr;
+  int16_t* lut = nullptr;
+};
+
+struct SlotBuffers {
+  cudaStream_t stream = nullptr;
+  DetectBuffers buf;
   std::mutex mtx;
+};
+
+// Buffers of a matcher launch: one pinned staging buffer and its device mirror (inputs in, top-k lists + winners out).
+struct MatchIO {
+  uint8_t* h_stage = nullptr;
+  size_t h_stage_cap = 0;
+  uint8_t* d_io = nullptr;
+  size_t d_io_cap = 0;
+  void release() {
+    if (h_stage) cudaFreeHost(h_stage);
+    cudaFree(d_io);
+  }
 };
 }  // namespace
 
 struct okb_frontend_state {
   SlotBuffers slots[kMaxSlots];
+  // batch calls: a stream of their own (never c->stream, so a batch does not queue behind a solve) and their buffers
+  cudaStream_t batch_stream = nullptr;
+  DetectBuffers batch_det;
+  MatchIO batch_match;
+  std::mutex batch_mtx;
   // pattern (device), per descriptor length
-  int pat_bytes = 0;
-  int* d_half = nullptr;
-  uint8_t *d_pi = nullptr, *d_pj = nullptr;
-  int16_t* d_lut = nullptr;
+  DevPattern pats[128 / 4 + 1];       // indexed by desc_bytes / 4
   std::mutex pat_mtx;
   // matcher buffers
   uint8_t *d_A = nullptr, *d_B = nullptr, *d_skipA = nullptr, *d_skipB = nullptr;
@@ -124,34 +165,30 @@ struct okb_frontend_state {
   uint32_t *d_rowptr = nullptr, *d_col = nullptr;
   uint16_t* d_dist = nullptr;
   size_t cap_rows = 0, cap_cand = 0;
-  uint8_t* h_stage = nullptr;      // pinned staging: descriptors in, top-k lists + winners out
-  size_t h_stage_cap = 0;
-  uint8_t* d_io = nullptr;         // device mirror of the staging buffer
-  size_t d_io_cap = 0;
+  MatchIO match_io;                // okb_hamming_match / _gated (on c->stream, under match_mtx)
+  std::atomic<int64_t> launches{0};   // frontend kernel launches (okb_kernel_launches adds them to the solver's)
   std::mutex match_mtx;
 };
 
 void okb_frontend_release(okb_ctx* c) {
   if (!c->frontend) return;
   okb_frontend_state* F = c->frontend;
-  if (F->h_stage) cudaFreeHost(F->h_stage);
-  cudaFree(F->d_io);
+  F->match_io.release();
+  F->batch_match.release();
+  F->batch_det.release();
+  if (F->batch_stream) cudaStreamDestroy(F->batch_stream);
   for (auto& s : F->slots) {
     if (s.stream) cudaStreamDestroy(s.stream);
-    cudaFree(s.d_img); cudaFree(s.d_score); cudaFree(s.d_integral); cudaFree(s.d_keys);
-    cudaFree(s.d_cell_start); cudaFree(s.d_cell_cur); cudaFree(s.d_order); cudaFree(s.d_acc); cudaFree(s.d_state); cudaFree(s.d_rounds);
-    cudaFree(s.d_count); cudaFree(s.d_kp); cudaFree(s.d_desc);
-    if (s.h_img) cudaFreeHost(s.h_img);
-    if (s.h_kp) cudaFreeHost(s.h_kp);
-    if (s.h_desc) cudaFreeHost(s.h_desc);
-    if (s.h_count) cudaFreeHost(s.h_count);
+    s.buf.release();
   }
-  cudaFree(F->d_half); cudaFree(F->d_pi); cudaFree(F->d_pj); cudaFree(F->d_lut);
+  for (auto& p : F->pats) { cudaFree(p.half); cudaFree(p.pi); cudaFree(p.pj); cudaFree(p.lut); }
   cudaFree(F->d_A); cudaFree(F->d_B); cudaFree(F->d_skipA); cudaFree(F->d_skipB); cudaFree(F->d_topk); cudaFree(F->d_pairs);
   cudaFree(F->d_rowptr); cudaFree(F->d_col); cudaFree(F->d_dist);
   delete F;
   c->frontend = nullptr;
 }
+
+int64_t okb_frontend_launches(const okb_ctx* c) { return c->frontend ? c->frontend->launches.load() : 0; }
 
 static okb_frontend_state* fe(okb_ctx* c) {
   static std::mutex m;
@@ -167,11 +204,18 @@ namespace {
 constexpr int HT_X = 32, HT_Y = 8;
 
 // Integer Harris score: Scharr gradients, 5x5 binomial window.  One thread per pixel; the tile's
-// gradient products live in shared memory.
-__global__ void __launch_bounds__(HT_X* HT_Y) k_harris(const uint8_t* __restrict__ img, int W, int H, int32_t* __restrict__ score) {
+// gradient products live in shared memory.  blockIdx.z is the image; the grid covers the largest image of the launch
+// and the tiles outside an image exit (the detector kernels below all index images the same way).
+__global__ void __launch_bounds__(HT_X* HT_Y) k_harris(const FeImage* __restrict__ tab, const uint8_t* __restrict__ in,
+                                                       int32_t* __restrict__ score_all) {
   __shared__ uint8_t tile[HT_Y + 6][HT_X + 6 + 2];
   __shared__ int32_t sxx[HT_Y + 4][HT_X + 4], syy[HT_Y + 4][HT_X + 4], sxy[HT_Y + 4][HT_X + 4];
+  const FeImage& im = tab[blockIdx.z];
+  const int W = im.W, H = im.H;
   const int bx = blockIdx.x * HT_X, by = blockIdx.y * HT_Y;
+  if (bx >= W || by >= H) return;
+  const uint8_t* __restrict__ img = in + im.img;
+  int32_t* __restrict__ score = score_all + im.px;
   const int tid = threadIdx.y * HT_X + threadIdx.x;
   for (int i = tid; i < (HT_Y + 6) * (HT_X + 6); i += HT_X * HT_Y) {
     const int ty = i / (HT_X + 6), tx = i % (HT_X + 6);
@@ -220,9 +264,16 @@ __global__ void __launch_bounds__(HT_X* HT_Y) k_harris(const uint8_t* __restrict
 }
 
 // 3x3 strict NMS + threshold + border -> sortable 64-bit keys (score desc, raster index asc)
-__global__ void k_nms(const int32_t* __restrict__ score, int W, int H, int32_t thr, unsigned long long* keys, int* count, int cap) {
+// (per image: keys [cap], candidate count at count[0] of its 4-int record)
+__global__ void k_nms(const FeImage* __restrict__ tab, const int32_t* __restrict__ score_all, int32_t thr, unsigned long long* keys_all,
+                      int* count_all, int cap) {
+  const FeImage& im = tab[blockIdx.z];
+  const int W = im.W, H = im.H;
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x < kBorder || x >= W - kBorder || y < kBorder || y >= H - kBorder) return;
+  const int32_t* __restrict__ score = score_all + im.px;
+  unsigned long long* keys = keys_all + (size_t)blockIdx.z * cap;
+  int* count = count_all + 4 * blockIdx.z;
   const int32_t s = score[(size_t)y * W + x];
   if (s < thr) return;
   bool mx = true;
@@ -245,7 +296,7 @@ __global__ void k_nms(const int32_t* __restrict__ score, int W, int H, int32_t t
 // accepted, accepted candidates kill their live neighbours (Blelloch et al.'s deterministic parallel MIS -- the result
 // is identical to the sequential greedy order, not merely equivalent).  Neighbours are found through a bucket grid
 // (cell size >= radius: 3x3 cells).  The accepted set is then ranked by counting (score order) and cut at max_kp.
-// One CTA of 1024 threads per image; all scratch lives in global memory.
+// One CTA of 1024 threads per image (blockIdx.x); all scratch lives in global memory, one UniScratch per image.
 constexpr int UT = 1024;
 constexpr int UNI_SN = 6144, UNI_SC = UNI_SN / 2;      // candidates / cells the shared-memory kernel holds
 __host__ __device__ inline bool uni_fits_smem(int n, int n_cells) { return n <= UNI_SN && n_cells <= UNI_SC; }
@@ -256,8 +307,19 @@ struct UniScratch {
   uint8_t* state;         // [cap] 0 alive, 1 pending, 2 accepted, 3 dead
   uint32_t* acc;          // [cap] accepted candidates
   uint32_t *blocker, *list0, *list1, *pend;   // [cap] each: rounds scratch
-  int max_cells;
 };
+// u32 words of one image's scratch (offsets in FeImage::uni): cell_start | cell_cur | order | acc | blocker | list0 | list1 | pend (state apart)
+__host__ __device__ inline size_t uni_stride(int max_cells, int cap) { return 2 * (size_t)max_cells + 1 + 6 * (size_t)cap; }
+__device__ inline UniScratch uni_scratch(uint32_t* base, uint8_t* state, int max_cells, int cap, int img) {
+  UniScratch s;
+  s.cell_start = base;
+  s.cell_cur = s.cell_start + max_cells + 1;
+  s.order = s.cell_cur + max_cells;
+  s.acc = s.order + cap;
+  s.blocker = s.acc + cap; s.list0 = s.blocker + cap; s.list1 = s.list0 + cap; s.pend = s.list1 + cap;
+  s.state = state + (size_t)img * cap;
+  return s;
+}
 __device__ __forceinline__ int uni_block_scan(int v, int* s_warp, int* total) {     // exclusive scan over the CTA
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int x = v;
@@ -277,15 +339,21 @@ __device__ __forceinline__ int uni_block_scan(int v, int* s_warp, int* total) { 
   *total = s_warp[31];
   return base + x - v;
 }
-__global__ void __launch_bounds__(UT) k_uniformity(const unsigned long long* __restrict__ keys, const int* __restrict__ count, int cap,
-                                                   int W, int H, double radius, int max_kp, UniScratch sc, okb_keypoint* kps, int* n_out) {
+__global__ void __launch_bounds__(UT, 2) k_uniformity(const FeImage* __restrict__ tab, const unsigned long long* __restrict__ keys_all,
+                                                   int* count_all, int cap, double radius, int max_kp, uint32_t* uni_base,
+                                                   uint8_t* uni_state, okb_keypoint* kps_all) {
   __shared__ int s_warp[32];
   __shared__ int s_n;
   const int tid = threadIdx.x;
-  const int n = min(*count, cap);
+  const int W = tab[blockIdx.x].W, H = tab[blockIdx.x].H;
+  const unsigned long long* __restrict__ keys = keys_all + (size_t)blockIdx.x * cap;
+  int* n_out = count_all + 4 * blockIdx.x + 1;
+  okb_keypoint* kps = kps_all + (size_t)blockIdx.x * max_kp;
+  const int n = min(n_out[-1], cap);
   const int cs = max(4, (int)ceil(radius));
   const int gw = (W + cs - 1) / cs, gh = (H + cs - 1) / cs, n_cells = gw * gh;
   if (uni_fits_smem(n, n_cells)) return;       // k_uniformity_smem (launched next) does this image
+  const UniScratch sc = uni_scratch(uni_base + tab[blockIdx.x].uni, uni_state, tab[blockIdx.x].max_cells, cap, blockIdx.x);
   const long long r2i = (long long)ceil(radius * radius - 1e-9);     // integer test: dx^2 + dy^2 < radius^2
   auto px = [&](int i, int& x, int& y) { const uint32_t idx = 0xFFFFFFFFu - (uint32_t)(keys[i] & 0xFFFFFFFFull); x = (int)(idx % (uint32_t)W); y = (int)(idx / (uint32_t)W); };
   // ---- bucket grid (counting sort by cell)
@@ -421,14 +489,18 @@ __device__ unsigned long long g_uni_prof[8];     // cycles of thread 0 per phase
 #else
 #define UNI_MARK(i) do { } while (0)
 #endif
-__global__ void __launch_bounds__(UT) k_uniformity_smem(const unsigned long long* __restrict__ keys, const int* __restrict__ count, int cap,
-                                                        int W, int H, double radius, int max_kp, okb_keypoint* kps, int* n_out) {
+__global__ void __launch_bounds__(UT) k_uniformity_smem(const FeImage* __restrict__ tab, const unsigned long long* __restrict__ keys_all,
+                                                        int* count_all, int cap, double radius, int max_kp, okb_keypoint* kps_all) {
   extern __shared__ __align__(16) unsigned char uni_raw[];
   UniSmem& S = *reinterpret_cast<UniSmem*>(uni_raw);
   __shared__ int s_warp[32];
   __shared__ int s_n, s_alive, s_pend;
   const int tid = threadIdx.x;
-  const int n = min(*count, cap);
+  const int W = tab[blockIdx.x].W, H = tab[blockIdx.x].H;
+  const unsigned long long* __restrict__ keys = keys_all + (size_t)blockIdx.x * cap;
+  int* n_out = count_all + 4 * blockIdx.x + 1;
+  okb_keypoint* kps = kps_all + (size_t)blockIdx.x * max_kp;
+  const int n = min(n_out[-1], cap);
   const int cs = max(4, (int)ceil(radius));
   const int gw = (W + cs - 1) / cs, gh = (H + cs - 1) / cs, n_cells = gw * gh;
   if (!uni_fits_smem(n, n_cells)) return;
@@ -583,11 +655,15 @@ __global__ void __launch_bounds__(UT) k_uniformity_smem(const unsigned long long
 // integral image (H+1) x (W+1), uint32
 // row pass: one warp per image row, 32 pixels per step (warp inclusive scan + running carry): coalesced byte loads
 // and 128-byte stores
-__global__ void __launch_bounds__(128) k_integral_rows(const uint8_t* __restrict__ img, int W, int H, uint32_t* II) {
+// (blockIdx.y: image)
+__global__ void __launch_bounds__(128) k_integral_rows(const FeImage* __restrict__ tab, const uint8_t* __restrict__ in, uint32_t* II_all) {
+  const FeImage& im = tab[blockIdx.y];
+  const int W = im.W, H = im.H;
   const int y = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (y > H) return;
-  uint32_t* row = II + (size_t)y * (W + 1);
+  const uint8_t* __restrict__ img = in + im.img;
+  uint32_t* row = II_all + im.ii + (size_t)y * (W + 1);
   if (y == 0) { for (int x = lane; x <= W; x += 32) row[x] = 0; return; }
   if (lane == 0) row[0] = 0;
   const uint8_t* src = img + (size_t)(y - 1) * W;
@@ -606,10 +682,14 @@ __global__ void __launch_bounds__(128) k_integral_rows(const uint8_t* __restrict
 }
 // column pass: a CTA owns 32 columns; its 16 warps split the rows into 16 segments (lanes = columns: every access is a
 // 128-byte row).  Pass 1 sums each segment, the segment offsets are combined through shared memory, pass 2 writes the
-// running sums.  Integer arithmetic: any summation order gives the same bits.
+// running sums.  Integer arithmetic: any summation order gives the same bits.  blockIdx.y: image.
 constexpr int IC_SEG = 16;
-__global__ void __launch_bounds__(32 * IC_SEG) k_integral_cols(int W, int H, uint32_t* II) {
+__global__ void __launch_bounds__(32 * IC_SEG) k_integral_cols(const FeImage* __restrict__ tab, uint32_t* II_all) {
   __shared__ uint32_t seg[IC_SEG][33];
+  const FeImage& im = tab[blockIdx.y];
+  const int W = im.W, H = im.H;
+  if (blockIdx.x * 32 > W) return;
+  uint32_t* II = II_all + im.ii;
   const int lane = threadIdx.x & 31, s_ = threadIdx.x >> 5;
   const int x = blockIdx.x * 32 + lane;
   const int rows = H + 1, per = (rows + IC_SEG - 1) / IC_SEG;
@@ -644,33 +724,46 @@ __device__ void undistort_gn(const CamIntr& cam, double d0, double d1, double* p
   pu[0] = x0; pu[1] = x1;
 }
 
-// warp per keypoint: gravity angle, 60 box-smoothed samples, 8*desc_bytes comparisons via ballot
-__global__ void __launch_bounds__(128) k_describe(const uint32_t* __restrict__ II, int W, int H, okb_camera camera, const double* gC,
-                                                  int rot_inv, const int* __restrict__ half, const uint8_t* __restrict__ pi,
+// Orientation exactly as Frame::describe (Frame.hpp(impl):128-151), thread per keypoint: back-project (5 Gauss-Newton
+// undistort iterations), project with Jacobian, atan2 of the projected gravity direction, in degrees, into
+// keypoint.angle.  blockIdx.y: image (its camera and gravity direction come from its table entry).  Launched only with
+// rotation invariance; k_describe reads the angle back.
+__global__ void __launch_bounds__(128) k_orient(const FeImage* __restrict__ tab, okb_keypoint* kps_all, int max_kp, const int* count_all) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= count_all[4 * blockIdx.y + 1]) return;
+  const FeImage& im = tab[blockIdx.y];
+  okb_keypoint& kp = kps_all[(size_t)blockIdx.y * max_kp + k];
+  const int x = (int)kp.x, y = (int)kp.y;
+  CamIntr cam;
+  cam_load(im.cam, cam);
+  const double* gC = im.gC;
+  double pu[2];
+  undistort_gn(cam, ((double)x - cam.cu) / cam.fu, ((double)y - cam.cv) / cam.fv, pu);
+  const double ep[3] = {pu[0], pu[1], 1.0};
+  double ip[2], J[6];
+  project<true>(cam, ep, ip, J);
+  const double e0 = J[0] * gC[0] + J[1] * gC[1] + J[2] * gC[2];
+  const double e1 = J[3] * gC[0] + J[4] * gC[1] + J[5] * gC[2];
+  kp.angle = (float)(atan2(e1, e0) / 3.14159265358979323846 * 180.0);
+}
+
+// warp per keypoint: 60 box-smoothed samples rotated by the keypoint's angle (k_orient, or 0), 8*desc_bytes
+// comparisons via ballot.  blockIdx.y: image.
+__global__ void __launch_bounds__(128) k_describe(const FeImage* __restrict__ tab, const uint32_t* __restrict__ II_all,
+                                                  const int* __restrict__ half, const uint8_t* __restrict__ pi,
                                                   const uint8_t* __restrict__ pj, const int16_t* __restrict__ lut, int desc_bytes,
-                                                  okb_keypoint* kps, const int* n_kp, uint8_t* desc) {
+                                                  const okb_keypoint* kps_all, int max_kp, const int* count_all, uint8_t* desc_all) {
   __shared__ uint32_t sS[4][64], sA[4][64];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const int k = blockIdx.x * 4 + wib;
-  if (k >= *n_kp) return;
-  const int x = (int)kps[k].x, y = (int)kps[k].y;
-  float ang = 0.0f;
-  if (rot_inv) {
-    if (lane == 0) {
-      CamIntr cam;
-      cam_load(camera, cam);
-      double pu[2];
-      undistort_gn(cam, ((double)x - cam.cu) / cam.fu, ((double)y - cam.cv) / cam.fv, pu);
-      const double ep[3] = {pu[0], pu[1], 1.0};
-      double ip[2], J[6];
-      project<true>(cam, ep, ip, J);
-      const double e0 = J[0] * gC[0] + J[1] * gC[1] + J[2] * gC[2];
-      const double e1 = J[3] * gC[0] + J[4] * gC[1] + J[5] * gC[2];
-      ang = (float)(atan2(e1, e0) / 3.14159265358979323846 * 180.0);
-      kps[k].angle = ang;
-    }
-    ang = __shfl_sync(0xffffffffu, ang, 0);
-  }
+  if (k >= count_all[4 * blockIdx.y + 1]) return;
+  const FeImage& im = tab[blockIdx.y];
+  const int W = im.W, H = im.H;
+  const uint32_t* __restrict__ II = II_all + im.ii;
+  const okb_keypoint& kp = kps_all[(size_t)blockIdx.y * max_kp + k];
+  uint8_t* desc = desc_all + (size_t)blockIdx.y * max_kp * desc_bytes;
+  const int x = (int)kp.x, y = (int)kp.y;
+  const float ang = kp.angle;
   const int bin = ((int)lround((double)ang / 360.0 * kRotBins)) & (kRotBins - 1);
   for (int p = lane; p < kPts; p += 32) {
     const int cx = x + lut[((size_t)bin * kPts + p) * 2], cy = y + lut[((size_t)bin * kPts + p) * 2 + 1];
@@ -692,21 +785,160 @@ __global__ void __launch_bounds__(128) k_describe(const uint32_t* __restrict__ I
 }
 }  // namespace
 
-static int ensure_pattern(okb_ctx* c, okb_frontend_state* F, int desc_bytes) {
+// The device pattern of one descriptor length.  Each length gets its own, kept until the context is destroyed, so
+// concurrent calls with different lengths never see a pattern replaced under them.
+static int ensure_pattern(okb_ctx* c, okb_frontend_state* F, int desc_bytes, DevPattern* out) {
   std::lock_guard<std::mutex> lk(F->pat_mtx);
-  if (F->pat_bytes == desc_bytes) return OKB_OK;
-  Pattern P = make_pattern(desc_bytes);
-  cudaFree(F->d_half); cudaFree(F->d_pi); cudaFree(F->d_pj); cudaFree(F->d_lut);
-  FE_CUDA(c, cudaMalloc(&F->d_half, sizeof(int) * kPts));
-  FE_CUDA(c, cudaMalloc(&F->d_pi, P.pi.size()));
-  FE_CUDA(c, cudaMalloc(&F->d_pj, P.pj.size()));
-  FE_CUDA(c, cudaMalloc(&F->d_lut, P.lut.size() * sizeof(int16_t)));
-  FE_CUDA(c, cudaMemcpy(F->d_half, P.half, sizeof(int) * kPts, cudaMemcpyHostToDevice));
-  FE_CUDA(c, cudaMemcpy(F->d_pi, P.pi.data(), P.pi.size(), cudaMemcpyHostToDevice));
-  FE_CUDA(c, cudaMemcpy(F->d_pj, P.pj.data(), P.pj.size(), cudaMemcpyHostToDevice));
-  FE_CUDA(c, cudaMemcpy(F->d_lut, P.lut.data(), P.lut.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
-  F->pat_bytes = desc_bytes;
+  DevPattern& D = F->pats[desc_bytes / 4];
+  if (!D.lut) {
+    Pattern P = make_pattern(desc_bytes);
+    DevPattern N;
+    FE_CUDA(c, cudaMalloc(&N.half, sizeof(int) * kPts));
+    FE_CUDA(c, cudaMalloc(&N.pi, P.pi.size()));
+    FE_CUDA(c, cudaMalloc(&N.pj, P.pj.size()));
+    FE_CUDA(c, cudaMalloc(&N.lut, P.lut.size() * sizeof(int16_t)));
+    FE_CUDA(c, cudaMemcpy(N.half, P.half, sizeof(int) * kPts, cudaMemcpyHostToDevice));
+    FE_CUDA(c, cudaMemcpy(N.pi, P.pi.data(), P.pi.size(), cudaMemcpyHostToDevice));
+    FE_CUDA(c, cudaMemcpy(N.pj, P.pj.data(), P.pj.size(), cudaMemcpyHostToDevice));
+    FE_CUDA(c, cudaMemcpy(N.lut, P.lut.data(), P.lut.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
+    D = N;
+  }
+  *out = D;
   return OKB_OK;
+}
+
+template <typename T>
+static int grow(okb_ctx* c, T** p, size_t* cap, size_t need) {
+  if (*cap >= need) return OKB_OK;
+  cudaFree(*p);
+  *p = nullptr; *cap = 0;
+  FE_CUDA(c, cudaMalloc(p, need * sizeof(T)));
+  *cap = need;
+  return OKB_OK;
+}
+
+template <typename T>
+static int grow_pinned(okb_ctx* c, T** p, size_t* cap, size_t need) {
+  if (*cap >= need) return OKB_OK;
+  if (*p) cudaFreeHost(*p);
+  *p = nullptr; *cap = 0;
+  FE_CUDA(c, cudaMallocHost(p, need * sizeof(T)));
+  *cap = need;
+  return OKB_OK;
+}
+
+// f(i) for every i in [0, n), spread over up to `threads` host threads (<= 0: 8, as okb_window_upload_batch), but
+// no more than one thread per 8 MB of `bytes` to move: below that, starting a thread costs more than it saves
+template <typename Fn>
+static void host_parallel(int n, int threads, size_t bytes, const Fn& f) {
+  const int by_bytes = (int)std::min<size_t>(1 + bytes / (8u << 20), 64);
+  const int T = std::max(1, std::min({threads > 0 ? threads : 8, n, by_bytes}));
+  if (T == 1) {
+    for (int i = 0; i < n; ++i) f(i);
+    return;
+  }
+  std::vector<std::thread> th;
+  th.reserve(T);
+  for (int t = 0; t < T; ++t)
+    th.emplace_back([=, &f]() {
+      for (int i = t; i < n; i += T) f(i);
+    });
+  for (auto& x : th) x.join();
+}
+
+static size_t up256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// Detect and describe n images with one parameter set on stream `st`, into buffers B: one H2D copy (image table and
+// packed images), 7 launches whatever n is, one D2H copy (counts, keypoints, descriptors), one synchronisation.
+// Arguments are checked by the callers; maxk = min(max_keypoints, max_out) >= 1.  n_out[i] = -1 marks an image with
+// more NMS candidates than kMaxCand (OKB_ERR_CAPACITY); the other images' outputs are written all the same.
+static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaStream_t st, int n, const okb_image_desc* ims,
+                      const okb_detect_params* prm, okb_keypoint* out_kp, uint8_t* out_desc, int max_out, int32_t* n_out, int host_threads) {
+  const int maxk = std::min(prm->max_keypoints, max_out), db = prm->desc_bytes;
+  DevPattern pat;
+  int rc = ensure_pattern(c, F, db, &pat);
+  if (rc) return rc;
+  std::vector<FeImage> tab(n);
+  size_t in_bytes = up256(sizeof(FeImage) * n), px = 0, ii = 0, uni = 0;
+  int Wmax = 0, Hmax = 0;
+  for (int i = 0; i < n; ++i) {
+    const okb_image_desc& d = ims[i];
+    FeImage& t = tab[i];
+    std::memset(&t, 0, sizeof t);
+    t.cam = d.cam;
+    t.gC[0] = -d.R_CW[2]; t.gC[1] = -d.R_CW[5]; t.gC[2] = -d.R_CW[8];
+    t.W = d.width; t.H = d.height;
+    t.img = in_bytes; t.px = px; t.ii = ii; t.uni = uni;
+    t.max_cells = ((d.width + 3) / 4) * ((d.height + 3) / 4);          // smallest cell is 4 px
+    uni += uni_stride(t.max_cells, kMaxCand);
+    in_bytes += up256((size_t)d.width * d.height);
+    px += (size_t)d.width * d.height;
+    ii += (size_t)(d.width + 1) * (d.height + 1);
+    Wmax = std::max(Wmax, d.width); Hmax = std::max(Hmax, d.height);
+  }
+  const size_t o_kp = up256(sizeof(int) * 4 * n), o_desc = o_kp + up256(sizeof(okb_keypoint) * n * maxk);
+  const size_t out_bytes = o_desc + (size_t)n * maxk * db;
+  if ((rc = grow_pinned(c, &B.h_in, &B.h_in_cap, in_bytes)) || (rc = grow(c, &B.d_in, &B.d_in_cap, in_bytes)) ||
+      (rc = grow(c, &B.d_score, &B.cap_score, px)) || (rc = grow(c, &B.d_integral, &B.cap_integral, ii)) ||
+      (rc = grow(c, &B.d_keys, &B.cap_keys, (size_t)n * kMaxCand)) || (rc = grow(c, &B.d_uni, &B.cap_uni, uni)) ||
+      (rc = grow(c, &B.d_state, &B.cap_state, (size_t)n * kMaxCand)) || (rc = grow(c, &B.d_out, &B.d_out_cap, out_bytes)) ||
+      (rc = grow_pinned(c, &B.h_out, &B.h_out_cap, out_bytes)))
+    return rc;
+  std::memcpy(B.h_in, tab.data(), sizeof(FeImage) * n);
+  host_parallel(n, host_threads, in_bytes, [&](int i) {
+    const okb_image_desc& d = ims[i];
+    uint8_t* dst = B.h_in + tab[i].img;
+    if (d.stride == d.width) std::memcpy(dst, d.img, (size_t)d.width * d.height);
+    else
+      for (int y = 0; y < d.height; ++y) std::memcpy(dst + (size_t)y * d.width, d.img + (size_t)y * d.stride, d.width);
+  });
+  FE_CUDA(c, cudaMemcpyAsync(B.d_in, B.h_in, in_bytes, cudaMemcpyHostToDevice, st));
+  FE_CUDA(c, cudaMemsetAsync(B.d_out, 0, sizeof(int) * 4 * n, st));      // per image: candidates, accepted, rounds, -
+  const FeImage* d_tab = reinterpret_cast<const FeImage*>(B.d_in);
+  int* d_count = reinterpret_cast<int*>(B.d_out);
+  okb_keypoint* d_kp = reinterpret_cast<okb_keypoint*>(B.d_out + o_kp);
+  uint8_t* d_desc = B.d_out + o_desc;
+  const dim3 hb(HT_X, HT_Y), hg((Wmax + HT_X - 1) / HT_X, (Hmax + HT_Y - 1) / HT_Y, n);
+  k_harris<<<hg, hb, 0, st>>>(d_tab, B.d_in, B.d_score);
+  const dim3 nb(32, 8), ng((Wmax + 31) / 32, (Hmax + 7) / 8, n);
+  k_nms<<<ng, nb, 0, st>>>(d_tab, B.d_score, (int32_t)std::ceil(prm->absolute_threshold), B.d_keys, d_count, kMaxCand);
+  k_uniformity<<<n, UT, 0, st>>>(d_tab, B.d_keys, d_count, kMaxCand, prm->uniformity_radius, maxk, B.d_uni, B.d_state, d_kp);
+  FE_CUDA(c, cudaFuncSetAttribute(k_uniformity_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(UniSmem)));
+  k_uniformity_smem<<<n, UT, sizeof(UniSmem), st>>>(d_tab, B.d_keys, d_count, kMaxCand, prm->uniformity_radius, maxk, d_kp);
+  k_integral_rows<<<dim3((Hmax + 1 + 3) / 4, n), 128, 0, st>>>(d_tab, B.d_in, B.d_integral);
+  k_integral_cols<<<dim3((Wmax + 1 + 31) / 32, n), 32 * IC_SEG, 0, st>>>(d_tab, B.d_integral);
+  if (prm->rotation_invariance) k_orient<<<dim3((maxk + 127) / 128, n), 128, 0, st>>>(d_tab, d_kp, maxk, d_count);
+  k_describe<<<dim3((maxk + 3) / 4, n), 128, 0, st>>>(d_tab, B.d_integral, pat.half, pat.pi, pat.pj, pat.lut, db, d_kp, maxk, d_count,
+                                                      d_desc);
+  F->launches += prm->rotation_invariance ? 8 : 7;
+  FE_CUDA(c, cudaGetLastError());
+  FE_CUDA(c, cudaMemcpyAsync(B.h_out, B.d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  FE_CUDA(c, cudaStreamSynchronize(st));
+  const int* h_count = reinterpret_cast<const int*>(B.h_out);
+  { static const bool dbg = getenv("OKB_FE_DEBUG") != nullptr;
+    if (dbg)
+      for (int i = 0; i < n; ++i)
+        fprintf(stderr, "[okb frontend] image %d: candidates %d accepted %d uniformity rounds %d\n", i, h_count[4 * i], h_count[4 * i + 1], h_count[4 * i + 2]);
+#ifdef OKB_UNI_PROF
+    if (dbg) { unsigned long long pr[8]; cudaMemcpyFromSymbol(pr, g_uni_prof, sizeof(pr)); fprintf(stderr, "[okb frontend] uniformity cycles: load %llu grid %llu accept %llu kill %llu rebuild %llu compact %llu rank %llu\n", pr[0], pr[1], pr[2], pr[3], pr[4], pr[5], pr[6]); }
+#endif
+  }
+  int status = OKB_OK;
+  for (int i = 0; i < n; ++i) {
+    n_out[i] = h_count[4 * i] > kMaxCand ? -1 : h_count[4 * i + 1];
+    if (n_out[i] < 0) status = OKB_ERR_CAPACITY;
+  }
+  host_parallel(n, host_threads, out_bytes, [&](int i) {
+    if (n_out[i] <= 0) return;
+    std::memcpy(out_kp + (size_t)i * max_out, B.h_out + o_kp + sizeof(okb_keypoint) * i * maxk, sizeof(okb_keypoint) * n_out[i]);
+    std::memcpy(out_desc + (size_t)i * max_out * db, B.h_out + o_desc + (size_t)i * maxk * db, (size_t)n_out[i] * db);
+  });
+  if (status) c->set_error("too many corner candidates");
+  return status;
+}
+
+static bool detect_params_ok(const okb_detect_params* prm, int max_out) {
+  return (prm->desc_bytes >= 4 && prm->desc_bytes <= 128 && (prm->desc_bytes % 4) == 0) && std::min(prm->max_keypoints, max_out) >= 1;
 }
 
 extern "C" int okb_detect_describe(okb_ctx* c, int cam_slot, const uint8_t* img, int width, int height, int stride,
@@ -714,88 +946,39 @@ extern "C" int okb_detect_describe(okb_ctx* c, int cam_slot, const uint8_t* img,
                                    okb_keypoint* out_kp, uint8_t* out_desc, int max_out, int* n_out) {
   if (!c || !img || !cam || !R_CW || !prm || !out_kp || !out_desc || !n_out) return OKB_ERR_INVALID_ARG;
   if (cam_slot < 0 || cam_slot >= kMaxSlots || width < 64 || height < 64 || stride < width) return OKB_ERR_INVALID_ARG;
-  if (prm->desc_bytes < 4 || prm->desc_bytes > 128 || (prm->desc_bytes % 4) != 0) return OKB_ERR_INVALID_ARG;
+  if (!detect_params_ok(prm, max_out)) return OKB_ERR_INVALID_ARG;
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
-  int rc = ensure_pattern(c, F, prm->desc_bytes);
-  if (rc) return rc;
   SlotBuffers& S = F->slots[cam_slot];
   std::lock_guard<std::mutex> lk(S.mtx);   // the reference guards each camera's detector with a mutex (Frontend.cpp:97)
-  const int W = width, H = height;
-  const int maxk = std::min(prm->max_keypoints, max_out);
-  if (maxk < 1) return OKB_ERR_INVALID_ARG;
   if (!S.stream) FE_CUDA(c, cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
-  if (S.W != W || S.H != H) {
-    cudaFree(S.d_img); cudaFree(S.d_score); cudaFree(S.d_integral); cudaFree(S.d_keys); cudaFree(S.d_count);
-    cudaFree(S.d_cell_start); cudaFree(S.d_cell_cur); cudaFree(S.d_order); cudaFree(S.d_acc); cudaFree(S.d_state); cudaFree(S.d_rounds);
-    if (S.h_img) cudaFreeHost(S.h_img);
-    if (S.h_count) cudaFreeHost(S.h_count);
-    FE_CUDA(c, cudaMalloc(&S.d_img, (size_t)W * H));
-    FE_CUDA(c, cudaMalloc(&S.d_score, sizeof(int32_t) * W * H));
-    FE_CUDA(c, cudaMalloc(&S.d_integral, sizeof(uint32_t) * (W + 1) * (H + 1)));
-    FE_CUDA(c, cudaMalloc(&S.d_keys, sizeof(unsigned long long) * kMaxCand));
-    FE_CUDA(c, cudaMalloc(&S.d_count, sizeof(int) * 4 + sizeof(double) * 4));      // candidates, accepted, rounds, - | gravity direction
-    S.max_cells = ((W + 3) / 4) * ((H + 3) / 4);          // smallest cell is 4 px
-    FE_CUDA(c, cudaMalloc(&S.d_cell_start, sizeof(uint32_t) * (S.max_cells + 1)));
-    FE_CUDA(c, cudaMalloc(&S.d_cell_cur, sizeof(uint32_t) * S.max_cells));
-    FE_CUDA(c, cudaMalloc(&S.d_order, sizeof(uint32_t) * kMaxCand));
-    FE_CUDA(c, cudaMalloc(&S.d_acc, sizeof(uint32_t) * kMaxCand));
-    FE_CUDA(c, cudaMalloc(&S.d_state, kMaxCand));
-    FE_CUDA(c, cudaMalloc(&S.d_rounds, sizeof(uint32_t) * 4 * kMaxCand));
-    FE_CUDA(c, cudaMallocHost(&S.h_img, (size_t)W * H));
-    FE_CUDA(c, cudaMallocHost(&S.h_count, sizeof(int) * 4));
-    S.W = W; S.H = H;
+  okb_image_desc d;
+  std::memset(&d, 0, sizeof d);
+  d.img = img; d.width = width; d.height = height; d.stride = stride;
+  d.cam = *cam;
+  std::memcpy(d.R_CW, R_CW, sizeof d.R_CW);
+  int32_t n = 0;
+  const int rc = detect_run(c, F, S.buf, S.stream, 1, &d, prm, out_kp, out_desc, max_out, &n, 1);
+  if (rc == OKB_OK) *n_out = n;
+  return rc;
+}
+
+extern "C" int okb_detect_describe_batch(okb_ctx* c, int n_images, const okb_image_desc* images, const okb_detect_params* prm,
+                                         okb_keypoint* out_kp, uint8_t* out_desc, int max_out, int32_t* n_out, int host_threads) {
+  if (!c || n_images < 0) return OKB_ERR_INVALID_ARG;
+  if (n_images == 0) return OKB_OK;
+  if (n_images > 65535) return OKB_ERR_INVALID_ARG;           // the image index is a grid dimension
+  if (!images || !prm || !out_kp || !out_desc || !n_out) return OKB_ERR_INVALID_ARG;
+  if (!detect_params_ok(prm, max_out)) return OKB_ERR_INVALID_ARG;
+  for (int i = 0; i < n_images; ++i) {
+    const okb_image_desc& d = images[i];
+    if (!d.img || d.width < 64 || d.height < 64 || d.stride < d.width) return OKB_ERR_INVALID_ARG;
   }
-  if (S.kp_cap < maxk || S.desc_cap < maxk * prm->desc_bytes) {
-    cudaFree(S.d_kp); cudaFree(S.d_desc);
-    if (S.h_kp) cudaFreeHost(S.h_kp);
-    if (S.h_desc) cudaFreeHost(S.h_desc);
-    FE_CUDA(c, cudaMalloc(&S.d_kp, sizeof(okb_keypoint) * maxk));
-    FE_CUDA(c, cudaMalloc(&S.d_desc, (size_t)maxk * prm->desc_bytes));
-    FE_CUDA(c, cudaMallocHost(&S.h_kp, sizeof(okb_keypoint) * maxk));
-    FE_CUDA(c, cudaMallocHost(&S.h_desc, (size_t)maxk * prm->desc_bytes));
-    S.kp_cap = maxk; S.desc_cap = maxk * prm->desc_bytes;
-  }
-  for (int y = 0; y < H; ++y) std::memcpy(S.h_img + (size_t)y * W, img + (size_t)y * stride, W);
-  cudaStream_t st = S.stream;
-  FE_CUDA(c, cudaMemcpyAsync(S.d_img, S.h_img, (size_t)W * H, cudaMemcpyHostToDevice, st));
-  FE_CUDA(c, cudaMemsetAsync(S.d_count, 0, sizeof(int) * 4, st));
-  // gravity direction in the camera frame: R_CW * (0,0,-1)
-  double gC[3] = {-R_CW[2], -R_CW[5], -R_CW[8]};
-  double* d_gC = reinterpret_cast<double*>(S.d_count + 4);
-  FE_CUDA(c, cudaMemcpyAsync(d_gC, gC, sizeof gC, cudaMemcpyHostToDevice, st));
-  const dim3 hb(HT_X, HT_Y), hg((W + HT_X - 1) / HT_X, (H + HT_Y - 1) / HT_Y);
-  k_harris<<<hg, hb, 0, st>>>(S.d_img, W, H, S.d_score);
-  const dim3 nb(32, 8), ng((W + 31) / 32, (H + 7) / 8);
-  k_nms<<<ng, nb, 0, st>>>(S.d_score, W, H, (int32_t)std::ceil(prm->absolute_threshold), S.d_keys, S.d_count, kMaxCand);
-  UniScratch us{S.d_cell_start, S.d_cell_cur, S.d_order, S.d_state, S.d_acc, S.d_rounds, S.d_rounds + kMaxCand, S.d_rounds + 2 * kMaxCand,
-                S.d_rounds + 3 * kMaxCand, S.max_cells};
-  k_uniformity<<<1, UT, 0, st>>>(S.d_keys, S.d_count, kMaxCand, W, H, prm->uniformity_radius, maxk, us, S.d_kp, S.d_count + 1);
-  {
-    FE_CUDA(c, cudaFuncSetAttribute(k_uniformity_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(UniSmem)));
-    k_uniformity_smem<<<1, UT, sizeof(UniSmem), st>>>(S.d_keys, S.d_count, kMaxCand, W, H, prm->uniformity_radius, maxk, S.d_kp, S.d_count + 1);
-  }
-  k_integral_rows<<<(H + 1 + 3) / 4, 128, 0, st>>>(S.d_img, W, H, S.d_integral);
-  k_integral_cols<<<(W + 1 + 31) / 32, 32 * IC_SEG, 0, st>>>(W, H, S.d_integral);
-  k_describe<<<(maxk + 3) / 4, 128, 0, st>>>(S.d_integral, W, H, *cam, d_gC, prm->rotation_invariance, F->d_half, F->d_pi, F->d_pj,
-                                             F->d_lut, prm->desc_bytes, S.d_kp, S.d_count + 1, S.d_desc);
-  c->launches += 7;
-  FE_CUDA(c, cudaGetLastError());
-  FE_CUDA(c, cudaMemcpyAsync(S.h_count, S.d_count, sizeof(int) * 4, cudaMemcpyDeviceToHost, st));
-  FE_CUDA(c, cudaMemcpyAsync(S.h_kp, S.d_kp, sizeof(okb_keypoint) * maxk, cudaMemcpyDeviceToHost, st));
-  FE_CUDA(c, cudaMemcpyAsync(S.h_desc, S.d_desc, (size_t)maxk * prm->desc_bytes, cudaMemcpyDeviceToHost, st));
-  FE_CUDA(c, cudaStreamSynchronize(st));
-  { static const bool dbg = getenv("OKB_FE_DEBUG") != nullptr; if (dbg) fprintf(stderr, "[okb frontend] candidates %d accepted %d uniformity rounds %d\n", S.h_count[0], S.h_count[1], S.h_count[2]);
-#ifdef OKB_UNI_PROF
-    if (dbg) { unsigned long long pr[8]; cudaMemcpyFromSymbol(pr, g_uni_prof, sizeof(pr)); fprintf(stderr, "[okb frontend] uniformity cycles: load %llu grid %llu accept %llu kill %llu rebuild %llu compact %llu rank %llu\n", pr[0], pr[1], pr[2], pr[3], pr[4], pr[5], pr[6]); }
-#endif
-  }
-  if (S.h_count[0] > kMaxCand) { c->set_error("too many corner candidates"); return OKB_ERR_CAPACITY; }
-  const int n = S.h_count[1];
-  std::memcpy(out_kp, S.h_kp, sizeof(okb_keypoint) * n);
-  std::memcpy(out_desc, S.h_desc, (size_t)n * prm->desc_bytes);
-  *n_out = n;
-  return OKB_OK;
+  cudaSetDevice(c->device);
+  okb_frontend_state* F = fe(c);
+  std::lock_guard<std::mutex> lk(F->batch_mtx);
+  if (!F->batch_stream) FE_CUDA(c, cudaStreamCreateWithFlags(&F->batch_stream, cudaStreamNonBlocking));
+  return detect_run(c, F, F->batch_det, F->batch_stream, n_images, images, prm, out_kp, out_desc, max_out, n_out, host_threads);
 }
 
 // =================================================================================================
@@ -806,7 +989,7 @@ extern "C" int okb_detect_describe(okb_ctx* c, int cam_slot, const uint8_t* img,
 // (A, B) pair inside the list kernel for pairs whose Hamming distance is below the threshold
 // =================================================================================================
 namespace {
-struct GateDev {
+struct __align__(8) GateDev {
   int mode;
   const double *kp_b, *kp_size_b, *proj_into_b, *proj_unc, *kp_a, *kp_size_a, *bearing_a, *bearing_b, *ray_sigma_a, *ray_sigma_b;
   CamIntr cam_a, cam_b;
@@ -910,18 +1093,46 @@ constexpr int MT = 32 * MW;
 constexpr int MB_TILE = 128;     // B descriptors staged per shared-memory tile
 constexpr int MAX_BEST = 8;
 
+// One match of a matcher launch (device table, one entry per job); pointers into the launch's staging mirror.  The
+// gate sits in the entry itself (last, so that a plain job's kernel copies only the words before it).
+struct __align__(8) MatchJobDev {
+  const uint32_t *A, *B;
+  const uint8_t *skipA, *skipB;    // may be null
+  okb_pair *topk, *pairs;
+  uint8_t* done;                   // [nA] k_assign scratch
+  int nA, nB, num_best, in_smem;   // in_smem: k_assign keeps the per-B winners in shared memory
+  float list_thr, gate_thr;
+  GateDev gate;                    // gated jobs only
+};
+
 // Warp per A descriptor.  Every lane computes the Hamming distance (XOR + __popc over NW words) of A to one of 32
 // consecutive B descriptors, staged tile by tile in shared memory for the CTA's 8 warps; the top-`num_best` list of
 // DenseMatcher::listBIteration (implementation/DenseMatcher.hpp:137-225) is kept replicated in the warp and updated
 // with exactly the reference's sequential rule -- candidates are taken in ascending B order (lowest set bit of the
 // ballot first), a candidate enters only if it beats the CURRENT worst entry (re-voted after every insertion, the
 // worst only shrinks), std::lower_bound position, i.e. before entries of equal distance.
+// blockIdx.y is the job; the grid covers the largest nA of the launch and CTAs past their job's nA exit.
 template <int NW, bool GATED>
-__global__ void __launch_bounds__(MT) k_hamming_topk(const uint32_t* __restrict__ A, int nA, const uint32_t* __restrict__ B, int nB,
-                                                     const uint8_t* __restrict__ skipA, const uint8_t* __restrict__ skipB, float list_thr,
-                                                     int num_best, okb_pair* __restrict__ topk, float gate_thr, const GateDev* __restrict__ gate) {
+__global__ void __launch_bounds__(MT, GATED ? (NW == 32 ? 1 : 2) : (NW <= 16 ? 3 : 2)) k_hamming_topk(const MatchJobDev* __restrict__ jobs) {
   __shared__ uint32_t sB[MB_TILE][NW + 1];
   __shared__ uint8_t sSkip[MB_TILE];
+  if ((int)blockIdx.x * MW >= jobs[blockIdx.y].nA) return;
+  // the job, gate included, is staged in shared memory once: its fields are then read where they are used, from fixed
+  // shared addresses, rather than held in registers across the loop
+  __shared__ MatchJobDev J;
+  constexpr int words = (GATED ? sizeof(MatchJobDev) : offsetof(MatchJobDev, gate)) / 8;
+  static_assert(words <= MT, "one word per thread");
+  if (threadIdx.x < words)
+    reinterpret_cast<unsigned long long*>(&J)[threadIdx.x] = reinterpret_cast<const unsigned long long*>(jobs + blockIdx.y)[threadIdx.x];
+  __syncthreads();
+  const uint32_t* const& A = J.A;
+  const uint32_t* const& B = J.B;
+  const uint8_t* const& skipA = J.skipA;
+  const uint8_t* const& skipB = J.skipB;
+  okb_pair* const& topk = J.topk;
+
+  const int &nA = J.nA, &nB = J.nB, &num_best = J.num_best;
+  const float &list_thr = J.list_thr, &gate_thr = J.gate_thr;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int a = blockIdx.x * MW + warp;
   const bool active = a < nA && !(skipA && skipA[a]);
@@ -950,7 +1161,7 @@ __global__ void __launch_bounds__(MT) k_hamming_topk(const uint32_t* __restrict_
         t = (float)dist;
         // VioKeyframeWindowMatchingAlgorithm::distance: the Hamming distance counts only below the threshold and
         // if the geometric gate passes, else FLT_MAX (which never enters a list)
-        if (GATED) t = (t < gate_thr && gate_verify(*gate, a, b0 + j)) ? t : 3.402823466e+38f;
+        if (GATED) t = (t < gate_thr && gate_verify(J.gate, a, b0 + j)) ? t : 3.402823466e+38f;
       }
       uint32_t mask = __ballot_sync(0xffffffffu, t < worst);
       while (mask) {
@@ -975,7 +1186,9 @@ __global__ void __launch_bounds__(MT) k_hamming_topk(const uint32_t* __restrict_
     }
   }
   if (a < nA && lane == 0) {
-    for (int k = 0; k < num_best; ++k) {
+#pragma unroll
+    for (int k = 0; k < MAX_BEST; ++k) {
+      if (k >= num_best) break;
       okb_pair p;
       p.index_a = active ? bi[k] : -1;
       p.distance = active ? bd[k] : list_thr;
@@ -993,9 +1206,15 @@ __global__ void __launch_bounds__(MT) k_hamming_topk(const uint32_t* __restrict_
 // list entries of all non-skipped A's), then b is free when A's turn comes, A takes it, nobody can displace A and A
 // touches no other b -- its outcome is independent of the order.  Those are assigned in parallel; only A's whose first
 // choice is contested walk serially (typically a small fraction).
+// One CTA per job (blockIdx.x).
 constexpr int AS_T = 256, AS_CHUNK = 256;
-__global__ void __launch_bounds__(AS_T) k_assign(const okb_pair* __restrict__ topk, int nA, int nB, int num_best, const uint8_t* __restrict__ skipA,
-                                                 okb_pair* pairs, uint8_t* done /* [nA] scratch */, int in_smem) {
+__global__ void __launch_bounds__(AS_T) k_assign(const MatchJobDev* __restrict__ jobs) {
+  const MatchJobDev& J = jobs[blockIdx.x];
+  const okb_pair* __restrict__ topk = J.topk;
+  const uint8_t* __restrict__ skipA = J.skipA;
+  okb_pair* pairs = J.pairs;
+  uint8_t* done = J.done;
+  const int nA = J.nA, nB = J.nB, num_best = J.num_best, in_smem = J.in_smem;
   extern __shared__ okb_pair s_dyn[];
   okb_pair* s_top = s_dyn;                                   // [AS_CHUNK][num_best]
   okb_pair* P = in_smem ? s_dyn + (size_t)AS_CHUNK * MAX_BEST : pairs;
@@ -1114,16 +1333,6 @@ __global__ void __launch_bounds__(1024) k_exclusive_scan(const uint32_t* counts,
 }
 }  // namespace
 
-template <typename T>
-static int grow(okb_ctx* c, T** p, size_t* cap, size_t need) {
-  if (*cap >= need) return OKB_OK;
-  cudaFree(*p);
-  *p = nullptr; *cap = 0;
-  FE_CUDA(c, cudaMalloc(p, need * sizeof(T)));
-  *cap = need;
-  return OKB_OK;
-}
-
 #define DISPATCH_NW(nw, CALL)                 \
   switch (nw) {                               \
     case 8: { constexpr int NW = 8; CALL; } break;   \
@@ -1145,122 +1354,186 @@ static int upload_descriptors(okb_ctx* c, okb_frontend_state* F, const uint8_t* 
   return OKB_OK;
 }
 
-static int ensure_io(okb_ctx* c, okb_frontend_state* F, size_t bytes) {
-  if (F->h_stage_cap < bytes) {
-    if (F->h_stage) cudaFreeHost(F->h_stage);
-    F->h_stage = nullptr; F->h_stage_cap = 0;
-    FE_CUDA(c, cudaMallocHost(&F->h_stage, bytes));
-    F->h_stage_cap = bytes;
-  }
-  if (F->d_io_cap < bytes) {
-    cudaFree(F->d_io);
-    F->d_io = nullptr; F->d_io_cap = 0;
-    FE_CUDA(c, cudaMalloc(&F->d_io, bytes));
-    F->d_io_cap = bytes;
-  }
-  return OKB_OK;
+static int ensure_io(okb_ctx* c, MatchIO& io, size_t bytes) {
+  int rc;
+  if ((rc = grow_pinned(c, &io.h_stage, &io.h_stage_cap, bytes))) return rc;
+  return grow(c, &io.d_io, &io.d_io_cap, bytes);
 }
 
-static int hamming_match_impl(okb_ctx* c, const uint8_t* A, int nA, const uint8_t* B, int nB, int desc_bytes, const uint8_t* skipA,
-                              const uint8_t* skipB, float threshold, int num_best, int use_ratio, const okb_match_gate* gate,
-                              okb_pair* out_topk, okb_pair* out_pairs) {
-  if (!c || nA < 0 || nB < 0 || num_best < 1 || num_best > MAX_BEST || (nB > 0 && !out_pairs)) return OKB_ERR_INVALID_ARG;
-  if (nA == 0 || nB == 0) {     // an empty list matches nothing (DenseMatcher::match on an empty MatchingAlgorithm): no device work
-    for (int i = 0; i < nB; ++i) { out_pairs[i].index_a = -1; out_pairs[i].distance = threshold; }
-    if (out_topk) for (size_t i = 0; i < (size_t)nA * num_best; ++i) { out_topk[i].index_a = -1; out_topk[i].distance = threshold; }
-    return OKB_OK;
-  }
-  if (!A || !B) return OKB_ERR_INVALID_ARG;
+// The single call's argument checks, for one job.
+static int match_job_check(okb_ctx* c, const okb_match_job& j, int desc_bytes) {
+  if (j.nA < 0 || j.nB < 0 || j.num_best < 1 || j.num_best > MAX_BEST || (j.nB > 0 && !j.out_pairs)) return OKB_ERR_INVALID_ARG;
+  if (j.nA == 0 || j.nB == 0) return OKB_OK;
+  if (!j.A || !j.B) return OKB_ERR_INVALID_ARG;
   if (desc_bytes % 4) { c->set_error("descriptor length must be a multiple of 4"); return OKB_ERR_UNSUPPORTED; }
+  const okb_match_gate* gate = j.gate;
   const int mode = gate ? gate->mode : OKB_GATE_NONE;
   if (mode != OKB_GATE_NONE && mode != OKB_GATE_3D2D && mode != OKB_GATE_2D2D) return OKB_ERR_INVALID_ARG;
   if (mode != OKB_GATE_NONE && (!gate->kp_b || !gate->kp_size_b)) return OKB_ERR_INVALID_ARG;
   if (mode == OKB_GATE_3D2D && (!gate->proj_into_b || !gate->proj_uncertainty)) return OKB_ERR_INVALID_ARG;
   if (mode == OKB_GATE_2D2D && (!gate->kp_a || !gate->kp_size_a || !gate->bearing_a || !gate->bearing_b || !gate->ray_sigma_a || !gate->ray_sigma_b))
     return OKB_ERR_INVALID_ARG;
+  return OKB_OK;
+}
+
+// n matches on stream `st` through staging buffers io: one pinned staging buffer, one copy in, one copy out:
+//   [job table (gates included) | per job: A | B | skipA | skipB | gate arrays]  ...  [per job: top-k lists | winners] [per job: scratch]
+// Plain jobs come first in the table, gated ones after them: one k_hamming_topk launch per kind, one k_assign launch.
+static int match_run(okb_ctx* c, MatchIO& io, cudaStream_t st, int n, const okb_match_job* jobs, int desc_bytes) {
+  int rc;
+  bool any = false;
+  for (int i = 0; i < n; ++i) {
+    if ((rc = match_job_check(c, jobs[i], desc_bytes))) return rc;
+    any = any || (jobs[i].nA > 0 && jobs[i].nB > 0);
+  }
+  const int nw = desc_bytes / 4;
+  if (any && nw != 8 && nw != 12 && nw != 16 && nw != 32) { c->set_error("descriptor length must be 32, 48, 64 or 128 bytes"); return OKB_ERR_UNSUPPORTED; }
+  std::vector<int> order;            // jobs with device work: plain, then gated
+  for (int pass = 0; pass < 2; ++pass)
+    for (int i = 0; i < n; ++i) {
+      const okb_match_job& j = jobs[i];
+      if (j.nA == 0 || j.nB == 0) {
+        if (pass) continue;
+        // an empty list matches nothing (DenseMatcher::match on an empty MatchingAlgorithm): no device work
+        for (int b = 0; b < j.nB; ++b) { j.out_pairs[b].index_a = -1; j.out_pairs[b].distance = j.threshold; }
+        if (j.out_topk) for (size_t k = 0; k < (size_t)j.nA * j.num_best; ++k) { j.out_topk[k].index_a = -1; j.out_topk[k].distance = j.threshold; }
+        continue;
+      }
+      const bool gated = j.gate && j.gate->mode != OKB_GATE_NONE;
+      if (gated == (pass == 1)) order.push_back(i);
+    }
+  const int nd = (int)order.size();
+  if (nd == 0) return OKB_OK;
+  auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+  struct Lay { size_t oA, oB, oSA, oSB, g_kpb, g_szb, g_proj, g_unc, g_kpa, g_sza, g_ba, g_bb, g_rsa, g_rsb, oT, oP, oD; };
+  std::vector<Lay> L(nd);
+  size_t off = up256(sizeof(MatchJobDev) * nd);
+  for (int t = 0; t < nd; ++t) {
+    const okb_match_job& j = jobs[order[t]];
+    const size_t nA = j.nA, nB = j.nB;
+    Lay& l = L[t];
+    l.oA = off; l.oB = l.oA + up16(nA * desc_bytes); l.oSA = l.oB + up16(nB * desc_bytes); l.oSB = l.oSA + up16(nA);
+    off = l.oSB + up16(nB);
+    if (j.gate && j.gate->mode != OKB_GATE_NONE) {
+      // gate arrays (doubles): kp_b 2nB | size_b nB | proj 2nA | unc 4nA | kp_a 2nA | size_a nA | bear_a 3nA | bear_b 3nB | rs_a nA | rs_b nB
+      l.g_kpb = off; l.g_szb = l.g_kpb + 16 * nB; l.g_proj = l.g_szb + up16(8 * nB); l.g_unc = l.g_proj + 16 * nA;
+      l.g_kpa = l.g_unc + 32 * nA; l.g_sza = l.g_kpa + 16 * nA; l.g_ba = l.g_sza + up16(8 * nA); l.g_bb = l.g_ba + up16(24 * nA);
+      l.g_rsa = l.g_bb + up16(24 * nB); l.g_rsb = l.g_rsa + up16(8 * nA);
+      off = l.g_rsb + up16(8 * nB);
+    }
+  }
+  const size_t in_bytes = off;
+  for (int t = 0; t < nd; ++t) {
+    const okb_match_job& j = jobs[order[t]];
+    L[t].oT = off; L[t].oP = off + sizeof(okb_pair) * (size_t)j.nA * j.num_best;
+    off = up16(L[t].oP + sizeof(okb_pair) * (size_t)j.nB);
+  }
+  const size_t out_end = off;
+  for (int t = 0; t < nd; ++t) { L[t].oD = off; off += up16((size_t)jobs[order[t]].nA); }
+  if ((rc = ensure_io(c, io, off))) return rc;
+  uint8_t* h = io.h_stage;
+  uint8_t* d = io.d_io;
+  const size_t sm_top = sizeof(okb_pair) * (size_t)AS_CHUNK * MAX_BEST;
+  size_t sm = sm_top;
+  int maxA[2] = {0, 0}, nkind[2] = {0, 0};
+  MatchJobDev* tab = reinterpret_cast<MatchJobDev*>(h);
+  for (int t = 0; t < nd; ++t) {
+    const okb_match_job& j = jobs[order[t]];
+    const Lay& l = L[t];
+    const int mode = j.gate ? j.gate->mode : OKB_GATE_NONE;
+    std::memcpy(h + l.oA, j.A, (size_t)j.nA * desc_bytes);
+    std::memcpy(h + l.oB, j.B, (size_t)j.nB * desc_bytes);
+    if (j.skipA) std::memcpy(h + l.oSA, j.skipA, j.nA);
+    if (j.skipB) std::memcpy(h + l.oSB, j.skipB, j.nB);
+    MatchJobDev jd;
+    std::memset(&jd, 0, sizeof jd);
+    jd.A = reinterpret_cast<const uint32_t*>(d + l.oA);
+    jd.B = reinterpret_cast<const uint32_t*>(d + l.oB);
+    jd.skipA = j.skipA ? d + l.oSA : nullptr;
+    jd.skipB = j.skipB ? d + l.oSB : nullptr;
+    jd.topk = reinterpret_cast<okb_pair*>(d + l.oT);
+    jd.pairs = reinterpret_cast<okb_pair*>(d + l.oP);
+    jd.done = d + l.oD;
+    jd.nA = j.nA; jd.nB = j.nB; jd.num_best = j.num_best;
+    // DenseMatcher.hpp(impl):188-193: with the ratio test the lists are built without a threshold
+    jd.list_thr = j.use_ratio ? 3.402823466e+38f : j.threshold;
+    jd.gate_thr = mode == OKB_GATE_NONE ? 0.f : j.threshold;
+    const size_t sm_b = (sizeof(okb_pair) + sizeof(int)) * (size_t)j.nB;        // per-B winners + list counts
+    jd.in_smem = sm_top + sm_b + 1024 <= (size_t)c->smem_optin ? 1 : 0;
+    if (jd.in_smem) sm = std::max(sm, sm_top + sm_b);
+    if (mode != OKB_GATE_NONE) {
+      const okb_match_gate* gate = j.gate;
+      GateDev gd;
+      std::memset(&gd, 0, sizeof gd);
+      gd.mode = mode;
+      auto put = [&](size_t o, const double* src, size_t cnt) -> const double* {
+        if (src) std::memcpy(h + o, src, 8 * cnt);
+        return reinterpret_cast<const double*>(d + o);
+      };
+      const size_t nA = j.nA, nB = j.nB;
+      gd.kp_b = put(l.g_kpb, gate->kp_b, 2 * nB); gd.kp_size_b = put(l.g_szb, gate->kp_size_b, nB);
+      if (mode == OKB_GATE_3D2D) { gd.proj_into_b = put(l.g_proj, gate->proj_into_b, 2 * nA); gd.proj_unc = put(l.g_unc, gate->proj_uncertainty, 4 * nA); }
+      else {
+        gd.kp_a = put(l.g_kpa, gate->kp_a, 2 * nA); gd.kp_size_a = put(l.g_sza, gate->kp_size_a, nA);
+        gd.bearing_a = put(l.g_ba, gate->bearing_a, 3 * nA); gd.bearing_b = put(l.g_bb, gate->bearing_b, 3 * nB);
+        gd.ray_sigma_a = put(l.g_rsa, gate->ray_sigma_a, nA); gd.ray_sigma_b = put(l.g_rsb, gate->ray_sigma_b, nB);
+        cam_load(gate->cam_a, gd.cam_a); cam_load(gate->cam_b, gd.cam_b);
+        gd.wa = gate->cam_a.width; gd.ha = gate->cam_a.height; gd.wb = gate->cam_b.width; gd.hb = gate->cam_b.height;
+        double q[4] = {gate->T_AB[3], gate->T_AB[4], gate->T_AB[5], gate->T_AB[6]};
+        qnormalize(q);
+        q2R(q, gd.R_AB);
+        gd.t_AB[0] = gate->T_AB[0]; gd.t_AB[1] = gate->T_AB[1]; gd.t_AB[2] = gate->T_AB[2];
+      }
+      jd.gate = gd;
+    }
+    tab[t] = jd;
+    const int kind = mode == OKB_GATE_NONE ? 0 : 1;
+    maxA[kind] = std::max(maxA[kind], j.nA);
+    ++nkind[kind];
+  }
+  FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, st));
+  const MatchJobDev* d_tab = reinterpret_cast<const MatchJobDev*>(d);
+  if (nkind[0])
+    DISPATCH_NW(nw, (k_hamming_topk<NW, false><<<dim3((maxA[0] + MW - 1) / MW, nkind[0]), MT, 0, st>>>(d_tab)));
+  if (nkind[1])
+    DISPATCH_NW(nw, (k_hamming_topk<NW, true><<<dim3((maxA[1] + MW - 1) / MW, nkind[1]), MT, 0, st>>>(d_tab + nkind[0])));
+  // the attribute is always set to the largest size any launch asks for, so concurrent calls never lower it under each other
+  if (sm > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
+  k_assign<<<nd, AS_T, sm, st>>>(d_tab);
+  c->frontend->launches += (nkind[0] > 0) + (nkind[1] > 0) + 1;
+  FE_CUDA(c, cudaGetLastError());
+  FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, st));
+  FE_CUDA(c, cudaStreamSynchronize(st));
+  for (int t = 0; t < nd; ++t) {
+    const okb_match_job& j = jobs[order[t]];
+    if (j.out_topk) std::memcpy(j.out_topk, h + L[t].oT, sizeof(okb_pair) * (size_t)j.nA * j.num_best);
+    std::memcpy(j.out_pairs, h + L[t].oP, sizeof(okb_pair) * (size_t)j.nB);
+  }
+  return OKB_OK;
+}
+
+static int hamming_match_single(okb_ctx* c, const uint8_t* A, int nA, const uint8_t* B, int nB, int desc_bytes, const uint8_t* skipA,
+                                const uint8_t* skipB, float threshold, int num_best, int use_ratio, const okb_match_gate* gate,
+                                okb_pair* out_topk, okb_pair* out_pairs) {
+  if (!c) return OKB_ERR_INVALID_ARG;
+  okb_match_job j;
+  std::memset(&j, 0, sizeof j);
+  j.A = A; j.B = B; j.skipA = skipA; j.skipB = skipB;
+  j.nA = nA; j.nB = nB; j.threshold = threshold; j.num_best = num_best; j.use_ratio = use_ratio;
+  j.gate = gate; j.out_topk = out_topk; j.out_pairs = out_pairs;
+  const int rc = match_job_check(c, j, desc_bytes);
+  if (rc) return rc;
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
   std::lock_guard<std::mutex> lk(F->match_mtx);
-  // one pinned staging buffer, one copy in, one copy out:
-  //   [A | B | skipA | skipB | gate arrays | GateDev]  ...  [top-k lists | winners | scratch]
-  auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
-  const size_t oA = 0, oB = up16((size_t)nA * desc_bytes), oSA = oB + up16((size_t)nB * desc_bytes), oSB = oSA + up16((size_t)nA);
-  size_t oG = oSB + up16((size_t)nB);
-  // gate arrays (doubles): kp_b 2nB | size_b nB | proj 2nA | unc 4nA | kp_a 2nA | size_a nA | bear_a 3nA | bear_b 3nB | rs_a nA | rs_b nB
-  const size_t g_kpb = oG, g_szb = g_kpb + 16 * (size_t)nB, g_proj = g_szb + up16(8 * (size_t)nB), g_unc = g_proj + 16 * (size_t)nA,
-               g_kpa = g_unc + 32 * (size_t)nA, g_sza = g_kpa + 16 * (size_t)nA, g_ba = g_sza + up16(8 * (size_t)nA), g_bb = g_ba + up16(24 * (size_t)nA),
-               g_rsa = g_bb + up16(24 * (size_t)nB), g_rsb = g_rsa + up16(8 * (size_t)nA), g_dev = g_rsb + up16(8 * (size_t)nB);
-  const size_t in_bytes = mode == OKB_GATE_NONE ? oG : g_dev + up16(sizeof(GateDev));
-  const size_t oT = in_bytes, oP = oT + sizeof(okb_pair) * (size_t)nA * num_best, oD = oP + sizeof(okb_pair) * (size_t)nB, total = oD + up16((size_t)nA);
-  int rc = ensure_io(c, F, total);
-  if (rc) return rc;
-  std::memcpy(F->h_stage + oA, A, (size_t)nA * desc_bytes);
-  std::memcpy(F->h_stage + oB, B, (size_t)nB * desc_bytes);
-  if (skipA) std::memcpy(F->h_stage + oSA, skipA, nA);
-  if (skipB) std::memcpy(F->h_stage + oSB, skipB, nB);
-  if (mode != OKB_GATE_NONE) {
-    GateDev gd;
-    std::memset(&gd, 0, sizeof gd);
-    gd.mode = mode;
-    auto put = [&](size_t off, const double* src, size_t n) -> const double* {
-      if (src) std::memcpy(F->h_stage + off, src, 8 * n);
-      return reinterpret_cast<const double*>(F->d_io + off);
-    };
-    gd.kp_b = put(g_kpb, gate->kp_b, 2 * (size_t)nB); gd.kp_size_b = put(g_szb, gate->kp_size_b, nB);
-    if (mode == OKB_GATE_3D2D) { gd.proj_into_b = put(g_proj, gate->proj_into_b, 2 * (size_t)nA); gd.proj_unc = put(g_unc, gate->proj_uncertainty, 4 * (size_t)nA); }
-    else {
-      gd.kp_a = put(g_kpa, gate->kp_a, 2 * (size_t)nA); gd.kp_size_a = put(g_sza, gate->kp_size_a, nA);
-      gd.bearing_a = put(g_ba, gate->bearing_a, 3 * (size_t)nA); gd.bearing_b = put(g_bb, gate->bearing_b, 3 * (size_t)nB);
-      gd.ray_sigma_a = put(g_rsa, gate->ray_sigma_a, nA); gd.ray_sigma_b = put(g_rsb, gate->ray_sigma_b, nB);
-      cam_load(gate->cam_a, gd.cam_a); cam_load(gate->cam_b, gd.cam_b);
-      gd.wa = gate->cam_a.width; gd.ha = gate->cam_a.height; gd.wb = gate->cam_b.width; gd.hb = gate->cam_b.height;
-      double q[4] = {gate->T_AB[3], gate->T_AB[4], gate->T_AB[5], gate->T_AB[6]};
-      qnormalize(q);
-      q2R(q, gd.R_AB);
-      gd.t_AB[0] = gate->T_AB[0]; gd.t_AB[1] = gate->T_AB[1]; gd.t_AB[2] = gate->T_AB[2];
-    }
-    std::memcpy(F->h_stage + g_dev, &gd, sizeof gd);
-  }
-  FE_CUDA(c, cudaMemcpyAsync(F->d_io, F->h_stage, in_bytes, cudaMemcpyHostToDevice, c->stream));
-  const uint8_t* dSA = skipA ? F->d_io + oSA : nullptr;
-  const uint8_t* dSB = skipB ? F->d_io + oSB : nullptr;
-  okb_pair* d_topk = reinterpret_cast<okb_pair*>(F->d_io + oT);
-  okb_pair* d_pairs = reinterpret_cast<okb_pair*>(F->d_io + oP);
-  const GateDev* d_gate = reinterpret_cast<const GateDev*>(F->d_io + g_dev);
-  // DenseMatcher.hpp(impl):188-193: with the ratio test the lists are built without a threshold
-  const float list_thr = use_ratio ? 3.402823466e+38f : threshold;
-  const int nw = desc_bytes / 4;
-  if (mode == OKB_GATE_NONE) {
-    DISPATCH_NW(nw, (k_hamming_topk<NW, false><<<(nA + MW - 1) / MW, MT, 0, c->stream>>>(
-                        reinterpret_cast<const uint32_t*>(F->d_io + oA), nA, reinterpret_cast<const uint32_t*>(F->d_io + oB), nB, dSA, dSB, list_thr,
-                        num_best, d_topk, 0.f, nullptr)));
-  } else {
-    DISPATCH_NW(nw, (k_hamming_topk<NW, true><<<(nA + MW - 1) / MW, MT, 0, c->stream>>>(
-                        reinterpret_cast<const uint32_t*>(F->d_io + oA), nA, reinterpret_cast<const uint32_t*>(F->d_io + oB), nB, dSA, dSB, list_thr,
-                        num_best, d_topk, threshold, d_gate)));
-  }
-  {
-    const size_t sm_top = sizeof(okb_pair) * (size_t)AS_CHUNK * MAX_BEST;
-    const size_t sm_b = (sizeof(okb_pair) + sizeof(int)) * (size_t)nB;        // per-B winners + list counts
-    const int in_smem = sm_top + sm_b + 1024 <= (size_t)c->smem_optin ? 1 : 0;
-    const size_t sm = sm_top + (in_smem ? sm_b : 0);
-    if (sm > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    k_assign<<<1, AS_T, sm, c->stream>>>(d_topk, nA, nB, num_best, dSA, d_pairs, F->d_io + oD, in_smem);
-  }
-  c->launches += 2;
-  FE_CUDA(c, cudaGetLastError());
-  FE_CUDA(c, cudaMemcpyAsync(F->h_stage + oT, F->d_io + oT, oD - oT, cudaMemcpyDeviceToHost, c->stream));
-  FE_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (out_topk) std::memcpy(out_topk, F->h_stage + oT, sizeof(okb_pair) * (size_t)nA * num_best);
-  std::memcpy(out_pairs, F->h_stage + oP, sizeof(okb_pair) * (size_t)nB);
-  return OKB_OK;
+  return match_run(c, F->match_io, c->stream, 1, &j, desc_bytes);
 }
 
 extern "C" int okb_hamming_match(okb_ctx* c, const uint8_t* A, int nA, const uint8_t* B, int nB, int desc_bytes, const uint8_t* skipA,
                                  const uint8_t* skipB, float threshold, int num_best, int use_ratio, float ratio_threshold,
                                  okb_pair* out_topk, okb_pair* out_pairs) {
   (void)ratio_threshold;   // the ratio test itself belongs to the serial epilogue on the caller's side
-  return hamming_match_impl(c, A, nA, B, nB, desc_bytes, skipA, skipB, threshold, num_best, use_ratio, nullptr, out_topk, out_pairs);
+  return hamming_match_single(c, A, nA, B, nB, desc_bytes, skipA, skipB, threshold, num_best, use_ratio, nullptr, out_topk, out_pairs);
 }
 
 extern "C" int okb_hamming_match_gated(okb_ctx* c, const uint8_t* A, int nA, const uint8_t* B, int nB, int desc_bytes, const uint8_t* skipA,
@@ -1268,7 +1541,18 @@ extern "C" int okb_hamming_match_gated(okb_ctx* c, const uint8_t* A, int nA, con
                                        const okb_match_gate* gate, okb_pair* out_topk, okb_pair* out_pairs) {
   (void)ratio_threshold;
   if (!gate) return OKB_ERR_INVALID_ARG;
-  return hamming_match_impl(c, A, nA, B, nB, desc_bytes, skipA, skipB, threshold, num_best, use_ratio, gate, out_topk, out_pairs);
+  return hamming_match_single(c, A, nA, B, nB, desc_bytes, skipA, skipB, threshold, num_best, use_ratio, gate, out_topk, out_pairs);
+}
+
+extern "C" int okb_hamming_match_batch(okb_ctx* c, int n_jobs, const okb_match_job* jobs, int desc_bytes) {
+  if (!c || n_jobs < 0) return OKB_ERR_INVALID_ARG;
+  if (n_jobs == 0) return OKB_OK;
+  if (n_jobs > 65535 || !jobs) return OKB_ERR_INVALID_ARG;        // the job index is a grid dimension
+  cudaSetDevice(c->device);
+  okb_frontend_state* F = fe(c);
+  std::lock_guard<std::mutex> lk(F->batch_mtx);
+  if (!F->batch_stream) FE_CUDA(c, cudaStreamCreateWithFlags(&F->batch_stream, cudaStreamNonBlocking));
+  return match_run(c, F->batch_match, F->batch_stream, n_jobs, jobs, desc_bytes);
 }
 
 extern "C" int okb_hamming_candidates(okb_ctx* c, const uint8_t* A, int nA, const uint8_t* B, int nB, int desc_bytes, float threshold,
@@ -1304,7 +1588,7 @@ extern "C" int okb_hamming_candidates(okb_ctx* c, const uint8_t* A, int nA, cons
                         reinterpret_cast<const uint32_t*>(F->d_A), nA, reinterpret_cast<const uint32_t*>(F->d_B), nB, threshold, d_counts,
                         F->d_rowptr, F->d_col, F->d_dist, cap, 1)));
   }
-  c->launches += 3;
+  F->launches += 3;
   FE_CUDA(c, cudaGetLastError());
   FE_CUDA(c, cudaMemcpyAsync(row_ptr, F->d_rowptr, sizeof(uint32_t) * (nA + 1), cudaMemcpyDeviceToHost, c->stream));
   FE_CUDA(c, cudaStreamSynchronize(c->stream));
