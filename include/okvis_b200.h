@@ -20,6 +20,7 @@
  *   okb_eval_marginalization  <- MarginalizationError::EvaluateWithMinimalJacobians okvis_ceres/src/MarginalizationError.cpp:893-946
  *   okb_window_marginalize    <- MarginalizationError::addResidualBlock / marginalizeOut / updateErrorComputation
  *                                okvis_ceres/src/MarginalizationError.cpp:127-435, 507-846 (driven by Estimator.cpp:434-773)
+ *   okb_window_marginalize_batch: no reference counterpart -- okb_window_marginalize on many resident windows in one launch
  *   okb_hamming_match         <- okvis::DenseMatcher::match            okvis_matcher/include/okvis/implementation/DenseMatcher.hpp:48-225
  *                                + assignbest                          okvis_matcher/src/DenseMatcher.cpp:69-110
  *   okb_hamming_match_gated   <- VioKeyframeWindowMatchingAlgorithm::distance + verifyMatch (hpp:132-144, cpp:304-339),
@@ -291,6 +292,16 @@ typedef struct okb_marg_job {
   const uint32_t* landmarks;        /* landmarks to marginalise: every observation they still have is linearised */
 } okb_marg_job;
 int okb_window_marginalize(okb_ctx* ctx, int win, const okb_marg_job* job);
+/* Batched okb_window_marginalize (no reference counterpart; serves hosts that keep many estimators on one GPU).
+ * jobs[i] describes slot win_first+i; jobs[i] == NULL: that slot is not touched (no commit, no wait on its solve, no
+ * copy), so its okb_optimize_async may still be running.  Each slot's result -- prior, H / b0, block list, x0, ImuError
+ * caches, download_marg status -- is bit-identical to okb_window_marginalize on it.  Every job is checked on the host
+ * before any device work: the first failure returns its status, names the slot in okb_last_error and leaves every
+ * slot unchanged.  count < 1 or a range outside max_windows: OKB_ERR_INVALID_ARG; all jobs NULL: no-op.  Pending
+ * edits of the job slots are committed first; one k_marginalize launch (one CTA per job) then runs on the transfer
+ * stream after the solver work already launched on the job slots only, and later calls on those slots are ordered
+ * after it.  Errors the device finds stay with their slot and surface as for the single call. */
+int okb_window_marginalize_batch(okb_ctx* ctx, int win_first, int count, const okb_marg_job* const* jobs);
 /* Reads the window's current marginalisation prior back (tests, host-side persistence): J [n][n], e0 [n], the
  * H / b0 it was factored from, block list, linearisation points.  Any pointer may be NULL; arrays must hold the
  * compiled-in maxima (n <= 160, 64 blocks).  status[4] = {device error code of the last okb_window_marginalize,

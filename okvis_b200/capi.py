@@ -163,6 +163,15 @@ class Context:
         """okb_window_marginalize; job from abi.make_marg_job."""
         self._check(lib().okb_window_marginalize(self._h, int(win), C.byref(job)))
 
+    def marginalize_batch(self, win_first, jobs):
+        """okb_window_marginalize_batch: jobs[i] (from abi.make_marg_job, or None to leave the slot alone) runs on slot
+        win_first + i."""
+        arr = (C.POINTER(abi.MargJob) * max(len(jobs), 1))()
+        for i, j in enumerate(jobs):
+            if j is not None:
+                arr[i] = C.pointer(j)
+        self._check(lib().okb_window_marginalize_batch(self._h, int(win_first), len(jobs), arr))
+
     def download_marg(self, win):
         n, nb = C.c_int32(0), C.c_int32(0)
         kind, idx = np.zeros(64, np.int32), np.zeros(64, np.uint32)

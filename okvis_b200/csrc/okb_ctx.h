@@ -70,6 +70,12 @@ struct okb_ctx {
   okb::SolverState* h_states = nullptr;  // pinned
   void* hook_buf = nullptr;
   size_t hook_bytes = 0;
+  // okb_window_marginalize*: task table + job payloads of a call, packed in pinned memory and copied in one piece
+  unsigned char* marg_host = nullptr;    // pinned
+  unsigned char* marg_dev = nullptr;
+  size_t marg_host_bytes = 0, marg_dev_bytes = 0;
+  cudaEvent_t marg_copied = nullptr;     // recorded after the H2D copy of marg_host
+  bool marg_busy = false;                // that copy may still be in flight (wait on marg_copied before rewriting)
   okb_frontend_state* frontend = nullptr;
   // landmark-sharded windows (okb_shard_*): this rank's mailbox and the peers' mailboxes as mapped on this device
   int shard_rank = 0, shard_world = 1, shard_box_cap = 0;

@@ -141,6 +141,9 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
   if (c->d_states) cudaFree(c->d_states);
   if (c->h_states) cudaFreeHost(c->h_states);
   if (c->hook_buf) cudaFree(c->hook_buf);
+  if (c->marg_host) cudaFreeHost(c->marg_host);
+  if (c->marg_dev) cudaFree(c->marg_dev);
+  if (c->marg_copied) cudaEventDestroy(c->marg_copied);
   for (auto& g : c->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   for (auto e : c->prof_events) cudaEventDestroy(e);
   if (c->ev_round) cudaEventDestroy(c->ev_round);
@@ -801,14 +804,12 @@ static int hook_alloc_fwd(okb_ctx* c, size_t bytes);
 static int check_range(okb_ctx* c, int first, int count);
 namespace {
 constexpr int kMargImuCap = 32, kMargSbpCap = 8;
-struct MargLayout { size_t kind, idx, prev, marg, imu, sbp, lms, payload_end, H, b, A, Q, T, Hn, bn, xlin, lmrec, lmV, lmvis, lmslot, clist, status, total; };
+// Work arrays and status word of one slot (WinStore::marg_scratch).
+struct MargLayout { size_t H, b, A, Q, T, Hn, bn, xlin, lmrec, lmV, lmvis, lmslot, clist, status, total; };
 MargLayout marg_layout(int lm_cap, int K_cap, int L_cap, int O_cap) {
   MargLayout m;
-  size_t o = sizeof(MargJobHeader);
+  size_t o = 0;
   auto take = [&](size_t bytes) { const size_t r = o; o = align_up(o + bytes, 16); return r; };
-  m.kind = take(4 * kMaxMargBlocks); m.idx = take(4 * kMaxMargBlocks); m.prev = take(4 * kMaxMargBlocks); m.marg = take(kMaxMargBlocks);
-  m.imu = take(4 * kMargImuCap); m.sbp = take(4 * kMargSbpCap); m.lms = take(4 * (size_t)lm_cap);
-  m.payload_end = o;
   const size_t NN = (size_t)kMargWork * kMargWork * 8;
   m.H = take(NN); m.b = take(8 * kMargWork); m.A = take(NN); m.Q = take(NN); m.T = take(NN); m.Hn = take(NN); m.bn = take(8 * kMargWork);
   m.xlin = take(8 * 9 * kMaxMargBlocks);
@@ -817,13 +818,25 @@ MargLayout marg_layout(int lm_cap, int K_cap, int L_cap, int O_cap) {
   m.total = o;
   return m;
 }
-MargScratch marg_pointers(unsigned char* base, const MargLayout& m) {
+// One job in the batch buffer of a call: header, then its index lists.
+struct MargPayload { size_t kind, idx, prev, marg, imu, sbp, lms, total; };
+MargPayload marg_payload(const okb_marg_job* job) {
+  MargPayload p;
+  size_t o = align_up(sizeof(MargJobHeader), 16);
+  auto take = [&](size_t bytes) { const size_t r = o; o = align_up(o + bytes, 16); return r; };
+  const size_t nb = (size_t)job->n_blocks;
+  p.kind = take(4 * nb); p.idx = take(4 * nb); p.prev = take(4 * nb); p.marg = take(nb);
+  p.imu = take(4 * (size_t)job->n_imu_terms); p.sbp = take(4 * (size_t)job->n_sb_priors); p.lms = take(4 * (size_t)job->n_landmarks);
+  p.total = o;
+  return p;
+}
+MargScratch marg_pointers(unsigned char* job, const MargPayload& p, unsigned char* base, const MargLayout& m) {
   MargScratch sc;
-  sc.hdr = reinterpret_cast<MargJobHeader*>(base);
-  sc.kind = reinterpret_cast<int32_t*>(base + m.kind); sc.idx = reinterpret_cast<uint32_t*>(base + m.idx);
-  sc.prev = reinterpret_cast<int32_t*>(base + m.prev); sc.marg = base + m.marg;
-  sc.imu_terms = reinterpret_cast<uint32_t*>(base + m.imu); sc.sb_priors = reinterpret_cast<uint32_t*>(base + m.sbp);
-  sc.landmarks = reinterpret_cast<uint32_t*>(base + m.lms);
+  sc.hdr = reinterpret_cast<MargJobHeader*>(job);
+  sc.kind = reinterpret_cast<int32_t*>(job + p.kind); sc.idx = reinterpret_cast<uint32_t*>(job + p.idx);
+  sc.prev = reinterpret_cast<int32_t*>(job + p.prev); sc.marg = job + p.marg;
+  sc.imu_terms = reinterpret_cast<uint32_t*>(job + p.imu); sc.sb_priors = reinterpret_cast<uint32_t*>(job + p.sbp);
+  sc.landmarks = reinterpret_cast<uint32_t*>(job + p.lms);
   auto dp = [&](size_t o) { return reinterpret_cast<double*>(base + o); };
   sc.H = dp(m.H); sc.b = dp(m.b); sc.A = dp(m.A); sc.Q = dp(m.Q); sc.T = dp(m.T); sc.Hn = dp(m.Hn); sc.bn = dp(m.bn); sc.xlin = dp(m.xlin);
   sc.lmrec = dp(m.lmrec); sc.lmV = dp(m.lmV); sc.lmvis = reinterpret_cast<uint32_t*>(base + m.lmvis);
@@ -831,71 +844,163 @@ MargScratch marg_pointers(unsigned char* base, const MargLayout& m) {
   sc.status = reinterpret_cast<int32_t*>(base + m.status);
   return sc;
 }
+
+// Dimensions of a job that passed marg_check.
+struct MargDims { int N = 0, n_keep = 0, nb_keep = 0, xdim = 0; };
+// Host checks of one job against the slot as the host mirror describes it (pending edits included).  On failure
+// returns the status and sets *why.
+int marg_check(const okb_ctx* c, int win, const okb_marg_job* job, MargDims& d, const char** why) {
+  if (!c->wins[win].uploaded) { *why = "window slot not uploaded"; return OKB_ERR_INVALID_ARG; }
+  const WinStore& S = c->wins[win];
+  const WinDev& W = c->host[win];
+  if (job->n_blocks < 1 || job->n_blocks > kMaxMargBlocks || job->n_imu_terms < 0 || job->n_imu_terms > kMargImuCap || job->n_sb_priors < 0 ||
+      job->n_sb_priors > kMargSbpCap || job->n_landmarks < 0 || !job->block_kind || !job->block_idx || !job->block_prev || !job->block_marginalize ||
+      (job->n_imu_terms && !job->imu_terms) || (job->n_sb_priors && !job->sb_priors) || (job->n_landmarks && !job->landmarks)) {
+    *why = "malformed job";
+    return OKB_ERR_INVALID_ARG;
+  }
+  d = MargDims();
+  for (int b = 0; b < job->n_blocks; ++b) {
+    const int kind = job->block_kind[b];
+    if (kind != OKB_BLOCK_POSE && kind != OKB_BLOCK_SPEED_BIAS) { *why = "block kind must be pose or speed/bias (extrinsics are fixed)"; return OKB_ERR_UNSUPPORTED; }
+    const int lim = kind == OKB_BLOCK_POSE ? W.K : W.NSB;
+    if ((int)job->block_idx[b] >= lim || job->block_prev[b] < -1 || job->block_prev[b] >= W.marg_nb) { *why = "block index out of range"; return OKB_ERR_INVALID_ARG; }
+    const int dim = kind == OKB_BLOCK_SPEED_BIAS ? 9 : 6;
+    d.N += dim;
+    if (!job->block_marginalize[b]) { d.n_keep += dim; d.nb_keep += 1; d.xdim += (kind == OKB_BLOCK_SPEED_BIAS) ? 9 : 7; }
+  }
+  for (int i = 0; i < job->n_imu_terms; ++i) if ((int)job->imu_terms[i] >= W.n_imu) { *why = "IMU term index out of range"; return OKB_ERR_INVALID_ARG; }
+  for (int i = 0; i < job->n_sb_priors; ++i) if ((int)job->sb_priors[i] >= W.n_sbp) { *why = "prior index out of range"; return OKB_ERR_INVALID_ARG; }
+  for (int i = 0; i < job->n_landmarks; ++i) if ((int)job->landmarks[i] >= W.L) { *why = "landmark index out of range"; return OKB_ERR_INVALID_ARG; }
+  if (d.N > kMargWork) { *why = "linear system larger than the compiled-in limit"; return OKB_ERR_CAPACITY; }
+  if (d.n_keep > kMaxMarg || d.n_keep > S.caps.MN) { *why = "resulting prior larger than reserved (okb_window_reserve max_marg_dim)"; return OKB_ERR_CAPACITY; }
+  return OKB_OK;
+}
+
+// The one path behind okb_window_marginalize (n = 1) and okb_window_marginalize_batch: jobs[t] runs on slot slots[t]
+// (ascending, distinct).  Every job is checked before any device work.  Then, on the transfer stream: the pending
+// edits of the job slots are committed, the task table and the job payloads go over in one H2D copy, each run of
+// consecutive job slots gets one WinDev copy, and one k_marginalize launch runs one CTA per job after the solver
+// work already launched on those slots.  Other slots are not touched.
+int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int n, bool batch) {
+  cudaSetDevice(c->device);
+  std::vector<MargDims> dims(n);
+  for (int t = 0; t < n; ++t) {
+    const char* why = "";
+    const int rc = marg_check(c, slots[t], jobs[t], dims[t], &why);
+    if (rc) {
+      c->set_error(batch ? "okb_window_marginalize_batch: slot " + std::to_string(slots[t]) + ": " + why : std::string("okb_window_marginalize: ") + why);
+      return rc;
+    }
+  }
+  cudaStream_t xs = c->stream_xfer;
+  // scratch of the job slots and the call's device buffer: growing frees the old ones, which waits for the transfer
+  // stream once
+  size_t bytes = align_up(sizeof(MargTask) * (size_t)n, 256);
+  std::vector<MargPayload> pay(n);
+  std::vector<size_t> off(n);
+  for (int t = 0; t < n; ++t) { pay[t] = marg_payload(jobs[t]); off[t] = bytes; bytes += pay[t].total; }
+  std::vector<char> grow(n, 0);
+  bool wait = c->marg_dev && bytes > c->marg_dev_bytes;
+  for (int t = 0; t < n; ++t) {
+    const WinStore& S = c->wins[slots[t]];
+    grow[t] = !S.marg_scratch || S.marg_lm_cap < jobs[t]->n_landmarks || S.marg_K_cap < S.caps.K || S.marg_L_cap < S.caps.L || S.marg_O_cap < S.caps.O;
+    wait = wait || (grow[t] && S.marg_scratch);
+  }
+  if (wait) OKB_CUDA(c, cudaStreamSynchronize(xs));
+  for (int t = 0; t < n; ++t) {
+    if (!grow[t]) continue;
+    WinStore& S = c->wins[slots[t]];
+    if (S.marg_scratch) { cudaFree(S.marg_scratch); S.marg_scratch = nullptr; }
+    S.marg_lm_cap = std::max(256, 2 * jobs[t]->n_landmarks); S.marg_K_cap = S.caps.K; S.marg_L_cap = S.caps.L; S.marg_O_cap = S.caps.O;
+    const MargLayout m = marg_layout(S.marg_lm_cap, S.marg_K_cap, S.marg_L_cap, S.marg_O_cap);
+    OKB_CUDA(c, cudaMalloc(&S.marg_scratch, m.total));
+    S.marg_scratch_bytes = m.total;
+    OKB_CUDA(c, cudaMemsetAsync(S.marg_scratch, 0, m.total, xs));
+  }
+  if (bytes > c->marg_dev_bytes) {
+    const size_t cap = align_up(std::max(bytes, std::max((size_t)64 << 10, 2 * c->marg_dev_bytes)), 4096);
+    if (c->marg_dev) cudaFree(c->marg_dev);
+    c->marg_dev = nullptr; c->marg_dev_bytes = 0;
+    OKB_CUDA(c, cudaMalloc(&c->marg_dev, cap));
+    c->marg_dev_bytes = cap;
+  }
+  // pending graph edits first: the jobs index the windows as they are now
+  std::vector<std::pair<int, int>> runs;       // (first slot, count) of consecutive job slots
+  for (int t = 0; t < n; ++t) {
+    if (!runs.empty() && runs.back().first + runs.back().second == slots[t]) runs.back().second += 1;
+    else runs.emplace_back(slots[t], 1);
+  }
+  for (const auto& r : runs) {
+    const int rc = commit_range(c, r.first, r.second);
+    if (rc) return rc;
+  }
+  // pack: the previous call's copy reads the pinned buffer until marg_copied
+  if (!c->marg_copied) OKB_CUDA(c, cudaEventCreateWithFlags(&c->marg_copied, cudaEventDisableTiming));
+  if (c->marg_busy) { OKB_CUDA(c, cudaEventSynchronize(c->marg_copied)); c->marg_busy = false; }
+  if (bytes > c->marg_host_bytes) {
+    if (c->marg_host) cudaFreeHost(c->marg_host);
+    c->marg_host = nullptr; c->marg_host_bytes = 0;
+    const size_t cap = c->marg_dev_bytes;
+    OKB_CUDA(c, cudaMallocHost(&c->marg_host, cap));
+    c->marg_host_bytes = cap;
+  }
+  MargTask* tasks = reinterpret_cast<MargTask*>(c->marg_host);
+  for (int t = 0; t < n; ++t) {
+    const okb_marg_job* job = jobs[t];
+    const WinStore& S = c->wins[slots[t]];
+    const MargPayload& p = pay[t];
+    unsigned char* q = c->marg_host + off[t];
+    std::memset(q, 0, p.total);
+    const MargJobHeader h{job->n_blocks, job->n_imu_terms, job->n_sb_priors, job->n_landmarks, dims[t].N, dims[t].n_keep, S.marg_lm_cap, 0};
+    std::memcpy(q, &h, sizeof h);
+    std::memcpy(q + p.kind, job->block_kind, 4 * (size_t)job->n_blocks);
+    std::memcpy(q + p.idx, job->block_idx, 4 * (size_t)job->n_blocks);
+    std::memcpy(q + p.prev, job->block_prev, 4 * (size_t)job->n_blocks);
+    std::memcpy(q + p.marg, job->block_marginalize, (size_t)job->n_blocks);
+    if (job->n_imu_terms) std::memcpy(q + p.imu, job->imu_terms, 4 * (size_t)job->n_imu_terms);
+    if (job->n_sb_priors) std::memcpy(q + p.sbp, job->sb_priors, 4 * (size_t)job->n_sb_priors);
+    if (job->n_landmarks) std::memcpy(q + p.lms, job->landmarks, 4 * (size_t)job->n_landmarks);
+    MargTask task{};
+    task.win = slots[t];
+    task.sc = marg_pointers(c->marg_dev + off[t], p, S.marg_scratch, marg_layout(S.marg_lm_cap, S.marg_K_cap, S.marg_L_cap, S.marg_O_cap));
+    tasks[t] = task;
+  }
+  // after the solver work already launched on the job slots
+  bool waited[okb_ctx::kDoneRing] = {};
+  for (int t = 0; t < n; ++t) {
+    const int k = c->wins[slots[t]].done_idx;
+    if (k >= 0 && !waited[k]) { OKB_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[k], 0)); waited[k] = true; }
+  }
+  OKB_CUDA(c, cudaMemcpyAsync(c->marg_dev, c->marg_host, bytes, cudaMemcpyHostToDevice, xs));
+  OKB_CUDA(c, cudaEventRecord(c->marg_copied, xs));
+  c->marg_busy = true;
+  for (const auto& r : runs)
+    OKB_CUDA(c, cudaMemcpyAsync(c->d_wins + r.first, &c->host[r.first], sizeof(WinDev) * r.second, cudaMemcpyHostToDevice, xs));
+  k_marginalize<<<n, M_THREADS, 0, xs>>>(c->d_wins, reinterpret_cast<const MargTask*>(c->marg_dev));
+  c->launches += 1;
+  OKB_CUDA(c, cudaGetLastError());
+  for (int t = 0; t < n; ++t) {
+    WinDev& W = c->host[slots[t]];
+    W.marg_n = dims[t].n_keep; W.marg_nb = dims[t].nb_keep; W.marg_xdim = dims[t].xdim;
+  }
+  return OKB_OK;
+}
 }  // namespace
 
 extern "C" int okb_window_marginalize(okb_ctx* c, int win, const okb_marg_job* job) {
   if (!c || !job || win < 0 || win >= c->max_windows) return OKB_ERR_INVALID_ARG;
-  if (!c->wins[win].uploaded) { c->set_error("window slot not uploaded"); return OKB_ERR_INVALID_ARG; }
-  cudaSetDevice(c->device);
-  int rc = commit_range(c, win, 1);            // pending graph edits first: the job indexes the window as it is now
-  if (rc) return rc;
-  WinStore& S = c->wins[win];
-  WinDev& W = c->host[win];
-  if (job->n_blocks < 1 || job->n_blocks > kMaxMargBlocks || job->n_imu_terms < 0 || job->n_imu_terms > kMargImuCap || job->n_sb_priors < 0 ||
-      job->n_sb_priors > kMargSbpCap || job->n_landmarks < 0 || !job->block_kind || !job->block_idx || !job->block_prev || !job->block_marginalize) {
-    c->set_error("okb_window_marginalize: malformed job");
-    return OKB_ERR_INVALID_ARG;
-  }
-  int N = 0, n_keep = 0, nb_keep = 0, xdim = 0;
-  for (int b = 0; b < job->n_blocks; ++b) {
-    const int kind = job->block_kind[b];
-    if (kind != OKB_BLOCK_POSE && kind != OKB_BLOCK_SPEED_BIAS) { c->set_error("okb_window_marginalize: block kind must be pose or speed/bias (extrinsics are fixed)"); return OKB_ERR_UNSUPPORTED; }
-    const int lim = kind == OKB_BLOCK_POSE ? W.K : W.NSB;
-    if ((int)job->block_idx[b] >= lim || job->block_prev[b] < -1 || job->block_prev[b] >= W.marg_nb) { c->set_error("okb_window_marginalize: block index out of range"); return OKB_ERR_INVALID_ARG; }
-    const int dim = kind == OKB_BLOCK_SPEED_BIAS ? 9 : 6;
-    N += dim;
-    if (!job->block_marginalize[b]) { n_keep += dim; nb_keep += 1; xdim += (kind == OKB_BLOCK_SPEED_BIAS) ? 9 : 7; }
-  }
-  for (int i = 0; i < job->n_imu_terms; ++i) if ((int)job->imu_terms[i] >= W.n_imu) { c->set_error("okb_window_marginalize: IMU term index out of range"); return OKB_ERR_INVALID_ARG; }
-  for (int i = 0; i < job->n_sb_priors; ++i) if ((int)job->sb_priors[i] >= W.n_sbp) { c->set_error("okb_window_marginalize: prior index out of range"); return OKB_ERR_INVALID_ARG; }
-  for (int i = 0; i < job->n_landmarks; ++i) if ((int)job->landmarks[i] >= W.L) { c->set_error("okb_window_marginalize: landmark index out of range"); return OKB_ERR_INVALID_ARG; }
-  if (N > kMargWork) { c->set_error("okb_window_marginalize: linear system larger than the compiled-in limit"); return OKB_ERR_CAPACITY; }
-  if (n_keep > kMaxMarg || n_keep > S.caps.MN) { c->set_error("okb_window_marginalize: resulting prior larger than reserved (okb_window_reserve max_marg_dim)"); return OKB_ERR_CAPACITY; }
-  // scratch
-  if (!S.marg_scratch || S.marg_lm_cap < job->n_landmarks || S.marg_K_cap < S.caps.K || S.marg_L_cap < S.caps.L || S.marg_O_cap < S.caps.O) {
-    if (S.marg_scratch) { OKB_CUDA(c, cudaStreamSynchronize(c->stream_xfer)); cudaFree(S.marg_scratch); S.marg_scratch = nullptr; }
-    S.marg_lm_cap = std::max(256, 2 * job->n_landmarks); S.marg_K_cap = S.caps.K; S.marg_L_cap = S.caps.L; S.marg_O_cap = S.caps.O;
-    const MargLayout m = marg_layout(S.marg_lm_cap, S.marg_K_cap, S.marg_L_cap, S.marg_O_cap);
-    OKB_CUDA(c, cudaMalloc(&S.marg_scratch, m.total));
-    S.marg_scratch_bytes = m.total;
-    OKB_CUDA(c, cudaMemsetAsync(S.marg_scratch, 0, m.total, c->stream_xfer));
-  }
-  const MargLayout m = marg_layout(S.marg_lm_cap, S.marg_K_cap, S.marg_L_cap, S.marg_O_cap);
-  rc = cmd_reserve(c, S, m.payload_end);
-  if (rc) return rc;
-  unsigned char* q = S.staging;
-  std::memset(q, 0, m.payload_end);
-  MargJobHeader h{job->n_blocks, job->n_imu_terms, job->n_sb_priors, job->n_landmarks, N, n_keep, S.marg_lm_cap, 0};
-  std::memcpy(q, &h, sizeof h);
-  std::memcpy(q + m.kind, job->block_kind, 4 * (size_t)job->n_blocks);
-  std::memcpy(q + m.idx, job->block_idx, 4 * (size_t)job->n_blocks);
-  std::memcpy(q + m.prev, job->block_prev, 4 * (size_t)job->n_blocks);
-  std::memcpy(q + m.marg, job->block_marginalize, (size_t)job->n_blocks);
-  if (job->n_imu_terms) std::memcpy(q + m.imu, job->imu_terms, 4 * (size_t)job->n_imu_terms);
-  if (job->n_sb_priors) std::memcpy(q + m.sbp, job->sb_priors, 4 * (size_t)job->n_sb_priors);
-  if (job->n_landmarks) std::memcpy(q + m.lms, job->landmarks, 4 * (size_t)job->n_landmarks);
-  cudaStream_t xs = c->stream_xfer;
-  if (S.done_idx >= 0) OKB_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
-  OKB_CUDA(c, cudaMemcpyAsync(S.marg_scratch, q, m.payload_end, cudaMemcpyHostToDevice, xs));
-  OKB_CUDA(c, cudaEventRecord(S.copied, xs));
-  S.staging_busy = true;
-  OKB_CUDA(c, cudaMemsetAsync(S.marg_scratch + m.status, 0, 16, xs));
-  OKB_CUDA(c, cudaMemcpyAsync(c->d_wins + win, &W, sizeof(WinDev), cudaMemcpyHostToDevice, xs));
-  k_marginalize<<<1, M_THREADS, 0, xs>>>(c->d_wins, win, marg_pointers(S.marg_scratch, m));
-  c->launches += 1;
-  OKB_CUDA(c, cudaGetLastError());
-  W.marg_n = n_keep; W.marg_nb = nb_keep; W.marg_xdim = xdim;
-  return OKB_OK;
+  return marg_run(c, &win, &job, 1, false);
+}
+
+extern "C" int okb_window_marginalize_batch(okb_ctx* c, int win_first, int count, const okb_marg_job* const* jobs) {
+  if (!c || !jobs || win_first < 0 || count < 1 || count > c->max_windows - win_first) return OKB_ERR_INVALID_ARG;
+  std::vector<int> slots;
+  std::vector<const okb_marg_job*> js;
+  for (int i = 0; i < count; ++i)
+    if (jobs[i]) { slots.push_back(win_first + i); js.push_back(jobs[i]); }
+  if (slots.empty()) return OKB_OK;
+  return marg_run(c, slots.data(), js.data(), (int)slots.size(), true);
 }
 
 extern "C" int okb_window_download_marg(okb_ctx* c, int win, int32_t* n, int32_t* n_blocks, int32_t* block_kind, uint32_t* block_idx, double* x0,

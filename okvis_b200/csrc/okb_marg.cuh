@@ -32,7 +32,7 @@ constexpr int M_THREADS = 256;
 constexpr int kMargRec = 72;            // doubles per (landmark, frame) record: W 18 | Z 18 | U 21 | bp 6 | Wy 6 | pad
 enum { MERR_BLOCK = 1, MERR_PREV = 2, MERR_TERM = 3, MERR_POSE_NOT_CONNECTED = 4, MERR_DIM = 5 };
 
-// Job as laid out in the slot's device scratch (header, then the index lists, 8-byte aligned).
+// Job as laid out in the batch buffer of the call (header, then the index lists, 16-byte aligned).
 struct MargJobHeader {
   int32_t n_blocks, n_imu, n_sbp, n_lm;
   int32_t N;              // dimension of the system before marginalising
@@ -41,10 +41,12 @@ struct MargJobHeader {
   int32_t _pad;
 };
 
-struct MargScratch {      // carved out of one device buffer per slot (okb_window_marginalize)
+struct MargScratch {
+  // the job: in the batch buffer of the call
   MargJobHeader* hdr;
   int32_t* kind; uint32_t* idx; int32_t* prev; uint8_t* marg;
   uint32_t* imu_terms; uint32_t* sb_priors; uint32_t* landmarks;
+  // work arrays and status: carved out of one device buffer per slot (WinStore::marg_scratch)
   double* H;              // [N][N] work system
   double* b;              // [N]
   double* A;              // [N][N] eigen work
@@ -60,6 +62,13 @@ struct MargScratch {      // carved out of one device buffer per slot (okb_windo
   int32_t* clist;         // [Ocap] indices of the observations to linearise, list order
   int32_t* status;        // [4]: error code, rank of the final H, rank of the dense V, sweeps
 };
+
+// One entry of k_marginalize's task table per CTA: the window it marginalises and where its job and scratch lie.
+struct alignas(16) MargTask {
+  int32_t win, _pad[3];
+  MargScratch sc;
+};
+static_assert(sizeof(MargTask) % 16 == 0, "MargTask is copied as 16-byte words");
 
 // 3x3 symmetric eigen-decomposition by cyclic Jacobi (S packed: 00 01 02 11 12 22); Q columns = eigenvectors
 __device__ inline void eig3_jacobi(const double* S, double* ev, double* Q) {
@@ -155,8 +164,15 @@ __device__ inline int jacobi_eig(double* A, double* Q, int n, double* s_cs /* [2
 
 __device__ __forceinline__ double marg_precond(double hii) { return (hii > 1.0e-9) ? sqrt(hii) : 1.0e-3; }
 
-__global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restrict__ wins, int win, MargScratch sc) {
-  const WinDev& W = wins[win];
+// One CTA per task: CTA b marginalises window tasks[b].win with the job and scratch of tasks[b].sc.  The task is
+// copied to shared memory once; the phases read its pointers from there.
+__global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restrict__ wins, const MargTask* __restrict__ tasks) {
+  __shared__ MargTask s_task;
+  if (threadIdx.x < sizeof(MargTask) / 16)
+    reinterpret_cast<int4*>(&s_task)[threadIdx.x] = reinterpret_cast<const int4*>(tasks + blockIdx.x)[threadIdx.x];
+  __syncthreads();
+  const MargScratch& sc = s_task.sc;
+  const WinDev& W = wins[s_task.win];
   GraphState* g = &W.st->g;
   const MargJobHeader J = *sc.hdr;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -174,6 +190,7 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
   // ---------------- phase 0: layout + linearisation points
   if (tid == 0) {
     int col = 0, err = 0;
+    for (int k = 0; k < 4; ++k) sc.status[k] = 0;     // this call's status word (read by okb_window_download_marg)
     for (int f = 0; f < kMaxFrames; ++f) { s_pose_blk[f] = -1; s_sb_blk[f] = -1; }
     for (int b = 0; b < NB; ++b) {
       const int kind = sc.kind[b];
