@@ -14,6 +14,7 @@
  *                                okvis_ceres/include/okvis/ceres/implementation/ReprojectionError.hpp:87-242
  *   okb_eval_imu              <- ImuError::EvaluateWithMinimalJacobians okvis_ceres/src/ImuError.cpp:514-685
  *   okb_imu_propagate         <- ImuError::propagation (static)        okvis_ceres/src/ImuError.cpp:287-504
+ *   okb_imu_propagate_batch: no reference counterpart -- okb_imu_propagate for many sessions in one launch
  *   okb_eval_pose_error       <- PoseError::EvaluateWithMinimalJacobians         okvis_ceres/src/PoseError.cpp:86-136
  *   okb_eval_speed_bias_error <- SpeedAndBiasError::EvaluateWithMinimalJacobians okvis_ceres/src/SpeedAndBiasError.cpp:89-116
  *   okb_eval_relative_pose    <- RelativePoseError::EvaluateWithMinimalJacobians okvis_ceres/src/RelativePoseError.cpp:84-162
@@ -385,6 +386,34 @@ int okb_eval_imu(okb_ctx* ctx, const okb_imu_params* params, const okb_imu_sampl
 int okb_imu_propagate(okb_ctx* ctx, const okb_imu_params* params, const okb_imu_sample* samples, int n_samples,
                       int64_t t0_ns, int64_t t1_ns, double* pose /*7 in/out*/, double* sb /*9 in/out*/,
                       double* covariance /*15x15 or NULL*/, double* jacobian /*15x15 or NULL*/, int* n_used);
+
+/* One ImuError::propagation of a batch (one session's prediction). */
+typedef struct okb_propagate_job {
+  const okb_imu_params* params;        /* per job: sessions may have different IMUs */
+  const okb_imu_sample* samples;       /* host, n_samples >= 2, as okb_imu_propagate */
+  int32_t n_samples, _pad;
+  int64_t t0_ns, t1_ns;
+  double* pose;                        /* 7, in/out */
+  double* speed_bias;                  /* 9, in/out */
+  double* covariance;                  /* 15x15 or NULL */
+  double* jacobian;                    /* 15x15 or NULL */
+  int32_t* n_used;                     /* or NULL */
+} okb_propagate_job;
+/* Batched okb_imu_propagate (no reference counterpart; serves hosts that keep many sessions on one GPU and predict
+ * all of them per camera frame or per IMU sample).  Each job's outputs -- pose, speed/bias, covariance, Jacobian,
+ * n_used -- are bit-identical to okb_imu_propagate on the same arguments.  As there, a job whose samples end before
+ * t1_ns gets n_used = -1 and its pose, speed/bias, covariance and Jacobian are left untouched; the call still returns
+ * OKB_OK.  Every job is checked on the host before any device work, with the single call's checks: the first failure
+ * returns OKB_ERR_INVALID_ARG, names the job index in okb_last_error and writes no job's outputs.  n_jobs == 0 is a
+ * no-op; n_jobs < 0, or jobs == NULL with n_jobs > 0, is invalid.
+ * Each call makes one H2D copy, one launch (one warp per job), one D2H copy and one synchronisation, whatever n_jobs
+ * is.  It runs on a stream of its own at the context's greatest priority and is serialised only with other
+ * propagation batches, so it never queues behind an okb_optimize_async, an okb_window_marginalize_batch or a frontend
+ * batch on the context, and it may run beside the single-block hooks.  okb_imu_propagate itself stays on the solver
+ * stream, ordered after solver work already launched.  Pinned and device buffers grow to the largest batch seen and
+ * are kept; a call that has to grow them frees the old ones, which waits for all work on the device (an
+ * okb_optimize_async in flight included).  Issue one batch of the largest size first to size them. */
+int okb_imu_propagate_batch(okb_ctx* ctx, int n_jobs, const okb_propagate_job* jobs);
 int okb_eval_pose_error(okb_ctx* ctx, const double* meas /*7*/, const double* sqrt_info /*36*/,
                         const double* pose /*7*/, double* r /*6*/, double* J /*6x6*/);
 int okb_eval_speed_bias_error(okb_ctx* ctx, const double* meas /*9*/, const double* sqrt_info /*81*/,

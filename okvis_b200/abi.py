@@ -111,6 +111,12 @@ class MatchJob(C.Structure):
                 ("gate", C.POINTER(MatchGate)), ("out_topk", C.c_void_p), ("out_pairs", C.c_void_p)]
 
 
+class PropagateJob(C.Structure):
+    _fields_ = [("params", C.POINTER(ImuParams)), ("samples", C.c_void_p), ("n_samples", C.c_int32), ("_pad", C.c_int32),
+                ("t0_ns", C.c_int64), ("t1_ns", C.c_int64), ("pose", c_double_p), ("speed_bias", c_double_p),
+                ("covariance", c_double_p), ("jacobian", c_double_p), ("n_used", C.POINTER(C.c_int32))]
+
+
 class WindowDesc(C.Structure):
     _fields_ = [("n_poses", C.c_int32), ("n_speed_bias", C.c_int32), ("n_extrinsics", C.c_int32),
                 ("n_landmarks", C.c_int32), ("n_cameras", C.c_int32), ("n_obs", C.c_int32),

@@ -321,15 +321,36 @@ class Context:
             self._check(rc)
         return r, J, sq, rc
 
-    def imu_propagate(self, params, samples, t0_ns, t1_ns, pose, sb, want_cov=True):
+    def imu_propagate(self, params, samples, t0_ns, t1_ns, pose, sb, want_cov=True, want_jac=True):
         pose, sb = np.array(pose, dtype=np.float64), np.array(sb, dtype=np.float64)
         samples = np.ascontiguousarray(samples)
         P, F = np.zeros((15, 15)), np.zeros((15, 15))
         n = C.c_int(0)
         self._check(lib().okb_imu_propagate(self._h, C.byref(params), _p(samples), len(samples), C.c_int64(int(t0_ns)),
-                                            C.c_int64(int(t1_ns)), _p(pose), _p(sb), _p(P) if want_cov else None, _p(F),
-                                            C.byref(n)))
+                                            C.c_int64(int(t1_ns)), _p(pose), _p(sb), _p(P) if want_cov else None,
+                                            _p(F) if want_jac else None, C.byref(n)))
         return n.value, pose, sb, P, F
+
+    def imu_propagate_batch(self, jobs):
+        """okb_imu_propagate_batch.  jobs: (params, samples, t0_ns, t1_ns, pose, sb[, want_cov[, want_jac]]) tuples, as
+        the arguments of imu_propagate.  Returns per job what imu_propagate returns."""
+        arr = (abi.PropagateJob * max(len(jobs), 1))()
+        out, keep = [], []
+        for j, job in zip(arr, jobs):
+            params, samples, t0_ns, t1_ns, pose, sb = job[:6]
+            want_cov, want_jac = (tuple(job[6:]) + (True, True))[:2]
+            pose, sb = np.array(pose, dtype=np.float64), np.array(sb, dtype=np.float64)
+            samples = np.ascontiguousarray(samples)
+            P, F, n = np.zeros((15, 15)), np.zeros((15, 15)), np.zeros(1, np.int32)
+            j.params, j.samples, j.n_samples = C.pointer(params), samples.ctypes.data, len(samples)
+            j.t0_ns, j.t1_ns = int(t0_ns), int(t1_ns)
+            j.pose, j.speed_bias = abi.dptr(pose), abi.dptr(sb)
+            j.covariance, j.jacobian = abi.dptr(P) if want_cov else None, abi.dptr(F) if want_jac else None
+            j.n_used = n.ctypes.data_as(C.POINTER(C.c_int32))
+            keep.append(samples)
+            out.append((n, pose, sb, P, F))
+        self._check(lib().okb_imu_propagate_batch(self._h, len(jobs), arr))
+        return [(int(n[0]), pose, sb, P, F) for n, pose, sb, P, F in out]
 
     def eval_pose_error(self, meas, sqrt_info, pose):
         r, J = np.zeros(6), np.zeros((6, 6))

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <atomic>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -42,6 +43,15 @@ struct WinStore {
   int marg_lm_cap = 0, marg_K_cap = 0, marg_L_cap = 0, marg_O_cap = 0;
 };
 
+// Buffers of okb_imu_propagate*: [job table | samples] in, [per-job outputs] out, in one pinned buffer and its device
+// mirror; they grow with the largest call and are kept.
+struct PropBuffers {
+  unsigned char* host = nullptr;     // pinned
+  unsigned char* dev = nullptr;
+  size_t bytes = 0;
+  std::mutex mtx;                    // serialises the calls that use these buffers
+};
+
 struct okb_frontend_state;
 
 struct okb_ctx {
@@ -76,6 +86,10 @@ struct okb_ctx {
   size_t marg_host_bytes = 0, marg_dev_bytes = 0;
   cudaEvent_t marg_copied = nullptr;     // recorded after the H2D copy of marg_host
   bool marg_busy = false;                // that copy may still be in flight (wait on marg_copied before rewriting)
+  // okb_imu_propagate (on `stream`) and okb_imu_propagate_batch (on stream_prop, created on first use) each own a set
+  PropBuffers prop_one, prop_batch;
+  cudaStream_t stream_prop = nullptr;
+  std::atomic<int64_t> prop_launches{0};   // counted apart from `launches`: a batch may run beside a solve's launches
   okb_frontend_state* frontend = nullptr;
   // landmark-sharded windows (okb_shard_*): this rank's mailbox and the peers' mailboxes as mapped on this device
   int shard_rank = 0, shard_world = 1, shard_box_cap = 0;

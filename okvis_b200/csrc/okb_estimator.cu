@@ -43,8 +43,9 @@ static void set_landmarks_attributes() {
 }
 
 // The transfer stream gets the highest priority: its small kernels (k_zero / k_prepare) are scheduled as soon
-// as CTA slots free up instead of waiting behind the solver kernels of other slots.
-static cudaError_t create_transfer_stream(cudaStream_t* s) {
+// as CTA slots free up instead of waiting behind the solver kernels of other slots.  The propagation stream gets it for
+// the same reason: its one-warp jobs are latency-bound.
+static cudaError_t create_high_priority_stream(cudaStream_t* s) {
   int lo = 0, hi = 0;
   cudaDeviceGetStreamPriorityRange(&lo, &hi);
   return cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, hi);
@@ -75,7 +76,7 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
   if (cudaStreamCreateWithPriority(&c->stream_imu, cudaStreamNonBlocking, prio_least) != cudaSuccess ||
       cudaEventCreateWithFlags(&c->ev_round, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&c->ev_imu, cudaEventDisableTiming) != cudaSuccess ||
-      create_transfer_stream(&c->stream_xfer) != cudaSuccess ||
+      create_high_priority_stream(&c->stream_xfer) != cudaSuccess ||
       cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess) {
     g_create_error = "cudaStreamCreate / cudaEventCreate failed";
     delete c;
@@ -144,6 +145,11 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
   if (c->marg_host) cudaFreeHost(c->marg_host);
   if (c->marg_dev) cudaFree(c->marg_dev);
   if (c->marg_copied) cudaEventDestroy(c->marg_copied);
+  for (PropBuffers* b : {&c->prop_one, &c->prop_batch}) {
+    if (b->host) cudaFreeHost(b->host);
+    if (b->dev) cudaFree(b->dev);
+  }
+  if (c->stream_prop) cudaStreamDestroy(c->stream_prop);
   for (auto& g : c->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   for (auto e : c->prof_events) cudaEventDestroy(e);
   if (c->ev_round) cudaEventDestroy(c->ev_round);
@@ -154,7 +160,9 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
 }
 
 extern "C" const char* okb_last_error(const okb_ctx* c) { return c ? c->error.c_str() : g_create_error.c_str(); }
-extern "C" int64_t okb_kernel_launches(const okb_ctx* c) { return c ? c->launches + okb_frontend_launches(c) : 0; }
+extern "C" int64_t okb_kernel_launches(const okb_ctx* c) {
+  return c ? c->launches + c->prop_launches.load() + okb_frontend_launches(c) : 0;
+}
 extern "C" void* okb_stream(const okb_ctx* c) { return c ? (void*)c->stream : nullptr; }
 
 // ---------------------------------------------------------------------------------------------
@@ -1583,13 +1591,32 @@ __global__ void k_hook_imu(okb_imu_params prm, const okb_imu_sample* s, int n, i
   for (int e = threadIdx.x; e < 225; e += 32) out[465 + e] = cache->sqrt_info[e];
   if (threadIdx.x == 0) out[690] = (double)(cache->redo_count - before);
 }
-__global__ void k_hook_propagate(okb_imu_params prm, const okb_imu_sample* s, int n, int64_t t0, int64_t t1, double* io /*16*/,
-                                 double* cov, double* jac, int want_cov, int want_jac, int* n_used) {
+// One job of k_propagate.  `samples` is a byte offset into the input region (job table | samples), `out` one into the
+// output region, where the job's record is pose 7 | speed/bias 9 | n_used (int32 in a double slot) | covariance 225
+// if want_cov | Jacobian 225 if want_jac.
+struct PropEntry {
+  okb_imu_params prm;
+  int64_t t0, t1;
+  uint64_t samples, out;
+  int32_t n, want_cov, want_jac, _pad;
+  double state[16];     // pose | speed/bias before the propagation
+};
+constexpr int kPropRecord = 17;   // doubles of an output record without covariance and Jacobian
+
+// One warp per job: ImuError::propagation with the job's scratch in shared memory.  The state is propagated in place in
+// the job's output record; imu_propagate leaves it unchanged when the samples end before t1 (n_used = -1).
+__global__ void __launch_bounds__(32) k_propagate(const unsigned char* __restrict__ in, unsigned char* __restrict__ out) {
   __shared__ double buf[kImuScratch];
+  const PropEntry& e = reinterpret_cast<const PropEntry*>(in)[blockIdx.x];
+  double* o = reinterpret_cast<double*>(out + e.out);
+  if (threadIdx.x < 16) o[threadIdx.x] = e.state[threadIdx.x];
+  __syncwarp();
+  double* cov = e.want_cov ? o + kPropRecord : nullptr;
+  double* jac = e.want_jac ? o + kPropRecord + (e.want_cov ? 225 : 0) : nullptr;
   WarpCtx cx;
-  const int steps = imu_propagate(cx, s, n, prm, t0, t1, io, io + 7, want_cov ? cov : nullptr, want_jac ? jac : nullptr,
-                                  imu_scratch(buf).wk);
-  if (threadIdx.x == 0) *n_used = steps;
+  const int steps = imu_propagate(cx, reinterpret_cast<const okb_imu_sample*>(in + e.samples), e.n, e.prm, e.t0, e.t1, o, o + 7,
+                                  cov, jac, imu_scratch(buf).wk);
+  if (threadIdx.x == 0) *reinterpret_cast<int32_t*>(o + 16) = steps;
 }
 __global__ void k_hook_pose(const double* in /* meas7 S36 pose7 */, double* out /* r6 J36 */) {
   if (threadIdx.x == 0) pose_error(in, in + 7, in + 43, out, out + 6);
@@ -1675,37 +1702,99 @@ extern "C" int okb_eval_imu(okb_ctx* c, const okb_imu_params* prm, const okb_imu
   return (int)h[690] > 0 ? 1 : 0;   // 1 = the evaluation re-preintegrated (not an error)
 }
 
+// The argument checks of okb_imu_propagate, per job: the reason a job is rejected, or nullptr.
+static const char* prop_invalid(const okb_propagate_job& j) {
+  if (!j.params) return "params is NULL";
+  if (!j.samples) return "samples is NULL";
+  if (j.n_samples < 2) return "n_samples < 2";
+  if (!j.pose) return "pose is NULL";
+  if (!j.speed_bias) return "speed_bias is NULL";
+  return nullptr;
+}
+
+// Propagates n checked jobs on stream st through buffers B (the caller holds B.mtx): one H2D copy of the job table and
+// all samples, one k_propagate launch (one warp per job), one D2H copy of the output records, one synchronisation.
+static int prop_run(okb_ctx* c, cudaStream_t st, PropBuffers& B, int n, const okb_propagate_job* jobs) {
+  std::vector<size_t> s_off(n), o_off(n);
+  size_t in_bytes = align_up(sizeof(PropEntry) * n, 256), out_bytes = 0;
+  for (int i = 0; i < n; ++i) {
+    s_off[i] = in_bytes;
+    in_bytes += align_up(sizeof(okb_imu_sample) * (size_t)jobs[i].n_samples, 16);
+    o_off[i] = out_bytes;
+    out_bytes += sizeof(double) * (kPropRecord + (jobs[i].covariance ? 225 : 0) + (jobs[i].jacobian ? 225 : 0));
+  }
+  const size_t out_at = align_up(in_bytes, 256), total = out_at + out_bytes;
+  if (total > B.bytes) {
+    if (B.host) cudaFreeHost(B.host);
+    if (B.dev) cudaFree(B.dev);
+    B.host = nullptr; B.dev = nullptr; B.bytes = 0;
+    const size_t cap = align_up(std::max(total, (size_t)64 << 10), 4096);
+    OKB_CUDA(c, cudaMallocHost(&B.host, cap));
+    OKB_CUDA(c, cudaMalloc(&B.dev, cap));
+    B.bytes = cap;
+  }
+  PropEntry* tab = reinterpret_cast<PropEntry*>(B.host);
+  for (int i = 0; i < n; ++i) {
+    const okb_propagate_job& j = jobs[i];
+    PropEntry& e = tab[i];
+    std::memset(&e, 0, sizeof e);
+    e.prm = *j.params;
+    e.t0 = j.t0_ns; e.t1 = j.t1_ns;
+    e.samples = s_off[i]; e.out = o_off[i];
+    e.n = j.n_samples; e.want_cov = j.covariance ? 1 : 0; e.want_jac = j.jacobian ? 1 : 0;
+    std::memcpy(e.state, j.pose, 7 * sizeof(double));
+    std::memcpy(e.state + 7, j.speed_bias, 9 * sizeof(double));
+    std::memcpy(B.host + s_off[i], j.samples, sizeof(okb_imu_sample) * (size_t)j.n_samples);
+  }
+  OKB_CUDA(c, cudaMemcpyAsync(B.dev, B.host, in_bytes, cudaMemcpyHostToDevice, st));
+  k_propagate<<<n, 32, 0, st>>>(B.dev, B.dev + out_at);
+  c->prop_launches += 1;
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(B.host + out_at, B.dev + out_at, out_bytes, cudaMemcpyDeviceToHost, st));
+  OKB_CUDA(c, cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i) {
+    const okb_propagate_job& j = jobs[i];
+    const double* o = reinterpret_cast<const double*>(B.host + out_at + o_off[i]);
+    int32_t used;
+    std::memcpy(&used, o + 16, sizeof used);
+    if (used >= 0) {
+      std::memcpy(j.pose, o, 7 * sizeof(double));
+      std::memcpy(j.speed_bias, o + 7, 9 * sizeof(double));
+      if (j.covariance) std::memcpy(j.covariance, o + kPropRecord, 225 * sizeof(double));
+      if (j.jacobian) std::memcpy(j.jacobian, o + kPropRecord + (j.covariance ? 225 : 0), 225 * sizeof(double));
+    }
+    if (j.n_used) *j.n_used = used;
+  }
+  return OKB_OK;
+}
+
+// A batch of one on the solver stream, so that it stays ordered after the solver work already launched.
 extern "C" int okb_imu_propagate(okb_ctx* c, const okb_imu_params* prm, const okb_imu_sample* samples, int n_samples,
                                  int64_t t0_ns, int64_t t1_ns, double* pose, double* sb, double* covariance, double* jacobian,
                                  int* n_used) {
-  if (!c || !prm || !samples || n_samples < 2 || !pose || !sb) return OKB_ERR_INVALID_ARG;
+  const okb_propagate_job j{prm, samples, n_samples, 0, t0_ns, t1_ns, pose, sb, covariance, jacobian, n_used};
+  if (!c || prop_invalid(j)) return OKB_ERR_INVALID_ARG;
   cudaSetDevice(c->device);
-  const size_t sbytes = align_up(sizeof(okb_imu_sample) * n_samples, 256);
-  int rc = hook_alloc(c, sbytes + sizeof(double) * (16 + 450 + 2));
-  if (rc) return rc;
-  unsigned char* base = reinterpret_cast<unsigned char*>(c->hook_buf);
-  okb_imu_sample* ds = reinterpret_cast<okb_imu_sample*>(base);
-  double* dio = reinterpret_cast<double*>(base + sbytes);
-  double* dcov = dio + 16;
-  double* djac = dcov + 225;
-  int* dn = reinterpret_cast<int*>(djac + 225);
-  double hio[16];
-  std::memcpy(hio, pose, 56); std::memcpy(hio + 7, sb, 72);
-  OKB_CUDA(c, cudaMemcpyAsync(ds, samples, sizeof(okb_imu_sample) * n_samples, cudaMemcpyHostToDevice, c->stream));
-  OKB_CUDA(c, cudaMemcpyAsync(dio, hio, sizeof hio, cudaMemcpyHostToDevice, c->stream));
-  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
-  k_hook_propagate<<<1, 32, 0, c->stream>>>(*prm, ds, n_samples, t0_ns, t1_ns, dio, dcov, djac, covariance ? 1 : 0, jacobian ? 1 : 0, dn);
-  c->launches += 1;
-  OKB_CUDA(c, cudaGetLastError());
-  int hn = 0;
-  OKB_CUDA(c, cudaMemcpyAsync(hio, dio, sizeof hio, cudaMemcpyDeviceToHost, c->stream));
-  if (covariance) OKB_CUDA(c, cudaMemcpyAsync(covariance, dcov, 225 * 8, cudaMemcpyDeviceToHost, c->stream));
-  if (jacobian) OKB_CUDA(c, cudaMemcpyAsync(jacobian, djac, 225 * 8, cudaMemcpyDeviceToHost, c->stream));
-  OKB_CUDA(c, cudaMemcpyAsync(&hn, dn, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (hn >= 0) { std::memcpy(pose, hio, 56); std::memcpy(sb, hio + 7, 72); }
-  if (n_used) *n_used = hn;
-  return OKB_OK;
+  std::lock_guard<std::mutex> lk(c->prop_one.mtx);
+  return prop_run(c, c->stream, c->prop_one, 1, &j);
+}
+
+extern "C" int okb_imu_propagate_batch(okb_ctx* c, int n_jobs, const okb_propagate_job* jobs) {
+  if (!c) return OKB_ERR_INVALID_ARG;
+  if (n_jobs < 0 || (n_jobs > 0 && !jobs)) {
+    c->set_error("okb_imu_propagate_batch: n_jobs < 0, or jobs is NULL");
+    return OKB_ERR_INVALID_ARG;
+  }
+  if (n_jobs == 0) return OKB_OK;
+  for (int i = 0; i < n_jobs; ++i)
+    if (const char* why = prop_invalid(jobs[i])) {
+      c->set_error("okb_imu_propagate_batch: job " + std::to_string(i) + ": " + why);
+      return OKB_ERR_INVALID_ARG;
+    }
+  cudaSetDevice(c->device);
+  std::lock_guard<std::mutex> lk(c->prop_batch.mtx);
+  if (!c->stream_prop) OKB_CUDA(c, create_high_priority_stream(&c->stream_prop));
+  return prop_run(c, c->stream_prop, c->prop_batch, n_jobs, jobs);
 }
 
 extern "C" int okb_eval_pose_error(okb_ctx* c, const double* meas, const double* sqrt_info, const double* pose, double* r, double* J) {
