@@ -100,14 +100,16 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
     return OKB_ERR_CUDA;
   }
   cudaMemset(c->d_states, 0, sizeof(SolverState) * max_windows);
-  cudaFuncSetAttribute(k_schur, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
+  cudaFuncSetAttribute(k_schur<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
+  cudaFuncSetAttribute(k_schur<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
   cudaFuncSetAttribute(k_imu, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemI_bytes());
   cudaFuncSetAttribute(k_imu, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(k_solve<S_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
   cudaFuncSetAttribute(k_solve<S_THREADS>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(k_solve<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
   cudaFuncSetAttribute(k_solve<512>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(k_schur, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_schur<256>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_schur<512>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   cudaFuncSetAttribute(k_quality, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
   set_landmarks_attributes<OKB_DIST_NONE>();
   set_landmarks_attributes<OKB_DIST_RADTAN>();
@@ -465,7 +467,7 @@ static int upload_pack(okb_ctx* c, int win, const okb_window_desc* D) {
     }
     if (!(ob.sqrt_info > 0.0)) { c->set_error("observation with non-positive sqrt information"); return OKB_ERR_INVALID_ARG; }
   }
-  if (smemA2_bytes(K, 4 * ((6 * K + 1 + 3) / 4), 0) > (size_t)c->smem_optin) { c->set_error("window does not fit kernel A shared memory"); return OKB_ERR_CAPACITY; }
+  if (smemA2_bytes(K, 0) > (size_t)c->smem_optin) { c->set_error("window does not fit kernel A shared memory"); return OKB_ERR_CAPACITY; }
 
   WinStore& S = c->wins[win];
   S.uploaded = false;        // true again only when the whole upload has been issued successfully
@@ -594,7 +596,7 @@ extern "C" int okb_window_add_frame(okb_ctx* c, int win, const double* pose, con
   if (rc) return rc;
   const int K1 = W->K + 1, NSB1 = W->NSB + (speed_bias ? 1 : 0);
   if (K1 > S->caps.K || NSB1 > S->caps.K || 6 * K1 + 9 * NSB1 > kMaxDense) { c->set_error("okb_window_add_frame: frame capacity exceeded (okb_window_reserve)"); return OKB_ERR_CAPACITY; }
-  if (smemA2_bytes(K1, 4 * ((6 * K1 + 1 + 3) / 4), 0) > (size_t)c->smem_optin) { c->set_error("window does not fit kernel A shared memory"); return OKB_ERR_CAPACITY; }
+  if (smemA2_bytes(K1, 0) > (size_t)c->smem_optin) { c->set_error("window does not fit kernel A shared memory"); return OKB_ERR_CAPACITY; }
   if (term) {
     if ((int)term->pose0 >= K1 || (int)term->pose1 >= K1 || (int)term->sb0 >= NSB1 || (int)term->sb1 >= NSB1 ||
         (uint64_t)term->sample_offset + term->sample_count > (uint64_t)n_samples || term->sample_count < 2) {
@@ -1216,27 +1218,24 @@ extern "C" int okb_window_reset(okb_ctx* c, int first, int count) {
 // Launch geometry of one optimize of windows [first, first+count): everything a captured CUDA graph depends on
 // besides the kernel arguments.
 struct RoundPlan {
-  int max_chunks = 1, max_imu = 0, max_cx = 1, lm_wide = 0, acc_copies = 1, chol_smem = 1, solve_threads = S_THREADS, gxQ = 1, shard = 0, push_gx = 1;
-  int lm_model = kDistAny, _pad = 0;      // (no padding bytes: the plan is compared bytewise as a graph key)
+  int max_chunks = 1, max_imu = 0, max_cx = 1, lm_wide = 0, acc_smem = 1, chol_smem = 1, solve_threads = S_THREADS, gxQ = 1, shard = 0, push_gx = 1;
+  int lm_model = kDistAny, schur_wide = 0;      // (no padding bytes: the plan is compared bytewise as a graph key)
   size_t smA = 0, smS = 0, smQ = 0;
 };
 static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
   P = RoundPlan();
   int chol_smem = 1;       // solve_mode of k_solve: 1 system in shared memory, 2 pose system + chain band, 0 chain band only
-  // Schur accumulator in shared memory if two CTAs per SM still fit (else one CTA; else accumulate in global memory)
-  int acc_copies = 1;
-  const size_t sm_two = ((size_t)c->smem_per_sm - 2048) / 2;
+  // k_schur: the frame-pair accumulators live in shared memory whenever they fit one CTA per SM (K <= 18), else in the
+  // chunk's global partial; 256-thread CTAs where two fit an SM, else one 512-thread CTA per SM
+  int acc_smem = 1;
   for (int i = first; i < first + count; ++i)
-    if (smemA2_bytes(c->host[i].K, c->host[i].dcp, 1) > std::min((size_t)c->smem_optin, sm_two) &&
-        smemA2_bytes(c->host[i].K, c->host[i].dcp, 0) <= sm_two) acc_copies = 0;
-  for (int i = first; i < first + count; ++i)
-    if (smemA2_bytes(c->host[i].K, c->host[i].dcp, acc_copies) > (size_t)c->smem_optin) acc_copies = 0;
+    if (smemA2_bytes(c->host[i].K, 1) > (size_t)c->smem_optin) acc_smem = 0;
   int maxL = 1;
   for (int i = first; i < first + count; ++i) {
     const WinDev& W = c->host[i];
     P.max_chunks = std::max(P.max_chunks, W.n_chunks);
     P.max_imu = std::max(P.max_imu, W.n_imu);
-    P.smA = std::max(P.smA, smemA2_bytes(W.K, W.dcp, acc_copies));
+    P.smA = std::max(P.smA, smemA2_bytes(W.K, acc_smem));
     P.max_cx = std::max(P.max_cx, (W.L + L1_THREADS - 1) / L1_THREADS);
     {      // the roomiest mode this window fits; the range runs in the most modest one (1 > 2 > 0)
       const int wm = smemS_bytes(W.d, W.dc, W.K, W.marg_n, W.n_imu, 1) <= (size_t)c->smem_optin ? 1
@@ -1264,7 +1263,8 @@ static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
       if (P.smS > (size_t)c->smem_optin) { c->set_error("window does not fit kernel S shared memory"); return OKB_ERR_CAPACITY; }
     }
   }
-  P.acc_copies = acc_copies; P.chol_smem = chol_smem;
+  P.acc_smem = acc_smem; P.chol_smem = chol_smem;
+  P.schur_wide = P.smA > ((size_t)c->smem_per_sm - 2048) / 2 ? 1 : 0;
   // k_landmarks: launches whose landmark tiles would fill less than half the SMs (few windows, the cfg-5 window) split
   // every tile's frame walk over a cluster of two 512-thread CTAs; the sums keep their order in either shape
   P.lm_wide = (2 * count * P.max_cx <= c->sm_count) ? 1 : 0;
@@ -1316,7 +1316,8 @@ static int launch_rounds(okb_ctx* c, int first, int count, const okb_solve_optio
       case OKB_DIST_RADTAN8: launch_landmarks<OKB_DIST_RADTAN8>(c, first, count, P); break;
       default: launch_landmarks<kDistAny>(c, first, count, P); break;
     }
-    k_schur<<<gridA, A2_THREADS, P.smA, c->stream>>>(c->d_wins, first, P.acc_copies, opt.max_iterations);
+    if (P.schur_wide) k_schur<512><<<gridA, 512, P.smA, c->stream>>>(c->d_wins, first, P.acc_smem, opt.max_iterations);
+    else k_schur<256><<<gridA, 256, P.smA, c->stream>>>(c->d_wins, first, P.acc_smem, opt.max_iterations);
     if (P.shard) {    // chunk reduction fused with the push half of the all-reduce over peer memory
       k_shard_push<<<dim3(P.push_gx, count), 256, 0, c->stream>>>(c->d_wins, first);
       c->launches += 1;

@@ -5,7 +5,7 @@
 //       reduced per (CTA, frame), then H_ll = sum_f M_f, g_l = -sum_f m_f and (H_ll + mu E)^-1 by 3x3 Cholesky.
 //   k_schur ("A2"): one CTA per (landmark chunk, window), tiles of 32 landmarks staged by TMA bulk copies:
 //       Y_f = W_f L^-T into a shared-memory tile, then the Schur complement as a block-sparse SYRK
-//       S += Y Y^T with one lane per 6x6 frame-block pair (details at the kernel).
+//       S += Y^T Y on the FP64 tensor cores, one 8x8 block per frame pair (details at the kernel).
 //   k_quality: post-solve landmark quality (Estimator.cpp:880-894), one thread per landmark.
 #pragma once
 #include <cooperative_groups.h>
@@ -15,7 +15,6 @@
 namespace okb {
 
 constexpr int L1_THREADS = 128;          // landmarks per k_landmarks CTA: one partH record per (CTA, frame)
-constexpr int A2_THREADS = 192;          // k_schur block (6 warps at 168 registers: two CTAs per SM)
 constexpr int A2_TILE = 32;              // landmarks per Y tile
 constexpr int kPartH = 32;               // doubles per (cx, frame) record: 27 H_pp/g_p + cost + stepnorm2 + pad
 
@@ -326,36 +325,45 @@ __global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 3 : 1) k_landmarks(
 }
 
 // ------------------------------------------------------------------------------------------------
-// A2: Schur complement of the landmark blocks,  S = sum_l Y_l Y_l^T  with  Y_l = W_l L_l^-T  (6K+1 rows: the
-// pose rows of the frames that see landmark l, plus the augmented row z_l = L_l^-1 g_l that yields the
-// reduced right-hand side).
+// A2: Schur complement of the landmark blocks,  S = sum_l Y_l^T Y_l  with  Y_l = W_l L_l^-T  plus the augmented row
+// z_l = L_l^-1 g_l that yields the reduced right-hand side.
 //
-// Landmarks arrive sorted by (first, last) observing frame, so a tile of 32 consecutive landmarks only
-// touches the frames [a, b] listed in W.tile_range.  The SYRK is done per 6x6 frame block: one lane owns one
-// block pair (36 accumulators in registers, 12 operand doubles per 36 multiply-adds) and KS <= 8 adjacent
-// lanes of the same warp split the tile's 96 columns.  The lane -> block-pair map covers the frames
-// [a, K-1] and is rebuilt only when the tile's first frame a changes (landmarks are sorted by it: at most K
-// times per chunk); lanes whose pair reaches beyond the tile's last frame b sit the tile out, and since pairs
-// are dealt to the warps row-major, whole warps skip narrow tiles.  On a rebuild the accumulators are summed
-// over the KS lanes with shuffles (fixed order) and added by one lane to the chunk's packed accumulator in
-// shared memory (or to the global partial for windows with many frames): one writer per element, no barrier
-// => deterministic.
+// Landmarks arrive sorted by (first, last) observing frame, so a tile of 32 consecutive landmarks only touches the
+// frames [a, b] listed in W.tile_range.  Per tile, Y is built for the frames of the range as 8 columns per frame over
+// the tile's 96 rows (3 per landmark): columns 0-5 hold Y_f, column 6 holds z (the same for every frame), column 7 is
+// zero.  The SYRK runs on the FP64 tensor cores (mma.sync.m8n8k4.f64): frame pair (i, j), i >= j, is one 8x8 block
+// Y_i^T Y_j whose [0:6, 0:6] is the Schur block and, for i == j, whose row 6 is frame i's right-hand-side update.
+// Every frame pair owns a fixed 8x8 accumulator for the whole chunk (shared memory, or the chunk's global partial for
+// windows with many frames); a tile adds one DMMA chain per pair of its range, so the accumulation order is the tile
+// order whatever the ranges => deterministic, and nothing moves when the range changes.
 // ------------------------------------------------------------------------------------------------
-constexpr int kLiStride = 9;   // L^-1 (6) | z (3), as in global memory (one bulk copy per tile)
+constexpr int kLiStride = 9;                   // L^-1 (6) | z (3), as in global memory (one bulk copy per tile)
+constexpr int kYFrame = 3 * A2_TILE * 8;       // doubles of one frame's Y block: 96 rows x 8 columns
 
-__host__ __device__ inline int schur_ldy(int dcp) { return dcp + 2; }   // Y row stride: rows shift by 16 B across banks
+// Y is stored in the order a m8n8k4 fragment is read: k-step s (rows 4s..4s+3) is 32 doubles, lane 4g + t holding
+// row 4s + t, column g (A[g][t] of Y_i^T and B[t][g] of Y_j alike).  The column index is XORed with s & 3 so that the
+// Y build (32 landmarks, rows 3 ll + c, one column at a time) stores without bank conflicts; the fragment read stays a
+// permutation of the 32 slots.
+__device__ __forceinline__ int schur_y_index(int k, int e) { return (k >> 2) * 32 + (k & 3) + ((e ^ ((k >> 2) & 3)) << 2); }
 
-// acc_copies: 1 = the chunk's Schur accumulator (packed lower triangle of the (dc+1) x (dc+1) matrix) lives in
-// shared memory; 0 = accumulate in the chunk's global partial instead (windows with many frames).
-__host__ __device__ inline size_t schur_acc_doubles(int K) { return (size_t)(6 * K + 1) * (6 * K + 2) / 2; }
-__host__ __device__ inline size_t smemA2_bytes(int K, int dcp, int acc_copies) {
-  size_t b = 16;                                                    // two mbarriers (TMA completion per buffer)
-  b += ((size_t)3 * A2_TILE * schur_ldy(dcp) + 8) * sizeof(double);   // Y tile, k-major (+ pad: the augmented-row lanes read 6 wide)
-  b += (size_t)2 * K * 6 * A2_TILE * sizeof(double);               // M tiles [f][e][ll] (double buffered)
-  b += (size_t)2 * A2_TILE * kLiStride * sizeof(double);           // L^-1 | z
-  b += (size_t)2 * A2_TILE * 4 * sizeof(double);                   // X
+// Element (r, c) of frame pair (i, j)'s 8x8 block in the chunk's partial (dcp x dcp, row-major lower triangle), or -1
+// for the padding and the right-hand-side entries that another block already carries.
+__device__ __forceinline__ int schur_elem(int i, int j, int r, int c, int dc, int dcp) {
+  if (r < 6 && c < 6) return (6 * i + r) * dcp + 6 * j + c;
+  if (i == j && r == 6 && c < 6) return dc * dcp + 6 * i + c;
+  return -1;
+}
+
+// acc_smem: 1 = the frame-pair accumulators (K(K+1)/2 blocks of 64 doubles) live in shared memory; 0 = accumulate in
+// the chunk's global partial instead (windows with many frames).
+__host__ __device__ inline size_t smemA2_bytes(int K, int acc_smem) {
+  size_t b = 16;                                                    // mbarrier (TMA completion)
+  b += (size_t)K * kYFrame * sizeof(double);                        // Y, fragment-major, one block per frame
+  b += (size_t)K * 6 * A2_TILE * sizeof(double);                   // M tile [f][e][ll]
+  b += (size_t)A2_TILE * kLiStride * sizeof(double);               // L^-1 | z
+  b += (size_t)A2_TILE * 4 * sizeof(double);                       // X
   b += (size_t)K * 4 * sizeof(double);                             // frame translations
-  b += (size_t)acc_copies * schur_acc_doubles(K) * sizeof(double);
+  b += (size_t)acc_smem * K * (K + 1) / 2 * 64 * sizeof(double);
   return b;
 }
 
@@ -382,8 +390,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   } while (!ok);
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void dmma_8x8x4(double& d0, double& d1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
+}
 
-__global__ void __launch_bounds__(A2_THREADS, 2) k_schur(const WinDev* __restrict__ wins, int win_first, int acc_copies, int max_iterations) {
+// NT = 256 where two CTAs fit an SM (cfg-2), else 512: 16 warps per SM either way.
+template <int NT>
+__global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* __restrict__ wins, int win_first, int acc_smem, int max_iterations) {
   const WinDev& W = wins[win_first + blockIdx.y];
   SolverState* st = W.st;
   if (st->done) return;
@@ -392,135 +405,78 @@ __global__ void __launch_bounds__(A2_THREADS, 2) k_schur(const WinDev* __restric
   if (st->iteration >= max_iterations) return;
   const int chunk = blockIdx.x;
   if (chunk >= W.n_chunks) return;
-  const int tid = threadIdx.x;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  constexpr int NW = NT / 32;
   const int K = W.K, dc = W.dc, dcp = W.dcp, L = W.L;
-  const int ldy = schur_ldy(dcp);
+  const int n_pairs = K * (K + 1) / 2;
 
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem_raw);            // [2]: TMA completion of tile buffer 0 / 1
-  double* Yt = reinterpret_cast<double*>(smem_raw + 16);
-  double* sMb = Yt + (size_t)3 * A2_TILE * ldy + 8;
-  double* sLib = sMb + (size_t)2 * K * 6 * A2_TILE;
-  double* sXb = sLib + 2 * A2_TILE * kLiStride;
-  double* tws = sXb + 2 * A2_TILE * 4;
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem_raw);            // TMA completion of the staged tile
+  double* Yt = reinterpret_cast<double*>(smem_raw + 16);             // [K][kYFrame]
+  double* sM = Yt + (size_t)K * kYFrame;                             // [K][6][32]
+  double* sLi = sM + (size_t)K * 6 * A2_TILE;
+  double* sX = sLi + A2_TILE * kLiStride;
+  double* tws = sX + A2_TILE * 4;
+  double* Sacc = tws + 4 * K;                                        // [n_pairs][64] when acc_smem
   double* Sp = W.partA + (size_t)chunk * W.partA_stride;
-  const bool acc_smem = acc_copies > 0;
-  const int acc_n = (dc + 1) * (dc + 2) / 2;
-  double* Sacc = acc_smem ? tws + 4 * K : Sp;     // packed lower triangles in shared memory, or the global partial itself
-  const int n_acc = acc_smem ? acc_copies * acc_n : dcp * dcp;
 
-  for (int f = tid; f < K; f += A2_THREADS) {
+  for (int f = tid; f < K; f += NT) {
     tws[4 * f] = W.pose_c[7 * f]; tws[4 * f + 1] = W.pose_c[7 * f + 1]; tws[4 * f + 2] = W.pose_c[7 * f + 2];
   }
-  for (int i = tid; i < n_acc; i += A2_THREADS) Sacc[i] = 0.0;
+  for (int i = tid; i < K * 3 * A2_TILE; i += NT)                // column 7: zero, never written again
+    Yt[(size_t)(i / (3 * A2_TILE)) * kYFrame + schur_y_index(i % (3 * A2_TILE), 7)] = 0.0;
+  if (acc_smem) for (int i = tid; i < n_pairs * 64; i += NT) Sacc[i] = 0.0;
+  else for (int i = tid; i < dcp * dcp; i += NT) Sp[i] = 0.0;
 
   const int lm_begin = chunk * W.lm_per_chunk;     // multiple of A2_TILE
   const int lm_end = min(L, lm_begin + W.lm_per_chunk);
 
-  // Asynchronous staging of one tile by the TMA engine (cp.async.bulk, issued by warp 0, completion on
-  // mbar[buf]); frames [fa, fb] only.  Global and shared layouts agree, so every piece is one contiguous copy:
+  // Asynchronous staging of one tile by the TMA engine (cp.async.bulk, issued by thread 0, completion on mbar);
+  // frames [fa, fb] only.  Global and shared layouts agree, so every piece is one contiguous copy:
   //   M  [tile][f][6][32] -> sM[f][6][32] : frames [fa, fb] are one contiguous block
   //   Li [l][9] -> sLi[32][9] (2304 B),  X = lm_c [l][4] -> sX[32][4] (1024 B)
-  // Rows beyond the chunk's last landmark read allocated padding (Lp) and are never used.
-  const int warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) { mbar_init(&mbar[0], 1); mbar_init(&mbar[1], 1); fence_proxy_async(); }
+  // Rows beyond the chunk's last landmark read allocated padding (Lp) and are never used.  The staging buffer is only
+  // read by the Y build, so the next tile's copies are issued right after it and land while the SYRK runs.
+  if (tid == 0) { mbar_init(mbar, 1); fence_proxy_async(); }
   __syncthreads();
-  uint32_t phase_bits = 0;      // bit b: parity to wait for on mbar[b]
-  auto stage = [&](int base, int buf, uint32_t tr) {
+  uint32_t parity = 0;
+  auto stage = [&](int base, uint32_t tr) {
     const int fa = tr & 0xffu, fb = tr >> 8;
-    if (fa > fb || warp != A2_THREADS / 32 - 1) return;      // the last warp issues the copies (the first one also builds the augmented row)
-    double* sM = sMb + (size_t)buf * K * 6 * A2_TILE;
-    double* sLi = sLib + buf * A2_TILE * kLiStride;
-    double* sX = sXb + buf * A2_TILE * 4;
-    // three copies per tile: the M block of frames [fa, fb] (contiguous in the tile-major layout), L^-1|z, X
-    if (lane == 0) {       // (the buffer's last generic-proxy reads are ordered before this point by the CTA barrier)
-      const uint32_t m_bytes = (uint32_t)(fb - fa + 1) * 6 * A2_TILE * 8;
-      mbar_arrive_expect_tx(&mbar[buf], m_bytes + A2_TILE * kLiStride * 8 + A2_TILE * 4 * 8);
-      bulk_g2s(sM + (size_t)fa * 6 * A2_TILE, W.lm_M + lm_M_index(base, fa, K), m_bytes, &mbar[buf]);
-      bulk_g2s(sLi, W.lm_Li + (size_t)kLiStride * base, A2_TILE * kLiStride * 8, &mbar[buf]);
-      bulk_g2s(sX, W.lm_c + 4 * (size_t)base, A2_TILE * 4 * 8, &mbar[buf]);
-    }
+    if (fa > fb || tid != 0) return;       // (the buffer's last generic-proxy reads are ordered before this point by a CTA barrier)
+    const uint32_t m_bytes = (uint32_t)(fb - fa + 1) * 6 * A2_TILE * 8;
+    mbar_arrive_expect_tx(mbar, m_bytes + A2_TILE * kLiStride * 8 + A2_TILE * 4 * 8);
+    bulk_g2s(sM + (size_t)fa * 6 * A2_TILE, W.lm_M + lm_M_index(base, fa, K), m_bytes, mbar);
+    bulk_g2s(sLi, W.lm_Li + (size_t)kLiStride * base, A2_TILE * kLiStride * 8, mbar);
+    bulk_g2s(sX, W.lm_c + 4 * (size_t)base, A2_TILE * 4 * 8, mbar);
   };
 
-  // ---- lane -> (block pair, column split) map of the current frame range: tid = kg * n_act + item
-  int cur_fa = -1, cur_fb = -1, lane_fmax = 0;
-  int KS = 1, kg = 0, n_act = 0, n_pairs = 0, n_pass = 1;
-  int a_off = 0, b_off = 0, row0 = 0, col0 = 0;
-  bool on = false, aug = false;
-  double acc[36];
-#pragma unroll
-  for (int i = 0; i < 36; ++i) acc[i] = 0.0;
-
-  auto decode = [&](int item, int fa) {
-    aug = false;
-    on = item < n_act;
-    if (!on) return;
-    if (item < n_pairs) {
-      int i = (int)((sqrtf(8.0f * (float)item + 1.0f) - 1.0f) * 0.5f);
-      while (i * (i + 1) / 2 > item) --i;
-      while ((i + 1) * (i + 2) / 2 <= item) ++i;
-      const int j = item - i * (i + 1) / 2;
-      row0 = 6 * (fa + i); col0 = 6 * (fa + j);
-      lane_fmax = fa + i;
+  // Frame pair (i, j)'s accumulator as this lane's C[g][2t], C[g][2t+1] of the 8x8 block: read before a DMMA chain
+  // (the global-memory latency overlaps the chain), written back with the chain added.  Each pair is taken by one warp
+  // per tile and tiles are separated by CTA barriers: one writer per element at a time.
+  const int g = lane >> 2, t2 = 2 * (lane & 3);
+  auto acc_load = [&](int i, int j, double& v0, double& v1) {
+    if (acc_smem) {
+      const double2 v = reinterpret_cast<const double2*>(Sacc + (size_t)(i * (i + 1) / 2 + j) * 64)[lane];
+      v0 = v.x; v1 = v.y;
     } else {
-      aug = true;
-      row0 = dc; col0 = 6 * (fa + item - n_pairs);
-      lane_fmax = fa + item - n_pairs;
+      const int e0 = schur_elem(i, j, g, t2, dc, dcp), e1 = schur_elem(i, j, g, t2 + 1, dc, dcp);
+      v0 = e0 >= 0 ? Sp[e0] : 0.0;
+      v1 = e1 >= 0 ? Sp[e1] : 0.0;
     }
-    a_off = row0; b_off = col0;
   };
-  // Adds the accumulators to the chunk accumulator and clears them.  Called at CTA-uniform points only.
-  // Shared-memory mode: column split kg owns copy kg, so all lanes add concurrently (a later flush that
-  // touches the same element from another lane is separated by the tile loop's barriers); the copies are
-  // summed in fixed order at the end => deterministic.  Global mode: KS rounds separated by barriers.
-  // Few instructions per element: flushes run on all 12 warps at once and are issue-bound.
-  double* Ssm = tws + 4 * K;
-  auto flush_smem = [&](int copy) {
-    double* cp = Ssm + (size_t)copy * acc_n + col0;
-    if (aug) {
-      double* rp = cp + (size_t)dc * (dc + 1) / 2;
-#pragma unroll
-      for (int c = 0; c < 6; ++c) rp[c] += acc[c];
-    } else if (row0 == col0) {        // diagonal block: lower triangle only
-#pragma unroll
-      for (int r = 0; r < 6; ++r) {
-        double* rp = cp + (size_t)(row0 + r) * (row0 + r + 1) / 2;
-#pragma unroll
-        for (int c = 0; c <= r; ++c) rp[c] += acc[r * 6 + c];
-      }
+  auto acc_store = [&](int i, int j, double v0, double v1) {
+    if (acc_smem) {
+      reinterpret_cast<double2*>(Sacc + (size_t)(i * (i + 1) / 2 + j) * 64)[lane] = make_double2(v0, v1);
     } else {
-#pragma unroll
-      for (int r = 0; r < 6; ++r) {
-        double* rp = cp + (size_t)(row0 + r) * (row0 + r + 1) / 2;
-        double t[6];
-#pragma unroll
-        for (int c = 0; c < 6; ++c) t[c] = rp[c];
-#pragma unroll
-        for (int c = 0; c < 6; ++c) rp[c] = t[c] + acc[r * 6 + c];
-      }
+      const int e0 = schur_elem(i, j, g, t2, dc, dcp), e1 = schur_elem(i, j, g, t2 + 1, dc, dcp);
+      if (e0 >= 0) Sp[e0] = v0;
+      if (e1 >= 0) Sp[e1] = v1;
     }
-  };
-  auto flush_global = [&]() {
-#pragma unroll
-    for (int i = 0; i < 36; ++i) {
-      const int rr = row0 + i / 6, cc = col0 + i % 6;
-      if ((!aug || i < 6) && cc <= rr) Sp[(size_t)rr * dcp + cc] += acc[i];
-    }
-  };
-  // The KS column splits of a block pair are adjacent lanes of one warp: they are summed with shuffles (fixed
-  // order) and the kg == 0 lane adds the result to the accumulator -- no barrier, one writer per element.
-  auto flush = [&]() {
-    // KS is a power of two: pairwise tree over the column splits (fixed shape => deterministic)
-    for (int o = KS >> 1; o > 0; o >>= 1) {
-#pragma unroll
-      for (int i = 0; i < 36; ++i) acc[i] += __shfl_down_sync(0xffffffffu, acc[i], o);
-    }
-    if (on && kg == 0) { if (acc_smem) flush_smem(0); else flush_global(); }
-#pragma unroll
-    for (int i = 0; i < 36; ++i) acc[i] = 0.0;
   };
 
-#ifdef OKB_SCHUR_PROF     // per-phase cycle counters of chunk 0 / thread 0 (costs ~18 registers: diagnostics builds only)
+#ifdef OKB_SCHUR_PROF     // per-phase cycle counters of chunk 0 / thread 0 (diagnostics builds only):
+  // 0 staging wait, 1 Y build, 2 barrier after the Y build, 3 DMMA + accumulator adds, 4 barrier after the SYRK,
+  // 5 write-back of the accumulators
   const bool prof = (tid == 0 && chunk == 0);
   unsigned long long t_ph = 0, ph[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   auto now = []() { return (unsigned long long)clock64(); };
@@ -529,141 +485,105 @@ __global__ void __launch_bounds__(A2_THREADS, 2) k_schur(const WinDev* __restric
 #else
 #define SCHUR_MARK(i) do { } while (0)
 #endif
-  int buf = 0;
-  // frame ranges are fetched two tiles ahead so that no global-load latency sits on the tile loop
-  const int last_tile = (lm_end - 1) >> 5;
-  uint32_t tr_cur = (lm_begin < lm_end) ? W.tile_range[lm_begin >> 5] : 1u;
-  uint32_t tr_n1 = (lm_begin + A2_TILE < lm_end) ? W.tile_range[(lm_begin >> 5) + 1] : 1u;
-  if (lm_begin < lm_end) stage(lm_begin, 0, tr_cur);
+  uint32_t tr_next = (lm_begin < lm_end) ? W.tile_range[lm_begin >> 5] : 1u;
+  if (lm_begin < lm_end) stage(lm_begin, tr_next);
   for (int base = lm_begin; base < lm_end; base += A2_TILE) {
-    const uint32_t tr_n2 = W.tile_range[min((base >> 5) + 2, last_tile)];
-    const int nl = min(A2_TILE, lm_end - base);
-    const double* sM = sMb + (size_t)buf * K * 6 * A2_TILE;
-    const double* sLi = sLib + buf * A2_TILE * kLiStride;
-    const double* sX = sXb + buf * A2_TILE * 4;
-    if ((tr_cur & 0xffu) <= (tr_cur >> 8)) {           // this tile was staged: wait for its bytes
-      mbar_wait(&mbar[buf], (phase_bits >> buf) & 1u);
-      phase_bits ^= 1u << buf;
-    }
-    __syncthreads();                       // the previous SYRK has finished (Y tile and the other buffer are free)
-    SCHUR_MARK(0);
-    if (base + A2_TILE < lm_end) stage(base + A2_TILE, buf ^ 1, tr_n1);   // overlaps with this tile's math
-    SCHUR_MARK(6);
-    const uint32_t tr = tr_cur;
-    tr_cur = tr_n1; tr_n1 = tr_n2;
+    const uint32_t tr = tr_next;
+    if (base + A2_TILE < lm_end) tr_next = W.tile_range[(base >> 5) + 1];
     const int fa = tr & 0xffu, fb = tr >> 8;
-    buf ^= 1;
-    if (fa > fb) continue;                 // no observed landmark in this tile (CTA-uniform)
-    const int u = fb - fa + 1;
-    // The lane -> block-pair map covers exactly the tile's frame range [fa, fb] and is rebuilt (after a flush of the
-    // register accumulators: a shuffle tree over the column splits + one shared-memory add per element) whenever the
-    // range changes.  Landmarks are sorted by (first, last) frame, so neighbouring tiles mostly share or shrink the
-    // range; every lane that is mapped does useful multiply-adds (narrow tiles get up to 8 column splits per pair).
-    if (fa != cur_fa || fb != cur_fb) {
-      flush();
-      cur_fa = fa; cur_fb = fb;
-      const int um = fb - fa + 1;
-      n_pairs = um * (um + 1) / 2;
-      n_act = n_pairs + um;
-      // block pairs are dealt to the warps (ipw per warp); inside a warp lane = pair * KS + split
-      constexpr int NW = A2_THREADS / 32;
-      const int ipw = (n_act + NW - 1) / NW;
-      if (ipw <= 32) {
-        n_pass = 1;
-        KS = 1;
-        while (2 * KS <= 8 && 2 * KS * ipw <= 32) KS *= 2;          // largest power of two that fits the warp
-        kg = lane % KS;
-        const int il = lane / KS;
-        decode(warp * ipw + il, fa);
-        on = on && il < ipw;
-      } else {                     // more block pairs than lanes (beyond 17 frames): one pair per lane, several passes
-        n_pass = (n_act + A2_THREADS - 1) / A2_THREADS;
-        KS = 1; kg = 0;
-      }
-    }
-    SCHUR_MARK(1);
-    // ---- augmented row z
-    if (tid < A2_TILE) {
-      const int ll = tid;
-      double* yz = Yt + (size_t)(3 * ll) * ldy + dc;
-      const bool v = ll < nl;
-      yz[0] = v ? sLi[ll * kLiStride + 6] : 0.0;
-      yz[ldy] = v ? sLi[ll * kLiStride + 7] : 0.0;
-      yz[2 * ldy] = v ? sLi[ll * kLiStride + 8] : 0.0;
-    }
-    // ---- Y_f = W_f L^-T for every (landmark, frame) pair of the tile, frames [fa, fb]
-    for (int pidx = tid; pidx < A2_TILE * u; pidx += A2_THREADS) {
-      const int ll = pidx % A2_TILE, f = fa + pidx / A2_TILE;      // landmark fastest: conflict-free reads of sM
-      double* y0 = Yt + (size_t)(3 * ll) * ldy + 6 * f;
-      double* y1 = y0 + ldy;
-      double* y2 = y1 + ldy;
-      double M0 = 0, M1 = 0, M2 = 0, M3 = 0, M4 = 0, M5 = 0;
-      if (ll < nl) {
-        const double* sp = sM + (size_t)(f * 6) * A2_TILE + ll;
-        M0 = sp[0]; M1 = sp[A2_TILE]; M2 = sp[2 * A2_TILE]; M3 = sp[3 * A2_TILE]; M4 = sp[4 * A2_TILE]; M5 = sp[5 * A2_TILE];
-      }
-      if (M0 != 0.0 || M3 != 0.0 || M5 != 0.0) {
+    const bool live = fa <= fb;            // some landmark of the tile is observed (CTA-uniform)
+    const int nl = min(A2_TILE, lm_end - base);
+    if (live) {
+      mbar_wait(mbar, parity);
+      parity ^= 1u;
+      SCHUR_MARK(0);
+      // ---- Y_f = W_f L^-T and z for every (landmark, frame) pair of the tile, frames [fa, fb]
+      for (int pidx = tid; pidx < A2_TILE * (fb - fa + 1); pidx += NT) {
+        const int ll = pidx % A2_TILE, f = fa + pidx / A2_TILE;      // landmark fastest: conflict-free reads of sM
+        double* y = Yt + (size_t)f * kYFrame;
+        const int k0 = 3 * ll, k1 = k0 + 1, k2 = k0 + 2;
+        double M0 = 0, M1 = 0, M2 = 0, M3 = 0, M4 = 0, M5 = 0;
+        if (ll < nl) {
+          const double* sp = sM + (size_t)(f * 6) * A2_TILE + ll;
+          M0 = sp[0]; M1 = sp[A2_TILE]; M2 = sp[2 * A2_TILE]; M3 = sp[3 * A2_TILE]; M4 = sp[4 * A2_TILE]; M5 = sp[5 * A2_TILE];
+        }
         const double* Li = sLi + ll * kLiStride;
-        const double w = sX[ll * 4 + 3];
-        const double p0 = sX[ll * 4] - tws[4 * f] * w, p1 = sX[ll * 4 + 1] - tws[4 * f + 1] * w, p2 = sX[ll * 4 + 2] - tws[4 * f + 2] * w;
-        const double N00 = M0 * Li[0], N01 = M0 * Li[1] + M1 * Li[2], N02 = M0 * Li[3] + M1 * Li[4] + M2 * Li[5];
-        const double N10 = M1 * Li[0], N11 = M1 * Li[1] + M3 * Li[2], N12 = M1 * Li[3] + M3 * Li[4] + M4 * Li[5];
-        const double N20 = M2 * Li[0], N21 = M2 * Li[1] + M4 * Li[2], N22 = M2 * Li[3] + M4 * Li[4] + M5 * Li[5];
-        y0[0] = -w * N00; y0[1] = -w * N10; y0[2] = -w * N20;
-        y1[0] = -w * N01; y1[1] = -w * N11; y1[2] = -w * N21;
-        y2[0] = -w * N02; y2[1] = -w * N12; y2[2] = -w * N22;
-        y0[3] = -(p1 * N20 - p2 * N10); y0[4] = -(p2 * N00 - p0 * N20); y0[5] = -(p0 * N10 - p1 * N00);
-        y1[3] = -(p1 * N21 - p2 * N11); y1[4] = -(p2 * N01 - p0 * N21); y1[5] = -(p0 * N11 - p1 * N01);
-        y2[3] = -(p1 * N22 - p2 * N12); y2[4] = -(p2 * N02 - p0 * N22); y2[5] = -(p0 * N12 - p1 * N02);
-      } else {
+        y[schur_y_index(k0, 6)] = ll < nl ? Li[6] : 0.0;
+        y[schur_y_index(k1, 6)] = ll < nl ? Li[7] : 0.0;
+        y[schur_y_index(k2, 6)] = ll < nl ? Li[8] : 0.0;
+        if (M0 != 0.0 || M3 != 0.0 || M5 != 0.0) {
+          const double w = sX[ll * 4 + 3];
+          const double p0 = sX[ll * 4] - tws[4 * f] * w, p1 = sX[ll * 4 + 1] - tws[4 * f + 1] * w, p2 = sX[ll * 4 + 2] - tws[4 * f + 2] * w;
+          const double N00 = M0 * Li[0], N01 = M0 * Li[1] + M1 * Li[2], N02 = M0 * Li[3] + M1 * Li[4] + M2 * Li[5];
+          const double N10 = M1 * Li[0], N11 = M1 * Li[1] + M3 * Li[2], N12 = M1 * Li[3] + M3 * Li[4] + M4 * Li[5];
+          const double N20 = M2 * Li[0], N21 = M2 * Li[1] + M4 * Li[2], N22 = M2 * Li[3] + M4 * Li[4] + M5 * Li[5];
+          y[schur_y_index(k0, 0)] = -w * N00; y[schur_y_index(k0, 1)] = -w * N10; y[schur_y_index(k0, 2)] = -w * N20;
+          y[schur_y_index(k1, 0)] = -w * N01; y[schur_y_index(k1, 1)] = -w * N11; y[schur_y_index(k1, 2)] = -w * N21;
+          y[schur_y_index(k2, 0)] = -w * N02; y[schur_y_index(k2, 1)] = -w * N12; y[schur_y_index(k2, 2)] = -w * N22;
+          y[schur_y_index(k0, 3)] = -(p1 * N20 - p2 * N10); y[schur_y_index(k0, 4)] = -(p2 * N00 - p0 * N20); y[schur_y_index(k0, 5)] = -(p0 * N10 - p1 * N00);
+          y[schur_y_index(k1, 3)] = -(p1 * N21 - p2 * N11); y[schur_y_index(k1, 4)] = -(p2 * N01 - p0 * N21); y[schur_y_index(k1, 5)] = -(p0 * N11 - p1 * N01);
+          y[schur_y_index(k2, 3)] = -(p1 * N22 - p2 * N12); y[schur_y_index(k2, 4)] = -(p2 * N02 - p0 * N22); y[schur_y_index(k2, 5)] = -(p0 * N12 - p1 * N02);
+        } else {
 #pragma unroll
-        for (int i = 0; i < 6; ++i) { y0[i] = 0.0; y1[i] = 0.0; y2[i] = 0.0; }
-      }
-    }
-    SCHUR_MARK(2);
-    __syncthreads();
-    SCHUR_MARK(3);
-    // ---- SYRK over the tile's 3*nl columns
-    const int ncols = 3 * nl;
-    for (int pass = 0; pass < n_pass; ++pass) {
-      if (n_pass > 1) decode(pass * A2_THREADS + tid, fa);
-      if (on && lane_fmax <= fb) {
-        const double* pa = Yt + a_off + (size_t)kg * ldy;
-        const double* pb = Yt + b_off + (size_t)kg * ldy;
-        const int step = KS * ldy;
-#pragma unroll 1
-        for (int k = kg; k < ncols; k += KS) {
-          const double2 a01 = *reinterpret_cast<const double2*>(pa);
-          const double2 a23 = *reinterpret_cast<const double2*>(pa + 2);
-          const double2 a45 = *reinterpret_cast<const double2*>(pa + 4);
-          const double2 b01 = *reinterpret_cast<const double2*>(pb);
-          const double2 b23 = *reinterpret_cast<const double2*>(pb + 2);
-          const double2 b45 = *reinterpret_cast<const double2*>(pb + 4);
-          const double av[6] = {a01.x, a01.y, a23.x, a23.y, a45.x, a45.y};
-          const double bv[6] = {b01.x, b01.y, b23.x, b23.y, b45.x, b45.y};
-#pragma unroll
-          for (int i = 0; i < 6; ++i)
-#pragma unroll
-            for (int j = 0; j < 6; ++j) acc[i * 6 + j] += av[i] * bv[j];
-          pa += step; pb += step;
+          for (int e = 0; e < 6; ++e) { y[schur_y_index(k0, e)] = 0.0; y[schur_y_index(k1, e)] = 0.0; y[schur_y_index(k2, e)] = 0.0; }
         }
       }
-      if (n_pass > 1) flush();
+      SCHUR_MARK(1);
     }
+    __syncthreads();                       // Y is complete; the staging buffer is free
+    SCHUR_MARK(2);
+    if (base + A2_TILE < lm_end) stage(base + A2_TILE, tr_next);
+    if (!live) continue;
+    // ---- SYRK: items of one or two frame pairs (i, j0), (i, j0 + 1) sharing row frame i, dealt to the warps in a
+    // fixed order.  Per k-step a two-pair item loads three fragments for two DMMAs.  Rows past the tile's last
+    // landmark are zero and are skipped.
+    const int u = fb - fa + 1;
+    const int ns = (3 * nl + 3) >> 2;
+    const int n_items = (u + 1) * (u + 1) / 4;      // sum over the rows il of ceil((il + 1) / 2)
+    for (int it = warp; it < n_items; it += NW) {
+      int il = 0, q = it;
+      while (q >= ((il + 2) >> 1)) { q -= (il + 2) >> 1; ++il; }
+      const int i = fa + il, j0 = fa + 2 * q;
+      const double* ya = Yt + (size_t)i * kYFrame;
+      const double* yb = Yt + (size_t)j0 * kYFrame;
+      double c0 = 0.0, c1 = 0.0, o0, o1;
+      acc_load(i, j0, o0, o1);
+      if (j0 < i) {                        // (warp-uniform)
+        double e0 = 0.0, e1 = 0.0, q0, q1;
+        acc_load(i, j0 + 1, q0, q1);
+#pragma unroll 4
+        for (int s = 0; s < ns; ++s) {
+          const int o = s * 32 + (lane ^ ((s & 3) << 2));
+          const double a = ya[o], b0 = yb[o], b1 = yb[kYFrame + o];
+          dmma_8x8x4(c0, c1, a, b0);
+          dmma_8x8x4(e0, e1, a, b1);
+        }
+        acc_store(i, j0 + 1, q0 + e0, q1 + e1);
+      } else {
+#pragma unroll 4
+        for (int s = 0; s < ns; ++s) {
+          const double a = ya[s * 32 + (lane ^ ((s & 3) << 2))];
+          dmma_8x8x4(c0, c1, a, a);
+        }
+      }
+      acc_store(i, j0, o0 + c0, o1 + c1);
+    }
+    SCHUR_MARK(3);
+    __syncthreads();                       // Y may be rebuilt
     SCHUR_MARK(4);
   }
-  __syncthreads();
-  if (n_pass == 1) flush();
   if (acc_smem) {
     __syncthreads();
-    for (int i = tid; i < (dc + 1) * dcp; i += A2_THREADS) {
-      const int r = i / dcp, cidx = i % dcp;
-      if (cidx <= r) {
-        const int e = r * (r + 1) / 2 + cidx;
-        double v = Sacc[e];
-        for (int q = 1; q < acc_copies; ++q) v += Sacc[(size_t)q * acc_n + e];
-        Sp[i] = v;
-      }
+    // unpack the 8x8 blocks into the packed lower triangle k_reduce_partials / k_solve read
+    for (int e = tid; e < n_pairs * 64; e += NT) {
+      const int p = e >> 6;
+      int i = (int)((sqrtf(8.0f * (float)p + 1.0f) - 1.0f) * 0.5f);
+      while (i * (i + 1) / 2 > p) --i;
+      while ((i + 1) * (i + 2) / 2 <= p) ++i;
+      const int j = p - i * (i + 1) / 2;
+      const int ln = (e & 63) >> 1;
+      const int idx = schur_elem(i, j, ln >> 2, 2 * (ln & 3) + (e & 1), dc, dcp);
+      if (idx >= 0) Sp[idx] = Sacc[e];
     }
   }
   SCHUR_MARK(5);
