@@ -365,6 +365,10 @@ int okb_profile_read(okb_ctx* ctx, double out[6]);
 /* Diagnostics: nanoseconds the reduced-solve kernel spent per internal phase during the last optimize of
  * `win` (dense terms, partial gather, assembly, Cholesky, substitution, back-substitution, dogleg). */
 int okb_debug_phase_ns(okb_ctx* ctx, int win, double out[16]);
+/* Diagnostics: the Schur-complement kernel's launch shape for an optimize of slots [first, first+count):
+ * out[0] = 1 if its accumulators live in shared memory (0: in global memory), out[1] = threads per CTA (256: two
+ * CTAs per SM, 512: one), out[2] = dynamic shared memory per CTA in bytes. */
+int okb_debug_schur_plan(okb_ctx* ctx, int first, int count, int32_t out[3]);
 /* Diagnostics: the mutable preintegration cache of ImuError term `term` (ImuError.hpp:251-276): the bias the
  * preintegration was done at, whether it is valid (0 = redo_), and how often it was redone. */
 int okb_debug_imu_cache(okb_ctx* ctx, int win, int term, double sb_ref[9], int32_t* valid, int32_t* redo_count);

@@ -218,6 +218,11 @@ class Context:
                  "p8", "p9", "p10", "p11", "p12", "p13", "p14", "p15"]   # OKB_SCHUR_PROF / OKB_CHOL_PROF builds: cycles
         return {n: v * 1e-3 for n, v in zip(names, out)}
 
+    def debug_schur_plan(self, first=0, count=1):
+        out = np.zeros(3, dtype=np.int32)
+        self._check(lib().okb_debug_schur_plan(self._h, int(first), int(count), _p(out)))
+        return {"acc_smem": bool(out[0]), "threads": int(out[1]), "smem_bytes": int(out[2])}
+
     def debug_imu_cache(self, win, term):
         ref = np.zeros(9)
         v, r = C.c_int32(0), C.c_int32(0)

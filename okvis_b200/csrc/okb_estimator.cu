@@ -1225,8 +1225,9 @@ struct RoundPlan {
 static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
   P = RoundPlan();
   int chol_smem = 1;       // solve_mode of k_solve: 1 system in shared memory, 2 pose system + chain band, 0 chain band only
-  // k_schur: the frame-pair accumulators live in shared memory whenever they fit one CTA per SM (K <= 18), else in the
-  // chunk's global partial; 256-thread CTAs where two fit an SM, else one 512-thread CTA per SM
+  // k_schur: the block-pair and right-hand-side accumulators live in shared memory whenever they fit one CTA per SM
+  // (K <= 22), else in the chunk's global partial; 256-thread CTAs where two fit an SM (K <= 12), else one 512-thread
+  // CTA per SM
   int acc_smem = 1;
   for (int i = first; i < first + count; ++i)
     if (smemA2_bytes(c->host[i].K, 1) > (size_t)c->smem_optin) acc_smem = 0;
@@ -1485,6 +1486,22 @@ extern "C" int okb_debug_imu_cache(okb_ctx* c, int win, int term, double sb_ref[
 }
 
 // diagnostics: accumulated k_solve phase times (ns) of the last optimize of `win`
+extern "C" int okb_debug_schur_plan(okb_ctx* c, int first, int count, int32_t out[3]) {
+  int rc = check_range(c, first, count);
+  if (rc) return rc;
+  if (!out) return OKB_ERR_INVALID_ARG;
+  cudaSetDevice(c->device);
+  rc = commit_range(c, first, count);
+  if (rc) return rc;
+  RoundPlan P;
+  rc = plan_rounds(c, first, count, P);
+  if (rc) return rc;
+  out[0] = P.acc_smem;
+  out[1] = P.schur_wide ? 512 : 256;
+  out[2] = (int32_t)P.smA;
+  return OKB_OK;
+}
+
 extern "C" int okb_debug_phase_ns(okb_ctx* c, int win, double out[16]) {
   if (!c || win < 0 || win >= c->max_windows || !out) return OKB_ERR_INVALID_ARG;
   for (int i = 0; i < 16; ++i) out[i] = (double)c->h_states[win].phase_ns[i];

@@ -5,7 +5,8 @@
 //       reduced per (CTA, frame), then H_ll = sum_f M_f, g_l = -sum_f m_f and (H_ll + mu E)^-1 by 3x3 Cholesky.
 //   k_schur ("A2"): one CTA per (landmark chunk, window), tiles of 32 landmarks staged by TMA bulk copies:
 //       Y_f = W_f L^-T into a shared-memory tile, then the Schur complement as a block-sparse SYRK
-//       S += Y^T Y on the FP64 tensor cores, one 8x8 block per frame pair (details at the kernel).
+//       S += Y^T Y on the FP64 tensor cores, the 6K pose columns packed into 8-column blocks, one 8x8 block per block
+//       pair (details at the kernel).
 //   k_quality: post-solve landmark quality (Estimator.cpp:880-894), one thread per landmark.
 #pragma once
 #include <cooperative_groups.h>
@@ -69,8 +70,8 @@ __host__ __device__ inline size_t smemL_bytes(int groups) {
 
 // Reduce-scatter of 32 values over a warp: on return lane e holds the sum over the warp's lanes of value e.  A fixed
 // butterfly (xor 16, 8, 4, 2, 1), 31 shuffles, so the summation order is the same on every launch.
-template <int O>
-__device__ __forceinline__ void reduce_scatter_step(double (&v)[32]) {     // v[0, 2 O) -> v[0, O): this lane's half
+template <int O, int N>
+__device__ __forceinline__ void reduce_scatter_step(double (&v)[N]) {      // v[0, 2 O) -> v[0, O): this lane's half
   const bool hi = (threadIdx.x & O) != 0;
 #pragma unroll
   for (int i = 0; i < O; ++i) {
@@ -325,46 +326,72 @@ __global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 3 : 1) k_landmarks(
 }
 
 // ------------------------------------------------------------------------------------------------
-// A2: Schur complement of the landmark blocks,  S = sum_l Y_l^T Y_l  with  Y_l = W_l L_l^-T  plus the augmented row
-// z_l = L_l^-1 g_l that yields the reduced right-hand side.
+// A2: Schur complement of the landmark blocks,  S = sum_l Y_l^T Y_l  with  Y_l = W_l L_l^-T, and the reduced
+// right-hand side  sum_l Y_l^T z_l  with  z_l = L_l^-1 g_l.
 //
 // Landmarks arrive sorted by (first, last) observing frame, so a tile of 32 consecutive landmarks only touches the
-// frames [a, b] listed in W.tile_range.  Per tile, Y is built for the frames of the range as 8 columns per frame over
-// the tile's 96 rows (3 per landmark): columns 0-5 hold Y_f, column 6 holds z (the same for every frame), column 7 is
-// zero.  The SYRK runs on the FP64 tensor cores (mma.sync.m8n8k4.f64): frame pair (i, j), i >= j, is one 8x8 block
-// Y_i^T Y_j whose [0:6, 0:6] is the Schur block and, for i == j, whose row 6 is frame i's right-hand-side update.
-// Every frame pair owns a fixed 8x8 accumulator for the whole chunk (shared memory, or the chunk's global partial for
-// windows with many frames); a tile adds one DMMA chain per pair of its range, so the accumulation order is the tile
-// order whatever the ranges => deterministic, and nothing moves when the range changes.
+// frames [a, b] listed in W.tile_range.  The window's 6K pose columns are packed densely into nB = ceil(6K / 8) blocks
+// of 8 columns: pose column (f, e) is column 6f + e, in block (6f + e) / 8.  Per tile, Y is built over the tile's 96
+// rows (3 per landmark) for the blocks [6a / 8, (6b + 5) / 8] the range touches; the columns of those blocks that lie
+// outside the range's frames (or past 6K) are written as zero.  The SYRK runs on the FP64 tensor cores
+// (mma.sync.m8n8k4.f64): block pair (bi, bj), bi >= bj, is one 8x8 block Y_bi^T Y_bj.  Every block pair owns a fixed
+// 8x8 accumulator for the whole chunk (shared memory, or the chunk's global partial for windows with many frames); a
+// tile adds one DMMA chain per pair of its blocks, so the accumulation order is the tile order whatever the ranges =>
+// deterministic, and nothing moves when the range changes.  The right-hand side is formed in the Y build: the warp that
+// builds frame f of a tile holds its 32 landmarks, and sums Y_f^T z over them with a fixed butterfly into frame f's
+// accumulator (one writer per frame and tile).
 // ------------------------------------------------------------------------------------------------
 constexpr int kLiStride = 9;                   // L^-1 (6) | z (3), as in global memory (one bulk copy per tile)
-constexpr int kYFrame = 3 * A2_TILE * 8;       // doubles of one frame's Y block: 96 rows x 8 columns
+// Y is stored column-major, one column of the tile's 96 rows (3 per landmark) every kYCol doubles, so pose column
+// (f, e) starts at the fixed offset (6f + e) kYCol.  The 4 doubles of padding make both accesses free of
+// bank conflicts: the Y build stores one column at rows 3 ll + c over a warp's 32 landmarks (3 ll mod 16 is a
+// permutation), and a m8n8k4 fragment read (lane 4g + t: row 4s + t, column g of the block, i.e. A[g][t] of Y_bi^T
+// and B[t][g] of Y_bj alike) hits 4g + t mod 16.
+constexpr int kYCol = 3 * A2_TILE + 4;
+constexpr int kYBlock = 8 * kYCol;             // doubles of one 8-column Y block
 
-// Y is stored in the order a m8n8k4 fragment is read: k-step s (rows 4s..4s+3) is 32 doubles, lane 4g + t holding
-// row 4s + t, column g (A[g][t] of Y_i^T and B[t][g] of Y_j alike).  The column index is XORed with s & 3 so that the
-// Y build (32 landmarks, rows 3 ll + c, one column at a time) stores without bank conflicts; the fragment read stays a
-// permutation of the 32 slots.
-__device__ __forceinline__ int schur_y_index(int k, int e) { return (k >> 2) * 32 + (k & 3) + ((e ^ ((k >> 2) & 3)) << 2); }
+__host__ __device__ inline int schur_blocks(int K) { return (6 * K + 7) / 8; }
 
-// Element (r, c) of frame pair (i, j)'s 8x8 block in the chunk's partial (dcp x dcp, row-major lower triangle), or -1
-// for the padding and the right-hand-side entries that another block already carries.
-__device__ __forceinline__ int schur_elem(int i, int j, int r, int c, int dc, int dcp) {
-  if (r < 6 && c < 6) return (6 * i + r) * dcp + 6 * j + c;
-  if (i == j && r == 6 && c < 6) return dc * dcp + 6 * i + c;
-  return -1;
+// Element (r, c) of block pair (bi, bj)'s 8x8 block, i.e. pose entry (R, C) = (8 bi + r, 8 bj + c), in the chunk's
+// partial (dcp x dcp, the full 6x6 block of every frame pair fR >= fC), or -1 for columns past the poses and the
+// entries above the diagonal of a diagonal block pair that belong to no stored frame pair.
+__device__ __forceinline__ int schur_elem(int bi, int bj, int r, int c, int K, int dcp) {
+  const int R = 8 * bi + r, C = 8 * bj + c;
+  if (R >= 6 * K || C >= 6 * K || R / 6 < C / 6) return -1;
+  return R * dcp + C;
+}
+// The mirror (C, R) of an entry of a frame's diagonal 6x6 block that the lower block triangle reaches only from below:
+// the frame straddles blocks bj < bi.  -1 for every other entry.
+__device__ __forceinline__ int schur_mirror(int bi, int bj, int r, int c, int K, int dcp) {
+  const int R = 8 * bi + r, C = 8 * bj + c;
+  if (bi == bj || R >= 6 * K || R / 6 != C / 6) return -1;
+  return C * dcp + R;
 }
 
-// acc_smem: 1 = the frame-pair accumulators (K(K+1)/2 blocks of 64 doubles) live in shared memory; 0 = accumulate in
-// the chunk's global partial instead (windows with many frames).
+// acc_smem: 1 = the block-pair accumulators (nB(nB+1)/2 blocks of 64 doubles) and the right-hand side (6K doubles)
+// live in shared memory; 0 = accumulate in the chunk's global partial instead (windows with many frames).
 __host__ __device__ inline size_t smemA2_bytes(int K, int acc_smem) {
+  const size_t nB = (size_t)schur_blocks(K);
   size_t b = 16;                                                    // mbarrier (TMA completion)
-  b += (size_t)K * kYFrame * sizeof(double);                        // Y, fragment-major, one block per frame
+  b += nB * kYBlock * sizeof(double);                               // Y, column-major, 8-column blocks
   b += (size_t)K * 6 * A2_TILE * sizeof(double);                   // M tile [f][e][ll]
   b += (size_t)A2_TILE * kLiStride * sizeof(double);               // L^-1 | z
   b += (size_t)A2_TILE * 4 * sizeof(double);                       // X
   b += (size_t)K * 4 * sizeof(double);                             // frame translations
-  b += (size_t)acc_smem * K * (K + 1) / 2 * 64 * sizeof(double);
+  b += (size_t)acc_smem * (nB * (nB + 1) / 2 * 64 + 6 * (size_t)K) * sizeof(double);
   return b;
+}
+
+// Sum over the warp of v[0..5] (v[6], v[7] zero): a reduce-scatter over the lane bits 4, 2, 1, then xor 8 and 16; lane
+// e < 6 ends with the sum of value e.  A fixed butterfly, so the summation order is the same on every launch.
+__device__ __forceinline__ double warp_sum6(double (&v)[8]) {
+  reduce_scatter_step<4>(v);
+  reduce_scatter_step<2>(v);
+  reduce_scatter_step<1>(v);
+  double s = v[0];
+  s += __shfl_xor_sync(0xffffffffu, s, 8);
+  s += __shfl_xor_sync(0xffffffffu, s, 16);
+  return s;
 }
 
 // ---- TMA bulk copies (cp.async.bulk, 1-D) completing on an mbarrier
@@ -408,24 +435,24 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr int NW = NT / 32;
   const int K = W.K, dc = W.dc, dcp = W.dcp, L = W.L;
-  const int n_pairs = K * (K + 1) / 2;
+  const int nB = schur_blocks(K);
+  const int n_pairs = nB * (nB + 1) / 2;
 
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint64_t* mbar = reinterpret_cast<uint64_t*>(smem_raw);            // TMA completion of the staged tile
-  double* Yt = reinterpret_cast<double*>(smem_raw + 16);             // [K][kYFrame]
-  double* sM = Yt + (size_t)K * kYFrame;                             // [K][6][32]
+  double* Yt = reinterpret_cast<double*>(smem_raw + 16);             // [nB][kYBlock]
+  double* sM = Yt + (size_t)nB * kYBlock;                            // [K][6][32]
   double* sLi = sM + (size_t)K * 6 * A2_TILE;
   double* sX = sLi + A2_TILE * kLiStride;
   double* tws = sX + A2_TILE * 4;
   double* Sacc = tws + 4 * K;                                        // [n_pairs][64] when acc_smem
   double* Sp = W.partA + (size_t)chunk * W.partA_stride;
+  double* rhs = acc_smem ? Sacc + (size_t)n_pairs * 64 : Sp + (size_t)dc * dcp;     // [6K] right-hand side
 
   for (int f = tid; f < K; f += NT) {
     tws[4 * f] = W.pose_c[7 * f]; tws[4 * f + 1] = W.pose_c[7 * f + 1]; tws[4 * f + 2] = W.pose_c[7 * f + 2];
   }
-  for (int i = tid; i < K * 3 * A2_TILE; i += NT)                // column 7: zero, never written again
-    Yt[(size_t)(i / (3 * A2_TILE)) * kYFrame + schur_y_index(i % (3 * A2_TILE), 7)] = 0.0;
-  if (acc_smem) for (int i = tid; i < n_pairs * 64; i += NT) Sacc[i] = 0.0;
+  if (acc_smem) for (int i = tid; i < n_pairs * 64 + 6 * K; i += NT) Sacc[i] = 0.0;
   else for (int i = tid; i < dcp * dcp; i += NT) Sp[i] = 0.0;
 
   const int lm_begin = chunk * W.lm_per_chunk;     // multiple of A2_TILE
@@ -450,16 +477,17 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
     bulk_g2s(sX, W.lm_c + 4 * (size_t)base, A2_TILE * 4 * 8, mbar);
   };
 
-  // Frame pair (i, j)'s accumulator as this lane's C[g][2t], C[g][2t+1] of the 8x8 block: read before a DMMA chain
-  // (the global-memory latency overlaps the chain), written back with the chain added.  Each pair is taken by one warp
-  // per tile and tiles are separated by CTA barriers: one writer per element at a time.
+  // Block pair (i, j)'s accumulator as this lane's C[g][2t], C[g][2t+1] of the 8x8 block: read before a DMMA chain
+  // (the global-memory latency overlaps the chain), written back with the chain added (and to the mirrored entry where
+  // the block holds the lower half of a straddling frame's diagonal block).  Each pair is taken by one warp per tile
+  // and tiles are separated by CTA barriers: one writer per element at a time.
   const int g = lane >> 2, t2 = 2 * (lane & 3);
   auto acc_load = [&](int i, int j, double& v0, double& v1) {
     if (acc_smem) {
       const double2 v = reinterpret_cast<const double2*>(Sacc + (size_t)(i * (i + 1) / 2 + j) * 64)[lane];
       v0 = v.x; v1 = v.y;
     } else {
-      const int e0 = schur_elem(i, j, g, t2, dc, dcp), e1 = schur_elem(i, j, g, t2 + 1, dc, dcp);
+      const int e0 = schur_elem(i, j, g, t2, K, dcp), e1 = schur_elem(i, j, g, t2 + 1, K, dcp);
       v0 = e0 >= 0 ? Sp[e0] : 0.0;
       v1 = e1 >= 0 ? Sp[e1] : 0.0;
     }
@@ -468,9 +496,12 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
     if (acc_smem) {
       reinterpret_cast<double2*>(Sacc + (size_t)(i * (i + 1) / 2 + j) * 64)[lane] = make_double2(v0, v1);
     } else {
-      const int e0 = schur_elem(i, j, g, t2, dc, dcp), e1 = schur_elem(i, j, g, t2 + 1, dc, dcp);
+      const int e0 = schur_elem(i, j, g, t2, K, dcp), e1 = schur_elem(i, j, g, t2 + 1, K, dcp);
+      const int m0 = schur_mirror(i, j, g, t2, K, dcp), m1 = schur_mirror(i, j, g, t2 + 1, K, dcp);
       if (e0 >= 0) Sp[e0] = v0;
       if (e1 >= 0) Sp[e1] = v1;
+      if (m0 >= 0) Sp[m0] = v0;
+      if (m1 >= 0) Sp[m1] = v1;
     }
   };
 
@@ -493,40 +524,57 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
     const int fa = tr & 0xffu, fb = tr >> 8;
     const bool live = fa <= fb;            // some landmark of the tile is observed (CTA-uniform)
     const int nl = min(A2_TILE, lm_end - base);
+    const int ba = (6 * fa) >> 3, bb = (6 * fb + 5) >> 3;      // the blocks the range touches
     if (live) {
       mbar_wait(mbar, parity);
       parity ^= 1u;
       SCHUR_MARK(0);
-      // ---- Y_f = W_f L^-T and z for every (landmark, frame) pair of the tile, frames [fa, fb]
+      // ---- Y_f = W_f L^-T for every (landmark, frame) pair of the tile, frames [fa, fb], and Y_f^T z.  A warp takes
+      // one frame of the 32 landmarks, so each store writes one column (conflict-free, see kYCol).  The warps of
+      // frames fa and fb also zero the columns of blocks ba and bb outside the range.
       for (int pidx = tid; pidx < A2_TILE * (fb - fa + 1); pidx += NT) {
         const int ll = pidx % A2_TILE, f = fa + pidx / A2_TILE;      // landmark fastest: conflict-free reads of sM
-        double* y = Yt + (size_t)f * kYFrame;
         const int k0 = 3 * ll, k1 = k0 + 1, k2 = k0 + 2;
+        auto zero_column = [&](int c) {
+          double* y = Yt + (size_t)c * kYCol;
+          y[k0] = 0.0; y[k1] = 0.0; y[k2] = 0.0;
+        };
+        if (f == fa) for (int c = 8 * ba; c < 6 * fa; ++c) zero_column(c);            // (warp-uniform)
+        if (f == fb) for (int c = 6 * fb + 6; c < 8 * bb + 8; ++c) zero_column(c);
         double M0 = 0, M1 = 0, M2 = 0, M3 = 0, M4 = 0, M5 = 0;
         if (ll < nl) {
           const double* sp = sM + (size_t)(f * 6) * A2_TILE + ll;
           M0 = sp[0]; M1 = sp[A2_TILE]; M2 = sp[2 * A2_TILE]; M3 = sp[3 * A2_TILE]; M4 = sp[4 * A2_TILE]; M5 = sp[5 * A2_TILE];
         }
         const double* Li = sLi + ll * kLiStride;
-        y[schur_y_index(k0, 6)] = ll < nl ? Li[6] : 0.0;
-        y[schur_y_index(k1, 6)] = ll < nl ? Li[7] : 0.0;
-        y[schur_y_index(k2, 6)] = ll < nl ? Li[8] : 0.0;
+        double y0[6], y1[6], y2[6];      // rows k0, k1, k2 of Y_f
         if (M0 != 0.0 || M3 != 0.0 || M5 != 0.0) {
           const double w = sX[ll * 4 + 3];
           const double p0 = sX[ll * 4] - tws[4 * f] * w, p1 = sX[ll * 4 + 1] - tws[4 * f + 1] * w, p2 = sX[ll * 4 + 2] - tws[4 * f + 2] * w;
           const double N00 = M0 * Li[0], N01 = M0 * Li[1] + M1 * Li[2], N02 = M0 * Li[3] + M1 * Li[4] + M2 * Li[5];
           const double N10 = M1 * Li[0], N11 = M1 * Li[1] + M3 * Li[2], N12 = M1 * Li[3] + M3 * Li[4] + M4 * Li[5];
           const double N20 = M2 * Li[0], N21 = M2 * Li[1] + M4 * Li[2], N22 = M2 * Li[3] + M4 * Li[4] + M5 * Li[5];
-          y[schur_y_index(k0, 0)] = -w * N00; y[schur_y_index(k0, 1)] = -w * N10; y[schur_y_index(k0, 2)] = -w * N20;
-          y[schur_y_index(k1, 0)] = -w * N01; y[schur_y_index(k1, 1)] = -w * N11; y[schur_y_index(k1, 2)] = -w * N21;
-          y[schur_y_index(k2, 0)] = -w * N02; y[schur_y_index(k2, 1)] = -w * N12; y[schur_y_index(k2, 2)] = -w * N22;
-          y[schur_y_index(k0, 3)] = -(p1 * N20 - p2 * N10); y[schur_y_index(k0, 4)] = -(p2 * N00 - p0 * N20); y[schur_y_index(k0, 5)] = -(p0 * N10 - p1 * N00);
-          y[schur_y_index(k1, 3)] = -(p1 * N21 - p2 * N11); y[schur_y_index(k1, 4)] = -(p2 * N01 - p0 * N21); y[schur_y_index(k1, 5)] = -(p0 * N11 - p1 * N01);
-          y[schur_y_index(k2, 3)] = -(p1 * N22 - p2 * N12); y[schur_y_index(k2, 4)] = -(p2 * N02 - p0 * N22); y[schur_y_index(k2, 5)] = -(p0 * N12 - p1 * N02);
+          y0[0] = -w * N00; y0[1] = -w * N10; y0[2] = -w * N20;
+          y1[0] = -w * N01; y1[1] = -w * N11; y1[2] = -w * N21;
+          y2[0] = -w * N02; y2[1] = -w * N12; y2[2] = -w * N22;
+          y0[3] = -(p1 * N20 - p2 * N10); y0[4] = -(p2 * N00 - p0 * N20); y0[5] = -(p0 * N10 - p1 * N00);
+          y1[3] = -(p1 * N21 - p2 * N11); y1[4] = -(p2 * N01 - p0 * N21); y1[5] = -(p0 * N11 - p1 * N01);
+          y2[3] = -(p1 * N22 - p2 * N12); y2[4] = -(p2 * N02 - p0 * N22); y2[5] = -(p0 * N12 - p1 * N02);
         } else {
 #pragma unroll
-          for (int e = 0; e < 6; ++e) { y[schur_y_index(k0, e)] = 0.0; y[schur_y_index(k1, e)] = 0.0; y[schur_y_index(k2, e)] = 0.0; }
+          for (int e = 0; e < 6; ++e) { y0[e] = 0.0; y1[e] = 0.0; y2[e] = 0.0; }
         }
+        const double z0 = ll < nl ? Li[6] : 0.0, z1 = ll < nl ? Li[7] : 0.0, z2 = ll < nl ? Li[8] : 0.0;
+        double* y = Yt + (size_t)(6 * f) * kYCol;
+        double v[8];
+#pragma unroll
+        for (int e = 0; e < 6; ++e) {
+          y[e * kYCol + k0] = y0[e]; y[e * kYCol + k1] = y1[e]; y[e * kYCol + k2] = y2[e];
+          v[e] = (y0[e] * z0 + y1[e] * z1) + y2[e] * z2;
+        }
+        v[6] = 0.0; v[7] = 0.0;
+        const double r = warp_sum6(v);
+        if (lane < 6) rhs[6 * f + lane] += r;
       }
       SCHUR_MARK(1);
     }
@@ -534,18 +582,18 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
     SCHUR_MARK(2);
     if (base + A2_TILE < lm_end) stage(base + A2_TILE, tr_next);
     if (!live) continue;
-    // ---- SYRK: items of one or two frame pairs (i, j0), (i, j0 + 1) sharing row frame i, dealt to the warps in a
+    // ---- SYRK: items of one or two block pairs (i, j0), (i, j0 + 1) sharing row block i, dealt to the warps in a
     // fixed order.  Per k-step a two-pair item loads three fragments for two DMMAs.  Rows past the tile's last
     // landmark are zero and are skipped.
-    const int u = fb - fa + 1;
+    const int ub = bb - ba + 1;
     const int ns = (3 * nl + 3) >> 2;
-    const int n_items = (u + 1) * (u + 1) / 4;      // sum over the rows il of ceil((il + 1) / 2)
+    const int n_items = (ub + 1) * (ub + 1) / 4;    // sum over the rows il of ceil((il + 1) / 2)
     for (int it = warp; it < n_items; it += NW) {
       int il = 0, q = it;
       while (q >= ((il + 2) >> 1)) { q -= (il + 2) >> 1; ++il; }
-      const int i = fa + il, j0 = fa + 2 * q;
-      const double* ya = Yt + (size_t)i * kYFrame;
-      const double* yb = Yt + (size_t)j0 * kYFrame;
+      const int i = ba + il, j0 = ba + 2 * q;
+      const double* ya = Yt + (size_t)i * kYBlock + g * kYCol + (lane & 3);      // this lane's fragment slot
+      const double* yb = Yt + (size_t)j0 * kYBlock + g * kYCol + (lane & 3);
       double c0 = 0.0, c1 = 0.0, o0, o1;
       acc_load(i, j0, o0, o1);
       if (j0 < i) {                        // (warp-uniform)
@@ -553,8 +601,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
         acc_load(i, j0 + 1, q0, q1);
 #pragma unroll 4
         for (int s = 0; s < ns; ++s) {
-          const int o = s * 32 + (lane ^ ((s & 3) << 2));
-          const double a = ya[o], b0 = yb[o], b1 = yb[kYFrame + o];
+          const double a = ya[4 * s], b0 = yb[4 * s], b1 = yb[kYBlock + 4 * s];
           dmma_8x8x4(c0, c1, a, b0);
           dmma_8x8x4(e0, e1, a, b1);
         }
@@ -562,7 +609,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
       } else {
 #pragma unroll 4
         for (int s = 0; s < ns; ++s) {
-          const double a = ya[s * 32 + (lane ^ ((s & 3) << 2))];
+          const double a = ya[4 * s];
           dmma_8x8x4(c0, c1, a, a);
         }
       }
@@ -574,17 +621,19 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
   }
   if (acc_smem) {
     __syncthreads();
-    // unpack the 8x8 blocks into the packed lower triangle k_reduce_partials / k_solve read
+    // unpack the 8x8 blocks into the frame-pair blocks k_reduce_partials / k_solve read, and the right-hand side
     for (int e = tid; e < n_pairs * 64; e += NT) {
       const int p = e >> 6;
       int i = (int)((sqrtf(8.0f * (float)p + 1.0f) - 1.0f) * 0.5f);
       while (i * (i + 1) / 2 > p) --i;
       while ((i + 1) * (i + 2) / 2 <= p) ++i;
       const int j = p - i * (i + 1) / 2;
-      const int ln = (e & 63) >> 1;
-      const int idx = schur_elem(i, j, ln >> 2, 2 * (ln & 3) + (e & 1), dc, dcp);
+      const int ln = (e & 63) >> 1, r = ln >> 2, c = 2 * (ln & 3) + (e & 1);
+      const int idx = schur_elem(i, j, r, c, K, dcp), mir = schur_mirror(i, j, r, c, K, dcp);
       if (idx >= 0) Sp[idx] = Sacc[e];
+      if (mir >= 0) Sp[mir] = Sacc[e];
     }
+    for (int e = tid; e < 6 * K; e += NT) Sp[(size_t)dc * dcp + e] = rhs[e];
   }
   SCHUR_MARK(5);
 #ifdef OKB_SCHUR_PROF
