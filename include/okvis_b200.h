@@ -320,9 +320,24 @@ int okb_window_reset(okb_ctx* ctx, int win_first, int win_count);
 int okb_optimize(okb_ctx* ctx, int win_first, int win_count, const okb_solve_options* opt,
                  okb_summary* summaries);
 /* Same as okb_optimize but does not synchronise or read anything back (for device-side timing);
- * call okb_optimize_finish to collect the summaries. */
+ * call okb_optimize_finish to collect the summaries.  The context keeps the slot tables of the last 8 launch
+ * sequences (each okb_optimize*_async, and each extra round okb_optimize*_finish launches): a 9th waits on the host
+ * until the oldest of them has finished on the device. */
 int okb_optimize_async(okb_ctx* ctx, int win_first, int win_count, const okb_solve_options* opt);
 int okb_optimize_finish(okb_ctx* ctx, int win_first, int win_count, okb_summary* summaries);
+/* Runs the solver on the n listed slots in one batch (no reference counterpart; serves hosts that keep many
+ * sessions on one GPU and rarely have a contiguous run of them ready at once).  slots[i] are distinct, uploaded
+ * slots, in any order; summaries [n] come back in list order (may be NULL).  Per slot the result -- summary,
+ * estimates, quality, ImuError caches -- is bit-identical to okb_optimize over a contiguous range that holds the same
+ * windows in the same order (the landmark chunking depends on the batch size).  Slots not listed are not committed,
+ * waited for, read or written; pending edits of the listed slots are committed once per run of consecutive slots.
+ * n < 1, a NULL pointer, a slot out of range, not uploaded or listed twice: OKB_ERR_INVALID_ARG; a landmark-sharded
+ * context: OKB_ERR_UNSUPPORTED (sharded windows use okb_optimize); both before any device work.
+ * The _async / _finish pair splits the call as okb_optimize_async / okb_optimize_finish do (including the host wait
+ * beyond 8 launch sequences in flight); _finish takes the same list. */
+int okb_optimize_slots(okb_ctx* ctx, int n, const int32_t* slots, const okb_solve_options* opt, okb_summary* summaries);
+int okb_optimize_slots_async(okb_ctx* ctx, int n, const int32_t* slots, const okb_solve_options* opt);
+int okb_optimize_slots_finish(okb_ctx* ctx, int n, const int32_t* slots, okb_summary* summaries);
 /* Copies the estimates back.  Any pointer may be NULL.  quality[l] = sqrt(lambda_min)/sqrt(lambda_max)
  * of the landmark's 3x3 Hessian block as in Estimator.cpp:880-894 (0 if lambda_min < 1e-12). */
 int okb_window_download(okb_ctx* ctx, int win, double* poses, double* speed_bias,

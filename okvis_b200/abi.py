@@ -217,4 +217,8 @@ def load_library(path=LIB_PATH):
     lib.okb_ctx_create.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_void_p)]
     lib.okb_ctx_destroy.argtypes = [C.c_void_p]
     lib.okb_ctx_destroy.restype = None
+    slots_t = C.POINTER(C.c_int32)
+    lib.okb_optimize_slots.argtypes = [C.c_void_p, C.c_int, slots_t, C.POINTER(SolveOptions), C.POINTER(Summary)]
+    lib.okb_optimize_slots_async.argtypes = [C.c_void_p, C.c_int, slots_t, C.POINTER(SolveOptions)]
+    lib.okb_optimize_slots_finish.argtypes = [C.c_void_p, C.c_int, slots_t, C.POINTER(Summary)]
     return lib

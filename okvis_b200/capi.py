@@ -260,6 +260,30 @@ class Context:
         self._check(lib().okb_optimize_finish(self._h, int(first), int(count), out))
         return [s.as_dict() for s in out]
 
+    @staticmethod
+    def _slot_list(slots):
+        arr = (C.c_int32 * len(slots))(*[int(x) for x in slots])
+        return len(slots), arr
+
+    def optimize_slots(self, slots, max_iterations=10, min_iterations=0, time_limit_s=-1.0, use_cauchy_loss=1):
+        """okb_optimize_slots: one batched solve of the listed slots (any order); summaries in list order."""
+        o = self._options(max_iterations, min_iterations, time_limit_s, use_cauchy_loss)
+        n, arr = self._slot_list(slots)
+        out = (abi.Summary * max(n, 1))()
+        self._check(lib().okb_optimize_slots(self._h, n, arr, C.byref(o), out))
+        return [s.as_dict() for s in out[:n]]
+
+    def optimize_slots_async(self, slots, max_iterations=10, min_iterations=0, time_limit_s=-1.0, use_cauchy_loss=1):
+        o = self._options(max_iterations, min_iterations, time_limit_s, use_cauchy_loss)
+        n, arr = self._slot_list(slots)
+        self._check(lib().okb_optimize_slots_async(self._h, n, arr, C.byref(o)))
+
+    def optimize_slots_finish(self, slots):
+        n, arr = self._slot_list(slots)
+        out = (abi.Summary * max(n, 1))()
+        self._check(lib().okb_optimize_slots_finish(self._h, n, arr, out))
+        return [s.as_dict() for s in out[:n]]
+
     def download(self, win, with_quality=True, dims=None):
         """dims = (n_poses, n_speed_bias, n_landmarks) when the window was changed incrementally since its upload."""
         if dims is None:

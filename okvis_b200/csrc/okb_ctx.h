@@ -73,6 +73,15 @@ struct okb_ctx {
   static constexpr int kDoneRing = 8;
   cudaEvent_t done_ring[kDoneRing] = {};
   int done_next = 0;
+  // Slot tables: the solver kernels find their windows as wins[win_slots[blockIdx]].  d_slot_tab holds the table of the
+  // optimize being launched on `stream` (a captured graph reads it, so any set of one size replays one graph); it is
+  // written by an H2D copy on `stream` from entry k of the pinned ring h_slot_ring, where k is the done_ring index
+  // the launch will mark, so an entry is rewritten only after done_ring[k] -- the last work that copied it -- is
+  // complete.  d_ident = 0, 1, 2, ...: the table of range calls on other streams (okb_window_reset).
+  int32_t* d_slot_tab = nullptr;
+  int32_t* d_ident = nullptr;
+  int32_t* h_slot_ring = nullptr;       // pinned, [kDoneRing][max_windows]
+  std::vector<int32_t> ident;           // host 0, 1, 2, ...: the slot list of a range call
   std::vector<WinStore> wins;
   std::vector<okb::WinDev> host;      // host mirror of d_wins
   okb::WinDev* d_wins = nullptr;
@@ -98,9 +107,10 @@ struct okb_ctx {
   unsigned char* shard_peer[okb::kMaxShard] = {};             // [rank]; own entry = shard_local
   bool shard_peer_ipc[okb::kMaxShard] = {};                   // opened with cudaIpcOpenMemHandle (closed at destroy)
   int64_t launches = 0;
-  // captured launch sequences of okb_optimize (run_rounds): key fields up to `exec`, compared bytewise
+  // captured launch sequences of okb_optimize* (run_rounds): key fields up to `exec`, compared bytewise; the windows
+  // come from d_slot_tab, so the key holds the batch size, not which slots
   struct GraphEntry {
-    int first, count, rounds, with_quality, opt_iter, opt_min, opt_cauchy, _pad;
+    int count, rounds, with_quality, opt_iter, opt_min, opt_cauchy;
     double opt_time;
     unsigned char plan[96];
     cudaGraphExec_t exec;

@@ -94,12 +94,18 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
   c->chunk_cap = std::max(1, std::min(kMaxChunks, (2 * c->sm_count) / max_windows));
   if (cudaMalloc(&c->d_wins, sizeof(WinDev) * max_windows) != cudaSuccess ||
       cudaMalloc(&c->d_states, sizeof(SolverState) * max_windows) != cudaSuccess ||
-      cudaMallocHost(&c->h_states, sizeof(SolverState) * max_windows) != cudaSuccess) {
+      cudaMallocHost(&c->h_states, sizeof(SolverState) * max_windows) != cudaSuccess ||
+      cudaMalloc(&c->d_slot_tab, sizeof(int32_t) * max_windows) != cudaSuccess ||
+      cudaMalloc(&c->d_ident, sizeof(int32_t) * max_windows) != cudaSuccess ||
+      cudaMallocHost(&c->h_slot_ring, sizeof(int32_t) * okb_ctx::kDoneRing * max_windows) != cudaSuccess) {
     g_create_error = "cudaMalloc failed";
     delete c;
     return OKB_ERR_CUDA;
   }
   cudaMemset(c->d_states, 0, sizeof(SolverState) * max_windows);
+  c->ident.resize(max_windows);
+  for (int i = 0; i < max_windows; ++i) c->ident[i] = i;
+  cudaMemcpy(c->d_ident, c->ident.data(), sizeof(int32_t) * max_windows, cudaMemcpyHostToDevice);
   cudaFuncSetAttribute(k_schur<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
   cudaFuncSetAttribute(k_schur<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin);
   cudaFuncSetAttribute(k_imu, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemI_bytes());
@@ -143,6 +149,9 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
   if (c->d_wins) cudaFree(c->d_wins);
   if (c->d_states) cudaFree(c->d_states);
   if (c->h_states) cudaFreeHost(c->h_states);
+  if (c->d_slot_tab) cudaFree(c->d_slot_tab);
+  if (c->d_ident) cudaFree(c->d_ident);
+  if (c->h_slot_ring) cudaFreeHost(c->h_slot_ring);
   if (c->hook_buf) cudaFree(c->hook_buf);
   if (c->marg_host) cudaFreeHost(c->marg_host);
   if (c->marg_dev) cudaFree(c->marg_dev);
@@ -185,12 +194,24 @@ int join_transfers(okb_ctx* c) {
   if (cudaEventRecord(c->ev_join, c->stream_xfer) != cudaSuccess) return 1;
   return cudaStreamWaitEvent(c->stream, c->ev_join, 0) != cudaSuccess;
 }
-// Marks solver-stream work on windows [first, first+count): later transfers of these windows wait for it.
-void mark_work(okb_ctx* c, int first, int count) {
+// Marks solver-stream work on the n listed windows: later transfers of these windows wait for it.
+void mark_work(okb_ctx* c, const int32_t* slots, int n) {
   const int k = c->done_next;
   c->done_next = (k + 1) % okb_ctx::kDoneRing;
   cudaEventRecord(c->done_ring[k], c->stream);
-  for (int i = first; i < first + count; ++i) c->wins[i].done_idx = k;
+  for (int t = 0; t < n; ++t) c->wins[slots[t]].done_idx = k;
+}
+// Calls f(first, count) for each run of consecutive slots of a list, in list order (a range is one run).
+template <class F>
+int for_runs(const int32_t* slots, int n, F&& f) {
+  for (int i = 0; i < n;) {
+    int j = i + 1;
+    while (j < n && slots[j] == slots[j - 1] + 1) ++j;
+    const int rc = f(slots[i], j - i);
+    if (rc) return rc;
+    i = j;
+  }
+  return 0;
 }
 
 inline bool caps_cover(const WinCaps& a, const WinCaps& b) {
@@ -1206,7 +1227,7 @@ extern "C" int okb_window_reset(okb_ctx* c, int first, int count) {
       waited[S.done_idx] = true;
     }
   }
-  k_reset<<<count, 128, 0, xs>>>(c->d_wins, first, 1);
+  k_reset<<<count, 128, 0, xs>>>(c->d_wins, c->d_ident + first, 1);
   c->launches += 1;
   OKB_CUDA(c, cudaGetLastError());
   return OKB_OK;
@@ -1215,25 +1236,25 @@ extern "C" int okb_window_reset(okb_ctx* c, int first, int count) {
 // ---------------------------------------------------------------------------------------------
 // optimize
 // ---------------------------------------------------------------------------------------------
-// Launch geometry of one optimize of windows [first, first+count): everything a captured CUDA graph depends on
+// Launch geometry of one optimize of the listed windows: everything a captured CUDA graph depends on
 // besides the kernel arguments.
 struct RoundPlan {
   int max_chunks = 1, max_imu = 0, max_cx = 1, lm_wide = 0, acc_smem = 1, chol_smem = 1, solve_threads = S_THREADS, gxQ = 1, shard = 0, push_gx = 1;
   int lm_model = kDistAny, schur_wide = 0;      // (no padding bytes: the plan is compared bytewise as a graph key)
   size_t smA = 0, smS = 0, smQ = 0;
 };
-static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
+static int plan_rounds(okb_ctx* c, const int32_t* slots, int count, RoundPlan& P) {
   P = RoundPlan();
   int chol_smem = 1;       // solve_mode of k_solve: 1 system in shared memory, 2 pose system + chain band, 0 chain band only
   // k_schur: the block-pair and right-hand-side accumulators live in shared memory whenever they fit one CTA per SM
   // (K <= 22), else in the chunk's global partial; 256-thread CTAs where two fit an SM (K <= 12), else one 512-thread
   // CTA per SM
   int acc_smem = 1;
-  for (int i = first; i < first + count; ++i)
-    if (smemA2_bytes(c->host[i].K, 1) > (size_t)c->smem_optin) acc_smem = 0;
+  for (int t = 0; t < count; ++t)
+    if (smemA2_bytes(c->host[slots[t]].K, 1) > (size_t)c->smem_optin) acc_smem = 0;
   int maxL = 1;
-  for (int i = first; i < first + count; ++i) {
-    const WinDev& W = c->host[i];
+  for (int t = 0; t < count; ++t) {
+    const WinDev& W = c->host[slots[t]];
     P.max_chunks = std::max(P.max_chunks, W.n_chunks);
     P.max_imu = std::max(P.max_imu, W.n_imu);
     P.smA = std::max(P.smA, smemA2_bytes(W.K, acc_smem));
@@ -1247,8 +1268,8 @@ static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
     P.smQ = std::max(P.smQ, (size_t)W.NS * sizeof(SlotCtx));
     maxL = std::max(maxL, W.L);
   }
-  for (int i = first; i < first + count; ++i) {
-    const WinDev& W = c->host[i];
+  for (int t = 0; t < count; ++t) {
+    const WinDev& W = c->host[slots[t]];
     P.smS = std::max(P.smS, smemS_bytes(W.d, W.dc, W.K, W.marg_n, W.n_imu, chol_smem));
   }
   if (P.smS > (size_t)c->smem_optin) { c->set_error("window does not fit kernel S shared memory"); return OKB_ERR_CAPACITY; }
@@ -1257,8 +1278,8 @@ static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
     if ((m == 0 || m == 2) && chol_smem != 0 && !(chol_smem == 2 && m == 2)) {
       chol_smem = m;
       P.smS = 0;
-      for (int i = first; i < first + count; ++i) {
-        const WinDev& W = c->host[i];
+      for (int t = 0; t < count; ++t) {
+        const WinDev& W = c->host[slots[t]];
         P.smS = std::max(P.smS, smemS_bytes(W.d, W.dc, W.K, W.marg_n, W.n_imu, chol_smem));
       }
       if (P.smS > (size_t)c->smem_optin) { c->set_error("window does not fit kernel S shared memory"); return OKB_ERR_CAPACITY; }
@@ -1270,9 +1291,9 @@ static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
   // every tile's frame walk over a cluster of two 512-thread CTAs; the sums keep their order in either shape
   P.lm_wide = (2 * count * P.max_cx <= c->sm_count) ? 1 : 0;
   // k_landmarks is instantiated per distortion model: the one every camera of the launch shares, else the run-time switch
-  P.lm_model = c->wins[first].cam_model;
-  for (int i = first + 1; i < first + count; ++i)
-    if (c->wins[i].cam_model != P.lm_model) P.lm_model = kDistAny;
+  P.lm_model = c->wins[slots[0]].cam_model;
+  for (int t = 1; t < count; ++t)
+    if (c->wins[slots[t]].cam_model != P.lm_model) P.lm_model = kDistAny;
   P.solve_threads = (2 * count <= c->sm_count) ? 512 : S_THREADS;      // few windows: one wide CTA per SM (all ranks of a sharded window choose alike)
   P.gxQ = std::max(1, std::min((maxL + 127) / 128, (4 * c->sm_count + count - 1) / count));
   P.shard = c->shard_world > 1 ? 1 : 0;
@@ -1281,7 +1302,7 @@ static int plan_rounds(okb_ctx* c, int first, int count, RoundPlan& P) {
 }
 
 template <int MODEL>
-static void launch_landmarks(okb_ctx* c, int first, int count, const RoundPlan& P) {
+static void launch_landmarks(okb_ctx* c, int count, const RoundPlan& P) {
   if (P.lm_wide) {     // one cluster of two CTAs per landmark tile
     cudaLaunchConfig_t cfg = {};
     cudaLaunchAttribute attr[1];
@@ -1289,46 +1310,46 @@ static void launch_landmarks(okb_ctx* c, int first, int count, const RoundPlan& 
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.gridDim = dim3(2 * P.max_cx, count); cfg.blockDim = dim3(4 * L1_THREADS); cfg.dynamicSmemBytes = smemL_bytes(4);
     cfg.stream = c->stream; cfg.attrs = attr; cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, k_landmarks<4, 2, MODEL>, (const WinDev*)c->d_wins, first);
+    cudaLaunchKernelEx(&cfg, k_landmarks<4, 2, MODEL>, (const WinDev*)c->d_wins, (const int32_t*)c->d_slot_tab);
   } else {
-    k_landmarks<2, 1, MODEL><<<dim3(P.max_cx, count), 2 * L1_THREADS, smemL_bytes(2), c->stream>>>(c->d_wins, first);
+    k_landmarks<2, 1, MODEL><<<dim3(P.max_cx, count), 2 * L1_THREADS, smemL_bytes(2), c->stream>>>(c->d_wins, c->d_slot_tab);
   }
 }
 
-static int launch_rounds(okb_ctx* c, int first, int count, const okb_solve_options& opt, int rounds, const RoundPlan& P) {
+static int launch_rounds(okb_ctx* c, int count, const okb_solve_options& opt, int rounds, const RoundPlan& P) {
   for (int r = 0; r < rounds; ++r) {
     const dim3 gridA(P.max_chunks, count);
     static const bool imu_serial = getenv("OKB_IMU_SERIAL") != nullptr;     // diagnostics: k_imu on the main stream, ahead of the landmark kernels
     if (P.max_imu > 0 && imu_serial) {
-      k_imu<<<dim3((P.max_imu + 32 / IMU_G - 1) / (32 / IMU_G), count), 32, smemI_bytes(), c->stream>>>(c->d_wins, first);
+      k_imu<<<dim3((P.max_imu + 32 / IMU_G - 1) / (32 / IMU_G), count), 32, smemI_bytes(), c->stream>>>(c->d_wins, c->d_slot_tab);
       c->launches += 1;
     } else if (P.max_imu > 0) {   // IMU terms only depend on the previous round's candidate: run beside the landmark kernels
       cudaEventRecord(c->ev_round, c->stream);
       cudaStreamWaitEvent(c->stream_imu, c->ev_round, 0);
-      k_imu<<<dim3((P.max_imu + 32 / IMU_G - 1) / (32 / IMU_G), count), 32, smemI_bytes(), c->stream_imu>>>(c->d_wins, first);
+      k_imu<<<dim3((P.max_imu + 32 / IMU_G - 1) / (32 / IMU_G), count), 32, smemI_bytes(), c->stream_imu>>>(c->d_wins, c->d_slot_tab);
       cudaEventRecord(c->ev_imu, c->stream_imu);
       c->launches += 1;
     }
     prof_begin(c, 0);
     switch (P.lm_model) {
-      case OKB_DIST_NONE: launch_landmarks<OKB_DIST_NONE>(c, first, count, P); break;
-      case OKB_DIST_RADTAN: launch_landmarks<OKB_DIST_RADTAN>(c, first, count, P); break;
-      case OKB_DIST_EQUIDISTANT: launch_landmarks<OKB_DIST_EQUIDISTANT>(c, first, count, P); break;
-      case OKB_DIST_RADTAN8: launch_landmarks<OKB_DIST_RADTAN8>(c, first, count, P); break;
-      default: launch_landmarks<kDistAny>(c, first, count, P); break;
+      case OKB_DIST_NONE: launch_landmarks<OKB_DIST_NONE>(c, count, P); break;
+      case OKB_DIST_RADTAN: launch_landmarks<OKB_DIST_RADTAN>(c, count, P); break;
+      case OKB_DIST_EQUIDISTANT: launch_landmarks<OKB_DIST_EQUIDISTANT>(c, count, P); break;
+      case OKB_DIST_RADTAN8: launch_landmarks<OKB_DIST_RADTAN8>(c, count, P); break;
+      default: launch_landmarks<kDistAny>(c, count, P); break;
     }
-    if (P.schur_wide) k_schur<512><<<gridA, 512, P.smA, c->stream>>>(c->d_wins, first, P.acc_smem, opt.max_iterations);
-    else k_schur<256><<<gridA, 256, P.smA, c->stream>>>(c->d_wins, first, P.acc_smem, opt.max_iterations);
+    if (P.schur_wide) k_schur<512><<<gridA, 512, P.smA, c->stream>>>(c->d_wins, c->d_slot_tab, P.acc_smem, opt.max_iterations);
+    else k_schur<256><<<gridA, 256, P.smA, c->stream>>>(c->d_wins, c->d_slot_tab, P.acc_smem, opt.max_iterations);
     if (P.shard) {    // chunk reduction fused with the push half of the all-reduce over peer memory
-      k_shard_push<<<dim3(P.push_gx, count), 256, 0, c->stream>>>(c->d_wins, first);
+      k_shard_push<<<dim3(P.push_gx, count), 256, 0, c->stream>>>(c->d_wins, c->d_slot_tab);
       c->launches += 1;
-    } else if (P.max_chunks > 1) { k_reduce_partials<<<dim3(8, count), 256, 0, c->stream>>>(c->d_wins, first); c->launches += 1; }
+    } else if (P.max_chunks > 1) { k_reduce_partials<<<dim3(8, count), 256, 0, c->stream>>>(c->d_wins, c->d_slot_tab); c->launches += 1; }
     prof_end(c);
     c->launches += 2;
     if (P.max_imu > 0 && !imu_serial) cudaStreamWaitEvent(c->stream, c->ev_imu, 0);
     prof_begin(c, 1);
-    if (P.solve_threads == 512) k_solve<512><<<count, 512, P.smS, c->stream>>>(c->d_wins, first, opt, P.chol_smem);
-    else k_solve<S_THREADS><<<count, S_THREADS, P.smS, c->stream>>>(c->d_wins, first, opt, P.chol_smem);
+    if (P.solve_threads == 512) k_solve<512><<<count, 512, P.smS, c->stream>>>(c->d_wins, c->d_slot_tab, opt, P.chol_smem);
+    else k_solve<S_THREADS><<<count, S_THREADS, P.smS, c->stream>>>(c->d_wins, c->d_slot_tab, opt, P.chol_smem);
     prof_end(c);
     c->launches += 1;
   }
@@ -1337,9 +1358,9 @@ static int launch_rounds(okb_ctx* c, int first, int count, const okb_solve_optio
 }
 
 // post-solve landmark quality (Estimator.cpp:880-894)
-static int launch_quality(okb_ctx* c, int first, int count, const RoundPlan& P) {
+static int launch_quality(okb_ctx* c, int count, const RoundPlan& P) {
   prof_begin(c, 2);
-  k_quality<<<dim3(P.gxQ, count), 128, P.smQ, c->stream>>>(c->d_wins, first);
+  k_quality<<<dim3(P.gxQ, count), 128, P.smQ, c->stream>>>(c->d_wins, c->d_slot_tab);
   prof_end(c);
   c->launches += 1;
   OKB_CUDA(c, cudaGetLastError());
@@ -1349,21 +1370,21 @@ static int launch_quality(okb_ctx* c, int first, int count, const RoundPlan& P) 
 // The fixed launch sequence of one optimize (rounds + quality pass) as a CUDA graph: captured once per launch
 // geometry / option set and replayed -- one host call instead of ~70 launches and ~40 event operations, which is
 // what bounds the latency of a single window (SURVEY 8d "B = 1").  OKB_NO_GRAPH=1 disables it (diagnostics).
-static int run_rounds(okb_ctx* c, int first, int count, const okb_solve_options& opt, int rounds, bool with_quality) {
+static int run_rounds(okb_ctx* c, const int32_t* slots, int count, const okb_solve_options& opt, int rounds, bool with_quality) {
   RoundPlan P;
-  int rc = plan_rounds(c, first, count, P);
+  int rc = plan_rounds(c, slots, count, P);
   if (rc) return rc;
   static const bool no_graph = getenv("OKB_NO_GRAPH") != nullptr;
   // landmark-sharded windows spin on their peers inside k_solve: their kernels must reach the device in stream order,
   // not behind whatever hardware queue a graph's internal branches were mapped to
   if (c->profile || no_graph || c->shard_world > 1) {
-    rc = launch_rounds(c, first, count, opt, rounds, P);
-    if (!rc && with_quality) rc = launch_quality(c, first, count, P);
+    rc = launch_rounds(c, count, opt, rounds, P);
+    if (!rc && with_quality) rc = launch_quality(c, count, P);
     return rc;
   }
   okb_ctx::GraphEntry key;
   std::memset(&key, 0, sizeof key);
-  key.first = first; key.count = count; key.rounds = rounds; key.with_quality = with_quality ? 1 : 0;
+  key.count = count; key.rounds = rounds; key.with_quality = with_quality ? 1 : 0;
   key.opt_iter = opt.max_iterations; key.opt_min = opt.min_iterations; key.opt_cauchy = opt.use_cauchy_loss; key.opt_time = opt.time_limit_s;
   static_assert(sizeof(RoundPlan) <= sizeof(key.plan), "plan blob");
   std::memcpy(key.plan, &P, sizeof P);
@@ -1377,8 +1398,8 @@ static int run_rounds(okb_ctx* c, int first, int count, const okb_solve_options&
   const int64_t l0 = c->launches;
   cudaGraph_t graph = nullptr;
   OKB_CUDA(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-  rc = launch_rounds(c, first, count, opt, rounds, P);
-  if (!rc && with_quality) rc = launch_quality(c, first, count, P);
+  rc = launch_rounds(c, count, opt, rounds, P);
+  if (!rc && with_quality) rc = launch_quality(c, count, P);
   const cudaError_t ce = cudaStreamEndCapture(c->stream, &graph);
   if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
   OKB_CUDA(c, ce);
@@ -1401,16 +1422,52 @@ static int run_rounds(okb_ctx* c, int first, int count, const okb_solve_options&
   return OKB_OK;
 }
 
-extern "C" int okb_optimize_async(okb_ctx* c, int first, int count, const okb_solve_options* opt) {
-  int rc = check_range(c, first, count);
-  if (rc) return rc;
-  if (!opt || opt->max_iterations < 0) return OKB_ERR_INVALID_ARG;
+// Checks a slot list of okb_optimize_slots*: n >= 1 distinct, uploaded slots, on a context without landmark sharding.
+static int check_slots(okb_ctx* c, int n, const int32_t* slots) {
+  if (!c) return OKB_ERR_INVALID_ARG;
+  if (n < 1 || !slots) { c->set_error(n < 1 ? "empty slot list" : "NULL slot list"); return OKB_ERR_INVALID_ARG; }
+  std::vector<char> seen(c->max_windows, 0);
+  for (int t = 0; t < n; ++t) {
+    const int s = slots[t];
+    const std::string at = "slots[" + std::to_string(t) + "] = " + std::to_string(s);
+    if (s < 0 || s >= c->max_windows) { c->set_error(at + ": out of range"); return OKB_ERR_INVALID_ARG; }
+    if (!c->wins[s].uploaded) { c->set_error(at + ": window slot not uploaded"); return OKB_ERR_INVALID_ARG; }
+    if (seen[s]) { c->set_error(at + ": listed twice"); return OKB_ERR_INVALID_ARG; }
+    seen[s] = 1;
+  }
+  if (c->shard_world > 1) { c->set_error("landmark-sharded windows are optimized with okb_optimize (a range)"); return OKB_ERR_UNSUPPORTED; }
+  return OKB_OK;
+}
+
+// Writes the slot table of the launch about to be issued on `stream` into d_slot_tab, from ring entry done_next: the
+// done_ring entry that mark_work records after this launch, so the entry's previous copy has completed when
+// done_ring[done_next] has.  Every caller calls mark_work after it, also when this or a later step fails.  With more
+// than kDoneRing launches in flight this waits on the host for the oldest one (documented in okvis_b200.h).
+static int stage_slots(okb_ctx* c, const int32_t* slots, int n) {
+  const int k = c->done_next;
+  OKB_CUDA(c, cudaEventSynchronize(c->done_ring[k]));
+  int32_t* h = c->h_slot_ring + (size_t)k * c->max_windows;
+  std::memcpy(h, slots, sizeof(int32_t) * n);
+  OKB_CUDA(c, cudaMemcpyAsync(c->d_slot_tab, h, sizeof(int32_t) * n, cudaMemcpyHostToDevice, c->stream));
+  return OKB_OK;
+}
+
+static int read_states(okb_ctx* c, const int32_t* slots, int n) {
+  return for_runs(slots, n, [&](int f, int m) {
+    OKB_CUDA(c, cudaMemcpyAsync(c->h_states + f, c->d_states + f, sizeof(SolverState) * m, cudaMemcpyDeviceToHost, c->stream));
+    return OKB_OK;
+  });
+}
+
+// The optimize of the n listed windows (checked): a range call passes c->ident.data() + first.
+static int optimize_async(okb_ctx* c, const int32_t* slots, int count, const okb_solve_options* opt) {
   cudaSetDevice(c->device);
-  rc = commit_range(c, first, count);       // pending graph commands of these slots (no-op when there are none)
+  // pending graph commands of these slots (no-op when there are none), one commit per run of consecutive slots
+  int rc = for_runs(slots, count, [&](int f, int m) { return commit_range(c, f, m); });
   if (rc) return rc;
   // chunking: enough CTAs for ~2 waves when the batch is small
-  for (int i = first; i < first + count; ++i) {
-    WinDev& W = c->host[i];
+  for (int t = 0; t < count; ++t) {
+    WinDev& W = c->host[slots[t]];
     int chunks = (2 * c->sm_count + count - 1) / count;
     chunks = std::max(1, std::min(chunks, c->chunk_cap));
     chunks = std::min(chunks, std::max(1, W.L / (2 * A2_TILE)));
@@ -1419,21 +1476,25 @@ extern "C" int okb_optimize_async(okb_ctx* c, int first, int count, const okb_so
     W.use_cauchy = opt->use_cauchy_loss ? 1 : 0;
   }
   if (join_transfers(c)) { c->set_error("stream ordering failed"); return OKB_ERR_CUDA; }
-  OKB_CUDA(c, cudaMemcpyAsync(c->d_wins + first, &c->host[first], sizeof(WinDev) * count, cudaMemcpyHostToDevice, c->stream));
-  k_reset<<<count, 128, 0, c->stream>>>(c->d_wins, first, 0);
-  c->launches += 1;
-  for (int i = first; i < first + count; ++i) c->wins[i].opt = *opt;     // okb_optimize_finish relaunches with the range's own options
-  // round 0 linearises at the initial state; each later round judges one step and proposes the next
-  rc = run_rounds(c, first, count, *opt, opt->max_iterations + 1, true);
+  rc = for_runs(slots, count, [&](int f, int m) {
+    OKB_CUDA(c, cudaMemcpyAsync(c->d_wins + f, &c->host[f], sizeof(WinDev) * m, cudaMemcpyHostToDevice, c->stream));
+    return OKB_OK;
+  });
   if (rc) return rc;
-  OKB_CUDA(c, cudaMemcpyAsync(c->h_states + first, c->d_states + first, sizeof(SolverState) * count, cudaMemcpyDeviceToHost, c->stream));
-  mark_work(c, first, count);
+  for (int t = 0; t < count; ++t) c->wins[slots[t]].opt = *opt;     // optimize_finish relaunches with the call's own options
+  rc = stage_slots(c, slots, count);
+  if (!rc) {
+    k_reset<<<count, 128, 0, c->stream>>>(c->d_wins, c->d_slot_tab, 0);
+    c->launches += 1;
+    // round 0 linearises at the initial state; each later round judges one step and proposes the next
+    rc = run_rounds(c, slots, count, *opt, opt->max_iterations + 1, true);
+  }
+  if (!rc) rc = read_states(c, slots, count);
+  mark_work(c, slots, count);
   return rc;
 }
 
-extern "C" int okb_optimize_finish(okb_ctx* c, int first, int count, okb_summary* out) {
-  int rc = check_range(c, first, count);
-  if (rc) return rc;
+static int optimize_finish(okb_ctx* c, const int32_t* slots, int count, okb_summary* out) {
   cudaSetDevice(c->device);
   // optimize_async already queued the landmark-quality pass and the copy of the solver states.  Rebuild
   // rounds (linear-solver failures) consume rounds without advancing the iteration count: keep launching
@@ -1441,29 +1502,62 @@ extern "C" int okb_optimize_finish(okb_ctx* c, int first, int count, okb_summary
   for (int guard = 0; guard < 64; ++guard) {
     OKB_CUDA(c, cudaStreamSynchronize(c->stream));
     bool all_done = true;
-    for (int i = first; i < first + count; ++i) all_done = all_done && c->h_states[i].done;
+    for (int t = 0; t < count; ++t) all_done = all_done && c->h_states[slots[t]].done;
     if (all_done) break;
-    rc = run_rounds(c, first, count, c->wins[first].opt, 2, true);
+    int rc = stage_slots(c, slots, count);
+    if (!rc) rc = run_rounds(c, slots, count, c->wins[slots[0]].opt, 2, true);
+    if (!rc) rc = read_states(c, slots, count);
+    mark_work(c, slots, count);
     if (rc) return rc;
-    OKB_CUDA(c, cudaMemcpyAsync(c->h_states + first, c->d_states + first, sizeof(SolverState) * count, cudaMemcpyDeviceToHost, c->stream));
-    mark_work(c, first, count);
   }
-  for (int i = first; i < first + count; ++i) {
-    const SolverState& s = c->h_states[i];
+  for (int t = 0; t < count; ++t) {
+    const SolverState& s = c->h_states[slots[t]];
     if (s.g.err) { c->set_error(graph_error_text(s.g.err)); return graph_error_status(s.g.err); }
-    WinStore& S = c->wins[i];
+    WinStore& S = c->wins[slots[t]];
     if (!S.cmd_used) S.obs_bound = s.g.n_obs;      // exact length of the compacted observation list
   }
   if (out) {
-    for (int i = 0; i < count; ++i) {
-      const SolverState& s = c->h_states[first + i];
-      okb_summary& o = out[i];
+    for (int t = 0; t < count; ++t) {
+      const SolverState& s = c->h_states[slots[t]];
+      okb_summary& o = out[t];
       o.initial_cost = s.initial_cost; o.final_cost = s.cost; o.iterations = s.iteration;
       o.num_successful_steps = s.num_successful; o.termination = s.done ? s.termination : OKB_TERM_FAILURE;
       o.imu_redo_count = s.imu_redo_final; o.final_radius = s.radius; o.solve_time_s = s.solve_time_s;
     }
   }
   return OKB_OK;
+}
+
+extern "C" int okb_optimize_async(okb_ctx* c, int first, int count, const okb_solve_options* opt) {
+  int rc = check_range(c, first, count);
+  if (rc) return rc;
+  if (!opt || opt->max_iterations < 0) return OKB_ERR_INVALID_ARG;
+  return optimize_async(c, c->ident.data() + first, count, opt);
+}
+
+extern "C" int okb_optimize_finish(okb_ctx* c, int first, int count, okb_summary* out) {
+  int rc = check_range(c, first, count);
+  if (rc) return rc;
+  return optimize_finish(c, c->ident.data() + first, count, out);
+}
+
+extern "C" int okb_optimize_slots_async(okb_ctx* c, int n, const int32_t* slots, const okb_solve_options* opt) {
+  int rc = check_slots(c, n, slots);
+  if (rc) return rc;
+  if (!opt || opt->max_iterations < 0) return OKB_ERR_INVALID_ARG;
+  return optimize_async(c, slots, n, opt);
+}
+
+extern "C" int okb_optimize_slots_finish(okb_ctx* c, int n, const int32_t* slots, okb_summary* summaries) {
+  int rc = check_slots(c, n, slots);
+  if (rc) return rc;
+  return optimize_finish(c, slots, n, summaries);
+}
+
+extern "C" int okb_optimize_slots(okb_ctx* c, int n, const int32_t* slots, const okb_solve_options* opt, okb_summary* summaries) {
+  int rc = okb_optimize_slots_async(c, n, slots, opt);
+  if (rc) return rc;
+  return okb_optimize_slots_finish(c, n, slots, summaries);
 }
 
 // diagnostics: the ImuError cache of term `term` (reference bias of the preintegration, valid flag, redo counter)
@@ -1494,7 +1588,7 @@ extern "C" int okb_debug_schur_plan(okb_ctx* c, int first, int count, int32_t ou
   rc = commit_range(c, first, count);
   if (rc) return rc;
   RoundPlan P;
-  rc = plan_rounds(c, first, count, P);
+  rc = plan_rounds(c, c->ident.data() + first, count, P);
   if (rc) return rc;
   out[0] = P.acc_smem;
   out[1] = P.schur_wide ? 512 : 256;

@@ -63,8 +63,8 @@ __device__ __forceinline__ double block_max(double v, double* red) {
 // ------------------------------------------------------------------------------------------------
 constexpr int IMU_G = 16;      // lanes per IMU term: 32 / IMU_G terms per warp
 __host__ __device__ inline size_t smemI_bytes() { return (size_t)(32 / IMU_G) * kImuScratch * sizeof(double); }
-__global__ void __launch_bounds__(32, 12) k_imu(const WinDev* __restrict__ wins, int win_first) {
-  const WinDev& W = wins[win_first + blockIdx.y];
+__global__ void __launch_bounds__(32, 12) k_imu(const WinDev* __restrict__ wins, const int32_t* __restrict__ win_slots) {
+  const WinDev& W = wins[win_slots[blockIdx.y]];
   if (W.st->done) return;
   const int grp = (threadIdx.x & 31) / IMU_G;
   const int t = blockIdx.x * (32 / IMU_G) + grp;
@@ -233,10 +233,10 @@ __host__ __device__ inline size_t smemS_bytes(int d, int dc, int K, int n_marg, 
 // NT = 256: two CTAs per SM (batched throughput); NT = 512: one CTA per SM with twice the threads for small batches
 // (latency: the parallel phases -- assembly, trailing updates, landmark back-substitution -- run twice as wide).
 template <int NT>
-__global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_solve(const WinDev* __restrict__ wins, int win_first, okb_solve_options opt,
+__global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_solve(const WinDev* __restrict__ wins, const int32_t* __restrict__ win_slots, okb_solve_options opt,
                                                         int solve_mode) {
   const int chol_in_smem = (solve_mode == 1);
-  const WinDev& W = wins[win_first + blockIdx.x];
+  const WinDev& W = wins[win_slots[blockIdx.x]];
   SolverState* st = W.st;
   if (st->done) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -948,9 +948,10 @@ __global__ void __launch_bounds__(256) k_prepare(const WinDev* __restrict__ wins
   }
 }
 
-// resets the solver state (and optionally the parameter state: the one of the last full upload) of a range of windows
-__global__ void k_reset(const WinDev* __restrict__ wins, int win_first, int restore_params) {
-  const WinDev& W = wins[win_first + blockIdx.x];
+// resets the solver state (and optionally the parameter state: the one of the last full upload) of the windows
+// wins[win_slots[blockIdx.x]]
+__global__ void k_reset(const WinDev* __restrict__ wins, const int32_t* __restrict__ win_slots, int restore_params) {
+  const WinDev& W = wins[win_slots[blockIdx.x]];
   const int tid = threadIdx.x;
   if (restore_params) {
     for (int i = tid; i < 7 * W.K; i += blockDim.x) { W.pose[i] = W.pose_init[i]; W.out[i] = W.pose_init[i]; }

@@ -91,8 +91,8 @@ __device__ __forceinline__ double warp_reduce_scatter32(double (&v)[32]) {
 // <FG = 2, CS = 1>: 256 threads, three CTAs (24 warps) per SM at <= 80 registers.  <4, 2> (launches whose tiles
 // would fill less than half the SMs): clusters of two 512-thread CTAs, one CTA per SM, 8 frames in flight per tile.
 template <int FG, int CS, int MODEL>
-__global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 3 : 1) k_landmarks(const WinDev* __restrict__ wins, int win_first) {
-  const WinDev& W = wins[win_first + blockIdx.y];
+__global__ void __launch_bounds__(FG * L1_THREADS, FG == 2 ? 3 : 1) k_landmarks(const WinDev* __restrict__ wins, const int32_t* __restrict__ win_slots) {
+  const WinDev& W = wins[win_slots[blockIdx.y]];
   SolverState* st = W.st;
   if (st->done) return;                // (uniform over a cluster: same window, same landmark tile)
   const int cx = blockIdx.x / CS, crank = blockIdx.x % CS;
@@ -423,8 +423,8 @@ __device__ __forceinline__ void dmma_8x8x4(double& d0, double& d1, double a, dou
 
 // NT = 256 where two CTAs fit an SM (cfg-2), else 512: 16 warps per SM either way.
 template <int NT>
-__global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* __restrict__ wins, int win_first, int acc_smem, int max_iterations) {
-  const WinDev& W = wins[win_first + blockIdx.y];
+__global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* __restrict__ wins, const int32_t* __restrict__ win_slots, int acc_smem, int max_iterations) {
+  const WinDev& W = wins[win_slots[blockIdx.y]];
   SolverState* st = W.st;
   if (st->done) return;
   // the step being judged in this round is the last one (iteration limit): k_solve will not build another
@@ -644,8 +644,8 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) k_schur(const WinDev* _
 
 // Sums the per-chunk Schur accumulators of a window into chunk 0 (fixed order => deterministic), in
 // parallel over the matrix elements, so that k_solve reads one partial regardless of the chunk count.
-__global__ void __launch_bounds__(256) k_reduce_partials(const WinDev* __restrict__ wins, int win_first) {
-  const WinDev& W = wins[win_first + blockIdx.y];
+__global__ void __launch_bounds__(256) k_reduce_partials(const WinDev* __restrict__ wins, const int32_t* __restrict__ win_slots) {
+  const WinDev& W = wins[win_slots[blockIdx.y]];
   if (W.st->done || W.n_chunks <= 1) return;
   const int n = W.dcp * W.dcp;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -678,8 +678,8 @@ __device__ __forceinline__ unsigned long long* shard_flag(const WinDev& W, int d
   return reinterpret_cast<unsigned long long*>(W.shard_mail[dst] + which) + parity * kMaxShard + src;
 }
 
-__global__ void __launch_bounds__(256) k_shard_push(const WinDev* __restrict__ wins, int win_first) {
-  const WinDev& W = wins[win_first + blockIdx.y];
+__global__ void __launch_bounds__(256) k_shard_push(const WinDev* __restrict__ wins, const int32_t* __restrict__ win_slots) {
+  const WinDev& W = wins[win_slots[blockIdx.y]];
   SolverState* st = W.st;
   if (st->done) return;
   const int world = W.shard_world, me = W.shard_rank;
@@ -724,8 +724,8 @@ __global__ void __launch_bounds__(256) k_shard_push(const WinDev* __restrict__ w
 // Post-solve landmark quality: H = sum J_lm^T J_lm (sqrt-information weighted, no robust weight)
 // at the final estimate; quality = sqrt(lambda_min)/sqrt(lambda_max), 0 if lambda_min < 1e-12.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_quality(const WinDev* __restrict__ wins, int win_first) {
-  const WinDev& W = wins[win_first + blockIdx.y];
+__global__ void __launch_bounds__(128) k_quality(const WinDev* __restrict__ wins, const int32_t* __restrict__ win_slots) {
+  const WinDev& W = wins[win_slots[blockIdx.y]];
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SlotCtx* slots = reinterpret_cast<SlotCtx*>(smem_raw);
   const int tid = threadIdx.x;
