@@ -306,7 +306,8 @@ int okb_window_marginalize_batch(okb_ctx* ctx, int win_first, int count, const o
 /* Reads the window's current marginalisation prior back (tests, host-side persistence): J [n][n], e0 [n], the
  * H / b0 it was factored from, block list, linearisation points.  Any pointer may be NULL; arrays must hold the
  * compiled-in maxima (n <= 160, 64 blocks).  status[4] = {device error code of the last okb_window_marginalize,
- * rank of H, rank of the dense marginalised block, Jacobi sweeps}. */
+ * rank of H, rank of the dense marginalised block, Jacobi sweeps: the larger count of the dense block's and the final H's
+ * eigen-decompositions, 40 if either stopped at its sweep cap without converging}. */
 int okb_window_download_marg(okb_ctx* ctx, int win, int32_t* n, int32_t* n_blocks, int32_t* block_kind, uint32_t* block_idx,
                              double* x0, double* J, double* e0, double* H, double* b0, int32_t* status);
 

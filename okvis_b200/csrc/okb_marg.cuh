@@ -60,7 +60,7 @@ struct MargScratch {
   uint32_t* lmvis;        // [lm_cap] frames with a record
   int32_t* lmslot;        // [Lcap] landmark -> slot + 1 (all zero between calls)
   int32_t* clist;         // [Ocap] indices of the observations to linearise, list order
-  int32_t* status;        // [4]: error code, rank of the final H, rank of the dense V, sweeps
+  int32_t* status;        // [4]: error code, rank of the final H, rank of the dense V, Jacobi sweeps (max of phases 5, 6)
 };
 
 // One entry of k_marginalize's task table per CTA: the window it marginalises and where its job and scratch lie.
@@ -503,7 +503,8 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
     sc.A[i] = 0.5 * (sc.Hn[i] + sc.Hn[(size_t)c * n + r]) / marg_precond(sc.Hn[(size_t)r * n + r]) / marg_precond(sc.Hn[(size_t)c * n + c]);
   }
   __syncthreads();
-  jacobi_eig(sc.A, sc.Q, n, s_cs, s_pq, s_red);
+  const int sw6 = jacobi_eig(sc.A, sc.Q, n, s_cs, s_pq, s_red);
+  if (tid == 0) sc.status[3] = max(sc.status[3], sw6);       // 40: one of the two decompositions did not converge
   double lmax = -1e300;
   for (int k = tid; k < n; k += M_THREADS) lmax = fmax(lmax, sc.A[(size_t)k * n + k]);
   lmax = (n > 0) ? block_max(lmax, s_red) : 0.0;
