@@ -349,6 +349,14 @@ int okb_window_download(okb_ctx* ctx, int win, double* poses, double* speed_bias
  * runs on the transfer stream: it waits only for solver work launched on these slots, not for other slots. */
 int okb_window_download_batch(okb_ctx* ctx, int win_first, int count, double* const* poses,
                               double* const* speed_bias, double* const* landmarks, double* const* quality);
+/* List form of okb_window_download_batch (no reference counterpart; serves hosts whose ready sessions are scattered
+ * over the slots).  slots[i] are distinct, uploaded slots in any order; the pointer tables are in list order, with NULL
+ * tables or entries allowed as there.  Only the listed slots are touched: their pending edits are committed once per
+ * run of consecutive slots, only their solver work is waited for, one D2H copy per slot and one synchronisation.
+ * Each slot's outputs are byte-identical to okb_window_download on it.  List errors are those of okb_optimize_slots
+ * (OKB_ERR_INVALID_ARG naming the entry, OKB_ERR_UNSUPPORTED on a landmark-sharded context), before any device work. */
+int okb_window_download_slots(okb_ctx* ctx, int n, const int32_t* slots, double* const* poses,
+                              double* const* speed_bias, double* const* landmarks, double* const* quality);
 
 /* ----------------------------------------------------- landmark-sharded single window (multi-GPU)
  * No reference counterpart (the reference is single-process CPU code); this is the partition SURVEY.md 8(e) row 2 /

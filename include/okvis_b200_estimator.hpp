@@ -10,6 +10,10 @@
 //                                       on the host + okb_window_marginalize for MarginalizationError's numerics
 //                                       (MarginalizationError.cpp:127-435, 507-846) + okb_window_remove_*;
 //   * state prediction in addStates() = okb_imu_propagate                            (ImuError.cpp:287-504).
+// A standalone Estimator owns a one-window context.  An EstimatorGroup (below) owns one context for many sessions, one
+// slot each, and runs addStates / optimize / applyMarginalizationStrategy for a list of them with one batched device
+// call per step (okb_imu_propagate_batch, okb_optimize_slots + okb_window_download_slots, okb_window_marginalize_batch);
+// the three calls are split into host halves and a device step that the single and the group forms share.
 // Eigen-free: poses are [t(3), q_xyzw(4)] arrays exactly as PoseParameterBlock stores them
 // (okvis_ceres/src/PoseParameterBlock.cpp:68-79), so an OKVIS build wraps these calls one-to-one (INTEGRATION.md
 // shows the adaptor a maintainer would add; the MultiFrame / cv types stay on the OKVIS side of it).
@@ -18,6 +22,7 @@
 #pragma once
 #include <algorithm>
 #include <array>
+#include <chrono>
 #include <cmath>
 #include <cstdint>
 #include <iterator>
@@ -65,14 +70,52 @@ using MapPointVector = std::vector<MapPoint>;
 // Device-side capacities of an Estimator's resident window (okb_window_reserve).
 struct EstimatorCapacity { int frames = 16, landmarks = 4096, observations = 65536, imu_samples = 8192, marg_dim = 160; };
 
+class EstimatorGroup;
+
 class Estimator {
+ private:
+  friend class EstimatorGroup;
+  using Clock = std::chrono::steady_clock;
+  static double seconds(Clock::time_point t0) { return std::chrono::duration<double>(Clock::now() - t0).count(); }
+
+  struct State { uint64_t id = 0; int64_t t_ns = 0; bool isKeyframe = false, hasSb = false; Pose7 T_WS{}; SpeedAndBias sb{}; bool hasImuTerm = false; std::vector<okb_imu_sample> imuFromPrev; };
+  struct BlockRef { int kind; uint64_t id; };
+  // addStates between its halves: the new state, and (predict) the propagation from the previous state still to run
+  struct PendingState { State st; std::vector<okb_imu_sample> samples; bool predict = false; int64_t t0_ns = 0; int used = 0; };
+  // applyMarginalizationStrategy between its halves: the bookkeeping's results and the device job (none: !anything)
+  struct MargPlan {
+    bool skip = true, anything = false, reDoFixation = false;
+    std::vector<uint64_t> removeFrames, removeAllButPose, landmarksGone;
+    std::vector<BlockRef> blocks;
+    std::vector<int32_t> prev, kinds;
+    std::vector<uint8_t> margFlag;
+    std::vector<uint32_t> idx, jobTerms, jobSbPriors, jobLandmarks;
+    okb_marg_job job{};
+    const okb_marg_job* deviceJob() {
+      if (!anything) return nullptr;
+      job = okb_marg_job{};
+      job.n_blocks = (int32_t)blocks.size(); job.n_imu_terms = (int32_t)jobTerms.size(); job.n_sb_priors = (int32_t)jobSbPriors.size();
+      job.n_landmarks = (int32_t)jobLandmarks.size();
+      job.block_kind = kinds.data(); job.block_idx = idx.data(); job.block_prev = prev.data(); job.block_marginalize = margFlag.data();
+      job.imu_terms = jobTerms.data(); job.sb_priors = jobSbPriors.data(); job.landmarks = jobLandmarks.data();
+      return &job;
+    }
+  };
+  // Estimates as the download returns them, sized for the window as it is now.
+  struct Estimates { std::vector<double> poses, sbs, lms, q; };
+
  public:
   using Capacity = EstimatorCapacity;
 
+  // A standalone session: its own context with one window, slot 0.
   explicit Estimator(int device = 0, Capacity cap = Capacity()) : cap_(cap) {
     if (okb_ctx_create(device, 1, &ctx_) != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(nullptr));
   }
-  ~Estimator() { okb_ctx_destroy(ctx_); }
+  // A session of `group`: takes the group's lowest free slot (throws std::runtime_error when the group is full) and
+  // gives it back on destruction.  The slot's window from a previous occupant is replaced by this session's first
+  // full upload (its first optimize / applyMarginalizationStrategy), which also drops its pending commands and prior.
+  explicit Estimator(EstimatorGroup& group, Capacity cap = Capacity());
+  ~Estimator();
   Estimator(const Estimator&) = delete;
   Estimator& operator=(const Estimator&) = delete;
 
@@ -92,49 +135,19 @@ class Estimator {
 
   // ---- Estimator::addStates (Estimator.cpp:110-343): first frame -> gravity-aligned pose + priors; later frames ->
   // propagate the last state through the IMU samples, add an ImuError term.
+  // Three halves, shared with EstimatorGroup::addStates: prepareState (checks, first-frame pose and priors),
+  // the prediction (okb_imu_propagate here, one okb_imu_propagate_batch in the group) and appendState.
   bool addStates(uint64_t frameId, int64_t timestamp_ns, const std::vector<ImuMeasurement>& imu, bool asKeyframe) {
-    if (!hasImu_ || states_.count(frameId)) return false;
-    if (!states_.empty() && frameId < states_.rbegin()->first) return false;      // ids grow with time, as IdProvider's do
-    State st;
-    st.id = frameId; st.t_ns = timestamp_ns; st.isKeyframe = asKeyframe; st.hasSb = true;
-    std::vector<okb_imu_sample> s = toSamples(imu);
-    if (states_.empty()) {
-      if (!initPoseFromImu(imu, st.T_WS)) return false;
-      st.sb.fill(0.0);
-      for (int k = 0; k < 3; ++k) st.sb[6 + k] = imu_.a0[k];
-      // PoseError, information diag(1e8,1e8,1e8,0,0,1e8) with the reference's LLT result (SURVEY 8a item 8)
-      okb_pose_prior pp{};
-      for (int k = 0; k < 7; ++k) pp.meas[k] = st.T_WS[k];
-      const double d[6] = {1e4, 1e4, 1e4, 0, 0, 1e8};
-      for (int k = 0; k < 6; ++k) pp.sqrt_info[k * 6 + k] = d[k];
-      posePriors_.push_back({frameId, pp});
-      okb_sb_prior sp{};                      // SpeedAndBiasError(speedAndBias, 1.0, sigma_bg^2, sigma_ba^2)
-      for (int k = 0; k < 9; ++k) sp.meas[k] = st.sb[k];
-      const double si[9] = {1, 1, 1, 1 / imu_.sigma_bg, 1 / imu_.sigma_bg, 1 / imu_.sigma_bg, 1 / imu_.sigma_ba, 1 / imu_.sigma_ba, 1 / imu_.sigma_ba};
-      for (int k = 0; k < 9; ++k) sp.sqrt_info[k * 9 + k] = si[k];
-      sbPriors_.push_back({frameId, sp});
-    } else {
-      const State& prev = states_.rbegin()->second;
-      if (!prev.hasSb) return false;
-      st.T_WS = prev.T_WS; st.sb = prev.sb;
-      int used = 0;
-      if (okb_imu_propagate(ctx_, &imu_, s.data(), (int)s.size(), prev.t_ns, timestamp_ns, st.T_WS.data(), st.sb.data(), nullptr, nullptr, &used) != OKB_OK || used < 1)
-        return false;
-      st.imuFromPrev = s;
-      st.hasImuTerm = true;
+    PendingState p;
+    if (!prepareState(frameId, timestamp_ns, imu, asKeyframe, p)) return false;
+    if (p.predict) {
+      const auto t0 = Clock::now();
+      const int rc = okb_imu_propagate(ctx_, &imu_, p.samples.data(), (int)p.samples.size(), p.t0_ns, timestamp_ns, p.st.T_WS.data(),
+                                       p.st.sb.data(), nullptr, nullptr, &p.used);
+      deviceSeconds_ += seconds(t0);
+      if (rc != OKB_OK) return false;
     }
-    const bool first = states_.empty();
-    const uint64_t prevId = first ? 0 : states_.rbegin()->first;
-    states_[frameId] = st;
-    if (!first) terms_.push_back({prevId, frameId});
-    if (resident_) {
-      okb_imu_term t{};
-      const State& prev = states_.at(prevId);
-      t.pose0 = posePos(prevId); t.sb0 = sbPos(prevId); t.pose1 = posePos(frameId); t.sb1 = sbPos(frameId);
-      t.t0_ns = prev.t_ns; t.t1_ns = timestamp_ns; t.sample_offset = 0; t.sample_count = (uint32_t)s.size();
-      check(okb_window_add_frame(ctx_, 0, st.T_WS.data(), st.sb.data(), &t, s.data(), (int)s.size()));
-    }
-    return true;
+    return appendState(p);
   }
 
   // ---- landmarks / observations (Estimator.cpp:345-413, implementation/Estimator.hpp:43-90)
@@ -148,7 +161,7 @@ class Estimator {
     else slot = slotCount_++;
     if ((int)slot >= cap_.landmarks) throw std::runtime_error("okvis_b200: landmark capacity of the resident window exceeded");
     lmSlot_[landmarkId] = slot; slotOwner_[slot] = landmarkId;
-    if (resident_) check(okb_window_set_landmarks(ctx_, 0, 1, &slot, hp.data()));
+    if (resident_) check(okb_window_set_landmarks(ctx_, slot_, 1, &slot, hp.data()));
     return true;
   }
   // returns the residual block id (0 = duplicate observation, like the reference's NULL)
@@ -165,7 +178,7 @@ class Estimator {
     const uint64_t id = ++nextResidualId_;
     obs_[id] = o;
     it->second.observations[kid] = id;
-    if (resident_) { okb_observation d = deviceObs(o); check(okb_window_add_observations(ctx_, 0, 1, &d)); }
+    if (resident_) { okb_observation d = deviceObs(o); check(okb_window_add_observations(ctx_, slot_, 1, &d)); }
     return id;
   }
   bool removeObservation(uint64_t residualBlockId) {
@@ -173,7 +186,7 @@ class Estimator {
     if (it == obs_.end()) return false;
     if (resident_) {
       okb_obs_key k{posePos(it->second.pose), lmSlot_.at(it->second.lm), it->second.cam, 0};
-      check(okb_window_remove_observations(ctx_, 0, 1, &k));
+      check(okb_window_remove_observations(ctx_, slot_, 1, &k));
     }
     eraseObsHost(it);
     return true;
@@ -189,12 +202,51 @@ class Estimator {
 
   // ---- Estimator::applyMarginalizationStrategy (Estimator.cpp:434-773).  Bookkeeping on the host, numerics
   // (linearisation at the first-estimate points, Schur complements, eigen-factorisation) on the device.
+  // Split at its device step, as EstimatorGroup's form is: planMarginalization -> okb_window_marginalize -> finishMarginalization.
   bool applyMarginalizationStrategy(size_t numKeyframes, size_t numImuFrames, MapPointVector& removedLandmarks) {
+    MargPlan p;
+    planMarginalization(numKeyframes, numImuFrames, removedLandmarks, p);
+    if (p.skip) return true;
+    if (const okb_marg_job* job = p.deviceJob()) {
+      const auto t0 = Clock::now();
+      const int rc = okb_window_marginalize(ctx_, slot_, job);
+      deviceSeconds_ += seconds(t0);
+      check(rc);
+    }
+    finishMarginalization(p);
+    return true;
+  }
+  bool applyMarginalizationStrategy(size_t numKeyframes, size_t numImuFrames) { MapPointVector r; return applyMarginalizationStrategy(numKeyframes, numImuFrames, r); }
+
+  // ---- Estimator::optimize (Estimator.cpp:843-906) + setOptimizationTimeLimit (:909-929)
+  bool setOptimizationTimeLimit(double timeLimit, int minIterations) { timeLimit_ = timeLimit; minIterations_ = minIterations; return true; }
+  void optimize(size_t numIter, size_t /*numThreads*/ = 1, bool /*verbose*/ = false) {
+    if (!prepareOptimize()) return;
+    const okb_solve_options opt = solveOptions(numIter);
+    Estimates e = estimateBuffers();
+    const auto t0 = Clock::now();
+    int rc = okb_optimize(ctx_, slot_, 1, &opt, &summary_);
+    if (rc == OKB_OK) rc = okb_window_download(ctx_, slot_, e.poses.data(), e.sbs.data(), e.lms.data(), e.q.data());
+    deviceSeconds_ += seconds(t0);
+    check(rc);
+    adoptEstimates(e);
+  }
+  const okb_summary& summary() const { return summary_; }
+  // bytes the last commit of the window moved host -> device (a frame's worth once the window is resident; 0 before)
+  int64_t lastUploadBytes() const { return resident_ ? okb_window_h2d_bytes(ctx_, slot_) : 0; }
+
+ private:
+  // applyMarginalizationStrategy, plan half: the reference's bookkeeping (removeObservation appends included) and the
+  // device job.  p.skip: fewer frames than numImuFrames + 1, nothing to do.
+  void planMarginalization(size_t numKeyframes, size_t numImuFrames, MapPointVector& removedLandmarks, MargPlan& p) {
     // keep the newest numImuFrames
     auto rit = states_.rbegin();
-    for (size_t k = 0; k < numImuFrames; ++k) { ++rit; if (rit == states_.rend()) return true; }
+    for (size_t k = 0; k < numImuFrames; ++k) { ++rit; if (rit == states_.rend()) return; }
+    p.skip = false;
     ensureResident();
-    std::vector<uint64_t> removeFrames, removeAllButPose, allLinearizedFrames;
+    std::vector<uint64_t>& removeFrames = p.removeFrames;
+    std::vector<uint64_t>& removeAllButPose = p.removeAllButPose;
+    std::vector<uint64_t> allLinearizedFrames;
     size_t countedKeyframes = 0;
     for (; rit != states_.rend(); ++rit) {
       if (!rit->second.isKeyframe || countedKeyframes >= numKeyframes) removeFrames.push_back(rit->first);
@@ -205,16 +257,21 @@ class Estimator {
     auto contains = [](const std::vector<uint64_t>& v, uint64_t q) { return std::find(v.begin(), v.end(), q) != v.end(); };
     // the linear system: blocks of the current prior first (their order), newly connected blocks appended in the
     // order MarginalizationError::addResidualBlock meets them
-    std::vector<BlockRef> blocks = margBlocks_;
-    std::vector<int32_t> prev(blocks.size());
+    std::vector<BlockRef>& blocks = p.blocks;
+    blocks = margBlocks_;
+    std::vector<int32_t>& prev = p.prev;
+    prev.resize(blocks.size());
     for (size_t i = 0; i < blocks.size(); ++i) prev[i] = (int32_t)i;
-    std::vector<uint8_t> margFlag(blocks.size(), 0);
+    std::vector<uint8_t>& margFlag = p.margFlag;
+    margFlag.assign(blocks.size(), 0);
     auto connect = [&](int kind, uint64_t id) -> size_t {
       for (size_t i = 0; i < blocks.size(); ++i) if (blocks[i].kind == kind && blocks[i].id == id) return i;
       blocks.push_back({kind, id}); prev.push_back(-1); margFlag.push_back(0);
       return blocks.size() - 1;
     };
-    std::vector<uint32_t> jobTerms, jobSbPriors, jobLandmarks;
+    std::vector<uint32_t>& jobTerms = p.jobTerms;
+    std::vector<uint32_t>& jobSbPriors = p.jobSbPriors;
+    std::vector<uint32_t>& jobLandmarks = p.jobLandmarks;
     std::set<size_t> termDone, sbPriorDone;
     auto linearizeTerm = [&](size_t ti) {
       if (!termDone.insert(ti).second) return;
@@ -222,7 +279,7 @@ class Estimator {
       connect(OKB_BLOCK_POSE, terms_[ti].second); connect(OKB_BLOCK_SPEED_BIAS, terms_[ti].second);
       jobTerms.push_back((uint32_t)ti);
     };
-    bool anything = false;
+    bool& anything = p.anything;
     // marginalize everything but pose (Estimator.cpp:483-554): the speed/bias block of every frame that left the IMU window
     for (uint64_t fid : removeAllButPose) {
       State& st = states_.at(fid);
@@ -235,8 +292,8 @@ class Estimator {
         if (sbPriors_[pi].frame == fid && sbPriorDone.insert(pi).second) jobSbPriors.push_back((uint32_t)pi);
     }
     // marginalize ONLY pose now (:556-733)
-    bool reDoFixation = false;
-    std::vector<uint64_t> landmarksGone;             // marginalised or deleted (device slots to clear)
+    bool& reDoFixation = p.reDoFixation;
+    std::vector<uint64_t>& landmarksGone = p.landmarksGone;      // marginalised or deleted (device slots to clear)
     if (!removeFrames.empty()) {
       const uint64_t currentKfId = allLinearizedFrames.at(0);
       for (uint64_t fid : removeFrames) {
@@ -286,34 +343,36 @@ class Estimator {
         ++pit;
       }
     }
-    // ---- numerics on the device (positions as the window is NOW)
+    // ---- the job for the numerics on the device (positions as the window is NOW)
     if (anything) {
-      std::vector<int32_t> kinds(blocks.size());
-      std::vector<uint32_t> idx(blocks.size());
-      for (size_t i = 0; i < blocks.size(); ++i) { kinds[i] = blocks[i].kind; idx[i] = blocks[i].kind == OKB_BLOCK_POSE ? posePos(blocks[i].id) : sbPos(blocks[i].id); }
-      okb_marg_job job{};
-      job.n_blocks = (int32_t)blocks.size(); job.n_imu_terms = (int32_t)jobTerms.size(); job.n_sb_priors = (int32_t)jobSbPriors.size();
-      job.n_landmarks = (int32_t)jobLandmarks.size();
-      job.block_kind = kinds.data(); job.block_idx = idx.data(); job.block_prev = prev.data(); job.block_marginalize = margFlag.data();
-      job.imu_terms = jobTerms.data(); job.sb_priors = jobSbPriors.data(); job.landmarks = jobLandmarks.data();
-      check(okb_window_marginalize(ctx_, 0, &job));
+      p.kinds.resize(blocks.size());
+      p.idx.resize(blocks.size());
+      for (size_t i = 0; i < blocks.size(); ++i) { p.kinds[i] = blocks[i].kind; p.idx[i] = blocks[i].kind == OKB_BLOCK_POSE ? posePos(blocks[i].id) : sbPos(blocks[i].id); }
+    }
+  }
+  // applyMarginalizationStrategy, finish half (after the device job ran): adopt the kept blocks, make the same
+  // structural edits on the device and in the host maps, re-fix the first pose.
+  void finishMarginalization(const MargPlan& p) {
+    const std::vector<uint64_t>& removeFrames = p.removeFrames;
+    auto contains = [](const std::vector<uint64_t>& v, uint64_t q) { return std::find(v.begin(), v.end(), q) != v.end(); };
+    if (p.anything) {
       std::vector<BlockRef> kept;
-      for (size_t i = 0; i < blocks.size(); ++i) if (!margFlag[i]) kept.push_back(blocks[i]);
+      for (size_t i = 0; i < p.blocks.size(); ++i) if (!p.margFlag[i]) kept.push_back(p.blocks[i]);
       margBlocks_.swap(kept);
     }
     // ---- the same structural edits on the device and in the host maps
-    for (uint64_t lid : landmarksGone) {
+    for (uint64_t lid : p.landmarksGone) {
       // observations still attached to a deleted landmark die with it on the device (okb_window_remove_landmarks)
       for (auto o = obs_.begin(); o != obs_.end();) o = (o->second.lm == lid) ? obs_.erase(o) : std::next(o);
       const uint32_t slot = lmSlot_.at(lid);
-      check(okb_window_remove_landmarks(ctx_, 0, 1, &slot));
+      check(okb_window_remove_landmarks(ctx_, slot_, 1, &slot));
       lmSlot_.erase(lid); slotOwner_.erase(slot); freeSlots_.insert(slot);
     }
-    for (uint64_t fid : removeAllButPose) {          // newest first: positions of older blocks do not move
+    for (uint64_t fid : p.removeAllButPose) {        // newest first: positions of older blocks do not move
       State& st = states_.at(fid);
       const bool whole = contains(removeFrames, fid);
       if (whole) {
-        check(okb_window_remove_frame(ctx_, 0, posePos(fid), st.hasSb ? sbPos(fid) : 0xffffffffu));
+        check(okb_window_remove_frame(ctx_, slot_, posePos(fid), st.hasSb ? sbPos(fid) : 0xffffffffu));
         for (auto o = obs_.begin(); o != obs_.end();) {
           if (o->second.pose == fid) {
             auto lm = landmarks_.find(o->second.lm);
@@ -322,15 +381,15 @@ class Estimator {
           } else ++o;
         }
       } else if (st.hasSb) {
-        check(okb_window_remove_speed_bias(ctx_, 0, sbPos(fid)));
+        check(okb_window_remove_speed_bias(ctx_, slot_, sbPos(fid)));
       }
       // host mirrors of the device lists (stable compaction, exactly what the interpreter does)
       eraseIf(terms_, [&](const TermRef& t) { return (t.first == fid || t.second == fid); });
-      eraseIf(sbPriors_, [&](const SbPrior& p) { return p.frame == fid; });
-      if (whole) { eraseIf(posePriors_, [&](const PosePrior& p) { return p.frame == fid; }); states_.erase(fid); }
+      eraseIf(sbPriors_, [&](const SbPrior& q) { return q.frame == fid; });
+      if (whole) { eraseIf(posePriors_, [&](const PosePrior& q) { return q.frame == fid; }); states_.erase(fid); }
       else st.hasSb = false;
     }
-    if (reDoFixation && !states_.empty()) {
+    if (p.reDoFixation && !states_.empty()) {
       // finally fix the first pose properly (Estimator.cpp:761-770): information diag(1e14 x3, 0, 0, 1e14); the
       // reference's LLT leaves diag(1e7,1e7,1e7,0,0,1e14) as the square root (SURVEY 8a item 8)
       const State& first = states_.begin()->second;
@@ -341,37 +400,42 @@ class Estimator {
       posePriors_.push_back({first.id, pp});
     }
     pushPriors();
+  }
+
+  // optimize, host half before the solve: false where there is nothing to solve
+  bool prepareOptimize() {
+    if (states_.empty() || cameras_.empty()) return false;
+    ensureResident();
     return true;
   }
-  bool applyMarginalizationStrategy(size_t numKeyframes, size_t numImuFrames) { MapPointVector r; return applyMarginalizationStrategy(numKeyframes, numImuFrames, r); }
-
-  // ---- Estimator::optimize (Estimator.cpp:843-906) + setOptimizationTimeLimit (:909-929)
-  bool setOptimizationTimeLimit(double timeLimit, int minIterations) { timeLimit_ = timeLimit; minIterations_ = minIterations; return true; }
-  void optimize(size_t numIter, size_t /*numThreads*/ = 1, bool /*verbose*/ = false) {
-    if (states_.empty() || cameras_.empty()) return;
-    ensureResident();
+  okb_solve_options solveOptions(size_t numIter) const {
     okb_solve_options opt{};
     opt.max_iterations = (int)numIter; opt.min_iterations = minIterations_; opt.time_limit_s = timeLimit_; opt.use_cauchy_loss = 1;
-    check(okb_optimize(ctx_, 0, 1, &opt, &summary_));
+    return opt;
+  }
+  Estimates estimateBuffers() const {
     const size_t K = states_.size(), NSB = numSb(), L = slotCount_ ? slotCount_ : 1;
-    std::vector<double> poses(7 * K), sbs(9 * std::max<size_t>(NSB, 1)), lms(4 * L), q(L);
-    check(okb_window_download(ctx_, 0, poses.data(), sbs.data(), lms.data(), q.data()));
+    Estimates e;
+    e.poses.resize(7 * K); e.sbs.resize(9 * std::max<size_t>(NSB, 1)); e.lms.resize(4 * L); e.q.resize(L);
+    return e;
+  }
+  // optimize, write-back half (Estimator.cpp:880-900): poses, speed/bias, and point + quality for every landmark
+  void adoptEstimates(const Estimates& e) {
     size_t i = 0, j = 0;
     for (auto& kv : states_) {
-      std::copy(poses.begin() + 7 * i, poses.begin() + 7 * i + 7, kv.second.T_WS.begin()); ++i;
-      if (kv.second.hasSb) { std::copy(sbs.begin() + 9 * j, sbs.begin() + 9 * j + 9, kv.second.sb.begin()); ++j; }
+      std::copy(e.poses.begin() + 7 * i, e.poses.begin() + 7 * i + 7, kv.second.T_WS.begin()); ++i;
+      if (kv.second.hasSb) { std::copy(e.sbs.begin() + 9 * j, e.sbs.begin() + 9 * j + 9, kv.second.sb.begin()); ++j; }
     }
-    for (auto& kv : landmarks_) {            // Estimator.cpp:880-900: point + quality written back for every landmark
+    for (auto& kv : landmarks_) {
       const uint32_t s = lmSlot_.at(kv.first);
-      std::copy(lms.begin() + 4 * s, lms.begin() + 4 * s + 4, kv.second.point.begin());
-      kv.second.quality = q[s];
+      std::copy(e.lms.begin() + 4 * s, e.lms.begin() + 4 * s + 4, kv.second.point.begin());
+      kv.second.quality = e.q[s];
       const Vec4& hp = kv.second.point;
       kv.second.distance = std::fabs(hp[3]) > 1e-8 ? std::sqrt(hp[0] * hp[0] + hp[1] * hp[1] + hp[2] * hp[2]) / std::fabs(hp[3]) : 1e300;
     }
   }
-  const okb_summary& summary() const { return summary_; }
-  // bytes the last commit of the window moved host -> device (a frame's worth once the window is resident)
-  int64_t lastUploadBytes() const { return okb_window_h2d_bytes(ctx_, 0); }
+
+ public:
 
   // ---- getters / setters (Estimator.cpp:931-1230)
   bool get_T_WS(uint64_t poseId, Pose7& T) const { auto it = states_.find(poseId); if (it == states_.end()) return false; T = it->second.T_WS; return true; }
@@ -387,13 +451,13 @@ class Estimator {
   bool set_T_WS(uint64_t poseId, const Pose7& T) {
     auto it = states_.find(poseId); if (it == states_.end()) return false;
     it->second.T_WS = T;
-    if (resident_) { const uint32_t p = posePos(poseId); check(okb_window_set_states(ctx_, 0, 1, &p, T.data(), 0, nullptr, nullptr)); }
+    if (resident_) { const uint32_t p = posePos(poseId); check(okb_window_set_states(ctx_, slot_, 1, &p, T.data(), 0, nullptr, nullptr)); }
     return true;
   }
   bool setSpeedAndBias(uint64_t poseId, size_t /*imuIdx*/, const SpeedAndBias& sb) {
     auto it = states_.find(poseId); if (it == states_.end() || !it->second.hasSb) return false;
     it->second.sb = sb;
-    if (resident_) { const uint32_t p = sbPos(poseId); check(okb_window_set_states(ctx_, 0, 0, nullptr, nullptr, 1, &p, sb.data())); }
+    if (resident_) { const uint32_t p = sbPos(poseId); check(okb_window_set_states(ctx_, slot_, 0, nullptr, nullptr, 1, &p, sb.data())); }
     return true;
   }
   bool setCameraSensorStates(uint64_t poseId, size_t cameraIdx, const Pose7& T_SCi) {
@@ -411,7 +475,7 @@ class Estimator {
   bool setLandmark(uint64_t id, const Vec4& hp) {
     auto it = landmarks_.find(id); if (it == landmarks_.end()) return false;
     it->second.point = hp;
-    if (resident_) { const uint32_t s = lmSlot_.at(id); check(okb_window_set_landmarks(ctx_, 0, 1, &s, hp.data())); }
+    if (resident_) { const uint32_t s = lmSlot_.at(id); check(okb_window_set_landmarks(ctx_, slot_, 1, &s, hp.data())); }
     return true;
   }
   bool isLandmarkAdded(uint64_t id) const { return landmarks_.count(id) != 0; }
@@ -460,10 +524,70 @@ class Estimator {
     return true;
   }
 
+  // Slot of the session's window in its context (0 for a standalone Estimator).
+  int slot() const { return slot_; }
+  // Seconds this session spent inside C-ABI calls that run and wait for device work (prediction, optimize + download,
+  // marginalisation); the rest of a call's wall time is host bookkeeping.  Group calls account on the group.
+  double deviceSeconds() const { return deviceSeconds_; }
+
  private:
-  struct State { uint64_t id = 0; int64_t t_ns = 0; bool isKeyframe = false, hasSb = false; Pose7 T_WS{}; SpeedAndBias sb{}; bool hasImuTerm = false; std::vector<okb_imu_sample> imuFromPrev; };
+
+  // addStates, host check / prepare half: nothing changes; false where the single call returns false before its
+  // prediction.  A prediction needs two samples at least (okb_imu_propagate rejects fewer): such a request fails here
+  // so that it cannot fail a group's whole prediction batch.
+  bool prepareState(uint64_t frameId, int64_t timestamp_ns, const std::vector<ImuMeasurement>& imu, bool asKeyframe, PendingState& p) const {
+    if (!hasImu_ || states_.count(frameId)) return false;
+    if (!states_.empty() && frameId < states_.rbegin()->first) return false;      // ids grow with time, as IdProvider's do
+    State& st = p.st;
+    st.id = frameId; st.t_ns = timestamp_ns; st.isKeyframe = asKeyframe; st.hasSb = true;
+    p.samples = toSamples(imu);
+    if (states_.empty()) {
+      if (!initPoseFromImu(imu, st.T_WS)) return false;
+      st.sb.fill(0.0);
+      for (int k = 0; k < 3; ++k) st.sb[6 + k] = imu_.a0[k];
+      return true;
+    }
+    const State& prev = states_.rbegin()->second;
+    if (!prev.hasSb || p.samples.size() < 2) return false;
+    st.T_WS = prev.T_WS; st.sb = prev.sb;
+    p.predict = true; p.t0_ns = prev.t_ns;
+    return true;
+  }
+  // addStates, append half: after the prediction wrote p.st's pose / speed-bias and p.used
+  bool appendState(PendingState& p) {
+    State& st = p.st;
+    const uint64_t frameId = st.id;
+    if (p.predict) {
+      if (p.used < 1) return false;
+      st.imuFromPrev = p.samples;
+      st.hasImuTerm = true;
+    } else {
+      // PoseError, information diag(1e8,1e8,1e8,0,0,1e8) with the reference's LLT result (SURVEY 8a item 8)
+      okb_pose_prior pp{};
+      for (int k = 0; k < 7; ++k) pp.meas[k] = st.T_WS[k];
+      const double d[6] = {1e4, 1e4, 1e4, 0, 0, 1e8};
+      for (int k = 0; k < 6; ++k) pp.sqrt_info[k * 6 + k] = d[k];
+      posePriors_.push_back({frameId, pp});
+      okb_sb_prior sp{};                      // SpeedAndBiasError(speedAndBias, 1.0, sigma_bg^2, sigma_ba^2)
+      for (int k = 0; k < 9; ++k) sp.meas[k] = st.sb[k];
+      const double si[9] = {1, 1, 1, 1 / imu_.sigma_bg, 1 / imu_.sigma_bg, 1 / imu_.sigma_bg, 1 / imu_.sigma_ba, 1 / imu_.sigma_ba, 1 / imu_.sigma_ba};
+      for (int k = 0; k < 9; ++k) sp.sqrt_info[k * 9 + k] = si[k];
+      sbPriors_.push_back({frameId, sp});
+    }
+    const bool first = states_.empty();
+    const uint64_t prevId = first ? 0 : states_.rbegin()->first;
+    states_[frameId] = st;
+    if (!first) terms_.push_back({prevId, frameId});
+    if (resident_) {
+      okb_imu_term t{};
+      const State& prev = states_.at(prevId);
+      t.pose0 = posePos(prevId); t.sb0 = sbPos(prevId); t.pose1 = posePos(frameId); t.sb1 = sbPos(frameId);
+      t.t0_ns = prev.t_ns; t.t1_ns = st.t_ns; t.sample_offset = 0; t.sample_count = (uint32_t)p.samples.size();
+      check(okb_window_add_frame(ctx_, slot_, st.T_WS.data(), st.sb.data(), &t, p.samples.data(), (int)p.samples.size()));
+    }
+    return true;
+  }
   struct Obs { uint64_t lm, pose; uint32_t cam; size_t kp; double z[2]; double sqrt_info; };
-  struct BlockRef { int kind; uint64_t id; };
   using TermRef = std::pair<uint64_t, uint64_t>;            // ImuError between two frame ids, in the device's list order
   struct PosePrior { uint64_t frame; okb_pose_prior p; };
   struct SbPrior { uint64_t frame; okb_sb_prior p; };
@@ -501,7 +625,7 @@ class Estimator {
     std::vector<okb_pose_prior> pps; std::vector<okb_sb_prior> sps;
     for (auto& p : posePriors_) { okb_pose_prior q = p.p; q.pose_idx = posePos(p.frame); pps.push_back(q); }
     for (auto& p : sbPriors_) { okb_sb_prior q = p.p; q.sb_idx = sbPos(p.frame); sps.push_back(q); }
-    check(okb_window_set_priors(ctx_, 0, (int)pps.size(), pps.data(), (int)sps.size(), sps.data(), nullptr));
+    check(okb_window_set_priors(ctx_, slot_, (int)pps.size(), pps.data(), (int)sps.size(), sps.data(), nullptr));
   }
   // First contact with the device: the whole graph once (okb_window_upload); everything after that is incremental.
   void ensureResident() {
@@ -535,12 +659,15 @@ class Estimator {
     d.poses = poses.data(); d.speed_bias = sbs.data(); d.extrinsics = ext.data(); d.extrinsics_fixed = extFixed.data(); d.landmarks = lms.data();
     d.cameras = cameras_.data(); d.obs = obs.data(); d.imu_terms = terms.data(); d.imu_samples = samples.data(); d.imu_params = imu_;
     d.pose_priors = pps.data(); d.sb_priors = sps.data();
-    check(okb_window_reserve(ctx_, 0, cap_.frames, cap_.landmarks, cap_.observations, cap_.imu_samples, cap_.marg_dim));
-    check(okb_window_upload(ctx_, 0, &d));
+    check(okb_window_reserve(ctx_, slot_, cap_.frames, cap_.landmarks, cap_.observations, cap_.imu_samples, cap_.marg_dim));
+    check(okb_window_upload(ctx_, slot_, &d));
     resident_ = true;
   }
 
   okb_ctx* ctx_ = nullptr;
+  EstimatorGroup* group_ = nullptr;          // nullptr: standalone, ctx_ is owned
+  int slot_ = 0;
+  double deviceSeconds_ = 0;
   Capacity cap_;
   bool resident_ = false;
   std::vector<ExtrinsicsEstimationParameters> extrinsicsParams_;
@@ -565,5 +692,183 @@ class Estimator {
   double timeLimit_ = -1.0; int minIterations_ = 0;
   okb_summary summary_{};
 };
+
+// Many okvis::Estimator sessions in one context: the group owns a context of `max_sessions` windows, each session of
+// the group (Estimator(group)) one slot of it.  Member calls of a session work as on a standalone Estimator; the group
+// calls below run one per-frame step of the ThreadedKFVio cycle for a list of its sessions with one batched device call:
+//   addStates                    -> one okb_imu_propagate_batch for every request that needs a prediction
+//   optimize                     -> one okb_optimize_slots per distinct option set + one okb_window_download_slots
+//   applyMarginalizationStrategy -> one okb_window_marginalize_batch over the span of the sessions' slots
+// Lists may be in any order and need not be contiguous.  A duplicate, a session of another group or a standalone
+// Estimator throws std::invalid_argument before anything changes.  Sessions not listed are not committed, waited for,
+// read or written.
+// Results: each session's estimates, summary and bookkeeping equal, bit for bit, what the same member calls made one
+// session at a time in a group of the same max_sessions give, as long as one optimize lists at most SMs/2 sessions
+// (66 on an H100; longer batches take another launch shape of the reduced solve) and every camera of its sessions
+// uses one distortion model (a batch whose cameras mix models runs the landmark kernel's run-time-switch
+// instantiation, which rounds differently).  Against a standalone Estimator the bookkeeping is identical.  So are the
+// estimates while a window holds at most 64 * floor(2 * SMs / max_sessions) landmarks; beyond that the one-window
+// context splits the landmark sums into more chunks, and the estimates agree to rounding.
+// Threading: as for the C-ABI context, the caller serialises group calls and the member calls of the group's sessions
+// (what Estimator's estimator_mutex_ does for one session in the reference).  Sessions are destroyed before their group.
+class EstimatorGroup {
+ public:
+  struct StatesRequest {
+    Estimator* session;
+    uint64_t frameId;
+    int64_t timestamp_ns;
+    std::vector<ImuMeasurement> imu;
+    bool asKeyframe;
+  };
+
+  EstimatorGroup(int device, int max_sessions) : max_(max_sessions) {
+    if (max_sessions < 1) throw std::invalid_argument("okvis_b200: a group holds at least one session");
+    if (okb_ctx_create(device, max_sessions, &ctx_) != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(nullptr));
+    for (int s = 0; s < max_sessions; ++s) free_.insert(s);
+  }
+  ~EstimatorGroup() { okb_ctx_destroy(ctx_); }
+  EstimatorGroup(const EstimatorGroup&) = delete;
+  EstimatorGroup& operator=(const EstimatorGroup&) = delete;
+
+  int maxSessions() const { return max_; }
+  int numSessions() const { return max_ - (int)free_.size(); }
+  int64_t kernelLaunches() const { return okb_kernel_launches(ctx_); }
+  // Seconds the group calls spent inside the batched C-ABI calls (see Estimator::deviceSeconds).
+  double deviceSeconds() const { return deviceSeconds_; }
+
+  // Estimator::addStates for each request; one result per request, as the single call returns it.
+  std::vector<bool> addStates(const std::vector<StatesRequest>& requests) {
+    std::vector<Estimator*> sessions;
+    for (const auto& r : requests) sessions.push_back(r.session);
+    validate(sessions);
+    const size_t n = requests.size();
+    std::vector<Estimator::PendingState> p(n);
+    std::vector<char> ok(n, 0);
+    std::vector<okb_propagate_job> jobs;
+    std::vector<size_t> of;
+    for (size_t i = 0; i < n; ++i) {
+      const StatesRequest& r = requests[i];
+      ok[i] = r.session->prepareState(r.frameId, r.timestamp_ns, r.imu, r.asKeyframe, p[i]);
+      if (!ok[i] || !p[i].predict) continue;
+      okb_propagate_job j{};
+      j.params = &r.session->imu_; j.samples = p[i].samples.data(); j.n_samples = (int32_t)p[i].samples.size();
+      j.t0_ns = p[i].t0_ns; j.t1_ns = r.timestamp_ns; j.pose = p[i].st.T_WS.data(); j.speed_bias = p[i].st.sb.data();
+      j.n_used = &p[i].used;
+      jobs.push_back(j); of.push_back(i);
+    }
+    if (!jobs.empty()) {
+      const auto t0 = Clock::now();
+      const int rc = okb_imu_propagate_batch(ctx_, (int)jobs.size(), jobs.data());
+      deviceSeconds_ += Estimator::seconds(t0);
+      if (rc != OKB_OK) for (size_t i : of) ok[i] = 0;        // as a failing okb_imu_propagate: addStates returns false
+    }
+    std::vector<bool> out(n);
+    for (size_t i = 0; i < n; ++i) out[i] = ok[i] && requests[i].session->appendState(p[i]);
+    return out;
+  }
+
+  // Estimator::optimize(numIter) for each session: sessions with nothing to solve are skipped as the single call skips
+  // them; the rest are solved with one okb_optimize_slots per distinct (numIter, minIterations, timeLimit), then
+  // downloaded with one okb_window_download_slots and written back.
+  void optimize(const std::vector<Estimator*>& sessions, size_t numIter) {
+    validate(sessions);
+    std::vector<Estimator*> live;
+    for (Estimator* e : sessions) if (e->prepareOptimize()) live.push_back(e);
+    if (live.empty()) return;
+    const size_t n = live.size();
+    std::vector<okb_solve_options> opt(n);
+    for (size_t i = 0; i < n; ++i) opt[i] = live[i]->solveOptions(numIter);
+    std::vector<Estimator::Estimates> e(n);
+    std::vector<int32_t> all(n);
+    std::vector<double*> poses(n), sbs(n), lms(n), q(n);
+    for (size_t i = 0; i < n; ++i) {
+      e[i] = live[i]->estimateBuffers();
+      all[i] = live[i]->slot_;
+      poses[i] = e[i].poses.data(); sbs[i] = e[i].sbs.data(); lms[i] = e[i].lms.data(); q[i] = e[i].q.data();
+    }
+    std::vector<char> done(n, 0);
+    const auto t0 = Clock::now();
+    for (size_t i = 0; i < n; ++i) {
+      if (done[i]) continue;
+      std::vector<int32_t> slots;
+      std::vector<size_t> members;
+      for (size_t k = i; k < n; ++k)
+        if (!done[k] && opt[k].min_iterations == opt[i].min_iterations && opt[k].time_limit_s == opt[i].time_limit_s) {
+          slots.push_back(live[k]->slot_); members.push_back(k); done[k] = 1;
+        }
+      std::vector<okb_summary> summ(slots.size());
+      const int rc = okb_optimize_slots(ctx_, (int)slots.size(), slots.data(), &opt[i], summ.data());
+      if (rc != OKB_OK) { deviceSeconds_ += Estimator::seconds(t0); check(rc); }
+      for (size_t m = 0; m < members.size(); ++m) live[members[m]]->summary_ = summ[m];
+    }
+    const int rc = okb_window_download_slots(ctx_, (int)n, all.data(), poses.data(), sbs.data(), lms.data(), q.data());
+    deviceSeconds_ += Estimator::seconds(t0);
+    check(rc);
+    for (size_t i = 0; i < n; ++i) live[i]->adoptEstimates(e[i]);
+  }
+
+  // Estimator::applyMarginalizationStrategy(numKeyframes, numImuFrames, removed[i]) for each session: every session
+  // plans (the host bookkeeping), one okb_window_marginalize_batch runs the jobs, every session finishes.  removed is
+  // resized to the list's length if shorter; removed[i] receives what sessions[i] removes.  A failing batch throws
+  // std::runtime_error naming the slot (Estimator::slot()) of the session whose job it rejected.
+  bool applyMarginalizationStrategy(const std::vector<Estimator*>& sessions, size_t numKeyframes, size_t numImuFrames,
+                                    std::vector<MapPointVector>& removed) {
+    validate(sessions);
+    const size_t n = sessions.size();
+    if (removed.size() < n) removed.resize(n);
+    std::vector<Estimator::MargPlan> p(n);
+    for (size_t i = 0; i < n; ++i) sessions[i]->planMarginalization(numKeyframes, numImuFrames, removed[i], p[i]);
+    int lo = max_, hi = -1;
+    std::vector<const okb_marg_job*> jobs(max_, nullptr);
+    for (size_t i = 0; i < n; ++i) {
+      if (p[i].skip) continue;
+      if (const okb_marg_job* j = p[i].deviceJob()) {
+        const int s = sessions[i]->slot_;
+        jobs[s] = j; lo = std::min(lo, s); hi = std::max(hi, s);
+      }
+    }
+    if (hi >= lo) {
+      const auto t0 = Clock::now();
+      const int rc = okb_window_marginalize_batch(ctx_, lo, hi - lo + 1, jobs.data() + lo);
+      deviceSeconds_ += Estimator::seconds(t0);
+      check(rc);
+    }
+    for (size_t i = 0; i < n; ++i) if (!p[i].skip) sessions[i]->finishMarginalization(p[i]);
+    return true;
+  }
+
+ private:
+  friend class Estimator;
+  using Clock = Estimator::Clock;
+
+  void check(int rc) const { if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx_)); }
+  void validate(const std::vector<Estimator*>& sessions) const {
+    std::set<const Estimator*> seen;
+    for (size_t i = 0; i < sessions.size(); ++i) {
+      const Estimator* e = sessions[i];
+      const std::string at = "okvis_b200: EstimatorGroup: entry " + std::to_string(i);
+      if (!e) throw std::invalid_argument(at + " is null");
+      if (e->group_ != this) throw std::invalid_argument(at + (e->group_ ? " is a session of another group" : " is a standalone Estimator"));
+      if (!seen.insert(e).second) throw std::invalid_argument(at + " lists a session twice");
+    }
+  }
+  int takeSlot() {
+    if (free_.empty()) throw std::runtime_error("okvis_b200: EstimatorGroup: all " + std::to_string(max_) + " sessions are taken");
+    const int s = *free_.begin();
+    free_.erase(free_.begin());
+    return s;
+  }
+
+  okb_ctx* ctx_ = nullptr;
+  int max_;
+  std::set<int> free_;
+  double deviceSeconds_ = 0;
+};
+
+inline Estimator::Estimator(EstimatorGroup& group, Capacity cap) : ctx_(group.ctx_), group_(&group), slot_(group.takeSlot()), cap_(cap) {}
+inline Estimator::~Estimator() {
+  if (group_) group_->free_.insert(slot_);
+  else okb_ctx_destroy(ctx_);
+}
 
 }  // namespace okvis_b200

@@ -221,4 +221,6 @@ def load_library(path=LIB_PATH):
     lib.okb_optimize_slots.argtypes = [C.c_void_p, C.c_int, slots_t, C.POINTER(SolveOptions), C.POINTER(Summary)]
     lib.okb_optimize_slots_async.argtypes = [C.c_void_p, C.c_int, slots_t, C.POINTER(SolveOptions)]
     lib.okb_optimize_slots_finish.argtypes = [C.c_void_p, C.c_int, slots_t, C.POINTER(Summary)]
+    tab_t = C.POINTER(C.POINTER(C.c_double))
+    lib.okb_window_download_slots.argtypes = [C.c_void_p, C.c_int, slots_t, tab_t, tab_t, tab_t, tab_t]
     return lib

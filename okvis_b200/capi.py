@@ -312,12 +312,16 @@ class Context:
 
     def alloc_outputs(self, first, count):
         """Host buffers for download_batch plus the pointer tables over them."""
+        return self.alloc_slot_outputs(range(first, first + count))
+
+    def alloc_slot_outputs(self, slots):
+        """Host buffers for download_slots (list order) plus the pointer tables over them."""
         outs = []
-        for i in range(first, first + count):
+        for i in slots:
             w = self._windows[i]
             outs.append(dict(poses=np.zeros_like(w.poses), speed_bias=np.zeros_like(w.speed_bias),
                              landmarks=np.zeros_like(w.landmarks), quality=np.zeros(len(w.landmarks))))
-        PP = C.POINTER(C.c_double) * count
+        PP = C.POINTER(C.c_double) * len(outs)
         tables = [PP(*[o[k].ctypes.data_as(C.POINTER(C.c_double)) for o in outs])
                   for k in ("poses", "speed_bias", "landmarks", "quality")]
         return outs, tables
@@ -325,6 +329,14 @@ class Context:
     def download_batch(self, first, count, out=None):
         outs, tables = out if out is not None else self.alloc_outputs(first, count)
         self._check(lib().okb_window_download_batch(self._h, int(first), int(count), *tables))
+        return outs
+
+    def download_slots(self, slots, out=None):
+        """okb_window_download_slots: the estimates of the listed slots (any order), in list order.  `out` as from
+        alloc_slot_outputs(slots) (the buffers follow each slot's uploaded window shape)."""
+        outs, tables = out if out is not None else self.alloc_slot_outputs(slots)
+        n, arr = self._slot_list(slots)
+        self._check(lib().okb_window_download_slots(self._h, n, arr, *tables))
         return outs
 
     # ---------------------------------------------------------------- single-block hooks

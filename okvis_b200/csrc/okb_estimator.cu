@@ -1636,43 +1636,60 @@ extern "C" int okb_window_download(okb_ctx* c, int win, double* poses, double* s
   return OKB_OK;
 }
 
-extern "C" int okb_window_download_batch(okb_ctx* c, int first, int count, double* const* poses, double* const* speed_bias,
-                                         double* const* landmarks, double* const* quality) {
-  int rc = check_range(c, first, count);
-  if (rc) return rc;
+// The one path behind okb_window_download_batch (a range passes c->ident.data() + first) and okb_window_download_slots
+// (checked list): pending edits committed once per run of consecutive listed slots, a wait on each distinct solver
+// event of the listed slots, one D2H copy per slot, one synchronisation.  Output tables are in list order.
+static int download_list(okb_ctx* c, const int32_t* slots, int count, double* const* poses, double* const* speed_bias,
+                         double* const* landmarks, double* const* quality) {
   cudaSetDevice(c->device);
-  rc = commit_range(c, first, count);
+  int rc = for_runs(slots, count, [&](int f, int m) { return commit_range(c, f, m); });
   if (rc) return rc;
   cudaStream_t xs = c->stream_xfer;
   bool waited[okb_ctx::kDoneRing] = {};
-  for (int i = first; i < first + count; ++i) {
-    WinStore& S = c->wins[i];
+  for (int t = 0; t < count; ++t) {
+    WinStore& S = c->wins[slots[t]];
     if (S.done_idx >= 0 && !waited[S.done_idx]) {
       OKB_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
       waited[S.done_idx] = true;
     }
   }
-  for (int i = first; i < first + count; ++i)
+  for (int t = 0; t < count; ++t) {
+    const int i = slots[t];
     OKB_CUDA(c, cudaMemcpyAsync(c->wins[i].out_staging, c->host[i].out, sizeof(double) * out_doubles(c->host[i]), cudaMemcpyDeviceToHost, xs));
-  WinStore& S0 = c->wins[first];
+  }
+  WinStore& S0 = c->wins[slots[0]];
   OKB_CUDA(c, cudaEventRecord(S0.down, xs));
   OKB_CUDA(c, cudaEventSynchronize(S0.down));
-  auto copy_out = [&](int i) {
-    const int k = i - first;
+  auto copy_out = [&](int k) {
+    const int i = slots[k];
     copy_out_window(c->host[i], c->wins[i], poses ? poses[k] : nullptr, speed_bias ? speed_bias[k] : nullptr,
                     landmarks ? landmarks[k] : nullptr, quality ? quality[k] : nullptr);
   };
   const int T = std::max(1, std::min(8, count / 32));
   if (T == 1) {
-    for (int i = first; i < first + count; ++i) copy_out(i);
+    for (int k = 0; k < count; ++k) copy_out(k);
   } else {
     std::vector<std::thread> th;
     th.reserve(T);
     for (int t = 0; t < T; ++t)
-      th.emplace_back([&, t]() { for (int i = first + t; i < first + count; i += T) copy_out(i); });
+      th.emplace_back([&, t]() { for (int k = t; k < count; k += T) copy_out(k); });
     for (auto& x : th) x.join();
   }
   return OKB_OK;
+}
+
+extern "C" int okb_window_download_batch(okb_ctx* c, int first, int count, double* const* poses, double* const* speed_bias,
+                                         double* const* landmarks, double* const* quality) {
+  int rc = check_range(c, first, count);
+  if (rc) return rc;
+  return download_list(c, c->ident.data() + first, count, poses, speed_bias, landmarks, quality);
+}
+
+extern "C" int okb_window_download_slots(okb_ctx* c, int n, const int32_t* slots, double* const* poses, double* const* speed_bias,
+                                         double* const* landmarks, double* const* quality) {
+  int rc = check_slots(c, n, slots);
+  if (rc) return rc;
+  return download_list(c, slots, n, poses, speed_bias, landmarks, quality);
 }
 
 // ---------------------------------------------------------------------------------------------
