@@ -259,7 +259,9 @@ int okb_window_set_states(okb_ctx* ctx, int win, int n_poses, const uint32_t* po
 int okb_window_set_priors(okb_ctx* ctx, int win, int n_pose_priors, const okb_pose_prior* pose_priors, int n_sb_priors,
                           const okb_sb_prior* sb_priors, const okb_marg_prior* marg);
 /* Ships the pending commands of slots [win_first, win_first+count) to the device (transfer stream; overlaps solver
- * work on other slots).  Optional: the calls that need the result do it themselves. */
+ * work on other slots).  Optional: the calls that need the result do it themselves.  On a landmark-sharded context it
+ * returns once the commands are applied on the device, and is NOT optional after edits: every rank commits before any
+ * rank's okb_optimize*, so that no rank's graph update still queues while its peers' solvers wait on the exchange. */
 int okb_window_commit(okb_ctx* ctx, int win_first, int count);
 
 /* Removes speed/bias block sb_idx together with the ImuError terms and SpeedAndBiasError priors attached to it; the
@@ -292,7 +294,28 @@ typedef struct okb_marg_job {
   const uint32_t* sb_priors;        /* SpeedAndBiasError terms to linearise */
   const uint32_t* landmarks;        /* landmarks to marginalise: every observation they still have is linearised */
 } okb_marg_job;
+/* Landmark-sharded windows (okb_shard_*, below): EVERY rank calls okb_window_marginalize* on the window, with the same
+ * dense part of the job (block lists, IMU terms, speed/bias priors) and, in `landmarks`, only the marginalised
+ * landmarks it holds, as local slots (global slot g lives on rank g % world at local slot g / world).  A rank that
+ * holds none of them still calls, with n_landmarks = 0.  Each rank linearises its own landmarks; their Schur terms are
+ * summed over the ranks through the shard mailbox in rank order, so the new prior -- J, e0, H / b0, block list, x0,
+ * status -- is bit-identical on all ranks.  The calls of all ranks may be issued from one host thread in rank order:
+ * no host wait inside the call depends on the peers (buffers the context outgrows are kept until it is destroyed).
+ * Device statuses beyond those of an unsharded window (download_marg status[0]):
+ *   6 (shard job)     the ranks' dense parts differ (okb_marg_job_fingerprint);
+ *   7 (shard timeout) a peer did not arrive within 4 s, or pushed a box of another exchange epoch;
+ * and a device error of any one rank (status 1-5, below) is reported by every rank.  A rank reporting any of these
+ * abandons the step before the dense marginalisation: its previous prior stays in place, and its next okb_optimize*
+ * fails until a full upload.  Statuses 6 and 1-5 are seen by every rank alike; a time-out only by the ranks that timed
+ * out (a peer arriving later completes the step), after which the ranks are out of step and the shard contexts must be
+ * recreated.  ImuError caches the step had already re-preintegrated keep their new state, as the
+ * reference's functor cache does after any evaluation.  Status codes of any window: 1 bad block list, 2 block_prev
+ * inconsistent with the current prior, 3 a listed term's blocks are not all listed, 4 a marginalised landmark is
+ * observed in a frame that is not listed, 5 dimension mismatch. */
 int okb_window_marginalize(okb_ctx* ctx, int win, const okb_marg_job* job);
+/* The 64-bit hash landmark-sharded ranks compare before summing: N, the kept dimension, the block lists and the
+ * IMU-term / speed/bias-prior lists of `job` (not its landmarks). */
+int okb_marg_job_fingerprint(const okb_marg_job* job, uint64_t* out);
 /* Batched okb_window_marginalize (no reference counterpart; serves hosts that keep many estimators on one GPU).
  * jobs[i] describes slot win_first+i; jobs[i] == NULL: that slot is not touched (no commit, no wait on its solve, no
  * copy), so its okb_optimize_async may still be running.  Each slot's result -- prior, H / b0, block list, x0, ImuError
@@ -301,7 +324,10 @@ int okb_window_marginalize(okb_ctx* ctx, int win, const okb_marg_job* job);
  * slot unchanged.  count < 1 or a range outside max_windows: OKB_ERR_INVALID_ARG; all jobs NULL: no-op.  Pending
  * edits of the job slots are committed first; one k_marginalize launch (one CTA per job) then runs on the transfer
  * stream after the solver work already launched on the job slots only, and later calls on those slots are ordered
- * after it.  Errors the device finds stay with their slot and surface as for the single call. */
+ * after it.  Errors the device finds stay with their slot and surface as for the single call.  On a landmark-sharded
+ * context every rank calls with the same slots, one exchange per slot, under the contract of okb_window_marginalize.
+ * Each job occupies one SM while it waits for its peers: ranks that share one device need the sum of their jobs per
+ * call to stay at most the device's SM count. */
 int okb_window_marginalize_batch(okb_ctx* ctx, int win_first, int count, const okb_marg_job* const* jobs);
 /* Reads the window's current marginalisation prior back (tests, host-side persistence): J [n][n], e0 [n], the
  * H / b0 it was factored from, block list, linearisation points.  Any pointer may be NULL; arrays must hold the

@@ -22,6 +22,15 @@ class OkbError(RuntimeError):
         self.code = code
 
 
+def marg_job_fingerprint(job):
+    """okb_marg_job_fingerprint: the hash landmark-sharded ranks compare (dense part of the job, not its landmarks)."""
+    out = C.c_uint64(0)
+    rc = lib().okb_marg_job_fingerprint(C.byref(job), C.byref(out))
+    if rc != 0:
+        raise OkbError(rc, "malformed job")
+    return out.value
+
+
 def _p(a):
     return C.c_void_p(a.ctypes.data) if a is not None else None
 

@@ -95,13 +95,21 @@ struct okb_ctx {
   size_t marg_host_bytes = 0, marg_dev_bytes = 0;
   cudaEvent_t marg_copied = nullptr;     // recorded after the H2D copy of marg_host
   bool marg_busy = false;                // that copy may still be in flight (wait on marg_copied before rewriting)
+  // Buffers a landmark-sharded context outgrew, freed with the context: cudaFree / cudaFreeHost wait for the whole
+  // device, and a peer rank on the same device may be spinning in k_marginalize until this rank's launch arrives.
+  // Growth doubles, so these stay bounded.
+  std::vector<unsigned char*> marg_retired_dev, marg_retired_host;
+  // Sharded contexts: pinned pack buffers whose H2D copy was still queued when the next call came; reused once `done`
+  // (recorded after that copy) has completed, so a pipelining host needs at most one buffer per call in flight.
+  struct MargPinned { unsigned char* p; size_t bytes; cudaEvent_t done; };
+  std::vector<MargPinned> marg_pool;
   // okb_imu_propagate (on `stream`) and okb_imu_propagate_batch (on stream_prop, created on first use) each own a set
   PropBuffers prop_one, prop_batch;
   cudaStream_t stream_prop = nullptr;
   std::atomic<int64_t> prop_launches{0};   // counted apart from `launches`: a batch may run beside a solve's launches
   okb_frontend_state* frontend = nullptr;
   // landmark-sharded windows (okb_shard_*): this rank's mailbox and the peers' mailboxes as mapped on this device
-  int shard_rank = 0, shard_world = 1, shard_box_cap = 0;
+  int shard_rank = 0, shard_world = 1, shard_box_cap = 0, shard_marg_cap = 0;
   size_t shard_win_bytes = 0;
   unsigned char* shard_local = nullptr;                       // cudaMalloc'ed, exported through cudaIpc
   unsigned char* shard_peer[okb::kMaxShard] = {};             // [rank]; own entry = shard_local

@@ -156,6 +156,9 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
   if (c->marg_host) cudaFreeHost(c->marg_host);
   if (c->marg_dev) cudaFree(c->marg_dev);
   if (c->marg_copied) cudaEventDestroy(c->marg_copied);
+  for (unsigned char* p : c->marg_retired_dev) cudaFree(p);
+  for (unsigned char* p : c->marg_retired_host) cudaFreeHost(p);
+  for (auto& e : c->marg_pool) { cudaFreeHost(e.p); cudaEventDestroy(e.done); }
   for (PropBuffers* b : {&c->prop_one, &c->prop_batch}) {
     if (b->host) cudaFreeHost(b->host);
     if (b->dev) cudaFree(b->dev);
@@ -375,6 +378,7 @@ static const char* graph_error_text(int e) {
     case GERR_SQRT_INFO: return "window graph: observation with non-positive sqrt information";
     case GERR_DIMS: return "window graph: host / device dimension mismatch";
     case GERR_MARG_REF: return "window graph: a removed frame is still referenced by the marginalisation prior";
+    case GERR_SHARD_MARG: return "window graph: a landmark-sharded marginalisation was abandoned on every rank (okb_window_download_marg status)";
     default: return "window graph: unknown error";
   }
 }
@@ -432,7 +436,12 @@ static int commit_range(okb_ctx* c, int first, int count) {
 
 extern "C" int okb_window_commit(okb_ctx* c, int first, int count) {
   if (!c || first < 0 || count < 1 || first + count > c->max_windows) return OKB_ERR_INVALID_ARG;
-  return commit_range(c, first, count);
+  const int rc = commit_range(c, first, count);
+  // landmark-sharded: the edits are applied before the call returns, so that no rank's graph compile is still queued
+  // when a peer's solver kernels start spinning on the exchange (a rank whose commit ran beside them arrived seconds
+  // late and its peers timed out)
+  if (!rc && c->shard_world > 1) OKB_CUDA(c, cudaStreamSynchronize(c->stream_xfer));
+  return rc;
 }
 
 // Full upload = a command stream that rebuilds the whole graph (host side: validation of what only the host can
@@ -542,7 +551,7 @@ static int upload_pack(okb_ctx* c, int win, const okb_window_desc* D) {
   W.marg_n = marg_n; W.marg_nb = marg_nb; W.marg_xdim = marg_xdim;
   W.imu_params = D->imu_params;
   derive_dims(W);
-  W.shard_rank = c->shard_rank; W.shard_world = c->shard_world; W.shard_box_cap = c->shard_box_cap;
+  W.shard_rank = c->shard_rank; W.shard_world = c->shard_world; W.shard_box_cap = c->shard_box_cap; W.shard_marg_cap = c->shard_marg_cap;
   if (c->shard_world > 1) {
     if (shard_box_doubles(K, W.dcp) > (size_t)c->shard_box_cap) { c->set_error("window exceeds the shard mailbox (max_frames of okb_shard_export)"); return OKB_ERR_CAPACITY; }
     for (int r = 0; r < c->shard_world; ++r) {
@@ -908,6 +917,30 @@ int marg_check(const okb_ctx* c, int win, const okb_marg_job* job, MargDims& d, 
   return OKB_OK;
 }
 
+// FNV-1a over the part of a job every rank of a landmark-sharded window must share: N, n_keep, the block lists, the
+// IMU-term and speed/bias-prior lists (each with its length).  The landmark list is the rank's own and is left out.
+uint64_t marg_job_fingerprint(const okb_marg_job* job) {
+  uint64_t h = 1469598103934665603ull;
+  auto mix = [&](const void* p, size_t bytes) {
+    const unsigned char* b = static_cast<const unsigned char*>(p);
+    for (size_t i = 0; i < bytes; ++i) { h ^= b[i]; h *= 1099511628211ull; }
+  };
+  const size_t nb = (size_t)std::max(job->n_blocks, 0);
+  int32_t dims[3] = {0, 0, job->n_blocks};
+  for (size_t b = 0; b < nb; ++b) {
+    const int dim = job->block_kind[b] == OKB_BLOCK_SPEED_BIAS ? 9 : 6;
+    dims[0] += dim;
+    if (!job->block_marginalize[b]) dims[1] += dim;
+  }
+  mix(dims, sizeof dims);
+  mix(job->block_kind, 4 * nb); mix(job->block_idx, 4 * nb); mix(job->block_prev, 4 * nb); mix(job->block_marginalize, nb);
+  mix(&job->n_imu_terms, 4);
+  if (job->n_imu_terms > 0) mix(job->imu_terms, 4 * (size_t)job->n_imu_terms);
+  mix(&job->n_sb_priors, 4);
+  if (job->n_sb_priors > 0) mix(job->sb_priors, 4 * (size_t)job->n_sb_priors);
+  return h;
+}
+
 // The one path behind okb_window_marginalize (n = 1) and okb_window_marginalize_batch: jobs[t] runs on slot slots[t]
 // (ascending, distinct).  Every job is checked before any device work.  Then, on the transfer stream: the pending
 // edits of the job slots are committed, the task table and the job payloads go over in one H2D copy, each run of
@@ -925,6 +958,10 @@ int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int 
     }
   }
   cudaStream_t xs = c->stream_xfer;
+  // Landmark-sharded context: all ranks' calls may come from one host thread in rank order, so nothing below may wait
+  // on the host for this rank's earlier launches (they may be spinning until a peer's launch arrives).  Outgrown
+  // buffers are retired rather than freed; the launch runs the sharded instantiation.
+  const bool sharded = c->shard_world > 1;
   // scratch of the job slots and the call's device buffer: growing frees the old ones, which waits for the transfer
   // stream once
   size_t bytes = align_up(sizeof(MargTask) * (size_t)n, 256);
@@ -938,11 +975,14 @@ int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int 
     grow[t] = !S.marg_scratch || S.marg_lm_cap < jobs[t]->n_landmarks || S.marg_K_cap < S.caps.K || S.marg_L_cap < S.caps.L || S.marg_O_cap < S.caps.O;
     wait = wait || (grow[t] && S.marg_scratch);
   }
-  if (wait) OKB_CUDA(c, cudaStreamSynchronize(xs));
+  if (wait && !sharded) OKB_CUDA(c, cudaStreamSynchronize(xs));
   for (int t = 0; t < n; ++t) {
     if (!grow[t]) continue;
     WinStore& S = c->wins[slots[t]];
-    if (S.marg_scratch) { cudaFree(S.marg_scratch); S.marg_scratch = nullptr; }
+    if (S.marg_scratch) {
+      if (sharded) c->marg_retired_dev.push_back(S.marg_scratch); else cudaFree(S.marg_scratch);
+      S.marg_scratch = nullptr;
+    }
     S.marg_lm_cap = std::max(256, 2 * jobs[t]->n_landmarks); S.marg_K_cap = S.caps.K; S.marg_L_cap = S.caps.L; S.marg_O_cap = S.caps.O;
     const MargLayout m = marg_layout(S.marg_lm_cap, S.marg_K_cap, S.marg_L_cap, S.marg_O_cap);
     OKB_CUDA(c, cudaMalloc(&S.marg_scratch, m.total));
@@ -951,7 +991,7 @@ int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int 
   }
   if (bytes > c->marg_dev_bytes) {
     const size_t cap = align_up(std::max(bytes, std::max((size_t)64 << 10, 2 * c->marg_dev_bytes)), 4096);
-    if (c->marg_dev) cudaFree(c->marg_dev);
+    if (c->marg_dev) { if (sharded) c->marg_retired_dev.push_back(c->marg_dev); else cudaFree(c->marg_dev); }
     c->marg_dev = nullptr; c->marg_dev_bytes = 0;
     OKB_CUDA(c, cudaMalloc(&c->marg_dev, cap));
     c->marg_dev_bytes = cap;
@@ -968,9 +1008,36 @@ int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int 
   }
   // pack: the previous call's copy reads the pinned buffer until marg_copied
   if (!c->marg_copied) OKB_CUDA(c, cudaEventCreateWithFlags(&c->marg_copied, cudaEventDisableTiming));
-  if (c->marg_busy) { OKB_CUDA(c, cudaEventSynchronize(c->marg_copied)); c->marg_busy = false; }
+  if (c->marg_busy) {
+    // sharded: that copy may queue behind this rank's previous k_marginalize, still waiting for its peers; pack into a
+    // fresh buffer instead
+    const cudaError_t q = sharded ? cudaEventQuery(c->marg_copied) : cudaSuccess;
+    if (q == cudaErrorNotReady) {
+      cudaGetLastError();
+      // park the buffer with an event after its copy; take a parked buffer whose copy has completed, if any
+      okb_ctx::MargPinned park{c->marg_host, c->marg_host_bytes, nullptr};
+      OKB_CUDA(c, cudaEventCreateWithFlags(&park.done, cudaEventDisableTiming));
+      OKB_CUDA(c, cudaEventRecord(park.done, xs));
+      c->marg_host = nullptr; c->marg_host_bytes = 0;
+      for (size_t i = 0; i < c->marg_pool.size(); ++i) {
+        okb_ctx::MargPinned& e = c->marg_pool[i];
+        if (e.bytes < bytes) continue;
+        const cudaError_t d = cudaEventQuery(e.done);
+        if (d == cudaErrorNotReady) { cudaGetLastError(); continue; }
+        OKB_CUDA(c, d);
+        cudaEventDestroy(e.done);
+        c->marg_host = e.p; c->marg_host_bytes = e.bytes;
+        c->marg_pool.erase(c->marg_pool.begin() + i);
+        break;
+      }
+      c->marg_pool.push_back(park);
+    } else {
+      OKB_CUDA(c, cudaEventSynchronize(c->marg_copied));
+    }
+    c->marg_busy = false;
+  }
   if (bytes > c->marg_host_bytes) {
-    if (c->marg_host) cudaFreeHost(c->marg_host);
+    if (c->marg_host) { if (sharded) c->marg_retired_host.push_back(c->marg_host); else cudaFreeHost(c->marg_host); }
     c->marg_host = nullptr; c->marg_host_bytes = 0;
     const size_t cap = c->marg_dev_bytes;
     OKB_CUDA(c, cudaMallocHost(&c->marg_host, cap));
@@ -994,6 +1061,7 @@ int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int 
     if (job->n_landmarks) std::memcpy(q + p.lms, job->landmarks, 4 * (size_t)job->n_landmarks);
     MargTask task{};
     task.win = slots[t];
+    if (sharded) task.fingerprint = marg_job_fingerprint(job);
     task.sc = marg_pointers(c->marg_dev + off[t], p, S.marg_scratch, marg_layout(S.marg_lm_cap, S.marg_K_cap, S.marg_L_cap, S.marg_O_cap));
     tasks[t] = task;
   }
@@ -1008,7 +1076,8 @@ int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int 
   c->marg_busy = true;
   for (const auto& r : runs)
     OKB_CUDA(c, cudaMemcpyAsync(c->d_wins + r.first, &c->host[r.first], sizeof(WinDev) * r.second, cudaMemcpyHostToDevice, xs));
-  k_marginalize<<<n, M_THREADS, 0, xs>>>(c->d_wins, reinterpret_cast<const MargTask*>(c->marg_dev));
+  if (sharded) k_marginalize<true><<<n, M_THREADS, 0, xs>>>(c->d_wins, reinterpret_cast<const MargTask*>(c->marg_dev));
+  else k_marginalize<false><<<n, M_THREADS, 0, xs>>>(c->d_wins, reinterpret_cast<const MargTask*>(c->marg_dev));
   c->launches += 1;
   OKB_CUDA(c, cudaGetLastError());
   for (int t = 0; t < n; ++t) {
@@ -1032,6 +1101,14 @@ extern "C" int okb_window_marginalize_batch(okb_ctx* c, int win_first, int count
     if (jobs[i]) { slots.push_back(win_first + i); js.push_back(jobs[i]); }
   if (slots.empty()) return OKB_OK;
   return marg_run(c, slots.data(), js.data(), (int)slots.size(), true);
+}
+
+extern "C" int okb_marg_job_fingerprint(const okb_marg_job* job, uint64_t* out) {
+  if (!job || !out || job->n_blocks < 0 || (job->n_blocks && (!job->block_kind || !job->block_idx || !job->block_prev || !job->block_marginalize)) ||
+      job->n_imu_terms < 0 || job->n_sb_priors < 0 || (job->n_imu_terms && !job->imu_terms) || (job->n_sb_priors && !job->sb_priors))
+    return OKB_ERR_INVALID_ARG;
+  *out = marg_job_fingerprint(job);
+  return OKB_OK;
 }
 
 extern "C" int okb_window_download_marg(okb_ctx* c, int win, int32_t* n, int32_t* n_blocks, int32_t* block_kind, uint32_t* block_idx, double* x0,
@@ -1083,7 +1160,8 @@ static int shard_alloc(okb_ctx* c, int rank, int world, int max_frames) {
   cudaSetDevice(c->device);
   const int dcp = 4 * ((6 * max_frames + 1 + 3) / 4);
   c->shard_box_cap = (int)shard_box_doubles(max_frames, dcp);
-  c->shard_win_bytes = shard_win_bytes(world, (size_t)c->shard_box_cap);
+  c->shard_marg_cap = (int)shard_marg_box_doubles(max_frames);
+  c->shard_win_bytes = shard_win_bytes(world, (size_t)c->shard_box_cap, (size_t)c->shard_marg_cap);
   const size_t total = c->shard_win_bytes * (size_t)c->max_windows;
   OKB_CUDA(c, cudaMalloc(&c->shard_local, total));
   OKB_CUDA(c, cudaMemset(c->shard_local, 0, total));

@@ -77,10 +77,22 @@ constexpr size_t kShardHeaderBytes = 4096;
 constexpr size_t kShardFlags1 = 0;       // u64 [2][kMaxShard]   reduced-system boxes ready
 constexpr size_t kShardFlags2 = 128;     // u64 [2][kMaxShard]   step scalars ready
 constexpr size_t kShardCounter = 256;    // u32                  last-CTA counter of k_shard_push (local use)
+constexpr size_t kShardMargEpoch = 384;  // u64                  epoch of the last marginalisation exchange (local use)
 constexpr size_t kShardScalars = 512;    // f64 [2][kMaxShard][16]
+constexpr size_t kShardFlagsM = 2560;    // u64 [2][kMaxShard]   marginalisation boxes ready
+static_assert(kShardScalars + 2 * kMaxShard * 16 * sizeof(double) <= kShardFlagsM &&
+              kShardFlagsM + 2 * kMaxShard * sizeof(unsigned long long) <= kShardHeaderBytes, "shard mailbox header layout");
 __host__ __device__ inline size_t shard_box_doubles(int K, int dcp) { return (size_t)dcp * dcp + (size_t)K * 32 + 8; }
-__host__ __device__ inline size_t shard_win_bytes(int world, size_t box_cap) {
-  return (kShardHeaderBytes + 2 * (size_t)world * box_cap * sizeof(double) + 255) & ~(size_t)255;
+// Marginalisation box (k_marginalize<true>): header [fingerprint, error word, epoch, pad] | pose-pose sums [P][P] | pose
+// rows of b [P], P = 6 * (pose blocks of the job) <= 6 * max_frames.  A region of [2][world] such boxes follows the
+// solver boxes, so a peer's marginalisation push never lands in a box a rank may still be reading for its last round.
+constexpr int kMargBoxHeader = 4;
+__host__ __device__ inline size_t shard_marg_box_doubles(int max_frames) {
+  const size_t p = 6 * (size_t)max_frames;
+  return kMargBoxHeader + p * p + p;
+}
+__host__ __device__ inline size_t shard_win_bytes(int world, size_t box_cap, size_t marg_cap) {
+  return (kShardHeaderBytes + 2 * (size_t)world * (box_cap + marg_cap) * sizeof(double) + 255) & ~(size_t)255;
 }
 
 // Everything kernels need to know about one window.  All pointers are device pointers into the
@@ -182,7 +194,8 @@ struct WinDev {
   // landmark sharding: this rank holds the landmarks / observations of its shard and all dense blocks
   int shard_rank, shard_world;                 // world <= 1: not sharded
   int shard_box_cap;                           // doubles per box
-  unsigned char* shard_mail[kMaxShard];        // this window's mailbox in every rank's memory, as mapped on this device
+  int shard_marg_cap;                          // doubles per marginalisation box (shard_marg_box_doubles)
+  unsigned char* shard_mail[kMaxShard];       // this window's mailbox in every rank's memory, as mapped on this device
   SolverState* st;
 };
 

@@ -41,7 +41,8 @@ enum {
 struct CmdHeader { uint32_t op, n, a, b; uint64_t payload_bytes; };   // payload follows, 8-byte aligned
 static_assert(sizeof(CmdHeader) == 24, "command header layout");
 
-enum { GERR_INDEX = 1, GERR_DUPLICATE = 2, GERR_SLOT_EXT = 3, GERR_CAPACITY = 4, GERR_SQRT_INFO = 5, GERR_DIMS = 6, GERR_MARG_REF = 7 };
+enum { GERR_INDEX = 1, GERR_DUPLICATE = 2, GERR_SLOT_EXT = 3, GERR_CAPACITY = 4, GERR_SQRT_INFO = 5, GERR_DIMS = 6, GERR_MARG_REF = 7,
+       GERR_SHARD_MARG = 8 };
 
 __device__ __forceinline__ void graph_error(GraphState* g, int code) { atomicCAS(&g->err, 0, code); }
 

@@ -674,6 +674,10 @@ __device__ __forceinline__ unsigned long long ld_acquire_sys_u64(const unsigned 
 __device__ __forceinline__ double* shard_box(const WinDev& W, int dst, int parity, int src) {
   return reinterpret_cast<double*>(W.shard_mail[dst] + kShardHeaderBytes) + ((size_t)parity * W.shard_world + src) * W.shard_box_cap;
 }
+__device__ __forceinline__ double* shard_marg_box(const WinDev& W, int dst, int parity, int src) {
+  return reinterpret_cast<double*>(W.shard_mail[dst] + kShardHeaderBytes) + 2 * (size_t)W.shard_world * W.shard_box_cap +
+         ((size_t)parity * W.shard_world + src) * W.shard_marg_cap;
+}
 __device__ __forceinline__ unsigned long long* shard_flag(const WinDev& W, int dst, size_t which, int parity, int src) {
   return reinterpret_cast<unsigned long long*>(W.shard_mail[dst] + which) + parity * kMaxShard + src;
 }

@@ -20,6 +20,12 @@
 //   phase 5  dense blocks to marginalise: V^+ through a parallel cyclic Jacobi eigen-decomposition, Schur complement
 //   phase 6  eigen-decomposition of the preconditioned reduced H -> J, e0, H0 = J^T J
 // All sums run in a fixed order: bit-reproducible.
+// Landmark-sharded windows run k_marginalize<true> on every rank: phases 0-3 see only replicated inputs, phase 4 sees
+// the rank's own landmarks.  Its per-element sums over them (pose x pose entries of H, pose rows of b) are pushed into
+// box [parity][rank] of every rank's mailbox instead of being added; after the flag exchange every rank adds the
+// `world` boxes in rank order and runs phases 5-6 on bit-identical inputs.  A job fingerprint and each rank's error word
+// travel with the boxes: a mismatch, an error on any rank or a peer time-out abandons the step on every rank before
+// phase 5 with one status, and the previous prior stays.
 #pragma once
 #include "okb_estimator.cuh"
 #include "okb_graph.cuh"
@@ -30,7 +36,9 @@ namespace okb {
 constexpr int kMargWork = 256;          // largest linear system (dense coordinates) built before marginalising
 constexpr int M_THREADS = 256;
 constexpr int kMargRec = 72;            // doubles per (landmark, frame) record: W 18 | Z 18 | U 21 | bp 6 | Wy 6 | pad
-enum { MERR_BLOCK = 1, MERR_PREV = 2, MERR_TERM = 3, MERR_POSE_NOT_CONNECTED = 4, MERR_DIM = 5 };
+enum { MERR_BLOCK = 1, MERR_PREV = 2, MERR_TERM = 3, MERR_POSE_NOT_CONNECTED = 4, MERR_DIM = 5,
+       MERR_SHARD_JOB = 6,         // the ranks' jobs differ in their replicated part (fingerprint)
+       MERR_SHARD_TIMEOUT = 7 };   // a peer did not arrive within kShardTimeoutNs
 
 // Job as laid out in the batch buffer of the call (header, then the index lists, 16-byte aligned).
 struct MargJobHeader {
@@ -64,8 +72,11 @@ struct MargScratch {
 };
 
 // One entry of k_marginalize's task table per CTA: the window it marginalises and where its job and scratch lie.
+// fingerprint: landmark-sharded windows only, the host's hash of the job's replicated part (MargJobHeader has no
+// 64-bit spare field).
 struct alignas(16) MargTask {
-  int32_t win, _pad[3];
+  int32_t win, _pad;
+  uint64_t fingerprint;
   MargScratch sc;
 };
 static_assert(sizeof(MargTask) % 16 == 0, "MargTask is copied as 16-byte words");
@@ -164,8 +175,18 @@ __device__ inline int jacobi_eig(double* A, double* Q, int n, double* s_cs /* [2
 
 __device__ __forceinline__ double marg_precond(double hii) { return (hii > 1.0e-9) ? sqrt(hii) : 1.0e-3; }
 
+// Box parity of a landmark-sharded window's next marginalisation exchange (the epoch lives in the rank's own mailbox
+// header, so it survives okb_window_reset and uploads like the solver's shard_epoch).
+__device__ __forceinline__ int marg_shard_parity(const WinDev& W) {
+  return (int)((*reinterpret_cast<const unsigned long long*>(W.shard_mail[W.shard_rank] + kShardMargEpoch) + 1ull) & 1ull);
+}
+
 // One CTA per task: CTA b marginalises window tasks[b].win with the job and scratch of tasks[b].sc.  The task is
-// copied to shared memory once; the phases read its pointers from there.
+// copied to shared memory once; the phases read its pointers from there.  kShard: the window is landmark-sharded (see
+// the top of this file); an error in phases 0-4 is pushed to the peers instead of ending the CTA early, so no peer
+// waits for a rank that has left.
+#pragma nv_diag_suppress 177      // label `exchange` is only jumped to in the sharded instantiation
+template <bool kShard>
 __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restrict__ wins, const MargTask* __restrict__ tasks) {
   __shared__ MargTask s_task;
   if (threadIdx.x < sizeof(MargTask) / 16)
@@ -218,7 +239,10 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
     s_i[0] = err;
   }
   __syncthreads();
-  if (s_i[0]) { if (tid == 0) { sc.status[0] = s_i[0]; graph_error(g, GERR_DIMS); } return; }
+  if (s_i[0]) {
+    if (tid == 0) { sc.status[0] = s_i[0]; graph_error(g, GERR_DIMS); }
+    if constexpr (kShard) goto exchange; else return;
+  }
   for (int b = tid; b < NB; b += M_THREADS) {
     const int kind = sc.kind[b], pv = sc.prev[b];
     const int w = (kind == OKB_BLOCK_SPEED_BIAS) ? 9 : 7;
@@ -244,10 +268,16 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
   // ---------------- phase 2: SpeedAndBiasError terms  r = S (meas - x),  J = -S
   for (int i = 0; i < J.n_sbp; ++i) {
     const uint32_t pi = sc.sb_priors[i];
-    if ((int)pi >= g->n_sbp) { if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); } return; }
+    if ((int)pi >= g->n_sbp) {
+      if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); }
+      if constexpr (kShard) goto exchange; else return;
+    }
     const okb_sb_prior& pr = W.sbp[pi];
     const int blk = ((int)pr.sb_idx < kMaxFrames) ? s_sb_blk[pr.sb_idx] : -1;
-    if (blk < 0) { if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); } return; }
+    if (blk < 0) {
+      if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); }
+      if constexpr (kShard) goto exchange; else return;
+    }
     const int o = s_col[blk];
     const double* x = sc.xlin + 9 * blk;
     if (tid < 81) {
@@ -270,10 +300,16 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
   // ---------------- phase 3: ImuError terms
   for (int i = 0; i < J.n_imu; ++i) {
     const uint32_t t = sc.imu_terms[i];
-    if ((int)t >= g->n_imu) { if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); } return; }
+    if ((int)t >= g->n_imu) {
+      if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); }
+      if constexpr (kShard) goto exchange; else return;
+    }
     const okb_imu_term& T = W.imu_terms[t];
     const int blks[4] = {s_pose_blk[T.pose0], s_sb_blk[T.sb0], s_pose_blk[T.pose1], s_sb_blk[T.sb1]};
-    if (blks[0] < 0 || blks[1] < 0 || blks[2] < 0 || blks[3] < 0) { if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); } return; }
+    if (blks[0] < 0 || blks[1] < 0 || blks[2] < 0 || blks[3] < 0) {
+      if (tid == 0) { sc.status[0] = MERR_TERM; graph_error(g, GERR_INDEX); }
+      if constexpr (kShard) goto exchange; else return;
+    }
     const ImuScratch isc = imu_scratch(s_imu);
     double* SF = isc.SF;
     double* r15 = isc.r15;
@@ -304,10 +340,17 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
     }
     __syncthreads();
   }
-  // ---------------- phase 4: landmarks to marginalise
-  const int n_lm = J.n_lm;
-  if (n_lm > 0) {
+  // ---------------- phase 4: landmarks to marginalise (sharded: the rank's own; a rank with none still pushes zeros)
+  if (const int n_lm = J.n_lm; kShard || n_lm > 0) {
     const int n_obs = g->n_obs;
+    const int mpar = kShard ? marg_shard_parity(W) : 0;
+    if constexpr (kShard) {       // packed pose coordinate of each row of H (s_ia is free until phase 5), count in s_i[3]
+      if (tid == 0) {
+        int p = 0;
+        for (int r = 0; r < N; ++r) s_ia[r] = (short)((sc.kind[s_rowblk[r]] == OKB_BLOCK_POSE) ? p++ : -1);
+        s_i[3] = p;
+      }
+    }
     for (int j = tid; j < n_lm; j += M_THREADS) {
       const uint32_t l = sc.landmarks[j];
       if ((int)l < g->L) sc.lmslot[l] = j + 1;
@@ -406,8 +449,8 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
       }
     }
     __syncthreads();
-    if (sc.status[0]) return;
-    // fixed-order reduction over the landmarks into the pose rows of H and b
+    if constexpr (!kShard) { if (sc.status[0]) return; }
+    // fixed-order reduction over the landmarks into the pose rows of H and b (sharded: into every rank's box)
     for (int i = tid; i < N * N; i += M_THREADS) {
       const int r = i / N, c = i % N;
       const int br = s_rowblk[r], bc = s_rowblk[c];
@@ -425,7 +468,12 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
           s += sc.lmrec[((size_t)j * K + fr) * kMargRec + 36 + hi * (hi + 1) / 2 + lo];
         }
       }
-      sc.H[i] += s;
+      if constexpr (kShard) {
+        const size_t o = kMargBoxHeader + (size_t)s_ia[r] * s_i[3] + s_ia[c];
+        for (int q = 0; q < W.shard_world; ++q) shard_marg_box(W, q, mpar, W.shard_rank)[o] = s;
+      } else {
+        sc.H[i] += s;
+      }
     }
     for (int r = tid; r < N; r += M_THREADS) {
       const int br = s_rowblk[r];
@@ -437,9 +485,73 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
         const double* rec = sc.lmrec + ((size_t)j * K + fr) * kMargRec;
         s += rec[57 + a] - rec[63 + a];
       }
-      sc.b[r] += s;
+      if constexpr (kShard) {
+        const size_t o = kMargBoxHeader + (size_t)s_i[3] * s_i[3] + s_ia[r];
+        for (int q = 0; q < W.shard_world; ++q) shard_marg_box(W, q, mpar, W.shard_rank)[o] = s;
+      } else {
+        sc.b[r] += s;
+      }
     }
     for (int j = tid; j < n_lm; j += M_THREADS) { const uint32_t l = sc.landmarks[j]; if ((int)l < g->L) sc.lmslot[l] = 0; }
+    __syncthreads();
+  }
+exchange:
+  if constexpr (kShard) {
+    // Push the header (job fingerprint, this rank's phase 0-4 error word), release this rank's flag in every mailbox,
+    // acquire the `world` flags in this rank's own; then every rank reads the same boxes.
+    __syncthreads();
+    const int world = W.shard_world, me = W.shard_rank;
+    unsigned long long* ep = reinterpret_cast<unsigned long long*>(W.shard_mail[me] + kShardMargEpoch);
+    const unsigned long long epoch = *ep + 1;
+    const int par = (int)(epoch & 1ull);
+    if (tid == 0) s_i[4] = 0;
+    if (tid < world) {
+      unsigned long long* hb = reinterpret_cast<unsigned long long*>(shard_marg_box(W, tid, par, me));
+      hb[0] = s_task.fingerprint;
+      hb[1] = (unsigned long long)(unsigned)sc.status[0];
+      hb[2] = epoch;
+    }
+    __threadfence_system();
+    __syncthreads();
+    if (tid < world) {
+      st_release_sys_u64(shard_flag(W, tid, kShardFlagsM, par, me), epoch);
+      const unsigned long long t0 = globaltimer_ns();
+      const unsigned long long* fl = shard_flag(W, me, kShardFlagsM, par, tid);
+      while (ld_acquire_sys_u64(fl) < epoch)
+        if (globaltimer_ns() - t0 > kShardTimeoutNs) { s_i[4] = MERR_SHARD_TIMEOUT; break; }
+    }
+    __syncthreads();
+    int st = s_i[4];
+    // a box pushed at another epoch: the ranks are out of step (a rank's earlier call never launched, or timed out)
+    for (int q = 0; q < world && !st; ++q)
+      if (__ldcg(reinterpret_cast<const unsigned long long*>(shard_marg_box(W, me, par, q)) + 2) != epoch) st = MERR_SHARD_TIMEOUT;
+    if (!st) {
+      const unsigned long long fp0 = __ldcg(reinterpret_cast<const unsigned long long*>(shard_marg_box(W, me, par, 0)));
+      for (int q = 0; q < world && !st; ++q)
+        if (__ldcg(reinterpret_cast<const unsigned long long*>(shard_marg_box(W, me, par, q))) != fp0) st = MERR_SHARD_JOB;
+      for (int q = 0; q < world && !st; ++q) st = (int)__ldcg(reinterpret_cast<const unsigned long long*>(shard_marg_box(W, me, par, q)) + 1);
+    }
+    if (st) {       // every rank took the same decision from the same boxes: the previous prior stays everywhere
+      if (tid == 0) { sc.status[0] = st; graph_error(g, GERR_SHARD_MARG); *ep = epoch; }
+      return;
+    }
+    const int P = s_i[3];
+    for (int i = tid; i < N * N; i += M_THREADS) {
+      const int r = i / N, c = i % N;
+      if (s_ia[r] < 0 || s_ia[c] < 0) continue;
+      const size_t o = kMargBoxHeader + (size_t)s_ia[r] * P + s_ia[c];
+      double s = 0.0;
+      for (int q = 0; q < world; ++q) s += __ldcg(shard_marg_box(W, me, par, q) + o);
+      sc.H[i] += s;
+    }
+    for (int r = tid; r < N; r += M_THREADS) {
+      if (s_ia[r] < 0) continue;
+      const size_t o = kMargBoxHeader + (size_t)P * P + s_ia[r];
+      double s = 0.0;
+      for (int q = 0; q < world; ++q) s += __ldcg(shard_marg_box(W, me, par, q) + o);
+      sc.b[r] += s;
+    }
+    if (tid == 0) *ep = epoch;
     __syncthreads();
   }
   // ---------------- phase 5: dense blocks to marginalise
@@ -545,6 +657,7 @@ __global__ void __launch_bounds__(M_THREADS) k_marginalize(const WinDev* __restr
     g->marg_n = n; g->marg_nb = nbk; g->marg_xdim = xo;
   }
 }
+#pragma nv_diag_default 177
 
 // CMD_REMOVE_SB of the graph interpreter lives in okb_graph.cuh; the download of the prior for tests / the host shim:
 __global__ void k_marg_export(const WinDev* __restrict__ wins, int win, double* out /* header 8 | kind nb | idx nb | x0 | J | e0 | H | b0 */, int cap) {

@@ -54,6 +54,70 @@ def shard_window(window, rank, world):
     return w, mine
 
 
+def owned_slots(idx, rank, world):
+    """(positions in `idx` of the global landmark slots rank `rank` holds, their local slots).  The rule shard_window
+    deals by: global slot g lives on rank g % world at local slot g // world.  Slots are chosen by the caller and stable,
+    so the rule holds while the window slides."""
+    idx = np.asarray(idx, np.int64).reshape(-1)
+    pos = np.nonzero(idx % world == rank)[0]
+    return pos, (idx[pos] // world).astype(np.uint32)
+
+
+def global_slots(local, rank, world):
+    """Inverse of owned_slots: the global slots of rank `rank`'s local slots."""
+    return np.asarray(local, np.int64) * world + rank
+
+
+def shard_marg_job(rank, world, block_kind, block_idx, block_prev, block_marginalize, imu_terms=(), sb_priors=(), landmarks=()):
+    """Rank `rank`'s okb_marg_job for a landmark-sharded window: the same dense part on every rank (blocks, IMU terms,
+    speed/bias priors), and of the global `landmarks` only those the rank holds, as local slots.  A rank that holds none
+    gets n_landmarks = 0 and must still call okb_window_marginalize*."""
+    from . import abi
+    _, local = owned_slots(landmarks, rank, world)
+    return abi.make_marg_job(block_kind, block_idx, block_prev, block_marginalize, imu_terms=imu_terms, sb_priors=sb_priors,
+                             landmarks=local)
+
+
+# Resident edits of a sliding landmark-sharded window: landmark edits go to the slot's owner, the dense edits (frames,
+# states, priors, speed/bias removal) to every rank unchanged.  Any other op is refused: its arguments may hold
+# landmark slots that would be read as local ones.
+LANDMARK_EDITS = ("set_landmarks", "remove_landmarks", "add_observations", "remove_observations")
+DENSE_EDITS = ("add_frame", "remove_frame", "set_states", "set_priors", "remove_speed_bias")
+
+
+def route_edit(op, rank, world, *args):
+    """Arguments of Context.<op>(win, *args) for rank `rank`, or None when the rank has nothing to do.  `args` are the
+    unsharded window's (global landmark slots)."""
+    if op in DENSE_EDITS:
+        return args
+    if op == "remove_observations":
+        (keys,) = args
+        k = np.asarray(keys, np.int64).reshape(-1, 3)          # (pose_idx, lm_idx, cam_idx)
+        pos, local = owned_slots(k[:, 1], rank, world)
+        if not len(pos):
+            return None
+        mine = k[pos].copy()
+        mine[:, 1] = local
+        return (mine,)
+    if op == "set_landmarks":
+        idx, xyzw = args
+        pos, local = owned_slots(idx, rank, world)
+        return (local, np.ascontiguousarray(np.asarray(xyzw, np.float64).reshape(-1, 4)[pos])) if len(pos) else None
+    if op == "remove_landmarks":
+        (idx,) = args
+        _, local = owned_slots(idx, rank, world)
+        return (local,) if len(local) else None
+    if op == "add_observations":
+        (obs,) = args
+        pos, local = owned_slots(obs["lm_idx"], rank, world)
+        if not len(pos):
+            return None
+        mine = obs[pos].copy()
+        mine["lm_idx"] = local
+        return (mine,)
+    raise ValueError("route_edit: %r is not a resident edit of a sharded window" % (op,))
+
+
 def merge_shard_results(n_landmarks, parts):
     """parts: list over ranks of (global landmark indices, download dict).  Dense blocks are identical on all ranks."""
     out = dict(poses=parts[0][1]["poses"], speed_bias=parts[0][1]["speed_bias"],
