@@ -28,6 +28,8 @@
  *                                ProbabilisticStereoTriangulator::stereoTriangulate (cpp:168-227), triangulateFast
  *   okb_hamming_candidates    <- VioKeyframeWindowMatchingAlgorithm::specificDescriptorDistance
  *                                okvis_frontend/include/okvis/VioKeyframeWindowMatchingAlgorithm.hpp:246-254
+ *   okb_track_3d2d_batch      <- the 3D-2D rounds of Frontend::matchToKeyframes / matchToLastFrame (Frontend.cpp:389-411,
+ *                                484-494): VioKeyframeWindowMatchingAlgorithm::doSetup + DenseMatcher::match + setBestMatch
  *   okb_detect_describe       <- okvis::Frontend::detectAndDescribe    okvis_frontend/src/Frontend.cpp:92-114
  *                                (Frame::detect / Frame::describe      okvis_cv/include/okvis/implementation/Frame.hpp:109-156)
  */
@@ -594,6 +596,78 @@ int okb_hamming_match_batch(okb_ctx* ctx, int n_jobs, const okb_match_job* jobs,
  * (row_ptr[nA] then holds the required capacity). */
 int okb_hamming_candidates(okb_ctx* ctx, const uint8_t* A, int nA, const uint8_t* B, int nB, int desc_bytes,
                            float threshold, uint32_t* row_ptr, uint32_t* col_idx, uint16_t* dist, int cap);
+
+/* ---- per-window feature store and 3D-2D tracking ------------------------------------------------------------------
+ * The keypoints, descriptors and keypoint -> landmark references of the frames of a resident window, kept on the device
+ * so that tracking a new frame against its window (the 3D-2D matches of Frontend::matchToKeyframes, Frontend.cpp:389-411,
+ * and of Frontend::matchToLastFrame, :484-494) needs no landmark download and no descriptor re-upload.
+ * A window's store holds `max_feature_frames` FEATURE SLOTS -- stable indices the caller picks, like landmark slots, and
+ * independent of window positions (okb_window_remove_frame never moves the store) -- with, per camera, up to
+ * `max_keypoints` keypoints: position and size, descriptor, landmark slot (-1 = none) and an `observed` bit ("the window
+ * holds this keypoint's observation").  It also holds one initialised flag per landmark slot (Estimator::
+ * setLandmarkInitialized); a slot starts uninitialised and okb_window_remove_landmarks clears it, together with every
+ * store reference to the removed slots.  The edit calls below append commands to the slot's pending stream (they
+ * need an uploaded window) and are applied in order with the graph edits at commit; a full upload drops the graph edits
+ * still pending but keeps the pending store edits, which follow it.  Full uploads and okb_window_reset leave the store
+ * as it is.  okb_window_reserve_features allocates the store (a window that never calls it gets none); call it after
+ * okb_window_reserve and before the slot's first upload, which then sizes the window's command buffer for one frame's
+ * features on top of a full upload (OKB_ERR_CAPACITY if the slot was uploaded without); the initialised flags cover
+ * the landmark capacity the slot has then.  Calling it again with other sizes commits what is pending and replaces the
+ * store by an empty one (waiting for the device). */
+int okb_window_reserve_features(okb_ctx* ctx, int win, int max_feature_frames, int max_cameras, int max_keypoints,
+                                int desc_bytes);
+/* Replaces the keypoints of (feat_slot, cam): n keypoints (x, y, size are used), their descriptors [n][desc_bytes],
+ * landmark slots (NULL: all -1) and observed bits (NULL: all 0). */
+int okb_window_set_features(okb_ctx* ctx, int win, int feat_slot, int cam, int n, const okb_keypoint* kp,
+                            const uint8_t* desc, const int32_t* lm_slot, const uint8_t* observed);
+/* Sets the landmark slot and observed bit of keypoints kp_idx[n] of (feat_slot, cam) -- the host-side changes of 2D-2D /
+ * stereo initialisation and RANSAC removals. */
+int okb_window_set_feature_landmarks(okb_ctx* ctx, int win, int feat_slot, int cam, int n, const int32_t* kp_idx,
+                                     const int32_t* lm_slot, const uint8_t* observed);
+/* Empties every camera of a feature slot (its frame left the window). */
+int okb_window_clear_features(okb_ctx* ctx, int win, int feat_slot);
+/* Estimator::setLandmarkInitialized for n landmark slots (flags[i] != 0: initialised). */
+int okb_window_set_landmark_initialized(okb_ctx* ctx, int win, int n, const uint32_t* idx, const uint8_t* flags);
+
+/* One VioKeyframeWindowMatchingAlgorithm 3D-2D match of a tracking job: frame A = feature slot feat_slot_a, camera
+ * cam_a, against the job's frame B in camera cam_b. */
+typedef struct okb_track_round { int32_t feat_slot_a, cam_a, cam_b, _pad; } okb_track_round;
+/* An accepted setBestMatch: keypoint kp_b of (B, cam_b) now refers to landmark slot lm_slot. */
+typedef struct okb_track_assoc { int32_t round, cam_b, kp_b, lm_slot, uncertain, _pad; } okb_track_assoc;
+typedef struct okb_track_job {
+  int32_t win;                  /* window slot */
+  int32_t pose_b;               /* frame B's position in the window (T_WS of doSetup) */
+  int32_t sb_b;                 /* its speed/bias block, -1: frame B is not in the IMU window */
+  int32_t feat_slot_b;          /* its feature slot */
+  float threshold;              /* briskMatchingThreshold_ (60) */
+  int32_t num_best;             /* top-k list length (Frontend's matcher: 4, no ratio test) */
+  int32_t n_rounds, _pad;
+  const okb_track_round* rounds;  /* [n_rounds], run in order */
+  /* outputs; capacities must cover the bounds: assoc_cap >= sum over rounds of B's keypoints in cam_b,
+   * uninit_cap >= sum over rounds of A's keypoints */
+  okb_track_assoc* assoc; int32_t assoc_cap;
+  int32_t* n_assoc;
+  int32_t* num_matches;         /* [n_rounds] numMatches_ */
+  int32_t* num_uncertain;       /* [n_rounds] numUncertainMatches_ */
+  uint32_t* uninit; int32_t uninit_cap;   /* landmark slots doSetup set to uninitialised, in order */
+  int32_t* n_uninit;
+} okb_track_job;
+/* Tracks frame B of each job against its window: per round, in order, VioKeyframeWindowMatchingAlgorithm::doSetup
+ * (okvis_frontend/src/VioKeyframeWindowMatchingAlgorithm.cpp:122-215, 238-255) from the store, the landmark estimates,
+ * pose, extrinsics and camera of the window and the window's observation counts; DenseMatcher::match with verifyMatch's
+ * chi-square gate (:304-339); setBestMatch's 3D-2D branch (:483-526).  Accepted matches are written into B's store
+ * entries (landmark slot, observed) and raise the landmark's count for the later rounds; cleared initialised flags are
+ * applied on the device.  Results come back in the reference's call order (round, then ascending B); the caller applies
+ * them to its own bookkeeping (Estimator::addObservation) -- the call adds no observation to the window.  Results per
+ * job are bit-identical to calling it alone.  Every job is checked on the host before any device work (uploaded
+ * window, store reserved, feature slots present, ranges of cameras, poses, speed/bias, num_best <= 8, output
+ * capacities, one descriptor length per call, a window listed twice, a round of frame B against itself in one
+ * camera): the first failure returns OKB_ERR_INVALID_ARG
+ * and names the job in okb_last_error.  A landmark-sharded context returns OKB_ERR_UNSUPPORTED.  Pending edits of the
+ * job windows are committed first, one commit per run of consecutive windows; the call then runs on the transfer stream after the solver work already launched on
+ * those windows only, with one H2D copy of the job table and one D2H copy of the results, and returns when they are
+ * back.  Later solver calls on those windows are ordered after it.  n_jobs == 0 is a no-op. */
+int okb_track_3d2d_batch(okb_ctx* ctx, int n_jobs, const okb_track_job* jobs);
 
 #ifdef __cplusplus
 }

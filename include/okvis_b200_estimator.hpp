@@ -68,13 +68,21 @@ using PointMap = std::map<uint64_t, MapPoint>;
 using MapPointVector = std::vector<MapPoint>;
 
 // Device-side capacities of an Estimator's resident window (okb_window_reserve).
-struct EstimatorCapacity { int frames = 16, landmarks = 4096, observations = 65536, imu_samples = 8192, marg_dim = 160; };
+// featureKeypoints > 0 also gives the window a feature store (okb_window_reserve_features) for the device-side 3D-2D
+// tracking of Frontend::matchToKeyframes3D2D / matchToLastFrame3D2D: one feature slot per frame, that many keypoints
+// per camera image.
+struct EstimatorCapacity {
+  int frames = 16, landmarks = 4096, observations = 65536, imu_samples = 8192, marg_dim = 160;
+  int featureKeypoints = 0, descriptorBytes = 48;
+};
 
 class EstimatorGroup;
+class Frontend;
 
 class Estimator {
  private:
   friend class EstimatorGroup;
+  friend class Frontend;
   using Clock = std::chrono::steady_clock;
   static double seconds(Clock::time_point t0) { return std::chrono::duration<double>(Clock::now() - t0).count(); }
 
@@ -179,6 +187,7 @@ class Estimator {
     obs_[id] = o;
     it->second.observations[kid] = id;
     if (resident_) { okb_observation d = deviceObs(o); check(okb_window_add_observations(ctx_, slot_, 1, &d)); }
+    setStoreLandmark(poseId, camIdx, keypointIdx, landmarkId, true);
     return id;
   }
   bool removeObservation(uint64_t residualBlockId) {
@@ -188,6 +197,8 @@ class Estimator {
       okb_obs_key k{posePos(it->second.pose), lmSlot_.at(it->second.lm), it->second.cam, 0};
       check(okb_window_remove_observations(ctx_, slot_, 1, &k));
     }
+    // the keypoint keeps its landmark but no longer holds the observation (skipB of doSetup, :238-250)
+    setStoreLandmark(it->second.pose, it->second.cam, it->second.kp, it->second.lm, false);
     eraseObsHost(it);
     return true;
   }
@@ -373,6 +384,7 @@ class Estimator {
       const bool whole = contains(removeFrames, fid);
       if (whole) {
         check(okb_window_remove_frame(ctx_, slot_, posePos(fid), st.hasSb ? sbPos(fid) : 0xffffffffu));
+        releaseFeatures(fid);
         for (auto o = obs_.begin(); o != obs_.end();) {
           if (o->second.pose == fid) {
             auto lm = landmarks_.find(o->second.lm);
@@ -480,7 +492,53 @@ class Estimator {
   }
   bool isLandmarkAdded(uint64_t id) const { return landmarks_.count(id) != 0; }
   bool isLandmarkInitialized(uint64_t id) const { auto it = lmInitialized_.find(id); return it != lmInitialized_.end() && it->second; }
-  void setLandmarkInitialized(uint64_t id, bool initialized) { if (landmarks_.count(id)) lmInitialized_[id] = initialized; }
+  void setLandmarkInitialized(uint64_t id, bool initialized) {
+    if (!landmarks_.count(id)) return;
+    lmInitialized_[id] = initialized;
+    if (resident_ && featReserved_) {
+      const uint32_t s = lmSlot_.at(id);
+      const uint8_t f = initialized ? 1 : 0;
+      check(okb_window_set_landmark_initialized(ctx_, slot_, 1, &s, &f));
+    }
+  }
+
+  // ---- the frame's features for device-side tracking (Capacity::featureKeypoints > 0): keypoints, descriptors
+  // [n][descriptorBytes] and the landmark id of every keypoint (0: none), as the MultiFrame holds them.  The frame takes
+  // a feature slot of the window's store; the slot is freed when the frame leaves the window.
+  void setFrameFeatures(uint64_t frameId, size_t cam, const std::vector<okb_keypoint>& keypoints, const std::vector<uint8_t>& descriptors,
+                        const std::vector<uint64_t>& landmarkIds) {
+    if (cap_.featureKeypoints <= 0) throw std::runtime_error("okvis_b200: setFrameFeatures needs Capacity::featureKeypoints > 0");
+    if (!states_.count(frameId) || cam >= cameras_.size()) throw std::runtime_error("okvis_b200: setFrameFeatures on unknown ids");
+    const size_t n = keypoints.size();
+    if (descriptors.size() != n * (size_t)cap_.descriptorBytes || landmarkIds.size() != n)
+      throw std::invalid_argument("okvis_b200: setFrameFeatures: descriptor / landmark id count mismatch");
+    ensureResident();
+    auto fs = featSlot_.find(frameId);
+    if (fs == featSlot_.end()) {
+      if (freeFeat_.empty()) throw std::runtime_error("okvis_b200: no free feature slot (Capacity::frames)");
+      fs = featSlot_.emplace(frameId, *freeFeat_.begin()).first;
+      freeFeat_.erase(freeFeat_.begin());
+      feats_[frameId].resize(cameras_.size());
+    }
+    std::vector<int32_t> slots(n, -1);
+    std::vector<uint8_t> observed(n, 0);
+    for (size_t k = 0; k < n; ++k) {
+      auto l = landmarks_.find(landmarkIds[k]);
+      if (landmarkIds[k] == 0 || l == landmarks_.end()) continue;
+      slots[k] = (int32_t)lmSlot_.at(landmarkIds[k]);
+      KeypointIdentifier kid; kid.frameId = frameId; kid.cameraIndex = cam; kid.keypointIndex = k;
+      observed[k] = l->second.observations.count(kid) ? 1 : 0;
+    }
+    check(okb_window_set_features(ctx_, slot_, fs->second, (int)cam, (int)n, keypoints.data(), descriptors.data(), slots.data(), observed.data()));
+    FrameFeatures& f = feats_[frameId][cam];
+    f.kp = keypoints; f.lm = landmarkIds;
+  }
+  // The landmark ids of a frame's keypoints as the store holds them (what the MultiFrame's landmarkId() should say).
+  std::vector<uint64_t> frameLandmarkIds(uint64_t frameId, size_t cam) const {
+    auto it = feats_.find(frameId);
+    if (it == feats_.end() || cam >= it->second.size()) return {};
+    return it->second[cam].lm;
+  }
   size_t numFrames() const { return states_.size(); }
   size_t numLandmarks() const { return landmarks_.size(); }
   uint64_t currentFrameId() const { return states_.empty() ? 0 : states_.rbegin()->first; }
@@ -615,6 +673,82 @@ class Estimator {
   static void eraseKey(MapPoint& mp, uint64_t residualId) {
     for (auto o = mp.observations.begin(); o != mp.observations.end();) o = (o->second == residualId) ? mp.observations.erase(o) : std::next(o);
   }
+  // the store's reference of one keypoint (no-op without a store, or when the frame has no features for the camera)
+  void setStoreLandmark(uint64_t frameId, size_t cam, size_t kp, uint64_t landmarkId, bool observed) {
+    if (!resident_ || !featReserved_) return;
+    auto f = feats_.find(frameId);
+    if (f == feats_.end() || cam >= f->second.size() || kp >= f->second[cam].kp.size()) return;
+    auto s = lmSlot_.find(landmarkId);
+    const int32_t k = (int32_t)kp, l = s == lmSlot_.end() ? -1 : (int32_t)s->second;
+    const uint8_t o = observed ? 1 : 0;
+    check(okb_window_set_feature_landmarks(ctx_, slot_, featSlot_.at(frameId), (int)cam, 1, &k, &l, &o));
+    f->second[cam].lm[kp] = landmarkId;
+  }
+  void releaseFeatures(uint64_t frameId) {
+    auto fs = featSlot_.find(frameId);
+    if (fs == featSlot_.end()) return;
+    check(okb_window_clear_features(ctx_, slot_, fs->second));
+    freeFeat_.insert(fs->second);
+    featSlot_.erase(fs);
+    feats_.erase(frameId);
+  }
+  // One okb_track_3d2d_batch job of this session: frame B = currentFrameId against the frames `frameA`, every camera
+  // im -> im that both frames have features for.  finishTrack applies the results through addObservation.
+  struct TrackPlan {
+    uint64_t frameB = 0;
+    std::vector<okb_track_round> rounds;
+    std::vector<okb_track_assoc> assoc;
+    std::vector<uint32_t> uninit;
+    std::vector<int32_t> numMatches, numUncertain;
+    int32_t nAssoc = 0, nUninit = 0;
+    okb_track_job job{};
+  };
+  bool planTrack(uint64_t currentFrameId, const std::vector<uint64_t>& frameA, float threshold, TrackPlan& p) {
+    auto fb = featSlot_.find(currentFrameId);
+    if (fb == featSlot_.end()) return false;
+    size_t sumA = 0, sumB = 0;
+    const auto& B = feats_.at(currentFrameId);
+    for (uint64_t a : frameA) {
+      auto fa = featSlot_.find(a);
+      if (fa == featSlot_.end()) continue;
+      const auto& A = feats_.at(a);
+      for (size_t im = 0; im < cameras_.size(); ++im) {
+        if (A[im].kp.empty() || B[im].kp.empty()) continue;
+        p.rounds.push_back(okb_track_round{fa->second, (int32_t)im, (int32_t)im, 0});
+        sumA += A[im].kp.size(); sumB += B[im].kp.size();
+      }
+    }
+    if (p.rounds.empty()) return false;
+    p.frameB = currentFrameId;
+    p.assoc.resize(std::max<size_t>(sumB, 1)); p.uninit.resize(std::max<size_t>(sumA, 1));
+    p.numMatches.resize(p.rounds.size()); p.numUncertain.resize(p.rounds.size());
+    okb_track_job& j = p.job;
+    j.win = slot_; j.pose_b = (int32_t)posePos(currentFrameId);
+    j.sb_b = states_.at(currentFrameId).hasSb ? (int32_t)sbPos(currentFrameId) : -1;
+    j.feat_slot_b = fb->second; j.threshold = threshold; j.num_best = 4;
+    j.n_rounds = (int32_t)p.rounds.size(); j.rounds = p.rounds.data();
+    j.assoc = p.assoc.data(); j.assoc_cap = (int32_t)p.assoc.size(); j.n_assoc = &p.nAssoc;
+    j.num_matches = p.numMatches.data(); j.num_uncertain = p.numUncertain.data();
+    j.uninit = p.uninit.data(); j.uninit_cap = (int32_t)p.uninit.size(); j.n_uninit = &p.nUninit;
+    return true;
+  }
+  // the host half of setBestMatch / doSetup, in the returned order: setLandmarkInitialized(false), addObservation
+  void finishTrack(const TrackPlan& p, int& numMatches, int& numUncertainMatches) {
+    for (int i = 0; i < p.nUninit; ++i) lmInitialized_[slotOwner_.at(p.uninit[i])] = false;     // the device cleared them
+    for (int i = 0; i < p.nAssoc; ++i) {
+      const okb_track_assoc& a = p.assoc[i];
+      const uint64_t lid = slotOwner_.at((uint32_t)a.lm_slot);
+      FrameFeatures& f = feats_.at(p.frameB)[a.cam_b];
+      const okb_keypoint& kp = f.kp[a.kp_b];
+      f.lm[a.kp_b] = lid;
+      const double z[2] = {kp.x, kp.y};
+      if (!addObservation(lid, p.frameB, a.cam_b, a.kp_b, z, kp.size))
+        setStoreLandmark(p.frameB, a.cam_b, a.kp_b, lid, false);     // refused: the keypoint names it, no observation
+    }
+    for (int32_t m : p.numMatches) numMatches += m;
+    for (int32_t u : p.numUncertain) numUncertainMatches += u;
+  }
+
   void eraseObsHost(std::map<uint64_t, Obs>::iterator it) {
     auto lm = landmarks_.find(it->second.lm);
     if (lm != landmarks_.end()) eraseKey(lm->second, it->first);
@@ -660,8 +794,20 @@ class Estimator {
     d.cameras = cameras_.data(); d.obs = obs.data(); d.imu_terms = terms.data(); d.imu_samples = samples.data(); d.imu_params = imu_;
     d.pose_priors = pps.data(); d.sb_priors = sps.data();
     check(okb_window_reserve(ctx_, slot_, cap_.frames, cap_.landmarks, cap_.observations, cap_.imu_samples, cap_.marg_dim));
+    if (cap_.featureKeypoints > 0)
+      check(okb_window_reserve_features(ctx_, slot_, cap_.frames, (int)cameras_.size(), cap_.featureKeypoints, cap_.descriptorBytes));
     check(okb_window_upload(ctx_, slot_, &d));
     resident_ = true;
+    if (cap_.featureKeypoints > 0) {
+      // a slot of a group may hold a previous session's store: every feature slot empty, every flag as this session has it
+      featReserved_ = true;
+      for (int f = 0; f < cap_.frames; ++f) { check(okb_window_clear_features(ctx_, slot_, f)); freeFeat_.insert(f); }
+      std::vector<uint32_t> idx(cap_.landmarks);
+      std::vector<uint8_t> flags(cap_.landmarks, 0);
+      for (int s = 0; s < cap_.landmarks; ++s) idx[s] = (uint32_t)s;
+      for (auto& kv : lmInitialized_) if (kv.second && lmSlot_.count(kv.first)) flags[lmSlot_.at(kv.first)] = 1;
+      check(okb_window_set_landmark_initialized(ctx_, slot_, cap_.landmarks, idx.data(), flags.data()));
+    }
   }
 
   okb_ctx* ctx_ = nullptr;
@@ -678,6 +824,13 @@ class Estimator {
   std::map<uint64_t, State> states_;
   PointMap landmarks_;
   std::map<uint64_t, bool> lmInitialized_;
+  // feature store: feature slot of each frame that has features, free slots, the host copy of the frames' keypoints
+  // (addObservation needs their positions / sizes) and of their landmark ids
+  struct FrameFeatures { std::vector<okb_keypoint> kp; std::vector<uint64_t> lm; };
+  bool featReserved_ = false;
+  std::map<uint64_t, int32_t> featSlot_;
+  std::set<int32_t> freeFeat_;
+  std::map<uint64_t, std::vector<FrameFeatures>> feats_;
   std::map<uint64_t, Obs> obs_;
   uint64_t nextResidualId_ = 0;
   // device mirrors: landmark slots, IMU term / prior lists in the device's order, blocks of the marginalisation prior
@@ -839,6 +992,7 @@ class EstimatorGroup {
 
  private:
   friend class Estimator;
+  friend class Frontend;
   using Clock = Estimator::Clock;
 
   void check(int rc) const { if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx_)); }

@@ -9,8 +9,12 @@
 // Eigen- and OpenCV-free: images are raw u8 rows, keypoints are okb_keypoint (the cv::KeyPoint fields the reference
 // uses), poses are [t(3), q_xyzw(4)].  INTEGRATION.md shows the adaptor an OKVIS build adds around these.
 //
-// Frontend::dataAssociationAndInitialization (Frontend.cpp:116-272) is NOT provided: it is the caller of the matcher
-// and owns MultiFrame / RANSAC / triangulation glue that stays on the OKVIS side (SURVEY.md 8f rows 2 and 4).
+// Of Frontend::dataAssociationAndInitialization (Frontend.cpp:116-272) the 3D-2D tracking is provided:
+// Frontend::matchToKeyframes3D2D / matchToLastFrame3D2D run the 3D-2D rounds of matchToKeyframes (:389-411) and
+// matchToLastFrame (:484-494) on the device (okb_track_3d2d_batch on the window's feature store, filled by
+// Estimator::setFrameFeatures) and apply them through Estimator::addObservation; the group forms make one call for many
+// sessions of an EstimatorGroup.  2D-2D matching, triangulation, RANSAC and the keyframe decision stay on the OKVIS side
+// with the MultiFrame (SURVEY.md 8f rows 2 and 4).
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -20,6 +24,7 @@
 #include <vector>
 
 #include "okvis_b200.h"
+#include "okvis_b200_estimator.hpp"
 
 namespace okvis_b200 {
 
@@ -103,7 +108,73 @@ class Frontend {
   int descriptorBytes() const { return descriptorBytes_; }
   okb_ctx* context() const { return ctx_; }
 
+  // ---- 3D-2D tracking of the current frame against the window (device: okb_track_3d2d_batch)
+  // landmarkIds[cam][k]: the frame's landmark ids after tracking (write them into the MultiFrame); the counts are the sums
+  // of numMatches_ / numUncertainMatches_ over the rounds.
+  struct TrackResult {
+    std::vector<std::vector<uint64_t>> landmarkIds;
+    int numMatches = 0, numUncertainMatches = 0;
+  };
+  // matchToKeyframes' 3D-2D loop (Frontend.cpp:389-411): keyframes by age from 1, every camera im -> im, at most 3
+  TrackResult matchToKeyframes3D2D(Estimator& estimator, uint64_t currentFrameId) {
+    return trackGroup(nullptr, {&estimator}, {currentFrameId}, true)[0];
+  }
+  // matchToLastFrame's 3D-2D pass (:484-494): nothing when the last frame is a keyframe
+  TrackResult matchToLastFrame3D2D(Estimator& estimator, uint64_t currentFrameId) {
+    return trackGroup(nullptr, {&estimator}, {currentFrameId}, false)[0];
+  }
+  // The same for sessions of one EstimatorGroup (any order, each listed once): one okb_track_3d2d_batch for all of them;
+  // results[i] equals the single call's on sessions[i].
+  std::vector<TrackResult> matchToKeyframes3D2D(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
+                                                const std::vector<uint64_t>& currentFrameIds) {
+    return trackGroup(&group, sessions, currentFrameIds, true);
+  }
+  std::vector<TrackResult> matchToLastFrame3D2D(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
+                                                const std::vector<uint64_t>& currentFrameIds) {
+    return trackGroup(&group, sessions, currentFrameIds, false);
+  }
+
  private:
+  std::vector<TrackResult> trackGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                      bool keyframes) {
+    if (sessions.size() != frameIds.size()) throw std::invalid_argument("okvis_b200: one current frame id per session");
+    if (group) group->validate(sessions);
+    const size_t n = sessions.size();
+    std::vector<Estimator::TrackPlan> plans(n);
+    std::vector<char> has(n, 0);
+    std::vector<okb_track_job> jobs;
+    for (size_t i = 0; i < n; ++i) {
+      Estimator& e = *sessions[i];
+      if (e.numFrames() < 2) continue;                 // just starting (Frontend.cpp:381-384, 470-473)
+      std::vector<uint64_t> frameA;
+      if (keyframes) {
+        for (size_t age = 1, kf = 0; age < e.numFrames() && kf < 3; ++age) {
+          const uint64_t id = e.frameIdByAge(age);
+          if (!e.isKeyframe(id)) continue;
+          frameA.push_back(id);
+          ++kf;
+        }
+      } else {
+        const uint64_t last = e.frameIdByAge(1);
+        if (!e.isKeyframe(last)) frameA.push_back(last);
+      }
+      has[i] = e.planTrack(frameIds[i], frameA, (float)briskMatchingThreshold_, plans[i]);
+    }
+    for (size_t i = 0; i < n; ++i) if (has[i]) jobs.push_back(plans[i].job);
+    if (!jobs.empty()) {
+      okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
+      const int rc = okb_track_3d2d_batch(ctx, (int)jobs.size(), jobs.data());
+      if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+    }
+    std::vector<TrackResult> out(n);
+    for (size_t i = 0; i < n; ++i) {
+      Estimator& e = *sessions[i];
+      if (has[i]) e.finishTrack(plans[i], out[i].numMatches, out[i].numUncertainMatches);
+      for (size_t c = 0; c < e.cameras_.size(); ++c) out[i].landmarkIds.push_back(e.frameLandmarkIds(frameIds[i], c));
+    }
+    return out;
+  }
+
   size_t numCameras_;
   okb_ctx* ctx_;
   bool owns_;

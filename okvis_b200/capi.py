@@ -540,6 +540,68 @@ class Context:
         j._keep = (A, B, sa, sb, gate)
         return j
 
+    # ---- feature store + 3D-2D tracking (okb_window_reserve_features .. okb_track_3d2d_batch)
+    def reserve_features(self, win, max_feature_frames, max_cameras, max_keypoints, desc_bytes=48):
+        self._check(lib().okb_window_reserve_features(self._h, int(win), int(max_feature_frames), int(max_cameras),
+                                                      int(max_keypoints), int(desc_bytes)))
+        self._feat = getattr(self, "_feat", {})
+        self._feat[int(win)] = int(max_keypoints)
+
+    def set_features(self, win, feat_slot, cam, kp, desc, lm_slot=None, observed=None):
+        """okb_window_set_features: kp is a keypoint_dtype array or an [n][3] array of (x, y, size)."""
+        kp = np.asarray(kp)
+        if kp.dtype != abi.keypoint_dtype:
+            k = np.zeros(len(kp), abi.keypoint_dtype)
+            if len(kp):
+                k["x"], k["y"], k["size"] = kp[:, 0], kp[:, 1], kp[:, 2]
+            kp = k
+        kp = np.ascontiguousarray(kp)
+        desc = np.ascontiguousarray(desc, dtype=np.uint8)
+        lm = np.ascontiguousarray(lm_slot, dtype=np.int32) if lm_slot is not None else None
+        ob = np.ascontiguousarray(observed, dtype=np.uint8) if observed is not None else None
+        self._check(lib().okb_window_set_features(self._h, int(win), int(feat_slot), int(cam), len(kp), _p(kp), _p(desc), _p(lm), _p(ob)))
+
+    def set_feature_landmarks(self, win, feat_slot, cam, kp_idx, lm_slot, observed):
+        k = np.ascontiguousarray(kp_idx, dtype=np.int32)
+        lm = np.ascontiguousarray(lm_slot, dtype=np.int32)
+        ob = np.ascontiguousarray(observed, dtype=np.uint8)
+        self._check(lib().okb_window_set_feature_landmarks(self._h, int(win), int(feat_slot), int(cam), len(k), _p(k), _p(lm), _p(ob)))
+
+    def clear_features(self, win, feat_slot):
+        self._check(lib().okb_window_clear_features(self._h, int(win), int(feat_slot)))
+
+    def set_landmark_initialized(self, win, idx, flags):
+        i = np.ascontiguousarray(idx, dtype=np.uint32)
+        f = np.ascontiguousarray(flags, dtype=np.uint8)
+        self._check(lib().okb_window_set_landmark_initialized(self._h, int(win), len(i), _p(i), _p(f)))
+
+    def track_3d2d_batch(self, jobs):
+        """okb_track_3d2d_batch.  jobs: dicts with win, pose_b, sb_b (-1: none), feat_slot_b, rounds [(feat_slot_a, cam_a,
+        cam_b), ...] and optionally threshold (60) and num_best (4).  Returns one dict per job: assoc (track_assoc_dtype,
+        call order), num_matches / num_uncertain per round, uninit (landmark slots cleared, in order)."""
+        arr = (abi.TrackJob * max(len(jobs), 1))()
+        outs = []
+        for i, j in enumerate(jobs):
+            rounds = list(j["rounds"])
+            cap = max(len(rounds) * getattr(self, "_feat", {}).get(int(j["win"]), 0), 1)
+            o = dict(rounds=(abi.TrackRound * max(len(rounds), 1))(), assoc=np.zeros(cap, abi.track_assoc_dtype),
+                     n_assoc=C.c_int32(0), num_matches=np.zeros(max(len(rounds), 1), np.int32),
+                     num_uncertain=np.zeros(max(len(rounds), 1), np.int32), uninit=np.zeros(cap, np.uint32), n_uninit=C.c_int32(0))
+            for r, (fa, ca, cb) in enumerate(rounds):
+                o["rounds"][r].feat_slot_a, o["rounds"][r].cam_a, o["rounds"][r].cam_b = int(fa), int(ca), int(cb)
+            t = arr[i]
+            t.win, t.pose_b, t.sb_b, t.feat_slot_b = int(j["win"]), int(j["pose_b"]), int(j.get("sb_b", -1)), int(j["feat_slot_b"])
+            t.threshold, t.num_best, t.n_rounds = float(j.get("threshold", 60.0)), int(j.get("num_best", 4)), len(rounds)
+            t.rounds = C.cast(o["rounds"], C.POINTER(abi.TrackRound))
+            t.assoc, t.assoc_cap, t.n_assoc = o["assoc"].ctypes.data, cap, C.pointer(o["n_assoc"])
+            t.num_matches = o["num_matches"].ctypes.data_as(C.POINTER(C.c_int32))
+            t.num_uncertain = o["num_uncertain"].ctypes.data_as(C.POINTER(C.c_int32))
+            t.uninit, t.uninit_cap, t.n_uninit = o["uninit"].ctypes.data_as(C.POINTER(C.c_uint32)), cap, C.pointer(o["n_uninit"])
+            outs.append((o, len(rounds)))
+        self._check(lib().okb_track_3d2d_batch(self._h, len(jobs), arr))
+        return [dict(assoc=o["assoc"][:o["n_assoc"].value].copy(), num_matches=o["num_matches"][:n].copy(),
+                     num_uncertain=o["num_uncertain"][:n].copy(), uninit=o["uninit"][:o["n_uninit"].value].copy()) for o, n in outs]
+
     def hamming_match_batch(self, jobs, desc_bytes):
         """okb_hamming_match_batch over `jobs`: make_match_job results, or dicts of its keyword arguments.  Returns one
         dict(topk, pairs) per job, like hamming_match / hamming_match_gated."""

@@ -41,7 +41,17 @@ struct WinStore {
   unsigned char* marg_scratch = nullptr;   // device scratch of okb_window_marginalize (okb_marg.cuh), allocated on first use
   size_t marg_scratch_bytes = 0;
   int marg_lm_cap = 0, marg_K_cap = 0, marg_L_cap = 0, marg_O_cap = 0;
+  // feature store (okb_window_reserve_features): one device allocation headed by the FeatStore struct, a host copy of
+  // that struct, and the keypoint count per (feature slot, camera) as committed / including pending commands (-1: none)
+  unsigned char* feat_mem = nullptr;
+  okb::FeatStore feat{};
+  std::vector<int> feat_n, feat_n_pending;
+  size_t feat_frame_bytes = 0;        // commands of one frame's features + every initialised flag: the device command
+                                      // buffer (plan_arena) holds them on top of a full upload
 };
+
+// Commits the pending commands of slots [first, first+count) on the transfer stream (okb_estimator.cu).
+int okb_commit_range(okb_ctx* c, int first, int count);
 
 // Buffers of okb_imu_propagate*: [job table | samples] in, [per-job outputs] out, in one pinned buffer and its device
 // mirror; they grow with the largest call and are kept.

@@ -134,6 +134,7 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
   for (auto& w : c->wins) {
     if (w.arena) cudaFree(w.arena);
     if (w.marg_scratch) cudaFree(w.marg_scratch);
+    if (w.feat_mem) cudaFree(w.feat_mem);
     if (w.staging) cudaFreeHost(w.staging);
     if (w.out_staging) cudaFreeHost(w.out_staging);
     if (w.copied) cudaEventDestroy(w.copied);
@@ -268,7 +269,7 @@ int plan_arena(okb_ctx* c, int win, const WinCaps& q) {
   const size_t o_bitmap = P.take(4 * (((size_t)NSc * Lc + 31) / 32 + 1));
   const size_t o_perm = P.take(4 * (size_t)Lpc), o_inv = P.take(4 * (size_t)Lpc), o_trange = P.take(4 * (size_t)(Lpc / 32 + 1)), o_vis = P.take(4 * (size_t)Lpc);
   const size_t o_slots = P.take(sizeof(SlotInfo) * NSPc);
-  const size_t cmd_cap = align_up(full_upload_bytes(q) + 65536, 256);
+  const size_t cmd_cap = align_up(full_upload_bytes(q) + S.feat_frame_bytes + 65536, 256);
   const size_t o_cmd = P.take(cmd_cap);
   // working state / scratch
   const size_t o_lm = P.take(8 * 4 * (size_t)Lpc), o_pose_i = P.take(8 * 7 * Kc), o_sb_i = P.take(8 * 9 * Kc);
@@ -337,6 +338,7 @@ int plan_arena(okb_ctx* c, int win, const WinCaps& q) {
   W.zero_ptr[0] = A + o_obsz; W.zero_ptr[1] = A + o_obsw; W.zero_ptr[2] = A + o_M;
   W.imu_cache = reinterpret_cast<ImuCache*>(A + o_cache); W.imu_out = dp(o_imu_out);
   W.st = c->d_states + win;
+  W.feat = S.feat_mem ? reinterpret_cast<FeatStore*>(S.feat_mem) : nullptr;
   W.n_chunks = 1; W.use_cauchy = 1;
   c->host[win] = W;
   return OKB_OK;
@@ -418,6 +420,7 @@ static int commit_range(okb_ctx* c, int first, int count) {
     W.cmd_bytes = (int)S.cmd_used; W.dirty = 1; W.full = S.full_pending ? 1 : 0;
     W.n_obs = S.obs_bound;
     S.cmd_used = 0; S.full_pending = false; S.committed = true;
+    S.feat_n = S.feat_n_pending;
     max_work = std::max(max_work, std::max(std::max(W.n_obs, 4 * W.L), std::max(7 * W.K, 9 * W.NSB)));
   }
   if (!any) return OKB_OK;
@@ -433,6 +436,8 @@ static int commit_range(okb_ctx* c, int first, int count) {
   for (int i = first; i < first + count; ++i) { c->host[i].cmd_bytes = 0; c->host[i].dirty = 0; c->host[i].full = 0; }
   return OKB_OK;
 }
+
+int okb_commit_range(okb_ctx* c, int first, int count) { return commit_range(c, first, count); }
 
 extern "C" int okb_window_commit(okb_ctx* c, int first, int count) {
   if (!c || first < 0 || count < 1 || first + count > c->max_windows) return OKB_ERR_INVALID_ARG;
@@ -509,8 +514,17 @@ static int upload_pack(okb_ctx* c, int win, const okb_window_desc* D) {
     int rc = plan_arena(c, win, S.arena ? caps_max(S.caps, need) : need);
     if (rc) return rc;
   }
-  S.cmd_used = 0;            // a full upload supersedes anything still pending
-  int rc = cmd_reserve(c, S, full_upload_bytes(need));
+  // a full upload supersedes the graph edits still pending; feature-store edits are kept and follow it
+  std::vector<unsigned char> store_cmds;
+  for (size_t o = 0; S.feat_mem && o < S.cmd_used;) {
+    CmdHeader h;
+    std::memcpy(&h, S.staging + o, sizeof h);
+    const size_t len = sizeof h + h.payload_bytes;
+    if (h.op >= CMD_SET_FEATURES && h.op <= CMD_SET_LM_INIT) store_cmds.insert(store_cmds.end(), S.staging + o, S.staging + o + len);
+    o += len;
+  }
+  S.cmd_used = 0;
+  int rc = cmd_reserve(c, S, full_upload_bytes(need) + store_cmds.size());
   if (rc) return rc;
   unsigned char* q;
   q = cmd_put(S, CMD_RESET_GRAPH, 0, (uint32_t)NE, (uint32_t)NC, 8 * 7 * (size_t)NE + sizeof(okb_camera) * NC);
@@ -544,6 +558,7 @@ static int upload_pack(okb_ctx* c, int win, const okb_window_desc* D) {
     std::memcpy(x + marg_xdim, D->marg->J, 8 * (size_t)marg_n * marg_n);
     std::memcpy(x + marg_xdim + (size_t)marg_n * marg_n, D->marg->e0, 8 * (size_t)marg_n);
   }
+  if (!store_cmds.empty()) { std::memcpy(S.staging + S.cmd_used, store_cmds.data(), store_cmds.size()); S.cmd_used += store_cmds.size(); }
   // host mirror of the dimensions
   WinDev& W = c->host[win];
   W.K = K; W.NSB = NSB; W.NE = NE; W.L = L; W.NC = NC;
@@ -833,6 +848,144 @@ extern "C" int okb_window_remove_speed_bias(okb_ctx* c, int win, uint32_t sb_idx
   W->n_sbp = (int)o;
   W->NSB -= 1;
   derive_dims(*W);
+  return OKB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// feature store of okb_track_3d2d_batch (FeatStore, okb_estimator.cuh); edits are graph commands like the others
+// ---------------------------------------------------------------------------------------------
+extern "C" int okb_window_reserve_features(okb_ctx* c, int win, int max_feature_frames, int max_cameras, int max_keypoints, int desc_bytes) {
+  if (!c || win < 0 || win >= c->max_windows || max_feature_frames < 1 || max_cameras < 1 || max_keypoints < 1) return OKB_ERR_INVALID_ARG;
+  if (desc_bytes != 32 && desc_bytes != 48 && desc_bytes != 64 && desc_bytes != 128) {
+    c->set_error("okb_window_reserve_features: descriptor length must be 32, 48, 64 or 128 bytes");
+    return OKB_ERR_INVALID_ARG;
+  }
+  if (max_keypoints > 65535 || max_cameras > 127) {     // the result records of okb_track_3d2d_batch pack them
+    c->set_error("okb_window_reserve_features: at most 65535 keypoints per image and 127 cameras");
+    return OKB_ERR_CAPACITY;
+  }
+  WinStore& S = c->wins[win];
+  const int lm_cap = std::max(S.reserve.L, S.caps.L);
+  if (lm_cap < 1) { c->set_error("okb_window_reserve_features: reserve or upload the window first"); return OKB_ERR_INVALID_ARG; }
+  cudaSetDevice(c->device);
+  const FeatStore& o = S.feat;
+  if (S.feat_mem && o.F == max_feature_frames && o.C == max_cameras && o.N == max_keypoints && o.D == desc_bytes && o.lm_cap == lm_cap)
+    return OKB_OK;
+  const size_t pad8 = 7;
+  const size_t frame_bytes = (size_t)max_cameras * (sizeof(CmdHeader) + 24 * (size_t)max_keypoints + (4 * (size_t)max_keypoints + pad8) +
+                                                    ((size_t)max_keypoints + pad8) + ((size_t)max_keypoints * desc_bytes + pad8)) +
+                             sizeof(CmdHeader) + 5 * (size_t)lm_cap + 2 * pad8;
+  if (S.arena && S.cmd_cap_dev < align_up(full_upload_bytes(S.caps) + frame_bytes + 65536, 256)) {
+    c->set_error("okb_window_reserve_features: the window's command buffer was planned without a feature store: reserve the "
+                 "features before the slot's first upload");
+    return OKB_ERR_CAPACITY;
+  }
+  if (S.feat_mem) {                     // replaced: commands already queued for the old store must not reach the new one
+    if (S.cmd_used) { const int rc = commit_range(c, win, 1); if (rc) return rc; }
+    OKB_CUDA(c, cudaStreamSynchronize(c->stream_xfer));
+    if (S.done_idx >= 0) OKB_CUDA(c, cudaEventSynchronize(c->done_ring[S.done_idx]));
+    OKB_CUDA(c, cudaFree(S.feat_mem));
+    S.feat_mem = nullptr;
+  }
+  const size_t images = (size_t)max_feature_frames * max_cameras, kps = images * max_keypoints;
+  ArenaPlan P;
+  P.take(sizeof(FeatStore));
+  const size_t o_n = P.take(4 * images), o_kp = P.take(16 * kps), o_size = P.take(8 * kps), o_desc = P.take(kps * desc_bytes);
+  const size_t o_lm = P.take(4 * kps), o_obs = P.take(kps), o_init = P.take((size_t)lm_cap);
+  unsigned char* m = nullptr;
+  OKB_CUDA(c, cudaMalloc(&m, P.total));
+  FeatStore F{};
+  F.F = max_feature_frames; F.C = max_cameras; F.N = max_keypoints; F.D = desc_bytes; F.lm_cap = lm_cap;
+  F.n = reinterpret_cast<int*>(m + o_n); F.kp = reinterpret_cast<double*>(m + o_kp); F.size = reinterpret_cast<double*>(m + o_size);
+  F.desc = reinterpret_cast<uint32_t*>(m + o_desc); F.lm = reinterpret_cast<int32_t*>(m + o_lm); F.observed = m + o_obs; F.lm_init = m + o_init;
+  cudaStream_t xs = c->stream_xfer;
+  OKB_CUDA(c, cudaMemsetAsync(m + o_n, 0xff, 4 * images, xs));                 // n = -1: no image
+  OKB_CUDA(c, cudaMemsetAsync(m + o_lm, 0xff, 4 * kps, xs));                   // lm = -1
+  OKB_CUDA(c, cudaMemsetAsync(m + o_obs, 0, o_init + lm_cap - o_obs, xs));      // observed bits, initialised flags
+  S.feat = F;
+  S.feat_mem = m;
+  S.feat_frame_bytes = frame_bytes;
+  OKB_CUDA(c, cudaMemcpyAsync(m, &S.feat, sizeof(FeatStore), cudaMemcpyHostToDevice, xs));
+  S.feat_n.assign(images, -1);
+  S.feat_n_pending.assign(images, -1);
+  FeatStore* dp = reinterpret_cast<FeatStore*>(m);
+  c->host[win].feat = dp;
+  OKB_CUDA(c, cudaMemcpyAsync(&c->d_wins[win].feat, &c->host[win].feat, sizeof(dp), cudaMemcpyHostToDevice, xs));
+  OKB_CUDA(c, cudaStreamSynchronize(xs));
+  return OKB_OK;
+}
+
+static int feat_begin(okb_ctx* c, int win, int feat_slot, int cam, size_t extra, WinStore** S, WinDev** W, const char* who) {
+  int rc = delta_begin(c, win, extra, S, W);
+  if (rc) return rc;
+  const FeatStore& F = (*S)->feat;
+  if (!(*S)->feat_mem) { c->set_error(std::string(who) + ": no feature store (okb_window_reserve_features)"); return OKB_ERR_INVALID_ARG; }
+  if (feat_slot < 0 || feat_slot >= F.F || cam < 0 || cam >= F.C) { c->set_error(std::string(who) + ": feature slot or camera out of range"); return OKB_ERR_INVALID_ARG; }
+  return OKB_OK;
+}
+
+extern "C" int okb_window_set_features(okb_ctx* c, int win, int feat_slot, int cam, int n, const okb_keypoint* kp, const uint8_t* desc,
+                                       const int32_t* lm_slot, const uint8_t* observed) {
+  if (!c || n < 0 || (n > 0 && (!kp || !desc))) return OKB_ERR_INVALID_ARG;
+  const int D = (win >= 0 && win < c->max_windows) ? c->wins[win].feat.D : 0;
+  const size_t bk = 24 * (size_t)n, bl = align_up(4 * (size_t)n, 8), bo = align_up((size_t)n, 8), bd = align_up((size_t)n * D, 8);
+  WinStore* S; WinDev* W;
+  int rc = feat_begin(c, win, feat_slot, cam, bk + bl + bo + bd, &S, &W, "okb_window_set_features");
+  if (rc) return rc;
+  if (n > S->feat.N) { c->set_error("okb_window_set_features: more keypoints than reserved"); return OKB_ERR_CAPACITY; }
+  for (int i = 0; lm_slot && i < n; ++i)
+    if (lm_slot[i] < -1) { c->set_error("okb_window_set_features: landmark slot below -1"); return OKB_ERR_INVALID_ARG; }
+  unsigned char* q = cmd_put(*S, CMD_SET_FEATURES, (uint32_t)n, (uint32_t)feat_slot, (uint32_t)cam, bk + bl + bo + bd);
+  double* x = reinterpret_cast<double*>(q);
+  for (int i = 0; i < n; ++i) { x[3 * i] = kp[i].x; x[3 * i + 1] = kp[i].y; x[3 * i + 2] = kp[i].size; }
+  int32_t* l = reinterpret_cast<int32_t*>(q + bk);
+  for (int i = 0; i < n; ++i) l[i] = lm_slot ? lm_slot[i] : -1;
+  if (observed) std::memcpy(q + bk + bl, observed, n); else std::memset(q + bk + bl, 0, n);
+  if (n) std::memcpy(q + bk + bl + bo, desc, (size_t)n * D);
+  S->feat_n_pending[(size_t)feat_slot * S->feat.C + cam] = n;
+  return OKB_OK;
+}
+
+extern "C" int okb_window_set_feature_landmarks(okb_ctx* c, int win, int feat_slot, int cam, int n, const int32_t* kp_idx,
+                                                const int32_t* lm_slot, const uint8_t* observed) {
+  if (!c || n < 1 || !kp_idx || !lm_slot || !observed) return OKB_ERR_INVALID_ARG;
+  const size_t b4 = align_up(4 * (size_t)n, 8), b1 = align_up((size_t)n, 8);
+  WinStore* S; WinDev* W;
+  int rc = feat_begin(c, win, feat_slot, cam, 2 * b4 + b1, &S, &W, "okb_window_set_feature_landmarks");
+  if (rc) return rc;
+  const int nk = S->feat_n_pending[(size_t)feat_slot * S->feat.C + cam];
+  for (int i = 0; i < n; ++i)
+    if (kp_idx[i] < 0 || kp_idx[i] >= nk || lm_slot[i] < -1) {
+      c->set_error("okb_window_set_feature_landmarks: keypoint index or landmark slot out of range");
+      return OKB_ERR_INVALID_ARG;
+    }
+  unsigned char* q = cmd_put(*S, CMD_SET_FEATURE_LMS, (uint32_t)n, (uint32_t)feat_slot, (uint32_t)cam, 2 * b4 + b1);
+  std::memcpy(q, kp_idx, 4 * (size_t)n);
+  std::memcpy(q + b4, lm_slot, 4 * (size_t)n);
+  std::memcpy(q + 2 * b4, observed, n);
+  return OKB_OK;
+}
+
+extern "C" int okb_window_clear_features(okb_ctx* c, int win, int feat_slot) {
+  WinStore* S; WinDev* W;
+  int rc = feat_begin(c, win, feat_slot, 0, 0, &S, &W, "okb_window_clear_features");
+  if (rc) return rc;
+  cmd_put(*S, CMD_CLEAR_FEATURES, 0, (uint32_t)feat_slot, 0, 0);
+  for (int k = 0; k < S->feat.C; ++k) S->feat_n_pending[(size_t)feat_slot * S->feat.C + k] = -1;
+  return OKB_OK;
+}
+
+extern "C" int okb_window_set_landmark_initialized(okb_ctx* c, int win, int n, const uint32_t* idx, const uint8_t* flags) {
+  if (!c || n < 1 || !idx || !flags) return OKB_ERR_INVALID_ARG;
+  const size_t b4 = align_up(4 * (size_t)n, 8), b1 = align_up((size_t)n, 8);
+  WinStore* S; WinDev* W;
+  int rc = feat_begin(c, win, 0, 0, b4 + b1, &S, &W, "okb_window_set_landmark_initialized");
+  if (rc) return rc;
+  for (int i = 0; i < n; ++i)
+    if ((int64_t)idx[i] >= S->feat.lm_cap) { c->set_error("okb_window_set_landmark_initialized: slot beyond the store's landmark capacity"); return OKB_ERR_CAPACITY; }
+  unsigned char* q = cmd_put(*S, CMD_SET_LM_INIT, (uint32_t)n, 0, 0, b4 + b1);
+  std::memcpy(q, idx, 4 * (size_t)n);
+  std::memcpy(q + b4, flags, n);
   return OKB_OK;
 }
 

@@ -107,6 +107,23 @@ __host__ __device__ inline size_t out_lm_offset(int K, int NSB) { return ((size_
 
 struct SlotCtx;   // per (frame, camera) transform + intrinsics at the candidate state (okb_kernels_lm.cuh)
 
+// Per-window feature store of okb_track_3d2d_batch (one device allocation per window that reserved it; the struct heads
+// it).  Image (f, c) = feature slot f, camera c; keypoint k of it is entry (f * C + c) * N + k.  Edited by the graph
+// commands CMD_SET_FEATURES .. CMD_SET_LM_INIT (okb_graph.cuh), read and written by the tracking kernels
+// (okb_frontend.cu).  Keypoints are kept in double, as Frame::getKeypoint / getKeypointSize hand them to the matcher.
+struct FeatStore {
+  int F, C, N, D;               // feature slots, cameras, keypoints per image, descriptor bytes
+  int lm_cap;                   // landmark slots covered by lm_init
+  int _pad;
+  int* n;                       // [F][C] keypoints of the image, -1: none
+  double* kp;                   // [F][C][N][2]
+  double* size;                 // [F][C][N]
+  uint32_t* desc;               // [F][C][N][D/4]
+  int32_t* lm;                  // [F][C][N] landmark slot, -1: none
+  uint8_t* observed;            // [F][C][N]
+  uint8_t* lm_init;             // [lm_cap] Estimator::isLandmarkInitialized
+};
+
 struct WinDev {
   // capacities the arena was planned for (okb_window_reserve / the largest upload); the current dimensions below
   // change with the graph commands
@@ -197,6 +214,7 @@ struct WinDev {
   int shard_marg_cap;                          // doubles per marginalisation box (shard_marg_box_doubles)
   unsigned char* shard_mail[kMaxShard];       // this window's mailbox in every rank's memory, as mapped on this device
   SolverState* st;
+  FeatStore* feat;                             // feature store (okb_window_reserve_features), nullptr: none
 };
 
 }  // namespace okb

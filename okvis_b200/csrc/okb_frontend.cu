@@ -168,6 +168,11 @@ struct okb_frontend_state {
   MatchIO match_io;                // okb_hamming_match / _gated (on c->stream, under match_mtx)
   std::atomic<int64_t> launches{0};   // frontend kernel launches (okb_kernel_launches adds them to the solver's)
   std::mutex match_mtx;
+  // okb_track_3d2d_batch (on c->stream_xfer, under track_mtx): job tables in / results out, and device scratch
+  MatchIO track_io;
+  uint8_t* track_scratch = nullptr;
+  size_t track_scratch_cap = 0;
+  std::mutex track_mtx;
 };
 
 void okb_frontend_release(okb_ctx* c) {
@@ -175,6 +180,8 @@ void okb_frontend_release(okb_ctx* c) {
   okb_frontend_state* F = c->frontend;
   F->match_io.release();
   F->batch_match.release();
+  F->track_io.release();
+  cudaFree(F->track_scratch);
   F->batch_det.release();
   if (F->batch_stream) cudaStreamDestroy(F->batch_stream);
   for (auto& s : F->slots) {
@@ -1598,5 +1605,417 @@ extern "C" int okb_hamming_candidates(okb_ctx* c, const uint8_t* A, int nA, cons
   if (ncopy && dist) FE_CUDA(c, cudaMemcpyAsync(dist, F->d_dist, sizeof(uint16_t) * ncopy, cudaMemcpyDeviceToHost, c->stream));
   FE_CUDA(c, cudaStreamSynchronize(c->stream));
   if (total > (uint32_t)cap) { c->set_error("candidate capacity too small"); return OKB_ERR_CAPACITY; }
+  return OKB_OK;
+}
+
+// =================================================================================================
+// 3D-2D tracking against resident windows (okb_track_3d2d_batch): the 3D-2D rounds of Frontend::matchToKeyframes
+// (okvis_frontend/src/Frontend.cpp:389-411) and matchToLastFrame (:484-494) on the window's feature store.  Per round,
+// for all jobs of the call at once:
+//   k_track_setup   VioKeyframeWindowMatchingAlgorithm::doSetup (VioKeyframeWindowMatchingAlgorithm.cpp:122-215, 238-255)
+//   k_hamming_topk<NW, true> + k_assign   DenseMatcher::match over verifyMatch's gate (the matcher kernels above, unchanged)
+//   k_track_apply   setBestMatch, 3D-2D branch (:483-526)
+// The setup of round r+1 reads what the apply of round r wrote -- B's landmark references and observed bits, the raised
+// observation counts, the cleared initialised flags, and, in a same-frame stereo round, A's own entries -- so the rounds
+// are launched in sequence on one stream with no host synchronisation between them.  Setup and apply run one CTA per
+// job: a round's work per A keypoint is one projection, and the flag clearing and the result list need the
+// reference's order within the job.
+// =================================================================================================
+namespace {
+// One job of a launch (device table, in the order of decreasing round count, so that the jobs of round r are a prefix).
+struct TrackJobDev {
+  const WinDev* W;
+  int pose_b, sb_b, feat_b, n_rounds;
+  float threshold;
+  int cnt_cap;
+  int* cnt;                 // [cnt_cap] observations per landmark slot, raised by every accepted match
+  int* hdr;                 // [2 n_rounds + 2] numMatches / numUncertainMatches per round, associations, cleared flags
+  uint2* assoc;             // {kp_b | round << 16 | cam_b << 24 | uncertain << 31, landmark slot}
+  uint32_t* uninit;
+};
+struct TrackRoundDev { int feat_a, cam_a, cam_b, _pad; };
+
+__device__ __forceinline__ bool track_live(const WinDev& W, int L, int l) {
+  // a landmark slot is in the graph iff it is below L and its estimate is not the all-zero vector the graph leaves in
+  // removed and unused slots (Estimator::isLandmarkAdded)
+  if (l < 0 || l >= L) return false;
+  const double4 x = *reinterpret_cast<const double4*>(W.m_lm + 4 * (size_t)l);
+  return x.x != 0.0 || x.y != 0.0 || x.z != 0.0 || x.w != 0.0;
+}
+
+constexpr int TK_T = 256;     // threads of the setup / apply CTAs (the projection chain needs more than 64 registers)
+
+// exclusive scan of one int per thread over a TK_T-thread CTA; *total = sum (all threads)
+__device__ __forceinline__ int track_scan(int v, int* s_warp, int* total) {
+  constexpr int NWT = TK_T / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+  __syncthreads();
+  if (lane == 31) s_warp[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    int w = lane < NWT ? s_warp[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < NWT; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
+    if (lane < NWT) s_warp[lane] = w;
+  }
+  __syncthreads();
+  *total = s_warp[NWT - 1];
+  return (warp ? s_warp[warp - 1] : 0) + x - v;
+}
+
+__global__ void __launch_bounds__(TK_T, 1) k_track_setup(const TrackJobDev* __restrict__ jobs, const MatchJobDev* __restrict__ tab,
+                                                      const TrackRoundDev* __restrict__ rinfo, int round) {
+  __shared__ int s_warp[TK_T / 32];
+  __shared__ int s_cand[TK_T];
+  const TrackJobDev& J = jobs[blockIdx.x];
+  const MatchJobDev& M = tab[blockIdx.x];
+  const TrackRoundDev R = rinfo[blockIdx.x];
+  const WinDev& W = *J.W;
+  const FeatStore& F = *W.feat;
+  const int tid = threadIdx.x;
+  const int L = min(W.st->g.L, J.cnt_cap);
+  if (round == 0) {
+    // observation counts of the window (landmark.observations.size()); later rounds see them raised by the matches
+    for (int i = tid; i < J.cnt_cap; i += TK_T) J.cnt[i] = 0;
+    for (int i = tid; i < 2 * J.n_rounds + 2; i += TK_T) J.hdr[i] = 0;
+    __syncthreads();
+    const int n_obs = W.st->g.n_obs;
+    for (int i = tid; i < n_obs; i += TK_T) {
+      const okb_observation& ob = W.m_obs[i];
+      if (ob.sqrt_info != 0.0 && (int)ob.lm_idx < L) atomicAdd(&J.cnt[ob.lm_idx], 1);
+    }
+    __syncthreads();
+  }
+  // skipB (:238-250): B keypoint k refers to a landmark of the graph that already holds this keypoint's observation
+  const size_t base_b = ((size_t)J.feat_b * F.C + R.cam_b) * F.N;
+  uint8_t* skipB = const_cast<uint8_t*>(M.skipB);
+  for (int b = tid; b < M.nB; b += TK_T) skipB[b] = (F.observed[base_b + b] && track_live(W, L, F.lm[base_b + b])) ? 1 : 0;
+  // UOplus (:127-142): velocity-scaled position variance when B is in the IMU window and A is another frame, else 4e-8
+  // (also the same-frame stereo 3D-2D match of matchStereo, Frontend.cpp:547-553)
+  double s = 4e-8;
+  if (J.sb_b >= 0 && R.feat_a != J.feat_b) {
+    const double* v = W.sb + 9 * (size_t)J.sb_b;
+    const double scale = fmax(1.0, sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]));
+    s = (scale * scale) * 1.0e-2;
+  }
+  SlotXf xf;       // T_CbW = (T_WSb T_SbCb)^-1
+  make_slot_xf(W.pose + 7 * (size_t)J.pose_b, W.ext + 7 * (size_t)R.cam_b, xf);
+  const okb_camera& camB = W.cams[R.cam_b];
+  CamIntr cam;
+  cam_load(camB, cam);
+  const size_t base_a = ((size_t)R.feat_a * F.C + R.cam_a) * F.N;
+  uint8_t* skipA = const_cast<uint8_t*>(M.skipA);
+  double* proj = const_cast<double*>(M.gate.proj_into_b);
+  double* unc = const_cast<double*>(M.gate.proj_unc);
+  for (int k0 = 0; k0 < M.nA; k0 += TK_T) {
+    const int k = k0 + tid;
+    int clear = 0;
+    if (k < M.nA) {
+      // doSetup for A keypoint k, in the reference's order (:165-215)
+      const int l = F.lm[base_a + k];
+      bool skip = true;
+      if (!track_live(W, L, l)) {                                       // 1. no landmark, or not in the graph
+      } else if (!(l < F.lm_cap && F.lm_init[l])) {                      // 2. not initialised
+      } else {
+        const double* X = W.m_lm + 4 * (size_t)l;
+        const double w = X[3];
+        double pc[3];
+        pc[0] = xf.R[0] * X[0] + xf.R[1] * X[1] + xf.R[2] * X[2] + xf.t[0] * w;
+        pc[1] = xf.R[3] * X[0] + xf.R[4] * X[1] + xf.R[5] * X[2] + xf.t[1] * w;
+        pc[2] = xf.R[6] * X[0] + xf.R[7] * X[1] + xf.R[8] * X[2] + xf.t[2] * w;
+        // 3. projectHomogeneous (PinholeCamera.hpp(impl):358-378): w < 0 projects -xyz; Successful = distortion valid,
+        //    inside the image, in front of the camera
+        if (w < 0) { pc[0] = -pc[0]; pc[1] = -pc[1]; pc[2] = -pc[2]; }
+        double ip[2], Jp[6];
+        const bool ok = project<true>(cam, pc, ip, Jp) && !(ip[0] < 0.0 || ip[1] < 0.0 || ip[0] >= (double)camB.width ||
+                                                           ip[1] >= (double)camB.height) && pc[2] > 0.0;
+        if (!ok) {
+        } else if (J.cnt[l] < 2) {                                       // 4. after the projection: fewer than 2 observations
+          clear = 1;
+        } else {                                                         // 5. projectionsIntoB_, J P_C J^T with P_C = s I3
+          skip = false;
+          proj[2 * k] = ip[0]; proj[2 * k + 1] = ip[1];
+          const double a0 = s * Jp[0], a1 = s * Jp[1], a2 = s * Jp[2], b0 = s * Jp[3], b1 = s * Jp[4], b2 = s * Jp[5];
+          unc[4 * k] = a0 * Jp[0] + a1 * Jp[1] + a2 * Jp[2];
+          unc[4 * k + 1] = a0 * Jp[3] + a1 * Jp[4] + a2 * Jp[5];
+          unc[4 * k + 2] = b0 * Jp[0] + b1 * Jp[1] + b2 * Jp[2];
+          unc[4 * k + 3] = b0 * Jp[3] + b1 * Jp[4] + b2 * Jp[5];
+        }
+      }
+      skipA[k] = skip ? 1 : 0;
+    }
+    // setLandmarkInitialized(false) in ascending k: a landmark two keypoints share is cleared (and listed) once
+    int total;
+    const int pos = track_scan(clear, s_warp, &total);
+    if (clear) s_cand[pos] = k;
+    __syncthreads();
+    if (tid == 0) {
+      const int h = 2 * J.n_rounds + 1;
+      int n_u = J.hdr[h];
+      for (int i = 0; i < total; ++i) {
+        const int l = F.lm[base_a + s_cand[i]];
+        if (F.lm_init[l]) { F.lm_init[l] = 0; J.uninit[n_u++] = (uint32_t)l; }
+      }
+      J.hdr[h] = n_u;
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(TK_T) k_track_apply(const TrackJobDev* __restrict__ jobs, const MatchJobDev* __restrict__ tab,
+                                                      const TrackRoundDev* __restrict__ rinfo, int round) {
+  __shared__ int s_warp[TK_T / 32];
+  const TrackJobDev& J = jobs[blockIdx.x];
+  const MatchJobDev& M = tab[blockIdx.x];
+  const TrackRoundDev R = rinfo[blockIdx.x];
+  const FeatStore& F = *J.W->feat;
+  const int tid = threadIdx.x;
+  const size_t base_a = ((size_t)R.feat_a * F.C + R.cam_a) * F.N;
+  const size_t base_b = ((size_t)J.feat_b * F.C + R.cam_b) * F.N;
+  const double* proj = M.gate.proj_into_b;
+  const double* unc = M.gate.proj_unc;
+  int n_assoc = J.hdr[2 * J.n_rounds], n_match = 0, n_unc = 0;
+  for (int b0 = 0; b0 < M.nB; b0 += TK_T) {
+    const int b = b0 + tid;
+    int acc = 0, uncertain = 0, l = -1;
+    if (b < M.nB) {
+      const okb_pair p = M.pairs[b];
+      // DenseMatcher::match calls setBestMatch for every B whose winner is below the threshold, B ascending
+      if (p.index_a >= 0 && p.distance < J.threshold) {
+        const int a = p.index_a;
+        l = F.lm[base_a + a];
+        // setBestMatch 3D-2D (:483-526): chi-square again, in double this time (Eigen's 2x2 inverse), > 4 rejects
+        const double sd = 0.8 * F.size[base_b + b] / 12.0;
+        const double U00 = sd * sd + unc[4 * a], U01 = unc[4 * a + 1], U10 = unc[4 * a + 2], U11 = sd * sd + unc[4 * a + 3];
+        const double e0 = proj[2 * a] - F.kp[2 * (base_b + b)], e1 = proj[2 * a + 1] - F.kp[2 * (base_b + b) + 1];
+        const double invdet = 1.0 / (U00 * U11 - U10 * U01);
+        const double i00 = U11 * invdet, i10 = -U10 * invdet, i01 = -U01 * invdet, i11 = U00 * invdet;
+        const double r0 = e0 * i00 + e1 * i10, r1 = e0 * i01 + e1 * i11;
+        const double chi2 = r0 * e0 + r1 * e1;
+        if (!(chi2 > 4.0)) {
+          acc = 1;
+          // saturated image uncertainty: counted, not rejected
+          const double nrm = sqrt(U00 * U00 + U10 * U10 + U01 * U01 + U11 * U11);
+          uncertain = nrm > 25.0 / (sd * sd * sqrt(2.0)) ? 1 : 0;
+        }
+      }
+    }
+    int total, total_u;
+    const int pos = track_scan(acc, s_warp, &total);
+    track_scan(acc & uncertain, s_warp, &total_u);
+    if (acc) {
+      // B's keypoint takes A's landmark and its observation; the count of the landmark rises for the later rounds
+      F.lm[base_b + b] = l;
+      F.observed[base_b + b] = 1;
+      if (l < J.cnt_cap) atomicAdd(&J.cnt[l], 1);
+      J.assoc[n_assoc + pos] = make_uint2((uint32_t)b | ((uint32_t)round << 16) | ((uint32_t)R.cam_b << 24) | ((uint32_t)uncertain << 31),
+                                          (uint32_t)l);
+    }
+    n_assoc += total; n_match += total; n_unc += total_u;
+  }
+  if (tid == 0) {
+    J.hdr[2 * round] = n_match;
+    J.hdr[2 * round + 1] = n_unc;
+    J.hdr[2 * J.n_rounds] = n_assoc;
+  }
+}
+}  // namespace
+
+// Host checks of one job (against the store as the pending commands leave it); "" = valid.
+static std::string track_job_invalid(okb_ctx* c, const okb_track_job& j, int desc_bytes, std::vector<char>& seen, size_t& sumA, size_t& sumB) {
+  if (j.win < 0 || j.win >= c->max_windows) return "window slot out of range";
+  const WinStore& S = c->wins[j.win];
+  const WinDev& W = c->host[j.win];
+  if (!S.uploaded) return "window slot not uploaded";
+  if (!S.feat_mem) return "window has no feature store (okb_window_reserve_features)";
+  if (seen[j.win]) return "window listed twice";
+  seen[j.win] = 1;
+  const FeatStore& F = S.feat;
+  if (F.D != desc_bytes) return "descriptor length differs from the call's first job";
+  if (j.pose_b < 0 || j.pose_b >= W.K) return "pose_b out of range";
+  if (j.sb_b < -1 || j.sb_b >= W.NSB) return "sb_b out of range";
+  if (j.feat_slot_b < 0 || j.feat_slot_b >= F.F) return "feat_slot_b out of range";
+  if (j.num_best < 1 || j.num_best > MAX_BEST) return "num_best out of range (1..8)";
+  if (j.n_rounds < 0 || (j.n_rounds > 0 && (!j.rounds || !j.num_matches || !j.num_uncertain))) return "round list or per-round outputs missing";
+  if (j.n_rounds > 255) return "more than 255 rounds";
+  if (!j.n_assoc || !j.n_uninit) return "n_assoc / n_uninit missing";
+  sumA = 0; sumB = 0;
+  for (int r = 0; r < j.n_rounds; ++r) {
+    const okb_track_round& R = j.rounds[r];
+    if (R.feat_slot_a < 0 || R.feat_slot_a >= F.F || R.cam_a < 0 || R.cam_a >= F.C) return "round " + std::to_string(r) + ": frame A out of range";
+    if (R.cam_b < 0 || R.cam_b >= F.C || R.cam_b >= W.NC || R.cam_b >= W.NE) return "round " + std::to_string(r) + ": cam_b out of range";
+    // the apply kernel writes B's image while it reads A's: one image cannot be both
+    if (R.feat_slot_a == j.feat_slot_b && R.cam_a == R.cam_b) return "round " + std::to_string(r) + ": frame B against itself in one camera";
+    const int nA = S.feat_n_pending[(size_t)R.feat_slot_a * F.C + R.cam_a], nB = S.feat_n_pending[(size_t)j.feat_slot_b * F.C + R.cam_b];
+    if (nA < 0 || nB < 0) return "round " + std::to_string(r) + ": feature slot has no keypoints for the camera";
+    sumA += nA; sumB += nB;
+  }
+  if ((size_t)std::max(j.assoc_cap, 0) < sumB || (sumB && !j.assoc)) return "assoc capacity below the B keypoints of all rounds";
+  if ((size_t)std::max(j.uninit_cap, 0) < sumA || (sumA && !j.uninit)) return "uninit capacity below the A keypoints of all rounds";
+  return "";
+}
+
+extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job* jobs) {
+  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
+  if (n_jobs == 0) return OKB_OK;
+  if (n_jobs > 65535) { c->set_error("okb_track_3d2d_batch: more than 65535 jobs"); return OKB_ERR_INVALID_ARG; }   // grid dimension
+  if (c->shard_world > 1) { c->set_error("okb_track_3d2d_batch: landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
+  const int desc_bytes = (jobs[0].win >= 0 && jobs[0].win < c->max_windows) ? c->wins[jobs[0].win].feat.D : 0;
+  std::vector<char> seen(c->max_windows, 0);
+  std::vector<size_t> sumA(n_jobs), sumB(n_jobs);
+  for (int i = 0; i < n_jobs; ++i) {
+    const std::string why = track_job_invalid(c, jobs[i], desc_bytes, seen, sumA[i], sumB[i]);
+    if (!why.empty()) { c->set_error("okb_track_3d2d_batch: jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
+  }
+  cudaSetDevice(c->device);
+  okb_frontend_state* F = fe(c);
+  std::lock_guard<std::mutex> lk(F->track_mtx);
+  // pending edits first (they may be the store edits this call reads), then after the solver work on these windows
+  {     // one commit per run of consecutive windows, so the launch count does not grow with the number of sessions
+    std::vector<int32_t> wl(n_jobs);
+    for (int i = 0; i < n_jobs; ++i) wl[i] = jobs[i].win;
+    std::sort(wl.begin(), wl.end());
+    for (int i = 0; i < n_jobs;) {
+      int k = i + 1;
+      while (k < n_jobs && wl[k] == wl[k - 1] + 1) ++k;
+      const int rc = okb_commit_range(c, wl[i], k - i);
+      if (rc) return rc;
+      i = k;
+    }
+  }
+  cudaStream_t xs = c->stream_xfer;
+  for (int i = 0; i < n_jobs; ++i) {
+    const WinStore& S = c->wins[jobs[i].win];
+    if (S.done_idx >= 0) FE_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
+  }
+  // jobs by decreasing round count: the jobs of round r are the first m[r]
+  std::vector<int> order(n_jobs);
+  for (int i = 0; i < n_jobs; ++i) order[i] = i;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return jobs[a].n_rounds > jobs[b].n_rounds; });
+  const int R = jobs[order[0]].n_rounds;
+  std::vector<int> m(R, 0);
+  for (int i = 0; i < n_jobs; ++i)
+    for (int r = 0; r < jobs[i].n_rounds; ++r) ++m[r];
+  // staging (pinned + device mirror): in  = [job table | per round: match table | round table]
+  //                                   out = [per job: header | associations | cleared slots]
+  // scratch (device only):           per job: counts; per (job, round): proj | unc | topk | pairs | skipA | skipB | done
+  auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+  size_t off = up256(sizeof(TrackJobDev) * n_jobs);
+  std::vector<size_t> o_tab(R), o_rinfo(R);
+  for (int r = 0; r < R; ++r) { o_tab[r] = off; off = up16(off + sizeof(MatchJobDev) * m[r]); o_rinfo[r] = off; off = up16(off + sizeof(TrackRoundDev) * m[r]); }
+  const size_t in_bytes = up256(off);
+  off = in_bytes;
+  std::vector<size_t> o_hdr(n_jobs), o_assoc(n_jobs), o_un(n_jobs);
+  for (int i = 0; i < n_jobs; ++i) {
+    o_hdr[i] = off; o_assoc[i] = up16(off + 4 * (2 * (size_t)jobs[i].n_rounds + 2)); o_un[i] = o_assoc[i] + 8 * sumB[i];
+    off = up16(o_un[i] + 4 * sumA[i]);
+  }
+  const size_t out_end = off;
+  int rc;
+  if ((rc = grow_pinned(c, &F->track_io.h_stage, &F->track_io.h_stage_cap, out_end))) return rc;
+  if ((rc = grow(c, &F->track_io.d_io, &F->track_io.d_io_cap, out_end))) return rc;
+  size_t so = 0;
+  std::vector<size_t> o_cnt(n_jobs);
+  for (int i = 0; i < n_jobs; ++i) { o_cnt[i] = so; so = up256(so + 4 * (size_t)std::max(c->host[jobs[i].win].L, 1)); }
+  std::vector<size_t> o_rs(n_jobs);     // per-job start of the round scratch
+  for (int i = 0; i < n_jobs; ++i) {
+    o_rs[i] = so;
+    const okb_track_job& j = jobs[i];
+    for (int r = 0; r < j.n_rounds; ++r) {
+      const WinStore& S = c->wins[j.win];
+      const size_t nA = S.feat_n_pending[(size_t)j.rounds[r].feat_slot_a * S.feat.C + j.rounds[r].cam_a];
+      const size_t nB = S.feat_n_pending[(size_t)j.feat_slot_b * S.feat.C + j.rounds[r].cam_b];
+      so = up256(so + 16 * nA + 32 * nA + sizeof(okb_pair) * nA * j.num_best + sizeof(okb_pair) * nB + up16(nA) + up16(nB) + up16(nA));
+    }
+  }
+  if ((rc = grow(c, &F->track_scratch, &F->track_scratch_cap, std::max<size_t>(so, 256)))) return rc;
+  uint8_t* h = F->track_io.h_stage;
+  uint8_t* d = F->track_io.d_io;
+  uint8_t* sc = F->track_scratch;
+  const size_t sm_top = sizeof(okb_pair) * (size_t)AS_CHUNK * MAX_BEST;
+  size_t sm = sm_top;
+  std::vector<int> maxA(R, 0);
+  TrackJobDev* tj = reinterpret_cast<TrackJobDev*>(h);
+  for (int t = 0; t < n_jobs; ++t) {
+    const int i = order[t];
+    const okb_track_job& j = jobs[i];
+    const WinStore& S = c->wins[j.win];
+    const FeatStore& FS = S.feat;
+    TrackJobDev J;
+    std::memset(&J, 0, sizeof J);
+    J.W = c->d_wins + j.win;
+    J.pose_b = j.pose_b; J.sb_b = j.sb_b; J.feat_b = j.feat_slot_b; J.n_rounds = j.n_rounds;
+    J.threshold = j.threshold;
+    J.cnt_cap = std::max(c->host[j.win].L, 1);
+    J.cnt = reinterpret_cast<int*>(sc + o_cnt[i]);
+    J.hdr = reinterpret_cast<int*>(d + o_hdr[i]);
+    J.assoc = reinterpret_cast<uint2*>(d + o_assoc[i]);
+    J.uninit = reinterpret_cast<uint32_t*>(d + o_un[i]);
+    tj[t] = J;
+    size_t q = o_rs[i];
+    for (int r = 0; r < j.n_rounds; ++r) {
+      const okb_track_round& Rr = j.rounds[r];
+      const size_t ia = (size_t)Rr.feat_slot_a * FS.C + Rr.cam_a, ib = (size_t)j.feat_slot_b * FS.C + Rr.cam_b;
+      const int nA = S.feat_n_pending[ia], nB = S.feat_n_pending[ib];
+      const size_t o_proj = q, o_unc = o_proj + 16 * (size_t)nA, o_top = o_unc + 32 * (size_t)nA, o_pairs = o_top + sizeof(okb_pair) * (size_t)nA * j.num_best;
+      const size_t o_sa = o_pairs + sizeof(okb_pair) * (size_t)nB, o_sb = o_sa + up16(nA), o_done = o_sb + up16(nB);
+      q = up256(o_done + up16(nA));
+      MatchJobDev jd;
+      std::memset(&jd, 0, sizeof jd);
+      jd.A = FS.desc + ia * FS.N * (FS.D / 4);
+      jd.B = FS.desc + ib * FS.N * (FS.D / 4);
+      jd.skipA = sc + o_sa; jd.skipB = sc + o_sb;
+      jd.topk = reinterpret_cast<okb_pair*>(sc + o_top);
+      jd.pairs = reinterpret_cast<okb_pair*>(sc + o_pairs);
+      jd.done = sc + o_done;
+      jd.nA = nA; jd.nB = nB; jd.num_best = j.num_best;
+      jd.list_thr = j.threshold; jd.gate_thr = j.threshold;          // Frontend's matcher: no ratio test
+      const size_t sm_b = (sizeof(okb_pair) + sizeof(int)) * (size_t)nB;
+      jd.in_smem = sm_top + sm_b + 1024 <= (size_t)c->smem_optin ? 1 : 0;
+      if (jd.in_smem) sm = std::max(sm, sm_top + sm_b);
+      jd.gate.mode = OKB_GATE_3D2D;
+      jd.gate.kp_b = FS.kp + 2 * ib * FS.N;
+      jd.gate.kp_size_b = FS.size + ib * FS.N;
+      jd.gate.proj_into_b = reinterpret_cast<const double*>(sc + o_proj);
+      jd.gate.proj_unc = reinterpret_cast<const double*>(sc + o_unc);
+      reinterpret_cast<MatchJobDev*>(h + o_tab[r])[t] = jd;
+      reinterpret_cast<TrackRoundDev*>(h + o_rinfo[r])[t] = TrackRoundDev{Rr.feat_slot_a, Rr.cam_a, Rr.cam_b, 0};
+      maxA[r] = std::max(maxA[r], nA);
+    }
+  }
+  FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
+  const TrackJobDev* d_jobs = reinterpret_cast<const TrackJobDev*>(d);
+  if (sm > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
+  const int nw = desc_bytes / 4;
+  for (int r = 0; r < R; ++r) {
+    const MatchJobDev* d_tab = reinterpret_cast<const MatchJobDev*>(d + o_tab[r]);
+    const TrackRoundDev* d_ri = reinterpret_cast<const TrackRoundDev*>(d + o_rinfo[r]);
+    k_track_setup<<<m[r], TK_T, 0, xs>>>(d_jobs, d_tab, d_ri, r);
+    DISPATCH_NW(nw, (k_hamming_topk<NW, true><<<dim3(std::max(1, (maxA[r] + MW - 1) / MW), m[r]), MT, 0, xs>>>(d_tab)));
+    k_assign<<<m[r], AS_T, sm, xs>>>(d_tab);
+    k_track_apply<<<m[r], TK_T, 0, xs>>>(d_jobs, d_tab, d_ri, r);
+  }
+  F->launches += 4 * (int64_t)R;
+  FE_CUDA(c, cudaGetLastError());
+  FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
+  FE_CUDA(c, cudaStreamSynchronize(xs));
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_track_job& j = jobs[i];
+    if (j.n_rounds == 0) { *j.n_assoc = 0; *j.n_uninit = 0; continue; }
+    const int32_t* hd = reinterpret_cast<const int32_t*>(h + o_hdr[i]);
+    for (int r = 0; r < j.n_rounds; ++r) { j.num_matches[r] = hd[2 * r]; j.num_uncertain[r] = hd[2 * r + 1]; }
+    const int na = hd[2 * j.n_rounds], nu = hd[2 * j.n_rounds + 1];
+    *j.n_assoc = na; *j.n_uninit = nu;
+    const uint2* as = reinterpret_cast<const uint2*>(h + o_assoc[i]);
+    for (int k = 0; k < na; ++k) {
+      okb_track_assoc& o = j.assoc[k];
+      o.kp_b = (int32_t)(as[k].x & 0xffffu); o.round = (int32_t)((as[k].x >> 16) & 0xffu); o.cam_b = (int32_t)((as[k].x >> 24) & 0x7fu);
+      o.uncertain = (int32_t)(as[k].x >> 31); o.lm_slot = (int32_t)as[k].y; o._pad = 0;
+    }
+    if (nu) std::memcpy(j.uninit, h + o_un[i], 4 * (size_t)nu);
+  }
   return OKB_OK;
 }

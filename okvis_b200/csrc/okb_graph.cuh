@@ -36,7 +36,12 @@ enum {
   CMD_SET_POSE_PRIORS = 14, // n; payload okb_pose_prior [n]
   CMD_SET_SB_PRIORS = 15,   // n; payload okb_sb_prior [n]
   CMD_REMOVE_SB = 17,       // a = speed/bias index: the block, the IMU terms and SpeedAndBiasError priors attached to it
-  CMD_SET_MARG = 16         // a = n, b = n_blocks; payload kind [b] i32, idx [b] u32 (each 8-byte padded), x0, J [n][n], e0 [n]
+  CMD_SET_MARG = 16,        // a = n, b = n_blocks; payload kind [b] i32, idx [b] u32 (each 8-byte padded), x0, J [n][n], e0 [n]
+  // feature store (FeatStore, okb_estimator.cuh); every array of a payload is 8-byte padded
+  CMD_SET_FEATURES = 18,    // n keypoints of image (a = feature slot, b = camera); payload x, y, size [n][3] f64, lm [n] i32, observed [n] u8, desc [n][D]
+  CMD_SET_FEATURE_LMS = 19, // n; a = feature slot, b = camera; payload kp_idx [n] i32, lm [n] i32, observed [n] u8
+  CMD_CLEAR_FEATURES = 20,  // a = feature slot: every camera's image emptied
+  CMD_SET_LM_INIT = 21      // n; payload idx [n] u32, flags [n] u8
 };
 struct CmdHeader { uint32_t op, n, a, b; uint64_t payload_bytes; };   // payload follows, 8-byte aligned
 static_assert(sizeof(CmdHeader) == 24, "command header layout");
@@ -263,6 +268,18 @@ __global__ void __launch_bounds__(1024) k_apply_commands(const WinDev* __restric
           okb_observation* ob = W.m_obs + i;
           if ((int)ob->lm_idx < L && W.m_mark[ob->lm_idx]) ob->sqrt_info = 0.0;
         }
+        if (W.feat) {
+          // the store forgets the removed slots (the reference's isLandmarkAdded(id) == false for a gone id), so a slot
+          // reused later is never reached through a keypoint that referred to its previous occupant
+          const FeatStore& F = *W.feat;
+          const int n_ent = F.F * F.C * F.N;
+          for (int e = tid; e < n_ent; e += NT) {
+            const int l = F.lm[e];
+            if (l >= 0 && l < L && W.m_mark[l]) { F.lm[e] = -1; F.observed[e] = 0; }
+          }
+          for (int i = tid; i < n; i += NT)
+            if ((int)idx[i] < F.lm_cap) F.lm_init[idx[i]] = 0;
+        }
         __syncthreads();
         for (int i = tid; i < n; i += NT)
           if ((int)idx[i] < L) { W.m_mark[idx[i]] = 0; *reinterpret_cast<double4*>(W.m_lm + 4 * (size_t)idx[i]) = make_double4(0, 0, 0, 0); }
@@ -451,6 +468,56 @@ __global__ void __launch_bounds__(1024) k_apply_commands(const WinDev* __restric
             else if ((int)W.marg_idx[b] > sbi) W.marg_idx[b]--;
           }
           g->NSB = NSB - 1;
+        }
+        break;
+      }
+      case CMD_SET_FEATURES: {
+        const int n = (int)h.n, f = (int)h.a, cm = (int)h.b;
+        if (!W.feat || f >= W.feat->F || cm >= W.feat->C || n > W.feat->N) { if (tid == 0) graph_error(g, GERR_INDEX); break; }
+        const FeatStore& F = *W.feat;
+        const size_t base = ((size_t)f * F.C + cm) * F.N;
+        const size_t bl = ((size_t)4 * n + 7) & ~(size_t)7, bo = ((size_t)n + 7) & ~(size_t)7;
+        const int32_t* lm = reinterpret_cast<const int32_t*>(pay + 24 * (size_t)n);
+        const uint8_t* ob = pay + 24 * (size_t)n + bl;
+        const uint32_t* desc = reinterpret_cast<const uint32_t*>(pay + 24 * (size_t)n + bl + bo);
+        for (int i = tid; i < n; i += NT) {
+          F.kp[2 * (base + i)] = pd[3 * i]; F.kp[2 * (base + i) + 1] = pd[3 * i + 1]; F.size[base + i] = pd[3 * i + 2];
+          F.lm[base + i] = lm[i]; F.observed[base + i] = ob[i];
+        }
+        const int dw = F.D / 4;
+        for (int i = tid; i < n * dw; i += NT) F.desc[base * dw + i] = desc[i];
+        if (tid == 0) F.n[f * F.C + cm] = n;
+        break;
+      }
+      case CMD_SET_FEATURE_LMS: {
+        const int n = (int)h.n, f = (int)h.a, cm = (int)h.b;
+        if (!W.feat || f >= W.feat->F || cm >= W.feat->C) { if (tid == 0) graph_error(g, GERR_INDEX); break; }
+        const FeatStore& F = *W.feat;
+        const size_t base = ((size_t)f * F.C + cm) * F.N;
+        const size_t b4 = ((size_t)4 * n + 7) & ~(size_t)7;
+        const int32_t* k = reinterpret_cast<const int32_t*>(pay);
+        const int32_t* lm = reinterpret_cast<const int32_t*>(pay + b4);
+        const uint8_t* ob = pay + 2 * b4;
+        const int nk = F.n[f * F.C + cm];
+        for (int i = tid; i < n; i += NT) {
+          if (k[i] < 0 || k[i] >= nk) { graph_error(g, GERR_INDEX); continue; }
+          F.lm[base + k[i]] = lm[i]; F.observed[base + k[i]] = ob[i];
+        }
+        break;
+      }
+      case CMD_CLEAR_FEATURES: {
+        if (!W.feat || (int)h.a >= W.feat->F) { if (tid == 0) graph_error(g, GERR_INDEX); break; }
+        if (tid < W.feat->C) W.feat->n[(int)h.a * W.feat->C + tid] = -1;
+        break;
+      }
+      case CMD_SET_LM_INIT: {
+        const int n = (int)h.n;
+        if (!W.feat) { if (tid == 0) graph_error(g, GERR_INDEX); break; }
+        const uint32_t* idx = reinterpret_cast<const uint32_t*>(pay);
+        const uint8_t* fl = pay + (((size_t)4 * n + 7) & ~(size_t)7);
+        for (int i = tid; i < n; i += NT) {
+          if ((int)idx[i] >= W.feat->lm_cap) { graph_error(g, GERR_INDEX); continue; }
+          W.feat->lm_init[idx[i]] = fl[i] ? 1 : 0;
         }
         break;
       }
