@@ -424,6 +424,14 @@ int okb_debug_schur_plan(okb_ctx* ctx, int first, int count, int32_t out[3]);
 /* Diagnostics: the mutable preintegration cache of ImuError term `term` (ImuError.hpp:251-276): the bias the
  * preintegration was done at, whether it is valid (0 = redo_), and how often it was redone. */
 int okb_debug_imu_cache(okb_ctx* ctx, int win, int term, double sb_ref[9], int32_t* valid, int32_t* redo_count);
+/* Diagnostics: what the window's last solver round evaluated for IMU terms [first_term, first_term + n_terms), as
+ * OKB_IMU_TERM_OUT doubles per term: the term's 30x30 block J^T J (row-major; J = [J0 J1 J2 J3], the four minimal
+ * Jacobians side by side: pose0, speed/bias0, pose1, speed/bias1), then J^T r (30), then the cost 0.5 |r|^2.  After
+ * okb_optimize with max_iterations = 0 that is the linearisation at the window's state.  Waits for the solver, commits
+ * nothing and launches nothing: after an edit (pending or committed) the output is stale, in the old term numbering,
+ * until the next optimize.  A range outside the window's current terms or a NULL `out`: OKB_ERR_INVALID_ARG. */
+#define OKB_IMU_TERM_OUT 931
+int okb_debug_imu_terms(okb_ctx* ctx, int win, int first_term, int n_terms, double* out);
 
 /* ------------------------------------------------- single-block test hooks
  * Mirror ErrorInterface::EvaluateWithMinimalJacobians (okvis_ceres/include/okvis/ceres/ErrorInterface.hpp:93-95).

@@ -16,6 +16,7 @@ OKB_ERR_INVALID_ARG, OKB_ERR_CUDA, OKB_ERR_UNSUPPORTED, OKB_ERR_CAPACITY, OKB_ER
     -1, -2, -3, -4, -5, -6)
 DIST_NONE, DIST_RADTAN, DIST_EQUIDISTANT, DIST_RADTAN8 = 0, 1, 2, 3
 BLOCK_POSE, BLOCK_SPEED_BIAS, BLOCK_EXTRINSICS = 0, 1, 2
+IMU_TERM_OUT = 931      # OKB_IMU_TERM_OUT: doubles per term of okb_debug_imu_terms (H30 | g30 | cost)
 TERMINATION = {0: "NO_CONVERGENCE", 1: "FUNCTION_TOLERANCE", 2: "PARAMETER_TOLERANCE", 3: "GRADIENT_TOLERANCE",
                4: "MIN_RADIUS", 5: "TIME_LIMIT", 6: "FAILURE"}
 

@@ -238,6 +238,13 @@ class Context:
         self._check(lib().okb_debug_imu_cache(self._h, int(win), int(term), _p(ref), C.byref(v), C.byref(r)))
         return ref, v.value, r.value
 
+    def debug_imu_terms(self, win, first_term, n_terms):
+        """okb_debug_imu_terms: (H30 [n][30][30], g30 [n][30], cost [n]) of the window's last k_imu launch (stale after
+        an edit)."""
+        out = np.zeros((int(n_terms), abi.IMU_TERM_OUT))
+        self._check(lib().okb_debug_imu_terms(self._h, int(win), int(first_term), int(n_terms), _p(out)))
+        return out[:, :900].reshape(-1, 30, 30), out[:, 900:930].copy(), out[:, 930].copy()
+
     def h2d_bytes(self, win):
         f = lib().okb_window_h2d_bytes
         f.restype = C.c_int64

@@ -452,6 +452,16 @@ extern "C" int okb_window_commit(okb_ctx* c, int first, int count) {
 // Full upload = a command stream that rebuilds the whole graph (host side: validation of what only the host can
 // reject synchronously + one pass of memcpy into the pinned command buffer; sorting / slot tables / duplicate
 // detection happen on the device).
+// An IMU term's samples must cover [t0, t1] with t0 < t1 (ImuError.cpp:86-89 asserts the first and refuses the last).
+// A term ending before t1 would never preintegrate and silently add nothing to every solve; one starting after t0
+// would integrate a shorter interval than the Delta_t its residual uses.
+static const char* imu_term_coverage(const okb_imu_term& T, const okb_imu_sample* s) {
+  if (!(T.t1_ns > T.t0_ns)) return "t1 is not after t0";
+  if (s[0].t_ns > T.t0_ns) return "first sample is after t0";
+  if (s[T.sample_count - 1].t_ns < T.t1_ns) return "last sample is before t1";
+  return nullptr;
+}
+
 static int upload_pack(okb_ctx* c, int win, const okb_window_desc* D) {
   if (!c || !D || win < 0 || win >= c->max_windows) return OKB_ERR_INVALID_ARG;
   cudaSetDevice(c->device);
@@ -491,6 +501,10 @@ static int upload_pack(okb_ctx* c, int win, const okb_window_desc* D) {
     if ((int)T.pose0 >= K || (int)T.pose1 >= K || (int)T.sb0 >= NSB || (int)T.sb1 >= NSB ||
         (uint64_t)T.sample_offset + (uint64_t)T.sample_count > (uint64_t)D->n_imu_samples || T.sample_count < 2) {
       c->set_error("IMU term index out of range");
+      return OKB_ERR_INVALID_ARG;
+    }
+    if (const char* why = imu_term_coverage(T, D->imu_samples + T.sample_offset)) {
+      c->set_error("IMU term " + std::to_string(t) + ": " + why);
       return OKB_ERR_INVALID_ARG;
     }
   }
@@ -646,6 +660,10 @@ extern "C" int okb_window_add_frame(okb_ctx* c, int win, const double* pose, con
     if ((int)term->pose0 >= K1 || (int)term->pose1 >= K1 || (int)term->sb0 >= NSB1 || (int)term->sb1 >= NSB1 ||
         (uint64_t)term->sample_offset + term->sample_count > (uint64_t)n_samples || term->sample_count < 2) {
       c->set_error("IMU term index out of range");
+      return OKB_ERR_INVALID_ARG;
+    }
+    if (const char* why = imu_term_coverage(*term, samples + term->sample_offset)) {
+      c->set_error("IMU term " + std::to_string(W->n_imu) + ": " + why);
       return OKB_ERR_INVALID_ARG;
     }
     if (W->n_imu + 1 > S->caps.T || W->n_samples + n_samples > S->caps.S) { c->set_error("okb_window_add_frame: IMU capacity exceeded (okb_window_reserve)"); return OKB_ERR_CAPACITY; }
@@ -1807,6 +1825,23 @@ extern "C" int okb_debug_imu_cache(okb_ctx* c, int win, int term, double sb_ref[
   if (sb_ref) std::memcpy(sb_ref, h.sb_ref, sizeof(double) * 9);
   if (valid) *valid = h.valid;
   if (redo_count) *redo_count = h.redo_count;
+  return OKB_OK;
+}
+
+// diagnostics: what the window's last k_imu launch wrote for terms [first_term, first_term + n_terms): H30 (row-major) |
+// g30 | cost per term.  Read-only: commits nothing and launches nothing, so after an edit the terms are renumbered and
+// the output is stale until the next optimize.
+extern "C" int okb_debug_imu_terms(okb_ctx* c, int win, int first_term, int n_terms, double* out) {
+  int rc = check_range(c, win, 1);
+  if (rc) return rc;
+  const WinDev& W = c->host[win];
+  if (!out || first_term < 0 || n_terms < 0 || first_term + n_terms > W.n_imu) return OKB_ERR_INVALID_ARG;
+  if (n_terms == 0) return OKB_OK;
+  cudaSetDevice(c->device);
+  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
+  OKB_CUDA(c, cudaStreamSynchronize(c->stream_imu));
+  OKB_CUDA(c, cudaMemcpy2D(out, sizeof(double) * OKB_IMU_TERM_OUT, W.imu_out + (size_t)first_term * kImuOut, sizeof(double) * kImuOut,
+                           sizeof(double) * OKB_IMU_TERM_OUT, (size_t)n_terms, cudaMemcpyDeviceToHost));
   return OKB_OK;
 }
 

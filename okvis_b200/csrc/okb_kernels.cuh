@@ -16,6 +16,7 @@ namespace okb {
 constexpr int S_THREADS = 256;    // two k_solve CTAs per SM (packed system: ~112 KB of shared memory each)
 constexpr int S_WARPS = S_THREADS / 32;
 constexpr int kImuOut = 932;     // doubles per IMU term produced by k_imu: H30 | g30 | cost | pad
+static_assert(OKB_IMU_TERM_OUT == 900 + 30 + 1 && OKB_IMU_TERM_OUT < kImuOut, "okb_debug_imu_terms copies H30 | g30 | cost");
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
   unsigned long long t;
