@@ -367,6 +367,13 @@ int okb_optimize_finish(okb_ctx* ctx, int win_first, int win_count, okb_summary*
 int okb_optimize_slots(okb_ctx* ctx, int n, const int32_t* slots, const okb_solve_options* opt, okb_summary* summaries);
 int okb_optimize_slots_async(okb_ctx* ctx, int n, const int32_t* slots, const okb_solve_options* opt);
 int okb_optimize_slots_finish(okb_ctx* ctx, int n, const int32_t* slots, okb_summary* summaries);
+/* Window groups of the batched solve.  A batch is split into groups of consecutive batch positions (sizes differing
+ * by at most one), each solved on its own stream and started behind the previous one, so that the latency-bound
+ * reduced solve of one group overlaps the landmark kernels of another.  Results are bit-identical for any group count.
+ * n = 0 (the default) chooses 4 groups for a batch of at least as many windows as the device has SMs, else one;
+ * n = 1..4 forces n groups (at most one per window) for every later okb_optimize* call.  Landmark-sharded contexts
+ * always solve in one group.  Other n: OKB_ERR_INVALID_ARG. */
+int okb_set_solve_groups(okb_ctx* ctx, int n);
 /* Copies the estimates back.  Any pointer may be NULL.  quality[l] = sqrt(lambda_min)/sqrt(lambda_max)
  * of the landmark's 3x3 Hessian block as in Estimator.cpp:880-894 (0 if lambda_min < 1e-12). */
 int okb_window_download(okb_ctx* ctx, int win, double* poses, double* speed_bias,
@@ -411,7 +418,9 @@ int okb_shard_stats(okb_ctx* ctx, int win, double out[4]);
 /* Optional per-kernel device timing: CUDA events on the context stream around every solver kernel
  * launch.  okb_profile_enable(ctx,1) clears the counters; okb_profile_read synchronises and returns
  * out[0] = ms in k_landmarks, out[1] = its launches, out[2] = ms in k_solve, out[3] = launches,
- * out[4] = ms in k_quality, out[5] = launches. */
+ * out[4] = ms in k_quality, out[5] = launches.  A solve in several window groups (okb_set_solve_groups) counts each
+ * round once, and times it from the earliest group's start of the kernels to the latest group's end; the groups run
+ * at the same time, so that span also holds other kernels of the other groups and the times are approximate. */
 int okb_profile_enable(okb_ctx* ctx, int on);
 int okb_profile_read(okb_ctx* ctx, double out[6]);
 /* Diagnostics: nanoseconds the reduced-solve kernel spent per internal phase during the last optimize of

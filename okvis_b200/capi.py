@@ -76,6 +76,10 @@ class Context:
     def profile_enable(self, on=True):
         self._check(lib().okb_profile_enable(self._h, int(on)))
 
+    def set_solve_groups(self, n=0):
+        """okb_set_solve_groups: window groups of later optimize calls, 0 = automatic, 1..4 forced."""
+        self._check(lib().okb_set_solve_groups(self._h, int(n)))
+
     def profile_read(self):
         out = np.zeros(6)
         self._check(lib().okb_profile_read(self._h, _p(out)))

@@ -74,6 +74,15 @@ struct okb_ctx {
   cudaStream_t stream = nullptr;
   cudaStream_t stream_imu = nullptr;     // k_imu runs beside the landmark kernels
   cudaEvent_t ev_round = nullptr, ev_imu = nullptr;
+  // Window groups of a batched solve (launch_rounds): group g runs its round chain on group_stream[g] with k_imu on
+  // group_imu[g].  Group 0 is the context's own chain: entry 0 aliases stream / stream_imu / ev_round / ev_imu and is
+  // not destroyed separately.  group_stagger[g] is recorded on group g's stream after its first k_landmarks, and group
+  // g+1 starts behind it; group_done[g] (g >= 1) joins group g back into `stream`.
+  static constexpr int kMaxSolveGroups = 4;
+  cudaStream_t group_stream[kMaxSolveGroups] = {}, group_imu[kMaxSolveGroups] = {};
+  cudaEvent_t group_round[kMaxSolveGroups] = {}, group_imu_done[kMaxSolveGroups] = {};
+  cudaEvent_t group_stagger[kMaxSolveGroups] = {}, group_done[kMaxSolveGroups] = {};
+  int solve_groups = 0;                  // okb_set_solve_groups: 0 = automatic (plan_rounds)
   // Transfers (window uploads / estimate downloads) run on their own stream so that they overlap solver
   // kernels of other windows.  ev_join orders the solver stream after all uploads issued so far;
   // done_ring[k] is recorded on the solver stream after each optimize / reset and transfers of the
@@ -140,6 +149,7 @@ struct okb_ctx {
   bool profile = false;
   std::vector<cudaEvent_t> prof_events;   // pairs (start, stop)
   std::vector<int> prof_kind;             // kernel id per pair
+  std::vector<int> prof_join;             // per pair: index of the first pair of its span (itself, unless grouped)
   size_t prof_used = 0;
   std::string error;
   std::mutex error_mu;                    // uploads of different slots may run on several host threads

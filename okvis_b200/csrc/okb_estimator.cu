@@ -82,6 +82,22 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
     delete c;
     return OKB_ERR_CUDA;
   }
+  c->group_stream[0] = c->stream; c->group_imu[0] = c->stream_imu;
+  c->group_round[0] = c->ev_round; c->group_imu_done[0] = c->ev_imu;
+  for (int g = 0; g < okb_ctx::kMaxSolveGroups; ++g) {      // further groups: the same priorities as group 0
+    bool ok = cudaEventCreateWithFlags(&c->group_stagger[g], cudaEventDisableTiming) == cudaSuccess;
+    if (g > 0)
+      ok = ok && cudaStreamCreateWithPriority(&c->group_stream[g], cudaStreamNonBlocking, prio_greatest) == cudaSuccess &&
+           cudaStreamCreateWithPriority(&c->group_imu[g], cudaStreamNonBlocking, prio_least) == cudaSuccess &&
+           cudaEventCreateWithFlags(&c->group_round[g], cudaEventDisableTiming) == cudaSuccess &&
+           cudaEventCreateWithFlags(&c->group_imu_done[g], cudaEventDisableTiming) == cudaSuccess &&
+           cudaEventCreateWithFlags(&c->group_done[g], cudaEventDisableTiming) == cudaSuccess;
+    if (!ok) {
+      g_create_error = "cudaStreamCreate / cudaEventCreate failed";
+      okb_ctx_destroy(c);
+      return OKB_ERR_CUDA;
+    }
+  }
   for (int k = 0; k < okb_ctx::kDoneRing; ++k) cudaEventCreateWithFlags(&c->done_ring[k], cudaEventDisableTiming);
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device_id);
@@ -167,6 +183,15 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
   if (c->stream_prop) cudaStreamDestroy(c->stream_prop);
   for (auto& g : c->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   for (auto e : c->prof_events) cudaEventDestroy(e);
+  for (int g = 0; g < okb_ctx::kMaxSolveGroups; ++g) {
+    if (c->group_stagger[g]) cudaEventDestroy(c->group_stagger[g]);
+    if (g == 0) continue;      // entry 0 aliases the context's own stream and events
+    if (c->group_round[g]) cudaEventDestroy(c->group_round[g]);
+    if (c->group_imu_done[g]) cudaEventDestroy(c->group_imu_done[g]);
+    if (c->group_done[g]) cudaEventDestroy(c->group_done[g]);
+    if (c->group_imu[g]) cudaStreamDestroy(c->group_imu[g]);
+    if (c->group_stream[g]) cudaStreamDestroy(c->group_stream[g]);
+  }
   if (c->ev_round) cudaEventDestroy(c->ev_round);
   if (c->ev_imu) cudaEventDestroy(c->ev_imu);
   if (c->stream_imu) cudaStreamDestroy(c->stream_imu);
@@ -1400,20 +1425,25 @@ extern "C" int okb_shard_stats(okb_ctx* c, int win, double out[4]) {
   return OKB_OK;
 }
 
-// ---- optional event timing around solver kernels
-static void prof_begin(okb_ctx* c, int kind) {
-  if (!c->profile) return;
+// ---- optional event timing around solver kernels.  Returns the pair's index; `join` >= 0 is the index of the pair
+// whose span this one widens: the groups of a grouped solve each time a round's phase on their own stream, and the
+// phase's span over the whole batch runs from the earliest group's begin to the latest group's end.
+static int prof_begin(okb_ctx* c, int kind, cudaStream_t s, int join = -1) {
+  if (!c->profile) return -1;
   if (c->prof_used + 2 > c->prof_events.size()) {
     cudaEvent_t a, b;
     cudaEventCreate(&a); cudaEventCreate(&b);
     c->prof_events.push_back(a); c->prof_events.push_back(b);
   }
+  const int i = (int)c->prof_kind.size();
   c->prof_kind.push_back(kind);
-  cudaEventRecord(c->prof_events[c->prof_used], c->stream);
+  c->prof_join.push_back(join < 0 ? i : join);
+  cudaEventRecord(c->prof_events[c->prof_used], s);
+  return i;
 }
-static void prof_end(okb_ctx* c) {
+static void prof_end(okb_ctx* c, cudaStream_t s) {
   if (!c->profile) return;
-  cudaEventRecord(c->prof_events[c->prof_used + 1], c->stream);
+  cudaEventRecord(c->prof_events[c->prof_used + 1], s);
   c->prof_used += 2;
 }
 extern "C" int okb_profile_enable(okb_ctx* c, int on) {
@@ -1423,6 +1453,12 @@ extern "C" int okb_profile_enable(okb_ctx* c, int on) {
   c->profile = on != 0;
   c->prof_used = 0;
   c->prof_kind.clear();
+  c->prof_join.clear();
+  return OKB_OK;
+}
+extern "C" int okb_set_solve_groups(okb_ctx* c, int n) {
+  if (!c || n < 0 || n > okb_ctx::kMaxSolveGroups) return OKB_ERR_INVALID_ARG;
+  c->solve_groups = n;
   return OKB_OK;
 }
 extern "C" int okb_profile_read(okb_ctx* c, double out[6]) {
@@ -1430,14 +1466,24 @@ extern "C" int okb_profile_read(okb_ctx* c, double out[6]) {
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
   for (int i = 0; i < 6; ++i) out[i] = 0.0;
-  for (size_t i = 0; i < c->prof_kind.size(); ++i) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, c->prof_events[2 * i], c->prof_events[2 * i + 1]);
-    out[2 * c->prof_kind[i]] += ms;
-    out[2 * c->prof_kind[i] + 1] += 1.0;
+  const size_t n = c->prof_kind.size();
+  std::vector<float> lo(n, 0.f), hi(n, 0.f);     // per span: earliest begin, latest end, from the span's first begin
+  for (size_t i = 0; i < n; ++i) {
+    const size_t j = (size_t)c->prof_join[i];      // j <= i
+    float b = 0.f, e = 0.f;
+    cudaEventElapsedTime(&b, c->prof_events[2 * j], c->prof_events[2 * i]);
+    cudaEventElapsedTime(&e, c->prof_events[2 * j], c->prof_events[2 * i + 1]);
+    lo[j] = j == i ? b : std::min(lo[j], b);
+    hi[j] = j == i ? e : std::max(hi[j], e);
   }
+  for (size_t i = 0; i < n; ++i)
+    if ((size_t)c->prof_join[i] == i) {
+      out[2 * c->prof_kind[i]] += hi[i] - lo[i];
+      out[2 * c->prof_kind[i] + 1] += 1.0;
+    }
   c->prof_used = 0;
   c->prof_kind.clear();
+  c->prof_join.clear();
   return OKB_OK;
 }
 
@@ -1490,6 +1536,7 @@ extern "C" int okb_window_reset(okb_ctx* c, int first, int count) {
 struct RoundPlan {
   int max_chunks = 1, max_imu = 0, max_cx = 1, lm_wide = 0, acc_smem = 1, chol_smem = 1, solve_threads = S_THREADS, gxQ = 1, shard = 0, push_gx = 1;
   int lm_model = kDistAny, schur_wide = 0;      // (no padding bytes: the plan is compared bytewise as a graph key)
+  int groups = 1, unused = 0;                   // window groups of launch_rounds (the second int keeps the ints 8-byte aligned)
   size_t smA = 0, smS = 0, smQ = 0;
 };
 static int plan_rounds(okb_ctx* c, const int32_t* slots, int count, RoundPlan& P) {
@@ -1547,60 +1594,86 @@ static int plan_rounds(okb_ctx* c, const int32_t* slots, int count, RoundPlan& P
   P.gxQ = std::max(1, std::min((maxL + 127) / 128, (4 * c->sm_count + count - 1) / count));
   P.shard = c->shard_world > 1 ? 1 : 0;
   P.push_gx = std::max(1, std::min(16, c->sm_count / std::max(1, count)));
+  // Window groups: a batch of at least one window per SM runs as kMaxSolveGroups groups, each on its own stream and
+  // started behind the previous one, so that one group's k_solve (barrier / latency bound) and each kernel's drain share
+  // the SMs with another group's k_landmarks / k_schur.  Four groups were the fastest or within 1 % of it at 132, 264,
+  // 528 and 1056 windows (DESIGN §5); smaller batches were not measured and keep one group.  Every field above is the
+  // full batch's: each group launches the same kernel shapes over its share of the slot table.  Landmark-sharded windows
+  // spin on their peers inside their kernels and stay in one group.
+  int G = c->solve_groups;
+  if (G == 0) G = count >= c->sm_count ? okb_ctx::kMaxSolveGroups : 1;
+  P.groups = P.shard ? 1 : std::max(1, std::min({G, okb_ctx::kMaxSolveGroups, count}));
   return OKB_OK;
 }
 
 template <int MODEL>
-static void launch_landmarks(okb_ctx* c, int count, const RoundPlan& P) {
+static void launch_landmarks(okb_ctx* c, int count, const int32_t* tab, cudaStream_t s, const RoundPlan& P) {
   if (P.lm_wide) {     // one cluster of two CTAs per landmark tile
     cudaLaunchConfig_t cfg = {};
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.gridDim = dim3(2 * P.max_cx, count); cfg.blockDim = dim3(4 * L1_THREADS); cfg.dynamicSmemBytes = smemL_bytes(4);
-    cfg.stream = c->stream; cfg.attrs = attr; cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, k_landmarks<4, 2, MODEL>, (const WinDev*)c->d_wins, (const int32_t*)c->d_slot_tab);
+    cfg.stream = s; cfg.attrs = attr; cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, k_landmarks<4, 2, MODEL>, (const WinDev*)c->d_wins, tab);
   } else {
-    k_landmarks<2, 1, MODEL><<<dim3(P.max_cx, count), 2 * L1_THREADS, smemL_bytes(2), c->stream>>>(c->d_wins, c->d_slot_tab);
+    k_landmarks<2, 1, MODEL><<<dim3(P.max_cx, count), 2 * L1_THREADS, smemL_bytes(2), s>>>(c->d_wins, tab);
   }
 }
 
+// The rounds of one optimize, group by group (RoundPlan::groups): group g owns slot-table entries [count*g/G,
+// count*(g+1)/G) and runs its chain on group_stream[g], which starts behind group g-1's first k_landmarks; the groups
+// join `stream` at the end.  Group 0 is `stream` itself, so one group is the plain chain.
 static int launch_rounds(okb_ctx* c, int count, const okb_solve_options& opt, int rounds, const RoundPlan& P) {
-  for (int r = 0; r < rounds; ++r) {
-    const dim3 gridA(P.max_chunks, count);
-    static const bool imu_serial = getenv("OKB_IMU_SERIAL") != nullptr;     // diagnostics: k_imu on the main stream, ahead of the landmark kernels
-    if (P.max_imu > 0 && imu_serial) {
-      k_imu<<<dim3((P.max_imu + 32 / IMU_G - 1) / (32 / IMU_G), count), 32, smemI_bytes(), c->stream>>>(c->d_wins, c->d_slot_tab);
-      c->launches += 1;
-    } else if (P.max_imu > 0) {   // IMU terms only depend on the previous round's candidate: run beside the landmark kernels
-      cudaEventRecord(c->ev_round, c->stream);
-      cudaStreamWaitEvent(c->stream_imu, c->ev_round, 0);
-      k_imu<<<dim3((P.max_imu + 32 / IMU_G - 1) / (32 / IMU_G), count), 32, smemI_bytes(), c->stream_imu>>>(c->d_wins, c->d_slot_tab);
-      cudaEventRecord(c->ev_imu, c->stream_imu);
+  static const bool imu_serial = getenv("OKB_IMU_SERIAL") != nullptr;     // diagnostics: k_imu on the main stream, ahead of the landmark kernels
+  const int G = P.groups;
+  int span[2] = {-1, -1};      // this round's profiled pairs of group 0, which the other groups' pairs widen
+  for (int r = 0; r < rounds; ++r)
+    for (int g = 0; g < G; ++g) {
+      const int first = (int)((int64_t)count * g / G), n = (int)((int64_t)count * (g + 1) / G) - first;
+      const int32_t* tab = c->d_slot_tab + first;
+      cudaStream_t s = c->group_stream[g];
+      if (r == 0 && g > 0) cudaStreamWaitEvent(s, c->group_stagger[g - 1], 0);
+      const dim3 gridA(P.max_chunks, n);
+      if (P.max_imu > 0 && imu_serial) {
+        k_imu<<<dim3((P.max_imu + 32 / IMU_G - 1) / (32 / IMU_G), n), 32, smemI_bytes(), s>>>(c->d_wins, tab);
+        c->launches += 1;
+      } else if (P.max_imu > 0) {   // IMU terms only depend on the previous round's candidate: run beside the landmark kernels
+        cudaEventRecord(c->group_round[g], s);
+        cudaStreamWaitEvent(c->group_imu[g], c->group_round[g], 0);
+        k_imu<<<dim3((P.max_imu + 32 / IMU_G - 1) / (32 / IMU_G), n), 32, smemI_bytes(), c->group_imu[g]>>>(c->d_wins, tab);
+        cudaEventRecord(c->group_imu_done[g], c->group_imu[g]);
+        c->launches += 1;
+      }
+      const int p0 = prof_begin(c, 0, s, g ? span[0] : -1);
+      if (g == 0) span[0] = p0;
+      switch (P.lm_model) {
+        case OKB_DIST_NONE: launch_landmarks<OKB_DIST_NONE>(c, n, tab, s, P); break;
+        case OKB_DIST_RADTAN: launch_landmarks<OKB_DIST_RADTAN>(c, n, tab, s, P); break;
+        case OKB_DIST_EQUIDISTANT: launch_landmarks<OKB_DIST_EQUIDISTANT>(c, n, tab, s, P); break;
+        case OKB_DIST_RADTAN8: launch_landmarks<OKB_DIST_RADTAN8>(c, n, tab, s, P); break;
+        default: launch_landmarks<kDistAny>(c, n, tab, s, P); break;
+      }
+      if (r == 0 && g + 1 < G) cudaEventRecord(c->group_stagger[g], s);
+      if (P.schur_wide) k_schur<512><<<gridA, 512, P.smA, s>>>(c->d_wins, tab, P.acc_smem, opt.max_iterations);
+      else k_schur<256><<<gridA, 256, P.smA, s>>>(c->d_wins, tab, P.acc_smem, opt.max_iterations);
+      if (P.shard) {    // chunk reduction fused with the push half of the all-reduce over peer memory
+        k_shard_push<<<dim3(P.push_gx, n), 256, 0, s>>>(c->d_wins, tab);
+        c->launches += 1;
+      } else if (P.max_chunks > 1) { k_reduce_partials<<<dim3(8, n), 256, 0, s>>>(c->d_wins, tab); c->launches += 1; }
+      prof_end(c, s);
+      c->launches += 2;
+      if (P.max_imu > 0 && !imu_serial) cudaStreamWaitEvent(s, c->group_imu_done[g], 0);
+      const int p1 = prof_begin(c, 1, s, g ? span[1] : -1);
+      if (g == 0) span[1] = p1;
+      if (P.solve_threads == 512) k_solve<512><<<n, 512, P.smS, s>>>(c->d_wins, tab, opt, P.chol_smem);
+      else k_solve<S_THREADS><<<n, S_THREADS, P.smS, s>>>(c->d_wins, tab, opt, P.chol_smem);
+      prof_end(c, s);
       c->launches += 1;
     }
-    prof_begin(c, 0);
-    switch (P.lm_model) {
-      case OKB_DIST_NONE: launch_landmarks<OKB_DIST_NONE>(c, count, P); break;
-      case OKB_DIST_RADTAN: launch_landmarks<OKB_DIST_RADTAN>(c, count, P); break;
-      case OKB_DIST_EQUIDISTANT: launch_landmarks<OKB_DIST_EQUIDISTANT>(c, count, P); break;
-      case OKB_DIST_RADTAN8: launch_landmarks<OKB_DIST_RADTAN8>(c, count, P); break;
-      default: launch_landmarks<kDistAny>(c, count, P); break;
-    }
-    if (P.schur_wide) k_schur<512><<<gridA, 512, P.smA, c->stream>>>(c->d_wins, c->d_slot_tab, P.acc_smem, opt.max_iterations);
-    else k_schur<256><<<gridA, 256, P.smA, c->stream>>>(c->d_wins, c->d_slot_tab, P.acc_smem, opt.max_iterations);
-    if (P.shard) {    // chunk reduction fused with the push half of the all-reduce over peer memory
-      k_shard_push<<<dim3(P.push_gx, count), 256, 0, c->stream>>>(c->d_wins, c->d_slot_tab);
-      c->launches += 1;
-    } else if (P.max_chunks > 1) { k_reduce_partials<<<dim3(8, count), 256, 0, c->stream>>>(c->d_wins, c->d_slot_tab); c->launches += 1; }
-    prof_end(c);
-    c->launches += 2;
-    if (P.max_imu > 0 && !imu_serial) cudaStreamWaitEvent(c->stream, c->ev_imu, 0);
-    prof_begin(c, 1);
-    if (P.solve_threads == 512) k_solve<512><<<count, 512, P.smS, c->stream>>>(c->d_wins, c->d_slot_tab, opt, P.chol_smem);
-    else k_solve<S_THREADS><<<count, S_THREADS, P.smS, c->stream>>>(c->d_wins, c->d_slot_tab, opt, P.chol_smem);
-    prof_end(c);
-    c->launches += 1;
+  for (int g = 1; g < G; ++g) {
+    cudaEventRecord(c->group_done[g], c->group_stream[g]);
+    cudaStreamWaitEvent(c->stream, c->group_done[g], 0);
   }
   OKB_CUDA(c, cudaGetLastError());
   return OKB_OK;
@@ -1608,9 +1681,9 @@ static int launch_rounds(okb_ctx* c, int count, const okb_solve_options& opt, in
 
 // post-solve landmark quality (Estimator.cpp:880-894)
 static int launch_quality(okb_ctx* c, int count, const RoundPlan& P) {
-  prof_begin(c, 2);
+  prof_begin(c, 2, c->stream);
   k_quality<<<dim3(P.gxQ, count), 128, P.smQ, c->stream>>>(c->d_wins, c->d_slot_tab);
-  prof_end(c);
+  prof_end(c, c->stream);
   c->launches += 1;
   OKB_CUDA(c, cudaGetLastError());
   return OKB_OK;
