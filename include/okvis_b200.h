@@ -30,6 +30,8 @@
  *                                okvis_frontend/include/okvis/VioKeyframeWindowMatchingAlgorithm.hpp:246-254
  *   okb_track_3d2d_batch      <- the 3D-2D rounds of Frontend::matchToKeyframes / matchToLastFrame (Frontend.cpp:389-411,
  *                                484-494): VioKeyframeWindowMatchingAlgorithm::doSetup + DenseMatcher::match + setBestMatch
+ *   okb_stereo_init_batch     <- the 2D-2D match of Frontend::matchStereo (Frontend.cpp:521-546): doSetup + DenseMatcher::
+ *                                match + setBestMatch's device half (stereoTriangulate, getUncertainty)
  *   okb_detect_describe       <- okvis::Frontend::detectAndDescribe    okvis_frontend/src/Frontend.cpp:92-114
  *                                (Frame::detect / Frame::describe      okvis_cv/include/okvis/implementation/Frame.hpp:109-156)
  */
@@ -685,6 +687,42 @@ typedef struct okb_track_job {
  * those windows only, with one H2D copy of the job table and one D2H copy of the results, and returns when they are
  * back.  Later solver calls on those windows are ordered after it.  n_jobs == 0 is a no-op. */
 int okb_track_3d2d_batch(okb_ctx* ctx, int n_jobs, const okb_track_job* jobs);
+
+/* ---- stereo landmark initialisation (Frontend::matchStereo, Frontend.cpp:521-572) ------------------------------------
+ * One job = one VioKeyframeWindowMatchingAlgorithm Match2D2D match as matchStereo issues it: setFrames(mfId, mfId, cam_a,
+ * cam_b) with usePoseUncertainty = false, so frames A and B are the job's frame -- one feature slot, two cameras. */
+typedef struct okb_stereo_match {   /* one setBestMatch that reached the landmark bookkeeping */
+  int32_t kp_a, kp_b;               /* keypoints of (frame, cam_a) / (frame, cam_b) */
+  int32_t lm_slot_a, lm_slot_b;     /* their landmark slots in the store (in the graph), -1: none; at most one is set */
+  int32_t can_be_initialized, _pad; /* canBeInitialized after stereoTriangulate and getUncertainty */
+  double hp_W[4];                   /* T_WCa * hP_Ca, not normalised (what addLandmark / setLandmark receive) */
+} okb_stereo_match;
+typedef struct okb_stereo_job {
+  int32_t win, pose, feat_slot, cam_a, cam_b;  /* window slot, the frame's position (T_WS), its feature slot, cameras */
+  float threshold;                             /* briskMatchingThreshold_ (60) */
+  int32_t num_best, _pad;                      /* top-k list length (Frontend's matcher: 4) */
+  okb_stereo_match* out; int32_t out_cap;      /* out_cap >= keypoints of (feat_slot, cam_b) */
+  int32_t* n_out;
+} okb_stereo_job;
+/* Per job, following the reference line by line and reading only the resident window and its store:
+ *   setFrames (VioKeyframeWindowMatchingAlgorithm.cpp:76-111): T_WCa = T_WS T_SCa, T_WCb = T_WS T_SCb,
+ *     T_CaCb = T_WCa^-1 T_WCb;
+ *   doSetup, 2D-2D branch (:124-146, 216-232, 256-274): UOplus = diag(4e-8 I3, 1e-8 I3), resetFrames' prior H_
+ *     (ProbabilisticStereoTriangulator.cpp:117-159), ray sigmas, backProject of every keypoint, and keypoints skipped
+ *     whose slot names an initialised landmark of the graph;
+ *   DenseMatcher::match with verifyMatch's 2D-2D gate (the matcher kernels of okb_hamming_match_gated);
+ *   setBestMatch, 2D-2D branch (:370-481), for every winner below the threshold in ascending B: nothing if both
+ *     keypoints name a landmark, else stereoTriangulate (:168-227) and, unless the rays are parallel, getUncertainty
+ *     (:253-355), which decides canBeInitialized.
+ * The records come back in that order; the caller applies them (addLandmark / setLandmark / setLandmarkInitialized /
+ * addObservation, and new landmark ids).  The call changes nothing in the window, its store or its flags.  Every job is
+ * checked on the host before any device work (uploaded window, store reserved, the feature slot present for both
+ * cameras, cam_a != cam_b in range, pose in range, num_best <= 8, out_cap, one descriptor length per call, a window
+ * listed twice): the first failure returns OKB_ERR_INVALID_ARG and names the job in okb_last_error.  A landmark-sharded
+ * context returns OKB_ERR_UNSUPPORTED.  Pending edits of the job windows are committed first; the call runs on the
+ * transfer stream after the solver work already launched on those windows, with one H2D copy of the job table and one
+ * D2H copy of the results, and returns when they are back.  n_jobs == 0 is a no-op. */
+int okb_stereo_init_batch(okb_ctx* ctx, int n_jobs, const okb_stereo_job* jobs);
 
 #ifdef __cplusplus
 }

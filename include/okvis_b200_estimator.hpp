@@ -704,19 +704,25 @@ class Estimator {
     okb_track_job job{};
   };
   bool planTrack(uint64_t currentFrameId, const std::vector<uint64_t>& frameA, float threshold, TrackPlan& p) {
+    std::vector<TrackRound> rounds;
+    for (uint64_t a : frameA)
+      for (size_t im = 0; im < cameras_.size(); ++im) rounds.push_back(TrackRound{a, im, im});
+    return planTrackRounds(currentFrameId, rounds, threshold, p);
+  }
+  // the same for an explicit round list (frame A, camera A, camera B); rounds without features on either side are dropped
+  struct TrackRound { uint64_t frameA; size_t camA, camB; };
+  bool planTrackRounds(uint64_t currentFrameId, const std::vector<TrackRound>& rounds, float threshold, TrackPlan& p) {
     auto fb = featSlot_.find(currentFrameId);
     if (fb == featSlot_.end()) return false;
     size_t sumA = 0, sumB = 0;
     const auto& B = feats_.at(currentFrameId);
-    for (uint64_t a : frameA) {
-      auto fa = featSlot_.find(a);
+    for (const TrackRound& r : rounds) {
+      auto fa = featSlot_.find(r.frameA);
       if (fa == featSlot_.end()) continue;
-      const auto& A = feats_.at(a);
-      for (size_t im = 0; im < cameras_.size(); ++im) {
-        if (A[im].kp.empty() || B[im].kp.empty()) continue;
-        p.rounds.push_back(okb_track_round{fa->second, (int32_t)im, (int32_t)im, 0});
-        sumA += A[im].kp.size(); sumB += B[im].kp.size();
-      }
+      const auto& A = feats_.at(r.frameA);
+      if (A[r.camA].kp.empty() || B[r.camB].kp.empty()) continue;
+      p.rounds.push_back(okb_track_round{fa->second, (int32_t)r.camA, (int32_t)r.camB, 0});
+      sumA += A[r.camA].kp.size(); sumB += B[r.camB].kp.size();
     }
     if (p.rounds.empty()) return false;
     p.frameB = currentFrameId;
@@ -747,6 +753,84 @@ class Estimator {
     }
     for (int32_t m : p.numMatches) numMatches += m;
     for (int32_t u : p.numUncertain) numUncertainMatches += u;
+  }
+
+  // One okb_stereo_init_batch job of this session: the 2D-2D match of matchStereo between cameras im0 and im1 of the
+  // current frame (setFrames(mfId, mfId, im0, im1)).  finishStereo applies the records as setBestMatch does.
+  struct StereoPlan {
+    uint64_t frame = 0;
+    size_t im0 = 0, im1 = 0;
+    std::vector<okb_stereo_match> out;
+    int32_t nOut = 0;
+    okb_stereo_job job{};
+  };
+  // Throws unless, in the frame, "the keypoint has a landmark id" is "its store slot names a landmark of the graph":
+  // the device's view of setBestMatch's lmIdA / lmIdB.
+  void checkFrameIds(uint64_t frameId) const {
+    auto f = feats_.find(frameId);
+    if (f == feats_.end()) return;
+    for (size_t c = 0; c < f->second.size(); ++c)
+      for (uint64_t id : f->second[c].lm)
+        if (id != 0 && !landmarks_.count(id))
+          throw std::runtime_error("okvis_b200: matchStereo: a keypoint of frame " + std::to_string(frameId) +
+                                   " names landmark " + std::to_string(id) + ", which is not in the graph");
+  }
+  bool planStereo(uint64_t frameId, size_t im0, size_t im1, float threshold, StereoPlan& p) {
+    auto fs = featSlot_.find(frameId);
+    if (fs == featSlot_.end()) return false;
+    const auto& F = feats_.at(frameId);
+    if (F[im0].kp.empty() || F[im1].kp.empty()) return false;
+    p.frame = frameId; p.im0 = im0; p.im1 = im1;
+    p.out.resize(F[im1].kp.size());
+    okb_stereo_job& j = p.job;
+    j.win = slot_; j.pose = (int32_t)posePos(frameId); j.feat_slot = fs->second; j.cam_a = (int32_t)im0; j.cam_b = (int32_t)im1;
+    j.threshold = threshold; j.num_best = 4;
+    j.out = p.out.data(); j.out_cap = (int32_t)p.out.size(); j.n_out = &p.nOut;
+    return true;
+  }
+  // the host half of setBestMatch's 2D-2D branch (VioKeyframeWindowMatchingAlgorithm.cpp:396-480), record by record
+  template <class NewId>
+  void finishStereo(const StereoPlan& p, const NewId& newId) {
+    auto& F = feats_.at(p.frame);
+    for (int i = 0; i < p.nOut; ++i) {
+      const okb_stereo_match& r = p.out[i];
+      const uint64_t idA = F[p.im0].lm[r.kp_a], idB = F[p.im1].lm[r.kp_b];
+      if ((idA != 0) != (r.lm_slot_a >= 0) || (idB != 0) != (r.lm_slot_b >= 0) ||
+          (idA && lmSlot_.at(idA) != (uint32_t)r.lm_slot_a) || (idB && lmSlot_.at(idB) != (uint32_t)r.lm_slot_b))
+        throw std::runtime_error("okvis_b200: matchStereo: the store and the frame's landmark ids disagree");
+      const bool cbi = r.can_be_initialized != 0;
+      const Vec4 hp{{r.hp_W[0], r.hp_W[1], r.hp_W[2], r.hp_W[3]}};
+      const bool insertA = idA == 0, insertB = idB == 0;
+      // both named: the device returns no record; both new: a new id; else the named one (in the graph, checkFrameIds)
+      const uint64_t lmId = (insertA && insertB) ? newId() : (insertA ? idB : idA);
+      if (insertA && insertB) {
+        addLandmark(lmId, hp);
+        setLandmarkInitialized(lmId, cbi);
+      } else if (cbi) {
+        setLandmarkInitialized(lmId, true);
+        setLandmark(lmId, hp);
+      }
+      if (insertA) observeStereo(p.frame, p.im0, r.kp_a, lmId);
+      if (insertB) observeStereo(p.frame, p.im1, r.kp_b, lmId);
+      if (cbi) setLandmark(lmId, hp);
+    }
+  }
+  void observeStereo(uint64_t frameId, size_t cam, size_t k, uint64_t lmId) {
+    FrameFeatures& f = feats_.at(frameId)[cam];
+    f.lm[k] = lmId;
+    const double z[2] = {f.kp[k].x, f.kp[k].y};
+    if (!addObservation(lmId, frameId, cam, k, z, f.kp[k].size))
+      setStoreLandmark(frameId, cam, k, lmId, false);      // refused: the keypoint names it, no observation
+  }
+  // matchStereo's last loop (Frontend.cpp:563-571): every keypoint still without an id gets one, in (camera, keypoint)
+  // order.  Frame bookkeeping only: the store keeps -1 for them, as no landmark of the graph has that id.
+  template <class NewId>
+  void nameRemainingKeypoints(uint64_t frameId, const NewId& newId) {
+    auto f = feats_.find(frameId);
+    if (f == feats_.end()) return;
+    for (auto& cam : f->second)
+      for (auto& id : cam.lm)
+        if (id == 0) id = newId();
   }
 
   void eraseObsHost(std::map<uint64_t, Obs>::iterator it) {

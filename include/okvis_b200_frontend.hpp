@@ -13,11 +13,15 @@
 // Frontend::matchToKeyframes3D2D / matchToLastFrame3D2D run the 3D-2D rounds of matchToKeyframes (:389-411) and
 // matchToLastFrame (:484-494) on the device (okb_track_3d2d_batch on the window's feature store, filled by
 // Estimator::setFrameFeatures) and apply them through Estimator::addObservation; the group forms make one call for many
-// sessions of an EstimatorGroup.  2D-2D matching, triangulation, RANSAC and the keyframe decision stay on the OKVIS side
-// with the MultiFrame (SURVEY.md 8f rows 2 and 4).
+// sessions of an EstimatorGroup.  Frontend::matchStereo creates the stereo landmarks of the current frame
+// (Frontend.cpp:521-572): per overlapping camera pair the 2D-2D match on the device (okb_stereo_init_batch: backProject,
+// gated match, stereoTriangulate, getUncertainty), setBestMatch's landmark bookkeeping on the host, then the pair's
+// same-frame 3D-2D passes (okb_track_3d2d_batch).  The 2D-2D rounds of matchToKeyframes / matchToLastFrame, RANSAC and
+// the keyframe decision stay on the OKVIS side with the MultiFrame (SURVEY.md 8f rows 2 and 4).
 #pragma once
 #include <cmath>
 #include <cstdint>
+#include <functional>
 #include <limits>
 #include <stdexcept>
 #include <string>
@@ -134,7 +138,73 @@ class Frontend {
     return trackGroup(&group, sessions, currentFrameIds, false);
   }
 
+  // ---- stereo landmark initialisation of the current frame (device: okb_stereo_init_batch + okb_track_3d2d_batch)
+  // Frontend::matchStereo (Frontend.cpp:521-572).  overlap[i][j]: NCameraSystem::hasOverlap(i, j).  For every pair
+  // im0 < im1 that overlaps: the 2D-2D match, its records applied as setBestMatch does (new landmarks take newId() in the
+  // order IdProvider::newId() would hand them out), then the 3D-2D passes (frame, im0 -> im1) and (frame, im1 -> im0).
+  // Finally every keypoint of the frame still without an id gets newId(), in (camera, keypoint) order -- frame
+  // bookkeeping only, reported by TrackResult::landmarkIds / Estimator::frameLandmarkIds.  Throws if a keypoint of the
+  // frame names a landmark that is not in the graph.  The counts are those of the 3D-2D passes.
+  TrackResult matchStereo(Estimator& estimator, uint64_t frameId, const std::function<uint64_t()>& newId,
+                          const std::vector<std::vector<bool>>& overlap) {
+    return stereoGroup(nullptr, {&estimator}, {frameId}, {newId}, overlap)[0];
+  }
+  // The same for sessions of one EstimatorGroup: one okb_stereo_init_batch and one okb_track_3d2d_batch per camera
+  // pair for all of them; each session's records are applied in list order with that session's newId.
+  std::vector<TrackResult> matchStereo(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                       const std::vector<std::function<uint64_t()>>& newIds, const std::vector<std::vector<bool>>& overlap) {
+    return stereoGroup(&group, sessions, frameIds, newIds, overlap);
+  }
+
  private:
+  std::vector<TrackResult> stereoGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                       const std::vector<std::function<uint64_t()>>& newIds, const std::vector<std::vector<bool>>& overlap) {
+    const size_t n = sessions.size();
+    if (frameIds.size() != n || newIds.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one id source per session");
+    if (group) group->validate(sessions);
+    if (n == 0) return {};
+    okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
+    const size_t C = sessions[0]->cameras_.size();
+    if (overlap.size() < C) throw std::invalid_argument("okvis_b200: matchStereo: overlap must be numCameras x numCameras");
+    for (size_t i = 0; i < n; ++i) {
+      if (sessions[i]->cameras_.size() != C) throw std::invalid_argument("okvis_b200: matchStereo: sessions with different camera counts");
+      sessions[i]->checkFrameIds(frameIds[i]);
+    }
+    std::vector<TrackResult> out(n);
+    for (size_t im0 = 0; im0 < C; ++im0)
+      for (size_t im1 = im0 + 1; im1 < C; ++im1) {
+        if (overlap[im0].size() < C || !overlap[im0][im1]) continue;
+        // the 2D-2D match (:532-546)
+        std::vector<Estimator::StereoPlan> sp(n);
+        std::vector<char> hs(n, 0);
+        std::vector<okb_stereo_job> sj;
+        for (size_t i = 0; i < n; ++i) {
+          hs[i] = sessions[i]->planStereo(frameIds[i], im0, im1, (float)briskMatchingThreshold_, sp[i]);
+          if (hs[i]) sj.push_back(sp[i].job);
+        }
+        if (!sj.empty() && okb_stereo_init_batch(ctx, (int)sj.size(), sj.data()) != OKB_OK)
+          throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+        for (size_t i = 0; i < n; ++i) if (hs[i]) sessions[i]->finishStereo(sp[i], newIds[i]);
+        // the 3D-2D and 2D-3D passes of the same pair (:547-553)
+        std::vector<Estimator::TrackPlan> tp(n);
+        std::vector<char> ht(n, 0);
+        std::vector<okb_track_job> tj;
+        for (size_t i = 0; i < n; ++i) {
+          const std::vector<Estimator::TrackRound> rounds{{frameIds[i], im0, im1}, {frameIds[i], im1, im0}};
+          ht[i] = sessions[i]->planTrackRounds(frameIds[i], rounds, (float)briskMatchingThreshold_, tp[i]);
+          if (ht[i]) tj.push_back(tp[i].job);
+        }
+        if (!tj.empty() && okb_track_3d2d_batch(ctx, (int)tj.size(), tj.data()) != OKB_OK)
+          throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+        for (size_t i = 0; i < n; ++i) if (ht[i]) sessions[i]->finishTrack(tp[i], out[i].numMatches, out[i].numUncertainMatches);
+      }
+    for (size_t i = 0; i < n; ++i) {
+      sessions[i]->nameRemainingKeypoints(frameIds[i], newIds[i]);
+      for (size_t c = 0; c < C; ++c) out[i].landmarkIds.push_back(sessions[i]->frameLandmarkIds(frameIds[i], c));
+    }
+    return out;
+  }
+
   std::vector<TrackResult> trackGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                       bool keyframes) {
     if (sessions.size() != frameIds.size()) throw std::invalid_argument("okvis_b200: one current frame id per session");

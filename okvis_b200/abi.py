@@ -124,6 +124,12 @@ class TrackJob(C.Structure):
                 ("uninit_cap", C.c_int32), ("n_uninit", C.POINTER(C.c_int32))]
 
 
+class StereoJob(C.Structure):
+    _fields_ = [("win", C.c_int32), ("pose", C.c_int32), ("feat_slot", C.c_int32), ("cam_a", C.c_int32), ("cam_b", C.c_int32),
+                ("threshold", C.c_float), ("num_best", C.c_int32), ("_pad", C.c_int32), ("out", C.c_void_p), ("out_cap", C.c_int32),
+                ("n_out", C.POINTER(C.c_int32))]
+
+
 class PropagateJob(C.Structure):
     _fields_ = [("params", C.POINTER(ImuParams)), ("samples", C.c_void_p), ("n_samples", C.c_int32), ("_pad", C.c_int32),
                 ("t0_ns", C.c_int64), ("t1_ns", C.c_int64), ("pose", c_double_p), ("speed_bias", c_double_p),
@@ -177,6 +183,8 @@ relpose_dtype = np.dtype([("ext0", "<u4"), ("ext1", "<u4"), ("sqrt_info", "<f8",
 keypoint_dtype = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"),
                            ("octave", "<i4")], align=True)
 pair_dtype = np.dtype([("index_a", "<i4"), ("distance", "<f4")], align=True)
+stereo_match_dtype = np.dtype([("kp_a", "<i4"), ("kp_b", "<i4"), ("lm_slot_a", "<i4"), ("lm_slot_b", "<i4"),
+                               ("can_be_initialized", "<i4"), ("_pad", "<i4"), ("hp_W", "<f8", (4,))], align=True)
 track_assoc_dtype = np.dtype([("round", "<i4"), ("cam_b", "<i4"), ("kp_b", "<i4"), ("lm_slot", "<i4"), ("uncertain", "<i4"),
                               ("_pad", "<i4")], align=True)
 

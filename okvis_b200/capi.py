@@ -613,6 +613,22 @@ class Context:
         return [dict(assoc=o["assoc"][:o["n_assoc"].value].copy(), num_matches=o["num_matches"][:n].copy(),
                      num_uncertain=o["num_uncertain"][:n].copy(), uninit=o["uninit"][:o["n_uninit"].value].copy()) for o, n in outs]
 
+    def stereo_init_batch(self, jobs):
+        """okb_stereo_init_batch.  jobs: dicts with win, pose, feat_slot, cam_a, cam_b and optionally threshold (60) and
+        num_best (4).  Returns one stereo_match_dtype array per job, in the reference's setBestMatch order."""
+        arr = (abi.StereoJob * max(len(jobs), 1))()
+        outs = []
+        for i, j in enumerate(jobs):
+            cap = max(getattr(self, "_feat", {}).get(int(j["win"]), 0), 1)
+            o = dict(out=np.zeros(cap, abi.stereo_match_dtype), n=C.c_int32(0))
+            t = arr[i]
+            t.win, t.pose, t.feat_slot, t.cam_a, t.cam_b = (int(j[k]) for k in ("win", "pose", "feat_slot", "cam_a", "cam_b"))
+            t.threshold, t.num_best = float(j.get("threshold", 60.0)), int(j.get("num_best", 4))
+            t.out, t.out_cap, t.n_out = o["out"].ctypes.data, int(j.get("out_cap", cap)), C.pointer(o["n"])
+            outs.append(o)
+        self._check(lib().okb_stereo_init_batch(self._h, len(jobs), arr))
+        return [o["out"][:o["n"].value].copy() for o in outs]
+
     def hamming_match_batch(self, jobs, desc_bytes):
         """okb_hamming_match_batch over `jobs`: make_match_job results, or dicts of its keyword arguments.  Returns one
         dict(topk, pairs) per job, like hamming_match / hamming_match_gated."""

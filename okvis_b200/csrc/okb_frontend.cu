@@ -173,6 +173,11 @@ struct okb_frontend_state {
   uint8_t* track_scratch = nullptr;
   size_t track_scratch_cap = 0;
   std::mutex track_mtx;
+  // okb_stereo_init_batch (on c->stream_xfer, under stereo_mtx), the same kind of buffers
+  MatchIO stereo_io;
+  uint8_t* stereo_scratch = nullptr;
+  size_t stereo_scratch_cap = 0;
+  std::mutex stereo_mtx;
 };
 
 void okb_frontend_release(okb_ctx* c) {
@@ -182,6 +187,8 @@ void okb_frontend_release(okb_ctx* c) {
   F->batch_match.release();
   F->track_io.release();
   cudaFree(F->track_scratch);
+  F->stereo_io.release();
+  cudaFree(F->stereo_scratch);
   F->batch_det.release();
   if (F->batch_stream) cudaStreamDestroy(F->batch_stream);
   for (auto& s : F->slots) {
@@ -1023,9 +1030,11 @@ __device__ __forceinline__ bool gate_reproj_err(const CamIntr& cam, int W, int H
   err = d0 * (w * d0) + d1 * (w * d1);
   return true;
 }
-__device__ bool gate_verify(const GateDev& g, int a, int b) {
-  if (g.mode == OKB_GATE_2D2D) {
-    // stereoTriangulate (ProbabilisticStereoTriangulator.cpp:168-227) -> triangulateFast (stereo_triangulation.cpp:51-125)
+// stereoTriangulate (ProbabilisticStereoTriangulator.cpp:168-227) -> triangulateFast (stereo_triangulation.cpp:51-125):
+// the return value is stereoTriangulate's; hpA and isParallel are set whenever it returns true.  Used by the 2D-2D gate
+// and by setBestMatch's re-triangulation in k_stereo_apply.
+__device__ __forceinline__ bool stereo_triangulate(const GateDev& g, int a, int b, double* hpA, bool& isParallel) {
+  {
     const double* ba = g.bearing_a + 3 * a;
     const double* bb = g.bearing_b + 3 * b;
     double e1[3], e2[3], eb[3];
@@ -1043,8 +1052,8 @@ __device__ bool gate_verify(const GateDev& g, int a, int b) {
     const double A11 = -(e2[0] * e2[0] + e2[1] * e2[1] + e2[2] * e2[2]);
     if (A10 < 0.0) { A10 = -A10; A01 = -A01; }
     const double det = A00 * A11 - A01 * A10;
-    double hpA[4];
     if (!(fabs(det) > 1.0e-6)) {
+      isParallel = true;
       double c[3];
       cross3(e1, e2, c);
       if (!(sqrt(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]) < 6 * sigma)) return false;
@@ -1052,6 +1061,7 @@ __device__ bool gate_verify(const GateDev& g, int a, int b) {
       const double n = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2] + v[3] * v[3]);
       hpA[0] = v[0] / n; hpA[1] = v[1] / n; hpA[2] = v[2] / n; hpA[3] = v[3] / n;
     } else {
+      isParallel = false;
       const double i00 = A11 / det, i01 = -A01 / det, i10 = -A10 / det, i11 = A00 / det;
       const double l0 = i00 * b0 + i01 * b1, l1 = i10 * b0 + i11 * b1;
       double mid[3], err[3], diff[3];
@@ -1081,6 +1091,13 @@ __device__ bool gate_verify(const GateDev& g, int a, int b) {
     hpB[3] = hpA[3];
     if (!gate_reproj_err(g.cam_b, g.wb, g.hb, g.kp_b + 2 * b, g.kp_size_b[b], hpB, errB)) return false;
     return !(errA > 4.0 || errB > 4.0);
+  }
+}
+__device__ bool gate_verify(const GateDev& g, int a, int b) {
+  if (g.mode == OKB_GATE_2D2D) {
+    double hpA[4];
+    bool isParallel;
+    return stereo_triangulate(g, a, b, hpA, isParallel);
   }
   // 3D-2D (VioKeyframeWindowMatchingAlgorithm.cpp:317-338)
   const double sd = 0.8 * g.kp_size_b[b] / 12.0;
@@ -2016,6 +2033,469 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
       o.uncertain = (int32_t)(as[k].x >> 31); o.lm_slot = (int32_t)as[k].y; o._pad = 0;
     }
     if (nu) std::memcpy(j.uninit, h + o_un[i], 4 * (size_t)nu);
+  }
+  return OKB_OK;
+}
+
+// =================================================================================================
+// Stereo landmark initialisation (okb_stereo_init_batch): the 2D-2D match of Frontend::matchStereo
+// (okvis_frontend/src/Frontend.cpp:521-546) on the window's feature store, frame A = frame B = the job's frame:
+//   k_stereo_setup  setFrames (VioKeyframeWindowMatchingAlgorithm.cpp:76-111) and doSetup's 2D-2D branch (:124-146,
+//                   216-232, 256-274): backProject, ray sigmas and skip flags per keypoint, in parallel over (job, image,
+//                   keypoint); one thread per job also writes the gate's geometry and resetFrames' prior H_
+//   k_hamming_topk<NW, true> + k_assign   DenseMatcher::match over verifyMatch's 2D-2D gate (unchanged)
+//   k_stereo_apply  setBestMatch's 2D-2D branch (:370-481) up to the landmark bookkeeping: a thread per B winner for
+//                   stereoTriangulate and getUncertainty's residuals, a warp per remaining 9x9 rank test, a CTA scan for
+//                   the ascending-B record list
+// The call writes nothing but its scratch and its results: the caller applies them.
+// =================================================================================================
+namespace {
+constexpr int kGeo = 7 + 9 + 3 + 36;     // per job: T_CaCb [t, q], C_WCa, r_WCa, H_ (6x6 pose block of resetFrames' prior)
+constexpr int kUJ = 6 + 12 + 6;          // per B keypoint: J_hpA_min 2x3, J_TB_min 2x6, J_hpB_min 2x3
+
+struct StereoJobDev {
+  const WinDev* W;
+  int pose, feat, cam_a, cam_b;
+  float threshold;
+  int _pad;
+  double* geo;              // [kGeo]
+  double* uj;               // [nB][kUJ] Jacobians of the winners that reach the rank test
+  int* n_out;
+  okb_stereo_match* out;    // [nB]
+};
+
+// okvis::kinematics::Transformation: (r, q) with q normalised on construction, C = q.toRotationMatrix()
+struct XfQ { double r[3], q[4], C[9]; };
+__device__ void xfq_make(const double* r, const double* q, XfQ& o) {
+  const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) o.q[k] = q[k] / n;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) o.r[k] = r[k];
+  q2R(o.q, o.C);
+}
+__device__ void xfq_mul(const XfQ& a, const XfQ& b, XfQ& o) {      // Transformation(C_a r_b + r_a, q_a q_b)
+  double r[3], q[4];
+  mat3vec(a.C, b.r, r);
+  r[0] += a.r[0]; r[1] += a.r[1]; r[2] += a.r[2];
+  qmul(a.q, b.q, q);
+  xfq_make(r, q, o);
+}
+__device__ void xfq_inv(const XfQ& a, XfQ& o) {                    // Transformation(-(C^T r), q.inverse())
+  double r[3], q[4];
+  mat3Tvec(a.C, a.r, r);
+  r[0] = -r[0]; r[1] = -r[1]; r[2] = -r[2];
+  const double n2 = a.q[0] * a.q[0] + a.q[1] * a.q[1] + a.q[2] * a.q[2] + a.q[3] * a.q[3];
+  q[0] = -a.q[0] / n2; q[1] = -a.q[1] / n2; q[2] = -a.q[2] / n2; q[3] = a.q[3] / n2;
+  xfq_make(r, q, o);
+}
+
+__global__ void __launch_bounds__(TK_T) k_stereo_setup(const StereoJobDev* __restrict__ jobs, MatchJobDev* tab) {
+  const StereoJobDev& J = jobs[blockIdx.y];
+  MatchJobDev& M = tab[blockIdx.y];
+  const WinDev& W = *J.W;
+  const FeatStore& F = *W.feat;
+  const int side = blockIdx.z;
+  if (blockIdx.x == 0 && side == 0 && threadIdx.x == 0) {
+    // setFrames: T_WCa = T_WS T_SCa, T_WCb = T_WS T_SCb, T_CaCb = T_WCa^-1 T_WCb
+    const double* P = W.pose + 7 * (size_t)J.pose;
+    const double* Ea = W.ext + 7 * (size_t)J.cam_a;
+    const double* Eb = W.ext + 7 * (size_t)J.cam_b;
+    XfQ T_WS, T_SCa, T_SCb, T_WCa, T_WCb, T_CaW, T_AB;
+    xfq_make(P, P + 3, T_WS);
+    xfq_make(Ea, Ea + 3, T_SCa);
+    xfq_make(Eb, Eb + 3, T_SCb);
+    xfq_mul(T_WS, T_SCa, T_WCa);
+    xfq_mul(T_WS, T_SCb, T_WCb);
+    xfq_inv(T_WCa, T_CaW);
+    xfq_mul(T_CaW, T_WCb, T_AB);
+    GateDev& g = M.gate;
+    cam_load(W.cams[J.cam_a], g.cam_a);
+    cam_load(W.cams[J.cam_b], g.cam_b);
+    g.wa = W.cams[J.cam_a].width; g.ha = W.cams[J.cam_a].height;
+    g.wb = W.cams[J.cam_b].width; g.hb = W.cams[J.cam_b].height;
+    for (int k = 0; k < 9; ++k) g.R_AB[k] = T_AB.C[k];
+    for (int k = 0; k < 3; ++k) g.t_AB[k] = T_AB.r[k];
+    double* geo = J.geo;
+    for (int k = 0; k < 3; ++k) geo[k] = T_AB.r[k];
+    for (int k = 0; k < 4; ++k) geo[3 + k] = T_AB.q[k];
+    for (int k = 0; k < 9; ++k) geo[7 + k] = T_WCa.C[k];
+    for (int k = 0; k < 3; ++k) geo[16 + k] = T_WCa.r[k];
+    // resetFrames (ProbabilisticStereoTriangulator.cpp:117-159): PoseError(T_AB, UOplus^-1) evaluated at T_AB,
+    // UOplus = diag(4e-8 I3, 1e-8 I3) (mfIdA == mfIdB); H_ = J_min^T J_min in the pose block
+    double S[36], r6[6], Jp[36];
+    for (int k = 0; k < 36; ++k) S[k] = 0.0;
+    for (int k = 0; k < 3; ++k) { S[7 * k] = sqrt(1.0 / 4e-8); S[7 * (k + 3)] = sqrt(1.0 / 1e-8); }
+    pose_error(geo, S, geo, r6, Jp);
+    for (int i = 0; i < 6; ++i)
+      for (int j = 0; j < 6; ++j) {
+        double s = 0.0;
+        for (int k = 0; k < 6; ++k) s += Jp[k * 6 + i] * Jp[k * 6 + j];
+        geo[19 + i * 6 + j] = s;
+      }
+  }
+  // doSetup, 2D-2D: per keypoint of (frame, cam_a) / (frame, cam_b) the ray sigma, the backProject bearing and skip
+  // when it names an initialised landmark of the graph
+  const int cam = side ? J.cam_b : J.cam_a;
+  const int n = side ? M.nB : M.nA;
+  const int k = blockIdx.x * TK_T + threadIdx.x;
+  if (k >= n) return;
+  const size_t e = ((size_t)J.feat * F.C + cam) * F.N + k;
+  const okb_camera& cm = W.cams[cam];
+  CamIntr ci;
+  cam_load(cm, ci);
+  const double sd = 0.8 * F.size[e] / 12.0;
+  double* rs = const_cast<double*>(side ? M.gate.ray_sigma_b : M.gate.ray_sigma_a);
+  rs[k] = sqrt(sqrt(2.0)) * sd / ci.fu;
+  // PinholeCamera::backProject (PinholeCamera.hpp(impl):426-444): (p - c) * (1 / f), the model's undistort
+  double pu[2];
+  undistort_gn(ci, (F.kp[2 * e] - ci.cu) * (1.0 / ci.fu), (F.kp[2 * e + 1] - ci.cv) * (1.0 / ci.fv), pu);
+  double* br = const_cast<double*>(side ? M.gate.bearing_b : M.gate.bearing_a) + 3 * (size_t)k;
+  br[0] = pu[0]; br[1] = pu[1]; br[2] = 1.0;
+  const int l = F.lm[e];
+  const bool skip = track_live(W, W.st->g.L, l) && l < F.lm_cap && F.lm_init[l];
+  const_cast<uint8_t*>(side ? M.skipB : M.skipA)[k] = skip ? 1 : 0;
+}
+
+// Rank test of getUncertainty (:349): H.colPivHouseholderQr().rank() < 9, by Eigen's ColPivHouseholderQR (column
+// pivoting on the downdated column norms, Householder reflectors) and its rank rule |R_ii| > 9 eps |max pivot| over the
+// nonzero pivots.  One warp; H column-major in shared memory, lane j < 9 owns column j.  Returns rank == 9.
+__device__ bool qr_full_rank9(double* H, double* s_tau, int lane) {
+  constexpr double eps = 2.220446049250313e-16;
+  double nu = 0.0, nd = 0.0;
+  if (lane < 9) {
+    double s = 0.0;
+    for (int i = 0; i < 9; ++i) s += H[lane * 9 + i] * H[lane * 9 + i];
+    nd = nu = sqrt(s);
+  }
+  double maxn = nd;
+  for (int o = 16; o > 0; o >>= 1) maxn = fmax(maxn, __shfl_xor_sync(0xffffffffu, maxn, o));
+  const double thr_helper = (maxn * eps) * (maxn * eps) / 9.0;
+  const double downdate_thr = sqrt(eps);
+  int nonzero = 9;
+  double maxpivot = 0.0;
+  for (int k = 0; k < 9; ++k) {
+    // biggest remaining updated norm, the first on ties (maxCoeff)
+    double bv = (lane >= k && lane < 9) ? nu : -1.0;
+    int bi = lane;
+    for (int o = 16; o > 0; o >>= 1) {
+      const double ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+    if (nonzero == 9 && bv * bv < thr_helper * (double)(9 - k)) nonzero = k;
+    if (bi != k) {
+      const double nu_k = __shfl_sync(0xffffffffu, nu, k), nd_k = __shfl_sync(0xffffffffu, nd, k);
+      const double nu_p = __shfl_sync(0xffffffffu, nu, bi), nd_p = __shfl_sync(0xffffffffu, nd, bi);
+      if (lane == k) { nu = nu_p; nd = nd_p; }
+      if (lane == bi) { nu = nu_k; nd = nd_k; }
+      if (lane < 9) {
+        const double x = H[k * 9 + lane];
+        H[k * 9 + lane] = H[bi * 9 + lane];
+        H[bi * 9 + lane] = x;
+      }
+    }
+    __syncwarp();
+    if (lane == 0) {
+      // makeHouseholderInPlace on rows k..8 of column k; R(k,k) = beta
+      double* v = H + k * 9;
+      const double c0 = v[k];
+      double tail = 0.0;
+      for (int i = k + 1; i < 9; ++i) tail += v[i] * v[i];
+      double tau, beta;
+      if (tail <= 2.2250738585072014e-308) {                   // numeric_limits<double>::min()
+        tau = 0.0; beta = c0;
+        for (int i = k + 1; i < 9; ++i) v[i] = 0.0;
+      } else {
+        beta = sqrt(c0 * c0 + tail);
+        if (c0 >= 0.0) beta = -beta;
+        for (int i = k + 1; i < 9; ++i) v[i] = v[i] / (c0 - beta);
+        tau = (beta - c0) / beta;
+      }
+      v[k] = beta;
+      *s_tau = tau;
+    }
+    __syncwarp();
+    maxpivot = fmax(maxpivot, fabs(H[k * 9 + k]));
+    if (lane > k && lane < 9) {
+      // applyHouseholderOnTheLeft to column `lane`, then downdate its norm (LAPACK xGEQP3)
+      const double tau = *s_tau;
+      const double* v = H + k * 9;
+      double* c = H + lane * 9;
+      double w = 0.0;
+      for (int i = k + 1; i < 9; ++i) w += v[i] * c[i];
+      w += c[k];
+      c[k] -= tau * w;
+      for (int i = k + 1; i < 9; ++i) c[i] -= tau * v[i] * w;
+      if (nu != 0.0) {
+        double t = fabs(c[k]) / nu;
+        t = (1.0 + t) * (1.0 - t);
+        t = t < 0.0 ? 0.0 : t;
+        const double t2 = t * (nu / nd) * (nu / nd);
+        if (t2 <= downdate_thr) {
+          double s = 0.0;
+          for (int i = k + 1; i < 9; ++i) s += c[i] * c[i];
+          nd = nu = sqrt(s);
+        } else {
+          nu *= sqrt(t);
+        }
+      }
+    }
+    __syncwarp();
+  }
+  const double thr = maxpivot * (eps * 9.0);
+  int rank = 0;
+  for (int i = 0; i < nonzero; ++i) rank += fabs(H[i * 9 + i]) > thr ? 1 : 0;
+  __syncwarp();
+  return rank == 9;
+}
+
+__global__ void __launch_bounds__(TK_T, 1) k_stereo_apply(const StereoJobDev* __restrict__ jobs, const MatchJobDev* __restrict__ tab) {
+  constexpr int NWT = TK_T / 32;
+  __shared__ int s_warp[NWT];
+  __shared__ int s_list[TK_T];
+  __shared__ uint8_t s_ok[TK_T];
+  __shared__ double s_H[NWT][81];
+  __shared__ double s_tau[NWT];
+  const StereoJobDev& J = jobs[blockIdx.x];
+  const MatchJobDev& M = tab[blockIdx.x];
+  const GateDev& g = M.gate;
+  const WinDev& W = *J.W;
+  const FeatStore& F = *W.feat;
+  const int L = W.st->g.L;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const size_t base_a = ((size_t)J.feat * F.C + J.cam_a) * F.N;
+  const size_t base_b = ((size_t)J.feat * F.C + J.cam_b) * F.N;
+  const double* geo = J.geo;
+  int n_out = 0;
+  for (int b0 = 0; b0 < M.nB; b0 += TK_T) {
+    const int b = b0 + tid;
+    int rec = 0, need_qr = 0, cbi = 0, a = -1, la = -1, lb = -1;
+    double hpW[4] = {0.0, 0.0, 0.0, 0.0};
+    if (b < M.nB) {
+      const okb_pair p = M.pairs[b];
+      // DenseMatcher::match calls setBestMatch for every B whose winner is below the threshold, B ascending
+      if (p.index_a >= 0 && p.distance < J.threshold) {
+        a = p.index_a;
+        la = F.lm[base_a + a]; la = track_live(W, L, la) ? la : -1;
+        lb = F.lm[base_b + b]; lb = track_live(W, L, lb) ? lb : -1;
+        double hpA[4];
+        bool parallel;
+        if (!(la >= 0 && lb >= 0) && stereo_triangulate(g, a, b, hpA, parallel)) {
+          rec = 1;
+          cbi = parallel ? 0 : 1;
+          if (cbi) {
+            // getUncertainty (:253-355): A's residual Jacobian at the triangulated point; then the point moved 20 %
+            // towards the baseline centre, where B's residual and both its Jacobians are evaluated (parametersB[1]
+            // aliases hPA)
+            const double I7[7] = {0, 0, 0, 0, 0, 0, 1};
+            double* uj = J.uj + (size_t)kUJ * b;
+            const double sdA = 0.8 * F.size[base_a + a] / 12.0, sdB = 0.8 * F.size[base_b + b] / 12.0;
+            double rA[2], rB[2];
+            reproj_full(W.cams[J.cam_a], I7, hpA, I7, F.kp + 2 * (base_a + a), sqrt(1.0 / (sdA * sdA)), rA, nullptr, uj, nullptr);
+            double hm[4];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) hm[k] = 0.8 * (hpA[k] - geo[k] / 2.0 * hpA[3]) + geo[k] / 2.0 * hpA[3];
+            hm[3] = hpA[3];
+            reproj_full(W.cams[J.cam_b], geo, hm, I7, F.kp + 2 * (base_b + b), sqrt(1.0 / (sdB * sdB)), rB, uj + 6, uj + 18, nullptr);
+            if (rB[0] * rB[0] + rB[1] * rB[1] < 4.0) cbi = 0;
+            else need_qr = 1;          // the rank of H decides
+          }
+          // T_WCa * hP_Ca
+          const double* C = geo + 7;
+          const double* r = geo + 16;
+#pragma unroll
+          for (int k = 0; k < 3; ++k) hpW[k] = C[3 * k] * hpA[0] + C[3 * k + 1] * hpA[1] + C[3 * k + 2] * hpA[2] + r[k] * hpA[3];
+          hpW[3] = hpA[3];
+        }
+      }
+    }
+    int total_q;
+    const int pos_q = track_scan(need_qr, s_warp, &total_q);
+    if (need_qr) s_list[pos_q] = b;
+    __syncthreads();
+    for (int i = warp; i < total_q; i += NWT) {
+      // H = H_ + J_hpA^T J_hpA (point block) + [J_TB J_hpB]^T [J_TB J_hpB], in the reference's order of additions
+      const double* uj = J.uj + (size_t)kUJ * s_list[i];
+      const double *JA = uj, *JT = uj + 6, *JH = uj + 18;
+      double* H = s_H[warp];
+      for (int e = lane; e < 81; e += 32) {
+        const int r = e % 9, c = e / 9;
+        double h;
+        if (r < 6 && c < 6) h = geo[19 + r * 6 + c] + (JT[r] * JT[c] + JT[6 + r] * JT[6 + c]);
+        else if (r < 6) h = JT[r] * JH[c - 6] + JT[6 + r] * JH[3 + c - 6];
+        else if (c < 6) h = JH[r - 6] * JT[c] + JH[3 + r - 6] * JT[6 + c];
+        else h = (JA[r - 6] * JA[c - 6] + JA[3 + r - 6] * JA[3 + c - 6]) + (JH[r - 6] * JH[c - 6] + JH[3 + r - 6] * JH[3 + c - 6]);
+        H[c * 9 + r] = h;
+      }
+      __syncwarp();
+      const bool ok = qr_full_rank9(H, &s_tau[warp], lane);
+      if (lane == 0) s_ok[i] = ok ? 1 : 0;
+    }
+    __syncthreads();
+    if (need_qr) cbi = s_ok[pos_q];
+    int total;
+    const int pos = track_scan(rec, s_warp, &total);
+    if (rec) {
+      okb_stereo_match& o = J.out[n_out + pos];
+      o.kp_a = a; o.kp_b = b; o.lm_slot_a = la; o.lm_slot_b = lb; o.can_be_initialized = cbi; o._pad = 0;
+      o.hp_W[0] = hpW[0]; o.hp_W[1] = hpW[1]; o.hp_W[2] = hpW[2]; o.hp_W[3] = hpW[3];
+    }
+    n_out += total;
+  }
+  if (tid == 0) *J.n_out = n_out;
+}
+}  // namespace
+
+// Host checks of one job (against the store as the pending commands leave it); "" = valid.
+static std::string stereo_job_invalid(okb_ctx* c, const okb_stereo_job& j, int desc_bytes, std::vector<char>& seen) {
+  if (j.win < 0 || j.win >= c->max_windows) return "window slot out of range";
+  const WinStore& S = c->wins[j.win];
+  const WinDev& W = c->host[j.win];
+  if (!S.uploaded) return "window slot not uploaded";
+  if (!S.feat_mem) return "window has no feature store (okb_window_reserve_features)";
+  if (seen[j.win]) return "window listed twice";
+  seen[j.win] = 1;
+  const FeatStore& F = S.feat;
+  if (F.D != desc_bytes) return "descriptor length differs from the call's first job";
+  if (j.pose < 0 || j.pose >= W.K) return "pose out of range";
+  if (j.feat_slot < 0 || j.feat_slot >= F.F) return "feat_slot out of range";
+  if (j.cam_a == j.cam_b) return "cam_a == cam_b";
+  for (int cam : {j.cam_a, j.cam_b})
+    if (cam < 0 || cam >= F.C || cam >= W.NC || cam >= W.NE) return "camera " + std::to_string(cam) + " out of range";
+  for (int cam : {j.cam_a, j.cam_b})
+    if (S.feat_n_pending[(size_t)j.feat_slot * F.C + cam] < 0) return "feature slot has no keypoints for camera " + std::to_string(cam);
+  if (j.num_best < 1 || j.num_best > MAX_BEST) return "num_best out of range (1..8)";
+  if (!j.n_out) return "n_out missing";
+  const int nB = S.feat_n_pending[(size_t)j.feat_slot * F.C + j.cam_b];
+  if (j.out_cap < nB || (nB && !j.out)) return "out capacity below the keypoints of (feat_slot, cam_b)";
+  return "";
+}
+
+extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_job* jobs) {
+  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
+  if (n_jobs == 0) return OKB_OK;
+  if (n_jobs > 65535) { c->set_error("okb_stereo_init_batch: more than 65535 jobs"); return OKB_ERR_INVALID_ARG; }   // grid dimension
+  if (c->shard_world > 1) { c->set_error("okb_stereo_init_batch: landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
+  const int desc_bytes = (jobs[0].win >= 0 && jobs[0].win < c->max_windows) ? c->wins[jobs[0].win].feat.D : 0;
+  std::vector<char> seen(c->max_windows, 0);
+  for (int i = 0; i < n_jobs; ++i) {
+    const std::string why = stereo_job_invalid(c, jobs[i], desc_bytes, seen);
+    if (!why.empty()) { c->set_error("okb_stereo_init_batch: jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
+  }
+  cudaSetDevice(c->device);
+  okb_frontend_state* F = fe(c);
+  std::lock_guard<std::mutex> lk(F->stereo_mtx);
+  {     // pending edits first, one commit per run of consecutive windows
+    std::vector<int32_t> wl(n_jobs);
+    for (int i = 0; i < n_jobs; ++i) wl[i] = jobs[i].win;
+    std::sort(wl.begin(), wl.end());
+    for (int i = 0; i < n_jobs;) {
+      int k = i + 1;
+      while (k < n_jobs && wl[k] == wl[k - 1] + 1) ++k;
+      const int rc = okb_commit_range(c, wl[i], k - i);
+      if (rc) return rc;
+      i = k;
+    }
+  }
+  cudaStream_t xs = c->stream_xfer;
+  for (int i = 0; i < n_jobs; ++i) {
+    const WinStore& S = c->wins[jobs[i].win];
+    if (S.done_idx >= 0) FE_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
+  }
+  // staging (pinned + device mirror): in  = [job table | match table]
+  //                                   out = [per job: count | records]
+  // scratch (device only), per job: geometry | bearings A, B | ray sigmas A, B | top-k | winners | skipA | skipB | done |
+  //                                 rank-test Jacobians
+  auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+  const size_t o_tab = up256(sizeof(StereoJobDev) * n_jobs);
+  const size_t in_bytes = up256(o_tab + sizeof(MatchJobDev) * n_jobs);
+  std::vector<int> nA(n_jobs), nB(n_jobs);
+  std::vector<size_t> o_out(n_jobs), o_sc(n_jobs);
+  size_t off = in_bytes, so = 0;
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_stereo_job& j = jobs[i];
+    const WinStore& S = c->wins[j.win];
+    nA[i] = S.feat_n_pending[(size_t)j.feat_slot * S.feat.C + j.cam_a];
+    nB[i] = S.feat_n_pending[(size_t)j.feat_slot * S.feat.C + j.cam_b];
+    o_out[i] = off;
+    off = up16(off + 16 + sizeof(okb_stereo_match) * (size_t)nB[i]);
+    o_sc[i] = so;
+    const size_t a = nA[i], b = nB[i];
+    so = up256(so + 8 * kGeo + 24 * a + 24 * b + 8 * a + 8 * b + sizeof(okb_pair) * a * j.num_best + sizeof(okb_pair) * b +
+               up16(a) + up16(b) + up16(a) + 8 * kUJ * b + 12 * 16);      // 12 arrays, each 16-byte aligned
+  }
+  const size_t out_end = off;
+  int rc;
+  if ((rc = grow_pinned(c, &F->stereo_io.h_stage, &F->stereo_io.h_stage_cap, out_end))) return rc;
+  if ((rc = grow(c, &F->stereo_io.d_io, &F->stereo_io.d_io_cap, out_end))) return rc;
+  if ((rc = grow(c, &F->stereo_scratch, &F->stereo_scratch_cap, std::max<size_t>(so, 256)))) return rc;
+  uint8_t* h = F->stereo_io.h_stage;
+  uint8_t* d = F->stereo_io.d_io;
+  uint8_t* sc = F->stereo_scratch;
+  const size_t sm_top = sizeof(okb_pair) * (size_t)AS_CHUNK * MAX_BEST;
+  size_t sm = sm_top;
+  int maxA = 0, maxN = 0;
+  StereoJobDev* tj = reinterpret_cast<StereoJobDev*>(h);
+  MatchJobDev* tm = reinterpret_cast<MatchJobDev*>(h + o_tab);
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_stereo_job& j = jobs[i];
+    const FeatStore& FS = c->wins[j.win].feat;
+    const size_t a = nA[i], b = nB[i];
+    size_t q = o_sc[i];
+    auto take = [&](size_t bytes) { const size_t o = q; q = up16(q + bytes); return sc + o; };
+    StereoJobDev J;
+    std::memset(&J, 0, sizeof J);
+    J.W = c->d_wins + j.win;
+    J.pose = j.pose; J.feat = j.feat_slot; J.cam_a = j.cam_a; J.cam_b = j.cam_b;
+    J.threshold = j.threshold;
+    J.geo = reinterpret_cast<double*>(take(8 * kGeo));
+    J.n_out = reinterpret_cast<int*>(d + o_out[i]);
+    J.out = reinterpret_cast<okb_stereo_match*>(d + o_out[i] + 16);
+    MatchJobDev jd;
+    std::memset(&jd, 0, sizeof jd);
+    const size_t ia = (size_t)j.feat_slot * FS.C + j.cam_a, ib = (size_t)j.feat_slot * FS.C + j.cam_b;
+    jd.A = FS.desc + ia * FS.N * (FS.D / 4);
+    jd.B = FS.desc + ib * FS.N * (FS.D / 4);
+    GateDev& g = jd.gate;                     // geometry and cameras: k_stereo_setup
+    g.mode = OKB_GATE_2D2D;
+    g.kp_a = FS.kp + 2 * ia * FS.N; g.kp_size_a = FS.size + ia * FS.N;
+    g.kp_b = FS.kp + 2 * ib * FS.N; g.kp_size_b = FS.size + ib * FS.N;
+    g.bearing_a = reinterpret_cast<const double*>(take(24 * a));
+    g.bearing_b = reinterpret_cast<const double*>(take(24 * b));
+    g.ray_sigma_a = reinterpret_cast<const double*>(take(8 * a));
+    g.ray_sigma_b = reinterpret_cast<const double*>(take(8 * b));
+    jd.topk = reinterpret_cast<okb_pair*>(take(sizeof(okb_pair) * a * j.num_best));
+    jd.pairs = reinterpret_cast<okb_pair*>(take(sizeof(okb_pair) * b));
+    jd.skipA = take(a); jd.skipB = take(b); jd.done = take(a);
+    J.uj = reinterpret_cast<double*>(take(8 * kUJ * b));
+    jd.nA = (int)a; jd.nB = (int)b; jd.num_best = j.num_best;
+    jd.list_thr = j.threshold; jd.gate_thr = j.threshold;          // Frontend's matcher: no ratio test
+    const size_t sm_b = (sizeof(okb_pair) + sizeof(int)) * b;
+    jd.in_smem = sm_top + sm_b + 1024 <= (size_t)c->smem_optin ? 1 : 0;
+    if (jd.in_smem) sm = std::max(sm, sm_top + sm_b);
+    tj[i] = J;
+    tm[i] = jd;
+    maxA = std::max(maxA, (int)a);
+    maxN = std::max(maxN, (int)std::max(a, b));
+  }
+  FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
+  const StereoJobDev* d_jobs = reinterpret_cast<const StereoJobDev*>(d);
+  MatchJobDev* d_tab = reinterpret_cast<MatchJobDev*>(d + o_tab);
+  if (sm > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
+  const int nw = desc_bytes / 4;
+  k_stereo_setup<<<dim3(std::max(1, (maxN + TK_T - 1) / TK_T), n_jobs, 2), TK_T, 0, xs>>>(d_jobs, d_tab);
+  DISPATCH_NW(nw, (k_hamming_topk<NW, true><<<dim3(std::max(1, (maxA + MW - 1) / MW), n_jobs), MT, 0, xs>>>(d_tab)));
+  k_assign<<<n_jobs, AS_T, sm, xs>>>(d_tab);
+  k_stereo_apply<<<n_jobs, TK_T, 0, xs>>>(d_jobs, d_tab);
+  F->launches += 4;
+  FE_CUDA(c, cudaGetLastError());
+  FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
+  FE_CUDA(c, cudaStreamSynchronize(xs));
+  for (int i = 0; i < n_jobs; ++i) {
+    const int n = *reinterpret_cast<const int32_t*>(h + o_out[i]);
+    *jobs[i].n_out = n;
+    if (n) std::memcpy(jobs[i].out, h + o_out[i] + 16, sizeof(okb_stereo_match) * (size_t)n);
   }
   return OKB_OK;
 }
