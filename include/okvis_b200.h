@@ -32,6 +32,8 @@
  *                                484-494): VioKeyframeWindowMatchingAlgorithm::doSetup + DenseMatcher::match + setBestMatch
  *   okb_stereo_init_batch     <- the 2D-2D match of Frontend::matchStereo (Frontend.cpp:521-546): doSetup + DenseMatcher::
  *                                match + setBestMatch's device half (stereoTriangulate, getUncertainty)
+ *   okb_match2d2d_batch       <- the 2D-2D rounds of Frontend::matchToKeyframes / matchToLastFrame (Frontend.cpp:413-452,
+ *                                499-509): the same, between an older frame and the current one
  *   okb_detect_describe       <- okvis::Frontend::detectAndDescribe    okvis_frontend/src/Frontend.cpp:92-114
  *                                (Frame::detect / Frame::describe      okvis_cv/include/okvis/implementation/Frame.hpp:109-156)
  */
@@ -721,8 +723,43 @@ typedef struct okb_stereo_job {
  * listed twice): the first failure returns OKB_ERR_INVALID_ARG and names the job in okb_last_error.  A landmark-sharded
  * context returns OKB_ERR_UNSUPPORTED.  Pending edits of the job windows are committed first; the call runs on the
  * transfer stream after the solver work already launched on those windows, with one H2D copy of the job table and one
- * D2H copy of the results, and returns when they are back.  n_jobs == 0 is a no-op. */
+ * D2H copy of the results, and returns when they are back.  n_jobs == 0 is a no-op.  It runs as okb_match2d2d_batch
+ * with frame A = frame B. */
 int okb_stereo_init_batch(okb_ctx* ctx, int n_jobs, const okb_stereo_job* jobs);
+
+/* ---- 2D-2D landmark initialisation against earlier frames (Frontend::matchToKeyframes :413-452, matchToLastFrame
+ * :499-509) -----------------------------------------------------------------------------------------------------------
+ * One job = one VioKeyframeWindowMatchingAlgorithm Match2D2D match: setFrames(olderFrameId, currentFrameId, cam_a, cam_b)
+ * with usePoseUncertainty = false.  Frame A is the older frame, frame B the current one; each is named by its position in
+ * the window (T_WS) and its feature slot.  A job with A = B (same slot and pose, cam_a != cam_b) is a stereo job and
+ * returns exactly the records of okb_stereo_init_batch. */
+typedef struct okb_match2d2d_job {
+  int32_t win;
+  int32_t pose_a, feat_slot_a, cam_a;   /* frame A: the older frame (its position in the window, feature slot, camera) */
+  int32_t pose_b, feat_slot_b, cam_b;   /* frame B: the current frame */
+  int32_t sb_current;                   /* speed/bias block of the window's current frame, -1: not in the IMU window */
+  float threshold;                      /* briskMatchingThreshold_ (60) */
+  int32_t num_best;                     /* top-k list length (4) */
+  okb_stereo_match* out; int32_t out_cap;   /* out_cap >= keypoints of (feat_slot_b, cam_b) */
+  int32_t* n_out;
+} okb_match2d2d_job;
+/* As okb_stereo_init_batch, with two frames:
+ *   setFrames: T_WCa = T_WSa T_SCa, T_WCb = T_WSb T_SCb, T_CaCb = T_WCa^-1 T_WCb;
+ *   doSetup's prior (:127-142): UOplus = diag(u I3, 1e-8 I3) with u = max(1, |v_current|)^2 * 1e-2 when A and B are
+ *     different frames (feat_slot_a != feat_slot_b) and sb_current >= 0, else u = 4e-8;
+ *   the rest as above: keypoints skipped whose store slot names an initialised landmark of the graph, the gated match,
+ *     and per winner below the threshold, in ascending B, a record unless both store slots name a landmark of the graph.
+ * hp_W = T_WCa hP_Ca.  lm_slot_a / lm_slot_b are the store's view: a keypoint that carries a landmark id only on the host
+ * (matchStereo names every keypoint, Frontend.cpp:563-571, but most of those ids never enter the graph) has slot -1 and
+ * is invisible to the device.  setBestMatch returns early when both keypoints carry an id (:373-375), so the caller drops
+ * the records whose two keypoints both carry one.  Host checks, per job and before any device work, each failure
+ * returning OKB_ERR_INVALID_ARG and naming the job: uploaded window, store reserved, both feature slots present for their
+ * cameras; cameras, poses and sb_current in range; feat_slot_a == feat_slot_b exactly when pose_a == pose_b; no match of
+ * one frame against itself in one camera; num_best <= 8; out_cap; one descriptor length per call; a window listed twice.
+ * A landmark-sharded context returns OKB_ERR_UNSUPPORTED; n_jobs == 0 is a no-op.  The call changes nothing in the window,
+ * its store or its flags; commits, stream order and copies are those of okb_stereo_init_batch (four launches, one H2D
+ * copy of the job table, one D2H copy of the results). */
+int okb_match2d2d_batch(okb_ctx* ctx, int n_jobs, const okb_match2d2d_job* jobs);
 
 #ifdef __cplusplus
 }

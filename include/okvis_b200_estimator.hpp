@@ -755,17 +755,19 @@ class Estimator {
     for (int32_t u : p.numUncertain) numUncertainMatches += u;
   }
 
-  // One okb_stereo_init_batch job of this session: the 2D-2D match of matchStereo between cameras im0 and im1 of the
-  // current frame (setFrames(mfId, mfId, im0, im1)).  finishStereo applies the records as setBestMatch does.
-  struct StereoPlan {
-    uint64_t frame = 0;
-    size_t im0 = 0, im1 = 0;
+  // One okb_match2d2d_batch job of this session: a Match2D2D round (frameA, camA) -> (frameB, camB), setFrames(frameA,
+  // frameB, camA, camB) -- an older frame against the current one (matchToKeyframes :413-452, matchToLastFrame
+  // :499-509), or frameA == frameB for matchStereo's match of two cameras of one frame.  finish2D2D applies the records.
+  struct Match2D2DPlan {
+    uint64_t frameA = 0, frameB = 0;
+    size_t camA = 0, camB = 0;
     std::vector<okb_stereo_match> out;
     int32_t nOut = 0;
-    okb_stereo_job job{};
+    okb_match2d2d_job job{};
   };
   // Throws unless, in the frame, "the keypoint has a landmark id" is "its store slot names a landmark of the graph":
-  // the device's view of setBestMatch's lmIdA / lmIdB.
+  // the device's view of setBestMatch's lmIdA / lmIdB.  Holds for the current frame before matchStereo names its
+  // remaining keypoints; finish2D2D checks the weaker "store slot >= 0 <=> the id names a landmark of the graph".
   void checkFrameIds(uint64_t frameId) const {
     auto f = feats_.find(frameId);
     if (f == feats_.end()) return;
@@ -775,45 +777,67 @@ class Estimator {
           throw std::runtime_error("okvis_b200: matchStereo: a keypoint of frame " + std::to_string(frameId) +
                                    " names landmark " + std::to_string(id) + ", which is not in the graph");
   }
-  bool planStereo(uint64_t frameId, size_t im0, size_t im1, float threshold, StereoPlan& p) {
-    auto fs = featSlot_.find(frameId);
-    if (fs == featSlot_.end()) return false;
-    const auto& F = feats_.at(frameId);
-    if (F[im0].kp.empty() || F[im1].kp.empty()) return false;
-    p.frame = frameId; p.im0 = im0; p.im1 = im1;
-    p.out.resize(F[im1].kp.size());
-    okb_stereo_job& j = p.job;
-    j.win = slot_; j.pose = (int32_t)posePos(frameId); j.feat_slot = fs->second; j.cam_a = (int32_t)im0; j.cam_b = (int32_t)im1;
+  bool plan2D2D(uint64_t frameA, size_t camA, uint64_t frameB, size_t camB, float threshold, Match2D2DPlan& p) {
+    auto fa = featSlot_.find(frameA), fb = featSlot_.find(frameB);
+    if (fa == featSlot_.end() || fb == featSlot_.end()) return false;
+    const auto& A = feats_.at(frameA);
+    const auto& B = feats_.at(frameB);
+    if (A[camA].kp.empty() || B[camB].kp.empty()) return false;
+    p.frameA = frameA; p.frameB = frameB; p.camA = camA; p.camB = camB;
+    p.out.resize(B[camB].kp.size());
+    okb_match2d2d_job& j = p.job;
+    j.win = slot_;
+    j.pose_a = (int32_t)posePos(frameA); j.feat_slot_a = fa->second; j.cam_a = (int32_t)camA;
+    j.pose_b = (int32_t)posePos(frameB); j.feat_slot_b = fb->second; j.cam_b = (int32_t)camB;
+    // doSetup's prior (:127-142) scales with the speed of the window's current frame while it is in the IMU window
+    const uint64_t cur = currentFrameId();
+    j.sb_current = isInImuWindow(cur) ? (int32_t)sbPos(cur) : -1;
     j.threshold = threshold; j.num_best = 4;
     j.out = p.out.data(); j.out_cap = (int32_t)p.out.size(); j.n_out = &p.nOut;
     return true;
   }
-  // the host half of setBestMatch's 2D-2D branch (VioKeyframeWindowMatchingAlgorithm.cpp:396-480), record by record
+  // The host half of setBestMatch's 2D-2D branch (VioKeyframeWindowMatchingAlgorithm.cpp:371-481), record by record.
+  // Returns numMatches_, the records that reached the landmark bookkeeping.  Throws unless each record's store slots
+  // agree with the host ids: slot >= 0 exactly when the id names a landmark of the graph, and then its slot.
   template <class NewId>
-  void finishStereo(const StereoPlan& p, const NewId& newId) {
-    auto& F = feats_.at(p.frame);
+  int finish2D2D(const Match2D2DPlan& p, const NewId& newId) {
+    auto& FA = feats_.at(p.frameA)[p.camA];
+    auto& FB = feats_.at(p.frameB)[p.camB];
+    auto agrees = [&](uint64_t id, int32_t slot) {
+      auto s = id ? lmSlot_.find(id) : lmSlot_.end();
+      return s == lmSlot_.end() ? slot < 0 : slot >= 0 && s->second == (uint32_t)slot;
+    };
+    int numMatches = 0;
     for (int i = 0; i < p.nOut; ++i) {
       const okb_stereo_match& r = p.out[i];
-      const uint64_t idA = F[p.im0].lm[r.kp_a], idB = F[p.im1].lm[r.kp_b];
-      if ((idA != 0) != (r.lm_slot_a >= 0) || (idB != 0) != (r.lm_slot_b >= 0) ||
-          (idA && lmSlot_.at(idA) != (uint32_t)r.lm_slot_a) || (idB && lmSlot_.at(idB) != (uint32_t)r.lm_slot_b))
-        throw std::runtime_error("okvis_b200: matchStereo: the store and the frame's landmark ids disagree");
+      const uint64_t idA = FA.lm[r.kp_a], idB = FB.lm[r.kp_b];
+      if (!agrees(idA, r.lm_slot_a) || !agrees(idB, r.lm_slot_b))
+        throw std::runtime_error("okvis_b200: 2D-2D match: the store and the frames' landmark ids disagree");
+      if (idA != 0 && idB != 0) continue;          // both carry an id, on the host only at least one of them (:373-375)
+      ++numMatches;
       const bool cbi = r.can_be_initialized != 0;
       const Vec4 hp{{r.hp_W[0], r.hp_W[1], r.hp_W[2], r.hp_W[3]}};
-      const bool insertA = idA == 0, insertB = idB == 0;
-      // both named: the device returns no record; both new: a new id; else the named one (in the graph, checkFrameIds)
-      const uint64_t lmId = (insertA && insertB) ? newId() : (insertA ? idB : idA);
+      bool insertA = idA == 0, insertB = idB == 0, insertPoint = false;
+      uint64_t lmId;
       if (insertA && insertB) {
+        lmId = newId();
+        insertPoint = true;
+      } else {
+        lmId = insertA ? idB : idA;
+        if (!landmarks_.count(lmId)) insertPoint = insertA = insertB = true;   // named on the host only: add it
+      }
+      if (insertPoint) {
         addLandmark(lmId, hp);
         setLandmarkInitialized(lmId, cbi);
       } else if (cbi) {
         setLandmarkInitialized(lmId, true);
         setLandmark(lmId, hp);
       }
-      if (insertA) observeStereo(p.frame, p.im0, r.kp_a, lmId);
-      if (insertB) observeStereo(p.frame, p.im1, r.kp_b, lmId);
+      if (insertA) observeStereo(p.frameA, p.camA, r.kp_a, lmId);
+      if (insertB) observeStereo(p.frameB, p.camB, r.kp_b, lmId);
       if (cbi) setLandmark(lmId, hp);
     }
+    return numMatches;
   }
   void observeStereo(uint64_t frameId, size_t cam, size_t k, uint64_t lmId) {
     FrameFeatures& f = feats_.at(frameId)[cam];

@@ -14,10 +14,12 @@
 // matchToLastFrame (:484-494) on the device (okb_track_3d2d_batch on the window's feature store, filled by
 // Estimator::setFrameFeatures) and apply them through Estimator::addObservation; the group forms make one call for many
 // sessions of an EstimatorGroup.  Frontend::matchStereo creates the stereo landmarks of the current frame
-// (Frontend.cpp:521-572): per overlapping camera pair the 2D-2D match on the device (okb_stereo_init_batch: backProject,
+// (Frontend.cpp:521-572): per overlapping camera pair the 2D-2D match on the device (okb_match2d2d_batch: backProject,
 // gated match, stereoTriangulate, getUncertainty), setBestMatch's landmark bookkeeping on the host, then the pair's
-// same-frame 3D-2D passes (okb_track_3d2d_batch).  The 2D-2D rounds of matchToKeyframes / matchToLastFrame, RANSAC and
-// the keyframe decision stay on the OKVIS side with the MultiFrame (SURVEY.md 8f rows 2 and 4).
+// same-frame 3D-2D passes (okb_track_3d2d_batch).  Frontend::matchToKeyframes2D2D / matchToLastFrame2D2D run the 2D-2D
+// rounds of matchToKeyframes (:413-452) and matchToLastFrame (:499-509) the same way (okb_match2d2d_batch, one call per
+// round, setBestMatch's bookkeeping on the host before the next round).  RANSAC (runRansac3d2d / runRansac2d2d, on
+// OpenGV) and the keyframe decision stay on the OKVIS side with the MultiFrame (SURVEY.md 8f rows 2 and 4).
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -138,7 +140,40 @@ class Frontend {
     return trackGroup(&group, sessions, currentFrameIds, false);
   }
 
-  // ---- stereo landmark initialisation of the current frame (device: okb_stereo_init_batch + okb_track_3d2d_batch)
+  // ---- 2D-2D landmark initialisation against earlier frames (device: okb_match2d2d_batch)
+  // matchToKeyframes' 2D-2D loop (Frontend.cpp:413-452): keyframes by age from 1, at most 2, every camera im -> im, one
+  // device call per round with the records applied as setBestMatch does (new landmarks take newId() in the order
+  // IdProvider::newId() would hand them out) before the next round: a round may add or initialise a landmark a later
+  // round must skip or reuse.  After each keyframe's rounds, afterKeyframe(kfcounter, olderFrameId) -- where the
+  // reference runs runRansac3d2d / runRansac2d2d (:432-447).  numMatches sums numMatches_ over the rounds (records that
+  // reached the landmark bookkeeping), numUncertainMatches is 0; landmarkIds are the current frame's ids (an older
+  // frame's: Estimator::frameLandmarkIds).  Keypoint ids that exist only on the host (matchStereo's last loop) are honoured.
+  TrackResult matchToKeyframes2D2D(Estimator& estimator, uint64_t currentFrameId, const std::function<uint64_t()>& newId,
+                                   const std::function<void(size_t, uint64_t)>& afterKeyframe = {}) {
+    std::function<void(size_t, size_t, uint64_t)> cb;
+    if (afterKeyframe) cb = [&](size_t, size_t kf, uint64_t id) { afterKeyframe(kf, id); };
+    return match2D2DGroup(nullptr, {&estimator}, {currentFrameId}, {newId}, true, cb)[0];
+  }
+  // matchToLastFrame's 2D-2D loop (:499-509): nothing when the last frame is a keyframe
+  TrackResult matchToLastFrame2D2D(Estimator& estimator, uint64_t currentFrameId, const std::function<uint64_t()>& newId) {
+    return match2D2DGroup(nullptr, {&estimator}, {currentFrameId}, {newId}, false, {})[0];
+  }
+  // The same for sessions of one EstimatorGroup: one okb_match2d2d_batch per round index for every session that has
+  // that round, each session's records applied in list order with its own newId; afterKeyframe(session, kfcounter,
+  // olderFrameId) runs per session.  results[i] and the ids equal the single call's on sessions[i].
+  std::vector<TrackResult> matchToKeyframes2D2D(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
+                                                const std::vector<uint64_t>& currentFrameIds,
+                                                const std::vector<std::function<uint64_t()>>& newIds,
+                                                const std::function<void(size_t, size_t, uint64_t)>& afterKeyframe = {}) {
+    return match2D2DGroup(&group, sessions, currentFrameIds, newIds, true, afterKeyframe);
+  }
+  std::vector<TrackResult> matchToLastFrame2D2D(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
+                                                const std::vector<uint64_t>& currentFrameIds,
+                                                const std::vector<std::function<uint64_t()>>& newIds) {
+    return match2D2DGroup(&group, sessions, currentFrameIds, newIds, false, {});
+  }
+
+  // ---- stereo landmark initialisation of the current frame (device: okb_match2d2d_batch + okb_track_3d2d_batch)
   // Frontend::matchStereo (Frontend.cpp:521-572).  overlap[i][j]: NCameraSystem::hasOverlap(i, j).  For every pair
   // im0 < im1 that overlaps: the 2D-2D match, its records applied as setBestMatch does (new landmarks take newId() in the
   // order IdProvider::newId() would hand them out), then the 3D-2D passes (frame, im0 -> im1) and (frame, im1 -> im0).
@@ -149,7 +184,7 @@ class Frontend {
                           const std::vector<std::vector<bool>>& overlap) {
     return stereoGroup(nullptr, {&estimator}, {frameId}, {newId}, overlap)[0];
   }
-  // The same for sessions of one EstimatorGroup: one okb_stereo_init_batch and one okb_track_3d2d_batch per camera
+  // The same for sessions of one EstimatorGroup: one okb_match2d2d_batch and one okb_track_3d2d_batch per camera
   // pair for all of them; each session's records are applied in list order with that session's newId.
   std::vector<TrackResult> matchStereo(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                        const std::vector<std::function<uint64_t()>>& newIds, const std::vector<std::vector<bool>>& overlap) {
@@ -157,6 +192,60 @@ class Frontend {
   }
 
  private:
+  std::vector<TrackResult> match2D2DGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                          const std::vector<std::function<uint64_t()>>& newIds, bool keyframes,
+                                          const std::function<void(size_t, size_t, uint64_t)>& afterKeyframe) {
+    const size_t n = sessions.size();
+    if (frameIds.size() != n || newIds.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one id source per session");
+    if (group) group->validate(sessions);
+    // per session its rounds (frame A, camera), in the reference's order; `last` closes a keyframe's rounds
+    struct Round { uint64_t frameA; size_t cam, kf; bool last; };
+    std::vector<std::vector<Round>> rounds(n);
+    size_t R = 0;
+    for (size_t i = 0; i < n; ++i) {
+      const Estimator& e = *sessions[i];
+      if (e.numFrames() < 2) continue;                 // just starting (Frontend.cpp:381-384, 470-473)
+      const size_t C = e.cameras_.size();
+      if (keyframes) {
+        for (size_t age = 1, kf = 0; age < e.numFrames() && kf < 2; ++age) {
+          const uint64_t id = e.frameIdByAge(age);
+          if (!e.isKeyframe(id)) continue;
+          for (size_t im = 0; im < C; ++im) rounds[i].push_back(Round{id, im, kf, im + 1 == C});
+          ++kf;
+        }
+      } else {
+        const uint64_t last = e.frameIdByAge(1);
+        if (!e.isKeyframe(last))
+          for (size_t im = 0; im < C; ++im) rounds[i].push_back(Round{last, im, 0, false});
+      }
+      R = std::max(R, rounds[i].size());
+    }
+    std::vector<TrackResult> out(n);
+    for (size_t r = 0; r < R; ++r) {
+      std::vector<Estimator::Match2D2DPlan> plans(n);
+      std::vector<char> has(n, 0);
+      std::vector<okb_match2d2d_job> jobs;
+      for (size_t i = 0; i < n; ++i) {
+        if (r >= rounds[i].size()) continue;
+        const Round& rd = rounds[i][r];
+        has[i] = sessions[i]->plan2D2D(rd.frameA, rd.cam, frameIds[i], rd.cam, (float)briskMatchingThreshold_, plans[i]);
+        if (has[i]) jobs.push_back(plans[i].job);
+      }
+      if (!jobs.empty()) {
+        okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
+        if (okb_match2d2d_batch(ctx, (int)jobs.size(), jobs.data()) != OKB_OK)
+          throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+      }
+      for (size_t i = 0; i < n; ++i) if (has[i]) out[i].numMatches += sessions[i]->finish2D2D(plans[i], newIds[i]);
+      if (afterKeyframe)
+        for (size_t i = 0; i < n; ++i)
+          if (r < rounds[i].size() && rounds[i][r].last) afterKeyframe(i, rounds[i][r].kf, rounds[i][r].frameA);
+    }
+    for (size_t i = 0; i < n; ++i)
+      for (size_t c = 0; c < sessions[i]->cameras_.size(); ++c) out[i].landmarkIds.push_back(sessions[i]->frameLandmarkIds(frameIds[i], c));
+    return out;
+  }
+
   std::vector<TrackResult> stereoGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                        const std::vector<std::function<uint64_t()>>& newIds, const std::vector<std::vector<bool>>& overlap) {
     const size_t n = sessions.size();
@@ -175,16 +264,16 @@ class Frontend {
       for (size_t im1 = im0 + 1; im1 < C; ++im1) {
         if (overlap[im0].size() < C || !overlap[im0][im1]) continue;
         // the 2D-2D match (:532-546)
-        std::vector<Estimator::StereoPlan> sp(n);
+        std::vector<Estimator::Match2D2DPlan> sp(n);
         std::vector<char> hs(n, 0);
-        std::vector<okb_stereo_job> sj;
+        std::vector<okb_match2d2d_job> sj;
         for (size_t i = 0; i < n; ++i) {
-          hs[i] = sessions[i]->planStereo(frameIds[i], im0, im1, (float)briskMatchingThreshold_, sp[i]);
+          hs[i] = sessions[i]->plan2D2D(frameIds[i], im0, frameIds[i], im1, (float)briskMatchingThreshold_, sp[i]);
           if (hs[i]) sj.push_back(sp[i].job);
         }
-        if (!sj.empty() && okb_stereo_init_batch(ctx, (int)sj.size(), sj.data()) != OKB_OK)
+        if (!sj.empty() && okb_match2d2d_batch(ctx, (int)sj.size(), sj.data()) != OKB_OK)
           throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
-        for (size_t i = 0; i < n; ++i) if (hs[i]) sessions[i]->finishStereo(sp[i], newIds[i]);
+        for (size_t i = 0; i < n; ++i) if (hs[i]) sessions[i]->finish2D2D(sp[i], newIds[i]);
         // the 3D-2D and 2D-3D passes of the same pair (:547-553)
         std::vector<Estimator::TrackPlan> tp(n);
         std::vector<char> ht(n, 0);

@@ -130,6 +130,13 @@ class StereoJob(C.Structure):
                 ("n_out", C.POINTER(C.c_int32))]
 
 
+class Match2D2DJob(C.Structure):
+    _fields_ = [("win", C.c_int32), ("pose_a", C.c_int32), ("feat_slot_a", C.c_int32), ("cam_a", C.c_int32),
+                ("pose_b", C.c_int32), ("feat_slot_b", C.c_int32), ("cam_b", C.c_int32), ("sb_current", C.c_int32),
+                ("threshold", C.c_float), ("num_best", C.c_int32), ("out", C.c_void_p), ("out_cap", C.c_int32),
+                ("n_out", C.POINTER(C.c_int32))]
+
+
 class PropagateJob(C.Structure):
     _fields_ = [("params", C.POINTER(ImuParams)), ("samples", C.c_void_p), ("n_samples", C.c_int32), ("_pad", C.c_int32),
                 ("t0_ns", C.c_int64), ("t1_ns", C.c_int64), ("pose", c_double_p), ("speed_bias", c_double_p),

@@ -629,6 +629,25 @@ class Context:
         self._check(lib().okb_stereo_init_batch(self._h, len(jobs), arr))
         return [o["out"][:o["n"].value].copy() for o in outs]
 
+    def match2d2d_batch(self, jobs):
+        """okb_match2d2d_batch.  jobs: dicts with win, pose_a, feat_slot_a, cam_a, pose_b, feat_slot_b, cam_b and
+        optionally sb_current (-1), threshold (60) and num_best (4).  Returns one stereo_match_dtype array per job, in
+        the reference's setBestMatch order."""
+        arr = (abi.Match2D2DJob * max(len(jobs), 1))()
+        outs = []
+        for i, j in enumerate(jobs):
+            cap = max(getattr(self, "_feat", {}).get(int(j["win"]), 0), 1)
+            o = dict(out=np.zeros(cap, abi.stereo_match_dtype), n=C.c_int32(0))
+            t = arr[i]
+            (t.win, t.pose_a, t.feat_slot_a, t.cam_a, t.pose_b, t.feat_slot_b, t.cam_b) = (
+                int(j[k]) for k in ("win", "pose_a", "feat_slot_a", "cam_a", "pose_b", "feat_slot_b", "cam_b"))
+            t.sb_current = int(j.get("sb_current", -1))
+            t.threshold, t.num_best = float(j.get("threshold", 60.0)), int(j.get("num_best", 4))
+            t.out, t.out_cap, t.n_out = o["out"].ctypes.data, int(j.get("out_cap", cap)), C.pointer(o["n"])
+            outs.append(o)
+        self._check(lib().okb_match2d2d_batch(self._h, len(jobs), arr))
+        return [o["out"][:o["n"].value].copy() for o in outs]
+
     def hamming_match_batch(self, jobs, desc_bytes):
         """okb_hamming_match_batch over `jobs`: make_match_job results, or dicts of its keyword arguments.  Returns one
         dict(topk, pairs) per job, like hamming_match / hamming_match_gated."""

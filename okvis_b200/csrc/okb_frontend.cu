@@ -173,7 +173,7 @@ struct okb_frontend_state {
   uint8_t* track_scratch = nullptr;
   size_t track_scratch_cap = 0;
   std::mutex track_mtx;
-  // okb_stereo_init_batch (on c->stream_xfer, under stereo_mtx), the same kind of buffers
+  // okb_match2d2d_batch / okb_stereo_init_batch (on c->stream_xfer, under stereo_mtx), the same kind of buffers
   MatchIO stereo_io;
   uint8_t* stereo_scratch = nullptr;
   size_t stereo_scratch_cap = 0;
@@ -2038,8 +2038,10 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
 }
 
 // =================================================================================================
-// Stereo landmark initialisation (okb_stereo_init_batch): the 2D-2D match of Frontend::matchStereo
-// (okvis_frontend/src/Frontend.cpp:521-546) on the window's feature store, frame A = frame B = the job's frame:
+// 2D-2D landmark initialisation (okb_match2d2d_batch): the 2D-2D rounds of Frontend::matchToKeyframes and
+// matchToLastFrame (okvis_frontend/src/Frontend.cpp:413-452, 499-509) on the window's feature store, frame A an older
+// frame and frame B the current one; okb_stereo_init_batch is its A = B case (the 2D-2D match of Frontend::matchStereo,
+// :521-546):
 //   k_stereo_setup  setFrames (VioKeyframeWindowMatchingAlgorithm.cpp:76-111) and doSetup's 2D-2D branch (:124-146,
 //                   216-232, 256-274): backProject, ray sigmas and skip flags per keypoint, in parallel over (job, image,
 //                   keypoint); one thread per job also writes the gate's geometry and resetFrames' prior H_
@@ -2055,9 +2057,10 @@ constexpr int kUJ = 6 + 12 + 6;          // per B keypoint: J_hpA_min 2x3, J_TB_
 
 struct StereoJobDev {
   const WinDev* W;
-  int pose, feat, cam_a, cam_b;
+  int pose_a, feat_a, cam_a, pose_b, feat_b, cam_b;
+  int sb;                   // speed/bias block whose speed scales UOplus' translation part, -1: 4e-8 (same frame, or
+                            // the current frame outside the IMU window)
   float threshold;
-  int _pad;
   double* geo;              // [kGeo]
   double* uj;               // [nB][kUJ] Jacobians of the winners that reach the rank test
   int* n_out;
@@ -2097,16 +2100,18 @@ __global__ void __launch_bounds__(TK_T) k_stereo_setup(const StereoJobDev* __res
   const FeatStore& F = *W.feat;
   const int side = blockIdx.z;
   if (blockIdx.x == 0 && side == 0 && threadIdx.x == 0) {
-    // setFrames: T_WCa = T_WS T_SCa, T_WCb = T_WS T_SCb, T_CaCb = T_WCa^-1 T_WCb
-    const double* P = W.pose + 7 * (size_t)J.pose;
+    // setFrames: T_WCa = T_WSa T_SCa, T_WCb = T_WSb T_SCb, T_CaCb = T_WCa^-1 T_WCb
+    const double* Pa = W.pose + 7 * (size_t)J.pose_a;
+    const double* Pb = W.pose + 7 * (size_t)J.pose_b;
     const double* Ea = W.ext + 7 * (size_t)J.cam_a;
     const double* Eb = W.ext + 7 * (size_t)J.cam_b;
-    XfQ T_WS, T_SCa, T_SCb, T_WCa, T_WCb, T_CaW, T_AB;
-    xfq_make(P, P + 3, T_WS);
+    XfQ T_WSa, T_WSb, T_SCa, T_SCb, T_WCa, T_WCb, T_CaW, T_AB;
+    xfq_make(Pa, Pa + 3, T_WSa);
+    xfq_make(Pb, Pb + 3, T_WSb);
     xfq_make(Ea, Ea + 3, T_SCa);
     xfq_make(Eb, Eb + 3, T_SCb);
-    xfq_mul(T_WS, T_SCa, T_WCa);
-    xfq_mul(T_WS, T_SCb, T_WCb);
+    xfq_mul(T_WSa, T_SCa, T_WCa);
+    xfq_mul(T_WSb, T_SCb, T_WCb);
     xfq_inv(T_WCa, T_CaW);
     xfq_mul(T_CaW, T_WCb, T_AB);
     GateDev& g = M.gate;
@@ -2121,11 +2126,19 @@ __global__ void __launch_bounds__(TK_T) k_stereo_setup(const StereoJobDev* __res
     for (int k = 0; k < 4; ++k) geo[3 + k] = T_AB.q[k];
     for (int k = 0; k < 9; ++k) geo[7 + k] = T_WCa.C[k];
     for (int k = 0; k < 3; ++k) geo[16 + k] = T_WCa.r[k];
-    // resetFrames (ProbabilisticStereoTriangulator.cpp:117-159): PoseError(T_AB, UOplus^-1) evaluated at T_AB,
-    // UOplus = diag(4e-8 I3, 1e-8 I3) (mfIdA == mfIdB); H_ = J_min^T J_min in the pose block
+    // doSetup's UOplus (:127-142): diag(u I3, 1e-8 I3), u velocity-scaled when the current frame is in the IMU window
+    // and A is another frame (the host passes sb = -1 otherwise), else 4e-8.  resetFrames
+    // (ProbabilisticStereoTriangulator.cpp:117-159): PoseError(T_AB, UOplus^-1) evaluated at T_AB; H_ = J_min^T J_min in
+    // the pose block
+    double u = 4e-8;
+    if (J.sb >= 0) {
+      const double* v = W.sb + 9 * (size_t)J.sb;
+      const double scale = fmax(1.0, sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]));
+      u = (scale * scale) * 1.0e-2;
+    }
     double S[36], r6[6], Jp[36];
     for (int k = 0; k < 36; ++k) S[k] = 0.0;
-    for (int k = 0; k < 3; ++k) { S[7 * k] = sqrt(1.0 / 4e-8); S[7 * (k + 3)] = sqrt(1.0 / 1e-8); }
+    for (int k = 0; k < 3; ++k) { S[7 * k] = sqrt(1.0 / u); S[7 * (k + 3)] = sqrt(1.0 / 1e-8); }
     pose_error(geo, S, geo, r6, Jp);
     for (int i = 0; i < 6; ++i)
       for (int j = 0; j < 6; ++j) {
@@ -2134,13 +2147,14 @@ __global__ void __launch_bounds__(TK_T) k_stereo_setup(const StereoJobDev* __res
         geo[19 + i * 6 + j] = s;
       }
   }
-  // doSetup, 2D-2D: per keypoint of (frame, cam_a) / (frame, cam_b) the ray sigma, the backProject bearing and skip
-  // when it names an initialised landmark of the graph
+  // doSetup, 2D-2D: per keypoint of (frame A, cam_a) / (frame B, cam_b) the ray sigma, the backProject bearing and
+  // skip when it names an initialised landmark of the graph
   const int cam = side ? J.cam_b : J.cam_a;
+  const int feat = side ? J.feat_b : J.feat_a;
   const int n = side ? M.nB : M.nA;
   const int k = blockIdx.x * TK_T + threadIdx.x;
   if (k >= n) return;
-  const size_t e = ((size_t)J.feat * F.C + cam) * F.N + k;
+  const size_t e = ((size_t)feat * F.C + cam) * F.N + k;
   const okb_camera& cm = W.cams[cam];
   CamIntr ci;
   cam_load(cm, ci);
@@ -2264,8 +2278,8 @@ __global__ void __launch_bounds__(TK_T, 1) k_stereo_apply(const StereoJobDev* __
   const FeatStore& F = *W.feat;
   const int L = W.st->g.L;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const size_t base_a = ((size_t)J.feat * F.C + J.cam_a) * F.N;
-  const size_t base_b = ((size_t)J.feat * F.C + J.cam_b) * F.N;
+  const size_t base_a = ((size_t)J.feat_a * F.C + J.cam_a) * F.N;
+  const size_t base_b = ((size_t)J.feat_b * F.C + J.cam_b) * F.N;
   const double* geo = J.geo;
   int n_out = 0;
   for (int b0 = 0; b0 < M.nB; b0 += TK_T) {
@@ -2348,7 +2362,7 @@ __global__ void __launch_bounds__(TK_T, 1) k_stereo_apply(const StereoJobDev* __
 }  // namespace
 
 // Host checks of one job (against the store as the pending commands leave it); "" = valid.
-static std::string stereo_job_invalid(okb_ctx* c, const okb_stereo_job& j, int desc_bytes, std::vector<char>& seen) {
+static std::string match2d2d_job_invalid(okb_ctx* c, const okb_match2d2d_job& j, int desc_bytes, std::vector<char>& seen) {
   if (j.win < 0 || j.win >= c->max_windows) return "window slot out of range";
   const WinStore& S = c->wins[j.win];
   const WinDev& W = c->host[j.win];
@@ -2358,30 +2372,35 @@ static std::string stereo_job_invalid(okb_ctx* c, const okb_stereo_job& j, int d
   seen[j.win] = 1;
   const FeatStore& F = S.feat;
   if (F.D != desc_bytes) return "descriptor length differs from the call's first job";
-  if (j.pose < 0 || j.pose >= W.K) return "pose out of range";
-  if (j.feat_slot < 0 || j.feat_slot >= F.F) return "feat_slot out of range";
-  if (j.cam_a == j.cam_b) return "cam_a == cam_b";
+  if (j.pose_a < 0 || j.pose_a >= W.K) return "pose_a out of range";
+  if (j.pose_b < 0 || j.pose_b >= W.K) return "pose_b out of range";
+  if (j.sb_current < -1 || j.sb_current >= W.NSB) return "sb_current out of range";
+  if (j.feat_slot_a < 0 || j.feat_slot_a >= F.F) return "feat_slot_a out of range";
+  if (j.feat_slot_b < 0 || j.feat_slot_b >= F.F) return "feat_slot_b out of range";
+  // one frame is one (position, feature slot) pair: the prior's velocity branch tests the slots, setFrames the poses
+  if ((j.feat_slot_a == j.feat_slot_b) != (j.pose_a == j.pose_b)) return "feat_slot_a == feat_slot_b but pose_a != pose_b, or the reverse";
   for (int cam : {j.cam_a, j.cam_b})
     if (cam < 0 || cam >= F.C || cam >= W.NC || cam >= W.NE) return "camera " + std::to_string(cam) + " out of range";
-  for (int cam : {j.cam_a, j.cam_b})
-    if (S.feat_n_pending[(size_t)j.feat_slot * F.C + cam] < 0) return "feature slot has no keypoints for camera " + std::to_string(cam);
+  if (j.feat_slot_a == j.feat_slot_b && j.cam_a == j.cam_b) return "frame matched against itself in one camera";
+  if (S.feat_n_pending[(size_t)j.feat_slot_a * F.C + j.cam_a] < 0) return "feature slot A has no keypoints for camera " + std::to_string(j.cam_a);
+  if (S.feat_n_pending[(size_t)j.feat_slot_b * F.C + j.cam_b] < 0) return "feature slot B has no keypoints for camera " + std::to_string(j.cam_b);
   if (j.num_best < 1 || j.num_best > MAX_BEST) return "num_best out of range (1..8)";
   if (!j.n_out) return "n_out missing";
-  const int nB = S.feat_n_pending[(size_t)j.feat_slot * F.C + j.cam_b];
-  if (j.out_cap < nB || (nB && !j.out)) return "out capacity below the keypoints of (feat_slot, cam_b)";
+  const int nB = S.feat_n_pending[(size_t)j.feat_slot_b * F.C + j.cam_b];
+  if (j.out_cap < nB || (nB && !j.out)) return "out capacity below the keypoints of (feat_slot_b, cam_b)";
   return "";
 }
 
-extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_job* jobs) {
-  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
-  if (n_jobs == 0) return OKB_OK;
-  if (n_jobs > 65535) { c->set_error("okb_stereo_init_batch: more than 65535 jobs"); return OKB_ERR_INVALID_ARG; }   // grid dimension
-  if (c->shard_world > 1) { c->set_error("okb_stereo_init_batch: landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
+// okb_match2d2d_batch and okb_stereo_init_batch (which passes its jobs with frame A = frame B); `fn` names the entry
+// point in the errors.
+static int match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs, const char* fn) {
+  if (n_jobs > 65535) { c->set_error(std::string(fn) + ": more than 65535 jobs"); return OKB_ERR_INVALID_ARG; }   // grid dimension
+  if (c->shard_world > 1) { c->set_error(std::string(fn) + ": landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
   const int desc_bytes = (jobs[0].win >= 0 && jobs[0].win < c->max_windows) ? c->wins[jobs[0].win].feat.D : 0;
   std::vector<char> seen(c->max_windows, 0);
   for (int i = 0; i < n_jobs; ++i) {
-    const std::string why = stereo_job_invalid(c, jobs[i], desc_bytes, seen);
-    if (!why.empty()) { c->set_error("okb_stereo_init_batch: jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
+    const std::string why = match2d2d_job_invalid(c, jobs[i], desc_bytes, seen);
+    if (!why.empty()) { c->set_error(std::string(fn) + ": jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
   }
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
@@ -2414,10 +2433,10 @@ extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_jo
   std::vector<size_t> o_out(n_jobs), o_sc(n_jobs);
   size_t off = in_bytes, so = 0;
   for (int i = 0; i < n_jobs; ++i) {
-    const okb_stereo_job& j = jobs[i];
+    const okb_match2d2d_job& j = jobs[i];
     const WinStore& S = c->wins[j.win];
-    nA[i] = S.feat_n_pending[(size_t)j.feat_slot * S.feat.C + j.cam_a];
-    nB[i] = S.feat_n_pending[(size_t)j.feat_slot * S.feat.C + j.cam_b];
+    nA[i] = S.feat_n_pending[(size_t)j.feat_slot_a * S.feat.C + j.cam_a];
+    nB[i] = S.feat_n_pending[(size_t)j.feat_slot_b * S.feat.C + j.cam_b];
     o_out[i] = off;
     off = up16(off + 16 + sizeof(okb_stereo_match) * (size_t)nB[i]);
     o_sc[i] = so;
@@ -2439,7 +2458,7 @@ extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_jo
   StereoJobDev* tj = reinterpret_cast<StereoJobDev*>(h);
   MatchJobDev* tm = reinterpret_cast<MatchJobDev*>(h + o_tab);
   for (int i = 0; i < n_jobs; ++i) {
-    const okb_stereo_job& j = jobs[i];
+    const okb_match2d2d_job& j = jobs[i];
     const FeatStore& FS = c->wins[j.win].feat;
     const size_t a = nA[i], b = nB[i];
     size_t q = o_sc[i];
@@ -2447,14 +2466,16 @@ extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_jo
     StereoJobDev J;
     std::memset(&J, 0, sizeof J);
     J.W = c->d_wins + j.win;
-    J.pose = j.pose; J.feat = j.feat_slot; J.cam_a = j.cam_a; J.cam_b = j.cam_b;
+    J.pose_a = j.pose_a; J.feat_a = j.feat_slot_a; J.cam_a = j.cam_a;
+    J.pose_b = j.pose_b; J.feat_b = j.feat_slot_b; J.cam_b = j.cam_b;
+    J.sb = j.feat_slot_a != j.feat_slot_b ? j.sb_current : -1;
     J.threshold = j.threshold;
     J.geo = reinterpret_cast<double*>(take(8 * kGeo));
     J.n_out = reinterpret_cast<int*>(d + o_out[i]);
     J.out = reinterpret_cast<okb_stereo_match*>(d + o_out[i] + 16);
     MatchJobDev jd;
     std::memset(&jd, 0, sizeof jd);
-    const size_t ia = (size_t)j.feat_slot * FS.C + j.cam_a, ib = (size_t)j.feat_slot * FS.C + j.cam_b;
+    const size_t ia = (size_t)j.feat_slot_a * FS.C + j.cam_a, ib = (size_t)j.feat_slot_b * FS.C + j.cam_b;
     jd.A = FS.desc + ia * FS.N * (FS.D / 4);
     jd.B = FS.desc + ib * FS.N * (FS.D / 4);
     GateDev& g = jd.gate;                     // geometry and cameras: k_stereo_setup
@@ -2498,4 +2519,22 @@ extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_jo
     if (n) std::memcpy(jobs[i].out, h + o_out[i] + 16, sizeof(okb_stereo_match) * (size_t)n);
   }
   return OKB_OK;
+}
+
+extern "C" int okb_match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs) {
+  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
+  if (n_jobs == 0) return OKB_OK;
+  return match2d2d_batch(c, n_jobs, jobs, "okb_match2d2d_batch");
+}
+
+extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_job* jobs) {
+  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
+  if (n_jobs == 0) return OKB_OK;
+  std::vector<okb_match2d2d_job> mj(n_jobs);
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_stereo_job& j = jobs[i];
+    mj[i] = okb_match2d2d_job{j.win, j.pose, j.feat_slot, j.cam_a, j.pose, j.feat_slot, j.cam_b, -1, j.threshold, j.num_best,
+                              j.out, j.out_cap, j.n_out};
+  }
+  return match2d2d_batch(c, n_jobs, mj.data(), "okb_stereo_init_batch");
 }
