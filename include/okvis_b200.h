@@ -34,6 +34,8 @@
  *                                match + setBestMatch's device half (stereoTriangulate, getUncertainty)
  *   okb_match2d2d_batch       <- the 2D-2D rounds of Frontend::matchToKeyframes / matchToLastFrame (Frontend.cpp:413-452,
  *                                499-509): the same, between an older frame and the current one
+ *   okb_keyframe_overlap_batch<- Frontend::doWeNeedANewKeyframe (Frontend.cpp:295-369): cv::convexHull, contourArea and
+ *                                pointPolygonTest over the current frame's keypoints, for many sessions in one launch
  *   okb_detect_describe       <- okvis::Frontend::detectAndDescribe    okvis_frontend/src/Frontend.cpp:92-114
  *                                (Frame::detect / Frame::describe      okvis_cv/include/okvis/implementation/Frame.hpp:109-156)
  */
@@ -760,6 +762,44 @@ typedef struct okb_match2d2d_job {
  * its store or its flags; commits, stream order and copies are those of okb_stereo_init_batch (four launches, one H2D
  * copy of the job table, one D2H copy of the results). */
 int okb_match2d2d_batch(okb_ctx* ctx, int n_jobs, const okb_match2d2d_job* jobs);
+
+/* ---- keyframe decision (Frontend::doWeNeedANewKeyframe, Frontend.cpp:295-369) ---------------------------------------
+ * One job = one session's current frame: cameras 0..n_cams-1 of a feature slot of a resident window.  Per camera, as
+ * the reference's loop over `im` computes it: the keypoints cast to float; "matched" = store slot >= 0 (landmarkId !=
+ * 0); fewer than 3 points or fewer than 3 matched points: skipped; else cv::convexHull of all points and of the matched
+ * points (float points, clockwise = false, cv2's vertex order), cv::contourArea of both, the points with
+ * cv::pointPolygonTest(matchesHull, p, false) > 0 (counted only when the matched hull has more than 2 vertices),
+ * overlap = area_matched / area_all and ratio = n_matched / (double)inside, IEEE results kept (inf, NaN). */
+typedef struct okb_keyframe_cam {
+  int32_t n_points, n_matched;          /* keypoints of the image, those with a store slot >= 0 */
+  int32_t hull_all, hull_matched;       /* vertex counts of the two hulls (0 when skipped) */
+  int32_t inside, skipped;              /* points strictly inside the matched hull; 1: the camera changes neither maximum */
+  double area_all, area_matched;        /* contourArea of the two hulls */
+  double overlap, ratio;                /* overlapArea, matchingRatio */
+} okb_keyframe_cam;
+typedef struct okb_keyframe_result {
+  double overlap, ratio;                /* std::max over the cameras that are not skipped, starting at 0 */
+  int32_t need_keyframe, _pad;          /* !(overlap > overlap_threshold && ratio > matching_ratio_threshold) */
+} okb_keyframe_result;
+typedef struct okb_keyframe_job {
+  int32_t win, feat_slot, n_cams;
+  float overlap_threshold;              /* keyframeInsertionOverlapThreshold_ (0.6f), compared in double */
+  float matching_ratio_threshold;       /* keyframeInsertionMatchingRatioThreshold_ (0.2f) */
+  int32_t _pad;
+  okb_keyframe_cam* cams;               /* [n_cams] */
+  okb_keyframe_result* out;
+} okb_keyframe_job;
+/* The keyframe decision of every job, one CTA per (job, camera) in one launch; the last CTA of a job takes the maxima
+ * in camera order (std::max(value, running): a NaN value wins, a NaN running maximum is replaced) and the decision.
+ * Every job is checked on the host before any device work (uploaded window, store reserved, n_cams in 1..the store's
+ * cameras, the feature slot present for each of them, cams and out present, a window listed twice): the first failure
+ * returns OKB_ERR_INVALID_ARG and names the job in okb_last_error.  A landmark-sharded context returns
+ * OKB_ERR_UNSUPPORTED.  Pending edits of the job windows are committed first (2D-2D bookkeeping and RANSAC removals
+ * arrive as store edits just before the decision); the call runs on the transfer stream after the solver work already
+ * launched on those windows, with one H2D copy of the job table and one D2H copy of the results, returns when they are
+ * back and changes nothing in the window or its store.  Results per job are bit-identical to calling it alone.
+ * n_jobs == 0 is a no-op. */
+int okb_keyframe_overlap_batch(okb_ctx* ctx, int n_jobs, const okb_keyframe_job* jobs);
 
 #ifdef __cplusplus
 }

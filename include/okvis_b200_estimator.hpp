@@ -533,6 +533,23 @@ class Estimator {
     FrameFeatures& f = feats_[frameId][cam];
     f.kp = keypoints; f.lm = landmarkIds;
   }
+  // MultiFrame::setLandmarkId(cam, kp, id) for a frame with features: the frame's host id and the store entry (the
+  // landmark's slot if `landmarkId` names a landmark of the graph, else -1; observed as the graph holds it).  This is
+  // how a RANSAC outlier is reported (setLandmarkId(..., 0), Frontend.cpp:631, 745): removeObservation alone keeps the
+  // store's slot, so the keypoint would still count as matched in the keyframe decision.
+  void setFrameLandmarkId(uint64_t frameId, size_t cam, size_t kp, uint64_t landmarkId) {
+    auto f = feats_.find(frameId);
+    if (f == feats_.end() || cam >= f->second.size() || kp >= f->second[cam].kp.size())
+      throw std::runtime_error("okvis_b200: setFrameLandmarkId on a keypoint without features");
+    bool observed = false;
+    auto l = landmarkId ? landmarks_.find(landmarkId) : landmarks_.end();
+    if (l != landmarks_.end()) {
+      KeypointIdentifier kid; kid.frameId = frameId; kid.cameraIndex = cam; kid.keypointIndex = kp;
+      observed = l->second.observations.count(kid) != 0;
+    }
+    setStoreLandmark(frameId, cam, kp, l != landmarks_.end() ? landmarkId : 0, observed);
+    f->second[cam].lm[kp] = landmarkId;
+  }
   // The landmark ids of a frame's keypoints as the store holds them (what the MultiFrame's landmarkId() should say).
   std::vector<uint64_t> frameLandmarkIds(uint64_t frameId, size_t cam) const {
     auto it = feats_.find(frameId);
@@ -855,6 +872,24 @@ class Estimator {
     for (auto& cam : f->second)
       for (auto& id : cam.lm)
         if (id == 0) id = newId();
+  }
+
+  // One okb_keyframe_overlap_batch job of this session's frame (every camera).  Throws unless, for every keypoint of
+  // the frame, "the host id is not 0" is "its store slot is >= 0" -- the device's view of landmarkId(im, k) != 0.
+  void planKeyframe(uint64_t frameId, float overlapThreshold, float matchingRatioThreshold, std::vector<okb_keyframe_cam>& cams,
+                    okb_keyframe_result& out, okb_keyframe_job& j) const {
+    auto fs = featSlot_.find(frameId);
+    if (fs == featSlot_.end()) throw std::runtime_error("okvis_b200: doWeNeedANewKeyframe: frame " + std::to_string(frameId) + " has no features");
+    for (const FrameFeatures& f : feats_.at(frameId))
+      for (uint64_t id : f.lm)
+        if (id != 0 && !landmarks_.count(id))
+          throw std::runtime_error("okvis_b200: doWeNeedANewKeyframe: a keypoint of frame " + std::to_string(frameId) + " names landmark " +
+                                   std::to_string(id) + ", which is not in the graph (its store slot is -1)");
+    cams.assign(cameras_.size(), okb_keyframe_cam{});
+    j = okb_keyframe_job{};
+    j.win = slot_; j.feat_slot = fs->second; j.n_cams = (int32_t)cameras_.size();
+    j.overlap_threshold = overlapThreshold; j.matching_ratio_threshold = matchingRatioThreshold;
+    j.cams = cams.data(); j.out = &out;
   }
 
   void eraseObsHost(std::map<uint64_t, Obs>::iterator it) {

@@ -18,13 +18,17 @@
 // gated match, stereoTriangulate, getUncertainty), setBestMatch's landmark bookkeeping on the host, then the pair's
 // same-frame 3D-2D passes (okb_track_3d2d_batch).  Frontend::matchToKeyframes2D2D / matchToLastFrame2D2D run the 2D-2D
 // rounds of matchToKeyframes (:413-452) and matchToLastFrame (:499-509) the same way (okb_match2d2d_batch, one call per
-// round, setBestMatch's bookkeeping on the host before the next round).  RANSAC (runRansac3d2d / runRansac2d2d, on
-// OpenGV) and the keyframe decision stay on the OKVIS side with the MultiFrame (SURVEY.md 8f rows 2 and 4).
+// round, setBestMatch's bookkeeping on the host before the next round).  Frontend::doWeNeedANewKeyframe (:295-369) runs
+// on the device (okb_keyframe_overlap_batch on the current frame's store view), and
+// Frontend::dataAssociationAndInitialization (:117-271) chains all of these for one frame.  RANSAC (runRansac3d2d /
+// runRansac2d2d, on OpenGV) stays with the adaptor, in RansacHooks, and reports outliers through
+// Estimator::removeObservation and Estimator::setFrameLandmarkId (SURVEY.md 8f row 4).
 #pragma once
 #include <cmath>
 #include <cstdint>
 #include <functional>
 #include <limits>
+#include <map>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -191,7 +195,177 @@ class Frontend {
     return stereoGroup(&group, sessions, frameIds, newIds, overlap);
   }
 
+  // ---- the keyframe decision (device: okb_keyframe_overlap_batch)
+  // Frontend::doWeNeedANewKeyframe (Frontend.cpp:295-369) for the frame's features as the store holds them:
+  // numFrames() < 2 gives true and an uninitialised Frontend false, both on the host; otherwise one device job with this
+  // Frontend's two thresholds.  Throws unless every keypoint of the frame with a host id has a store slot and the reverse
+  // (a removed landmark must be reported with Estimator::setFrameLandmarkId).  cams / result (optional) receive the
+  // per-camera values and the maxima of the device call, and are left empty when the host answers.
+  bool doWeNeedANewKeyframe(const Estimator& estimator, uint64_t currentFrameId, std::vector<okb_keyframe_cam>* cams = nullptr,
+                            okb_keyframe_result* result = nullptr) {
+    std::vector<std::vector<okb_keyframe_cam>> c;
+    std::vector<okb_keyframe_result> r;
+    const bool need = keyframeGroup(nullptr, {&estimator}, {currentFrameId}, {(char)(isInitialized_ ? 1 : 0)}, &c, &r)[0];
+    if (cams) *cams = c[0];
+    if (result) *result = r[0];
+    return need;
+  }
+  // The same for sessions of one EstimatorGroup: one okb_keyframe_overlap_batch for every session that needs the device.
+  // One Frontend serves many sessions here, so each session's initialisation flag is passed in.
+  std::vector<bool> doWeNeedANewKeyframe(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                         const std::vector<char>& initialized, std::vector<std::vector<okb_keyframe_cam>>* cams = nullptr,
+                                         std::vector<okb_keyframe_result>* results = nullptr) {
+    std::vector<const Estimator*> cs(sessions.begin(), sessions.end());
+    group.validate(sessions);
+    return keyframeGroup(&group, cs, frameIds, initialized, cams, results);
+  }
+
+  // ---- one frame of Frontend::dataAssociationAndInitialization (Frontend.cpp:117-271)
+  // The three places where the reference runs RANSAC, each receiving the session index (0 for the single form) and that
+  // session's initialisation flag.  The adaptor keeps OpenGV there and reports outliers through
+  // Estimator::removeObservation and Estimator::setFrameLandmarkId(..., 0).  An empty hook means no RANSAC.
+  struct RansacHooks {
+    // after each keyframe's 2D-2D rounds of matchToKeyframes (:432-447): runRansac3d2d when kfcounter == 0 and
+    // initialised, runRansac2d2d while not initialised; returns rotationOnly_tmp (empty hook: false)
+    std::function<bool(size_t session, bool initialized, size_t kfcounter, uint64_t olderFrameId)> afterKeyframe;
+    // matchToLastFrame, between its 3D-2D and 2D-2D rounds (:496-497): runRansac3d2d
+    std::function<void(size_t session, bool initialized)> afterLastFrame3D2D;
+    // matchToLastFrame, after its 2D-2D rounds (:512-515): runRansac2d2d while not initialised
+    std::function<void(size_t session, bool initialized)> afterLastFrame2D2D;
+  };
+  struct FrameResult {
+    std::vector<std::vector<uint64_t>> landmarkIds;   // the frame's ids per camera after matchStereo
+    int num3dMatches = 0;                             // matchToKeyframes' retCtr (its 3D-2D and 2D-2D matches)
+    // the keyframe decision's device values (empty when the host answered) and the frame's ids as the decision saw them
+    std::vector<okb_keyframe_cam> keyframeCams;
+    okb_keyframe_result keyframe{};
+    std::vector<std::vector<uint64_t>> keyframeIds;
+  };
+  // The reference's per-frame sequence, built from the calls above: when numFrames() > 1, matchToKeyframes3D2D and
+  // matchToKeyframes2D2D (rotationOnly starts true and takes the first keyframe's afterKeyframe result), isInitialized
+  // as at :184-189, *asKeyframe = *asKeyframe || doWeNeedANewKeyframe, then matchToLastFrame3D2D, afterLastFrame3D2D,
+  // matchToLastFrame2D2D, afterLastFrame2D2D (the matchToLastFrame part only when the last frame is not a keyframe, as
+  // the reference returns early there); otherwise *asKeyframe = true.  Finally matchStereo.  Reads and sets this
+  // Frontend's isInitialized_.  setKeyframe(frameId, *asKeyframe) stays with the caller (ThreadedKFVio.cpp:507-525).
+  FrameResult dataAssociationAndInitialization(Estimator& estimator, uint64_t frameId, const std::function<uint64_t()>& newId,
+                                               const std::vector<std::vector<bool>>& overlap, bool* asKeyframe,
+                                               const RansacHooks& hooks = {}) {
+    std::vector<char> init{(char)(isInitialized_ ? 1 : 0)}, kf{(char)(*asKeyframe ? 1 : 0)};
+    FrameResult r = associateGroup(nullptr, {&estimator}, {frameId}, {newId}, overlap, kf, hooks, init)[0];
+    isInitialized_ = init[0] != 0;
+    *asKeyframe = kf[0] != 0;
+    return r;
+  }
+  // The same for sessions of one EstimatorGroup, with one flag per session in `asKeyframe` and `initialized` (read and
+  // set).  Sessions may differ in camera count: matchStereo runs once per camera count, `overlap` covering the largest.
+  // results[i], the flags and every hook call equal the single form's on sessions[i].
+  std::vector<FrameResult> dataAssociationAndInitialization(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
+                                                            const std::vector<uint64_t>& frameIds,
+                                                            const std::vector<std::function<uint64_t()>>& newIds,
+                                                            const std::vector<std::vector<bool>>& overlap, std::vector<char>& asKeyframe,
+                                                            const RansacHooks& hooks, std::vector<char>& initialized) {
+    group.validate(sessions);
+    return associateGroup(&group, sessions, frameIds, newIds, overlap, asKeyframe, hooks, initialized);
+  }
+
  private:
+  std::vector<bool> keyframeGroup(EstimatorGroup* group, const std::vector<const Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                  const std::vector<char>& initialized, std::vector<std::vector<okb_keyframe_cam>>* cams,
+                                  std::vector<okb_keyframe_result>* results) {
+    const size_t n = sessions.size();
+    if (frameIds.size() != n || initialized.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one initialisation flag per session");
+    std::vector<bool> need(n, false);
+    std::vector<std::vector<okb_keyframe_cam>> c(n);
+    std::vector<okb_keyframe_result> r(n, okb_keyframe_result{});
+    std::vector<okb_keyframe_job> jobs;
+    for (size_t i = 0; i < n; ++i) {
+      if (sessions[i]->numFrames() < 2) { need[i] = true; continue; }    // just starting (:299-302)
+      if (!initialized[i]) continue;                                     // (:304-305)
+      okb_keyframe_job j;
+      sessions[i]->planKeyframe(frameIds[i], keyframeInsertionOverlapThreshold_, keyframeInsertionMatchingRatioThreshold_, c[i], r[i], j);
+      jobs.push_back(j);
+    }
+    if (!jobs.empty()) {
+      okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
+      if (okb_keyframe_overlap_batch(ctx, (int)jobs.size(), jobs.data()) != OKB_OK)
+        throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+      for (size_t i = 0; i < n; ++i) if (!c[i].empty()) need[i] = r[i].need_keyframe != 0;
+    }
+    if (cams) *cams = c;
+    if (results) *results = r;
+    return need;
+  }
+
+  std::vector<FrameResult> associateGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                          const std::vector<std::function<uint64_t()>>& newIds, const std::vector<std::vector<bool>>& overlap,
+                                          std::vector<char>& asKeyframe, const RansacHooks& hooks, std::vector<char>& initialized) {
+    const size_t n = sessions.size();
+    if (frameIds.size() != n || newIds.size() != n || asKeyframe.size() != n || initialized.size() != n)
+      throw std::invalid_argument("okvis_b200: one frame id, id source and flag pair per session");
+    std::vector<FrameResult> out(n);
+    // the sessions past their first frame (:142), in list order, with their positions in `sessions`
+    std::vector<size_t> at;
+    for (size_t i = 0; i < n; ++i) {
+      if (sessions[i]->numFrames() > 1) at.push_back(i);
+      else asKeyframe[i] = 1;                                            // first frame (:234-235)
+    }
+    if (!at.empty()) {
+      std::vector<Estimator*> s;
+      std::vector<uint64_t> f;
+      std::vector<std::function<uint64_t()>> ni;
+      for (size_t i : at) { s.push_back(sessions[i]); f.push_back(frameIds[i]); ni.push_back(newIds[i]); }
+      // matchToKeyframes (:373-460)
+      const std::vector<TrackResult> kf3 = trackGroup(group, s, f, true);
+      std::vector<char> rotationOnly(at.size(), 1), first(at.size(), 1);
+      auto afterKeyframe = [&](size_t k, size_t kf, uint64_t older) {
+        const bool tmp = hooks.afterKeyframe ? hooks.afterKeyframe(at[k], initialized[at[k]] != 0, kf, older) : false;
+        if (first[k]) { rotationOnly[k] = tmp ? 1 : 0; first[k] = 0; }
+      };
+      const std::vector<TrackResult> kf2 = match2D2DGroup(group, s, f, ni, true, afterKeyframe);
+      for (size_t k = 0; k < at.size(); ++k) {
+        out[at[k]].num3dMatches = kf3[k].numMatches + kf2[k].numMatches;
+        if (!initialized[at[k]] && !rotationOnly[k]) initialized[at[k]] = 1;     // (:184-189)
+      }
+      // the keyframe decision (:196)
+      std::vector<char> init(at.size());
+      for (size_t k = 0; k < at.size(); ++k) init[k] = initialized[at[k]];
+      std::vector<const Estimator*> cs(s.begin(), s.end());
+      std::vector<std::vector<okb_keyframe_cam>> kc;
+      std::vector<okb_keyframe_result> kr;
+      const std::vector<bool> need = keyframeGroup(group, cs, f, init, &kc, &kr);
+      for (size_t k = 0; k < at.size(); ++k) {
+        asKeyframe[at[k]] = (asKeyframe[at[k]] || need[k]) ? 1 : 0;
+        FrameResult& o = out[at[k]];
+        o.keyframeCams = kc[k]; o.keyframe = kr[k];
+        for (size_t c = 0; c < s[k]->cameras_.size(); ++c) o.keyframeIds.push_back(s[k]->frameLandmarkIds(f[k], c));
+      }
+      // matchToLastFrame (:463-518): nothing when the last frame is a keyframe
+      std::vector<char> last(at.size());
+      for (size_t k = 0; k < at.size(); ++k) last[k] = s[k]->isKeyframe(s[k]->frameIdByAge(1)) ? 0 : 1;
+      trackGroup(group, s, f, false);
+      if (hooks.afterLastFrame3D2D)
+        for (size_t k = 0; k < at.size(); ++k) if (last[k]) hooks.afterLastFrame3D2D(at[k], initialized[at[k]] != 0);
+      match2D2DGroup(group, s, f, ni, false, {});
+      if (hooks.afterLastFrame2D2D)
+        for (size_t k = 0; k < at.size(); ++k) if (last[k]) hooks.afterLastFrame2D2D(at[k], initialized[at[k]] != 0);
+    }
+    // matchStereo (:237-268), once per camera count
+    std::map<size_t, std::vector<size_t>> byCams;
+    for (size_t i = 0; i < n; ++i) byCams[sessions[i]->cameras_.size()].push_back(i);
+    for (auto& kv : byCams) {
+      std::vector<Estimator*> s;
+      std::vector<uint64_t> f;
+      std::vector<std::function<uint64_t()>> ni;
+      for (size_t i : kv.second) { s.push_back(sessions[i]); f.push_back(frameIds[i]); ni.push_back(newIds[i]); }
+      std::vector<std::vector<bool>> ov(kv.first, std::vector<bool>(kv.first, false));
+      for (size_t a = 0; a < kv.first && a < overlap.size(); ++a)
+        for (size_t b = 0; b < kv.first && b < overlap[a].size(); ++b) ov[a][b] = overlap[a][b];
+      const std::vector<TrackResult> st = stereoGroup(group, s, f, ni, ov);
+      for (size_t k = 0; k < kv.second.size(); ++k) out[kv.second[k]].landmarkIds = st[k].landmarkIds;
+    }
+    return out;
+  }
+
   std::vector<TrackResult> match2D2DGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                           const std::vector<std::function<uint64_t()>>& newIds, bool keyframes,
                                           const std::function<void(size_t, size_t, uint64_t)>& afterKeyframe) {

@@ -137,6 +137,22 @@ class Match2D2DJob(C.Structure):
                 ("n_out", C.POINTER(C.c_int32))]
 
 
+class KeyframeCam(C.Structure):
+    _fields_ = [("n_points", C.c_int32), ("n_matched", C.c_int32), ("hull_all", C.c_int32), ("hull_matched", C.c_int32),
+                ("inside", C.c_int32), ("skipped", C.c_int32), ("area_all", C.c_double), ("area_matched", C.c_double),
+                ("overlap", C.c_double), ("ratio", C.c_double)]
+
+
+class KeyframeResult(C.Structure):
+    _fields_ = [("overlap", C.c_double), ("ratio", C.c_double), ("need_keyframe", C.c_int32), ("_pad", C.c_int32)]
+
+
+class KeyframeJob(C.Structure):
+    _fields_ = [("win", C.c_int32), ("feat_slot", C.c_int32), ("n_cams", C.c_int32), ("overlap_threshold", C.c_float),
+                ("matching_ratio_threshold", C.c_float), ("_pad", C.c_int32), ("cams", C.POINTER(KeyframeCam)),
+                ("out", C.POINTER(KeyframeResult))]
+
+
 class PropagateJob(C.Structure):
     _fields_ = [("params", C.POINTER(ImuParams)), ("samples", C.c_void_p), ("n_samples", C.c_int32), ("_pad", C.c_int32),
                 ("t0_ns", C.c_int64), ("t1_ns", C.c_int64), ("pose", c_double_p), ("speed_bias", c_double_p),

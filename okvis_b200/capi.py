@@ -648,6 +648,27 @@ class Context:
         self._check(lib().okb_match2d2d_batch(self._h, len(jobs), arr))
         return [o["out"][:o["n"].value].copy() for o in outs]
 
+    def keyframe_overlap_batch(self, jobs):
+        """okb_keyframe_overlap_batch.  jobs: dicts with win, feat_slot, n_cams and optionally overlap_threshold (0.6)
+        and matching_ratio_threshold (0.2), passed as floats.  Returns one dict per job: need_keyframe (bool), overlap and
+        ratio (the maxima) and cams (one dict of okb_keyframe_cam's fields per camera)."""
+        arr = (abi.KeyframeJob * max(len(jobs), 1))()
+        outs = []
+        for i, j in enumerate(jobs):
+            n = int(j["n_cams"])
+            o = dict(cams=(abi.KeyframeCam * max(n, 1))(), out=abi.KeyframeResult())
+            t = arr[i]
+            t.win, t.feat_slot, t.n_cams = int(j["win"]), int(j["feat_slot"]), n
+            t.overlap_threshold = float(j.get("overlap_threshold", 0.6))
+            t.matching_ratio_threshold = float(j.get("matching_ratio_threshold", 0.2))
+            t.cams = C.cast(o["cams"], C.POINTER(abi.KeyframeCam)) if j.get("cams", True) is not None else None
+            t.out = C.pointer(o["out"]) if j.get("out", True) is not None else None
+            outs.append((o, n))
+        self._check(lib().okb_keyframe_overlap_batch(self._h, len(jobs), arr))
+        return [dict(need_keyframe=bool(o["out"].need_keyframe), overlap=o["out"].overlap, ratio=o["out"].ratio,
+                     cams=[{k: getattr(o["cams"][c], k) for k, _ in abi.KeyframeCam._fields_} for c in range(n)])
+                for o, n in outs]
+
     def hamming_match_batch(self, jobs, desc_bytes):
         """okb_hamming_match_batch over `jobs`: make_match_job results, or dicts of its keyword arguments.  Returns one
         dict(topk, pairs) per job, like hamming_match / hamming_match_gated."""

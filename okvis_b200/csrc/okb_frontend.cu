@@ -178,6 +178,12 @@ struct okb_frontend_state {
   uint8_t* stereo_scratch = nullptr;
   size_t stereo_scratch_cap = 0;
   std::mutex stereo_mtx;
+  // okb_keyframe_overlap_batch (on c->stream_xfer, under kf_mtx): job table in / results out, and the point buffers of
+  // the images too large for shared memory
+  MatchIO kf_io;
+  uint8_t* kf_scratch = nullptr;
+  size_t kf_scratch_cap = 0;
+  std::mutex kf_mtx;
 };
 
 void okb_frontend_release(okb_ctx* c) {
@@ -189,6 +195,8 @@ void okb_frontend_release(okb_ctx* c) {
   cudaFree(F->track_scratch);
   F->stereo_io.release();
   cudaFree(F->stereo_scratch);
+  F->kf_io.release();
+  cudaFree(F->kf_scratch);
   F->batch_det.release();
   if (F->batch_stream) cudaStreamDestroy(F->batch_stream);
   for (auto& s : F->slots) {
@@ -2537,4 +2545,491 @@ extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_jo
                               j.out, j.out_cap, j.n_out};
   }
   return match2d2d_batch(c, n_jobs, mj.data(), "okb_stereo_init_batch");
+}
+
+// =================================================================================================
+// Keyframe decision (okb_keyframe_overlap_batch): Frontend::doWeNeedANewKeyframe (okvis_frontend/src/Frontend.cpp:
+// 295-369) on the window's feature store, one CTA per (job, camera) in one launch.  Per camera and per hull (all points,
+// then the matched ones), block-wide:
+//   1. the eight extreme points in x, y, x+y and x-y, and a stable compaction of the points not inside their octagon
+//      by more than 2^-12 of the bounding box (Akl-Toussaint; those points cannot be hull vertices under any rounding
+//      of the scan below, tests/keyframe_reference.py checks it), each with its index in cv::convexHull's input;
+//   2. a bitonic sort of the survivors by (x, y, index) in shared memory (or in global scratch for an image with more
+//      keypoints than the launch's shared-memory capacity);
+//   3. cv::convexHull's Sklansky scan, one thread per quarter chain, differences in float and the convexity in double;
+//      one thread assembles the hull in OpenCV's order (clockwise = false, the cyclic shift by input index) and sums
+//      contourArea in that order;
+// then a block-wide cv::pointPolygonTest of every point against the matched hull.  The last CTA of a job takes the
+// maxima and the decision.  The call writes nothing but its scratch and its results.
+// =================================================================================================
+namespace {
+constexpr int KF_T = TK_T;               // threads per CTA (track_scan assumes TK_T)
+constexpr int KF_SMEM_PTS = 2048;        // largest image kept in shared memory (buffers of 24 B per point)
+
+struct KfCtaDev {                        // one (job, camera)
+  const WinDev* W;
+  int feat, cam, job, n_cams;
+  float thr_o, thr_r;
+  okb_keyframe_cam* cams;                // the job's [n_cams] records (device staging)
+  okb_keyframe_result* res;
+  int* done;                             // CTAs of the job finished (zeroed by the H2D copy)
+  uint8_t* buf;                          // point buffers in global scratch, nullptr: shared memory
+  int cap;                               // power of two >= the points the buffers hold
+  int _pad;
+};
+
+__host__ __device__ inline size_t kf_buf_bytes(int cap) { return 24 * (size_t)cap + 64; }
+
+// sortable image of a float (x + 0: -0 sorts as +0, as CHullCmpPoints compares) and back
+__device__ __forceinline__ uint32_t kf_f2s(float f) {
+  const uint32_t u = __float_as_uint(__fadd_rn(f, 0.0f));
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float kf_s2f(uint32_t s) { return __uint_as_float((s & 0x80000000u) ? (s & 0x7fffffffu) : ~s); }
+__device__ __forceinline__ int kf_sign_f(float v) { return (v > 0.f) - (v < 0.f); }
+__device__ __forceinline__ int kf_sign_d(double v) { return (v > 0.0) - (v < 0.0); }
+
+struct KfBuf {                           // [cap] sort keys (x, y) | [cap] input index | [cap] hull | 2 x [cap + 8] stacks
+  unsigned long long* key;
+  uint32_t* idx;
+  int* hull;
+  int* sa;
+  int* sb;
+  __device__ KfBuf(uint8_t* p, int cap) {
+    key = reinterpret_cast<unsigned long long*>(p);
+    idx = reinterpret_cast<uint32_t*>(p + 8 * (size_t)cap);
+    hull = reinterpret_cast<int*>(p + 12 * (size_t)cap);
+    sa = reinterpret_cast<int*>(p + 16 * (size_t)cap);
+    sb = sa + cap + 8;
+  }
+  __device__ float x(int i) const { return kf_s2f((uint32_t)(key[i] >> 32)); }
+  __device__ float y(int i) const { return kf_s2f((uint32_t)key[i]); }
+};
+
+// Sklansky_ (OpenCV imgproc/src/convhull.cpp) over the sorted points; returns the stack size
+__device__ int kf_sklansky(const KfBuf& B, int start, int end, int* stack, int nsign, int sign2) {
+  const int incr = end > start ? 1 : -1;
+  int pprev = start, pcur = pprev + incr, pnext = pcur + incr;
+  int stacksize = 3;
+  if (start == end || (B.x(start) == B.x(end) && B.y(start) == B.y(end))) { stack[0] = start; return 1; }
+  stack[0] = pprev; stack[1] = pcur; stack[2] = pnext;
+  end += incr;
+  while (pnext != end) {
+    const float cury = B.y(pcur), nexty = B.y(pnext);
+    const float by = __fsub_rn(nexty, cury);
+    if (kf_sign_f(by) != nsign) {
+      const float ax = __fsub_rn(B.x(pcur), B.x(pprev));
+      const float bx = __fsub_rn(B.x(pnext), B.x(pcur));
+      const float ay = __fsub_rn(cury, B.y(pprev));
+      const double convexity = (double)ay * bx - (double)ax * by;       // products exact: a contraction changes nothing
+      if (kf_sign_d(convexity) == sign2 && (ax != 0.f || ay != 0.f)) {
+        pprev = pcur; pcur = pnext; pnext += incr;
+        stack[stacksize++] = pnext;
+      } else if (pprev == start) {
+        pcur = pnext; stack[1] = pcur; pnext += incr; stack[2] = pnext;
+      } else {
+        stack[stacksize - 2] = pnext; pcur = pprev; pprev = stack[stacksize - 4]; --stacksize;
+      }
+    } else {
+      pnext += incr;
+      stack[stacksize - 1] = pnext;
+    }
+  }
+  return --stacksize;
+}
+
+template <typename T, typename Op>
+__device__ __forceinline__ T kf_reduce(T v, T* s, Op op) {     // block-wide; s: [KF_T / 32]; result in every thread
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
+  __syncthreads();
+  if (lane == 0) s[warp] = v;
+  __syncthreads();
+  T r = s[0];
+  for (int w = 1; w < KF_T / 32; ++w) r = op(r, s[w]);
+  return r;
+}
+
+struct KfShared {
+  int warp_i[KF_T / 32];
+  double warp_d[KF_T / 32];
+  double ext[8];                        // extreme values
+  int ext_k[8];                         // first keypoint attaining them
+  unsigned long long ymin, ymax;        // (sortable y, sorted position) of the first minimum / maximum
+  int m, nout, cnt[4];
+  double area;
+};
+
+// cv::convexHull of the points of the image (matched_only: those with a store slot >= 0; n_in of them), then contourArea.  Leaves the
+// hull (sorted positions, OpenCV's order) in B.hull[0..nout), the sorted points in B.key, and returns nout; *area in
+// every thread.
+__device__ int kf_hull(const FeatStore& F, size_t base, int n, int n_in, bool matched_only, const KfBuf& B, int cap, KfShared& S,
+                       double* area) {
+  const int tid = threadIdx.x;
+  auto in = [&](int k) { return !matched_only || F.lm[base + k] >= 0; };
+  auto px = [&](int k) { return (double)(float)F.kp[2 * (base + k)]; };
+  auto py = [&](int k) { return (double)(float)F.kp[2 * (base + k) + 1]; };
+  // 1. extremes: E, NE, N, NW, W, SW, S, SE (counter-clockwise, y up); first keypoint index of each maximum
+  double e[8];
+#pragma unroll
+  for (int d = 0; d < 8; ++d) e[d] = -INFINITY;
+  for (int k = tid; k < n; k += KF_T) {
+    if (!in(k)) continue;
+    const double x = px(k), y = py(k);
+    const double v[8] = {x, x + y, y, y - x, -x, -x - y, -y, x - y};
+#pragma unroll
+    for (int d = 0; d < 8; ++d) e[d] = fmax(e[d], v[d]);
+  }
+#pragma unroll
+  for (int d = 0; d < 8; ++d) {
+    const double r = kf_reduce(e[d], S.warp_d, [](double a, double b) { return fmax(a, b); });
+    if (tid == 0) { S.ext[d] = r; S.ext_k[d] = INT_MAX; }
+  }
+  __syncthreads();
+  for (int k = tid; k < n; k += KF_T) {
+    if (!in(k)) continue;
+    const double x = px(k), y = py(k);
+    const double v[8] = {x, x + y, y, y - x, -x, -x - y, -y, x - y};
+#pragma unroll
+    for (int d = 0; d < 8; ++d)
+      if (v[d] == S.ext[d]) atomicMin(&S.ext_k[d], k);
+  }
+  __syncthreads();
+  double vx[8], vy[8];
+#pragma unroll
+  for (int d = 0; d < 8; ++d) { vx[d] = px(S.ext_k[d]); vy[d] = py(S.ext_k[d]); }
+  const double D = fmax(S.ext[0] + S.ext[4], S.ext[2] + S.ext[6]);
+  int edges = 0;
+#pragma unroll
+  for (int d = 0; d < 8; ++d) edges += (vx[(d + 1) & 7] != vx[d] || vy[(d + 1) & 7] != vy[d]) ? 1 : 0;
+  // stable compaction of the survivors, each with its index among the hull's input points
+  int run_in = 0, run_out = 0;
+  for (int k0 = 0; k0 < n; k0 += KF_T) {
+    const int k = k0 + tid;
+    const int inc = k < n && in(k) ? 1 : 0;
+    int keep = 0;
+    if (inc) {
+      keep = 1;
+      if (edges > 0 && n_in >= 4) {          // a set of 4 points at least, as tests/keyframe_reference.py:extreme_filter
+        const double x = px(k), y = py(k);
+        bool inside = true;
+#pragma unroll
+        for (int d = 0; d < 8; ++d) {
+          const double ex = vx[(d + 1) & 7] - vx[d], ey = vy[(d + 1) & 7] - vy[d];
+          if (ex == 0.0 && ey == 0.0) continue;
+          inside = inside && (ex * (y - vy[d]) - ey * (x - vx[d]) > 0x1p-12 * D * fmax(fabs(ex), fabs(ey)));
+        }
+        keep = inside ? 0 : 1;
+      }
+    }
+    int t_in, t_out;
+    const int r_in = track_scan(inc, S.warp_i, &t_in);
+    const int r_out = track_scan(keep, S.warp_i, &t_out);
+    if (keep) {
+      const int o = run_out + r_out;
+      B.key[o] = ((unsigned long long)kf_f2s((float)F.kp[2 * (base + k)]) << 32) | kf_f2s((float)F.kp[2 * (base + k) + 1]);
+      B.idx[o] = (uint32_t)(run_in + r_in);
+    }
+    run_in += t_in; run_out += t_out;
+  }
+  const int m = run_out;
+  int P = 1;
+  while (P < m) P <<= 1;
+  for (int i = m + tid; i < P; i += KF_T) { B.key[i] = ~0ull; B.idx[i] = ~0u; }
+  __syncthreads();
+  // 2. bitonic sort by (x, y, index)
+  for (int k = 2; k <= P; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < P; i += KF_T) {
+        const int l = i ^ j;
+        if (l > i) {
+          const unsigned long long ka = B.key[i], kb = B.key[l];
+          const uint32_t ia = B.idx[i], ib = B.idx[l];
+          const bool gt = ka > kb || (ka == kb && ia > ib);
+          if (gt == ((i & k) == 0)) { B.key[i] = kb; B.key[l] = ka; B.idx[i] = ib; B.idx[l] = ia; }
+        }
+      }
+      __syncthreads();
+    }
+  // the first minimum and maximum of y in sorted order
+  if (tid == 0) { S.ymin = ~0ull; S.ymax = ~0ull; }
+  __syncthreads();
+  unsigned long long lmin = ~0ull, lmax = ~0ull;
+  for (int i = tid; i < m; i += KF_T) {
+    const uint32_t sy = (uint32_t)B.key[i];
+    lmin = min(lmin, ((unsigned long long)sy << 32) | (uint32_t)i);
+    lmax = min(lmax, ((unsigned long long)(~sy) << 32) | (uint32_t)i);
+  }
+  atomicMin(&S.ymin, lmin);
+  atomicMin(&S.ymax, lmax);
+  __syncthreads();
+  const int miny = (int)(uint32_t)S.ymin, maxy = (int)(uint32_t)S.ymax;
+  const bool single = B.x(0) == B.x(m - 1) && B.y(0) == B.y(m - 1);
+  // 3. the four quarter chains, one thread each: tl | tr in stack A, bl | br in stack B
+  if (!single && tid < 4) {
+    int* st = tid < 2 ? B.sa + (tid == 1 ? maxy + 3 : 0) : B.sb + (tid == 3 ? miny + 3 : 0);
+    if (tid == 0) S.cnt[0] = kf_sklansky(B, 0, maxy, st, -1, 1);
+    else if (tid == 1) S.cnt[1] = kf_sklansky(B, m - 1, maxy, st, -1, -1);
+    else if (tid == 2) S.cnt[2] = kf_sklansky(B, 0, miny, st, 1, -1);
+    else S.cnt[3] = kf_sklansky(B, m - 1, miny, st, 1, 1);
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int nout = 0;
+    if (single) {
+      B.hull[nout++] = 0;
+    } else {
+      // clockwise = false: the upper chains swap roles
+      const int* tl = B.sa + maxy + 3; int tl_count = S.cnt[1];
+      const int* tr = B.sa; int tr_count = S.cnt[0];
+      for (int i = 0; i < tl_count - 1; ++i) B.hull[nout++] = tl[i];
+      for (int i = tr_count - 1; i > 0; --i) B.hull[nout++] = tr[i];
+      const int stop_idx = tr_count > 2 ? tr[1] : tl_count > 2 ? tl[tl_count - 2] : -1;
+      const int* bl = B.sb; int bl_count = S.cnt[2];
+      const int* br = B.sb + miny + 3; int br_count = S.cnt[3];
+      if (stop_idx >= 0) {
+        const int check_idx = bl_count > 2 ? bl[1] : bl_count + br_count > 2 ? br[2 - bl_count] : -1;
+        if (check_idx == stop_idx || (check_idx >= 0 && B.x(check_idx) == B.x(stop_idx) && B.y(check_idx) == B.y(stop_idx))) {
+          bl_count = min(bl_count, 2);         // all points on one line
+          br_count = min(br_count, 2);
+        }
+      }
+      for (int i = 0; i < bl_count - 1; ++i) B.hull[nout++] = bl[i];
+      for (int i = br_count - 1; i > 0; --i) B.hull[nout++] = br[i];
+      // the cyclic shift that makes the input indices ascend or descend, where one does
+      if (nout >= 3) {
+        int min_idx = 0, max_idx = 0, lt = 0;
+        for (int i = 1; i < nout; ++i) {
+          const uint32_t v = B.idx[B.hull[i]];
+          lt += B.idx[B.hull[i - 1]] < v;
+          if (lt > 1 && lt <= i - 2) break;
+          if (v < B.idx[B.hull[min_idx]]) min_idx = i;
+          if (v > B.idx[B.hull[max_idx]]) max_idx = i;
+        }
+        const int mmdist = abs(max_idx - min_idx);
+        if ((mmdist == 1 || mmdist == nout - 1) && (lt <= 1 || lt >= nout - 2)) {
+          const bool ascending = (max_idx + 1) % nout == min_idx;
+          const int i0 = ascending ? min_idx : max_idx;
+          int j = i0, i;
+          if (i0 > 0) {
+            int* tmp = B.sa;                   // the chains are copied out
+            for (i = 0; i < nout; ++i) {
+              const int cur = tmp[i] = B.hull[j];
+              const int nj = j + 1 < nout ? j + 1 : 0;
+              if (i < nout - 1 && (ascending != (B.idx[cur] < B.idx[B.hull[nj]]))) break;
+              j = nj;
+            }
+            if (i == nout)
+              for (int q = 0; q < nout; ++q) B.hull[q] = tmp[q];
+          }
+        }
+      }
+    }
+    // contourArea, in hull order from the last vertex
+    double a00 = 0.0;
+    float prevx = B.x(B.hull[nout - 1]), prevy = B.y(B.hull[nout - 1]);
+    for (int i = 0; i < nout; ++i) {
+      const float qx = B.x(B.hull[i]), qy = B.y(B.hull[i]);
+      a00 += (double)prevx * qy - (double)prevy * qx;
+      prevx = qx; prevy = qy;
+    }
+    S.area = fabs(a00 * 0.5);
+    S.nout = nout;
+    S.m = m;
+  }
+  __syncthreads();
+  *area = S.area;
+  const int nout = S.nout;
+  __syncthreads();
+  return nout;
+}
+
+__global__ void __launch_bounds__(KF_T) k_keyframe_overlap(const KfCtaDev* __restrict__ ctas) {
+  extern __shared__ __align__(16) uint8_t kf_smem[];
+  __shared__ KfShared S;
+  const KfCtaDev& J = ctas[blockIdx.x];
+  const FeatStore& F = *J.W->feat;
+  const int tid = threadIdx.x;
+  const KfBuf B(J.buf ? J.buf : kf_smem, J.cap);
+  const size_t base = ((size_t)J.feat * F.C + J.cam) * F.N;
+  const int n = F.n[(size_t)J.feat * F.C + J.cam];
+  int nm_local = 0;
+  for (int k = tid; k < n; k += KF_T) nm_local += F.lm[base + k] >= 0 ? 1 : 0;
+  const int nm = kf_reduce(nm_local, S.warp_i, [](int a, int b) { return a + b; });
+  okb_keyframe_cam rec;
+  memset(&rec, 0, sizeof rec);
+  rec.n_points = n; rec.n_matched = nm; rec.skipped = 1;
+  if (n >= 3 && nm >= 3) {
+    double area_all, area_m;
+    const int h_all = kf_hull(F, base, n, n, false, B, J.cap, S, &area_all);
+    const int h_m = kf_hull(F, base, n, nm, true, B, J.cap, S, &area_m);
+    // the matched hull's vertices, in order, into the stacks (float2 per vertex)
+    float2* poly = reinterpret_cast<float2*>(B.sa);
+    for (int i = tid; i < h_m; i += KF_T) poly[i] = make_float2(B.x(B.hull[i]), B.y(B.hull[i]));
+    __syncthreads();
+    int inside = 0;
+    if (h_m > 2) {
+      // cv::pointPolygonTest(matchesHull, p, false) > 0 for every point
+      for (int k = tid; k < n; k += KF_T) {
+        const float ptx = (float)F.kp[2 * (base + k)], pty = (float)F.kp[2 * (base + k) + 1];
+        float2 v = poly[h_m - 1];
+        int counter = 0, res = 1;
+        for (int i = 0; i < h_m; ++i) {
+          const float2 v0 = v;
+          v = poly[i];
+          if ((v0.y <= pty && v.y <= pty) || (v0.y > pty && v.y > pty) || (v0.x < ptx && v.x < ptx)) {
+            if (pty == v.y && (ptx == v.x || (pty == v0.y && ((v0.x <= ptx && ptx <= v.x) || (v.x <= ptx && ptx <= v0.x))))) { res = 0; break; }
+            continue;
+          }
+          double dist = (double)__fsub_rn(pty, v0.y) * __fsub_rn(v.x, v0.x) - (double)__fsub_rn(ptx, v0.x) * __fsub_rn(v.y, v0.y);
+          if (dist == 0.0) { res = 0; break; }
+          if (v.y < v0.y) dist = -dist;
+          counter += dist > 0.0;
+        }
+        if (res != 0 && (counter & 1)) ++inside;
+      }
+      inside = kf_reduce(inside, S.warp_i, [](int a, int b) { return a + b; });
+    }
+    rec.skipped = 0;
+    rec.hull_all = h_all; rec.hull_matched = h_m; rec.inside = inside;
+    rec.area_all = area_all; rec.area_matched = area_m;
+    rec.overlap = area_m / area_all;
+    rec.ratio = (double)nm / (double)inside;
+  }
+  if (tid == 0) {
+    J.cams[J.cam] = rec;
+    __threadfence();
+    if (atomicAdd(J.done, 1) == J.n_cams - 1) {
+      __threadfence();
+      // the maxima in camera order, std::max(value, running) = (value < running) ? running : value
+      double overlap = 0.0, ratio = 0.0;
+      for (int c = 0; c < J.n_cams; ++c) {
+        const volatile okb_keyframe_cam& r = J.cams[c];
+        if (r.skipped) continue;
+        const double o = r.overlap, q = r.ratio;
+        overlap = (o < overlap) ? overlap : o;
+        ratio = (q < ratio) ? ratio : q;
+      }
+      okb_keyframe_result out;
+      out.overlap = overlap; out.ratio = ratio;
+      out.need_keyframe = (overlap > (double)J.thr_o && ratio > (double)J.thr_r) ? 0 : 1;
+      out._pad = 0;
+      *J.res = out;
+    }
+  }
+}
+}  // namespace
+
+// Host checks of one job (against the store as the pending commands leave it); "" = valid.
+static std::string keyframe_job_invalid(okb_ctx* c, const okb_keyframe_job& j, std::vector<char>& seen) {
+  if (j.win < 0 || j.win >= c->max_windows) return "window slot out of range";
+  const WinStore& S = c->wins[j.win];
+  if (!S.uploaded) return "window slot not uploaded";
+  if (!S.feat_mem) return "window has no feature store (okb_window_reserve_features)";
+  if (seen[j.win]) return "window listed twice";
+  seen[j.win] = 1;
+  const FeatStore& F = S.feat;
+  if (j.feat_slot < 0 || j.feat_slot >= F.F) return "feat_slot out of range";
+  if (j.n_cams < 1 || j.n_cams > F.C) return "n_cams out of range (1..the store's cameras)";
+  for (int cam = 0; cam < j.n_cams; ++cam)
+    if (S.feat_n_pending[(size_t)j.feat_slot * F.C + cam] < 0) return "feature slot has no keypoints for camera " + std::to_string(cam);
+  if (!j.cams || !j.out) return "cams / out missing";
+  return "";
+}
+
+extern "C" int okb_keyframe_overlap_batch(okb_ctx* c, int n_jobs, const okb_keyframe_job* jobs) {
+  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
+  if (n_jobs == 0) return OKB_OK;
+  if (c->shard_world > 1) { c->set_error("okb_keyframe_overlap_batch: landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
+  std::vector<char> seen(c->max_windows, 0);
+  for (int i = 0; i < n_jobs; ++i) {
+    const std::string why = keyframe_job_invalid(c, jobs[i], seen);
+    if (!why.empty()) { c->set_error("okb_keyframe_overlap_batch: jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
+  }
+  cudaSetDevice(c->device);
+  okb_frontend_state* F = fe(c);
+  std::lock_guard<std::mutex> lk(F->kf_mtx);
+  {     // pending edits first, one commit per run of consecutive windows
+    std::vector<int32_t> wl(n_jobs);
+    for (int i = 0; i < n_jobs; ++i) wl[i] = jobs[i].win;
+    std::sort(wl.begin(), wl.end());
+    for (int i = 0; i < n_jobs;) {
+      int k = i + 1;
+      while (k < n_jobs && wl[k] == wl[k - 1] + 1) ++k;
+      const int rc = okb_commit_range(c, wl[i], k - i);
+      if (rc) return rc;
+      i = k;
+    }
+  }
+  cudaStream_t xs = c->stream_xfer;
+  for (int i = 0; i < n_jobs; ++i) {
+    const WinStore& S = c->wins[jobs[i].win];
+    if (S.done_idx >= 0) FE_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
+  }
+  // staging (pinned + device mirror): in  = [per job: done counter | CTA table]
+  //                                   out = [per job: result | camera records]
+  // scratch (device only): the point buffers of the images above the shared-memory capacity
+  int n_cta = 0;
+  for (int i = 0; i < n_jobs; ++i) n_cta += jobs[i].n_cams;
+  const size_t o_tab = up256(sizeof(int) * (size_t)n_jobs);
+  const size_t in_bytes = up256(o_tab + sizeof(KfCtaDev) * (size_t)n_cta);
+  std::vector<size_t> o_out(n_jobs);
+  size_t off = in_bytes;
+  for (int i = 0; i < n_jobs; ++i) {
+    o_out[i] = off;
+    off = up256(off + sizeof(okb_keyframe_result) + sizeof(okb_keyframe_cam) * (size_t)jobs[i].n_cams);
+  }
+  const size_t out_end = off;
+  auto pow2 = [](int v) { int p = 32; while (p < v) p <<= 1; return p; };
+  int smem_cap = 32;
+  size_t so = 0;
+  std::vector<size_t> o_sc(n_cta, SIZE_MAX);
+  std::vector<int> caps(n_cta);
+  for (int i = 0, t = 0; i < n_jobs; ++i) {
+    const WinStore& S = c->wins[jobs[i].win];
+    for (int cam = 0; cam < jobs[i].n_cams; ++cam, ++t) {
+      const int n = S.feat_n_pending[(size_t)jobs[i].feat_slot * S.feat.C + cam];
+      caps[t] = pow2(n);
+      if (n <= KF_SMEM_PTS) smem_cap = std::max(smem_cap, caps[t]);
+      else { o_sc[t] = so; so = up256(so + kf_buf_bytes(caps[t])); }
+    }
+  }
+  int rc;
+  if ((rc = grow_pinned(c, &F->kf_io.h_stage, &F->kf_io.h_stage_cap, out_end))) return rc;
+  if ((rc = grow(c, &F->kf_io.d_io, &F->kf_io.d_io_cap, out_end))) return rc;
+  if (so && (rc = grow(c, &F->kf_scratch, &F->kf_scratch_cap, so))) return rc;
+  uint8_t* h = F->kf_io.h_stage;
+  uint8_t* d = F->kf_io.d_io;
+  std::memset(h, 0, o_tab);
+  KfCtaDev* tc = reinterpret_cast<KfCtaDev*>(h + o_tab);
+  for (int i = 0, t = 0; i < n_jobs; ++i) {
+    const okb_keyframe_job& j = jobs[i];
+    for (int cam = 0; cam < j.n_cams; ++cam, ++t) {
+      KfCtaDev J;
+      std::memset(&J, 0, sizeof J);
+      J.W = c->d_wins + j.win;
+      J.feat = j.feat_slot; J.cam = cam; J.job = i; J.n_cams = j.n_cams;
+      J.thr_o = j.overlap_threshold; J.thr_r = j.matching_ratio_threshold;
+      J.res = reinterpret_cast<okb_keyframe_result*>(d + o_out[i]);
+      J.cams = reinterpret_cast<okb_keyframe_cam*>(d + o_out[i] + sizeof(okb_keyframe_result));
+      J.done = reinterpret_cast<int*>(d) + i;
+      J.buf = o_sc[t] == SIZE_MAX ? nullptr : F->kf_scratch + o_sc[t];
+      J.cap = o_sc[t] == SIZE_MAX ? smem_cap : caps[t];
+      tc[t] = J;
+    }
+  }
+  const size_t smem = kf_buf_bytes(smem_cap);
+  FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
+  if (smem > 48 * 1024) FE_CUDA(c, cudaFuncSetAttribute(k_keyframe_overlap, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_keyframe_overlap<<<n_cta, KF_T, smem, xs>>>(reinterpret_cast<const KfCtaDev*>(d + o_tab));
+  F->launches += 1;
+  FE_CUDA(c, cudaGetLastError());
+  FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
+  FE_CUDA(c, cudaStreamSynchronize(xs));
+  for (int i = 0; i < n_jobs; ++i) {
+    *jobs[i].out = *reinterpret_cast<const okb_keyframe_result*>(h + o_out[i]);
+    std::memcpy(jobs[i].cams, h + o_out[i] + sizeof(okb_keyframe_result), sizeof(okb_keyframe_cam) * (size_t)jobs[i].n_cams);
+  }
+  return OKB_OK;
 }
