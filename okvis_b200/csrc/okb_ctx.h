@@ -50,8 +50,9 @@ struct WinStore {
                                       // buffer (plan_arena) holds them on top of a full upload
 };
 
-// Commits the pending commands of slots [first, first+count) on the transfer stream (okb_estimator.cu).
-int okb_commit_range(okb_ctx* c, int first, int count);
+// Commits the pending commands of the n listed slots on the transfer stream, once per run of consecutive slots after
+// sorting, then makes the transfer stream wait once on each distinct solver event of those slots (okb_estimator.cu).
+int okb_commit_windows(okb_ctx* c, const int32_t* wins, int n);
 
 // Buffers of okb_imu_propagate*: [job table | samples] in, [per-job outputs] out, in one pinned buffer and its device
 // mirror; they grow with the largest call and are kept.

@@ -462,7 +462,18 @@ static int commit_range(okb_ctx* c, int first, int count) {
   return OKB_OK;
 }
 
-int okb_commit_range(okb_ctx* c, int first, int count) { return commit_range(c, first, count); }
+int okb_commit_windows(okb_ctx* c, const int32_t* wins, int n) {
+  std::vector<int32_t> sorted(wins, wins + n);
+  std::sort(sorted.begin(), sorted.end());
+  const int rc = for_runs(sorted.data(), n, [&](int f, int m) { return commit_range(c, f, m); });
+  if (rc) return rc;
+  bool waited[okb_ctx::kDoneRing] = {};
+  for (int i = 0; i < n; ++i) {
+    const int k = c->wins[wins[i]].done_idx;
+    if (k >= 0 && !waited[k]) { OKB_CUDA(c, cudaStreamWaitEvent(c->stream_xfer, c->done_ring[k], 0)); waited[k] = true; }
+  }
+  return OKB_OK;
+}
 
 extern "C" int okb_window_commit(okb_ctx* c, int first, int count) {
   if (!c || first < 0 || count < 1 || first + count > c->max_windows) return OKB_ERR_INVALID_ARG;

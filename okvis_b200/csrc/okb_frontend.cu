@@ -134,15 +134,19 @@ struct SlotBuffers {
   std::mutex mtx;
 };
 
-// Buffers of a matcher launch: one pinned staging buffer and its device mirror (inputs in, top-k lists + winners out).
-struct MatchIO {
-  uint8_t* h_stage = nullptr;
-  size_t h_stage_cap = 0;
-  uint8_t* d_io = nullptr;
-  size_t d_io_cap = 0;
+// Buffers of one kind of table-driven call: a pinned staging buffer and its device mirror (tables in, results out, one
+// copy each way), device-only scratch, and the mutex that serialises the calls using them.  They grow with the largest
+// call and are kept.  The Hamming matcher's sets are held under match_mtx / batch_mtx, which guard other buffers too.
+struct CallBuffers {
+  uint8_t* h_stage = nullptr;      // pinned
+  uint8_t* d_stage = nullptr;
+  uint8_t* d_scratch = nullptr;
+  size_t h_stage_cap = 0, d_stage_cap = 0, d_scratch_cap = 0;
+  std::mutex mtx;
   void release() {
     if (h_stage) cudaFreeHost(h_stage);
-    cudaFree(d_io);
+    cudaFree(d_stage);
+    cudaFree(d_scratch);
   }
 };
 }  // namespace
@@ -152,7 +156,7 @@ struct okb_frontend_state {
   // batch calls: a stream of their own (never c->stream, so a batch does not queue behind a solve) and their buffers
   cudaStream_t batch_stream = nullptr;
   DetectBuffers batch_det;
-  MatchIO batch_match;
+  CallBuffers batch_match;
   std::mutex batch_mtx;
   // pattern (device), per descriptor length
   DevPattern pats[128 / 4 + 1];       // indexed by desc_bytes / 4
@@ -165,38 +169,19 @@ struct okb_frontend_state {
   uint32_t *d_rowptr = nullptr, *d_col = nullptr;
   uint16_t* d_dist = nullptr;
   size_t cap_rows = 0, cap_cand = 0;
-  MatchIO match_io;                // okb_hamming_match / _gated (on c->stream, under match_mtx)
+  CallBuffers match_io;            // okb_hamming_match / _gated (on c->stream, under match_mtx)
   std::atomic<int64_t> launches{0};   // frontend kernel launches (okb_kernel_launches adds them to the solver's)
   std::mutex match_mtx;
-  // okb_track_3d2d_batch (on c->stream_xfer, under track_mtx): job tables in / results out, and device scratch
-  MatchIO track_io;
-  uint8_t* track_scratch = nullptr;
-  size_t track_scratch_cap = 0;
-  std::mutex track_mtx;
-  // okb_match2d2d_batch / okb_stereo_init_batch (on c->stream_xfer, under stereo_mtx), the same kind of buffers
-  MatchIO stereo_io;
-  uint8_t* stereo_scratch = nullptr;
-  size_t stereo_scratch_cap = 0;
-  std::mutex stereo_mtx;
-  // okb_keyframe_overlap_batch (on c->stream_xfer, under kf_mtx): job table in / results out, and the point buffers of
-  // the images too large for shared memory
-  MatchIO kf_io;
-  uint8_t* kf_scratch = nullptr;
-  size_t kf_scratch_cap = 0;
-  std::mutex kf_mtx;
+  // the calls on a window's feature store, on c->stream_xfer, one set each so that different calls overlap:
+  CallBuffers track;               // okb_track_3d2d_batch
+  CallBuffers stereo;              // okb_match2d2d_batch / okb_stereo_init_batch
+  CallBuffers kf;                  // okb_keyframe_overlap_batch (scratch: images too large for shared memory)
 };
 
 void okb_frontend_release(okb_ctx* c) {
   if (!c->frontend) return;
   okb_frontend_state* F = c->frontend;
-  F->match_io.release();
-  F->batch_match.release();
-  F->track_io.release();
-  cudaFree(F->track_scratch);
-  F->stereo_io.release();
-  cudaFree(F->stereo_scratch);
-  F->kf_io.release();
-  cudaFree(F->kf_scratch);
+  for (CallBuffers* b : {&F->match_io, &F->batch_match, &F->track, &F->stereo, &F->kf}) b->release();
   F->batch_det.release();
   if (F->batch_stream) cudaStreamDestroy(F->batch_stream);
   for (auto& s : F->slots) {
@@ -342,7 +327,10 @@ __device__ inline UniScratch uni_scratch(uint32_t* base, uint8_t* state, int max
   s.state = state + (size_t)img * cap;
   return s;
 }
-__device__ __forceinline__ int uni_block_scan(int v, int* s_warp, int* total) {     // exclusive scan over the CTA
+// exclusive scan of one int per thread over an NT-thread CTA (s_warp: NT / 32 shared ints); *total = sum (all threads)
+template <int NT>
+__device__ __forceinline__ int block_scan(int v, int* s_warp, int* total) {
+  constexpr int NWT = NT / 32;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int x = v;
 #pragma unroll
@@ -351,15 +339,14 @@ __device__ __forceinline__ int uni_block_scan(int v, int* s_warp, int* total) { 
   if (lane == 31) s_warp[warp] = x;
   __syncthreads();
   if (warp == 0) {
-    int w = s_warp[lane];
+    int w = lane < NWT ? s_warp[lane] : 0;
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-    s_warp[lane] = w;
+    for (int o = 1; o < NWT; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
+    if (lane < NWT) s_warp[lane] = w;
   }
   __syncthreads();
-  const int base = warp ? s_warp[warp - 1] : 0;
-  *total = s_warp[31];
-  return base + x - v;
+  *total = s_warp[NWT - 1];
+  return (warp ? s_warp[warp - 1] : 0) + x - v;
 }
 __global__ void __launch_bounds__(UT, 2) k_uniformity(const FeImage* __restrict__ tab, const unsigned long long* __restrict__ keys_all,
                                                    int* count_all, int cap, double radius, int max_kp, uint32_t* uni_base,
@@ -388,7 +375,7 @@ __global__ void __launch_bounds__(UT, 2) k_uniformity(const FeImage* __restrict_
     const int c = base + tid;
     const int v = (c < n_cells) ? (int)sc.cell_cur[c] : 0;
     int total;
-    const int ex = uni_block_scan(v, s_warp, &total);
+    const int ex = block_scan<UT>(v, s_warp, &total);
     if (c < n_cells) sc.cell_start[c] = (uint32_t)(run + ex);
     run += total;
     __syncthreads();
@@ -549,7 +536,7 @@ __global__ void __launch_bounds__(UT) k_uniformity_smem(const FeImage* __restric
       const int c = base + tid;
       const int v = (c < n_cells) ? (int)cnt32[c] : 0;
       int total;
-      const int ex = uni_block_scan(v, s_warp, &total);
+      const int ex = block_scan<UT>(v, s_warp, &total);
       if (c < n_cells) S.cell_start[c] = (unsigned short)(run + ex);
       run += total;
       __syncthreads();
@@ -869,6 +856,29 @@ static void host_parallel(int n, int threads, size_t bytes, const Fn& f) {
 }
 
 static size_t up256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// Lays arrays out one after another in a buffer: take() returns the offset of the next `bytes` and pads their end to
+// `align`, so the array after them starts aligned; `off` is the size so far.  Callers lay a buffer out once, keep the
+// offsets and fill from them.
+namespace {
+struct Carve {
+  size_t off = 0;
+  size_t take(size_t bytes, size_t align = 16) {
+    const size_t o = off;
+    off = (off + bytes + align - 1) / align * align;
+    return o;
+  }
+};
+}  // namespace
+
+// Grows B to `stage` bytes of staging (pinned and its device mirror) and `scratch` bytes of device scratch.
+static int reserve(okb_ctx* c, CallBuffers& B, size_t stage, size_t scratch) {
+  int rc;
+  if ((rc = grow_pinned(c, &B.h_stage, &B.h_stage_cap, stage)) || (rc = grow(c, &B.d_stage, &B.d_stage_cap, stage)) ||
+      (rc = grow(c, &B.d_scratch, &B.d_scratch_cap, scratch)))
+    return rc;
+  return OKB_OK;
+}
 
 // Detect and describe n images with one parameter set on stream `st`, into buffers B: one H2D copy (image table and
 // packed images), 7 launches whatever n is, one D2H copy (counts, keypoints, descriptors), one synchronisation.
@@ -1356,13 +1366,33 @@ __global__ void __launch_bounds__(1024) k_exclusive_scan(const uint32_t* counts,
     const int i = base + threadIdx.x;
     const int v = (i < n) ? (int)counts[i] : 0;
     int total;
-    const int ex = uni_block_scan(v, s_warp, &total);
+    const int ex = block_scan<1024>(v, s_warp, &total);
     if (i < n) row_ptr[i] = (uint32_t)(run + ex);
     run += total;
     __syncthreads();
   }
   if (threadIdx.x == 0) row_ptr[n] = (uint32_t)run;
 }
+
+// k_assign's dynamic shared memory over one call: the staged top-k lists, and the per-B winners and list counts of every
+// job whose winners fit beside them (fit() decides the job's in_smem).  set_attribute() runs once per call: it raises
+// the kernel's limit to the largest size any launch asks for, so that concurrent calls never lower it under each other.
+struct AssignSmem {
+  static constexpr size_t kTop = sizeof(okb_pair) * (size_t)AS_CHUNK * MAX_BEST;
+  size_t bytes = kTop;
+  void fit(const okb_ctx* c, MatchJobDev& jd) {
+    const size_t need = kTop + (sizeof(okb_pair) + sizeof(int)) * (size_t)jd.nB;
+    jd.in_smem = need + 1024 <= (size_t)c->smem_optin ? 1 : 0;
+    if (jd.in_smem) bytes = std::max(bytes, need);
+  }
+  int set_attribute(okb_ctx* c) const {
+    if (bytes > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
+    return OKB_OK;
+  }
+};
+
+// Offsets of a store-backed match's arrays in the call's device scratch (carve_match lays them out).
+struct MatchScratch { size_t topk, pairs, skipA, skipB, done; };
 }  // namespace
 
 #define DISPATCH_NW(nw, CALL)                 \
@@ -1374,6 +1404,51 @@ __global__ void __launch_bounds__(1024) k_exclusive_scan(const uint32_t* counts,
     default: c->set_error("descriptor length must be 32, 48, 64 or 128 bytes"); return OKB_ERR_UNSUPPORTED; \
   }
 
+// The matcher over device table d_tab: n[0] plain jobs, then n[1] gated ones.  One k_hamming_topk<NW, GATED> launch per
+// kind present, its grid covering the kind's largest nA (max_a), then one k_assign over all of them.
+static int launch_matcher(okb_ctx* c, cudaStream_t st, const MatchJobDev* d_tab, int nw, const int n[2], const int max_a[2],
+                          const AssignSmem& sm) {
+  auto grid = [&](int kind) { return dim3(std::max(1, (max_a[kind] + MW - 1) / MW), n[kind]); };
+  if (n[0]) DISPATCH_NW(nw, (k_hamming_topk<NW, false><<<grid(0), MT, 0, st>>>(d_tab)));
+  if (n[1]) DISPATCH_NW(nw, (k_hamming_topk<NW, true><<<grid(1), MT, 0, st>>>(d_tab + n[0])));
+  k_assign<<<n[0] + n[1], AS_T, sm.bytes, st>>>(d_tab);
+  c->frontend->launches += (n[0] > 0) + (n[1] > 0) + 1;
+  return OKB_OK;
+}
+
+static MatchScratch carve_match(Carve& sc, size_t nA, size_t nB, int num_best) {
+  MatchScratch m;
+  m.topk = sc.take(sizeof(okb_pair) * nA * num_best);
+  m.pairs = sc.take(sizeof(okb_pair) * nB);
+  m.skipA = sc.take(nA);
+  m.skipB = sc.take(nB);
+  m.done = sc.take(nA);
+  return m;
+}
+
+// The matcher entry of a job on a window's feature store: A and B are store images ia and ib (feature slot * C + camera)
+// with nA and nB keypoints, B's keypoints feed the gate, the arrays lie at m in the device scratch sc, and both
+// thresholds are `threshold` (the Frontend's matcher makes no ratio test).  The caller sets the gate's mode and the
+// rest of its arrays.
+static MatchJobDev store_match_job(const okb_ctx* c, const FeatStore& FS, size_t ia, size_t ib, int nA, int nB, int num_best,
+                                   float threshold, uint8_t* sc, const MatchScratch& m, AssignSmem& sm) {
+  MatchJobDev jd;
+  std::memset(&jd, 0, sizeof jd);
+  jd.A = FS.desc + ia * FS.N * (FS.D / 4);
+  jd.B = FS.desc + ib * FS.N * (FS.D / 4);
+  jd.skipA = sc + m.skipA;
+  jd.skipB = sc + m.skipB;
+  jd.topk = reinterpret_cast<okb_pair*>(sc + m.topk);
+  jd.pairs = reinterpret_cast<okb_pair*>(sc + m.pairs);
+  jd.done = sc + m.done;
+  jd.nA = nA; jd.nB = nB; jd.num_best = num_best;
+  jd.list_thr = threshold; jd.gate_thr = threshold;
+  jd.gate.kp_b = FS.kp + 2 * ib * FS.N;
+  jd.gate.kp_size_b = FS.size + ib * FS.N;
+  sm.fit(c, jd);
+  return jd;
+}
+
 static int upload_descriptors(okb_ctx* c, okb_frontend_state* F, const uint8_t* A, int nA, const uint8_t* B, int nB, int bytes,
                               const uint8_t* skipA, const uint8_t* skipB) {
   int rc;
@@ -1384,12 +1459,6 @@ static int upload_descriptors(okb_ctx* c, okb_frontend_state* F, const uint8_t* 
   if (skipA) FE_CUDA(c, cudaMemcpyAsync(F->d_A + (size_t)nA * bytes, skipA, nA, cudaMemcpyHostToDevice, c->stream));
   if (skipB) FE_CUDA(c, cudaMemcpyAsync(F->d_B + (size_t)nB * bytes, skipB, nB, cudaMemcpyHostToDevice, c->stream));
   return OKB_OK;
-}
-
-static int ensure_io(okb_ctx* c, MatchIO& io, size_t bytes) {
-  int rc;
-  if ((rc = grow_pinned(c, &io.h_stage, &io.h_stage_cap, bytes))) return rc;
-  return grow(c, &io.d_io, &io.d_io_cap, bytes);
 }
 
 // The single call's argument checks, for one job.
@@ -1411,7 +1480,7 @@ static int match_job_check(okb_ctx* c, const okb_match_job& j, int desc_bytes) {
 // n matches on stream `st` through staging buffers io: one pinned staging buffer, one copy in, one copy out:
 //   [job table (gates included) | per job: A | B | skipA | skipB | gate arrays]  ...  [per job: top-k lists | winners] [per job: scratch]
 // Plain jobs come first in the table, gated ones after them: one k_hamming_topk launch per kind, one k_assign launch.
-static int match_run(okb_ctx* c, MatchIO& io, cudaStream_t st, int n, const okb_match_job* jobs, int desc_bytes) {
+static int match_run(okb_ctx* c, CallBuffers& io, cudaStream_t st, int n, const okb_match_job* jobs, int desc_bytes) {
   int rc;
   bool any = false;
   for (int i = 0; i < n; ++i) {
@@ -1436,37 +1505,33 @@ static int match_run(okb_ctx* c, MatchIO& io, cudaStream_t st, int n, const okb_
     }
   const int nd = (int)order.size();
   if (nd == 0) return OKB_OK;
-  auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
   struct Lay { size_t oA, oB, oSA, oSB, g_kpb, g_szb, g_proj, g_unc, g_kpa, g_sza, g_ba, g_bb, g_rsa, g_rsb, oT, oP, oD; };
   std::vector<Lay> L(nd);
-  size_t off = up256(sizeof(MatchJobDev) * nd);
+  Carve q;
+  q.take(sizeof(MatchJobDev) * nd, 256);
   for (int t = 0; t < nd; ++t) {
     const okb_match_job& j = jobs[order[t]];
     const size_t nA = j.nA, nB = j.nB;
     Lay& l = L[t];
-    l.oA = off; l.oB = l.oA + up16(nA * desc_bytes); l.oSA = l.oB + up16(nB * desc_bytes); l.oSB = l.oSA + up16(nA);
-    off = l.oSB + up16(nB);
-    if (j.gate && j.gate->mode != OKB_GATE_NONE) {
-      // gate arrays (doubles): kp_b 2nB | size_b nB | proj 2nA | unc 4nA | kp_a 2nA | size_a nA | bear_a 3nA | bear_b 3nB | rs_a nA | rs_b nB
-      l.g_kpb = off; l.g_szb = l.g_kpb + 16 * nB; l.g_proj = l.g_szb + up16(8 * nB); l.g_unc = l.g_proj + 16 * nA;
-      l.g_kpa = l.g_unc + 32 * nA; l.g_sza = l.g_kpa + 16 * nA; l.g_ba = l.g_sza + up16(8 * nA); l.g_bb = l.g_ba + up16(24 * nA);
-      l.g_rsa = l.g_bb + up16(24 * nB); l.g_rsb = l.g_rsa + up16(8 * nA);
-      off = l.g_rsb + up16(8 * nB);
+    l.oA = q.take(nA * desc_bytes); l.oB = q.take(nB * desc_bytes); l.oSA = q.take(nA); l.oSB = q.take(nB);
+    if (j.gate && j.gate->mode != OKB_GATE_NONE) {      // gate arrays (doubles)
+      l.g_kpb = q.take(16 * nB); l.g_szb = q.take(8 * nB); l.g_proj = q.take(16 * nA); l.g_unc = q.take(32 * nA);
+      l.g_kpa = q.take(16 * nA); l.g_sza = q.take(8 * nA); l.g_ba = q.take(24 * nA); l.g_bb = q.take(24 * nB);
+      l.g_rsa = q.take(8 * nA); l.g_rsb = q.take(8 * nB);
     }
   }
-  const size_t in_bytes = off;
+  const size_t in_bytes = q.off;
   for (int t = 0; t < nd; ++t) {
     const okb_match_job& j = jobs[order[t]];
-    L[t].oT = off; L[t].oP = off + sizeof(okb_pair) * (size_t)j.nA * j.num_best;
-    off = up16(L[t].oP + sizeof(okb_pair) * (size_t)j.nB);
+    L[t].oT = q.take(sizeof(okb_pair) * (size_t)j.nA * j.num_best);
+    L[t].oP = q.take(sizeof(okb_pair) * (size_t)j.nB);
   }
-  const size_t out_end = off;
-  for (int t = 0; t < nd; ++t) { L[t].oD = off; off += up16((size_t)jobs[order[t]].nA); }
-  if ((rc = ensure_io(c, io, off))) return rc;
+  const size_t out_end = q.off;
+  for (int t = 0; t < nd; ++t) L[t].oD = q.take((size_t)jobs[order[t]].nA);
+  if ((rc = reserve(c, io, q.off, 0))) return rc;
   uint8_t* h = io.h_stage;
-  uint8_t* d = io.d_io;
-  const size_t sm_top = sizeof(okb_pair) * (size_t)AS_CHUNK * MAX_BEST;
-  size_t sm = sm_top;
+  uint8_t* d = io.d_stage;
+  AssignSmem sm;
   int maxA[2] = {0, 0}, nkind[2] = {0, 0};
   MatchJobDev* tab = reinterpret_cast<MatchJobDev*>(h);
   for (int t = 0; t < nd; ++t) {
@@ -1490,9 +1555,7 @@ static int match_run(okb_ctx* c, MatchIO& io, cudaStream_t st, int n, const okb_
     // DenseMatcher.hpp(impl):188-193: with the ratio test the lists are built without a threshold
     jd.list_thr = j.use_ratio ? 3.402823466e+38f : j.threshold;
     jd.gate_thr = mode == OKB_GATE_NONE ? 0.f : j.threshold;
-    const size_t sm_b = (sizeof(okb_pair) + sizeof(int)) * (size_t)j.nB;        // per-B winners + list counts
-    jd.in_smem = sm_top + sm_b + 1024 <= (size_t)c->smem_optin ? 1 : 0;
-    if (jd.in_smem) sm = std::max(sm, sm_top + sm_b);
+    sm.fit(c, jd);
     if (mode != OKB_GATE_NONE) {
       const okb_match_gate* gate = j.gate;
       GateDev gd;
@@ -1524,15 +1587,8 @@ static int match_run(okb_ctx* c, MatchIO& io, cudaStream_t st, int n, const okb_
     ++nkind[kind];
   }
   FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, st));
-  const MatchJobDev* d_tab = reinterpret_cast<const MatchJobDev*>(d);
-  if (nkind[0])
-    DISPATCH_NW(nw, (k_hamming_topk<NW, false><<<dim3((maxA[0] + MW - 1) / MW, nkind[0]), MT, 0, st>>>(d_tab)));
-  if (nkind[1])
-    DISPATCH_NW(nw, (k_hamming_topk<NW, true><<<dim3((maxA[1] + MW - 1) / MW, nkind[1]), MT, 0, st>>>(d_tab + nkind[0])));
-  // the attribute is always set to the largest size any launch asks for, so concurrent calls never lower it under each other
-  if (sm > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
-  k_assign<<<nd, AS_T, sm, st>>>(d_tab);
-  c->frontend->launches += (nkind[0] > 0) + (nkind[1] > 0) + 1;
+  if ((rc = sm.set_attribute(c)) || (rc = launch_matcher(c, st, reinterpret_cast<const MatchJobDev*>(d), nw, nkind, maxA, sm)))
+    return rc;
   FE_CUDA(c, cudaGetLastError());
   FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, st));
   FE_CUDA(c, cudaStreamSynchronize(st));
@@ -1670,27 +1726,6 @@ __device__ __forceinline__ bool track_live(const WinDev& W, int L, int l) {
 
 constexpr int TK_T = 256;     // threads of the setup / apply CTAs (the projection chain needs more than 64 registers)
 
-// exclusive scan of one int per thread over a TK_T-thread CTA; *total = sum (all threads)
-__device__ __forceinline__ int track_scan(int v, int* s_warp, int* total) {
-  constexpr int NWT = TK_T / 32;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-  __syncthreads();
-  if (lane == 31) s_warp[warp] = x;
-  __syncthreads();
-  if (warp == 0) {
-    int w = lane < NWT ? s_warp[lane] : 0;
-#pragma unroll
-    for (int o = 1; o < NWT; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-    if (lane < NWT) s_warp[lane] = w;
-  }
-  __syncthreads();
-  *total = s_warp[NWT - 1];
-  return (warp ? s_warp[warp - 1] : 0) + x - v;
-}
-
 __global__ void __launch_bounds__(TK_T, 1) k_track_setup(const TrackJobDev* __restrict__ jobs, const MatchJobDev* __restrict__ tab,
                                                       const TrackRoundDev* __restrict__ rinfo, int round) {
   __shared__ int s_warp[TK_T / 32];
@@ -1774,7 +1809,7 @@ __global__ void __launch_bounds__(TK_T, 1) k_track_setup(const TrackJobDev* __re
     }
     // setLandmarkInitialized(false) in ascending k: a landmark two keypoints share is cleared (and listed) once
     int total;
-    const int pos = track_scan(clear, s_warp, &total);
+    const int pos = block_scan<TK_T>(clear, s_warp, &total);
     if (clear) s_cand[pos] = k;
     __syncthreads();
     if (tid == 0) {
@@ -1829,8 +1864,8 @@ __global__ void __launch_bounds__(TK_T) k_track_apply(const TrackJobDev* __restr
       }
     }
     int total, total_u;
-    const int pos = track_scan(acc, s_warp, &total);
-    track_scan(acc & uncertain, s_warp, &total_u);
+    const int pos = block_scan<TK_T>(acc, s_warp, &total);
+    block_scan<TK_T>(acc & uncertain, s_warp, &total_u);
     if (acc) {
       // B's keypoint takes A's landmark and its observation; the count of the landmark rises for the later rounds
       F.lm[base_b + b] = l;
@@ -1849,17 +1884,52 @@ __global__ void __launch_bounds__(TK_T) k_track_apply(const TrackJobDev* __restr
 }
 }  // namespace
 
-// Host checks of one job (against the store as the pending commands leave it); "" = valid.
-static std::string track_job_invalid(okb_ctx* c, const okb_track_job& j, int desc_bytes, std::vector<char>& seen, size_t& sumA, size_t& sumB) {
-  if (j.win < 0 || j.win >= c->max_windows) return "window slot out of range";
-  const WinStore& S = c->wins[j.win];
-  const WinDev& W = c->host[j.win];
+// The host checks every job of a call on the feature store makes of its window; "" = valid.
+static std::string store_window_invalid(okb_ctx* c, int win, std::vector<char>& seen) {
+  if (win < 0 || win >= c->max_windows) return "window slot out of range";
+  const WinStore& S = c->wins[win];
   if (!S.uploaded) return "window slot not uploaded";
   if (!S.feat_mem) return "window has no feature store (okb_window_reserve_features)";
-  if (seen[j.win]) return "window listed twice";
-  seen[j.win] = 1;
+  if (seen[win]) return "window listed twice";
+  seen[win] = 1;
+  return "";
+}
+
+// The argument checks of a call `fn` on the feature store, before any device work: an empty call is a no-op (OKB_OK, and
+// the caller returns), more than max_jobs jobs and a landmark-sharded context are refused, and invalid(i, seen) checks
+// job i against the store as the pending commands leave it ("" = valid; the first failure is reported as
+// "fn: jobs[i]: why").
+template <typename Job, typename Invalid>
+static int store_call_checks(okb_ctx* c, const char* fn, int n_jobs, const Job* jobs, int max_jobs, const Invalid& invalid) {
+  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
+  if (n_jobs == 0) return OKB_OK;
+  if (n_jobs > max_jobs) { c->set_error(std::string(fn) + ": more than " + std::to_string(max_jobs) + " jobs"); return OKB_ERR_INVALID_ARG; }
+  if (c->shard_world > 1) { c->set_error(std::string(fn) + ": landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
+  std::vector<char> seen(c->max_windows, 0);
+  for (int i = 0; i < n_jobs; ++i) {
+    const std::string why = invalid(i, seen);
+    if (!why.empty()) { c->set_error(std::string(fn) + ": jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
+  }
+  return OKB_OK;
+}
+
+// Pending edits of the jobs' windows first (they may be the store edits the call reads), then after the solver work on
+// those windows.
+template <typename Job>
+static int commit_job_windows(okb_ctx* c, const Job* jobs, int n_jobs) {
+  std::vector<int32_t> wl(n_jobs);
+  for (int i = 0; i < n_jobs; ++i) wl[i] = jobs[i].win;
+  return okb_commit_windows(c, wl.data(), n_jobs);
+}
+
+// Host checks of one job (first_win: the window of the call's first job, already checked); "" = valid.
+static std::string track_job_invalid(okb_ctx* c, const okb_track_job& j, int first_win, std::vector<char>& seen) {
+  const std::string why = store_window_invalid(c, j.win, seen);
+  if (!why.empty()) return why;
+  const WinStore& S = c->wins[j.win];
+  const WinDev& W = c->host[j.win];
   const FeatStore& F = S.feat;
-  if (F.D != desc_bytes) return "descriptor length differs from the call's first job";
+  if (F.D != c->wins[first_win].feat.D) return "descriptor length differs from the call's first job";
   if (j.pose_b < 0 || j.pose_b >= W.K) return "pose_b out of range";
   if (j.sb_b < -1 || j.sb_b >= W.NSB) return "sb_b out of range";
   if (j.feat_slot_b < 0 || j.feat_slot_b >= F.F) return "feat_slot_b out of range";
@@ -1867,7 +1937,7 @@ static std::string track_job_invalid(okb_ctx* c, const okb_track_job& j, int des
   if (j.n_rounds < 0 || (j.n_rounds > 0 && (!j.rounds || !j.num_matches || !j.num_uncertain))) return "round list or per-round outputs missing";
   if (j.n_rounds > 255) return "more than 255 rounds";
   if (!j.n_assoc || !j.n_uninit) return "n_assoc / n_uninit missing";
-  sumA = 0; sumB = 0;
+  size_t sumA = 0, sumB = 0;
   for (int r = 0; r < j.n_rounds; ++r) {
     const okb_track_round& R = j.rounds[r];
     if (R.feat_slot_a < 0 || R.feat_slot_a >= F.F || R.cam_a < 0 || R.cam_a >= F.C) return "round " + std::to_string(r) + ": frame A out of range";
@@ -1884,38 +1954,16 @@ static std::string track_job_invalid(okb_ctx* c, const okb_track_job& j, int des
 }
 
 extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job* jobs) {
-  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
-  if (n_jobs == 0) return OKB_OK;
-  if (n_jobs > 65535) { c->set_error("okb_track_3d2d_batch: more than 65535 jobs"); return OKB_ERR_INVALID_ARG; }   // grid dimension
-  if (c->shard_world > 1) { c->set_error("okb_track_3d2d_batch: landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
-  const int desc_bytes = (jobs[0].win >= 0 && jobs[0].win < c->max_windows) ? c->wins[jobs[0].win].feat.D : 0;
-  std::vector<char> seen(c->max_windows, 0);
-  std::vector<size_t> sumA(n_jobs), sumB(n_jobs);
-  for (int i = 0; i < n_jobs; ++i) {
-    const std::string why = track_job_invalid(c, jobs[i], desc_bytes, seen, sumA[i], sumB[i]);
-    if (!why.empty()) { c->set_error("okb_track_3d2d_batch: jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
-  }
+  int rc = store_call_checks(c, "okb_track_3d2d_batch", n_jobs, jobs, 65535, [&](int i, std::vector<char>& seen) {   // grid dimension
+    return track_job_invalid(c, jobs[i], jobs[0].win, seen);
+  });
+  if (rc || n_jobs == 0) return rc;
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
-  std::lock_guard<std::mutex> lk(F->track_mtx);
-  // pending edits first (they may be the store edits this call reads), then after the solver work on these windows
-  {     // one commit per run of consecutive windows, so the launch count does not grow with the number of sessions
-    std::vector<int32_t> wl(n_jobs);
-    for (int i = 0; i < n_jobs; ++i) wl[i] = jobs[i].win;
-    std::sort(wl.begin(), wl.end());
-    for (int i = 0; i < n_jobs;) {
-      int k = i + 1;
-      while (k < n_jobs && wl[k] == wl[k - 1] + 1) ++k;
-      const int rc = okb_commit_range(c, wl[i], k - i);
-      if (rc) return rc;
-      i = k;
-    }
-  }
+  CallBuffers& B = F->track;
+  std::lock_guard<std::mutex> lk(B.mtx);
+  if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
   cudaStream_t xs = c->stream_xfer;
-  for (int i = 0; i < n_jobs; ++i) {
-    const WinStore& S = c->wins[jobs[i].win];
-    if (S.done_idx >= 0) FE_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
-  }
   // jobs by decreasing round count: the jobs of round r are the first m[r]
   std::vector<int> order(n_jobs);
   for (int i = 0; i < n_jobs; ++i) order[i] = i;
@@ -1926,104 +1974,83 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
     for (int r = 0; r < jobs[i].n_rounds; ++r) ++m[r];
   // staging (pinned + device mirror): in  = [job table | per round: match table | round table]
   //                                   out = [per job: header | associations | cleared slots]
-  // scratch (device only):           per job: counts; per (job, round): proj | unc | topk | pairs | skipA | skipB | done
-  auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
-  size_t off = up256(sizeof(TrackJobDev) * n_jobs);
+  // scratch (device only), per job: counts; per (job, round): proj | unc | the matcher's arrays
+  Carve st, sc;
+  st.take(sizeof(TrackJobDev) * n_jobs, 256);
   std::vector<size_t> o_tab(R), o_rinfo(R);
-  for (int r = 0; r < R; ++r) { o_tab[r] = off; off = up16(off + sizeof(MatchJobDev) * m[r]); o_rinfo[r] = off; off = up16(off + sizeof(TrackRoundDev) * m[r]); }
-  const size_t in_bytes = up256(off);
-  off = in_bytes;
-  std::vector<size_t> o_hdr(n_jobs), o_assoc(n_jobs), o_un(n_jobs);
+  for (int r = 0; r < R; ++r) { o_tab[r] = st.take(sizeof(MatchJobDev) * m[r]); o_rinfo[r] = st.take(sizeof(TrackRoundDev) * m[r]); }
+  const size_t in_bytes = st.off;
+  struct RoundLay { int nA, nB; size_t proj, unc; MatchScratch ms; };
+  std::vector<RoundLay> rl;                 // per (job, round); job i's rounds from rl[r0[i]]
+  std::vector<size_t> o_hdr(n_jobs), o_assoc(n_jobs), o_un(n_jobs), o_cnt(n_jobs), r0(n_jobs);
   for (int i = 0; i < n_jobs; ++i) {
-    o_hdr[i] = off; o_assoc[i] = up16(off + 4 * (2 * (size_t)jobs[i].n_rounds + 2)); o_un[i] = o_assoc[i] + 8 * sumB[i];
-    off = up16(o_un[i] + 4 * sumA[i]);
-  }
-  const size_t out_end = off;
-  int rc;
-  if ((rc = grow_pinned(c, &F->track_io.h_stage, &F->track_io.h_stage_cap, out_end))) return rc;
-  if ((rc = grow(c, &F->track_io.d_io, &F->track_io.d_io_cap, out_end))) return rc;
-  size_t so = 0;
-  std::vector<size_t> o_cnt(n_jobs);
-  for (int i = 0; i < n_jobs; ++i) { o_cnt[i] = so; so = up256(so + 4 * (size_t)std::max(c->host[jobs[i].win].L, 1)); }
-  std::vector<size_t> o_rs(n_jobs);     // per-job start of the round scratch
-  for (int i = 0; i < n_jobs; ++i) {
-    o_rs[i] = so;
     const okb_track_job& j = jobs[i];
+    const WinStore& S = c->wins[j.win];
+    r0[i] = rl.size();
+    o_cnt[i] = sc.take(4 * (size_t)std::max(c->host[j.win].L, 1));
+    size_t sumA = 0, sumB = 0;
     for (int r = 0; r < j.n_rounds; ++r) {
-      const WinStore& S = c->wins[j.win];
-      const size_t nA = S.feat_n_pending[(size_t)j.rounds[r].feat_slot_a * S.feat.C + j.rounds[r].cam_a];
-      const size_t nB = S.feat_n_pending[(size_t)j.feat_slot_b * S.feat.C + j.rounds[r].cam_b];
-      so = up256(so + 16 * nA + 32 * nA + sizeof(okb_pair) * nA * j.num_best + sizeof(okb_pair) * nB + up16(nA) + up16(nB) + up16(nA));
+      RoundLay x;
+      x.nA = S.feat_n_pending[(size_t)j.rounds[r].feat_slot_a * S.feat.C + j.rounds[r].cam_a];
+      x.nB = S.feat_n_pending[(size_t)j.feat_slot_b * S.feat.C + j.rounds[r].cam_b];
+      x.proj = sc.take(16 * (size_t)x.nA);
+      x.unc = sc.take(32 * (size_t)x.nA);
+      x.ms = carve_match(sc, x.nA, x.nB, j.num_best);
+      rl.push_back(x);
+      sumA += x.nA; sumB += x.nB;
     }
+    o_hdr[i] = st.take(4 * (2 * (size_t)j.n_rounds + 2));
+    o_assoc[i] = st.take(8 * sumB);
+    o_un[i] = st.take(4 * sumA);
   }
-  if ((rc = grow(c, &F->track_scratch, &F->track_scratch_cap, std::max<size_t>(so, 256)))) return rc;
-  uint8_t* h = F->track_io.h_stage;
-  uint8_t* d = F->track_io.d_io;
-  uint8_t* sc = F->track_scratch;
-  const size_t sm_top = sizeof(okb_pair) * (size_t)AS_CHUNK * MAX_BEST;
-  size_t sm = sm_top;
+  const size_t out_end = st.off;
+  if ((rc = reserve(c, B, out_end, sc.off))) return rc;
+  uint8_t* h = B.h_stage;
+  uint8_t* d = B.d_stage;
+  AssignSmem sm;
   std::vector<int> maxA(R, 0);
   TrackJobDev* tj = reinterpret_cast<TrackJobDev*>(h);
   for (int t = 0; t < n_jobs; ++t) {
     const int i = order[t];
     const okb_track_job& j = jobs[i];
-    const WinStore& S = c->wins[j.win];
-    const FeatStore& FS = S.feat;
+    const FeatStore& FS = c->wins[j.win].feat;
     TrackJobDev J;
     std::memset(&J, 0, sizeof J);
     J.W = c->d_wins + j.win;
     J.pose_b = j.pose_b; J.sb_b = j.sb_b; J.feat_b = j.feat_slot_b; J.n_rounds = j.n_rounds;
     J.threshold = j.threshold;
     J.cnt_cap = std::max(c->host[j.win].L, 1);
-    J.cnt = reinterpret_cast<int*>(sc + o_cnt[i]);
+    J.cnt = reinterpret_cast<int*>(B.d_scratch + o_cnt[i]);
     J.hdr = reinterpret_cast<int*>(d + o_hdr[i]);
     J.assoc = reinterpret_cast<uint2*>(d + o_assoc[i]);
     J.uninit = reinterpret_cast<uint32_t*>(d + o_un[i]);
     tj[t] = J;
-    size_t q = o_rs[i];
     for (int r = 0; r < j.n_rounds; ++r) {
       const okb_track_round& Rr = j.rounds[r];
+      const RoundLay& x = rl[r0[i] + r];
       const size_t ia = (size_t)Rr.feat_slot_a * FS.C + Rr.cam_a, ib = (size_t)j.feat_slot_b * FS.C + Rr.cam_b;
-      const int nA = S.feat_n_pending[ia], nB = S.feat_n_pending[ib];
-      const size_t o_proj = q, o_unc = o_proj + 16 * (size_t)nA, o_top = o_unc + 32 * (size_t)nA, o_pairs = o_top + sizeof(okb_pair) * (size_t)nA * j.num_best;
-      const size_t o_sa = o_pairs + sizeof(okb_pair) * (size_t)nB, o_sb = o_sa + up16(nA), o_done = o_sb + up16(nB);
-      q = up256(o_done + up16(nA));
-      MatchJobDev jd;
-      std::memset(&jd, 0, sizeof jd);
-      jd.A = FS.desc + ia * FS.N * (FS.D / 4);
-      jd.B = FS.desc + ib * FS.N * (FS.D / 4);
-      jd.skipA = sc + o_sa; jd.skipB = sc + o_sb;
-      jd.topk = reinterpret_cast<okb_pair*>(sc + o_top);
-      jd.pairs = reinterpret_cast<okb_pair*>(sc + o_pairs);
-      jd.done = sc + o_done;
-      jd.nA = nA; jd.nB = nB; jd.num_best = j.num_best;
-      jd.list_thr = j.threshold; jd.gate_thr = j.threshold;          // Frontend's matcher: no ratio test
-      const size_t sm_b = (sizeof(okb_pair) + sizeof(int)) * (size_t)nB;
-      jd.in_smem = sm_top + sm_b + 1024 <= (size_t)c->smem_optin ? 1 : 0;
-      if (jd.in_smem) sm = std::max(sm, sm_top + sm_b);
+      MatchJobDev jd = store_match_job(c, FS, ia, ib, x.nA, x.nB, j.num_best, j.threshold, B.d_scratch, x.ms, sm);
       jd.gate.mode = OKB_GATE_3D2D;
-      jd.gate.kp_b = FS.kp + 2 * ib * FS.N;
-      jd.gate.kp_size_b = FS.size + ib * FS.N;
-      jd.gate.proj_into_b = reinterpret_cast<const double*>(sc + o_proj);
-      jd.gate.proj_unc = reinterpret_cast<const double*>(sc + o_unc);
+      jd.gate.proj_into_b = reinterpret_cast<const double*>(B.d_scratch + x.proj);
+      jd.gate.proj_unc = reinterpret_cast<const double*>(B.d_scratch + x.unc);
       reinterpret_cast<MatchJobDev*>(h + o_tab[r])[t] = jd;
       reinterpret_cast<TrackRoundDev*>(h + o_rinfo[r])[t] = TrackRoundDev{Rr.feat_slot_a, Rr.cam_a, Rr.cam_b, 0};
-      maxA[r] = std::max(maxA[r], nA);
+      maxA[r] = std::max(maxA[r], x.nA);
     }
   }
   FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
   const TrackJobDev* d_jobs = reinterpret_cast<const TrackJobDev*>(d);
-  if (sm > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
-  const int nw = desc_bytes / 4;
+  if ((rc = sm.set_attribute(c))) return rc;
+  const int nw = c->wins[jobs[0].win].feat.D / 4;
   for (int r = 0; r < R; ++r) {
     const MatchJobDev* d_tab = reinterpret_cast<const MatchJobDev*>(d + o_tab[r]);
     const TrackRoundDev* d_ri = reinterpret_cast<const TrackRoundDev*>(d + o_rinfo[r]);
+    const int n[2] = {0, m[r]}, max_a[2] = {0, maxA[r]};
     k_track_setup<<<m[r], TK_T, 0, xs>>>(d_jobs, d_tab, d_ri, r);
-    DISPATCH_NW(nw, (k_hamming_topk<NW, true><<<dim3(std::max(1, (maxA[r] + MW - 1) / MW), m[r]), MT, 0, xs>>>(d_tab)));
-    k_assign<<<m[r], AS_T, sm, xs>>>(d_tab);
+    if ((rc = launch_matcher(c, xs, d_tab, nw, n, max_a, sm))) return rc;
     k_track_apply<<<m[r], TK_T, 0, xs>>>(d_jobs, d_tab, d_ri, r);
   }
-  F->launches += 4 * (int64_t)R;
+  F->launches += 2 * (int64_t)R;
   FE_CUDA(c, cudaGetLastError());
   FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
   FE_CUDA(c, cudaStreamSynchronize(xs));
@@ -2333,7 +2360,7 @@ __global__ void __launch_bounds__(TK_T, 1) k_stereo_apply(const StereoJobDev* __
       }
     }
     int total_q;
-    const int pos_q = track_scan(need_qr, s_warp, &total_q);
+    const int pos_q = block_scan<TK_T>(need_qr, s_warp, &total_q);
     if (need_qr) s_list[pos_q] = b;
     __syncthreads();
     for (int i = warp; i < total_q; i += NWT) {
@@ -2357,7 +2384,7 @@ __global__ void __launch_bounds__(TK_T, 1) k_stereo_apply(const StereoJobDev* __
     __syncthreads();
     if (need_qr) cbi = s_ok[pos_q];
     int total;
-    const int pos = track_scan(rec, s_warp, &total);
+    const int pos = block_scan<TK_T>(rec, s_warp, &total);
     if (rec) {
       okb_stereo_match& o = J.out[n_out + pos];
       o.kp_a = a; o.kp_b = b; o.lm_slot_a = la; o.lm_slot_b = lb; o.can_be_initialized = cbi; o._pad = 0;
@@ -2369,17 +2396,14 @@ __global__ void __launch_bounds__(TK_T, 1) k_stereo_apply(const StereoJobDev* __
 }
 }  // namespace
 
-// Host checks of one job (against the store as the pending commands leave it); "" = valid.
-static std::string match2d2d_job_invalid(okb_ctx* c, const okb_match2d2d_job& j, int desc_bytes, std::vector<char>& seen) {
-  if (j.win < 0 || j.win >= c->max_windows) return "window slot out of range";
+// Host checks of one job (first_win: the window of the call's first job, already checked); "" = valid.
+static std::string match2d2d_job_invalid(okb_ctx* c, const okb_match2d2d_job& j, int first_win, std::vector<char>& seen) {
+  const std::string why = store_window_invalid(c, j.win, seen);
+  if (!why.empty()) return why;
   const WinStore& S = c->wins[j.win];
   const WinDev& W = c->host[j.win];
-  if (!S.uploaded) return "window slot not uploaded";
-  if (!S.feat_mem) return "window has no feature store (okb_window_reserve_features)";
-  if (seen[j.win]) return "window listed twice";
-  seen[j.win] = 1;
   const FeatStore& F = S.feat;
-  if (F.D != desc_bytes) return "descriptor length differs from the call's first job";
+  if (F.D != c->wins[first_win].feat.D) return "descriptor length differs from the call's first job";
   if (j.pose_a < 0 || j.pose_a >= W.K) return "pose_a out of range";
   if (j.pose_b < 0 || j.pose_b >= W.K) return "pose_b out of range";
   if (j.sb_current < -1 || j.sb_current >= W.NSB) return "sb_current out of range";
@@ -2402,75 +2426,52 @@ static std::string match2d2d_job_invalid(okb_ctx* c, const okb_match2d2d_job& j,
 // okb_match2d2d_batch and okb_stereo_init_batch (which passes its jobs with frame A = frame B); `fn` names the entry
 // point in the errors.
 static int match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs, const char* fn) {
-  if (n_jobs > 65535) { c->set_error(std::string(fn) + ": more than 65535 jobs"); return OKB_ERR_INVALID_ARG; }   // grid dimension
-  if (c->shard_world > 1) { c->set_error(std::string(fn) + ": landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
-  const int desc_bytes = (jobs[0].win >= 0 && jobs[0].win < c->max_windows) ? c->wins[jobs[0].win].feat.D : 0;
-  std::vector<char> seen(c->max_windows, 0);
-  for (int i = 0; i < n_jobs; ++i) {
-    const std::string why = match2d2d_job_invalid(c, jobs[i], desc_bytes, seen);
-    if (!why.empty()) { c->set_error(std::string(fn) + ": jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
-  }
+  int rc = store_call_checks(c, fn, n_jobs, jobs, 65535, [&](int i, std::vector<char>& seen) {      // grid dimension
+    return match2d2d_job_invalid(c, jobs[i], jobs[0].win, seen);
+  });
+  if (rc || n_jobs == 0) return rc;
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
-  std::lock_guard<std::mutex> lk(F->stereo_mtx);
-  {     // pending edits first, one commit per run of consecutive windows
-    std::vector<int32_t> wl(n_jobs);
-    for (int i = 0; i < n_jobs; ++i) wl[i] = jobs[i].win;
-    std::sort(wl.begin(), wl.end());
-    for (int i = 0; i < n_jobs;) {
-      int k = i + 1;
-      while (k < n_jobs && wl[k] == wl[k - 1] + 1) ++k;
-      const int rc = okb_commit_range(c, wl[i], k - i);
-      if (rc) return rc;
-      i = k;
-    }
-  }
+  CallBuffers& B = F->stereo;
+  std::lock_guard<std::mutex> lk(B.mtx);
+  if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
   cudaStream_t xs = c->stream_xfer;
-  for (int i = 0; i < n_jobs; ++i) {
-    const WinStore& S = c->wins[jobs[i].win];
-    if (S.done_idx >= 0) FE_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
-  }
   // staging (pinned + device mirror): in  = [job table | match table]
   //                                   out = [per job: count | records]
-  // scratch (device only), per job: geometry | bearings A, B | ray sigmas A, B | top-k | winners | skipA | skipB | done |
-  //                                 rank-test Jacobians
-  auto up16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
-  const size_t o_tab = up256(sizeof(StereoJobDev) * n_jobs);
-  const size_t in_bytes = up256(o_tab + sizeof(MatchJobDev) * n_jobs);
-  std::vector<int> nA(n_jobs), nB(n_jobs);
-  std::vector<size_t> o_out(n_jobs), o_sc(n_jobs);
-  size_t off = in_bytes, so = 0;
+  // scratch (device only), per job: geometry | bearings A, B | ray sigmas A, B | the matcher's arrays | rank-test Jacobians
+  struct JobLay { int nA, nB; size_t out, geo, ba, bb, rsa, rsb, uj; MatchScratch ms; };
+  std::vector<JobLay> L(n_jobs);
+  Carve st, sc;
+  st.take(sizeof(StereoJobDev) * n_jobs, 256);
+  const size_t o_tab = st.take(sizeof(MatchJobDev) * n_jobs, 256);
+  const size_t in_bytes = st.off;
   for (int i = 0; i < n_jobs; ++i) {
     const okb_match2d2d_job& j = jobs[i];
     const WinStore& S = c->wins[j.win];
-    nA[i] = S.feat_n_pending[(size_t)j.feat_slot_a * S.feat.C + j.cam_a];
-    nB[i] = S.feat_n_pending[(size_t)j.feat_slot_b * S.feat.C + j.cam_b];
-    o_out[i] = off;
-    off = up16(off + 16 + sizeof(okb_stereo_match) * (size_t)nB[i]);
-    o_sc[i] = so;
-    const size_t a = nA[i], b = nB[i];
-    so = up256(so + 8 * kGeo + 24 * a + 24 * b + 8 * a + 8 * b + sizeof(okb_pair) * a * j.num_best + sizeof(okb_pair) * b +
-               up16(a) + up16(b) + up16(a) + 8 * kUJ * b + 12 * 16);      // 12 arrays, each 16-byte aligned
+    JobLay& l = L[i];
+    l.nA = S.feat_n_pending[(size_t)j.feat_slot_a * S.feat.C + j.cam_a];
+    l.nB = S.feat_n_pending[(size_t)j.feat_slot_b * S.feat.C + j.cam_b];
+    const size_t a = l.nA, b = l.nB;
+    l.out = st.take(16 + sizeof(okb_stereo_match) * b);
+    l.geo = sc.take(8 * kGeo);
+    l.ba = sc.take(24 * a); l.bb = sc.take(24 * b);
+    l.rsa = sc.take(8 * a); l.rsb = sc.take(8 * b);
+    l.ms = carve_match(sc, a, b, j.num_best);
+    l.uj = sc.take(8 * kUJ * b);
   }
-  const size_t out_end = off;
-  int rc;
-  if ((rc = grow_pinned(c, &F->stereo_io.h_stage, &F->stereo_io.h_stage_cap, out_end))) return rc;
-  if ((rc = grow(c, &F->stereo_io.d_io, &F->stereo_io.d_io_cap, out_end))) return rc;
-  if ((rc = grow(c, &F->stereo_scratch, &F->stereo_scratch_cap, std::max<size_t>(so, 256)))) return rc;
-  uint8_t* h = F->stereo_io.h_stage;
-  uint8_t* d = F->stereo_io.d_io;
-  uint8_t* sc = F->stereo_scratch;
-  const size_t sm_top = sizeof(okb_pair) * (size_t)AS_CHUNK * MAX_BEST;
-  size_t sm = sm_top;
+  const size_t out_end = st.off;
+  if ((rc = reserve(c, B, out_end, sc.off))) return rc;
+  uint8_t* h = B.h_stage;
+  uint8_t* d = B.d_stage;
+  uint8_t* s = B.d_scratch;
+  AssignSmem sm;
   int maxA = 0, maxN = 0;
   StereoJobDev* tj = reinterpret_cast<StereoJobDev*>(h);
   MatchJobDev* tm = reinterpret_cast<MatchJobDev*>(h + o_tab);
   for (int i = 0; i < n_jobs; ++i) {
     const okb_match2d2d_job& j = jobs[i];
     const FeatStore& FS = c->wins[j.win].feat;
-    const size_t a = nA[i], b = nB[i];
-    size_t q = o_sc[i];
-    auto take = [&](size_t bytes) { const size_t o = q; q = up16(q + bytes); return sc + o; };
+    const JobLay& l = L[i];
     StereoJobDev J;
     std::memset(&J, 0, sizeof J);
     J.W = c->d_wins + j.win;
@@ -2478,67 +2479,51 @@ static int match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs
     J.pose_b = j.pose_b; J.feat_b = j.feat_slot_b; J.cam_b = j.cam_b;
     J.sb = j.feat_slot_a != j.feat_slot_b ? j.sb_current : -1;
     J.threshold = j.threshold;
-    J.geo = reinterpret_cast<double*>(take(8 * kGeo));
-    J.n_out = reinterpret_cast<int*>(d + o_out[i]);
-    J.out = reinterpret_cast<okb_stereo_match*>(d + o_out[i] + 16);
-    MatchJobDev jd;
-    std::memset(&jd, 0, sizeof jd);
+    J.geo = reinterpret_cast<double*>(s + l.geo);
+    J.uj = reinterpret_cast<double*>(s + l.uj);
+    J.n_out = reinterpret_cast<int*>(d + l.out);
+    J.out = reinterpret_cast<okb_stereo_match*>(d + l.out + 16);
     const size_t ia = (size_t)j.feat_slot_a * FS.C + j.cam_a, ib = (size_t)j.feat_slot_b * FS.C + j.cam_b;
-    jd.A = FS.desc + ia * FS.N * (FS.D / 4);
-    jd.B = FS.desc + ib * FS.N * (FS.D / 4);
+    MatchJobDev jd = store_match_job(c, FS, ia, ib, l.nA, l.nB, j.num_best, j.threshold, s, l.ms, sm);
     GateDev& g = jd.gate;                     // geometry and cameras: k_stereo_setup
     g.mode = OKB_GATE_2D2D;
     g.kp_a = FS.kp + 2 * ia * FS.N; g.kp_size_a = FS.size + ia * FS.N;
-    g.kp_b = FS.kp + 2 * ib * FS.N; g.kp_size_b = FS.size + ib * FS.N;
-    g.bearing_a = reinterpret_cast<const double*>(take(24 * a));
-    g.bearing_b = reinterpret_cast<const double*>(take(24 * b));
-    g.ray_sigma_a = reinterpret_cast<const double*>(take(8 * a));
-    g.ray_sigma_b = reinterpret_cast<const double*>(take(8 * b));
-    jd.topk = reinterpret_cast<okb_pair*>(take(sizeof(okb_pair) * a * j.num_best));
-    jd.pairs = reinterpret_cast<okb_pair*>(take(sizeof(okb_pair) * b));
-    jd.skipA = take(a); jd.skipB = take(b); jd.done = take(a);
-    J.uj = reinterpret_cast<double*>(take(8 * kUJ * b));
-    jd.nA = (int)a; jd.nB = (int)b; jd.num_best = j.num_best;
-    jd.list_thr = j.threshold; jd.gate_thr = j.threshold;          // Frontend's matcher: no ratio test
-    const size_t sm_b = (sizeof(okb_pair) + sizeof(int)) * b;
-    jd.in_smem = sm_top + sm_b + 1024 <= (size_t)c->smem_optin ? 1 : 0;
-    if (jd.in_smem) sm = std::max(sm, sm_top + sm_b);
+    g.bearing_a = reinterpret_cast<const double*>(s + l.ba);
+    g.bearing_b = reinterpret_cast<const double*>(s + l.bb);
+    g.ray_sigma_a = reinterpret_cast<const double*>(s + l.rsa);
+    g.ray_sigma_b = reinterpret_cast<const double*>(s + l.rsb);
     tj[i] = J;
     tm[i] = jd;
-    maxA = std::max(maxA, (int)a);
-    maxN = std::max(maxN, (int)std::max(a, b));
+    maxA = std::max(maxA, l.nA);
+    maxN = std::max(maxN, std::max(l.nA, l.nB));
   }
   FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
   const StereoJobDev* d_jobs = reinterpret_cast<const StereoJobDev*>(d);
   MatchJobDev* d_tab = reinterpret_cast<MatchJobDev*>(d + o_tab);
-  if (sm > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
-  const int nw = desc_bytes / 4;
+  if ((rc = sm.set_attribute(c))) return rc;
+  const int n[2] = {0, n_jobs}, max_a[2] = {0, maxA};
   k_stereo_setup<<<dim3(std::max(1, (maxN + TK_T - 1) / TK_T), n_jobs, 2), TK_T, 0, xs>>>(d_jobs, d_tab);
-  DISPATCH_NW(nw, (k_hamming_topk<NW, true><<<dim3(std::max(1, (maxA + MW - 1) / MW), n_jobs), MT, 0, xs>>>(d_tab)));
-  k_assign<<<n_jobs, AS_T, sm, xs>>>(d_tab);
+  if ((rc = launch_matcher(c, xs, d_tab, c->wins[jobs[0].win].feat.D / 4, n, max_a, sm))) return rc;
   k_stereo_apply<<<n_jobs, TK_T, 0, xs>>>(d_jobs, d_tab);
-  F->launches += 4;
+  F->launches += 2;
   FE_CUDA(c, cudaGetLastError());
   FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
   FE_CUDA(c, cudaStreamSynchronize(xs));
   for (int i = 0; i < n_jobs; ++i) {
-    const int n = *reinterpret_cast<const int32_t*>(h + o_out[i]);
-    *jobs[i].n_out = n;
-    if (n) std::memcpy(jobs[i].out, h + o_out[i] + 16, sizeof(okb_stereo_match) * (size_t)n);
+    const int n_rec = *reinterpret_cast<const int32_t*>(h + L[i].out);
+    *jobs[i].n_out = n_rec;
+    if (n_rec) std::memcpy(jobs[i].out, h + L[i].out + 16, sizeof(okb_stereo_match) * (size_t)n_rec);
   }
   return OKB_OK;
 }
 
 extern "C" int okb_match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs) {
-  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
-  if (n_jobs == 0) return OKB_OK;
   return match2d2d_batch(c, n_jobs, jobs, "okb_match2d2d_batch");
 }
 
 extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_job* jobs) {
-  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
-  if (n_jobs == 0) return OKB_OK;
-  std::vector<okb_match2d2d_job> mj(n_jobs);
+  if (n_jobs > 0 && !jobs) return OKB_ERR_INVALID_ARG;      // read here; match2d2d_batch checks the rest
+  std::vector<okb_match2d2d_job> mj(std::max(n_jobs, 0));
   for (int i = 0; i < n_jobs; ++i) {
     const okb_stereo_job& j = jobs[i];
     mj[i] = okb_match2d2d_job{j.win, j.pose, j.feat_slot, j.cam_a, j.pose, j.feat_slot, j.cam_b, -1, j.threshold, j.num_best,
@@ -2563,7 +2548,7 @@ extern "C" int okb_stereo_init_batch(okb_ctx* c, int n_jobs, const okb_stereo_jo
 // maxima and the decision.  The call writes nothing but its scratch and its results.
 // =================================================================================================
 namespace {
-constexpr int KF_T = TK_T;               // threads per CTA (track_scan assumes TK_T)
+constexpr int KF_T = TK_T;               // threads per CTA
 constexpr int KF_SMEM_PTS = 2048;        // largest image kept in shared memory (buffers of 24 B per point)
 
 struct KfCtaDev {                        // one (job, camera)
@@ -2724,8 +2709,8 @@ __device__ int kf_hull(const FeatStore& F, size_t base, int n, int n_in, bool ma
       }
     }
     int t_in, t_out;
-    const int r_in = track_scan(inc, S.warp_i, &t_in);
-    const int r_out = track_scan(keep, S.warp_i, &t_out);
+    const int r_in = block_scan<KF_T>(inc, S.warp_i, &t_in);
+    const int r_out = block_scan<KF_T>(keep, S.warp_i, &t_out);
     if (keep) {
       const int o = run_out + r_out;
       B.key[o] = ((unsigned long long)kf_f2s((float)F.kp[2 * (base + k)]) << 32) | kf_f2s((float)F.kp[2 * (base + k) + 1]);
@@ -2921,14 +2906,11 @@ __global__ void __launch_bounds__(KF_T) k_keyframe_overlap(const KfCtaDev* __res
 }
 }  // namespace
 
-// Host checks of one job (against the store as the pending commands leave it); "" = valid.
+// Host checks of one job; "" = valid.
 static std::string keyframe_job_invalid(okb_ctx* c, const okb_keyframe_job& j, std::vector<char>& seen) {
-  if (j.win < 0 || j.win >= c->max_windows) return "window slot out of range";
+  const std::string why = store_window_invalid(c, j.win, seen);
+  if (!why.empty()) return why;
   const WinStore& S = c->wins[j.win];
-  if (!S.uploaded) return "window slot not uploaded";
-  if (!S.feat_mem) return "window has no feature store (okb_window_reserve_features)";
-  if (seen[j.win]) return "window listed twice";
-  seen[j.win] = 1;
   const FeatStore& F = S.feat;
   if (j.feat_slot < 0 || j.feat_slot >= F.F) return "feat_slot out of range";
   if (j.n_cams < 1 || j.n_cams > F.C) return "n_cams out of range (1..the store's cameras)";
@@ -2939,51 +2921,29 @@ static std::string keyframe_job_invalid(okb_ctx* c, const okb_keyframe_job& j, s
 }
 
 extern "C" int okb_keyframe_overlap_batch(okb_ctx* c, int n_jobs, const okb_keyframe_job* jobs) {
-  if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
-  if (n_jobs == 0) return OKB_OK;
-  if (c->shard_world > 1) { c->set_error("okb_keyframe_overlap_batch: landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
-  std::vector<char> seen(c->max_windows, 0);
-  for (int i = 0; i < n_jobs; ++i) {
-    const std::string why = keyframe_job_invalid(c, jobs[i], seen);
-    if (!why.empty()) { c->set_error("okb_keyframe_overlap_batch: jobs[" + std::to_string(i) + "]: " + why); return OKB_ERR_INVALID_ARG; }
-  }
+  int rc = store_call_checks(c, "okb_keyframe_overlap_batch", n_jobs, jobs, INT_MAX,
+                             [&](int i, std::vector<char>& seen) { return keyframe_job_invalid(c, jobs[i], seen); });
+  if (rc || n_jobs == 0) return rc;
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
-  std::lock_guard<std::mutex> lk(F->kf_mtx);
-  {     // pending edits first, one commit per run of consecutive windows
-    std::vector<int32_t> wl(n_jobs);
-    for (int i = 0; i < n_jobs; ++i) wl[i] = jobs[i].win;
-    std::sort(wl.begin(), wl.end());
-    for (int i = 0; i < n_jobs;) {
-      int k = i + 1;
-      while (k < n_jobs && wl[k] == wl[k - 1] + 1) ++k;
-      const int rc = okb_commit_range(c, wl[i], k - i);
-      if (rc) return rc;
-      i = k;
-    }
-  }
+  CallBuffers& B = F->kf;
+  std::lock_guard<std::mutex> lk(B.mtx);
+  if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
   cudaStream_t xs = c->stream_xfer;
-  for (int i = 0; i < n_jobs; ++i) {
-    const WinStore& S = c->wins[jobs[i].win];
-    if (S.done_idx >= 0) FE_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
-  }
   // staging (pinned + device mirror): in  = [per job: done counter | CTA table]
   //                                   out = [per job: result | camera records]
   // scratch (device only): the point buffers of the images above the shared-memory capacity
   int n_cta = 0;
   for (int i = 0; i < n_jobs; ++i) n_cta += jobs[i].n_cams;
-  const size_t o_tab = up256(sizeof(int) * (size_t)n_jobs);
-  const size_t in_bytes = up256(o_tab + sizeof(KfCtaDev) * (size_t)n_cta);
+  Carve st, sc;
+  st.take(sizeof(int) * (size_t)n_jobs, 256);
+  const size_t o_tab = st.take(sizeof(KfCtaDev) * (size_t)n_cta, 256);
+  const size_t in_bytes = st.off;
   std::vector<size_t> o_out(n_jobs);
-  size_t off = in_bytes;
-  for (int i = 0; i < n_jobs; ++i) {
-    o_out[i] = off;
-    off = up256(off + sizeof(okb_keyframe_result) + sizeof(okb_keyframe_cam) * (size_t)jobs[i].n_cams);
-  }
-  const size_t out_end = off;
+  for (int i = 0; i < n_jobs; ++i) o_out[i] = st.take(sizeof(okb_keyframe_result) + sizeof(okb_keyframe_cam) * (size_t)jobs[i].n_cams, 256);
+  const size_t out_end = st.off;
   auto pow2 = [](int v) { int p = 32; while (p < v) p <<= 1; return p; };
   int smem_cap = 32;
-  size_t so = 0;
   std::vector<size_t> o_sc(n_cta, SIZE_MAX);
   std::vector<int> caps(n_cta);
   for (int i = 0, t = 0; i < n_jobs; ++i) {
@@ -2992,15 +2952,12 @@ extern "C" int okb_keyframe_overlap_batch(okb_ctx* c, int n_jobs, const okb_keyf
       const int n = S.feat_n_pending[(size_t)jobs[i].feat_slot * S.feat.C + cam];
       caps[t] = pow2(n);
       if (n <= KF_SMEM_PTS) smem_cap = std::max(smem_cap, caps[t]);
-      else { o_sc[t] = so; so = up256(so + kf_buf_bytes(caps[t])); }
+      else o_sc[t] = sc.take(kf_buf_bytes(caps[t]), 256);
     }
   }
-  int rc;
-  if ((rc = grow_pinned(c, &F->kf_io.h_stage, &F->kf_io.h_stage_cap, out_end))) return rc;
-  if ((rc = grow(c, &F->kf_io.d_io, &F->kf_io.d_io_cap, out_end))) return rc;
-  if (so && (rc = grow(c, &F->kf_scratch, &F->kf_scratch_cap, so))) return rc;
-  uint8_t* h = F->kf_io.h_stage;
-  uint8_t* d = F->kf_io.d_io;
+  if ((rc = reserve(c, B, out_end, sc.off))) return rc;
+  uint8_t* h = B.h_stage;
+  uint8_t* d = B.d_stage;
   std::memset(h, 0, o_tab);
   KfCtaDev* tc = reinterpret_cast<KfCtaDev*>(h + o_tab);
   for (int i = 0, t = 0; i < n_jobs; ++i) {
@@ -3014,7 +2971,7 @@ extern "C" int okb_keyframe_overlap_batch(okb_ctx* c, int n_jobs, const okb_keyf
       J.res = reinterpret_cast<okb_keyframe_result*>(d + o_out[i]);
       J.cams = reinterpret_cast<okb_keyframe_cam*>(d + o_out[i] + sizeof(okb_keyframe_result));
       J.done = reinterpret_cast<int*>(d) + i;
-      J.buf = o_sc[t] == SIZE_MAX ? nullptr : F->kf_scratch + o_sc[t];
+      J.buf = o_sc[t] == SIZE_MAX ? nullptr : B.d_scratch + o_sc[t];
       J.cap = o_sc[t] == SIZE_MAX ? smem_cap : caps[t];
       tc[t] = J;
     }
