@@ -54,13 +54,22 @@ struct WinStore {
 // sorting, then makes the transfer stream wait once on each distinct solver event of those slots (okb_estimator.cu).
 int okb_commit_windows(okb_ctx* c, const int32_t* wins, int n);
 
-// Buffers of okb_imu_propagate*: [job table | samples] in, [per-job outputs] out, in one pinned buffer and its device
-// mirror; they grow with the largest call and are kept.
-struct PropBuffers {
-  unsigned char* host = nullptr;     // pinned
-  unsigned char* dev = nullptr;
-  size_t bytes = 0;
-  std::mutex mtx;                    // serialises the calls that use these buffers
+// Buffers of one kind of table-driven call: a pinned staging buffer and its device mirror (tables in, results out, one
+// copy each way), device-only scratch, and the mutex that serialises the calls using them.  They grow with the largest
+// call and are kept.  The Hamming matcher's sets are held under match_mtx / batch_mtx, which guard other buffers too.
+struct CallBuffers {
+  uint8_t* h_stage = nullptr;      // pinned
+  uint8_t* d_stage = nullptr;
+  uint8_t* d_scratch = nullptr;
+  size_t h_stage_cap = 0, d_stage_cap = 0, d_scratch_cap = 0;
+  std::mutex mtx;
+  // Grows the buffers to `stage` bytes of staging (pinned and its device mirror) and `scratch` bytes of device scratch.
+  int reserve(okb_ctx* c, size_t stage, size_t scratch);
+  void release() {
+    if (h_stage) cudaFreeHost(h_stage);
+    cudaFree(d_stage);
+    cudaFree(d_scratch);
+  }
 };
 
 struct okb_frontend_state;
@@ -107,7 +116,7 @@ struct okb_ctx {
   okb::WinDev* d_wins = nullptr;
   okb::SolverState* d_states = nullptr;
   okb::SolverState* h_states = nullptr;  // pinned
-  void* hook_buf = nullptr;
+  unsigned char* hook_buf = nullptr;
   size_t hook_bytes = 0;
   // okb_window_marginalize*: task table + job payloads of a call, packed in pinned memory and copied in one piece
   unsigned char* marg_host = nullptr;    // pinned
@@ -124,7 +133,8 @@ struct okb_ctx {
   struct MargPinned { unsigned char* p; size_t bytes; cudaEvent_t done; };
   std::vector<MargPinned> marg_pool;
   // okb_imu_propagate (on `stream`) and okb_imu_propagate_batch (on stream_prop, created on first use) each own a set
-  PropBuffers prop_one, prop_batch;
+  // of staging buffers ([job table | samples] in, [per-job outputs] out; no scratch)
+  CallBuffers prop_one, prop_batch;
   cudaStream_t stream_prop = nullptr;
   std::atomic<int64_t> prop_launches{0};   // counted apart from `launches`: a batch may run beside a solve's launches
   okb_frontend_state* frontend = nullptr;
@@ -156,6 +166,57 @@ struct okb_ctx {
   std::mutex error_mu;                    // uploads of different slots may run on several host threads
   void set_error(const std::string& e) { std::lock_guard<std::mutex> g(error_mu); error = e; }
 };
+
+// Returns OKB_ERR_CUDA with the failing call and the CUDA error as the context's error text unless `call` succeeds.
+#define OKB_CUDA(ctx, call)                                                     \
+  do {                                                                          \
+    cudaError_t e_ = (call);                                                    \
+    if (e_ != cudaSuccess) {                                                    \
+      (ctx)->set_error(std::string(#call) + ": " + cudaGetErrorString(e_));     \
+      return OKB_ERR_CUDA;                                                      \
+    }                                                                           \
+  } while (0)
+
+// Grows the device allocation *p to at least `need` elements: frees it and allocates exactly `need`; contents are lost.
+template <typename T>
+int grow(okb_ctx* c, T** p, size_t* cap, size_t need) {
+  if (*cap >= need) return OKB_OK;
+  cudaFree(*p);
+  *p = nullptr; *cap = 0;
+  OKB_CUDA(c, cudaMalloc(p, need * sizeof(T)));
+  *cap = need;
+  return OKB_OK;
+}
+
+// grow for pinned host memory.
+template <typename T>
+int grow_pinned(okb_ctx* c, T** p, size_t* cap, size_t need) {
+  if (*cap >= need) return OKB_OK;
+  if (*p) cudaFreeHost(*p);
+  *p = nullptr; *cap = 0;
+  OKB_CUDA(c, cudaMallocHost(p, need * sizeof(T)));
+  *cap = need;
+  return OKB_OK;
+}
+
+inline int CallBuffers::reserve(okb_ctx* c, size_t stage, size_t scratch) {
+  int rc;
+  if ((rc = grow_pinned(c, &h_stage, &h_stage_cap, stage)) || (rc = grow(c, &d_stage, &d_stage_cap, stage)) ||
+      (rc = grow(c, &d_scratch, &d_scratch_cap, scratch)))
+    return rc;
+  return OKB_OK;
+}
+
+// Makes `stream` wait once on each distinct solver event (done_ring entry) of the n listed slots, so that what is
+// queued on it next runs after the solver work already launched on them.
+inline int wait_solver_work(okb_ctx* c, cudaStream_t stream, const int32_t* slots, int n) {
+  bool waited[okb_ctx::kDoneRing] = {};
+  for (int i = 0; i < n; ++i) {
+    const int k = c->wins[slots[i]].done_idx;
+    if (k >= 0 && !waited[k]) { OKB_CUDA(c, cudaStreamWaitEvent(stream, c->done_ring[k], 0)); waited[k] = true; }
+  }
+  return OKB_OK;
+}
 
 void okb_frontend_release(okb_ctx* c);
 int64_t okb_frontend_launches(const okb_ctx* c);   // kernel launches of the frontend calls (counted atomically)

@@ -8,7 +8,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include "okb_ctx.h"
@@ -20,15 +19,6 @@
 using namespace okb;
 
 static std::string g_create_error;
-
-#define OKB_CUDA(ctx, call)                                                                             \
-  do {                                                                                                  \
-    cudaError_t e_ = (call);                                                                            \
-    if (e_ != cudaSuccess) {                                                                            \
-      (ctx)->set_error(std::string(#call) + ": " + cudaGetErrorString(e_));                             \
-      return OKB_ERR_CUDA;                                                                              \
-    }                                                                                                   \
-  } while (0)
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -70,7 +60,7 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
   if (cudaSetDevice(device_id) == cudaSuccess) cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest);
   if (cudaSetDevice(device_id) != cudaSuccess || cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, prio_greatest) != cudaSuccess) {
     g_create_error = "cudaSetDevice / cudaStreamCreate failed";
-    delete c;
+    okb_ctx_destroy(c);
     return OKB_ERR_CUDA;
   }
   if (cudaStreamCreateWithPriority(&c->stream_imu, cudaStreamNonBlocking, prio_least) != cudaSuccess ||
@@ -79,7 +69,7 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
       create_high_priority_stream(&c->stream_xfer) != cudaSuccess ||
       cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess) {
     g_create_error = "cudaStreamCreate / cudaEventCreate failed";
-    delete c;
+    okb_ctx_destroy(c);
     return OKB_ERR_CUDA;
   }
   c->group_stream[0] = c->stream; c->group_imu[0] = c->stream_imu;
@@ -115,7 +105,7 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
       cudaMalloc(&c->d_ident, sizeof(int32_t) * max_windows) != cudaSuccess ||
       cudaMallocHost(&c->h_slot_ring, sizeof(int32_t) * okb_ctx::kDoneRing * max_windows) != cudaSuccess) {
     g_create_error = "cudaMalloc failed";
-    delete c;
+    okb_ctx_destroy(c);
     return OKB_ERR_CUDA;
   }
   cudaMemset(c->d_states, 0, sizeof(SolverState) * max_windows);
@@ -145,7 +135,7 @@ extern "C" int okb_ctx_create(int device_id, int max_windows, okb_ctx** out) {
 extern "C" void okb_ctx_destroy(okb_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
-  cudaStreamSynchronize(c->stream);
+  if (c->stream) cudaStreamSynchronize(c->stream);      // null when okb_ctx_create failed before creating it
   if (c->stream_xfer) cudaStreamSynchronize(c->stream_xfer);
   for (auto& w : c->wins) {
     if (w.arena) cudaFree(w.arena);
@@ -176,10 +166,8 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
   for (unsigned char* p : c->marg_retired_dev) cudaFree(p);
   for (unsigned char* p : c->marg_retired_host) cudaFreeHost(p);
   for (auto& e : c->marg_pool) { cudaFreeHost(e.p); cudaEventDestroy(e.done); }
-  for (PropBuffers* b : {&c->prop_one, &c->prop_batch}) {
-    if (b->host) cudaFreeHost(b->host);
-    if (b->dev) cudaFree(b->dev);
-  }
+  c->prop_one.release();
+  c->prop_batch.release();
   if (c->stream_prop) cudaStreamDestroy(c->stream_prop);
   for (auto& g : c->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   for (auto e : c->prof_events) cudaEventDestroy(e);
@@ -195,7 +183,7 @@ extern "C" void okb_ctx_destroy(okb_ctx* c) {
   if (c->ev_round) cudaEventDestroy(c->ev_round);
   if (c->ev_imu) cudaEventDestroy(c->ev_imu);
   if (c->stream_imu) cudaStreamDestroy(c->stream_imu);
-  cudaStreamDestroy(c->stream);
+  if (c->stream) cudaStreamDestroy(c->stream);
   delete c;
 }
 
@@ -209,15 +197,6 @@ extern "C" void* okb_stream(const okb_ctx* c) { return c ? (void*)c->stream : nu
 // window graph: capacities, arena, command staging, commit (device side: okb_graph.cuh)
 // ---------------------------------------------------------------------------------------------
 namespace {
-struct ArenaPlan {
-  size_t total = 0;
-  size_t take(size_t bytes) {
-    const size_t o = total;
-    total = align_up(total + bytes, 256);
-    return o;
-  }
-};
-
 // Orders the solver stream after every transfer issued so far.
 int join_transfers(okb_ctx* c) {
   if (cudaEventRecord(c->ev_join, c->stream_xfer) != cudaSuccess) return 1;
@@ -230,19 +209,6 @@ void mark_work(okb_ctx* c, const int32_t* slots, int n) {
   cudaEventRecord(c->done_ring[k], c->stream);
   for (int t = 0; t < n; ++t) c->wins[slots[t]].done_idx = k;
 }
-// Calls f(first, count) for each run of consecutive slots of a list, in list order (a range is one run).
-template <class F>
-int for_runs(const int32_t* slots, int n, F&& f) {
-  for (int i = 0; i < n;) {
-    int j = i + 1;
-    while (j < n && slots[j] == slots[j - 1] + 1) ++j;
-    const int rc = f(slots[i], j - i);
-    if (rc) return rc;
-    i = j;
-  }
-  return 0;
-}
-
 inline bool caps_cover(const WinCaps& a, const WinCaps& b) {
   return a.K >= b.K && a.L >= b.L && a.O >= b.O && a.S >= b.S && a.T >= b.T && a.NE >= b.NE && a.NC >= b.NC && a.PP >= b.PP && a.MN >= b.MN;
 }
@@ -275,56 +241,48 @@ void derive_dims(WinDev& W) {
 // full upload).
 int plan_arena(okb_ctx* c, int win, const WinCaps& q) {
   WinStore& S = c->wins[win];
-  ArenaPlan P;
+  Carve P;
+  auto take = [&P](size_t bytes) { return P.take(bytes, 256); };     // every array on a 256-byte boundary
   int CPc = 1;
   while (CPc < q.NC) CPc <<= 1;
   const int Kc = q.K, Lc = q.L, Lpc = (Lc + 31) & ~31;
   const int NSc = Kc * CPc, NSPc = (NSc + 31) / 32 * 32;
   const int dcc = 6 * Kc, dcap = 15 * Kc, dcpc = 4 * ((dcc + 1 + 3) / 4);
   const int MN = std::max(q.MN, 1), MB = kMaxMargBlocks;
-  const size_t o_pose = P.take(8 * 7 * Kc), o_sb = P.take(8 * 9 * Kc), o_ext = P.take(8 * 7 * q.NE), o_mlm = P.take(8 * 4 * (size_t)Lpc);
-  const size_t o_out = P.take(8 * (16 * (size_t)Kc + 4 + 5 * (size_t)Lc));
-  const size_t o_cams = P.take(sizeof(okb_camera) * q.NC), o_obs = P.take(sizeof(okb_observation) * (size_t)std::max(q.O, 1));
-  const size_t o_imut = P.take(sizeof(okb_imu_term) * std::max(q.T, 1)), o_samp = P.take(sizeof(okb_imu_sample) * (size_t)std::max(q.S, 1));
-  const size_t o_pp = P.take(sizeof(okb_pose_prior) * std::max(q.PP, 1)), o_sbp = P.take(sizeof(okb_sb_prior) * std::max(q.PP, 1));
-  const size_t o_mkind = P.take(4 * MB), o_midx = P.take(4 * MB), o_mcol = P.take(4 * MB), o_moff = P.take(4 * MB);
-  const size_t o_mx0 = P.take(8 * 9 * MB), o_mJ = P.take(8 * (size_t)MN * MN), o_me0 = P.take(8 * MN), o_mH0 = P.take(8 * (size_t)MN * MN);
-  const size_t o_mHs = P.take(8 * (size_t)MN * MN), o_mb0 = P.take(8 * MN);
-  const size_t o_mlmi = P.take(8 * 4 * (size_t)Lpc), o_mark = P.take(Lpc), o_mvis = P.take(4 * (size_t)Lpc);
-  const size_t o_bitmap = P.take(4 * (((size_t)NSc * Lc + 31) / 32 + 1));
-  const size_t o_perm = P.take(4 * (size_t)Lpc), o_inv = P.take(4 * (size_t)Lpc), o_trange = P.take(4 * (size_t)(Lpc / 32 + 1)), o_vis = P.take(4 * (size_t)Lpc);
-  const size_t o_slots = P.take(sizeof(SlotInfo) * NSPc);
+  const size_t o_pose = take(8 * 7 * Kc), o_sb = take(8 * 9 * Kc), o_ext = take(8 * 7 * q.NE), o_mlm = take(8 * 4 * (size_t)Lpc);
+  const size_t o_out = take(8 * (16 * (size_t)Kc + 4 + 5 * (size_t)Lc));
+  const size_t o_cams = take(sizeof(okb_camera) * q.NC), o_obs = take(sizeof(okb_observation) * (size_t)std::max(q.O, 1));
+  const size_t o_imut = take(sizeof(okb_imu_term) * std::max(q.T, 1)), o_samp = take(sizeof(okb_imu_sample) * (size_t)std::max(q.S, 1));
+  const size_t o_pp = take(sizeof(okb_pose_prior) * std::max(q.PP, 1)), o_sbp = take(sizeof(okb_sb_prior) * std::max(q.PP, 1));
+  const size_t o_mkind = take(4 * MB), o_midx = take(4 * MB), o_mcol = take(4 * MB), o_moff = take(4 * MB);
+  const size_t o_mx0 = take(8 * 9 * MB), o_mJ = take(8 * (size_t)MN * MN), o_me0 = take(8 * MN), o_mH0 = take(8 * (size_t)MN * MN);
+  const size_t o_mHs = take(8 * (size_t)MN * MN), o_mb0 = take(8 * MN);
+  const size_t o_mlmi = take(8 * 4 * (size_t)Lpc), o_mark = take(Lpc), o_mvis = take(4 * (size_t)Lpc);
+  const size_t o_bitmap = take(4 * (((size_t)NSc * Lc + 31) / 32 + 1));
+  const size_t o_perm = take(4 * (size_t)Lpc), o_inv = take(4 * (size_t)Lpc), o_trange = take(4 * (size_t)(Lpc / 32 + 1)), o_vis = take(4 * (size_t)Lpc);
+  const size_t o_slots = take(sizeof(SlotInfo) * NSPc);
   const size_t cmd_cap = align_up(full_upload_bytes(q) + S.feat_frame_bytes + 65536, 256);
-  const size_t o_cmd = P.take(cmd_cap);
+  const size_t o_cmd = take(cmd_cap);
   // working state / scratch
-  const size_t o_lm = P.take(8 * 4 * (size_t)Lpc), o_pose_i = P.take(8 * 7 * Kc), o_sb_i = P.take(8 * 9 * Kc);
-  const size_t o_pose_c = P.take(8 * 7 * Kc), o_sb_c = P.take(8 * 9 * Kc), o_lm_c = P.take(8 * 4 * (size_t)Lpc);
+  const size_t o_lm = take(8 * 4 * (size_t)Lpc), o_pose_i = take(8 * 7 * Kc), o_sb_i = take(8 * 9 * Kc);
+  const size_t o_pose_c = take(8 * 7 * Kc), o_sb_c = take(8 * 9 * Kc), o_lm_c = take(8 * 4 * (size_t)Lpc);
   size_t o_lmg[2], o_lmE[2], o_gd[2], o_Ed[2];
-  for (int b = 0; b < 2; ++b) { o_lmg[b] = P.take(8 * 3 * (size_t)Lc); o_lmE[b] = P.take(8 * 3 * (size_t)Lc); }
-  const size_t o_Rinv = P.take(8 * 6 * (size_t)Lc), o_slotctx = P.take(sizeof(SlotCtx) * NSPc);
-  const size_t o_gn = P.take(8 * 3 * (size_t)Lc), o_Li = P.take(8 * 9 * (size_t)Lpc), o_scale = P.take(8 * 3 * (size_t)Lc);
+  for (int b = 0; b < 2; ++b) { o_lmg[b] = take(8 * 3 * (size_t)Lc); o_lmE[b] = take(8 * 3 * (size_t)Lc); }
+  const size_t o_Rinv = take(8 * 6 * (size_t)Lc), o_slotctx = take(sizeof(SlotCtx) * NSPc);
+  const size_t o_gn = take(8 * 3 * (size_t)Lc), o_Li = take(8 * 9 * (size_t)Lpc), o_scale = take(8 * 3 * (size_t)Lc);
   const int n_cx = (Lc + L1_THREADS - 1) / L1_THREADS;
-  const size_t o_partH = P.take(8 * (size_t)n_cx * Kc * kPartH), o_part = P.take(8 * (size_t)dcpc * dcpc * c->chunk_cap);
-  const size_t o_Hd = P.take(8 * (size_t)dcap * dcap);
-  for (int b = 0; b < 2; ++b) { o_gd[b] = P.take(8 * dcap); o_Ed[b] = P.take(8 * dcap); }
-  const size_t o_ud = P.take(8 * dcap), o_scd = P.take(8 * dcap), o_chol = P.take(8 * (size_t)(dcap + 1) * (dcap + 1));
-  const size_t o_obsz = P.take(sizeof(double2) * (size_t)Lc * NSc), o_obsw = P.take(8 * (size_t)Lc * NSc), o_M = P.take(8 * 6 * (size_t)Lpc * Kc);
-  const size_t o_quality = P.take(8 * (size_t)Lc);
-  const size_t o_cache = P.take(sizeof(ImuCache) * std::max(q.T, 1)), o_imu_out = P.take(8 * kImuOut * std::max(q.T, 1));
+  const size_t o_partH = take(8 * (size_t)n_cx * Kc * kPartH), o_part = take(8 * (size_t)dcpc * dcpc * c->chunk_cap);
+  const size_t o_Hd = take(8 * (size_t)dcap * dcap);
+  for (int b = 0; b < 2; ++b) { o_gd[b] = take(8 * dcap); o_Ed[b] = take(8 * dcap); }
+  const size_t o_ud = take(8 * dcap), o_scd = take(8 * dcap), o_chol = take(8 * (size_t)(dcap + 1) * (dcap + 1));
+  const size_t o_obsz = take(sizeof(double2) * (size_t)Lc * NSc), o_obsw = take(8 * (size_t)Lc * NSc), o_M = take(8 * 6 * (size_t)Lpc * Kc);
+  const size_t o_quality = take(8 * (size_t)Lc);
+  const size_t o_cache = take(sizeof(ImuCache) * std::max(q.T, 1)), o_imu_out = take(8 * kImuOut * std::max(q.T, 1));
 
-  if (S.arena_bytes < P.total) {
-    if (S.arena) cudaFree(S.arena);
-    S.arena = nullptr; S.arena_bytes = 0;
-    OKB_CUDA(c, cudaMalloc(&S.arena, P.total));
-    S.arena_bytes = P.total;
-  }
-  const size_t out_bytes = 8 * (16 * (size_t)Kc + 4 + 5 * (size_t)Lc);
-  if (S.out_bytes < out_bytes) {
-    if (S.out_staging) cudaFreeHost(S.out_staging);
-    S.out_staging = nullptr; S.out_bytes = 0;
-    OKB_CUDA(c, cudaMallocHost(&S.out_staging, out_bytes));
-    S.out_bytes = out_bytes;
-  }
+  int rc;
+  if ((rc = grow(c, &S.arena, &S.arena_bytes, P.off)) ||
+      (rc = grow_pinned(c, &S.out_staging, &S.out_bytes, 8 * (16 * (size_t)Kc + 4 + 5 * (size_t)Lc))))
+    return rc;
   if (!S.down) OKB_CUDA(c, cudaEventCreateWithFlags(&S.down, cudaEventDisableTiming));
   if (!S.copied) OKB_CUDA(c, cudaEventCreateWithFlags(&S.copied, cudaEventDisableTiming));
   // the m_mark scratch must be all zero between commands; dead landmark slots must hold finite values
@@ -467,12 +425,7 @@ int okb_commit_windows(okb_ctx* c, const int32_t* wins, int n) {
   std::sort(sorted.begin(), sorted.end());
   const int rc = for_runs(sorted.data(), n, [&](int f, int m) { return commit_range(c, f, m); });
   if (rc) return rc;
-  bool waited[okb_ctx::kDoneRing] = {};
-  for (int i = 0; i < n; ++i) {
-    const int k = c->wins[wins[i]].done_idx;
-    if (k >= 0 && !waited[k]) { OKB_CUDA(c, cudaStreamWaitEvent(c->stream_xfer, c->done_ring[k], 0)); waited[k] = true; }
-  }
-  return OKB_OK;
+  return wait_solver_work(c, c->stream_xfer, wins, n);
 }
 
 extern "C" int okb_window_commit(okb_ctx* c, int first, int count) {
@@ -647,23 +600,12 @@ extern "C" int okb_window_upload(okb_ctx* c, int win, const okb_window_desc* D) 
 
 extern "C" int okb_window_upload_batch(okb_ctx* c, int first, int count, const okb_window_desc* descs, int host_threads) {
   if (!c || !descs || count < 1 || first < 0 || first + count > c->max_windows) return OKB_ERR_INVALID_ARG;
-  int T = host_threads > 0 ? host_threads : 8;
-  T = std::max(1, std::min(T, count));
-  std::vector<int> rcs(T, OKB_OK);
-  if (T == 1) {
-    for (int i = 0; i < count && !rcs[0]; ++i) rcs[0] = upload_pack(c, first + i, descs + i);
-  } else {
-    std::vector<std::thread> th;
-    th.reserve(T);
-    for (int t = 0; t < T; ++t)
-      th.emplace_back([=, &rcs]() {
-        for (int i = t; i < count; i += T) {
-          const int rc = upload_pack(c, first + i, descs + i);
-          if (rc) { rcs[t] = rc; return; }
-        }
-      });
-    for (auto& x : th) x.join();
-  }
+  const int T = std::max(1, std::min(host_threads > 0 ? host_threads : 8, count));
+  std::vector<int> rcs(T, OKB_OK);      // per thread: its first error, after which it packs nothing more
+  parallel_for(count, T, [&](int i) {
+    int& rc = rcs[i % T];
+    if (!rc) rc = upload_pack(c, first + i, descs + i);
+  });
   for (int t = 0; t < T; ++t)
     if (rcs[t]) return rcs[t];
   return commit_range(c, first, count);
@@ -942,12 +884,13 @@ extern "C" int okb_window_reserve_features(okb_ctx* c, int win, int max_feature_
     S.feat_mem = nullptr;
   }
   const size_t images = (size_t)max_feature_frames * max_cameras, kps = images * max_keypoints;
-  ArenaPlan P;
-  P.take(sizeof(FeatStore));
-  const size_t o_n = P.take(4 * images), o_kp = P.take(16 * kps), o_size = P.take(8 * kps), o_desc = P.take(kps * desc_bytes);
-  const size_t o_lm = P.take(4 * kps), o_obs = P.take(kps), o_init = P.take((size_t)lm_cap);
+  Carve P;
+  P.take(sizeof(FeatStore), 256);
+  const size_t o_n = P.take(4 * images, 256), o_kp = P.take(16 * kps, 256), o_size = P.take(8 * kps, 256);
+  const size_t o_desc = P.take(kps * desc_bytes, 256), o_lm = P.take(4 * kps, 256), o_obs = P.take(kps, 256);
+  const size_t o_init = P.take((size_t)lm_cap, 256);
   unsigned char* m = nullptr;
-  OKB_CUDA(c, cudaMalloc(&m, P.total));
+  OKB_CUDA(c, cudaMalloc(&m, P.off));
   FeatStore F{};
   F.F = max_feature_frames; F.C = max_cameras; F.N = max_keypoints; F.D = desc_bytes; F.lm_cap = lm_cap;
   F.n = reinterpret_cast<int*>(m + o_n); F.kp = reinterpret_cast<double*>(m + o_kp); F.size = reinterpret_cast<double*>(m + o_size);
@@ -1047,7 +990,6 @@ extern "C" int okb_window_set_landmark_initialized(okb_ctx* c, int win, int n, c
 // device-side marginalisation (okb_marg.cuh): MarginalizationError::addResidualBlock / marginalizeOut /
 // updateErrorComputation (okvis_ceres/src/MarginalizationError.cpp:127-435, 507-846)
 // ---------------------------------------------------------------------------------------------
-static int hook_alloc_fwd(okb_ctx* c, size_t bytes);
 static int check_range(okb_ctx* c, int first, int count);
 namespace {
 constexpr int kMargImuCap = 32, kMargSbpCap = 8;
@@ -1055,26 +997,25 @@ constexpr int kMargImuCap = 32, kMargSbpCap = 8;
 struct MargLayout { size_t H, b, A, Q, T, Hn, bn, xlin, lmrec, lmV, lmvis, lmslot, clist, status, total; };
 MargLayout marg_layout(int lm_cap, int K_cap, int L_cap, int O_cap) {
   MargLayout m;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t r = o; o = align_up(o + bytes, 16); return r; };
+  Carve P;
   const size_t NN = (size_t)kMargWork * kMargWork * 8;
-  m.H = take(NN); m.b = take(8 * kMargWork); m.A = take(NN); m.Q = take(NN); m.T = take(NN); m.Hn = take(NN); m.bn = take(8 * kMargWork);
-  m.xlin = take(8 * 9 * kMaxMargBlocks);
-  m.lmrec = take(8 * (size_t)lm_cap * K_cap * kMargRec); m.lmV = take(8 * 16 * (size_t)lm_cap); m.lmvis = take(4 * (size_t)lm_cap);
-  m.lmslot = take(4 * (size_t)std::max(L_cap, 1)); m.clist = take(4 * (size_t)std::max(O_cap, 1)); m.status = take(16);
-  m.total = o;
+  m.H = P.take(NN); m.b = P.take(8 * kMargWork); m.A = P.take(NN); m.Q = P.take(NN); m.T = P.take(NN); m.Hn = P.take(NN);
+  m.bn = P.take(8 * kMargWork); m.xlin = P.take(8 * 9 * kMaxMargBlocks);
+  m.lmrec = P.take(8 * (size_t)lm_cap * K_cap * kMargRec); m.lmV = P.take(8 * 16 * (size_t)lm_cap); m.lmvis = P.take(4 * (size_t)lm_cap);
+  m.lmslot = P.take(4 * (size_t)std::max(L_cap, 1)); m.clist = P.take(4 * (size_t)std::max(O_cap, 1)); m.status = P.take(16);
+  m.total = P.off;
   return m;
 }
 // One job in the batch buffer of a call: header, then its index lists.
 struct MargPayload { size_t kind, idx, prev, marg, imu, sbp, lms, total; };
 MargPayload marg_payload(const okb_marg_job* job) {
   MargPayload p;
-  size_t o = align_up(sizeof(MargJobHeader), 16);
-  auto take = [&](size_t bytes) { const size_t r = o; o = align_up(o + bytes, 16); return r; };
+  Carve P;
+  P.take(sizeof(MargJobHeader));
   const size_t nb = (size_t)job->n_blocks;
-  p.kind = take(4 * nb); p.idx = take(4 * nb); p.prev = take(4 * nb); p.marg = take(nb);
-  p.imu = take(4 * (size_t)job->n_imu_terms); p.sbp = take(4 * (size_t)job->n_sb_priors); p.lms = take(4 * (size_t)job->n_landmarks);
-  p.total = o;
+  p.kind = P.take(4 * nb); p.idx = P.take(4 * nb); p.prev = P.take(4 * nb); p.marg = P.take(nb);
+  p.imu = P.take(4 * (size_t)job->n_imu_terms); p.sbp = P.take(4 * (size_t)job->n_sb_priors); p.lms = P.take(4 * (size_t)job->n_landmarks);
+  p.total = P.off;
   return p;
 }
 MargScratch marg_pointers(unsigned char* job, const MargPayload& p, unsigned char* base, const MargLayout& m) {
@@ -1204,15 +1145,8 @@ int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int 
     c->marg_dev_bytes = cap;
   }
   // pending graph edits first: the jobs index the windows as they are now
-  std::vector<std::pair<int, int>> runs;       // (first slot, count) of consecutive job slots
-  for (int t = 0; t < n; ++t) {
-    if (!runs.empty() && runs.back().first + runs.back().second == slots[t]) runs.back().second += 1;
-    else runs.emplace_back(slots[t], 1);
-  }
-  for (const auto& r : runs) {
-    const int rc = commit_range(c, r.first, r.second);
-    if (rc) return rc;
-  }
+  int rc = for_runs(slots, n, [&](int f, int m) { return commit_range(c, f, m); });
+  if (rc) return rc;
   // pack: the previous call's copy reads the pinned buffer until marg_copied
   if (!c->marg_copied) OKB_CUDA(c, cudaEventCreateWithFlags(&c->marg_copied, cudaEventDisableTiming));
   if (c->marg_busy) {
@@ -1273,16 +1207,15 @@ int marg_run(okb_ctx* c, const int* slots, const okb_marg_job* const* jobs, int 
     tasks[t] = task;
   }
   // after the solver work already launched on the job slots
-  bool waited[okb_ctx::kDoneRing] = {};
-  for (int t = 0; t < n; ++t) {
-    const int k = c->wins[slots[t]].done_idx;
-    if (k >= 0 && !waited[k]) { OKB_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[k], 0)); waited[k] = true; }
-  }
+  if ((rc = wait_solver_work(c, xs, slots, n))) return rc;
   OKB_CUDA(c, cudaMemcpyAsync(c->marg_dev, c->marg_host, bytes, cudaMemcpyHostToDevice, xs));
   OKB_CUDA(c, cudaEventRecord(c->marg_copied, xs));
   c->marg_busy = true;
-  for (const auto& r : runs)
-    OKB_CUDA(c, cudaMemcpyAsync(c->d_wins + r.first, &c->host[r.first], sizeof(WinDev) * r.second, cudaMemcpyHostToDevice, xs));
+  rc = for_runs(slots, n, [&](int f, int m) {
+    OKB_CUDA(c, cudaMemcpyAsync(c->d_wins + f, &c->host[f], sizeof(WinDev) * m, cudaMemcpyHostToDevice, xs));
+    return OKB_OK;
+  });
+  if (rc) return rc;
   if (sharded) k_marginalize<true><<<n, M_THREADS, 0, xs>>>(c->d_wins, reinterpret_cast<const MargTask*>(c->marg_dev));
   else k_marginalize<false><<<n, M_THREADS, 0, xs>>>(c->d_wins, reinterpret_cast<const MargTask*>(c->marg_dev));
   c->launches += 1;
@@ -1326,7 +1259,7 @@ extern "C" int okb_window_download_marg(okb_ctx* c, int win, int32_t* n, int32_t
   rc = commit_range(c, win, 1);
   if (rc) return rc;
   const int cap = 8 + 2 * kMaxMargBlocks + 9 * kMaxMargBlocks + 2 * kMaxMarg * kMaxMarg + 2 * kMaxMarg;
-  rc = hook_alloc_fwd(c, sizeof(double) * cap);
+  rc = grow(c, &c->hook_buf, &c->hook_bytes, sizeof(double) * cap);
   if (rc) return rc;
   WinStore& S = c->wins[win];
   cudaStream_t xs = c->stream_xfer;
@@ -1525,14 +1458,7 @@ extern "C" int okb_window_reset(okb_ctx* c, int first, int count) {
   // preparing it, so it overlaps a solve that is running on other slots; the next okb_optimize* of the slot joins the
   // transfer stream as it does for uploads.
   cudaStream_t xs = c->stream_xfer;
-  bool waited[okb_ctx::kDoneRing] = {};
-  for (int i = first; i < first + count; ++i) {
-    const WinStore& S = c->wins[i];
-    if (S.done_idx >= 0 && !waited[S.done_idx]) {
-      OKB_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
-      waited[S.done_idx] = true;
-    }
-  }
+  if ((rc = wait_solver_work(c, xs, c->ident.data() + first, count))) return rc;
   k_reset<<<count, 128, 0, xs>>>(c->d_wins, c->d_ident + first, 1);
   c->launches += 1;
   OKB_CUDA(c, cudaGetLastError());
@@ -1969,23 +1895,6 @@ static void copy_out_window(const WinDev& W, const WinStore& S, double* poses, d
   if (quality) std::memcpy(quality, o + out_lm_offset(W.K, W.NSB) + 4 * (size_t)W.L, sizeof(double) * (size_t)W.L);
 }
 
-extern "C" int okb_window_download(okb_ctx* c, int win, double* poses, double* speed_bias, double* landmarks, double* quality) {
-  int rc = check_range(c, win, 1);
-  if (rc) return rc;
-  cudaSetDevice(c->device);
-  rc = commit_range(c, win, 1);
-  if (rc) return rc;
-  const WinDev& W = c->host[win];
-  WinStore& S = c->wins[win];
-  cudaStream_t xs = c->stream_xfer;
-  if (S.done_idx >= 0) OKB_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
-  OKB_CUDA(c, cudaMemcpyAsync(S.out_staging, W.out, sizeof(double) * out_doubles(W), cudaMemcpyDeviceToHost, xs));
-  OKB_CUDA(c, cudaEventRecord(S.down, xs));
-  OKB_CUDA(c, cudaEventSynchronize(S.down));
-  copy_out_window(W, S, poses, speed_bias, landmarks, quality);
-  return OKB_OK;
-}
-
 // The one path behind okb_window_download_batch (a range passes c->ident.data() + first) and okb_window_download_slots
 // (checked list): pending edits committed once per run of consecutive listed slots, a wait on each distinct solver
 // event of the listed slots, one D2H copy per slot, one synchronisation.  Output tables are in list order.
@@ -1995,14 +1904,7 @@ static int download_list(okb_ctx* c, const int32_t* slots, int count, double* co
   int rc = for_runs(slots, count, [&](int f, int m) { return commit_range(c, f, m); });
   if (rc) return rc;
   cudaStream_t xs = c->stream_xfer;
-  bool waited[okb_ctx::kDoneRing] = {};
-  for (int t = 0; t < count; ++t) {
-    WinStore& S = c->wins[slots[t]];
-    if (S.done_idx >= 0 && !waited[S.done_idx]) {
-      OKB_CUDA(c, cudaStreamWaitEvent(xs, c->done_ring[S.done_idx], 0));
-      waited[S.done_idx] = true;
-    }
-  }
+  if ((rc = wait_solver_work(c, xs, slots, count))) return rc;
   for (int t = 0; t < count; ++t) {
     const int i = slots[t];
     OKB_CUDA(c, cudaMemcpyAsync(c->wins[i].out_staging, c->host[i].out, sizeof(double) * out_doubles(c->host[i]), cudaMemcpyDeviceToHost, xs));
@@ -2010,22 +1912,18 @@ static int download_list(okb_ctx* c, const int32_t* slots, int count, double* co
   WinStore& S0 = c->wins[slots[0]];
   OKB_CUDA(c, cudaEventRecord(S0.down, xs));
   OKB_CUDA(c, cudaEventSynchronize(S0.down));
-  auto copy_out = [&](int k) {
+  parallel_for(count, std::max(1, std::min(8, count / 32)), [&](int k) {
     const int i = slots[k];
     copy_out_window(c->host[i], c->wins[i], poses ? poses[k] : nullptr, speed_bias ? speed_bias[k] : nullptr,
                     landmarks ? landmarks[k] : nullptr, quality ? quality[k] : nullptr);
-  };
-  const int T = std::max(1, std::min(8, count / 32));
-  if (T == 1) {
-    for (int k = 0; k < count; ++k) copy_out(k);
-  } else {
-    std::vector<std::thread> th;
-    th.reserve(T);
-    for (int t = 0; t < T; ++t)
-      th.emplace_back([&, t]() { for (int k = t; k < count; k += T) copy_out(k); });
-    for (auto& x : th) x.join();
-  }
+  });
   return OKB_OK;
+}
+
+extern "C" int okb_window_download(okb_ctx* c, int win, double* poses, double* speed_bias, double* landmarks, double* quality) {
+  const int rc = check_range(c, win, 1);
+  if (rc) return rc;
+  return download_list(c, c->ident.data() + win, 1, &poses, &speed_bias, &landmarks, &quality);
 }
 
 extern "C" int okb_window_download_batch(okb_ctx* c, int first, int count, double* const* poses, double* const* speed_bias,
@@ -2105,24 +2003,13 @@ __global__ void k_hook_relpose(const double* in /* S36 p0 p1 */, double* out /* 
 }
 }  // namespace
 
-static int hook_alloc(okb_ctx* c, size_t bytes);
-static int hook_alloc_fwd(okb_ctx* c, size_t bytes) { return hook_alloc(c, bytes); }
-static int hook_alloc(okb_ctx* c, size_t bytes) {
-  if (c->hook_bytes >= bytes) return OKB_OK;
-  if (c->hook_buf) cudaFree(c->hook_buf);
-  c->hook_buf = nullptr; c->hook_bytes = 0;
-  OKB_CUDA(c, cudaMalloc(&c->hook_buf, bytes));
-  c->hook_bytes = bytes;
-  return OKB_OK;
-}
-
 extern "C" int okb_eval_reprojection(okb_ctx* c, int n, const okb_camera* cam, const double* pose, const double* landmark,
                                      const double* extrinsics, const double* z, const double* sqrt_info, double* r,
                                      double* J_pose, double* J_lm, double* J_ext) {
   if (!c || n < 1 || !cam) return OKB_ERR_INVALID_ARG;
   cudaSetDevice(c->device);
   const size_t nin = (size_t)n * (7 + 4 + 7 + 2 + 1), nout = (size_t)n * (2 + 12 + 6 + 12);
-  int rc = hook_alloc(c, (nin + nout) * sizeof(double));
+  int rc = grow(c, &c->hook_buf, &c->hook_bytes, (nin + nout) * sizeof(double));
   if (rc) return rc;
   double* d = reinterpret_cast<double*>(c->hook_buf);
   double *dp = d, *dl = dp + 7 * (size_t)n, *de = dl + 4 * (size_t)n, *dz = de + 7 * (size_t)n, *dq = dz + 2 * (size_t)n;
@@ -2151,9 +2038,9 @@ extern "C" int okb_eval_imu(okb_ctx* c, const okb_imu_params* prm, const okb_imu
   cudaSetDevice(c->device);
   const size_t sbytes = align_up(sizeof(okb_imu_sample) * n_samples, 256);
   const size_t total = sbytes + align_up(sizeof(ImuCache), 256) + sizeof(double) * (32 + 9 + 7 + 700);
-  int rc = hook_alloc(c, total);
+  int rc = grow(c, &c->hook_buf, &c->hook_bytes, total);
   if (rc) return rc;
-  unsigned char* base = reinterpret_cast<unsigned char*>(c->hook_buf);
+  unsigned char* base = c->hook_buf;
   okb_imu_sample* ds = reinterpret_cast<okb_imu_sample*>(base);
   ImuCache* dc = reinterpret_cast<ImuCache*>(base + sbytes);
   double* din = reinterpret_cast<double*>(base + sbytes + align_up(sizeof(ImuCache), 256));
@@ -2193,26 +2080,19 @@ static const char* prop_invalid(const okb_propagate_job& j) {
 
 // Propagates n checked jobs on stream st through buffers B (the caller holds B.mtx): one H2D copy of the job table and
 // all samples, one k_propagate launch (one warp per job), one D2H copy of the output records, one synchronisation.
-static int prop_run(okb_ctx* c, cudaStream_t st, PropBuffers& B, int n, const okb_propagate_job* jobs) {
+static int prop_run(okb_ctx* c, cudaStream_t st, CallBuffers& B, int n, const okb_propagate_job* jobs) {
   std::vector<size_t> s_off(n), o_off(n);
-  size_t in_bytes = align_up(sizeof(PropEntry) * n, 256), out_bytes = 0;
+  Carve in, out;
+  in.take(sizeof(PropEntry) * n, 256);
   for (int i = 0; i < n; ++i) {
-    s_off[i] = in_bytes;
-    in_bytes += align_up(sizeof(okb_imu_sample) * (size_t)jobs[i].n_samples, 16);
-    o_off[i] = out_bytes;
-    out_bytes += sizeof(double) * (kPropRecord + (jobs[i].covariance ? 225 : 0) + (jobs[i].jacobian ? 225 : 0));
+    s_off[i] = in.take(sizeof(okb_imu_sample) * (size_t)jobs[i].n_samples);
+    o_off[i] = out.take(sizeof(double) * (kPropRecord + (jobs[i].covariance ? 225 : 0) + (jobs[i].jacobian ? 225 : 0)), 8);
   }
-  const size_t out_at = align_up(in_bytes, 256), total = out_at + out_bytes;
-  if (total > B.bytes) {
-    if (B.host) cudaFreeHost(B.host);
-    if (B.dev) cudaFree(B.dev);
-    B.host = nullptr; B.dev = nullptr; B.bytes = 0;
-    const size_t cap = align_up(std::max(total, (size_t)64 << 10), 4096);
-    OKB_CUDA(c, cudaMallocHost(&B.host, cap));
-    OKB_CUDA(c, cudaMalloc(&B.dev, cap));
-    B.bytes = cap;
-  }
-  PropEntry* tab = reinterpret_cast<PropEntry*>(B.host);
+  const size_t in_bytes = in.off, out_bytes = out.off, out_at = align_up(in_bytes, 256);
+  const int rc = B.reserve(c, align_up(std::max(out_at + out_bytes, (size_t)64 << 10), 4096), 0);
+  if (rc) return rc;
+  unsigned char *host = B.h_stage, *dev = B.d_stage;
+  PropEntry* tab = reinterpret_cast<PropEntry*>(host);
   for (int i = 0; i < n; ++i) {
     const okb_propagate_job& j = jobs[i];
     PropEntry& e = tab[i];
@@ -2223,17 +2103,17 @@ static int prop_run(okb_ctx* c, cudaStream_t st, PropBuffers& B, int n, const ok
     e.n = j.n_samples; e.want_cov = j.covariance ? 1 : 0; e.want_jac = j.jacobian ? 1 : 0;
     std::memcpy(e.state, j.pose, 7 * sizeof(double));
     std::memcpy(e.state + 7, j.speed_bias, 9 * sizeof(double));
-    std::memcpy(B.host + s_off[i], j.samples, sizeof(okb_imu_sample) * (size_t)j.n_samples);
+    std::memcpy(host + s_off[i], j.samples, sizeof(okb_imu_sample) * (size_t)j.n_samples);
   }
-  OKB_CUDA(c, cudaMemcpyAsync(B.dev, B.host, in_bytes, cudaMemcpyHostToDevice, st));
-  k_propagate<<<n, 32, 0, st>>>(B.dev, B.dev + out_at);
+  OKB_CUDA(c, cudaMemcpyAsync(dev, host, in_bytes, cudaMemcpyHostToDevice, st));
+  k_propagate<<<n, 32, 0, st>>>(dev, dev + out_at);
   c->prop_launches += 1;
   OKB_CUDA(c, cudaGetLastError());
-  OKB_CUDA(c, cudaMemcpyAsync(B.host + out_at, B.dev + out_at, out_bytes, cudaMemcpyDeviceToHost, st));
+  OKB_CUDA(c, cudaMemcpyAsync(host + out_at, dev + out_at, out_bytes, cudaMemcpyDeviceToHost, st));
   OKB_CUDA(c, cudaStreamSynchronize(st));
   for (int i = 0; i < n; ++i) {
     const okb_propagate_job& j = jobs[i];
-    const double* o = reinterpret_cast<const double*>(B.host + out_at + o_off[i]);
+    const double* o = reinterpret_cast<const double*>(host + out_at + o_off[i]);
     int32_t used;
     std::memcpy(&used, o + 16, sizeof used);
     if (used >= 0) {
@@ -2276,21 +2156,28 @@ extern "C" int okb_imu_propagate_batch(okb_ctx* c, int n_jobs, const okb_propaga
   return prop_run(c, c->stream_prop, c->prop_batch, n_jobs, jobs);
 }
 
-extern "C" int okb_eval_pose_error(okb_ctx* c, const double* meas, const double* sqrt_info, const double* pose, double* r, double* J) {
-  if (!c) return OKB_ERR_INVALID_ARG;
+// One single-CTA hook on the solver stream: nin packed input doubles in one H2D copy, a synchronisation, one launch of
+// kernel(in, out) with `threads` threads, nout output doubles in one D2H copy, a synchronisation.
+static int run_hook(okb_ctx* c, void (*kernel)(const double*, double*), int threads, const double* in, int nin, double* out, int nout) {
   cudaSetDevice(c->device);
-  int rc = hook_alloc(c, sizeof(double) * (50 + 42));
+  const int rc = grow(c, &c->hook_buf, &c->hook_bytes, sizeof(double) * (nin + nout));
   if (rc) return rc;
   double* d = reinterpret_cast<double*>(c->hook_buf);
-  double h[50];
-  std::memcpy(h, meas, 56); std::memcpy(h + 7, sqrt_info, 288); std::memcpy(h + 43, pose, 56);
-  OKB_CUDA(c, cudaMemcpyAsync(d, h, sizeof h, cudaMemcpyHostToDevice, c->stream));
+  OKB_CUDA(c, cudaMemcpyAsync(d, in, sizeof(double) * nin, cudaMemcpyHostToDevice, c->stream));
   OKB_CUDA(c, cudaStreamSynchronize(c->stream));
-  k_hook_pose<<<1, 32, 0, c->stream>>>(d, d + 50);
+  kernel<<<1, threads, 0, c->stream>>>(d, d + nin);
   c->launches += 1;
-  double o[42];
-  OKB_CUDA(c, cudaMemcpyAsync(o, d + 50, sizeof o, cudaMemcpyDeviceToHost, c->stream));
+  OKB_CUDA(c, cudaMemcpyAsync(out, d + nin, sizeof(double) * nout, cudaMemcpyDeviceToHost, c->stream));
   OKB_CUDA(c, cudaStreamSynchronize(c->stream));
+  return OKB_OK;
+}
+
+extern "C" int okb_eval_pose_error(okb_ctx* c, const double* meas, const double* sqrt_info, const double* pose, double* r, double* J) {
+  if (!c) return OKB_ERR_INVALID_ARG;
+  double h[50], o[42];
+  std::memcpy(h, meas, 56); std::memcpy(h + 7, sqrt_info, 288); std::memcpy(h + 43, pose, 56);
+  const int rc = run_hook(c, k_hook_pose, 32, h, 50, o, 42);
+  if (rc) return rc;
   if (r) std::memcpy(r, o, 48);
   if (J) std::memcpy(J, o + 6, 288);
   return OKB_OK;
@@ -2310,19 +2197,10 @@ __global__ void k_hook_sb(const double* in /* meas9 S81 sb9 */, double* out /* r
 
 extern "C" int okb_eval_speed_bias_error(okb_ctx* c, const double* meas, const double* sqrt_info, const double* sb, double* r, double* J) {
   if (!c || !meas || !sqrt_info || !sb) return OKB_ERR_INVALID_ARG;
-  cudaSetDevice(c->device);
-  int rc = hook_alloc(c, sizeof(double) * (99 + 90));
-  if (rc) return rc;
-  double* d = reinterpret_cast<double*>(c->hook_buf);
-  double h[99];
+  double h[99], o[90];
   std::memcpy(h, meas, 72); std::memcpy(h + 9, sqrt_info, 648); std::memcpy(h + 90, sb, 72);
-  OKB_CUDA(c, cudaMemcpyAsync(d, h, sizeof h, cudaMemcpyHostToDevice, c->stream));
-  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
-  k_hook_sb<<<1, 96, 0, c->stream>>>(d, d + 99);
-  c->launches += 1;
-  double o[90];
-  OKB_CUDA(c, cudaMemcpyAsync(o, d + 99, sizeof o, cudaMemcpyDeviceToHost, c->stream));
-  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
+  const int rc = run_hook(c, k_hook_sb, 96, h, 99, o, 90);
+  if (rc) return rc;
   if (r) std::memcpy(r, o, 72);
   if (J) std::memcpy(J, o + 9, 648);
   return OKB_OK;
@@ -2331,19 +2209,10 @@ extern "C" int okb_eval_speed_bias_error(okb_ctx* c, const double* meas, const d
 extern "C" int okb_eval_relative_pose(okb_ctx* c, const double* sqrt_info, const double* pose0, const double* pose1, double* r,
                                       double* J0, double* J1) {
   if (!c) return OKB_ERR_INVALID_ARG;
-  cudaSetDevice(c->device);
-  int rc = hook_alloc(c, sizeof(double) * (50 + 78));
-  if (rc) return rc;
-  double* d = reinterpret_cast<double*>(c->hook_buf);
-  double h[50];
+  double h[50], o[78];
   std::memcpy(h, sqrt_info, 288); std::memcpy(h + 36, pose0, 56); std::memcpy(h + 43, pose1, 56);
-  OKB_CUDA(c, cudaMemcpyAsync(d, h, sizeof h, cudaMemcpyHostToDevice, c->stream));
-  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
-  k_hook_relpose<<<1, 32, 0, c->stream>>>(d, d + 50);
-  c->launches += 1;
-  double o[78];
-  OKB_CUDA(c, cudaMemcpyAsync(o, d + 50, sizeof o, cudaMemcpyDeviceToHost, c->stream));
-  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
+  const int rc = run_hook(c, k_hook_relpose, 32, h, 50, o, 78);
+  if (rc) return rc;
   if (r) std::memcpy(r, o, 48);
   if (J0) std::memcpy(J0, o + 6, 288);
   if (J1) std::memcpy(J1, o + 42, 288);
@@ -2394,9 +2263,9 @@ extern "C" int okb_eval_marginalization(okb_ctx* c, const okb_marg_prior* m, con
   if (cc != n) return OKB_ERR_INVALID_ARG;
   const size_t ints = align_up(sizeof(int32_t) * 3 * nb, 256);
   const size_t total = ints + sizeof(double) * (2 * xo + (size_t)2 * n * n + 2 * n);
-  int rc = hook_alloc(c, total);
+  int rc = grow(c, &c->hook_buf, &c->hook_bytes, total);
   if (rc) return rc;
-  unsigned char* base = reinterpret_cast<unsigned char*>(c->hook_buf);
+  unsigned char* base = c->hook_buf;
   int32_t* dk = reinterpret_cast<int32_t*>(base);
   double* dx0 = reinterpret_cast<double*>(base + ints);
   double *dx = dx0 + xo, *dJ = dx + xo, *de0 = dJ + (size_t)n * n, *dr = de0 + n, *dJe = dr + n;

@@ -16,22 +16,13 @@
 #include <cstring>
 #include <atomic>
 #include <mutex>
-#include <thread>
 #include <vector>
 
 #include "okb_ctx.h"
+#include "okb_hostpack.hpp"
 #include "okb_math.cuh"
 
 using namespace okb;
-
-#define FE_CUDA(ctx, call)                                                      \
-  do {                                                                          \
-    cudaError_t e_ = (call);                                                    \
-    if (e_ != cudaSuccess) {                                                    \
-      (ctx)->set_error(std::string(#call) + ": " + cudaGetErrorString(e_));     \
-      return OKB_ERR_CUDA;                                                      \
-    }                                                                           \
-  } while (0)
 
 namespace {
 constexpr int kBorder = 16;
@@ -132,22 +123,6 @@ struct SlotBuffers {
   cudaStream_t stream = nullptr;
   DetectBuffers buf;
   std::mutex mtx;
-};
-
-// Buffers of one kind of table-driven call: a pinned staging buffer and its device mirror (tables in, results out, one
-// copy each way), device-only scratch, and the mutex that serialises the calls using them.  They grow with the largest
-// call and are kept.  The Hamming matcher's sets are held under match_mtx / batch_mtx, which guard other buffers too.
-struct CallBuffers {
-  uint8_t* h_stage = nullptr;      // pinned
-  uint8_t* d_stage = nullptr;
-  uint8_t* d_scratch = nullptr;
-  size_t h_stage_cap = 0, d_stage_cap = 0, d_scratch_cap = 0;
-  std::mutex mtx;
-  void release() {
-    if (h_stage) cudaFreeHost(h_stage);
-    cudaFree(d_stage);
-    cudaFree(d_scratch);
-  }
 };
 }  // namespace
 
@@ -802,37 +777,17 @@ static int ensure_pattern(okb_ctx* c, okb_frontend_state* F, int desc_bytes, Dev
   if (!D.lut) {
     Pattern P = make_pattern(desc_bytes);
     DevPattern N;
-    FE_CUDA(c, cudaMalloc(&N.half, sizeof(int) * kPts));
-    FE_CUDA(c, cudaMalloc(&N.pi, P.pi.size()));
-    FE_CUDA(c, cudaMalloc(&N.pj, P.pj.size()));
-    FE_CUDA(c, cudaMalloc(&N.lut, P.lut.size() * sizeof(int16_t)));
-    FE_CUDA(c, cudaMemcpy(N.half, P.half, sizeof(int) * kPts, cudaMemcpyHostToDevice));
-    FE_CUDA(c, cudaMemcpy(N.pi, P.pi.data(), P.pi.size(), cudaMemcpyHostToDevice));
-    FE_CUDA(c, cudaMemcpy(N.pj, P.pj.data(), P.pj.size(), cudaMemcpyHostToDevice));
-    FE_CUDA(c, cudaMemcpy(N.lut, P.lut.data(), P.lut.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
+    OKB_CUDA(c, cudaMalloc(&N.half, sizeof(int) * kPts));
+    OKB_CUDA(c, cudaMalloc(&N.pi, P.pi.size()));
+    OKB_CUDA(c, cudaMalloc(&N.pj, P.pj.size()));
+    OKB_CUDA(c, cudaMalloc(&N.lut, P.lut.size() * sizeof(int16_t)));
+    OKB_CUDA(c, cudaMemcpy(N.half, P.half, sizeof(int) * kPts, cudaMemcpyHostToDevice));
+    OKB_CUDA(c, cudaMemcpy(N.pi, P.pi.data(), P.pi.size(), cudaMemcpyHostToDevice));
+    OKB_CUDA(c, cudaMemcpy(N.pj, P.pj.data(), P.pj.size(), cudaMemcpyHostToDevice));
+    OKB_CUDA(c, cudaMemcpy(N.lut, P.lut.data(), P.lut.size() * sizeof(int16_t), cudaMemcpyHostToDevice));
     D = N;
   }
   *out = D;
-  return OKB_OK;
-}
-
-template <typename T>
-static int grow(okb_ctx* c, T** p, size_t* cap, size_t need) {
-  if (*cap >= need) return OKB_OK;
-  cudaFree(*p);
-  *p = nullptr; *cap = 0;
-  FE_CUDA(c, cudaMalloc(p, need * sizeof(T)));
-  *cap = need;
-  return OKB_OK;
-}
-
-template <typename T>
-static int grow_pinned(okb_ctx* c, T** p, size_t* cap, size_t need) {
-  if (*cap >= need) return OKB_OK;
-  if (*p) cudaFreeHost(*p);
-  *p = nullptr; *cap = 0;
-  FE_CUDA(c, cudaMallocHost(p, need * sizeof(T)));
-  *cap = need;
   return OKB_OK;
 }
 
@@ -841,43 +796,7 @@ static int grow_pinned(okb_ctx* c, T** p, size_t* cap, size_t need) {
 template <typename Fn>
 static void host_parallel(int n, int threads, size_t bytes, const Fn& f) {
   const int by_bytes = (int)std::min<size_t>(1 + bytes / (8u << 20), 64);
-  const int T = std::max(1, std::min({threads > 0 ? threads : 8, n, by_bytes}));
-  if (T == 1) {
-    for (int i = 0; i < n; ++i) f(i);
-    return;
-  }
-  std::vector<std::thread> th;
-  th.reserve(T);
-  for (int t = 0; t < T; ++t)
-    th.emplace_back([=, &f]() {
-      for (int i = t; i < n; i += T) f(i);
-    });
-  for (auto& x : th) x.join();
-}
-
-static size_t up256(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// Lays arrays out one after another in a buffer: take() returns the offset of the next `bytes` and pads their end to
-// `align`, so the array after them starts aligned; `off` is the size so far.  Callers lay a buffer out once, keep the
-// offsets and fill from them.
-namespace {
-struct Carve {
-  size_t off = 0;
-  size_t take(size_t bytes, size_t align = 16) {
-    const size_t o = off;
-    off = (off + bytes + align - 1) / align * align;
-    return o;
-  }
-};
-}  // namespace
-
-// Grows B to `stage` bytes of staging (pinned and its device mirror) and `scratch` bytes of device scratch.
-static int reserve(okb_ctx* c, CallBuffers& B, size_t stage, size_t scratch) {
-  int rc;
-  if ((rc = grow_pinned(c, &B.h_stage, &B.h_stage_cap, stage)) || (rc = grow(c, &B.d_stage, &B.d_stage_cap, stage)) ||
-      (rc = grow(c, &B.d_scratch, &B.d_scratch_cap, scratch)))
-    return rc;
-  return OKB_OK;
+  parallel_for(n, std::max(1, std::min({threads > 0 ? threads : 8, n, by_bytes})), f);
 }
 
 // Detect and describe n images with one parameter set on stream `st`, into buffers B: one H2D copy (image table and
@@ -891,7 +810,9 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
   int rc = ensure_pattern(c, F, db, &pat);
   if (rc) return rc;
   std::vector<FeImage> tab(n);
-  size_t in_bytes = up256(sizeof(FeImage) * n), px = 0, ii = 0, uni = 0;
+  Carve in;                     // [FeImage table | packed images], each on a 256-byte boundary
+  in.take(sizeof(FeImage) * n, 256);
+  size_t px = 0, ii = 0, uni = 0;
   int Wmax = 0, Hmax = 0;
   for (int i = 0; i < n; ++i) {
     const okb_image_desc& d = ims[i];
@@ -900,15 +821,17 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
     t.cam = d.cam;
     t.gC[0] = -d.R_CW[2]; t.gC[1] = -d.R_CW[5]; t.gC[2] = -d.R_CW[8];
     t.W = d.width; t.H = d.height;
-    t.img = in_bytes; t.px = px; t.ii = ii; t.uni = uni;
+    t.img = in.take((size_t)d.width * d.height, 256); t.px = px; t.ii = ii; t.uni = uni;
     t.max_cells = ((d.width + 3) / 4) * ((d.height + 3) / 4);          // smallest cell is 4 px
     uni += uni_stride(t.max_cells, kMaxCand);
-    in_bytes += up256((size_t)d.width * d.height);
     px += (size_t)d.width * d.height;
     ii += (size_t)(d.width + 1) * (d.height + 1);
     Wmax = std::max(Wmax, d.width); Hmax = std::max(Hmax, d.height);
   }
-  const size_t o_kp = up256(sizeof(int) * 4 * n), o_desc = o_kp + up256(sizeof(okb_keypoint) * n * maxk);
+  const size_t in_bytes = in.off;
+  Carve out;                    // [counts n x 4 | keypoints n x maxk | descriptors n x maxk x desc_bytes]
+  out.take(sizeof(int) * 4 * n, 256);
+  const size_t o_kp = out.take(sizeof(okb_keypoint) * n * maxk, 256), o_desc = out.off;
   const size_t out_bytes = o_desc + (size_t)n * maxk * db;
   if ((rc = grow_pinned(c, &B.h_in, &B.h_in_cap, in_bytes)) || (rc = grow(c, &B.d_in, &B.d_in_cap, in_bytes)) ||
       (rc = grow(c, &B.d_score, &B.cap_score, px)) || (rc = grow(c, &B.d_integral, &B.cap_integral, ii)) ||
@@ -924,8 +847,8 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
     else
       for (int y = 0; y < d.height; ++y) std::memcpy(dst + (size_t)y * d.width, d.img + (size_t)y * d.stride, d.width);
   });
-  FE_CUDA(c, cudaMemcpyAsync(B.d_in, B.h_in, in_bytes, cudaMemcpyHostToDevice, st));
-  FE_CUDA(c, cudaMemsetAsync(B.d_out, 0, sizeof(int) * 4 * n, st));      // per image: candidates, accepted, rounds, -
+  OKB_CUDA(c, cudaMemcpyAsync(B.d_in, B.h_in, in_bytes, cudaMemcpyHostToDevice, st));
+  OKB_CUDA(c, cudaMemsetAsync(B.d_out, 0, sizeof(int) * 4 * n, st));      // per image: candidates, accepted, rounds, -
   const FeImage* d_tab = reinterpret_cast<const FeImage*>(B.d_in);
   int* d_count = reinterpret_cast<int*>(B.d_out);
   okb_keypoint* d_kp = reinterpret_cast<okb_keypoint*>(B.d_out + o_kp);
@@ -935,7 +858,7 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
   const dim3 nb(32, 8), ng((Wmax + 31) / 32, (Hmax + 7) / 8, n);
   k_nms<<<ng, nb, 0, st>>>(d_tab, B.d_score, (int32_t)std::ceil(prm->absolute_threshold), B.d_keys, d_count, kMaxCand);
   k_uniformity<<<n, UT, 0, st>>>(d_tab, B.d_keys, d_count, kMaxCand, prm->uniformity_radius, maxk, B.d_uni, B.d_state, d_kp);
-  FE_CUDA(c, cudaFuncSetAttribute(k_uniformity_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(UniSmem)));
+  OKB_CUDA(c, cudaFuncSetAttribute(k_uniformity_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(UniSmem)));
   k_uniformity_smem<<<n, UT, sizeof(UniSmem), st>>>(d_tab, B.d_keys, d_count, kMaxCand, prm->uniformity_radius, maxk, d_kp);
   k_integral_rows<<<dim3((Hmax + 1 + 3) / 4, n), 128, 0, st>>>(d_tab, B.d_in, B.d_integral);
   k_integral_cols<<<dim3((Wmax + 1 + 31) / 32, n), 32 * IC_SEG, 0, st>>>(d_tab, B.d_integral);
@@ -943,9 +866,9 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
   k_describe<<<dim3((maxk + 3) / 4, n), 128, 0, st>>>(d_tab, B.d_integral, pat.half, pat.pi, pat.pj, pat.lut, db, d_kp, maxk, d_count,
                                                       d_desc);
   F->launches += prm->rotation_invariance ? 8 : 7;
-  FE_CUDA(c, cudaGetLastError());
-  FE_CUDA(c, cudaMemcpyAsync(B.h_out, B.d_out, out_bytes, cudaMemcpyDeviceToHost, st));
-  FE_CUDA(c, cudaStreamSynchronize(st));
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(B.h_out, B.d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  OKB_CUDA(c, cudaStreamSynchronize(st));
   const int* h_count = reinterpret_cast<const int*>(B.h_out);
   { static const bool dbg = getenv("OKB_FE_DEBUG") != nullptr;
     if (dbg)
@@ -983,7 +906,7 @@ extern "C" int okb_detect_describe(okb_ctx* c, int cam_slot, const uint8_t* img,
   okb_frontend_state* F = fe(c);
   SlotBuffers& S = F->slots[cam_slot];
   std::lock_guard<std::mutex> lk(S.mtx);   // the reference guards each camera's detector with a mutex (Frontend.cpp:97)
-  if (!S.stream) FE_CUDA(c, cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
+  if (!S.stream) OKB_CUDA(c, cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
   okb_image_desc d;
   std::memset(&d, 0, sizeof d);
   d.img = img; d.width = width; d.height = height; d.stride = stride;
@@ -1009,7 +932,7 @@ extern "C" int okb_detect_describe_batch(okb_ctx* c, int n_images, const okb_ima
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
   std::lock_guard<std::mutex> lk(F->batch_mtx);
-  if (!F->batch_stream) FE_CUDA(c, cudaStreamCreateWithFlags(&F->batch_stream, cudaStreamNonBlocking));
+  if (!F->batch_stream) OKB_CUDA(c, cudaStreamCreateWithFlags(&F->batch_stream, cudaStreamNonBlocking));
   return detect_run(c, F, F->batch_det, F->batch_stream, n_images, images, prm, out_kp, out_desc, max_out, n_out, host_threads);
 }
 
@@ -1386,7 +1309,7 @@ struct AssignSmem {
     if (jd.in_smem) bytes = std::max(bytes, need);
   }
   int set_attribute(okb_ctx* c) const {
-    if (bytes > 48 * 1024 - 512) FE_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
+    if (bytes > 48 * 1024 - 512) OKB_CUDA(c, cudaFuncSetAttribute(k_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin - 1024));
     return OKB_OK;
   }
 };
@@ -1454,10 +1377,10 @@ static int upload_descriptors(okb_ctx* c, okb_frontend_state* F, const uint8_t* 
   int rc;
   if ((rc = grow(c, &F->d_A, &F->capA, (size_t)nA * bytes + nA))) return rc;
   if ((rc = grow(c, &F->d_B, &F->capB, (size_t)nB * bytes + nB))) return rc;
-  FE_CUDA(c, cudaMemcpyAsync(F->d_A, A, (size_t)nA * bytes, cudaMemcpyHostToDevice, c->stream));
-  FE_CUDA(c, cudaMemcpyAsync(F->d_B, B, (size_t)nB * bytes, cudaMemcpyHostToDevice, c->stream));
-  if (skipA) FE_CUDA(c, cudaMemcpyAsync(F->d_A + (size_t)nA * bytes, skipA, nA, cudaMemcpyHostToDevice, c->stream));
-  if (skipB) FE_CUDA(c, cudaMemcpyAsync(F->d_B + (size_t)nB * bytes, skipB, nB, cudaMemcpyHostToDevice, c->stream));
+  OKB_CUDA(c, cudaMemcpyAsync(F->d_A, A, (size_t)nA * bytes, cudaMemcpyHostToDevice, c->stream));
+  OKB_CUDA(c, cudaMemcpyAsync(F->d_B, B, (size_t)nB * bytes, cudaMemcpyHostToDevice, c->stream));
+  if (skipA) OKB_CUDA(c, cudaMemcpyAsync(F->d_A + (size_t)nA * bytes, skipA, nA, cudaMemcpyHostToDevice, c->stream));
+  if (skipB) OKB_CUDA(c, cudaMemcpyAsync(F->d_B + (size_t)nB * bytes, skipB, nB, cudaMemcpyHostToDevice, c->stream));
   return OKB_OK;
 }
 
@@ -1528,7 +1451,7 @@ static int match_run(okb_ctx* c, CallBuffers& io, cudaStream_t st, int n, const 
   }
   const size_t out_end = q.off;
   for (int t = 0; t < nd; ++t) L[t].oD = q.take((size_t)jobs[order[t]].nA);
-  if ((rc = reserve(c, io, q.off, 0))) return rc;
+  if ((rc = io.reserve(c, q.off, 0))) return rc;
   uint8_t* h = io.h_stage;
   uint8_t* d = io.d_stage;
   AssignSmem sm;
@@ -1586,12 +1509,12 @@ static int match_run(okb_ctx* c, CallBuffers& io, cudaStream_t st, int n, const 
     maxA[kind] = std::max(maxA[kind], j.nA);
     ++nkind[kind];
   }
-  FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, st));
+  OKB_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, st));
   if ((rc = sm.set_attribute(c)) || (rc = launch_matcher(c, st, reinterpret_cast<const MatchJobDev*>(d), nw, nkind, maxA, sm)))
     return rc;
-  FE_CUDA(c, cudaGetLastError());
-  FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, st));
-  FE_CUDA(c, cudaStreamSynchronize(st));
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, st));
+  OKB_CUDA(c, cudaStreamSynchronize(st));
   for (int t = 0; t < nd; ++t) {
     const okb_match_job& j = jobs[order[t]];
     if (j.out_topk) std::memcpy(j.out_topk, h + L[t].oT, sizeof(okb_pair) * (size_t)j.nA * j.num_best);
@@ -1639,7 +1562,7 @@ extern "C" int okb_hamming_match_batch(okb_ctx* c, int n_jobs, const okb_match_j
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
   std::lock_guard<std::mutex> lk(F->batch_mtx);
-  if (!F->batch_stream) FE_CUDA(c, cudaStreamCreateWithFlags(&F->batch_stream, cudaStreamNonBlocking));
+  if (!F->batch_stream) OKB_CUDA(c, cudaStreamCreateWithFlags(&F->batch_stream, cudaStreamNonBlocking));
   return match_run(c, F->batch_match, F->batch_stream, n_jobs, jobs, desc_bytes);
 }
 
@@ -1677,14 +1600,14 @@ extern "C" int okb_hamming_candidates(okb_ctx* c, const uint8_t* A, int nA, cons
                         F->d_rowptr, F->d_col, F->d_dist, cap, 1)));
   }
   F->launches += 3;
-  FE_CUDA(c, cudaGetLastError());
-  FE_CUDA(c, cudaMemcpyAsync(row_ptr, F->d_rowptr, sizeof(uint32_t) * (nA + 1), cudaMemcpyDeviceToHost, c->stream));
-  FE_CUDA(c, cudaStreamSynchronize(c->stream));
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(row_ptr, F->d_rowptr, sizeof(uint32_t) * (nA + 1), cudaMemcpyDeviceToHost, c->stream));
+  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
   const uint32_t total = row_ptr[nA];
   const uint32_t ncopy = std::min<uint32_t>(total, (uint32_t)cap);
-  if (ncopy && col_idx) FE_CUDA(c, cudaMemcpyAsync(col_idx, F->d_col, sizeof(uint32_t) * ncopy, cudaMemcpyDeviceToHost, c->stream));
-  if (ncopy && dist) FE_CUDA(c, cudaMemcpyAsync(dist, F->d_dist, sizeof(uint16_t) * ncopy, cudaMemcpyDeviceToHost, c->stream));
-  FE_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (ncopy && col_idx) OKB_CUDA(c, cudaMemcpyAsync(col_idx, F->d_col, sizeof(uint32_t) * ncopy, cudaMemcpyDeviceToHost, c->stream));
+  if (ncopy && dist) OKB_CUDA(c, cudaMemcpyAsync(dist, F->d_dist, sizeof(uint16_t) * ncopy, cudaMemcpyDeviceToHost, c->stream));
+  OKB_CUDA(c, cudaStreamSynchronize(c->stream));
   if (total > (uint32_t)cap) { c->set_error("candidate capacity too small"); return OKB_ERR_CAPACITY; }
   return OKB_OK;
 }
@@ -2004,7 +1927,7 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
     o_un[i] = st.take(4 * sumA);
   }
   const size_t out_end = st.off;
-  if ((rc = reserve(c, B, out_end, sc.off))) return rc;
+  if ((rc = B.reserve(c, out_end, sc.off))) return rc;
   uint8_t* h = B.h_stage;
   uint8_t* d = B.d_stage;
   AssignSmem sm;
@@ -2038,7 +1961,7 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
       maxA[r] = std::max(maxA[r], x.nA);
     }
   }
-  FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
+  OKB_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
   const TrackJobDev* d_jobs = reinterpret_cast<const TrackJobDev*>(d);
   if ((rc = sm.set_attribute(c))) return rc;
   const int nw = c->wins[jobs[0].win].feat.D / 4;
@@ -2051,9 +1974,9 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
     k_track_apply<<<m[r], TK_T, 0, xs>>>(d_jobs, d_tab, d_ri, r);
   }
   F->launches += 2 * (int64_t)R;
-  FE_CUDA(c, cudaGetLastError());
-  FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
-  FE_CUDA(c, cudaStreamSynchronize(xs));
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
+  OKB_CUDA(c, cudaStreamSynchronize(xs));
   for (int i = 0; i < n_jobs; ++i) {
     const okb_track_job& j = jobs[i];
     if (j.n_rounds == 0) { *j.n_assoc = 0; *j.n_uninit = 0; continue; }
@@ -2460,7 +2383,7 @@ static int match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs
     l.uj = sc.take(8 * kUJ * b);
   }
   const size_t out_end = st.off;
-  if ((rc = reserve(c, B, out_end, sc.off))) return rc;
+  if ((rc = B.reserve(c, out_end, sc.off))) return rc;
   uint8_t* h = B.h_stage;
   uint8_t* d = B.d_stage;
   uint8_t* s = B.d_scratch;
@@ -2497,7 +2420,7 @@ static int match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs
     maxA = std::max(maxA, l.nA);
     maxN = std::max(maxN, std::max(l.nA, l.nB));
   }
-  FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
+  OKB_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
   const StereoJobDev* d_jobs = reinterpret_cast<const StereoJobDev*>(d);
   MatchJobDev* d_tab = reinterpret_cast<MatchJobDev*>(d + o_tab);
   if ((rc = sm.set_attribute(c))) return rc;
@@ -2506,9 +2429,9 @@ static int match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs
   if ((rc = launch_matcher(c, xs, d_tab, c->wins[jobs[0].win].feat.D / 4, n, max_a, sm))) return rc;
   k_stereo_apply<<<n_jobs, TK_T, 0, xs>>>(d_jobs, d_tab);
   F->launches += 2;
-  FE_CUDA(c, cudaGetLastError());
-  FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
-  FE_CUDA(c, cudaStreamSynchronize(xs));
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
+  OKB_CUDA(c, cudaStreamSynchronize(xs));
   for (int i = 0; i < n_jobs; ++i) {
     const int n_rec = *reinterpret_cast<const int32_t*>(h + L[i].out);
     *jobs[i].n_out = n_rec;
@@ -2955,7 +2878,7 @@ extern "C" int okb_keyframe_overlap_batch(okb_ctx* c, int n_jobs, const okb_keyf
       else o_sc[t] = sc.take(kf_buf_bytes(caps[t]), 256);
     }
   }
-  if ((rc = reserve(c, B, out_end, sc.off))) return rc;
+  if ((rc = B.reserve(c, out_end, sc.off))) return rc;
   uint8_t* h = B.h_stage;
   uint8_t* d = B.d_stage;
   std::memset(h, 0, o_tab);
@@ -2977,13 +2900,13 @@ extern "C" int okb_keyframe_overlap_batch(okb_ctx* c, int n_jobs, const okb_keyf
     }
   }
   const size_t smem = kf_buf_bytes(smem_cap);
-  FE_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
-  if (smem > 48 * 1024) FE_CUDA(c, cudaFuncSetAttribute(k_keyframe_overlap, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  OKB_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
+  if (smem > 48 * 1024) OKB_CUDA(c, cudaFuncSetAttribute(k_keyframe_overlap, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_keyframe_overlap<<<n_cta, KF_T, smem, xs>>>(reinterpret_cast<const KfCtaDev*>(d + o_tab));
   F->launches += 1;
-  FE_CUDA(c, cudaGetLastError());
-  FE_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
-  FE_CUDA(c, cudaStreamSynchronize(xs));
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
+  OKB_CUDA(c, cudaStreamSynchronize(xs));
   for (int i = 0; i < n_jobs; ++i) {
     *jobs[i].out = *reinterpret_cast<const okb_keyframe_result*>(h + o_out[i]);
     std::memcpy(jobs[i].cams, h + o_out[i] + sizeof(okb_keyframe_result), sizeof(okb_keyframe_cam) * (size_t)jobs[i].n_cams);

@@ -1,12 +1,57 @@
-// Host-side packing helpers of okb_window_upload (plain C++, no CUDA): the internal landmark order.
-// Kept in a header so that tests/hostcheck can exercise it without a GPU.
+// Host-side helpers of the library's calls (plain C++, no CUDA): buffer layout, runs of consecutive slots, host-thread
+// spreading and the internal landmark order of okb_window_upload.
+// Kept in a header so that tests/hostcheck can exercise them without a GPU.
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 
 #include <algorithm>
+#include <thread>
 #include <vector>
 
 namespace okb {
+
+// Lays arrays out one after another in a buffer: take() returns the offset of the next `bytes` and pads their end to
+// `align`, so the array after them starts aligned; `off` is the size so far.  Callers lay a buffer out once, keep the
+// offsets and fill from them.
+struct Carve {
+  size_t off = 0;
+  size_t take(size_t bytes, size_t align = 16) {
+    const size_t o = off;
+    off = (off + bytes + align - 1) / align * align;
+    return o;
+  }
+};
+
+// Calls f(first, count) for each run of consecutive slots of a list, in list order (a range is one run); stops at and
+// returns the first nonzero result.
+template <class F>
+int for_runs(const int32_t* slots, int n, F&& f) {
+  for (int i = 0; i < n;) {
+    int j = i + 1;
+    while (j < n && slots[j] == slots[j - 1] + 1) ++j;
+    const int rc = f(slots[i], j - i);
+    if (rc) return rc;
+    i = j;
+  }
+  return 0;
+}
+
+// f(i) for every i in [0, n): thread t of T runs i = t, t + T, ... in that order; T == 1 runs inline.
+template <class F>
+void parallel_for(int n, int T, const F& f) {
+  if (T <= 1) {
+    for (int i = 0; i < n; ++i) f(i);
+    return;
+  }
+  std::vector<std::thread> th;
+  th.reserve(T);
+  for (int t = 0; t < T; ++t)
+    th.emplace_back([=, &f]() {
+      for (int i = t; i < n; i += T) f(i);
+    });
+  for (auto& x : th) x.join();
+}
 
 // Sort key of a landmark with frame-visibility mask m: first observing frame * 32 + last observing frame;
 // landmarks without observations sort last.
