@@ -36,6 +36,8 @@
  *                                499-509): the same, between an older frame and the current one
  *   okb_keyframe_overlap_batch<- Frontend::doWeNeedANewKeyframe (Frontend.cpp:295-369): cv::convexHull, contourArea and
  *                                pointPolygonTest over the current frame's keypoints, for many sessions in one launch
+ *   okb_ransac_3d2d_batch     <- Frontend::runRansac3d2d (Frontend.cpp:575-642): FrameNoncentralAbsoluteAdapter's
+ *                                correspondences, FrameAbsolutePoseSacProblem's score; own sampler and generalised P3P
  *   okb_detect_describe       <- okvis::Frontend::detectAndDescribe    okvis_frontend/src/Frontend.cpp:92-114
  *                                (Frame::detect / Frame::describe      okvis_cv/include/okvis/implementation/Frame.hpp:109-156)
  */
@@ -800,6 +802,49 @@ typedef struct okb_keyframe_job {
  * back and changes nothing in the window or its store.  Results per job are bit-identical to calling it alone.
  * n_jobs == 0 is a no-op. */
 int okb_keyframe_overlap_batch(okb_ctx* ctx, int n_jobs, const okb_keyframe_job* jobs);
+
+/* ---- 3D-2D outlier rejection (Frontend::runRansac3d2d, Frontend.cpp:575-642) ------------------------------------------
+ * One job = one session's current frame: cameras 0..n_cams-1 of a feature slot of a resident window.  Per job:
+ *   correspondences as FrameNoncentralAbsoluteAdapter (FrameNoncentralAbsoluteAdapter.cpp:65-160) collects them, cameras
+ *     ascending, then keypoints ascending: the store slot names a landmark of the graph, that landmark has at least 2
+ *     observations in the window (sqrt_info != 0) and |hp[3]| >= 1e-8; point hp.head<3>() / hp[3], bearing = the
+ *     normalised backProject (a failed backProject leaves a NaN bearing: never an inlier, never in a usable sample),
+ *     sigmaAngle = sqrt(2) sigma^2 / fu^2 with sigma = 0.8 size / 12;
+ *   fewer than 2 frames in the window: ret = 1; fewer than 5 correspondences: ret = n_correspondences; no outliers;
+ *   max_iterations hypotheses, each 4 distinct correspondences drawn by a counter-based generator keyed by (seed,
+ *     hypothesis, draw) -- independent of the job's position in the batch -- the first 3 solved by a generalised P3P,
+ *     the 4th choosing the solution of lowest score; no adaptive stop (DESIGN.md 6f);
+ *   score |normalize(C_SC^T (T_WS^-1 X - r_SC)) - bearing|^2 / sigmaAngle (FrameAbsolutePoseSacProblem.hpp:134-160),
+ *     inlier iff score < threshold; the most inliers win, ties to the lowest hypothesis;
+ *   ret = n_inliers; when n_inliers >= 10 every other correspondence is an outlier record (Frontend.cpp:613-640). */
+typedef struct okb_ransac_outlier { int32_t cam, kp, lm_slot; } okb_ransac_outlier;
+typedef struct okb_ransac_result {
+  int32_t ret;                          /* what runRansac3d2d returns */
+  int32_t n_correspondences, n_inliers;
+  int32_t best;                         /* winning hypothesis, -1: no hypothesis had a model */
+  int32_t n_outliers, _pad;
+  double T_WS[7];                       /* the winner's model [t, q_xyzw], zero when best == -1 */
+} okb_ransac_result;
+typedef struct okb_ransac_job {
+  int32_t win, feat_slot, n_cams;
+  int32_t max_iterations;               /* hypotheses, 1..64 (the reference: 50) */
+  double threshold;                     /* ransac.threshold_ (9) */
+  uint64_t seed;
+  int32_t* hyp_inliers;                 /* [max_iterations] inliers of every hypothesis, or NULL */
+  okb_ransac_outlier* outliers;         /* [outlier_cap], correspondence order */
+  int32_t outlier_cap, _pad;            /* >= the keypoints of the frame in cameras 0..n_cams-1 */
+  okb_ransac_result* out;
+} okb_ransac_job;
+/* One CTA per job in one launch.  Every job is checked on the host before any device work (uploaded window, store
+ * reserved, n_cams in 1..the store's, the window's extrinsics and cameras (at most 16), the feature slot present for
+ * each camera, max_iterations in 1..64, a finite positive threshold, out present, outlier capacity, a window listed
+ * twice): the first failure returns OKB_ERR_INVALID_ARG and names the job in okb_last_error.  A landmark-sharded context
+ * returns OKB_ERR_UNSUPPORTED.  Pending edits of the job windows are committed first (removals from earlier rounds);
+ * the call runs on the transfer stream after the solver work already launched on those windows, with one H2D copy of
+ * the job table and one D2H copy of the results, returns when they are back and changes nothing in the window or its
+ * store: the caller applies the removals.  Results per job are bit-identical to calling it alone.  n_jobs == 0 is a
+ * no-op. */
+int okb_ransac_3d2d_batch(okb_ctx* ctx, int n_jobs, const okb_ransac_job* jobs);
 
 #ifdef __cplusplus
 }

@@ -892,6 +892,44 @@ class Estimator {
     j.cams = cams.data(); j.out = &out;
   }
 
+  // One okb_ransac_3d2d_batch job of this session's frame (every camera) with Frontend::runRansac3d2d's parameters
+  // (ransac.threshold_ = 9, max_iterations_ = 50) and `seed`.  finishRansac3d2d applies the device's outliers.
+  struct RansacPlan {
+    uint64_t frameId = 0;
+    std::vector<okb_ransac_outlier> outliers;
+    okb_ransac_result result{};
+    okb_ransac_job job{};
+  };
+  void planRansac3d2d(uint64_t frameId, uint64_t seed, RansacPlan& p) {
+    auto fs = featSlot_.find(frameId);
+    if (fs == featSlot_.end()) throw std::runtime_error("okvis_b200: runRansac3d2d: frame " + std::to_string(frameId) + " has no features");
+    size_t n = 0;
+    for (const FrameFeatures& f : feats_.at(frameId)) n += f.kp.size();
+    p.frameId = frameId;
+    p.outliers.assign(std::max<size_t>(n, 1), okb_ransac_outlier{});
+    p.result = okb_ransac_result{};
+    p.job = okb_ransac_job{};
+    p.job.win = slot_; p.job.feat_slot = fs->second; p.job.n_cams = (int32_t)cameras_.size();
+    p.job.max_iterations = 50; p.job.threshold = 9.0; p.job.seed = seed;
+    p.job.outliers = p.outliers.data(); p.job.outlier_cap = (int32_t)n; p.job.out = &p.result;
+  }
+  // Frontend.cpp:613-640 for the device's outliers, in correspondence order: removeObservation (when removeOutliers),
+  // then the keypoint's id set to 0.  This order, not the reference's: removeObservation rewrites the store entry to
+  // (landmark, not observed), which would undo an id cleared before it.  Throws unless each outlier's store slot is the
+  // slot of the keypoint's host id.  Returns what runRansac3d2d returns.
+  int finishRansac3d2d(const RansacPlan& p, bool removeOutliers) {
+    for (int i = 0; i < p.result.n_outliers; ++i) {
+      const okb_ransac_outlier& o = p.outliers[i];
+      const uint64_t id = feats_.at(p.frameId)[o.cam].lm[o.kp];
+      auto s = id ? lmSlot_.find(id) : lmSlot_.end();
+      if (s == lmSlot_.end() || s->second != (uint32_t)o.lm_slot)
+        throw std::runtime_error("okvis_b200: runRansac3d2d: the store and the frame's landmark ids disagree");
+      if (removeOutliers) removeObservation(id, p.frameId, (size_t)o.cam, (size_t)o.kp);
+      setFrameLandmarkId(p.frameId, (size_t)o.cam, (size_t)o.kp, 0);
+    }
+    return p.result.ret;
+  }
+
   void eraseObsHost(std::map<uint64_t, Obs>::iterator it) {
     auto lm = landmarks_.find(it->second.lm);
     if (lm != landmarks_.end()) eraseKey(lm->second, it->first);

@@ -20,9 +20,12 @@
 // rounds of matchToKeyframes (:413-452) and matchToLastFrame (:499-509) the same way (okb_match2d2d_batch, one call per
 // round, setBestMatch's bookkeeping on the host before the next round).  Frontend::doWeNeedANewKeyframe (:295-369) runs
 // on the device (okb_keyframe_overlap_batch on the current frame's store view), and
-// Frontend::dataAssociationAndInitialization (:117-271) chains all of these for one frame.  RANSAC (runRansac3d2d /
-// runRansac2d2d, on OpenGV) stays with the adaptor, in RansacHooks, and reports outliers through
-// Estimator::removeObservation and Estimator::setFrameLandmarkId (SURVEY.md 8f row 4).
+// Frontend::dataAssociationAndInitialization (:117-271) chains all of these for one frame.  Frontend::runRansac3d2d
+// (:575-642) rejects 3D-2D outliers on the device (okb_ransac_3d2d_batch: the adapter's correspondences, the project's
+// own sampler and generalised P3P, the reference's score and decision) and applies them through
+// Estimator::removeObservation and Estimator::setFrameLandmarkId; with RansacHooks::device3d2d set,
+// dataAssociationAndInitialization runs it at both of the reference's call points.  runRansac2d2d (on OpenGV) stays
+// with the adaptor, in RansacHooks.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -37,6 +40,24 @@
 #include "okvis_b200_estimator.hpp"
 
 namespace okvis_b200 {
+
+// Frontend::RansacHooks (declared here so that its defaults hold in Frontend's default arguments): the three places
+// where the reference runs RANSAC, each receiving the session index (0 for the single form) and that
+// session's initialisation flag.  The adaptor keeps OpenGV there and reports outliers through
+// Estimator::removeObservation and Estimator::setFrameLandmarkId(..., 0).  An empty hook means no RANSAC.
+struct FrontendRansacHooks {
+  // true: runRansac3d2d on the device at both of its call points, before the hooks there are called -- after the
+  // first keyframe's 2D-2D rounds for initialised sessions (:434-436) and after matchToLastFrame's 3D-2D rounds
+  // (:496-497) -- one device call for all sessions that reach the point; afterKeyframe is then left with runRansac2d2d
+  bool device3d2d = false;
+  // after each keyframe's 2D-2D rounds of matchToKeyframes (:432-447): runRansac3d2d when kfcounter == 0 and
+  // initialised, runRansac2d2d while not initialised; returns rotationOnly_tmp (empty hook: false)
+  std::function<bool(size_t session, bool initialized, size_t kfcounter, uint64_t olderFrameId)> afterKeyframe;
+  // matchToLastFrame, between its 3D-2D and 2D-2D rounds (:496-497): runRansac3d2d
+  std::function<void(size_t session, bool initialized)> afterLastFrame3D2D;
+  // matchToLastFrame, after its 2D-2D rounds (:512-515): runRansac2d2d while not initialised
+  std::function<void(size_t session, bool initialized)> afterLastFrame2D2D;
+};
 
 class Frontend {
  public:
@@ -220,19 +241,23 @@ class Frontend {
     return keyframeGroup(&group, cs, frameIds, initialized, cams, results);
   }
 
+  // ---- 3D-2D outlier rejection (device: okb_ransac_3d2d_batch)
+  // Frontend::runRansac3d2d (Frontend.cpp:575-642) on the current frame's features: numFrames() < 2 returns 1 on the
+  // host; otherwise one device job (threshold 9, 50 hypotheses, seed = currentFrameId) and, for every outlier,
+  // Estimator::removeObservation (when removeOutliers) and then Estimator::setFrameLandmarkId(..., 0), which leaves the
+  // keypoint with host id 0, store slot -1 and no observation.  Returns what the reference returns.
+  int runRansac3d2d(Estimator& estimator, uint64_t currentFrameId, bool removeOutliers = true) {
+    return ransacGroup(nullptr, {&estimator}, {currentFrameId}, removeOutliers)[0];
+  }
+  // The same for sessions of one EstimatorGroup: one okb_ransac_3d2d_batch for every session with 2 frames or more;
+  // results[i] and the removals equal the single call's on sessions[i].
+  std::vector<int> runRansac3d2d(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& currentFrameIds,
+                                 bool removeOutliers = true) {
+    return ransacGroup(&group, sessions, currentFrameIds, removeOutliers);
+  }
+
   // ---- one frame of Frontend::dataAssociationAndInitialization (Frontend.cpp:117-271)
-  // The three places where the reference runs RANSAC, each receiving the session index (0 for the single form) and that
-  // session's initialisation flag.  The adaptor keeps OpenGV there and reports outliers through
-  // Estimator::removeObservation and Estimator::setFrameLandmarkId(..., 0).  An empty hook means no RANSAC.
-  struct RansacHooks {
-    // after each keyframe's 2D-2D rounds of matchToKeyframes (:432-447): runRansac3d2d when kfcounter == 0 and
-    // initialised, runRansac2d2d while not initialised; returns rotationOnly_tmp (empty hook: false)
-    std::function<bool(size_t session, bool initialized, size_t kfcounter, uint64_t olderFrameId)> afterKeyframe;
-    // matchToLastFrame, between its 3D-2D and 2D-2D rounds (:496-497): runRansac3d2d
-    std::function<void(size_t session, bool initialized)> afterLastFrame3D2D;
-    // matchToLastFrame, after its 2D-2D rounds (:512-515): runRansac2d2d while not initialised
-    std::function<void(size_t session, bool initialized)> afterLastFrame2D2D;
-  };
+  using RansacHooks = FrontendRansacHooks;
   struct FrameResult {
     std::vector<std::vector<uint64_t>> landmarkIds;   // the frame's ids per camera after matchStereo
     int num3dMatches = 0;                             // matchToKeyframes' retCtr (its 3D-2D and 2D-2D matches)
@@ -321,7 +346,15 @@ class Frontend {
         const bool tmp = hooks.afterKeyframe ? hooks.afterKeyframe(at[k], initialized[at[k]] != 0, kf, older) : false;
         if (first[k]) { rotationOnly[k] = tmp ? 1 : 0; first[k] = 0; }
       };
-      const std::vector<TrackResult> kf2 = match2D2DGroup(group, s, f, ni, true, afterKeyframe);
+      std::function<void(const std::vector<size_t>&)> firstKeyframeRansac;
+      if (hooks.device3d2d)
+        firstKeyframeRansac = [&](const std::vector<size_t>& ks) {      // kfcounter == 0 && isInitialized_ (:434-436)
+          std::vector<Estimator*> rs;
+          std::vector<uint64_t> rf;
+          for (size_t k : ks) if (initialized[at[k]]) { rs.push_back(s[k]); rf.push_back(f[k]); }
+          if (!rs.empty()) ransacGroup(group, rs, rf, true);
+        };
+      const std::vector<TrackResult> kf2 = match2D2DGroup(group, s, f, ni, true, afterKeyframe, firstKeyframeRansac);
       for (size_t k = 0; k < at.size(); ++k) {
         out[at[k]].num3dMatches = kf3[k].numMatches + kf2[k].numMatches;
         if (!initialized[at[k]] && !rotationOnly[k]) initialized[at[k]] = 1;     // (:184-189)
@@ -343,6 +376,12 @@ class Frontend {
       std::vector<char> last(at.size());
       for (size_t k = 0; k < at.size(); ++k) last[k] = s[k]->isKeyframe(s[k]->frameIdByAge(1)) ? 0 : 1;
       trackGroup(group, s, f, false);
+      if (hooks.device3d2d) {                                              // (:496-497)
+        std::vector<Estimator*> rs;
+        std::vector<uint64_t> rf;
+        for (size_t k = 0; k < at.size(); ++k) if (last[k]) { rs.push_back(s[k]); rf.push_back(f[k]); }
+        if (!rs.empty()) ransacGroup(group, rs, rf, true);
+      }
       if (hooks.afterLastFrame3D2D)
         for (size_t k = 0; k < at.size(); ++k) if (last[k]) hooks.afterLastFrame3D2D(at[k], initialized[at[k]] != 0);
       match2D2DGroup(group, s, f, ni, false, {});
@@ -368,7 +407,8 @@ class Frontend {
 
   std::vector<TrackResult> match2D2DGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                           const std::vector<std::function<uint64_t()>>& newIds, bool keyframes,
-                                          const std::function<void(size_t, size_t, uint64_t)>& afterKeyframe) {
+                                          const std::function<void(size_t, size_t, uint64_t)>& afterKeyframe,
+                                          const std::function<void(const std::vector<size_t>&)>& firstKeyframeDone = {}) {
     const size_t n = sessions.size();
     if (frameIds.size() != n || newIds.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one id source per session");
     if (group) group->validate(sessions);
@@ -411,6 +451,12 @@ class Frontend {
           throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
       }
       for (size_t i = 0; i < n; ++i) if (has[i]) out[i].numMatches += sessions[i]->finish2D2D(plans[i], newIds[i]);
+      if (firstKeyframeDone) {                         // the sessions whose first keyframe's rounds end here, before afterKeyframe
+        std::vector<size_t> done;
+        for (size_t i = 0; i < n; ++i)
+          if (r < rounds[i].size() && rounds[i][r].last && rounds[i][r].kf == 0) done.push_back(i);
+        if (!done.empty()) firstKeyframeDone(done);
+      }
       if (afterKeyframe)
         for (size_t i = 0; i < n; ++i)
           if (r < rounds[i].size() && rounds[i][r].last) afterKeyframe(i, rounds[i][r].kf, rounds[i][r].frameA);
@@ -465,6 +511,30 @@ class Frontend {
       sessions[i]->nameRemainingKeypoints(frameIds[i], newIds[i]);
       for (size_t c = 0; c < C; ++c) out[i].landmarkIds.push_back(sessions[i]->frameLandmarkIds(frameIds[i], c));
     }
+    return out;
+  }
+
+  std::vector<int> ransacGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                               bool removeOutliers) {
+    const size_t n = sessions.size();
+    if (frameIds.size() != n) throw std::invalid_argument("okvis_b200: one current frame id per session");
+    if (group) group->validate(sessions);
+    std::vector<int> out(n, 1);                        // nothing to match against, just starting (:579-582)
+    std::vector<Estimator::RansacPlan> plans(n);
+    std::vector<char> has(n, 0);
+    std::vector<okb_ransac_job> jobs;
+    for (size_t i = 0; i < n; ++i) {
+      if (sessions[i]->numFrames() < 2) continue;
+      sessions[i]->planRansac3d2d(frameIds[i], frameIds[i], plans[i]);
+      has[i] = 1;
+      jobs.push_back(plans[i].job);
+    }
+    if (!jobs.empty()) {
+      okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
+      if (okb_ransac_3d2d_batch(ctx, (int)jobs.size(), jobs.data()) != OKB_OK)
+        throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+    }
+    for (size_t i = 0; i < n; ++i) if (has[i]) out[i] = sessions[i]->finishRansac3d2d(plans[i], removeOutliers);
     return out;
   }
 

@@ -153,6 +153,17 @@ class KeyframeJob(C.Structure):
                 ("out", C.POINTER(KeyframeResult))]
 
 
+class RansacResult(C.Structure):
+    _fields_ = [("ret", C.c_int32), ("n_correspondences", C.c_int32), ("n_inliers", C.c_int32), ("best", C.c_int32),
+                ("n_outliers", C.c_int32), ("_pad", C.c_int32), ("T_WS", C.c_double * 7)]
+
+
+class RansacJob(C.Structure):
+    _fields_ = [("win", C.c_int32), ("feat_slot", C.c_int32), ("n_cams", C.c_int32), ("max_iterations", C.c_int32),
+                ("threshold", C.c_double), ("seed", C.c_uint64), ("hyp_inliers", C.POINTER(C.c_int32)),
+                ("outliers", C.c_void_p), ("outlier_cap", C.c_int32), ("_pad", C.c_int32), ("out", C.POINTER(RansacResult))]
+
+
 class PropagateJob(C.Structure):
     _fields_ = [("params", C.POINTER(ImuParams)), ("samples", C.c_void_p), ("n_samples", C.c_int32), ("_pad", C.c_int32),
                 ("t0_ns", C.c_int64), ("t1_ns", C.c_int64), ("pose", c_double_p), ("speed_bias", c_double_p),
@@ -208,6 +219,7 @@ keypoint_dtype = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle"
 pair_dtype = np.dtype([("index_a", "<i4"), ("distance", "<f4")], align=True)
 stereo_match_dtype = np.dtype([("kp_a", "<i4"), ("kp_b", "<i4"), ("lm_slot_a", "<i4"), ("lm_slot_b", "<i4"),
                                ("can_be_initialized", "<i4"), ("_pad", "<i4"), ("hp_W", "<f8", (4,))], align=True)
+ransac_outlier_dtype = np.dtype([("cam", "<i4"), ("kp", "<i4"), ("lm_slot", "<i4")], align=True)
 track_assoc_dtype = np.dtype([("round", "<i4"), ("cam_b", "<i4"), ("kp_b", "<i4"), ("lm_slot", "<i4"), ("uncertain", "<i4"),
                               ("_pad", "<i4")], align=True)
 

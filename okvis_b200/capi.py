@@ -669,6 +669,33 @@ class Context:
                      cams=[{k: getattr(o["cams"][c], k) for k, _ in abi.KeyframeCam._fields_} for c in range(n)])
                 for o, n in outs]
 
+    def ransac_3d2d_batch(self, jobs):
+        """okb_ransac_3d2d_batch.  jobs: dicts with win, feat_slot, n_cams, seed and optionally max_iterations (50) and
+        threshold (9.0).  Returns one dict per job: okb_ransac_result's fields (T_WS as an array of 7), hyp_inliers (the
+        inliers of every hypothesis) and outliers (ransac_outlier_dtype, correspondence order)."""
+        arr = (abi.RansacJob * max(len(jobs), 1))()
+        outs = []
+        for i, j in enumerate(jobs):
+            n_hyp = int(j.get("max_iterations", 50))
+            cap = int(j.get("outlier_cap", max(int(j["n_cams"]), 0) * getattr(self, "_feat", {}).get(int(j["win"]), 0)))
+            o = dict(res=abi.RansacResult(), hyp=np.zeros(max(n_hyp, 1), np.int32), outl=np.zeros(max(cap, 1), abi.ransac_outlier_dtype))
+            t = arr[i]
+            t.win, t.feat_slot, t.n_cams, t.max_iterations = int(j["win"]), int(j["feat_slot"]), int(j["n_cams"]), n_hyp
+            t.threshold, t.seed = float(j.get("threshold", 9.0)), int(j["seed"]) & 0xFFFFFFFFFFFFFFFF
+            t.hyp_inliers = o["hyp"].ctypes.data_as(C.POINTER(C.c_int32))
+            t.outliers, t.outlier_cap = o["outl"].ctypes.data, cap
+            t.out = C.pointer(o["res"]) if j.get("out", True) is not None else None
+            outs.append((o, n_hyp))
+        self._check(lib().okb_ransac_3d2d_batch(self._h, len(jobs), arr))
+        res = []
+        for o, n_hyp in outs:
+            r = {k: getattr(o["res"], k) for k, _ in abi.RansacResult._fields_ if k not in ("_pad", "T_WS")}
+            r["T_WS"] = np.array(o["res"].T_WS[:])
+            r["hyp_inliers"] = o["hyp"][:n_hyp].copy()
+            r["outliers"] = o["outl"][:r["n_outliers"]].copy()
+            res.append(r)
+        return res
+
     def hamming_match_batch(self, jobs, desc_bytes):
         """okb_hamming_match_batch over `jobs`: make_match_job results, or dicts of its keyword arguments.  Returns one
         dict(topk, pairs) per job, like hamming_match / hamming_match_gated."""

@@ -151,12 +151,13 @@ struct okb_frontend_state {
   CallBuffers track;               // okb_track_3d2d_batch
   CallBuffers stereo;              // okb_match2d2d_batch / okb_stereo_init_batch
   CallBuffers kf;                  // okb_keyframe_overlap_batch (scratch: images too large for shared memory)
+  CallBuffers ransac;              // okb_ransac_3d2d_batch
 };
 
 void okb_frontend_release(okb_ctx* c) {
   if (!c->frontend) return;
   okb_frontend_state* F = c->frontend;
-  for (CallBuffers* b : {&F->match_io, &F->batch_match, &F->track, &F->stereo, &F->kf}) b->release();
+  for (CallBuffers* b : {&F->match_io, &F->batch_match, &F->track, &F->stereo, &F->kf, &F->ransac}) b->release();
   F->batch_det.release();
   if (F->batch_stream) cudaStreamDestroy(F->batch_stream);
   for (auto& s : F->slots) {
@@ -2910,6 +2911,552 @@ extern "C" int okb_keyframe_overlap_batch(okb_ctx* c, int n_jobs, const okb_keyf
   for (int i = 0; i < n_jobs; ++i) {
     *jobs[i].out = *reinterpret_cast<const okb_keyframe_result*>(h + o_out[i]);
     std::memcpy(jobs[i].cams, h + o_out[i] + sizeof(okb_keyframe_result), sizeof(okb_keyframe_cam) * (size_t)jobs[i].n_cams);
+  }
+  return OKB_OK;
+}
+
+// =================================================================================================
+// 3D-2D outlier rejection (okb_ransac_3d2d_batch): Frontend::runRansac3d2d (okvis_frontend/src/Frontend.cpp:575-642) on
+// the window's feature store, one CTA per job in one launch (DESIGN.md 6f; tests/ransac_reference.py restates it):
+//   1. the observation counts of the window's landmarks, then FrameNoncentralAbsoluteAdapter's correspondences
+//      (FrameNoncentralAbsoluteAdapter.cpp:65-160) compacted in (camera, keypoint) order by a block scan;
+//   2. one thread per hypothesis: 4 distinct correspondences from a counter-based SplitMix64 draw, a generalised P3P on
+//      the first 3 (an octic in the first depth whose positive roots are bracketed by the roots of its derivatives),
+//      the 4th picking the solution of lowest score;
+//   3. the whole CTA scores hypotheses x correspondences (FrameAbsolutePoseSacProblem.hpp:134-160), a warp per
+//      hypothesis; thread 0 takes the winner (most inliers, the lowest index on ties);
+//   4. with at least 10 inliers, the other correspondences as outlier records in correspondence order (block scan).
+// The call writes nothing but its scratch and its results.
+// =================================================================================================
+namespace {
+constexpr int RS_T = 256;
+constexpr int RS_MAX_HYP = 64;
+constexpr int RS_MAX_CAMS = 16;
+constexpr int RS_CD = 10;          // doubles per correspondence: point X_W (3), bearing (3), ray C_SC bearing (3), sigmaAngle
+constexpr int RS_BISECT = 60;      // bisection steps per bracketed root, every derivative level
+constexpr int RS_POLISH = 2;       // Gauss-Newton steps on the three distance equations
+
+struct RansacJobDev {
+  const WinDev* W;
+  int feat, n_cams, n_hyp, cnt_cap;
+  double threshold;
+  unsigned long long seed;
+  int* cnt;                        // [cnt_cap] observations per landmark slot (scratch)
+  double* cd;                      // [n_kp][RS_CD] correspondences (scratch)
+  int* ci;                         // [n_kp][3] camera, keypoint, landmark slot (scratch)
+  okb_ransac_result* res;
+  int* hyp;                        // [n_hyp] inliers per hypothesis
+  okb_ransac_outlier* outl;
+};
+
+// SplitMix64's output for the counter (hypothesis h, draw c) of a seed: the state after h * 2^32 + c + 1 steps
+__device__ __forceinline__ unsigned long long rs_draw(unsigned long long seed, int h, int c) {
+  unsigned long long z = seed + 0x9E3779B97F4A7C15ull * ((((unsigned long long)h) << 32) + (unsigned long long)c + 1ull);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+// 4 distinct indices in [0, n) (multiply-shift of the draw's high word); a duplicate is redrawn with the next counter,
+// at most 64 draws (false: no sample)
+__device__ bool rs_sample(unsigned long long seed, int h, int n, int* idx) {
+  int m = 0;
+  for (int c = 0; c < 64 && m < 4; ++c) {
+    const int v = (int)(((rs_draw(seed, h, c) >> 32) * (unsigned long long)n) >> 32);
+    bool dup = false;
+    for (int i = 0; i < m; ++i) dup = dup || idx[i] == v;
+    if (!dup) idx[m++] = v;
+  }
+  return m == 4;
+}
+
+__device__ __forceinline__ double rs_dot(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+__device__ __forceinline__ double rs_horner(const double* c, int m, double x) {
+  double v = c[m];
+  for (int i = m - 1; i >= 0; --i) v = v * x + c[i];
+  return v;
+}
+// r = p q (degrees np, nq)
+__device__ void rs_umul(const double* p, int np, const double* q, int nq, double* r) {
+  for (int k = 0; k <= np + nq; ++k) r[k] = 0.0;
+  for (int i = 0; i <= np; ++i)
+    for (int j = 0; j <= nq; ++j) r[i + j] += p[i] * q[j];
+}
+// C = A B for polynomials in (x, y) of total degree <= 4, M[i][j] = coefficient of x^i y^j
+__device__ void rs_bmul(const double (*A)[5], const double (*B)[5], double (*Cm)[5]) {
+  for (int i = 0; i < 5; ++i)
+    for (int j = 0; j < 5; ++j) Cm[i][j] = 0.0;
+  for (int i1 = 0; i1 < 5; ++i1)
+    for (int j1 = 0; i1 + j1 < 5; ++j1) {
+      if (A[i1][j1] == 0.0) continue;
+      for (int i2 = 0; i1 + i2 < 5; ++i2)
+        for (int j2 = 0; i1 + i2 + j1 + j2 < 5; ++j2) Cm[i1 + i2][j1 + j2] += A[i1][j1] * B[i2][j2];
+    }
+}
+
+// The roots of p (degree <= 8) in (0, B], B = Cauchy's bound of p made monic after dropping leading coefficients below
+// 1e-14 of the largest, ascending.  Level m = 1..n takes the (n-m)-th derivative: between consecutive roots of the level
+// below (and 0, B) it is monotone, and each sign change is bisected RS_BISECT times.
+__device__ int rs_positive_roots(const double* p, double* roots) {
+  double mx = 0.0;
+  for (int i = 0; i <= 8; ++i) {
+    if (!isfinite(p[i])) return 0;
+    mx = fmax(mx, fabs(p[i]));
+  }
+  int n = 8;
+  while (n > 0 && !(fabs(p[n]) > 1e-14 * mx)) --n;
+  if (n == 0) return 0;
+  double q[9];
+  for (int i = 0; i <= n; ++i) q[i] = p[i] / p[n];
+  double bound = 0.0;
+  for (int i = 0; i < n; ++i) bound = fmax(bound, fabs(q[i]));
+  bound += 1.0;
+  int nr = 0;
+  for (int m = 1; m <= n; ++m) {
+    double c[9];
+    for (int i = 0; i <= m; ++i) {
+      double f = q[i + n - m];
+      for (int t = i + 1; t <= i + n - m; ++t) f *= (double)t;
+      c[i] = f;
+    }
+    double nxt[8];
+    int k = 0;
+    double lo = 0.0, flo = rs_horner(c, m, 0.0);
+    for (int e = 0; e <= nr; ++e) {
+      const double hi = e < nr ? roots[e] : bound;
+      const double fhi = rs_horner(c, m, hi);
+      if ((flo < 0.0 && fhi >= 0.0) || (flo > 0.0 && fhi <= 0.0)) {
+        const bool neg = flo < 0.0;
+        double a = lo, b = hi;
+        for (int it = 0; it < RS_BISECT; ++it) {
+          const double mid = 0.5 * (a + b);
+          if ((rs_horner(c, m, mid) < 0.0) == neg) a = mid; else b = mid;
+        }
+        nxt[k++] = 0.5 * (a + b);
+      }
+      lo = hi; flo = fhi;
+    }
+    for (int i = 0; i < k; ++i) roots[i] = nxt[i];
+    nr = k;
+  }
+  return nr;
+}
+
+// Generalised P3P: rays c_i + l_i f_i (body frame, |f_i| = 1) through world points X_i, i = 0..2.  Depths solve
+// Q_ij = |c_i + l_i f_i - c_j - l_j f_j|^2 - |X_i - X_j|^2 = 0 (DESIGN.md 6f): the problem scaled to unit size, the
+// resultant of Q02 and Q12 in l_2 reduced modulo Q01 in l_1 to alpha l_1 + beta, the octic alpha^2 b - alpha beta a + beta^2
+// in l_0, its positive roots, l_1 = -beta / alpha, l_2 = -D_q / D_p, RS_POLISH Gauss-Newton steps; admissible when every
+// depth is positive and every equation holds to 1e-10 of |X_i - X_j|^2.  emit(R, t) (X = R p + t) per admissible
+// solution, ascending l_0; (R, t) from the two triangles by the triad of their first edge and normal, about the
+// centroids.
+template <typename Emit>
+__device__ void rs_gp3p(const double (*c)[3], const double (*f)[3], const double (*X)[3], Emit&& emit) {
+  double dX[3][3];
+  for (int k = 0; k < 3; ++k) { dX[0][k] = X[0][k] - X[1][k]; dX[1][k] = X[0][k] - X[2][k]; dX[2][k] = X[1][k] - X[2][k]; }
+  const double D01 = rs_dot(dX[0], dX[0]), D02 = rs_dot(dX[1], dX[1]), D12 = rs_dot(dX[2], dX[2]);
+  const double s = sqrt(fmax(D01, fmax(D02, D12)));
+  if (!(s > 0.0) || !isfinite(s)) return;
+  const double is = 1.0 / s;
+  double c01[3], c02[3], c12[3];
+  for (int k = 0; k < 3; ++k) {
+    c01[k] = (c[0][k] - c[1][k]) * is; c02[k] = (c[0][k] - c[2][k]) * is; c12[k] = (c[1][k] - c[2][k]) * is;
+  }
+  const double d01 = D01 * is * is, d02 = D02 * is * is, d12 = D12 * is * is;
+  const double f01 = rs_dot(f[0], f[1]), f02 = rs_dot(f[0], f[2]), f12 = rs_dot(f[1], f[2]);
+  const double k01 = rs_dot(c01, c01) - d01, k02 = rs_dot(c02, c02) - d02, k12 = rs_dot(c12, c12) - d12;
+  const double g0_01 = rs_dot(f[0], c01), g1_01 = rs_dot(f[1], c01), g0_02 = rs_dot(f[0], c02), g2_02 = rs_dot(f[2], c02);
+  const double g1_12 = rs_dot(f[1], c12), g2_12 = rs_dot(f[2], c12), g2_01 = rs_dot(f[2], c01);
+  double Dp[5][5] = {}, Dq[5][5] = {}, R1[5][5] = {}, P1[5][5] = {}, T1[5][5], T2[5][5], S[5][5];
+  Dp[1][0] = 2.0 * f02; Dp[0][1] = -2.0 * f12; Dp[0][0] = 2.0 * g2_01;
+  Dq[0][2] = 1.0; Dq[0][1] = 2.0 * g1_12; Dq[0][0] = k12 - k02; Dq[1][0] = -2.0 * g0_02; Dq[2][0] = -1.0;
+  R1[2][0] = 1.0; R1[1][0] = 2.0 * g0_02; R1[0][0] = k02;
+  P1[1][0] = -2.0 * f02; P1[0][0] = -2.0 * g2_02;
+  rs_bmul(Dp, R1, T1);
+  rs_bmul(Dq, P1, T2);
+  for (int i = 0; i < 5; ++i)
+    for (int j = 0; j < 5; ++j) T1[i][j] -= T2[i][j];
+  rs_bmul(Dp, T1, S);
+  rs_bmul(Dq, Dq, T2);
+  for (int i = 0; i < 5; ++i)
+    for (int j = 0; j < 5; ++j) S[i][j] += T2[i][j];
+  // S modulo Q01 = l_1^2 + a l_1 + b: l_1^2 = -a l_1 - b, l_1^3 = (a^2 - b) l_1 + a b, l_1^4 = (2 a b - a^3) l_1 + b^2 - a^2 b
+  const double a[2] = {-2.0 * g1_01, -2.0 * f01};
+  const double b[3] = {k01, 2.0 * g0_01, 1.0};
+  double A2[3], AB[4], A3[4], A2B[5], B2[5], r3y[3], r4y[4], r4c[5];
+  rs_umul(a, 1, a, 1, A2);
+  rs_umul(a, 1, b, 2, AB);
+  rs_umul(A2, 2, a, 1, A3);
+  rs_umul(A2, 2, b, 2, A2B);
+  rs_umul(b, 2, b, 2, B2);
+  for (int i = 0; i < 3; ++i) r3y[i] = A2[i] - b[i];
+  for (int i = 0; i < 4; ++i) r4y[i] = 2.0 * AB[i] - A3[i];
+  for (int i = 0; i < 5; ++i) r4c[i] = B2[i] - A2B[i];
+  double sk[5][5];                                  // sk[k] = coefficient of l_1^k, a polynomial in l_0 of degree 4 - k
+  for (int k = 0; k < 5; ++k)
+    for (int i = 0; i < 5; ++i) sk[k][i] = S[i][k];
+  double al[9] = {}, be[9] = {}, t[9];
+  for (int i = 0; i < 4; ++i) al[i] = sk[1][i];
+  rs_umul(a, 1, sk[2], 2, t);  for (int i = 0; i < 4; ++i) al[i] -= t[i];
+  rs_umul(r3y, 2, sk[3], 1, t); for (int i = 0; i < 4; ++i) al[i] += t[i];
+  rs_umul(r4y, 3, sk[4], 0, t); for (int i = 0; i < 4; ++i) al[i] += t[i];
+  for (int i = 0; i < 5; ++i) be[i] = sk[0][i];
+  rs_umul(b, 2, sk[2], 2, t);  for (int i = 0; i < 5; ++i) be[i] -= t[i];
+  rs_umul(AB, 3, sk[3], 1, t); for (int i = 0; i < 5; ++i) be[i] += t[i];
+  rs_umul(r4c, 4, sk[4], 0, t); for (int i = 0; i < 5; ++i) be[i] += t[i];
+  double oct[9], u[9];
+  rs_umul(al, 3, al, 3, u);   rs_umul(u, 6, b, 2, oct);
+  rs_umul(al, 3, be, 4, u);   rs_umul(u, 7, a, 1, t);  for (int i = 0; i < 9; ++i) oct[i] -= t[i];
+  rs_umul(be, 4, be, 4, u);   for (int i = 0; i < 9; ++i) oct[i] += u[i];
+  double roots[8];
+  const int nr = rs_positive_roots(oct, roots);
+  for (int r = 0; r < nr; ++r) {
+    double x = roots[r];
+    const double alx = rs_horner(al, 3, x), bex = rs_horner(be, 4, x);
+    if (alx == 0.0) continue;
+    double y = -bex / alx;
+    const double dp = 2.0 * f02 * x - 2.0 * f12 * y + 2.0 * g2_01;
+    if (dp == 0.0) continue;
+    const double dq = y * y + 2.0 * g1_12 * y + (k12 - k02) - x * x - 2.0 * g0_02 * x;
+    double z = -dq / dp;
+    for (int it = 0; it < RS_POLISH; ++it) {
+      const double F0 = x * x + y * y - 2.0 * f01 * x * y + 2.0 * g0_01 * x - 2.0 * g1_01 * y + k01;
+      const double F1 = x * x + z * z - 2.0 * f02 * x * z + 2.0 * g0_02 * x - 2.0 * g2_02 * z + k02;
+      const double F2 = y * y + z * z - 2.0 * f12 * y * z + 2.0 * g1_12 * y - 2.0 * g2_12 * z + k12;
+      const double A = 2.0 * x - 2.0 * f01 * y + 2.0 * g0_01, B = 2.0 * y - 2.0 * f01 * x - 2.0 * g1_01;
+      const double C = 2.0 * x - 2.0 * f02 * z + 2.0 * g0_02, D = 2.0 * z - 2.0 * f02 * x - 2.0 * g2_02;
+      const double E = 2.0 * y - 2.0 * f12 * z + 2.0 * g1_12, G = 2.0 * z - 2.0 * f12 * y - 2.0 * g2_12;
+      const double det = -A * D * E - B * C * G;
+      if (!(det != 0.0) || !isfinite(det)) break;
+      x += (F0 * D * E + B * F1 * G - B * D * F2) / det;
+      y += (-A * F1 * G + A * D * F2 + F0 * C * G) / det;
+      z += (A * F1 * E + B * C * F2 - F0 * C * E) / det;
+    }
+    if (!(x > 0.0 && y > 0.0 && z > 0.0) || !isfinite(x + y + z)) continue;
+    const double lam[3] = {x, y, z};
+    double pp[3][3];                                  // scaled body points
+    for (int i = 0; i < 3; ++i)
+      for (int k = 0; k < 3; ++k) pp[i][k] = c[i][k] * is + lam[i] * f[i][k];
+    const int pr[3][2] = {{0, 1}, {0, 2}, {1, 2}};
+    const double dd[3] = {d01, d02, d12};
+    bool ok = true;
+    for (int e = 0; e < 3; ++e) {
+      double v[3];
+      for (int k = 0; k < 3; ++k) v[k] = pp[pr[e][0]][k] - pp[pr[e][1]][k];
+      ok = ok && fabs(rs_dot(v, v) - dd[e]) <= 1e-10 * dd[e];
+    }
+    if (!ok) continue;
+    double p[3][3];                                   // body points, metric
+    for (int i = 0; i < 3; ++i)
+      for (int k = 0; k < 3; ++k) p[i][k] = c[i][k] + (lam[i] * s) * f[i][k];
+    double Fp[3][3], Fx[3][3];                        // rows: e1, e2, n
+    for (int side = 0; side < 2; ++side) {
+      const double (*P)[3] = side ? X : p;
+      double (*Fr)[3] = side ? Fx : Fp;
+      double u1[3], u2[3], nn[3];
+      for (int k = 0; k < 3; ++k) { u1[k] = P[1][k] - P[0][k]; u2[k] = P[2][k] - P[0][k]; }
+      nn[0] = u1[1] * u2[2] - u1[2] * u2[1]; nn[1] = u1[2] * u2[0] - u1[0] * u2[2]; nn[2] = u1[0] * u2[1] - u1[1] * u2[0];
+      const double i1 = 1.0 / sqrt(rs_dot(u1, u1)), in = 1.0 / sqrt(rs_dot(nn, nn));
+      for (int k = 0; k < 3; ++k) { Fr[0][k] = u1[k] * i1; Fr[2][k] = nn[k] * in; }
+      Fr[1][0] = Fr[2][1] * Fr[0][2] - Fr[2][2] * Fr[0][1];
+      Fr[1][1] = Fr[2][2] * Fr[0][0] - Fr[2][0] * Fr[0][2];
+      Fr[1][2] = Fr[2][0] * Fr[0][1] - Fr[2][1] * Fr[0][0];
+    }
+    double R[9], tt[3];
+    for (int r0 = 0; r0 < 3; ++r0)
+      for (int c0 = 0; c0 < 3; ++c0) R[3 * r0 + c0] = Fx[0][r0] * Fp[0][c0] + Fx[1][r0] * Fp[1][c0] + Fx[2][r0] * Fp[2][c0];
+    if (!isfinite(R[0] + R[1] + R[2] + R[3] + R[4] + R[5] + R[6] + R[7] + R[8])) continue;
+    double pc[3], xc[3];
+    for (int k = 0; k < 3; ++k) { pc[k] = (p[0][k] + p[1][k] + p[2][k]) / 3.0; xc[k] = (X[0][k] + X[1][k] + X[2][k]) / 3.0; }
+    for (int k = 0; k < 3; ++k) tt[k] = xc[k] - (R[3 * k] * pc[0] + R[3 * k + 1] * pc[1] + R[3 * k + 2] * pc[2]);
+    emit(R, tt);
+  }
+}
+
+// FrameAbsolutePoseSacProblem::getSelectedDistancesToModel for one correspondence: model (R, t) = T_WS, the camera's
+// (C_SC row-major, r_SC)
+__device__ __forceinline__ double rs_score(const double* R, const double* t, const double* cd, const double* ext) {
+  double body[3];
+  for (int r = 0; r < 3; ++r) {
+    const double ti = -(R[r] * t[0] + R[3 + r] * t[1] + R[6 + r] * t[2]);
+    body[r] = R[r] * cd[0] + R[3 + r] * cd[1] + R[6 + r] * cd[2] + ti;
+  }
+  const double v[3] = {body[0] - ext[9], body[1] - ext[10], body[2] - ext[11]};
+  double rep[3];
+  for (int r = 0; r < 3; ++r) rep[r] = ext[r] * v[0] + ext[3 + r] * v[1] + ext[6 + r] * v[2];
+  const double nrm = sqrt(rs_dot(rep, rep));
+  const double e[3] = {rep[0] / nrm - cd[3], rep[1] / nrm - cd[4], rep[2] / nrm - cd[5]};
+  return rs_dot(e, e) / cd[9];
+}
+
+__global__ void __launch_bounds__(RS_T) k_ransac_3d2d(const RansacJobDev* __restrict__ jobs) {
+  __shared__ int s_warp[RS_T / 32];
+  __shared__ double s_ext[RS_MAX_CAMS][12];         // C_SC (row-major), r_SC
+  __shared__ double s_model[RS_MAX_HYP][12];        // R (row-major), t
+  __shared__ int s_cnt[RS_MAX_HYP];
+  __shared__ int s_ok[RS_MAX_HYP];
+  __shared__ int s_best;
+  const RansacJobDev& J = jobs[blockIdx.x];
+  const WinDev& W = *J.W;
+  const FeatStore& F = *W.feat;
+  const int tid = threadIdx.x;
+  okb_ransac_result res;
+  memset(&res, 0, sizeof res);
+  res.best = -1;
+  if (W.st->g.K < 2) {                              // Frontend.cpp:579-582
+    res.ret = 1;
+    if (tid == 0) *J.res = res;
+    for (int h = tid; h < J.n_hyp; h += RS_T) J.hyp[h] = 0;
+    return;
+  }
+  // observation counts (landmark.observations.size())
+  const int L = min(W.st->g.L, J.cnt_cap);
+  for (int i = tid; i < J.cnt_cap; i += RS_T) J.cnt[i] = 0;
+  if (tid < J.n_cams) {
+    XfQ T;
+    const double* E = W.ext + 7 * (size_t)tid;
+    xfq_make(E, E + 3, T);
+    for (int k = 0; k < 9; ++k) s_ext[tid][k] = T.C[k];
+    for (int k = 0; k < 3; ++k) s_ext[tid][9 + k] = T.r[k];
+  }
+  __syncthreads();
+  const int n_obs = W.st->g.n_obs;
+  for (int i = tid; i < n_obs; i += RS_T) {
+    const okb_observation& ob = W.m_obs[i];
+    if (ob.sqrt_info != 0.0 && (int)ob.lm_idx < L) atomicAdd(&J.cnt[ob.lm_idx], 1);
+  }
+  __syncthreads();
+  // the adapter's correspondences, cameras ascending, keypoints ascending
+  int n = 0;
+  for (int cam = 0; cam < J.n_cams; ++cam) {
+    const int nk = F.n[(size_t)J.feat * F.C + cam];
+    const size_t base = ((size_t)J.feat * F.C + cam) * F.N;
+    CamIntr ci;
+    cam_load(W.cams[cam], ci);
+    for (int k0 = 0; k0 < nk; k0 += RS_T) {
+      const int k = k0 + tid;
+      int take = 0, l = -1;
+      if (k < nk) {
+        l = F.lm[base + k];
+        if (track_live(W, L, l) && J.cnt[l] >= 2 && fabs(W.m_lm[4 * (size_t)l + 3]) >= 1.0e-8) take = 1;
+      }
+      int total;
+      const int pos = block_scan<RS_T>(take, s_warp, &total);
+      if (take) {
+        double* cd = J.cd + (size_t)(n + pos) * RS_CD;
+        const double* hp = W.m_lm + 4 * (size_t)l;
+        for (int r = 0; r < 3; ++r) cd[r] = hp[r] / hp[3];
+        // PinholeCamera::backProject (its return value ignored), then bearing.normalize()
+        double pu[2];
+        undistort_gn(ci, (F.kp[2 * (base + k)] - ci.cu) * (1.0 / ci.fu), (F.kp[2 * (base + k) + 1] - ci.cv) * (1.0 / ci.fv), pu);
+        double br[3] = {pu[0], pu[1], 1.0};
+        const double n2 = rs_dot(br, br);
+        if (n2 > 0.0) { const double in = sqrt(n2); br[0] /= in; br[1] /= in; br[2] /= in; }
+        for (int r = 0; r < 3; ++r) cd[3 + r] = br[r];
+        for (int r = 0; r < 3; ++r) cd[6 + r] = s_ext[cam][3 * r] * br[0] + s_ext[cam][3 * r + 1] * br[1] + s_ext[cam][3 * r + 2] * br[2];
+        const double sd = 0.8 * F.size[base + k] / 12.0;
+        cd[9] = sqrt(2.0) * sd * sd / (ci.fu * ci.fu);
+        int* cr = J.ci + 3 * (size_t)(n + pos);
+        cr[0] = cam; cr[1] = k; cr[2] = l;
+      }
+      n += total;
+    }
+  }
+  res.n_correspondences = n;
+  if (n < 5) {                                      // Frontend.cpp:593-596
+    res.ret = n;
+    if (tid == 0) *J.res = res;
+    for (int h = tid; h < J.n_hyp; h += RS_T) J.hyp[h] = 0;
+    return;
+  }
+  __syncthreads();                                  // the correspondences are in global scratch
+  // hypotheses, a thread each
+  if (tid < J.n_hyp) {
+    int idx[4];
+    int ok = 0;
+    if (rs_sample(J.seed, tid, n, idx)) {
+      const double* q[4];
+      bool finite = true;
+      for (int i = 0; i < 4; ++i) {
+        q[i] = J.cd + (size_t)idx[i] * RS_CD;
+        finite = finite && isfinite(q[i][3] + q[i][4] + q[i][5]);
+      }
+      if (finite) {
+        double c[3][3], f[3][3], X[3][3];
+        for (int i = 0; i < 3; ++i) {
+          const int cam = J.ci[3 * (size_t)idx[i]];
+          for (int k = 0; k < 3; ++k) { c[i][k] = s_ext[cam][9 + k]; f[i][k] = q[i][6 + k]; X[i][k] = q[i][k]; }
+        }
+        const double* ext4 = s_ext[J.ci[3 * (size_t)idx[3]]];
+        double best = INFINITY;
+        rs_gp3p(c, f, X, [&](const double* R, const double* t) {
+          const double sc = rs_score(R, t, q[3], ext4);
+          if (sc < best) {
+            best = sc;
+            for (int k = 0; k < 9; ++k) s_model[tid][k] = R[k];
+            for (int k = 0; k < 3; ++k) s_model[tid][9 + k] = t[k];
+          }
+        });
+        ok = best < INFINITY ? 1 : 0;
+      }
+    }
+    s_ok[tid] = ok;
+  }
+  __syncthreads();
+  // inliers of every hypothesis, a warp each
+  const int lane = tid & 31, warp = tid >> 5;
+  for (int h = warp; h < J.n_hyp; h += RS_T / 32) {
+    int cnt = 0;
+    if (s_ok[h])
+      for (int k = lane; k < n; k += 32) {
+        const double* cd = J.cd + (size_t)k * RS_CD;
+        cnt += rs_score(s_model[h], s_model[h] + 9, cd, s_ext[J.ci[3 * (size_t)k]]) < J.threshold ? 1 : 0;
+      }
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    if (lane == 0) s_cnt[h] = cnt;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int best = -1, bc = -1;
+    for (int h = 0; h < J.n_hyp; ++h) {
+      J.hyp[h] = s_cnt[h];
+      if (s_ok[h] && s_cnt[h] > bc) { best = h; bc = s_cnt[h]; }
+    }
+    s_best = best;
+  }
+  __syncthreads();
+  const int best = s_best;
+  res.best = best;
+  res.n_inliers = best >= 0 ? s_cnt[best] : 0;
+  res.ret = res.n_inliers;
+  if (best >= 0) {
+    const double* M = s_model[best];
+    double q[4];
+    // Eigen's Quaternion(Matrix3d)
+    const double tr = M[0] + M[4] + M[8];
+    if (tr > 0.0) {
+      double s = sqrt(tr + 1.0);
+      q[3] = 0.5 * s; s = 0.5 / s;
+      q[0] = (M[7] - M[5]) * s; q[1] = (M[2] - M[6]) * s; q[2] = (M[3] - M[1]) * s;
+    } else {
+      int i = 0;
+      if (M[4] > M[0]) i = 1;
+      if (M[8] > M[4 * i]) i = 2;
+      const int j = (i + 1) % 3, k = (j + 1) % 3;
+      double s = sqrt(M[4 * i] - M[4 * j] - M[4 * k] + 1.0);
+      q[i] = 0.5 * s; s = 0.5 / s;
+      q[3] = (M[3 * k + j] - M[3 * j + k]) * s;
+      q[j] = (M[3 * j + i] + M[3 * i + j]) * s;
+      q[k] = (M[3 * k + i] + M[3 * i + k]) * s;
+    }
+    for (int r = 0; r < 3; ++r) res.T_WS[r] = M[9 + r];
+    for (int r = 0; r < 4; ++r) res.T_WS[3 + r] = q[r];
+  }
+  // Frontend.cpp:613-640: with at least 10 inliers, every other correspondence is removed
+  int n_out = 0;
+  if (res.n_inliers >= 10) {
+    const double* M = s_model[best];
+    for (int k0 = 0; k0 < n; k0 += RS_T) {
+      const int k = k0 + tid;
+      int o = 0;
+      if (k < n) o = rs_score(M, M + 9, J.cd + (size_t)k * RS_CD, s_ext[J.ci[3 * (size_t)k]]) < J.threshold ? 0 : 1;
+      int total;
+      const int pos = block_scan<RS_T>(o, s_warp, &total);
+      if (o) {
+        const int* cr = J.ci + 3 * (size_t)k;
+        J.outl[n_out + pos] = okb_ransac_outlier{cr[0], cr[1], cr[2]};
+      }
+      n_out += total;
+    }
+  }
+  res.n_outliers = n_out;
+  if (tid == 0) *J.res = res;
+}
+}  // namespace
+
+// Host checks of one job; "" = valid.
+static std::string ransac_job_invalid(okb_ctx* c, const okb_ransac_job& j, std::vector<char>& seen) {
+  const std::string why = store_window_invalid(c, j.win, seen);
+  if (!why.empty()) return why;
+  const WinStore& S = c->wins[j.win];
+  const WinDev& W = c->host[j.win];
+  const FeatStore& F = S.feat;
+  if (j.feat_slot < 0 || j.feat_slot >= F.F) return "feat_slot out of range";
+  if (j.n_cams < 1 || j.n_cams > F.C || j.n_cams > W.NE || j.n_cams > W.NC || j.n_cams > RS_MAX_CAMS)
+    return "n_cams out of range (1..the store's cameras, the window's extrinsics and cameras, 16)";
+  size_t n_kp = 0;
+  for (int cam = 0; cam < j.n_cams; ++cam) {
+    const int nk = S.feat_n_pending[(size_t)j.feat_slot * F.C + cam];
+    if (nk < 0) return "feature slot has no keypoints for camera " + std::to_string(cam);
+    n_kp += nk;
+  }
+  if (j.max_iterations < 1 || j.max_iterations > RS_MAX_HYP) return "max_iterations out of range (1..64)";
+  if (!(j.threshold > 0.0) || !std::isfinite(j.threshold)) return "threshold not finite and positive";
+  if (!j.out) return "out missing";
+  if ((size_t)std::max(j.outlier_cap, 0) < n_kp || (n_kp && !j.outliers)) return "outlier capacity below the frame's keypoints";
+  return "";
+}
+
+extern "C" int okb_ransac_3d2d_batch(okb_ctx* c, int n_jobs, const okb_ransac_job* jobs) {
+  int rc = store_call_checks(c, "okb_ransac_3d2d_batch", n_jobs, jobs, INT_MAX,
+                             [&](int i, std::vector<char>& seen) { return ransac_job_invalid(c, jobs[i], seen); });
+  if (rc || n_jobs == 0) return rc;
+  cudaSetDevice(c->device);
+  okb_frontend_state* F = fe(c);
+  CallBuffers& B = F->ransac;
+  std::lock_guard<std::mutex> lk(B.mtx);
+  if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
+  cudaStream_t xs = c->stream_xfer;
+  // staging (pinned + device mirror): in  = [job table]
+  //                                   out = [per job: result | hypothesis inliers | outlier records]
+  // scratch (device only), per job: observation counts | correspondences | their indices
+  Carve st, sc;
+  st.take(sizeof(RansacJobDev) * (size_t)n_jobs, 256);
+  const size_t in_bytes = st.off;
+  std::vector<size_t> o_res(n_jobs), o_hyp(n_jobs), o_out(n_jobs), o_cnt(n_jobs), o_cd(n_jobs), o_ci(n_jobs);
+  std::vector<int> n_kp(n_jobs, 0);
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_ransac_job& j = jobs[i];
+    const WinStore& S = c->wins[j.win];
+    for (int cam = 0; cam < j.n_cams; ++cam) n_kp[i] += S.feat_n_pending[(size_t)j.feat_slot * S.feat.C + cam];
+    o_res[i] = st.take(sizeof(okb_ransac_result));
+    o_hyp[i] = st.take(4 * (size_t)j.max_iterations);
+    o_out[i] = st.take(sizeof(okb_ransac_outlier) * (size_t)n_kp[i]);
+    o_cnt[i] = sc.take(4 * (size_t)std::max(c->host[j.win].L, 1));
+    o_cd[i] = sc.take(8 * RS_CD * (size_t)n_kp[i]);
+    o_ci[i] = sc.take(12 * (size_t)n_kp[i]);
+  }
+  const size_t out_end = st.off;
+  if ((rc = B.reserve(c, out_end, sc.off))) return rc;
+  uint8_t* h = B.h_stage;
+  uint8_t* d = B.d_stage;
+  RansacJobDev* tj = reinterpret_cast<RansacJobDev*>(h);
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_ransac_job& j = jobs[i];
+    RansacJobDev J;
+    std::memset(&J, 0, sizeof J);
+    J.W = c->d_wins + j.win;
+    J.feat = j.feat_slot; J.n_cams = j.n_cams; J.n_hyp = j.max_iterations;
+    J.cnt_cap = std::max(c->host[j.win].L, 1);
+    J.threshold = j.threshold;
+    J.seed = (unsigned long long)j.seed;
+    J.cnt = reinterpret_cast<int*>(B.d_scratch + o_cnt[i]);
+    J.cd = reinterpret_cast<double*>(B.d_scratch + o_cd[i]);
+    J.ci = reinterpret_cast<int*>(B.d_scratch + o_ci[i]);
+    J.res = reinterpret_cast<okb_ransac_result*>(d + o_res[i]);
+    J.hyp = reinterpret_cast<int*>(d + o_hyp[i]);
+    J.outl = reinterpret_cast<okb_ransac_outlier*>(d + o_out[i]);
+    tj[i] = J;
+  }
+  OKB_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
+  k_ransac_3d2d<<<n_jobs, RS_T, 0, xs>>>(reinterpret_cast<const RansacJobDev*>(d));
+  F->launches += 1;
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
+  OKB_CUDA(c, cudaStreamSynchronize(xs));
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_ransac_job& j = jobs[i];
+    *j.out = *reinterpret_cast<const okb_ransac_result*>(h + o_res[i]);
+    if (j.hyp_inliers) std::memcpy(j.hyp_inliers, h + o_hyp[i], 4 * (size_t)j.max_iterations);
+    if (j.out->n_outliers) std::memcpy(j.outliers, h + o_out[i], sizeof(okb_ransac_outlier) * (size_t)j.out->n_outliers);
   }
   return OKB_OK;
 }
