@@ -40,6 +40,8 @@
  *                                correspondences, FrameAbsolutePoseSacProblem's score; own sampler and generalised P3P
  *   okb_detect_describe       <- okvis::Frontend::detectAndDescribe    okvis_frontend/src/Frontend.cpp:92-114
  *                                (Frame::detect / Frame::describe      okvis_cv/include/okvis/implementation/Frame.hpp:109-156)
+ *   okb_detect_describe_store_batch <- the same for every camera of many sessions' frames, written straight into the
+ *                                windows' feature stores
  */
 #ifndef OKVIS_B200_H_
 #define OKVIS_B200_H_
@@ -645,6 +647,12 @@ int okb_window_reserve_features(okb_ctx* ctx, int win, int max_feature_frames, i
  * landmark slots (NULL: all -1) and observed bits (NULL: all 0). */
 int okb_window_set_features(okb_ctx* ctx, int win, int feat_slot, int cam, int n, const okb_keypoint* kp,
                             const uint8_t* desc, const int32_t* lm_slot, const uint8_t* observed);
+/* Diagnostic read-back of the committed store entry (feat_slot, cam), after the work queued on the window's store:
+ * *n = its keypoint count (-1: none); then, for the first *n keypoints and for each pointer that is not NULL, the
+ * keypoints kp [n][2] and sizes size [n] as the store holds them (double), desc [n][desc_bytes], lm_slot [n] and
+ * observed [n].  Size the arrays for the store's max_keypoints.  Pending edits are not committed and not seen. */
+int okb_debug_features(okb_ctx* ctx, int win, int feat_slot, int cam, int32_t* n, double* kp, double* size, uint8_t* desc,
+                       int32_t* lm_slot, uint8_t* observed);
 /* Sets the landmark slot and observed bit of keypoints kp_idx[n] of (feat_slot, cam) -- the host-side changes of 2D-2D /
  * stereo initialisation and RANSAC removals. */
 int okb_window_set_feature_landmarks(okb_ctx* ctx, int win, int feat_slot, int cam, int n, const int32_t* kp_idx,
@@ -845,6 +853,37 @@ typedef struct okb_ransac_job {
  * store: the caller applies the removals.  Results per job are bit-identical to calling it alone.  n_jobs == 0 is a
  * no-op. */
 int okb_ransac_3d2d_batch(okb_ctx* ctx, int n_jobs, const okb_ransac_job* jobs);
+
+/* ---- detection straight into the feature store (Frontend::detectAndDescribe, Frontend.cpp:92-114, for every camera of
+ * a frame whose features the window's store is to hold) ---------------------------------------------------------------
+ * One session's frame: images[c] is detected, described and written into camera c of feature slot feat_slot of window
+ * win, for c < n_cams (other cameras of the slot are left as they are). */
+typedef struct okb_detect_store_job {
+  int32_t win, feat_slot, n_cams, _pad;
+  const okb_image_desc* images;    /* [n_cams], as okb_detect_describe_batch */
+  okb_keypoint* out_kp;            /* [n_cams][max_out] */
+  uint8_t* out_desc;               /* [n_cams][max_out][desc_bytes], or NULL */
+  int32_t* n_out;                  /* [n_cams] */
+} okb_detect_store_job;
+/* Per image, n_out / out_kp / out_desc are bit-identical to what okb_detect_describe_batch returns for it with the
+ * same parameters, and the store entry (win, feat_slot, camera) then holds what okb_window_set_features(win, feat_slot,
+ * camera, n, kp, desc, NULL, NULL) followed by a commit leaves there: x, y and size widened to double, the descriptors,
+ * landmark slot -1 and observed 0 for every keypoint, n keypoints.  The host's keypoint counts follow, so later store
+ * edits (okb_window_set_feature_landmarks, okb_window_clear_features) apply to the new features.  An image with more NMS
+ * candidates than the detector holds gets n_out = -1 and keeps its store entry; every other image is written and the
+ * call returns OKB_ERR_CAPACITY.
+ * Every job is checked on the host before any device work (uploaded window, store reserved, feat_slot in range, n_cams
+ * in 1..the store's cameras, params->desc_bytes = the store's descriptor length, the store's keypoints per image >=
+ * min(max_keypoints, max_out), out_kp and n_out present, each image as okb_detect_describe_batch checks it, at most
+ * 65535 images in all, a window listed twice): the first failure returns OKB_ERR_INVALID_ARG and names the job in
+ * okb_last_error.  A landmark-sharded context returns OKB_ERR_UNSUPPORTED; n_jobs == 0 is a no-op.
+ * Pending edits of the job windows are committed first, and the store writes are ordered after that commit and after
+ * the solver work already launched on those windows: a clear of the slot queued before the call does not erase the new
+ * features, one queued after it does.  The detection runs as okb_detect_describe_batch over all images of the call (its
+ * stream, buffers and serialisation), plus one launch that writes the store; the D2H copy carries the counts and
+ * keypoints, and the descriptors only when a job asks for them.  Returns when the store holds the features. */
+int okb_detect_describe_store_batch(okb_ctx* ctx, int n_jobs, const okb_detect_store_job* jobs, const okb_detect_params* params,
+                                    int max_out, int host_threads);
 
 #ifdef __cplusplus
 }

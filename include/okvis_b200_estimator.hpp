@@ -513,13 +513,7 @@ class Estimator {
     if (descriptors.size() != n * (size_t)cap_.descriptorBytes || landmarkIds.size() != n)
       throw std::invalid_argument("okvis_b200: setFrameFeatures: descriptor / landmark id count mismatch");
     ensureResident();
-    auto fs = featSlot_.find(frameId);
-    if (fs == featSlot_.end()) {
-      if (freeFeat_.empty()) throw std::runtime_error("okvis_b200: no free feature slot (Capacity::frames)");
-      fs = featSlot_.emplace(frameId, *freeFeat_.begin()).first;
-      freeFeat_.erase(freeFeat_.begin());
-      feats_[frameId].resize(cameras_.size());
-    }
+    auto fs = takeFeatureSlot(frameId);
     std::vector<int32_t> slots(n, -1);
     std::vector<uint8_t> observed(n, 0);
     for (size_t k = 0; k < n; ++k) {
@@ -700,6 +694,17 @@ class Estimator {
     const uint8_t o = observed ? 1 : 0;
     check(okb_window_set_feature_landmarks(ctx_, slot_, featSlot_.at(frameId), (int)cam, 1, &k, &l, &o));
     f->second[cam].lm[kp] = landmarkId;
+  }
+  // the frame's feature slot, taken from the free ones when the frame has none yet
+  std::map<uint64_t, int32_t>::iterator takeFeatureSlot(uint64_t frameId) {
+    auto fs = featSlot_.find(frameId);
+    if (fs == featSlot_.end()) {
+      if (freeFeat_.empty()) throw std::runtime_error("okvis_b200: no free feature slot (Capacity::frames)");
+      fs = featSlot_.emplace(frameId, *freeFeat_.begin()).first;
+      freeFeat_.erase(freeFeat_.begin());
+      feats_[frameId].resize(cameras_.size());
+    }
+    return fs;
   }
   void releaseFeatures(uint64_t frameId) {
     auto fs = featSlot_.find(frameId);
@@ -928,6 +933,56 @@ class Estimator {
       setFrameLandmarkId(p.frameId, (size_t)o.cam, (size_t)o.kp, 0);
     }
     return p.result.ret;
+  }
+
+  // One okb_detect_describe_store_batch job of this session's frame: images[c] for camera c, detected with `prm` into the
+  // frame's feature slot.  checkDetectStore throws what planDetectStore would, without touching anything;
+  // planDetectStore takes (or reuses) the frame's feature slot as setFrameFeatures does; finishDetectStore records the
+  // host keypoints with every landmark id 0 (the store holds slot -1, observed 0 for them).
+  struct DetectStorePlan {
+    uint64_t frameId = 0;
+    int maxOut = 0;
+    std::vector<okb_image_desc> images;
+    std::vector<okb_keypoint> kp;         // [camera][maxOut]
+    std::vector<int32_t> n;
+    okb_detect_store_job job{};
+  };
+  void checkDetectStore(uint64_t frameId, size_t nImages, const okb_detect_params& prm) const {
+    if (cap_.featureKeypoints <= 0) throw std::runtime_error("okvis_b200: detectAndDescribe into the store needs Capacity::featureKeypoints > 0");
+    if (!states_.count(frameId))
+      throw std::runtime_error("okvis_b200: detectAndDescribe: frame " + std::to_string(frameId) + " is not in the window (call addStates first)");
+    if (cap_.featureKeypoints < prm.max_keypoints)
+      throw std::invalid_argument("okvis_b200: detectAndDescribe: Capacity::featureKeypoints is below the detector's maximum keypoints");
+    if (prm.desc_bytes != cap_.descriptorBytes)
+      throw std::invalid_argument("okvis_b200: detectAndDescribe: the descriptor length differs from Capacity::descriptorBytes");
+    if (nImages != cameras_.size()) throw std::invalid_argument("okvis_b200: detectAndDescribe: one image per camera");
+  }
+  void planDetectStore(uint64_t frameId, const std::vector<okb_image_desc>& images, const okb_detect_params& prm, DetectStorePlan& p) {
+    checkDetectStore(frameId, images.size(), prm);
+    ensureResident();
+    auto fs = takeFeatureSlot(frameId);
+    const size_t C = cameras_.size();
+    p.frameId = frameId;
+    p.maxOut = prm.max_keypoints;
+    p.images = images;
+    p.kp.assign(C * (size_t)p.maxOut, okb_keypoint{});
+    p.n.assign(C, 0);
+    p.job = okb_detect_store_job{};
+    p.job.win = slot_; p.job.feat_slot = fs->second; p.job.n_cams = (int32_t)C;
+    p.job.images = p.images.data(); p.job.out_kp = p.kp.data(); p.job.out_desc = nullptr; p.job.n_out = p.n.data();
+  }
+  // Returns the keypoints per camera; a camera over the detector's candidate capacity (n = -1) keeps its features.
+  std::vector<std::vector<okb_keypoint>> finishDetectStore(const DetectStorePlan& p) {
+    std::vector<std::vector<okb_keypoint>> out(cameras_.size());
+    for (size_t c = 0; c < cameras_.size(); ++c) {
+      if (p.n[c] < 0) continue;
+      const okb_keypoint* k = p.kp.data() + c * (size_t)p.maxOut;
+      out[c].assign(k, k + p.n[c]);
+      FrameFeatures& f = feats_.at(p.frameId)[c];
+      f.kp = out[c];
+      f.lm.assign(out[c].size(), 0);
+    }
+    return out;
   }
 
   void eraseObsHost(std::map<uint64_t, Obs>::iterator it) {

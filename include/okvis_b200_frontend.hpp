@@ -25,7 +25,10 @@
 // own sampler and generalised P3P, the reference's score and decision) and applies them through
 // Estimator::removeObservation and Estimator::setFrameLandmarkId; with RansacHooks::device3d2d set,
 // dataAssociationAndInitialization runs it at both of the reference's call points.  runRansac2d2d (on OpenGV) stays
-// with the adaptor, in RansacHooks.
+// with the adaptor, in RansacHooks.  Frontend::detectAndDescribe(estimator, frameId, images) detects every camera of a
+// frame straight into the frame's feature slot of the estimator's store (okb_detect_describe_store_batch: one device
+// call, the descriptors stay on the device), in place of the single-image detectAndDescribe + setFrameFeatures; its
+// EstimatorGroup form makes one call for many sessions.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -76,18 +79,9 @@ class Frontend {
   int detectAndDescribe(size_t cameraIndex, const uint8_t* image, int width, int height, int stride, const okb_camera& geometry,
                         const double T_WC[7], std::vector<okb_keypoint>& keypoints, std::vector<uint8_t>& descriptors) {
     if (cameraIndex >= numCameras_) throw std::runtime_error("okvis_b200: camera index out of range");
-    // R_CW = C_WC^T from the quaternion of T_WC
-    const double x = T_WC[3], y = T_WC[4], z = T_WC[5], w = T_WC[6];
-    const double C[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                         2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                         2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
-    const double R_CW[9] = {C[0], C[3], C[6], C[1], C[4], C[7], C[2], C[5], C[8]};
-    okb_detect_params p{};
-    p.uniformity_radius = briskDetectionThreshold_;          // the "detection threshold" of the yaml is brisk's uniformity radius (Frontend.cpp:828-831)
-    p.absolute_threshold = briskDetectionAbsoluteThreshold_;
-    p.max_keypoints = (int32_t)briskDetectionMaximumKeypoints_;
-    p.desc_bytes = descriptorBytes_;
-    p.rotation_invariance = briskDescriptionRotationInvariance_ ? 1 : 0;
+    double R_CW[9];
+    rotationCW(T_WC, R_CW);
+    const okb_detect_params p = detectParams();
     keypoints.resize(briskDetectionMaximumKeypoints_);
     descriptors.resize(briskDetectionMaximumKeypoints_ * (size_t)descriptorBytes_);
     int n = 0;
@@ -98,6 +92,30 @@ class Frontend {
     descriptors.resize((size_t)n * descriptorBytes_);
     isInitialized_ = true;
     return n;
+  }
+
+  // One camera's image of a frame, as the reference's detectAndDescribe(cameraIndex, frame, T_WC, ...) receives it: the
+  // pixels (row stride `stride` bytes) and the camera's pose T_WC [t, q_xyzw].
+  struct CameraImage {
+    const uint8_t* image = nullptr;
+    int width = 0, height = 0, stride = 0;
+    Pose7 T_WC{};
+  };
+  // detectAndDescribe for every camera of a frame, straight into the frame's feature slot of the estimator's window
+  // (okb_detect_describe_store_batch: one device call, the descriptors never leave the device).  images[c] is camera c
+  // of the estimator, whose geometry is used.  The frame must be in the window (addStates first), and the estimator's
+  // Capacity must hold this Frontend's maximum keypoints and descriptor length.  The frame's features then stand as
+  // after Estimator::setFrameFeatures with every landmark id 0.  Returns the keypoints per camera, equal to the
+  // single-image detectAndDescribe's.
+  std::vector<std::vector<okb_keypoint>> detectAndDescribe(Estimator& estimator, uint64_t frameId, const std::vector<CameraImage>& images) {
+    return detectStoreGroup(nullptr, {&estimator}, {frameId}, {images})[0];
+  }
+  // The same for sessions of one EstimatorGroup (any order, each listed once): one okb_detect_describe_store_batch for
+  // all of them; results[i] equals the single form's on sessions[i].
+  std::vector<std::vector<std::vector<okb_keypoint>>> detectAndDescribe(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
+                                                                        const std::vector<uint64_t>& frameIds,
+                                                                        const std::vector<std::vector<CameraImage>>& images) {
+    return detectStoreGroup(&group, sessions, frameIds, images);
   }
 
   // Frontend::propagation (Frontend.cpp:274-292): ImuError::propagation on the device; covariance / jacobian 15x15 or null.
@@ -511,6 +529,58 @@ class Frontend {
       sessions[i]->nameRemainingKeypoints(frameIds[i], newIds[i]);
       for (size_t c = 0; c < C; ++c) out[i].landmarkIds.push_back(sessions[i]->frameLandmarkIds(frameIds[i], c));
     }
+    return out;
+  }
+
+  // R_CW = C_WC^T from the quaternion of T_WC
+  static void rotationCW(const double T_WC[7], double R_CW[9]) {
+    const double x = T_WC[3], y = T_WC[4], z = T_WC[5], w = T_WC[6];
+    const double C[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                         2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                         2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
+    const double R[9] = {C[0], C[3], C[6], C[1], C[4], C[7], C[2], C[5], C[8]};
+    for (int k = 0; k < 9; ++k) R_CW[k] = R[k];
+  }
+  okb_detect_params detectParams() const {
+    okb_detect_params p{};
+    p.uniformity_radius = briskDetectionThreshold_;          // the "detection threshold" of the yaml is brisk's uniformity radius (Frontend.cpp:828-831)
+    p.absolute_threshold = briskDetectionAbsoluteThreshold_;
+    p.max_keypoints = (int32_t)briskDetectionMaximumKeypoints_;
+    p.desc_bytes = descriptorBytes_;
+    p.rotation_invariance = briskDescriptionRotationInvariance_ ? 1 : 0;
+    return p;
+  }
+
+  std::vector<std::vector<std::vector<okb_keypoint>>> detectStoreGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions,
+                                                                       const std::vector<uint64_t>& frameIds,
+                                                                       const std::vector<std::vector<CameraImage>>& images) {
+    const size_t n = sessions.size();
+    if (frameIds.size() != n || images.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one image list per session");
+    if (group) group->validate(sessions);
+    const okb_detect_params prm = detectParams();
+    for (size_t i = 0; i < n; ++i) sessions[i]->checkDetectStore(frameIds[i], images[i].size(), prm);   // before any device work
+    std::vector<Estimator::DetectStorePlan> plans(n);
+    std::vector<okb_detect_store_job> jobs(n);
+    for (size_t i = 0; i < n; ++i) {
+      Estimator& e = *sessions[i];
+      std::vector<okb_image_desc> ims(images[i].size());
+      for (size_t c = 0; c < ims.size(); ++c) {
+        const CameraImage& im = images[i][c];
+        ims[c].img = im.image; ims[c].width = im.width; ims[c].height = im.height; ims[c].stride = im.stride;
+        ims[c].cam = e.cameras_[c];
+        rotationCW(im.T_WC.data(), ims[c].R_CW);
+      }
+      e.planDetectStore(frameIds[i], ims, prm, plans[i]);
+      jobs[i] = plans[i].job;
+    }
+    std::vector<std::vector<std::vector<okb_keypoint>>> out(n);
+    if (n == 0) return out;
+    okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
+    const int rc = okb_detect_describe_store_batch(ctx, (int)n, jobs.data(), &prm, prm.max_keypoints, 0);
+    if (rc != OKB_OK && rc != OKB_ERR_CAPACITY) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+    for (size_t i = 0; i < n; ++i) out[i] = sessions[i]->finishDetectStore(plans[i]);   // the store and the host agree, also on capacity
+    if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+    isInitialized_ = true;
     return out;
   }
 

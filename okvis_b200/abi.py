@@ -164,6 +164,11 @@ class RansacJob(C.Structure):
                 ("outliers", C.c_void_p), ("outlier_cap", C.c_int32), ("_pad", C.c_int32), ("out", C.POINTER(RansacResult))]
 
 
+class DetectStoreJob(C.Structure):
+    _fields_ = [("win", C.c_int32), ("feat_slot", C.c_int32), ("n_cams", C.c_int32), ("_pad", C.c_int32),
+                ("images", C.POINTER(ImageDesc)), ("out_kp", C.c_void_p), ("out_desc", C.c_void_p), ("n_out", C.POINTER(C.c_int32))]
+
+
 class PropagateJob(C.Structure):
     _fields_ = [("params", C.POINTER(ImuParams)), ("samples", C.c_void_p), ("n_samples", C.c_int32), ("_pad", C.c_int32),
                 ("t0_ns", C.c_int64), ("t1_ns", C.c_int64), ("pose", c_double_p), ("speed_bias", c_double_p),

@@ -497,16 +497,17 @@ class Context:
                                               C.byref(prm), _p(kps), _p(desc), max_keypoints, C.byref(n)))
         return kps[:n.value].copy(), desc[:n.value].copy()
 
-    def detect_describe_batch(self, imgs, cams, R_CWs, uniformity_radius=40.0, absolute_threshold=800.0, max_keypoints=400,
-                              desc_bytes=48, rotation_invariance=True, host_threads=0, return_status=False):
-        """okb_detect_describe_batch: one (keypoints, descriptors) per image, each equal to detect_describe on it.
-        `imgs` are 2-D uint8 arrays (rows may be strided).  With return_status the call returns (results, status) instead
-        of raising OKB_ERR_CAPACITY; an image over the candidate capacity then gives None."""
-        n = len(imgs)
+    @staticmethod
+    def _detect_params(uniformity_radius, absolute_threshold, max_keypoints, desc_bytes, rotation_invariance):
         prm = abi.DetectParams()
         prm.uniformity_radius, prm.absolute_threshold = uniformity_radius, absolute_threshold
         prm.max_keypoints, prm.desc_bytes, prm.rotation_invariance = max_keypoints, desc_bytes, int(rotation_invariance)
-        descs = (abi.ImageDesc * max(n, 1))()
+        return prm
+
+    @staticmethod
+    def _image_descs(imgs, cams, R_CWs):
+        """okb_image_desc array over 2-D uint8 images (rows may be strided) and the arrays it points into."""
+        descs = (abi.ImageDesc * max(len(imgs), 1))()
         keep = []
         for i, (img, cam, R) in enumerate(zip(imgs, cams, R_CWs)):
             img = np.asarray(img, dtype=np.uint8)
@@ -520,6 +521,16 @@ class Context:
             C.memmove(C.addressof(d.cam), np.array([cam], abi.camera_dtype).ctypes.data, C.sizeof(abi.Camera))
             for k, v in enumerate(np.asarray(R, dtype=np.float64).reshape(9)):
                 d.R_CW[k] = float(v)
+        return descs, keep
+
+    def detect_describe_batch(self, imgs, cams, R_CWs, uniformity_radius=40.0, absolute_threshold=800.0, max_keypoints=400,
+                              desc_bytes=48, rotation_invariance=True, host_threads=0, return_status=False):
+        """okb_detect_describe_batch: one (keypoints, descriptors) per image, each equal to detect_describe on it.
+        `imgs` are 2-D uint8 arrays (rows may be strided).  With return_status the call returns (results, status) instead
+        of raising OKB_ERR_CAPACITY; an image over the candidate capacity then gives None."""
+        n = len(imgs)
+        prm = self._detect_params(uniformity_radius, absolute_threshold, max_keypoints, desc_bytes, rotation_invariance)
+        descs, keep = self._image_descs(imgs, cams, R_CWs)
         kps = np.zeros((n, max_keypoints), abi.keypoint_dtype)
         desc = np.zeros((n, max_keypoints, desc_bytes), np.uint8)
         n_out = np.zeros(n, np.int32)
@@ -529,6 +540,48 @@ class Context:
             self._check(rc)
         out = [(kps[i, :m].copy(), desc[i, :m].copy()) if m >= 0 else None for i, m in enumerate(n_out.tolist())]
         return (out, rc) if return_status else out
+
+    def detect_describe_store_batch(self, jobs, uniformity_radius=40.0, absolute_threshold=800.0, max_keypoints=400,
+                                    desc_bytes=48, rotation_invariance=True, host_threads=0, return_status=False, max_out=None):
+        """okb_detect_describe_store_batch.  jobs: dicts with win, feat_slot, imgs, cams, R_CWs (one image per camera, as
+        detect_describe_batch takes them) and optionally want_desc (True).  Returns one list per job of (keypoints,
+        descriptors or None) per camera, each equal to detect_describe_batch on that image; the images' features are then
+        in the store entries (win, feat_slot, camera).  return_status as detect_describe_batch."""
+        max_out = max_keypoints if max_out is None else int(max_out)
+        prm = self._detect_params(uniformity_radius, absolute_threshold, max_keypoints, desc_bytes, rotation_invariance)
+        arr = (abi.DetectStoreJob * max(len(jobs), 1))()
+        outs, keep = [], []
+        for i, j in enumerate(jobs):
+            n = len(j["imgs"])
+            descs, k = self._image_descs(j["imgs"], j["cams"], j["R_CWs"])
+            o = dict(kp=np.zeros((max(n, 1), max_out), abi.keypoint_dtype), n=np.zeros(max(n, 1), np.int32),
+                     desc=np.zeros((max(n, 1), max_out, desc_bytes), np.uint8) if j.get("want_desc", True) else None)
+            keep += [descs, k]
+            t = arr[i]
+            t.win, t.feat_slot, t.n_cams = int(j["win"]), int(j["feat_slot"]), n
+            t.images = C.cast(descs, C.POINTER(abi.ImageDesc))
+            t.out_kp, t.out_desc = o["kp"].ctypes.data, o["desc"].ctypes.data if o["desc"] is not None else None
+            t.n_out = o["n"].ctypes.data_as(C.POINTER(C.c_int32))
+            outs.append((o, n))
+        rc = lib().okb_detect_describe_store_batch(self._h, len(jobs), arr, C.byref(prm), max_out, int(host_threads))
+        if rc != 0 and not (return_status and rc == abi.OKB_ERR_CAPACITY):
+            self._check(rc)
+        res = [[(o["kp"][c, :m].copy(), o["desc"][c, :m].copy() if o["desc"] is not None else None) if m >= 0 else None
+                for c, m in enumerate(o["n"][:n].tolist())] for o, n in outs]
+        return (res, rc) if return_status else res
+
+    def debug_features(self, win, feat_slot, cam):
+        """okb_debug_features: the committed store entry (win, feat_slot, cam) as a dict of n, kp [n][2], size, desc,
+        lm_slot and observed (n = -1: no image; the arrays are then empty)."""
+        N, D = self._feat_shape[int(win)]
+        n = C.c_int32(0)
+        kp, size = np.zeros((N, 2)), np.zeros(N)
+        desc, lm, ob = np.zeros((N, D), np.uint8), np.zeros(N, np.int32), np.zeros(N, np.uint8)
+        self._check(lib().okb_debug_features(self._h, int(win), int(feat_slot), int(cam), C.byref(n), _p(kp), _p(size), _p(desc),
+                                             _p(lm), _p(ob)))
+        m = max(n.value, 0)
+        return dict(n=n.value, kp=kp[:m].copy(), size=size[:m].copy(), desc=desc[:m].copy(), lm_slot=lm[:m].copy(),
+                    observed=ob[:m].copy())
 
     @staticmethod
     def make_match_job(A, B, skipA=None, skipB=None, threshold=60.0, num_best=4, use_ratio=False, gate=None, want_topk=True):
@@ -557,6 +610,8 @@ class Context:
                                                       int(max_keypoints), int(desc_bytes)))
         self._feat = getattr(self, "_feat", {})
         self._feat[int(win)] = int(max_keypoints)
+        self._feat_shape = getattr(self, "_feat_shape", {})
+        self._feat_shape[int(win)] = (int(max_keypoints), int(desc_bytes))
 
     def set_features(self, win, feat_slot, cam, kp, desc, lm_slot=None, observed=None):
         """okb_window_set_features: kp is a keypoint_dtype array or an [n][3] array of (x, y, size)."""

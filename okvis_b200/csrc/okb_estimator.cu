@@ -986,6 +986,28 @@ extern "C" int okb_window_set_landmark_initialized(okb_ctx* c, int win, int n, c
   return OKB_OK;
 }
 
+extern "C" int okb_debug_features(okb_ctx* c, int win, int feat_slot, int cam, int32_t* n, double* kp, double* size, uint8_t* desc,
+                                  int32_t* lm_slot, uint8_t* observed) {
+  if (!c || win < 0 || win >= c->max_windows || !n) return OKB_ERR_INVALID_ARG;
+  const WinStore& S = c->wins[win];
+  const FeatStore& F = S.feat;
+  if (!S.feat_mem) { c->set_error("okb_debug_features: no feature store (okb_window_reserve_features)"); return OKB_ERR_INVALID_ARG; }
+  if (feat_slot < 0 || feat_slot >= F.F || cam < 0 || cam >= F.C) { c->set_error("okb_debug_features: feature slot or camera out of range"); return OKB_ERR_INVALID_ARG; }
+  cudaSetDevice(c->device);
+  OKB_CUDA(c, cudaStreamSynchronize(c->stream_xfer));     // commits (and the store calls, which block) run there
+  const size_t img = (size_t)feat_slot * F.C + cam, base = img * F.N;
+  int32_t m = -1;
+  OKB_CUDA(c, cudaMemcpy(&m, F.n + img, sizeof m, cudaMemcpyDeviceToHost));
+  *n = m;
+  if (m <= 0) return OKB_OK;
+  if (kp) OKB_CUDA(c, cudaMemcpy(kp, F.kp + 2 * base, 16 * (size_t)m, cudaMemcpyDeviceToHost));
+  if (size) OKB_CUDA(c, cudaMemcpy(size, F.size + base, 8 * (size_t)m, cudaMemcpyDeviceToHost));
+  if (desc) OKB_CUDA(c, cudaMemcpy(desc, F.desc + base * (F.D / 4), (size_t)m * F.D, cudaMemcpyDeviceToHost));
+  if (lm_slot) OKB_CUDA(c, cudaMemcpy(lm_slot, F.lm + base, 4 * (size_t)m, cudaMemcpyDeviceToHost));
+  if (observed) OKB_CUDA(c, cudaMemcpy(observed, F.observed + base, (size_t)m, cudaMemcpyDeviceToHost));
+  return OKB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // device-side marginalisation (okb_marg.cuh): MarginalizationError::addResidualBlock / marginalizeOut /
 // updateErrorComputation (okvis_ceres/src/MarginalizationError.cpp:127-435, 507-846)

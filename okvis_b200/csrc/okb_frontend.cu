@@ -124,12 +124,32 @@ struct SlotBuffers {
   DetectBuffers buf;
   std::mutex mtx;
 };
+
+// One image's host outputs of a detect launch: [max_out] keypoints, [max_out][desc_bytes] descriptors (nullptr: not
+// wanted) and its count.
+struct DetectOut {
+  okb_keypoint* kp;
+  uint8_t* desc;
+  int32_t* n;
+};
+
+// One image's store entry (okb_detect_describe_store_batch): the device addresses of keypoint 0 of (feat_slot, cam) in
+// each array of the window's FeatStore, and of the entry's count.
+struct StoreDest {
+  double* kp;                   // [N][2]
+  double* size;
+  uint32_t* desc;               // [N][D/4]
+  int32_t* lm;
+  uint8_t* observed;
+  int* n;
+};
 }  // namespace
 
 struct okb_frontend_state {
   SlotBuffers slots[kMaxSlots];
   // batch calls: a stream of their own (never c->stream, so a batch does not queue behind a solve) and their buffers
   cudaStream_t batch_stream = nullptr;
+  cudaEvent_t store_ready = nullptr;  // okb_detect_describe_store_batch: recorded after its commit on c->stream_xfer
   DetectBuffers batch_det;
   CallBuffers batch_match;
   std::mutex batch_mtx;
@@ -160,6 +180,7 @@ void okb_frontend_release(okb_ctx* c) {
   for (CallBuffers* b : {&F->match_io, &F->batch_match, &F->track, &F->stereo, &F->kf, &F->ransac}) b->release();
   F->batch_det.release();
   if (F->batch_stream) cudaStreamDestroy(F->batch_stream);
+  if (F->store_ready) cudaEventDestroy(F->store_ready);
   for (auto& s : F->slots) {
     if (s.stream) cudaStreamDestroy(s.stream);
     s.buf.release();
@@ -768,6 +789,28 @@ __global__ void __launch_bounds__(128) k_describe(const FeImage* __restrict__ ta
     if (lane == 0) out[w] = word;
   }
 }
+
+// CTA per image: its keypoints and descriptors from the launch's output buffer into its store entry, as
+// CMD_SET_FEATURES writes them (okb_graph.cuh): x, y, size widened to double, landmark slot -1, observed 0, the
+// descriptor words, then the count.  An image over the candidate capacity keeps its entry.
+__global__ void __launch_bounds__(256) k_store_features(const StoreDest* __restrict__ dst, const int* __restrict__ count_all, int max_cand,
+                                                        const okb_keypoint* __restrict__ kps_all, int max_kp,
+                                                        const uint8_t* __restrict__ desc_all, int desc_bytes) {
+  const int i = blockIdx.x;
+  if (count_all[4 * i] > max_cand) return;
+  const int n = count_all[4 * i + 1];
+  const StoreDest d = dst[i];
+  const okb_keypoint* kp = kps_all + (size_t)i * max_kp;
+  for (int k = threadIdx.x; k < n; k += blockDim.x) {
+    const okb_keypoint p = kp[k];
+    d.kp[2 * k] = p.x; d.kp[2 * k + 1] = p.y; d.size[k] = p.size;
+    d.lm[k] = -1; d.observed[k] = 0;
+  }
+  const int words = n * (desc_bytes / 4);
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(desc_all + (size_t)i * max_kp * desc_bytes);
+  for (int k = threadIdx.x; k < words; k += blockDim.x) d.desc[k] = src[k];
+  if (threadIdx.x == 0) *d.n = n;
+}
 }  // namespace
 
 // The device pattern of one descriptor length.  Each length gets its own, kept until the context is destroyed, so
@@ -801,18 +844,22 @@ static void host_parallel(int n, int threads, size_t bytes, const Fn& f) {
 }
 
 // Detect and describe n images with one parameter set on stream `st`, into buffers B: one H2D copy (image table and
-// packed images), 7 launches whatever n is, one D2H copy (counts, keypoints, descriptors), one synchronisation.
-// Arguments are checked by the callers; maxk = min(max_keypoints, max_out) >= 1.  n_out[i] = -1 marks an image with
-// more NMS candidates than kMaxCand (OKB_ERR_CAPACITY); the other images' outputs are written all the same.
+// packed images), 7 launches whatever n is, one D2H copy (counts, keypoints, and descriptors when some outs[i].desc is
+// set), one synchronisation.  With `dests`, image i is also written into the store entry dests[i] by one more launch,
+// k_store_features, queued after `store_after` (an event the caller recorded).  Arguments are checked by the callers;
+// maxk = min(max_keypoints, max_out) >= 1.  *outs[i].n = -1 marks an image with more NMS candidates than kMaxCand
+// (OKB_ERR_CAPACITY); the other images' outputs are written all the same.
 static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaStream_t st, int n, const okb_image_desc* ims,
-                      const okb_detect_params* prm, okb_keypoint* out_kp, uint8_t* out_desc, int max_out, int32_t* n_out, int host_threads) {
+                      const okb_detect_params* prm, const DetectOut* outs, int max_out, const StoreDest* dests, cudaEvent_t store_after,
+                      int host_threads) {
   const int maxk = std::min(prm->max_keypoints, max_out), db = prm->desc_bytes;
   DevPattern pat;
   int rc = ensure_pattern(c, F, db, &pat);
   if (rc) return rc;
   std::vector<FeImage> tab(n);
-  Carve in;                     // [FeImage table | packed images], each on a 256-byte boundary
+  Carve in;                     // [FeImage table | StoreDest table (with dests) | packed images], each on a 256-byte boundary
   in.take(sizeof(FeImage) * n, 256);
+  const size_t o_dest = dests ? in.take(sizeof(StoreDest) * n, 256) : 0;
   size_t px = 0, ii = 0, uni = 0;
   int Wmax = 0, Hmax = 0;
   for (int i = 0; i < n; ++i) {
@@ -841,6 +888,7 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
       (rc = grow_pinned(c, &B.h_out, &B.h_out_cap, out_bytes)))
     return rc;
   std::memcpy(B.h_in, tab.data(), sizeof(FeImage) * n);
+  if (dests) std::memcpy(B.h_in + o_dest, dests, sizeof(StoreDest) * n);
   host_parallel(n, host_threads, in_bytes, [&](int i) {
     const okb_image_desc& d = ims[i];
     uint8_t* dst = B.h_in + tab[i].img;
@@ -867,8 +915,15 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
   k_describe<<<dim3((maxk + 3) / 4, n), 128, 0, st>>>(d_tab, B.d_integral, pat.half, pat.pi, pat.pj, pat.lut, db, d_kp, maxk, d_count,
                                                       d_desc);
   F->launches += prm->rotation_invariance ? 8 : 7;
+  if (dests) {
+    OKB_CUDA(c, cudaStreamWaitEvent(st, store_after, 0));
+    k_store_features<<<n, 256, 0, st>>>(reinterpret_cast<const StoreDest*>(B.d_in + o_dest), d_count, kMaxCand, d_kp, maxk, d_desc, db);
+    F->launches += 1;
+  }
   OKB_CUDA(c, cudaGetLastError());
-  OKB_CUDA(c, cudaMemcpyAsync(B.h_out, B.d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  bool want_desc = false;
+  for (int i = 0; i < n && !want_desc; ++i) want_desc = outs[i].desc != nullptr;
+  OKB_CUDA(c, cudaMemcpyAsync(B.h_out, B.d_out, want_desc ? out_bytes : o_desc, cudaMemcpyDeviceToHost, st));
   OKB_CUDA(c, cudaStreamSynchronize(st));
   const int* h_count = reinterpret_cast<const int*>(B.h_out);
   { static const bool dbg = getenv("OKB_FE_DEBUG") != nullptr;
@@ -881,13 +936,14 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
   }
   int status = OKB_OK;
   for (int i = 0; i < n; ++i) {
-    n_out[i] = h_count[4 * i] > kMaxCand ? -1 : h_count[4 * i + 1];
-    if (n_out[i] < 0) status = OKB_ERR_CAPACITY;
+    *outs[i].n = h_count[4 * i] > kMaxCand ? -1 : h_count[4 * i + 1];
+    if (*outs[i].n < 0) status = OKB_ERR_CAPACITY;
   }
-  host_parallel(n, host_threads, out_bytes, [&](int i) {
-    if (n_out[i] <= 0) return;
-    std::memcpy(out_kp + (size_t)i * max_out, B.h_out + o_kp + sizeof(okb_keypoint) * i * maxk, sizeof(okb_keypoint) * n_out[i]);
-    std::memcpy(out_desc + (size_t)i * max_out * db, B.h_out + o_desc + (size_t)i * maxk * db, (size_t)n_out[i] * db);
+  host_parallel(n, host_threads, want_desc ? out_bytes : o_desc, [&](int i) {
+    const int m = *outs[i].n;
+    if (m <= 0) return;
+    std::memcpy(outs[i].kp, B.h_out + o_kp + sizeof(okb_keypoint) * i * maxk, sizeof(okb_keypoint) * m);
+    if (outs[i].desc) std::memcpy(outs[i].desc, B.h_out + o_desc + (size_t)i * maxk * db, (size_t)m * db);
   });
   if (status) c->set_error("too many corner candidates");
   return status;
@@ -896,6 +952,8 @@ static int detect_run(okb_ctx* c, okb_frontend_state* F, DetectBuffers& B, cudaS
 static bool detect_params_ok(const okb_detect_params* prm, int max_out) {
   return (prm->desc_bytes >= 4 && prm->desc_bytes <= 128 && (prm->desc_bytes % 4) == 0) && std::min(prm->max_keypoints, max_out) >= 1;
 }
+
+static bool batch_image_ok(const okb_image_desc& d) { return d.img && d.width >= 64 && d.height >= 64 && d.stride >= d.width; }
 
 extern "C" int okb_detect_describe(okb_ctx* c, int cam_slot, const uint8_t* img, int width, int height, int stride,
                                    const okb_camera* cam, const double R_CW[9], const okb_detect_params* prm,
@@ -914,7 +972,8 @@ extern "C" int okb_detect_describe(okb_ctx* c, int cam_slot, const uint8_t* img,
   d.cam = *cam;
   std::memcpy(d.R_CW, R_CW, sizeof d.R_CW);
   int32_t n = 0;
-  const int rc = detect_run(c, F, S.buf, S.stream, 1, &d, prm, out_kp, out_desc, max_out, &n, 1);
+  const DetectOut out{out_kp, out_desc, &n};
+  const int rc = detect_run(c, F, S.buf, S.stream, 1, &d, prm, &out, max_out, nullptr, nullptr, 1);
   if (rc == OKB_OK) *n_out = n;
   return rc;
 }
@@ -926,15 +985,16 @@ extern "C" int okb_detect_describe_batch(okb_ctx* c, int n_images, const okb_ima
   if (n_images > 65535) return OKB_ERR_INVALID_ARG;           // the image index is a grid dimension
   if (!images || !prm || !out_kp || !out_desc || !n_out) return OKB_ERR_INVALID_ARG;
   if (!detect_params_ok(prm, max_out)) return OKB_ERR_INVALID_ARG;
-  for (int i = 0; i < n_images; ++i) {
-    const okb_image_desc& d = images[i];
-    if (!d.img || d.width < 64 || d.height < 64 || d.stride < d.width) return OKB_ERR_INVALID_ARG;
-  }
+  for (int i = 0; i < n_images; ++i)
+    if (!batch_image_ok(images[i])) return OKB_ERR_INVALID_ARG;
+  std::vector<DetectOut> outs(n_images);
+  for (int i = 0; i < n_images; ++i)
+    outs[i] = DetectOut{out_kp + (size_t)i * max_out, out_desc + (size_t)i * max_out * prm->desc_bytes, n_out + i};
   cudaSetDevice(c->device);
   okb_frontend_state* F = fe(c);
   std::lock_guard<std::mutex> lk(F->batch_mtx);
   if (!F->batch_stream) OKB_CUDA(c, cudaStreamCreateWithFlags(&F->batch_stream, cudaStreamNonBlocking));
-  return detect_run(c, F, F->batch_det, F->batch_stream, n_images, images, prm, out_kp, out_desc, max_out, n_out, host_threads);
+  return detect_run(c, F, F->batch_det, F->batch_stream, n_images, images, prm, outs.data(), max_out, nullptr, nullptr, host_threads);
 }
 
 // =================================================================================================
@@ -3459,4 +3519,72 @@ extern "C" int okb_ransac_3d2d_batch(okb_ctx* c, int n_jobs, const okb_ransac_jo
     if (j.out->n_outliers) std::memcpy(j.outliers, h + o_out[i], sizeof(okb_ransac_outlier) * (size_t)j.out->n_outliers);
   }
   return OKB_OK;
+}
+
+// =================================================================================================
+// detection straight into the feature store (okb_detect_describe_store_batch): detect_run over every image of the call
+// on the batch stream, with one store destination per image; k_store_features waits for the commit of the job windows
+// =================================================================================================
+// Host checks of one job; "" = valid.  *images counts the images of the call so far.
+static std::string detect_store_job_invalid(okb_ctx* c, const okb_detect_store_job& j, const okb_detect_params& prm, int max_out,
+                                            int* images, std::vector<char>& seen) {
+  const std::string why = store_window_invalid(c, j.win, seen);
+  if (!why.empty()) return why;
+  const FeatStore& F = c->wins[j.win].feat;
+  if (j.feat_slot < 0 || j.feat_slot >= F.F) return "feat_slot out of range";
+  if (j.n_cams < 1 || j.n_cams > F.C) return "n_cams out of range (1..the store's cameras)";
+  if (prm.desc_bytes != F.D) return "params->desc_bytes differs from the store's descriptor length";
+  if (F.N < std::min(prm.max_keypoints, max_out)) return "the store holds fewer keypoints per image than min(max_keypoints, max_out)";
+  if (!j.images || !j.out_kp || !j.n_out) return "images / out_kp / n_out missing";
+  for (int cam = 0; cam < j.n_cams; ++cam)
+    if (!batch_image_ok(j.images[cam])) return "images[" + std::to_string(cam) + "]: no pixels, smaller than 64 x 64 or stride < width";
+  if ((*images += j.n_cams) > 65535) return "more than 65535 images in the call";     // the image index is a grid dimension
+  return "";
+}
+
+extern "C" int okb_detect_describe_store_batch(okb_ctx* c, int n_jobs, const okb_detect_store_job* jobs, const okb_detect_params* prm,
+                                               int max_out, int host_threads) {
+  const char* fn = "okb_detect_describe_store_batch";
+  if (c && n_jobs > 0 && (!prm || !detect_params_ok(prm, max_out))) {
+    c->set_error(std::string(fn) + ": params missing, or a descriptor length / min(max_keypoints, max_out) out of range");
+    return OKB_ERR_INVALID_ARG;
+  }
+  int n = 0;
+  int rc = store_call_checks(c, fn, n_jobs, jobs, 65535,
+                             [&](int i, std::vector<char>& seen) { return detect_store_job_invalid(c, jobs[i], *prm, max_out, &n, seen); });
+  if (rc || n_jobs == 0) return rc;
+  const int db = prm->desc_bytes;
+  std::vector<okb_image_desc> ims;
+  std::vector<DetectOut> outs;
+  std::vector<StoreDest> dests;
+  ims.reserve(n); outs.reserve(n); dests.reserve(n);
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_detect_store_job& j = jobs[i];
+    const FeatStore& FS = c->wins[j.win].feat;
+    for (int cam = 0; cam < j.n_cams; ++cam) {
+      const size_t img = (size_t)j.feat_slot * FS.C + cam, base = img * FS.N;
+      ims.push_back(j.images[cam]);
+      outs.push_back(DetectOut{j.out_kp + (size_t)cam * max_out, j.out_desc ? j.out_desc + (size_t)cam * max_out * db : nullptr, j.n_out + cam});
+      dests.push_back(StoreDest{FS.kp + 2 * base, FS.size + base, FS.desc + base * (FS.D / 4), FS.lm + base, FS.observed + base, FS.n + img});
+    }
+  }
+  cudaSetDevice(c->device);
+  okb_frontend_state* F = fe(c);
+  std::lock_guard<std::mutex> lk(F->batch_mtx);
+  if (!F->batch_stream) OKB_CUDA(c, cudaStreamCreateWithFlags(&F->batch_stream, cudaStreamNonBlocking));
+  if (!F->store_ready) OKB_CUDA(c, cudaEventCreateWithFlags(&F->store_ready, cudaEventDisableTiming));
+  if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
+  OKB_CUDA(c, cudaEventRecord(F->store_ready, c->stream_xfer));
+  rc = detect_run(c, F, F->batch_det, F->batch_stream, n, ims.data(), prm, outs.data(), max_out, dests.data(), F->store_ready, host_threads);
+  if (rc != OKB_OK && rc != OKB_ERR_CAPACITY) return rc;
+  for (int i = 0; i < n_jobs; ++i) {       // the host's counts follow the entries written (an image over capacity kept its own)
+    WinStore& S = c->wins[jobs[i].win];
+    for (int cam = 0; cam < jobs[i].n_cams; ++cam) {
+      const int m = jobs[i].n_out[cam];
+      if (m < 0) continue;
+      const size_t img = (size_t)jobs[i].feat_slot * S.feat.C + cam;
+      S.feat_n[img] = S.feat_n_pending[img] = m;
+    }
+  }
+  return rc;
 }
