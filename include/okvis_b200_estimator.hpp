@@ -5,15 +5,15 @@
 //   * the keyframe window lives on the device (one slot of the context); addStates / addLandmark / addObservation /
 //     removeObservation / set_* forward ONE command each (okb_window_add_frame, ...), so a frame's worth of data
 //     crosses PCIe per optimize() -- never the window;
-//   * optimize()                      = okb_optimize + okb_window_download           (Estimator.cpp:843-906)
+//   * optimize()                      = okb_optimize_slots + okb_window_download_slots (Estimator.cpp:843-906)
 //   * applyMarginalizationStrategy()  = the reference's bookkeeping (which blocks / residuals, Estimator.cpp:434-773)
-//                                       on the host + okb_window_marginalize for MarginalizationError's numerics
+//                                       on the host + okb_window_marginalize_batch for MarginalizationError's numerics
 //                                       (MarginalizationError.cpp:127-435, 507-846) + okb_window_remove_*;
-//   * state prediction in addStates() = okb_imu_propagate                            (ImuError.cpp:287-504).
-// A standalone Estimator owns a one-window context.  An EstimatorGroup (below) owns one context for many sessions, one
-// slot each, and runs addStates / optimize / applyMarginalizationStrategy for a list of them with one batched device
-// call per step (okb_imu_propagate_batch, okb_optimize_slots + okb_window_download_slots, okb_window_marginalize_batch);
-// the three calls are split into host halves and a device step that the single and the group forms share.
+//   * state prediction in addStates() = okb_imu_propagate_batch                        (ImuError.cpp:287-504).
+// An EstimatorGroup (below) owns one context for many sessions, one slot each, and runs addStates / optimize /
+// applyMarginalizationStrategy for a list of them with one batched device call per step, between host halves of the
+// session.  A standalone Estimator is a group of one: it owns a one-window EstimatorGroup, takes its slot 0, and its
+// own addStates / optimize / applyMarginalizationStrategy run the group's list bodies on the list {this}.
 // Eigen-free: poses are [t(3), q_xyzw(4)] arrays exactly as PoseParameterBlock stores them
 // (okvis_ceres/src/PoseParameterBlock.cpp:68-79), so an OKVIS build wraps these calls one-to-one (INTEGRATION.md
 // shows the adaptor a maintainer would add; the MultiFrame / cv types stay on the OKVIS side of it).
@@ -27,6 +27,7 @@
 #include <cstdint>
 #include <iterator>
 #include <map>
+#include <memory>
 #include <ostream>
 #include <set>
 #include <stdexcept>
@@ -76,6 +77,11 @@ struct EstimatorCapacity {
   int featureKeypoints = 0, descriptorBytes = 48;
 };
 
+// Throws std::runtime_error with the context's last error unless rc is OKB_OK.
+inline void throwIfFailed(okb_ctx* ctx, int rc) {
+  if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+}
+
 class EstimatorGroup;
 class Frontend;
 
@@ -83,8 +89,6 @@ class Estimator {
  private:
   friend class EstimatorGroup;
   friend class Frontend;
-  using Clock = std::chrono::steady_clock;
-  static double seconds(Clock::time_point t0) { return std::chrono::duration<double>(Clock::now() - t0).count(); }
 
   struct State { uint64_t id = 0; int64_t t_ns = 0; bool isKeyframe = false, hasSb = false; Pose7 T_WS{}; SpeedAndBias sb{}; bool hasImuTerm = false; std::vector<okb_imu_sample> imuFromPrev; };
   struct BlockRef { int kind; uint64_t id; };
@@ -115,10 +119,8 @@ class Estimator {
  public:
   using Capacity = EstimatorCapacity;
 
-  // A standalone session: its own context with one window, slot 0.
-  explicit Estimator(int device = 0, Capacity cap = Capacity()) : cap_(cap) {
-    if (okb_ctx_create(device, 1, &ctx_) != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(nullptr));
-  }
+  // A standalone session: a group of one (its own context with one window), slot 0.
+  explicit Estimator(int device = 0, Capacity cap = Capacity());
   // A session of `group`: takes the group's lowest free slot (throws std::runtime_error when the group is full) and
   // gives it back on destruction.  The slot's window from a previous occupant is replaced by this session's first
   // full upload (its first optimize / applyMarginalizationStrategy), which also drops its pending commands and prior.
@@ -143,20 +145,9 @@ class Estimator {
 
   // ---- Estimator::addStates (Estimator.cpp:110-343): first frame -> gravity-aligned pose + priors; later frames ->
   // propagate the last state through the IMU samples, add an ImuError term.
-  // Three halves, shared with EstimatorGroup::addStates: prepareState (checks, first-frame pose and priors),
-  // the prediction (okb_imu_propagate here, one okb_imu_propagate_batch in the group) and appendState.
-  bool addStates(uint64_t frameId, int64_t timestamp_ns, const std::vector<ImuMeasurement>& imu, bool asKeyframe) {
-    PendingState p;
-    if (!prepareState(frameId, timestamp_ns, imu, asKeyframe, p)) return false;
-    if (p.predict) {
-      const auto t0 = Clock::now();
-      const int rc = okb_imu_propagate(ctx_, &imu_, p.samples.data(), (int)p.samples.size(), p.t0_ns, timestamp_ns, p.st.T_WS.data(),
-                                       p.st.sb.data(), nullptr, nullptr, &p.used);
-      deviceSeconds_ += seconds(t0);
-      if (rc != OKB_OK) return false;
-    }
-    return appendState(p);
-  }
+  // EstimatorGroup::addStates for this session alone: prepareState (checks, first-frame pose and priors), the
+  // prediction (okb_imu_propagate_batch) and appendState.
+  bool addStates(uint64_t frameId, int64_t timestamp_ns, const std::vector<ImuMeasurement>& imu, bool asKeyframe);
 
   // ---- landmarks / observations (Estimator.cpp:345-413, implementation/Estimator.hpp:43-90)
   bool addLandmark(uint64_t landmarkId, const Vec4& hp) {
@@ -169,7 +160,7 @@ class Estimator {
     else slot = slotCount_++;
     if ((int)slot >= cap_.landmarks) throw std::runtime_error("okvis_b200: landmark capacity of the resident window exceeded");
     lmSlot_[landmarkId] = slot; slotOwner_[slot] = landmarkId;
-    if (resident_) check(okb_window_set_landmarks(ctx_, slot_, 1, &slot, hp.data()));
+    if (resident_) throwIfFailed(ctx_, okb_window_set_landmarks(ctx_, slot_, 1, &slot, hp.data()));
     return true;
   }
   // returns the residual block id (0 = duplicate observation, like the reference's NULL)
@@ -186,7 +177,7 @@ class Estimator {
     const uint64_t id = ++nextResidualId_;
     obs_[id] = o;
     it->second.observations[kid] = id;
-    if (resident_) { okb_observation d = deviceObs(o); check(okb_window_add_observations(ctx_, slot_, 1, &d)); }
+    if (resident_) { okb_observation d = deviceObs(o); throwIfFailed(ctx_, okb_window_add_observations(ctx_, slot_, 1, &d)); }
     setStoreLandmark(poseId, camIdx, keypointIdx, landmarkId, true);
     return id;
   }
@@ -195,7 +186,7 @@ class Estimator {
     if (it == obs_.end()) return false;
     if (resident_) {
       okb_obs_key k{posePos(it->second.pose), lmSlot_.at(it->second.lm), it->second.cam, 0};
-      check(okb_window_remove_observations(ctx_, slot_, 1, &k));
+      throwIfFailed(ctx_, okb_window_remove_observations(ctx_, slot_, 1, &k));
     }
     // the keypoint keeps its landmark but no longer holds the observation (skipB of doSetup, :238-250)
     setStoreLandmark(it->second.pose, it->second.cam, it->second.kp, it->second.lm, false);
@@ -213,35 +204,14 @@ class Estimator {
 
   // ---- Estimator::applyMarginalizationStrategy (Estimator.cpp:434-773).  Bookkeeping on the host, numerics
   // (linearisation at the first-estimate points, Schur complements, eigen-factorisation) on the device.
-  // Split at its device step, as EstimatorGroup's form is: planMarginalization -> okb_window_marginalize -> finishMarginalization.
-  bool applyMarginalizationStrategy(size_t numKeyframes, size_t numImuFrames, MapPointVector& removedLandmarks) {
-    MargPlan p;
-    planMarginalization(numKeyframes, numImuFrames, removedLandmarks, p);
-    if (p.skip) return true;
-    if (const okb_marg_job* job = p.deviceJob()) {
-      const auto t0 = Clock::now();
-      const int rc = okb_window_marginalize(ctx_, slot_, job);
-      deviceSeconds_ += seconds(t0);
-      check(rc);
-    }
-    finishMarginalization(p);
-    return true;
-  }
+  // EstimatorGroup's form for this session alone: planMarginalization -> okb_window_marginalize_batch -> finishMarginalization.
+  bool applyMarginalizationStrategy(size_t numKeyframes, size_t numImuFrames, MapPointVector& removedLandmarks);
   bool applyMarginalizationStrategy(size_t numKeyframes, size_t numImuFrames) { MapPointVector r; return applyMarginalizationStrategy(numKeyframes, numImuFrames, r); }
 
   // ---- Estimator::optimize (Estimator.cpp:843-906) + setOptimizationTimeLimit (:909-929)
   bool setOptimizationTimeLimit(double timeLimit, int minIterations) { timeLimit_ = timeLimit; minIterations_ = minIterations; return true; }
-  void optimize(size_t numIter, size_t /*numThreads*/ = 1, bool /*verbose*/ = false) {
-    if (!prepareOptimize()) return;
-    const okb_solve_options opt = solveOptions(numIter);
-    Estimates e = estimateBuffers();
-    const auto t0 = Clock::now();
-    int rc = okb_optimize(ctx_, slot_, 1, &opt, &summary_);
-    if (rc == OKB_OK) rc = okb_window_download(ctx_, slot_, e.poses.data(), e.sbs.data(), e.lms.data(), e.q.data());
-    deviceSeconds_ += seconds(t0);
-    check(rc);
-    adoptEstimates(e);
-  }
+  // EstimatorGroup::optimize for this session alone.
+  void optimize(size_t numIter, size_t /*numThreads*/ = 1, bool /*verbose*/ = false);
   const okb_summary& summary() const { return summary_; }
   // bytes the last commit of the window moved host -> device (a frame's worth once the window is resident; 0 before)
   int64_t lastUploadBytes() const { return resident_ ? okb_window_h2d_bytes(ctx_, slot_) : 0; }
@@ -376,14 +346,14 @@ class Estimator {
       // observations still attached to a deleted landmark die with it on the device (okb_window_remove_landmarks)
       for (auto o = obs_.begin(); o != obs_.end();) o = (o->second.lm == lid) ? obs_.erase(o) : std::next(o);
       const uint32_t slot = lmSlot_.at(lid);
-      check(okb_window_remove_landmarks(ctx_, slot_, 1, &slot));
+      throwIfFailed(ctx_, okb_window_remove_landmarks(ctx_, slot_, 1, &slot));
       lmSlot_.erase(lid); slotOwner_.erase(slot); freeSlots_.insert(slot);
     }
     for (uint64_t fid : p.removeAllButPose) {        // newest first: positions of older blocks do not move
       State& st = states_.at(fid);
       const bool whole = contains(removeFrames, fid);
       if (whole) {
-        check(okb_window_remove_frame(ctx_, slot_, posePos(fid), st.hasSb ? sbPos(fid) : 0xffffffffu));
+        throwIfFailed(ctx_, okb_window_remove_frame(ctx_, slot_, posePos(fid), st.hasSb ? sbPos(fid) : 0xffffffffu));
         releaseFeatures(fid);
         for (auto o = obs_.begin(); o != obs_.end();) {
           if (o->second.pose == fid) {
@@ -393,7 +363,7 @@ class Estimator {
           } else ++o;
         }
       } else if (st.hasSb) {
-        check(okb_window_remove_speed_bias(ctx_, slot_, sbPos(fid)));
+        throwIfFailed(ctx_, okb_window_remove_speed_bias(ctx_, slot_, sbPos(fid)));
       }
       // host mirrors of the device lists (stable compaction, exactly what the interpreter does)
       eraseIf(terms_, [&](const TermRef& t) { return (t.first == fid || t.second == fid); });
@@ -414,22 +384,16 @@ class Estimator {
     pushPriors();
   }
 
-  // optimize, host half before the solve: false where there is nothing to solve
-  bool prepareOptimize() {
+  // optimize, host half before the solve: false where there is nothing to solve; else the window is resident, and opt
+  // and e are the solve options and the buffers of the download
+  bool prepareOptimize(size_t numIter, okb_solve_options& opt, Estimates& e) {
     if (states_.empty() || cameras_.empty()) return false;
     ensureResident();
-    return true;
-  }
-  okb_solve_options solveOptions(size_t numIter) const {
-    okb_solve_options opt{};
+    opt = okb_solve_options{};
     opt.max_iterations = (int)numIter; opt.min_iterations = minIterations_; opt.time_limit_s = timeLimit_; opt.use_cauchy_loss = 1;
-    return opt;
-  }
-  Estimates estimateBuffers() const {
     const size_t K = states_.size(), NSB = numSb(), L = slotCount_ ? slotCount_ : 1;
-    Estimates e;
     e.poses.resize(7 * K); e.sbs.resize(9 * std::max<size_t>(NSB, 1)); e.lms.resize(4 * L); e.q.resize(L);
-    return e;
+    return true;
   }
   // optimize, write-back half (Estimator.cpp:880-900): poses, speed/bias, and point + quality for every landmark
   void adoptEstimates(const Estimates& e) {
@@ -463,13 +427,13 @@ class Estimator {
   bool set_T_WS(uint64_t poseId, const Pose7& T) {
     auto it = states_.find(poseId); if (it == states_.end()) return false;
     it->second.T_WS = T;
-    if (resident_) { const uint32_t p = posePos(poseId); check(okb_window_set_states(ctx_, slot_, 1, &p, T.data(), 0, nullptr, nullptr)); }
+    if (resident_) { const uint32_t p = posePos(poseId); throwIfFailed(ctx_, okb_window_set_states(ctx_, slot_, 1, &p, T.data(), 0, nullptr, nullptr)); }
     return true;
   }
   bool setSpeedAndBias(uint64_t poseId, size_t /*imuIdx*/, const SpeedAndBias& sb) {
     auto it = states_.find(poseId); if (it == states_.end() || !it->second.hasSb) return false;
     it->second.sb = sb;
-    if (resident_) { const uint32_t p = sbPos(poseId); check(okb_window_set_states(ctx_, slot_, 0, nullptr, nullptr, 1, &p, sb.data())); }
+    if (resident_) { const uint32_t p = sbPos(poseId); throwIfFailed(ctx_, okb_window_set_states(ctx_, slot_, 0, nullptr, nullptr, 1, &p, sb.data())); }
     return true;
   }
   bool setCameraSensorStates(uint64_t poseId, size_t cameraIdx, const Pose7& T_SCi) {
@@ -487,7 +451,7 @@ class Estimator {
   bool setLandmark(uint64_t id, const Vec4& hp) {
     auto it = landmarks_.find(id); if (it == landmarks_.end()) return false;
     it->second.point = hp;
-    if (resident_) { const uint32_t s = lmSlot_.at(id); check(okb_window_set_landmarks(ctx_, slot_, 1, &s, hp.data())); }
+    if (resident_) { const uint32_t s = lmSlot_.at(id); throwIfFailed(ctx_, okb_window_set_landmarks(ctx_, slot_, 1, &s, hp.data())); }
     return true;
   }
   bool isLandmarkAdded(uint64_t id) const { return landmarks_.count(id) != 0; }
@@ -498,7 +462,7 @@ class Estimator {
     if (resident_ && featReserved_) {
       const uint32_t s = lmSlot_.at(id);
       const uint8_t f = initialized ? 1 : 0;
-      check(okb_window_set_landmark_initialized(ctx_, slot_, 1, &s, &f));
+      throwIfFailed(ctx_, okb_window_set_landmark_initialized(ctx_, slot_, 1, &s, &f));
     }
   }
 
@@ -523,7 +487,7 @@ class Estimator {
       KeypointIdentifier kid; kid.frameId = frameId; kid.cameraIndex = cam; kid.keypointIndex = k;
       observed[k] = l->second.observations.count(kid) ? 1 : 0;
     }
-    check(okb_window_set_features(ctx_, slot_, fs->second, (int)cam, (int)n, keypoints.data(), descriptors.data(), slots.data(), observed.data()));
+    throwIfFailed(ctx_, okb_window_set_features(ctx_, slot_, fs->second, (int)cam, (int)n, keypoints.data(), descriptors.data(), slots.data(), observed.data()));
     FrameFeatures& f = feats_[frameId][cam];
     f.kp = keypoints; f.lm = landmarkIds;
   }
@@ -601,9 +565,9 @@ class Estimator {
 
  private:
 
-  // addStates, host check / prepare half: nothing changes; false where the single call returns false before its
-  // prediction.  A prediction needs two samples at least (okb_imu_propagate rejects fewer): such a request fails here
-  // so that it cannot fail a group's whole prediction batch.
+  // addStates, host check / prepare half: nothing changes; false where addStates returns false before its
+  // prediction.  A prediction needs two samples at least (okb_imu_propagate_batch rejects a job with fewer): such a
+  // request fails here so that it cannot fail a group's whole prediction batch.
   bool prepareState(uint64_t frameId, int64_t timestamp_ns, const std::vector<ImuMeasurement>& imu, bool asKeyframe, PendingState& p) const {
     if (!hasImu_ || states_.count(frameId)) return false;
     if (!states_.empty() && frameId < states_.rbegin()->first) return false;      // ids grow with time, as IdProvider's do
@@ -652,7 +616,7 @@ class Estimator {
       const State& prev = states_.at(prevId);
       t.pose0 = posePos(prevId); t.sb0 = sbPos(prevId); t.pose1 = posePos(frameId); t.sb1 = sbPos(frameId);
       t.t0_ns = prev.t_ns; t.t1_ns = st.t_ns; t.sample_offset = 0; t.sample_count = (uint32_t)p.samples.size();
-      check(okb_window_add_frame(ctx_, slot_, st.T_WS.data(), st.sb.data(), &t, p.samples.data(), (int)p.samples.size()));
+      throwIfFailed(ctx_, okb_window_add_frame(ctx_, slot_, st.T_WS.data(), st.sb.data(), &t, p.samples.data(), (int)p.samples.size()));
     }
     return true;
   }
@@ -667,7 +631,6 @@ class Estimator {
     for (size_t i = 0; i < imu.size(); ++i) { s[i].t_ns = imu[i].t_ns; for (int k = 0; k < 3; ++k) { s[i].gyro[k] = imu[i].gyro[k]; s[i].acc[k] = imu[i].acc[k]; } }
     return s;
   }
-  void check(int rc) const { if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx_)); }
   uint32_t posePos(uint64_t id) const { return (uint32_t)std::distance(states_.begin(), states_.find(id)); }
   uint32_t sbPos(uint64_t id) const {
     uint32_t p = 0;
@@ -692,7 +655,7 @@ class Estimator {
     auto s = lmSlot_.find(landmarkId);
     const int32_t k = (int32_t)kp, l = s == lmSlot_.end() ? -1 : (int32_t)s->second;
     const uint8_t o = observed ? 1 : 0;
-    check(okb_window_set_feature_landmarks(ctx_, slot_, featSlot_.at(frameId), (int)cam, 1, &k, &l, &o));
+    throwIfFailed(ctx_, okb_window_set_feature_landmarks(ctx_, slot_, featSlot_.at(frameId), (int)cam, 1, &k, &l, &o));
     f->second[cam].lm[kp] = landmarkId;
   }
   // the frame's feature slot, taken from the free ones when the frame has none yet
@@ -709,13 +672,32 @@ class Estimator {
   void releaseFeatures(uint64_t frameId) {
     auto fs = featSlot_.find(frameId);
     if (fs == featSlot_.end()) return;
-    check(okb_window_clear_features(ctx_, slot_, fs->second));
+    throwIfFailed(ctx_, okb_window_clear_features(ctx_, slot_, fs->second));
     freeFeat_.insert(fs->second);
     featSlot_.erase(fs);
     feats_.erase(frameId);
   }
-  // One okb_track_3d2d_batch job of this session: frame B = currentFrameId against the frames `frameA`, every camera
-  // im -> im that both frames have features for.  finishTrack applies the results through addObservation.
+  // A round of the current frame against frame A: camera camA of frame A against camera camB of the current frame (a
+  // 3D-2D tracking round, or the camera pair of a 2D-2D match).
+  struct TrackRound { uint64_t frameA; size_t camA, camB; };
+  // The rounds of matchToKeyframes (Frontend.cpp:389-452) or, keyframes false, of matchToLastFrame (:484-509), in the
+  // reference's order: every camera im -> im against each older frame by age from 1 -- the keyframes, at most
+  // maxKeyframes of them, or the last frame unless it is a keyframe.  None before the second frame (:381-384, 470-473).
+  std::vector<TrackRound> olderFrameRounds(bool keyframes, size_t maxKeyframes) const {
+    std::vector<uint64_t> older;
+    if (keyframes) {
+      for (size_t age = 1; age < states_.size() && older.size() < maxKeyframes; ++age)
+        if (isKeyframe(frameIdByAge(age))) older.push_back(frameIdByAge(age));
+    } else if (states_.size() > 1 && !isKeyframe(frameIdByAge(1))) {
+      older.push_back(frameIdByAge(1));
+    }
+    std::vector<TrackRound> rounds;
+    for (uint64_t a : older)
+      for (size_t im = 0; im < cameras_.size(); ++im) rounds.push_back(TrackRound{a, im, im});
+    return rounds;
+  }
+  // One okb_track_3d2d_batch job of this session: frame B = currentFrameId against `rounds`; rounds without features
+  // on either side are dropped.  finishTrack applies the results through addObservation.
   struct TrackPlan {
     uint64_t frameB = 0;
     std::vector<okb_track_round> rounds;
@@ -725,14 +707,6 @@ class Estimator {
     int32_t nAssoc = 0, nUninit = 0;
     okb_track_job job{};
   };
-  bool planTrack(uint64_t currentFrameId, const std::vector<uint64_t>& frameA, float threshold, TrackPlan& p) {
-    std::vector<TrackRound> rounds;
-    for (uint64_t a : frameA)
-      for (size_t im = 0; im < cameras_.size(); ++im) rounds.push_back(TrackRound{a, im, im});
-    return planTrackRounds(currentFrameId, rounds, threshold, p);
-  }
-  // the same for an explicit round list (frame A, camera A, camera B); rounds without features on either side are dropped
-  struct TrackRound { uint64_t frameA; size_t camA, camB; };
   bool planTrackRounds(uint64_t currentFrameId, const std::vector<TrackRound>& rounds, float threshold, TrackPlan& p) {
     auto fb = featSlot_.find(currentFrameId);
     if (fb == featSlot_.end()) return false;
@@ -995,7 +969,7 @@ class Estimator {
     std::vector<okb_pose_prior> pps; std::vector<okb_sb_prior> sps;
     for (auto& p : posePriors_) { okb_pose_prior q = p.p; q.pose_idx = posePos(p.frame); pps.push_back(q); }
     for (auto& p : sbPriors_) { okb_sb_prior q = p.p; q.sb_idx = sbPos(p.frame); sps.push_back(q); }
-    check(okb_window_set_priors(ctx_, slot_, (int)pps.size(), pps.data(), (int)sps.size(), sps.data(), nullptr));
+    throwIfFailed(ctx_, okb_window_set_priors(ctx_, slot_, (int)pps.size(), pps.data(), (int)sps.size(), sps.data(), nullptr));
   }
   // First contact with the device: the whole graph once (okb_window_upload); everything after that is incremental.
   void ensureResident() {
@@ -1029,26 +1003,27 @@ class Estimator {
     d.poses = poses.data(); d.speed_bias = sbs.data(); d.extrinsics = ext.data(); d.extrinsics_fixed = extFixed.data(); d.landmarks = lms.data();
     d.cameras = cameras_.data(); d.obs = obs.data(); d.imu_terms = terms.data(); d.imu_samples = samples.data(); d.imu_params = imu_;
     d.pose_priors = pps.data(); d.sb_priors = sps.data();
-    check(okb_window_reserve(ctx_, slot_, cap_.frames, cap_.landmarks, cap_.observations, cap_.imu_samples, cap_.marg_dim));
+    throwIfFailed(ctx_, okb_window_reserve(ctx_, slot_, cap_.frames, cap_.landmarks, cap_.observations, cap_.imu_samples, cap_.marg_dim));
     if (cap_.featureKeypoints > 0)
-      check(okb_window_reserve_features(ctx_, slot_, cap_.frames, (int)cameras_.size(), cap_.featureKeypoints, cap_.descriptorBytes));
-    check(okb_window_upload(ctx_, slot_, &d));
+      throwIfFailed(ctx_, okb_window_reserve_features(ctx_, slot_, cap_.frames, (int)cameras_.size(), cap_.featureKeypoints, cap_.descriptorBytes));
+    throwIfFailed(ctx_, okb_window_upload(ctx_, slot_, &d));
     resident_ = true;
     if (cap_.featureKeypoints > 0) {
       // a slot of a group may hold a previous session's store: every feature slot empty, every flag as this session has it
       featReserved_ = true;
-      for (int f = 0; f < cap_.frames; ++f) { check(okb_window_clear_features(ctx_, slot_, f)); freeFeat_.insert(f); }
+      for (int f = 0; f < cap_.frames; ++f) { throwIfFailed(ctx_, okb_window_clear_features(ctx_, slot_, f)); freeFeat_.insert(f); }
       std::vector<uint32_t> idx(cap_.landmarks);
       std::vector<uint8_t> flags(cap_.landmarks, 0);
       for (int s = 0; s < cap_.landmarks; ++s) idx[s] = (uint32_t)s;
       for (auto& kv : lmInitialized_) if (kv.second && lmSlot_.count(kv.first)) flags[lmSlot_.at(kv.first)] = 1;
-      check(okb_window_set_landmark_initialized(ctx_, slot_, cap_.landmarks, idx.data(), flags.data()));
+      throwIfFailed(ctx_, okb_window_set_landmark_initialized(ctx_, slot_, cap_.landmarks, idx.data(), flags.data()));
     }
   }
 
-  okb_ctx* ctx_ = nullptr;
-  EstimatorGroup* group_ = nullptr;          // nullptr: standalone, ctx_ is owned
-  int slot_ = 0;
+  std::unique_ptr<EstimatorGroup> own_;      // a standalone session's group of one; declared first, destroyed last
+  EstimatorGroup* group_;
+  okb_ctx* ctx_;                             // group_'s
+  int slot_;
   double deviceSeconds_ = 0;
   Capacity cap_;
   bool resident_ = false;
@@ -1130,6 +1105,39 @@ class EstimatorGroup {
     std::vector<Estimator*> sessions;
     for (const auto& r : requests) sessions.push_back(r.session);
     validate(sessions);
+    return addStates(requests, deviceSeconds_);
+  }
+
+  // Estimator::optimize(numIter) for each session: sessions with nothing to solve are skipped as the single call skips
+  // them; the rest are solved with one okb_optimize_slots per distinct (numIter, minIterations, timeLimit), then
+  // downloaded with one okb_window_download_slots and written back.
+  void optimize(const std::vector<Estimator*>& sessions, size_t numIter) {
+    validate(sessions);
+    optimize(sessions, numIter, deviceSeconds_);
+  }
+
+  // Estimator::applyMarginalizationStrategy(numKeyframes, numImuFrames, removed[i]) for each session: every session
+  // plans (the host bookkeeping), one okb_window_marginalize_batch runs the jobs, every session finishes.  removed is
+  // resized to the list's length if shorter; removed[i] receives what sessions[i] removes.  A failing batch throws
+  // std::runtime_error naming the slot (Estimator::slot()) of the session whose job it rejected.
+  bool applyMarginalizationStrategy(const std::vector<Estimator*>& sessions, size_t numKeyframes, size_t numImuFrames,
+                                    std::vector<MapPointVector>& removed) {
+    validate(sessions);
+    if (removed.size() < sessions.size()) removed.resize(sessions.size());
+    std::vector<MapPointVector*> to;
+    for (size_t i = 0; i < sessions.size(); ++i) to.push_back(&removed[i]);
+    return applyMarginalizationStrategy(sessions, numKeyframes, numImuFrames, to, deviceSeconds_);
+  }
+
+ private:
+  friend class Estimator;
+  friend class Frontend;
+  using Clock = std::chrono::steady_clock;
+  static double seconds(Clock::time_point t0) { return std::chrono::duration<double>(Clock::now() - t0).count(); }
+
+  // The bodies of the three group calls and of a session's own calls (on the list {session}), for a validated list.
+  // The time of their device calls is added to `deviceTime`: the group's deviceSeconds_ or the session's.
+  std::vector<bool> addStates(const std::vector<StatesRequest>& requests, double& deviceTime) {
     const size_t n = requests.size();
     std::vector<Estimator::PendingState> p(n);
     std::vector<char> ok(n, 0);
@@ -1148,30 +1156,25 @@ class EstimatorGroup {
     if (!jobs.empty()) {
       const auto t0 = Clock::now();
       const int rc = okb_imu_propagate_batch(ctx_, (int)jobs.size(), jobs.data());
-      deviceSeconds_ += Estimator::seconds(t0);
-      if (rc != OKB_OK) for (size_t i : of) ok[i] = 0;        // as a failing okb_imu_propagate: addStates returns false
+      deviceTime += seconds(t0);
+      if (rc != OKB_OK) for (size_t i : of) ok[i] = 0;        // a failed prediction: addStates returns false
     }
     std::vector<bool> out(n);
     for (size_t i = 0; i < n; ++i) out[i] = ok[i] && requests[i].session->appendState(p[i]);
     return out;
   }
 
-  // Estimator::optimize(numIter) for each session: sessions with nothing to solve are skipped as the single call skips
-  // them; the rest are solved with one okb_optimize_slots per distinct (numIter, minIterations, timeLimit), then
-  // downloaded with one okb_window_download_slots and written back.
-  void optimize(const std::vector<Estimator*>& sessions, size_t numIter) {
-    validate(sessions);
+  void optimize(const std::vector<Estimator*>& sessions, size_t numIter, double& deviceTime) {
     std::vector<Estimator*> live;
-    for (Estimator* e : sessions) if (e->prepareOptimize()) live.push_back(e);
+    std::vector<okb_solve_options> opt(sessions.size());
+    std::vector<Estimator::Estimates> e(sessions.size());
+    for (Estimator* s : sessions)                                  // opt[i], e[i]: live[i]'s
+      if (s->prepareOptimize(numIter, opt[live.size()], e[live.size()])) live.push_back(s);
     if (live.empty()) return;
     const size_t n = live.size();
-    std::vector<okb_solve_options> opt(n);
-    for (size_t i = 0; i < n; ++i) opt[i] = live[i]->solveOptions(numIter);
-    std::vector<Estimator::Estimates> e(n);
     std::vector<int32_t> all(n);
     std::vector<double*> poses(n), sbs(n), lms(n), q(n);
     for (size_t i = 0; i < n; ++i) {
-      e[i] = live[i]->estimateBuffers();
       all[i] = live[i]->slot_;
       poses[i] = e[i].poses.data(); sbs[i] = e[i].sbs.data(); lms[i] = e[i].lms.data(); q[i] = e[i].q.data();
     }
@@ -1187,31 +1190,24 @@ class EstimatorGroup {
         }
       std::vector<okb_summary> summ(slots.size());
       const int rc = okb_optimize_slots(ctx_, (int)slots.size(), slots.data(), &opt[i], summ.data());
-      if (rc != OKB_OK) { deviceSeconds_ += Estimator::seconds(t0); check(rc); }
+      if (rc != OKB_OK) { deviceTime += seconds(t0); throwIfFailed(ctx_, rc); }
       for (size_t m = 0; m < members.size(); ++m) live[members[m]]->summary_ = summ[m];
     }
     const int rc = okb_window_download_slots(ctx_, (int)n, all.data(), poses.data(), sbs.data(), lms.data(), q.data());
-    deviceSeconds_ += Estimator::seconds(t0);
-    check(rc);
+    deviceTime += seconds(t0);
+    throwIfFailed(ctx_, rc);
     for (size_t i = 0; i < n; ++i) live[i]->adoptEstimates(e[i]);
   }
 
-  // Estimator::applyMarginalizationStrategy(numKeyframes, numImuFrames, removed[i]) for each session: every session
-  // plans (the host bookkeeping), one okb_window_marginalize_batch runs the jobs, every session finishes.  removed is
-  // resized to the list's length if shorter; removed[i] receives what sessions[i] removes.  A failing batch throws
-  // std::runtime_error naming the slot (Estimator::slot()) of the session whose job it rejected.
   bool applyMarginalizationStrategy(const std::vector<Estimator*>& sessions, size_t numKeyframes, size_t numImuFrames,
-                                    std::vector<MapPointVector>& removed) {
-    validate(sessions);
+                                    const std::vector<MapPointVector*>& removed, double& deviceTime) {
     const size_t n = sessions.size();
-    if (removed.size() < n) removed.resize(n);
     std::vector<Estimator::MargPlan> p(n);
-    for (size_t i = 0; i < n; ++i) sessions[i]->planMarginalization(numKeyframes, numImuFrames, removed[i], p[i]);
+    for (size_t i = 0; i < n; ++i) sessions[i]->planMarginalization(numKeyframes, numImuFrames, *removed[i], p[i]);
     int lo = max_, hi = -1;
     std::vector<const okb_marg_job*> jobs(max_, nullptr);
     for (size_t i = 0; i < n; ++i) {
-      if (p[i].skip) continue;
-      if (const okb_marg_job* j = p[i].deviceJob()) {
+      if (const okb_marg_job* j = p[i].deviceJob()) {        // none where the plan skips
         const int s = sessions[i]->slot_;
         jobs[s] = j; lo = std::min(lo, s); hi = std::max(hi, s);
       }
@@ -1219,26 +1215,20 @@ class EstimatorGroup {
     if (hi >= lo) {
       const auto t0 = Clock::now();
       const int rc = okb_window_marginalize_batch(ctx_, lo, hi - lo + 1, jobs.data() + lo);
-      deviceSeconds_ += Estimator::seconds(t0);
-      check(rc);
+      deviceTime += seconds(t0);
+      throwIfFailed(ctx_, rc);
     }
     for (size_t i = 0; i < n; ++i) if (!p[i].skip) sessions[i]->finishMarginalization(p[i]);
     return true;
   }
 
- private:
-  friend class Estimator;
-  friend class Frontend;
-  using Clock = Estimator::Clock;
-
-  void check(int rc) const { if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx_)); }
   void validate(const std::vector<Estimator*>& sessions) const {
     std::set<const Estimator*> seen;
     for (size_t i = 0; i < sessions.size(); ++i) {
       const Estimator* e = sessions[i];
       const std::string at = "okvis_b200: EstimatorGroup: entry " + std::to_string(i);
       if (!e) throw std::invalid_argument(at + " is null");
-      if (e->group_ != this) throw std::invalid_argument(at + (e->group_ ? " is a session of another group" : " is a standalone Estimator"));
+      if (e->group_ != this) throw std::invalid_argument(at + (e->own_ ? " is a standalone Estimator" : " is a session of another group"));
       if (!seen.insert(e).second) throw std::invalid_argument(at + " lists a session twice");
     }
   }
@@ -1255,10 +1245,18 @@ class EstimatorGroup {
   double deviceSeconds_ = 0;
 };
 
-inline Estimator::Estimator(EstimatorGroup& group, Capacity cap) : ctx_(group.ctx_), group_(&group), slot_(group.takeSlot()), cap_(cap) {}
-inline Estimator::~Estimator() {
-  if (group_) group_->free_.insert(slot_);
-  else okb_ctx_destroy(ctx_);
+inline Estimator::Estimator(int device, Capacity cap)
+    : own_(new EstimatorGroup(device, 1)), group_(own_.get()), ctx_(group_->ctx_), slot_(group_->takeSlot()), cap_(cap) {}
+inline Estimator::Estimator(EstimatorGroup& group, Capacity cap) : group_(&group), ctx_(group.ctx_), slot_(group.takeSlot()), cap_(cap) {}
+// The slot goes back before own_, and with it a standalone session's context, is destroyed.
+inline Estimator::~Estimator() { group_->free_.insert(slot_); }
+
+inline bool Estimator::addStates(uint64_t frameId, int64_t timestamp_ns, const std::vector<ImuMeasurement>& imu, bool asKeyframe) {
+  return group_->addStates({{this, frameId, timestamp_ns, imu, asKeyframe}}, deviceSeconds_)[0];
+}
+inline void Estimator::optimize(size_t numIter, size_t, bool) { group_->optimize({this}, numIter, deviceSeconds_); }
+inline bool Estimator::applyMarginalizationStrategy(size_t numKeyframes, size_t numImuFrames, MapPointVector& removedLandmarks) {
+  return group_->applyMarginalizationStrategy({this}, numKeyframes, numImuFrames, {&removedLandmarks}, deviceSeconds_);
 }
 
 }  // namespace okvis_b200

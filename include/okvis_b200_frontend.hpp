@@ -28,7 +28,9 @@
 // with the adaptor, in RansacHooks.  Frontend::detectAndDescribe(estimator, frameId, images) detects every camera of a
 // frame straight into the frame's feature slot of the estimator's store (okb_detect_describe_store_batch: one device
 // call, the descriptors stay on the device), in place of the single-image detectAndDescribe + setFrameFeatures; its
-// EstimatorGroup form makes one call for many sessions.
+// EstimatorGroup form makes one call for many sessions.  Each call has one body: a group form validates its list once,
+// before any device work, and a single form runs the same body on its session alone, in the session's group (a
+// standalone Estimator's group of one).
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -85,9 +87,8 @@ class Frontend {
     keypoints.resize(briskDetectionMaximumKeypoints_);
     descriptors.resize(briskDetectionMaximumKeypoints_ * (size_t)descriptorBytes_);
     int n = 0;
-    const int rc = okb_detect_describe(ctx_, (int)cameraIndex, image, width, height, stride, &geometry, R_CW, &p, keypoints.data(), descriptors.data(),
-                                       (int)briskDetectionMaximumKeypoints_, &n);
-    if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx_));
+    throwIfFailed(ctx_, okb_detect_describe(ctx_, (int)cameraIndex, image, width, height, stride, &geometry, R_CW, &p, keypoints.data(),
+                                            descriptors.data(), (int)briskDetectionMaximumKeypoints_, &n));
     keypoints.resize(n);
     descriptors.resize((size_t)n * descriptorBytes_);
     isInitialized_ = true;
@@ -108,14 +109,15 @@ class Frontend {
   // after Estimator::setFrameFeatures with every landmark id 0.  Returns the keypoints per camera, equal to the
   // single-image detectAndDescribe's.
   std::vector<std::vector<okb_keypoint>> detectAndDescribe(Estimator& estimator, uint64_t frameId, const std::vector<CameraImage>& images) {
-    return detectStoreGroup(nullptr, {&estimator}, {frameId}, {images})[0];
+    return detectStoreGroup(*estimator.group_, {&estimator}, {frameId}, {images})[0];
   }
   // The same for sessions of one EstimatorGroup (any order, each listed once): one okb_detect_describe_store_batch for
   // all of them; results[i] equals the single form's on sessions[i].
   std::vector<std::vector<std::vector<okb_keypoint>>> detectAndDescribe(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
                                                                         const std::vector<uint64_t>& frameIds,
                                                                         const std::vector<std::vector<CameraImage>>& images) {
-    return detectStoreGroup(&group, sessions, frameIds, images);
+    group.validate(sessions);
+    return detectStoreGroup(group, sessions, frameIds, images);
   }
 
   // Frontend::propagation (Frontend.cpp:274-292): ImuError::propagation on the device; covariance / jacobian 15x15 or null.
@@ -166,21 +168,23 @@ class Frontend {
   };
   // matchToKeyframes' 3D-2D loop (Frontend.cpp:389-411): keyframes by age from 1, every camera im -> im, at most 3
   TrackResult matchToKeyframes3D2D(Estimator& estimator, uint64_t currentFrameId) {
-    return trackGroup(nullptr, {&estimator}, {currentFrameId}, true)[0];
+    return trackGroup(*estimator.group_, {&estimator}, {currentFrameId}, true)[0];
   }
   // matchToLastFrame's 3D-2D pass (:484-494): nothing when the last frame is a keyframe
   TrackResult matchToLastFrame3D2D(Estimator& estimator, uint64_t currentFrameId) {
-    return trackGroup(nullptr, {&estimator}, {currentFrameId}, false)[0];
+    return trackGroup(*estimator.group_, {&estimator}, {currentFrameId}, false)[0];
   }
   // The same for sessions of one EstimatorGroup (any order, each listed once): one okb_track_3d2d_batch for all of them;
   // results[i] equals the single call's on sessions[i].
   std::vector<TrackResult> matchToKeyframes3D2D(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
                                                 const std::vector<uint64_t>& currentFrameIds) {
-    return trackGroup(&group, sessions, currentFrameIds, true);
+    group.validate(sessions);
+    return trackGroup(group, sessions, currentFrameIds, true);
   }
   std::vector<TrackResult> matchToLastFrame3D2D(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
                                                 const std::vector<uint64_t>& currentFrameIds) {
-    return trackGroup(&group, sessions, currentFrameIds, false);
+    group.validate(sessions);
+    return trackGroup(group, sessions, currentFrameIds, false);
   }
 
   // ---- 2D-2D landmark initialisation against earlier frames (device: okb_match2d2d_batch)
@@ -195,11 +199,11 @@ class Frontend {
                                    const std::function<void(size_t, uint64_t)>& afterKeyframe = {}) {
     std::function<void(size_t, size_t, uint64_t)> cb;
     if (afterKeyframe) cb = [&](size_t, size_t kf, uint64_t id) { afterKeyframe(kf, id); };
-    return match2D2DGroup(nullptr, {&estimator}, {currentFrameId}, {newId}, true, cb)[0];
+    return match2D2DGroup(*estimator.group_, {&estimator}, {currentFrameId}, {newId}, true, cb)[0];
   }
   // matchToLastFrame's 2D-2D loop (:499-509): nothing when the last frame is a keyframe
   TrackResult matchToLastFrame2D2D(Estimator& estimator, uint64_t currentFrameId, const std::function<uint64_t()>& newId) {
-    return match2D2DGroup(nullptr, {&estimator}, {currentFrameId}, {newId}, false, {})[0];
+    return match2D2DGroup(*estimator.group_, {&estimator}, {currentFrameId}, {newId}, false, {})[0];
   }
   // The same for sessions of one EstimatorGroup: one okb_match2d2d_batch per round index for every session that has
   // that round, each session's records applied in list order with its own newId; afterKeyframe(session, kfcounter,
@@ -208,12 +212,14 @@ class Frontend {
                                                 const std::vector<uint64_t>& currentFrameIds,
                                                 const std::vector<std::function<uint64_t()>>& newIds,
                                                 const std::function<void(size_t, size_t, uint64_t)>& afterKeyframe = {}) {
-    return match2D2DGroup(&group, sessions, currentFrameIds, newIds, true, afterKeyframe);
+    group.validate(sessions);
+    return match2D2DGroup(group, sessions, currentFrameIds, newIds, true, afterKeyframe);
   }
   std::vector<TrackResult> matchToLastFrame2D2D(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
                                                 const std::vector<uint64_t>& currentFrameIds,
                                                 const std::vector<std::function<uint64_t()>>& newIds) {
-    return match2D2DGroup(&group, sessions, currentFrameIds, newIds, false, {});
+    group.validate(sessions);
+    return match2D2DGroup(group, sessions, currentFrameIds, newIds, false, {});
   }
 
   // ---- stereo landmark initialisation of the current frame (device: okb_match2d2d_batch + okb_track_3d2d_batch)
@@ -225,13 +231,14 @@ class Frontend {
   // frame names a landmark that is not in the graph.  The counts are those of the 3D-2D passes.
   TrackResult matchStereo(Estimator& estimator, uint64_t frameId, const std::function<uint64_t()>& newId,
                           const std::vector<std::vector<bool>>& overlap) {
-    return stereoGroup(nullptr, {&estimator}, {frameId}, {newId}, overlap)[0];
+    return stereoGroup(*estimator.group_, {&estimator}, {frameId}, {newId}, overlap)[0];
   }
   // The same for sessions of one EstimatorGroup: one okb_match2d2d_batch and one okb_track_3d2d_batch per camera
   // pair for all of them; each session's records are applied in list order with that session's newId.
   std::vector<TrackResult> matchStereo(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                        const std::vector<std::function<uint64_t()>>& newIds, const std::vector<std::vector<bool>>& overlap) {
-    return stereoGroup(&group, sessions, frameIds, newIds, overlap);
+    group.validate(sessions);
+    return stereoGroup(group, sessions, frameIds, newIds, overlap);
   }
 
   // ---- the keyframe decision (device: okb_keyframe_overlap_batch)
@@ -244,7 +251,7 @@ class Frontend {
                             okb_keyframe_result* result = nullptr) {
     std::vector<std::vector<okb_keyframe_cam>> c;
     std::vector<okb_keyframe_result> r;
-    const bool need = keyframeGroup(nullptr, {&estimator}, {currentFrameId}, {(char)(isInitialized_ ? 1 : 0)}, &c, &r)[0];
+    const bool need = keyframeGroup(*estimator.group_, {&estimator}, {currentFrameId}, {(char)(isInitialized_ ? 1 : 0)}, &c, &r)[0];
     if (cams) *cams = c[0];
     if (result) *result = r[0];
     return need;
@@ -256,7 +263,7 @@ class Frontend {
                                          std::vector<okb_keyframe_result>* results = nullptr) {
     std::vector<const Estimator*> cs(sessions.begin(), sessions.end());
     group.validate(sessions);
-    return keyframeGroup(&group, cs, frameIds, initialized, cams, results);
+    return keyframeGroup(group, cs, frameIds, initialized, cams, results);
   }
 
   // ---- 3D-2D outlier rejection (device: okb_ransac_3d2d_batch)
@@ -265,13 +272,14 @@ class Frontend {
   // Estimator::removeObservation (when removeOutliers) and then Estimator::setFrameLandmarkId(..., 0), which leaves the
   // keypoint with host id 0, store slot -1 and no observation.  Returns what the reference returns.
   int runRansac3d2d(Estimator& estimator, uint64_t currentFrameId, bool removeOutliers = true) {
-    return ransacGroup(nullptr, {&estimator}, {currentFrameId}, removeOutliers)[0];
+    return ransacGroup(*estimator.group_, {&estimator}, {currentFrameId}, removeOutliers)[0];
   }
   // The same for sessions of one EstimatorGroup: one okb_ransac_3d2d_batch for every session with 2 frames or more;
   // results[i] and the removals equal the single call's on sessions[i].
   std::vector<int> runRansac3d2d(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& currentFrameIds,
                                  bool removeOutliers = true) {
-    return ransacGroup(&group, sessions, currentFrameIds, removeOutliers);
+    group.validate(sessions);
+    return ransacGroup(group, sessions, currentFrameIds, removeOutliers);
   }
 
   // ---- one frame of Frontend::dataAssociationAndInitialization (Frontend.cpp:117-271)
@@ -294,7 +302,7 @@ class Frontend {
                                                const std::vector<std::vector<bool>>& overlap, bool* asKeyframe,
                                                const RansacHooks& hooks = {}) {
     std::vector<char> init{(char)(isInitialized_ ? 1 : 0)}, kf{(char)(*asKeyframe ? 1 : 0)};
-    FrameResult r = associateGroup(nullptr, {&estimator}, {frameId}, {newId}, overlap, kf, hooks, init)[0];
+    FrameResult r = associateGroup(*estimator.group_, {&estimator}, {frameId}, {newId}, overlap, kf, hooks, init)[0];
     isInitialized_ = init[0] != 0;
     *asKeyframe = kf[0] != 0;
     return r;
@@ -308,11 +316,13 @@ class Frontend {
                                                             const std::vector<std::vector<bool>>& overlap, std::vector<char>& asKeyframe,
                                                             const RansacHooks& hooks, std::vector<char>& initialized) {
     group.validate(sessions);
-    return associateGroup(&group, sessions, frameIds, newIds, overlap, asKeyframe, hooks, initialized);
+    return associateGroup(group, sessions, frameIds, newIds, overlap, asKeyframe, hooks, initialized);
   }
 
  private:
-  std::vector<bool> keyframeGroup(EstimatorGroup* group, const std::vector<const Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+  // The bodies of the calls above, for a list the group form has validated (a single form lists its session alone
+  // and passes the session's group, the group of one of a standalone Estimator included).
+  std::vector<bool> keyframeGroup(EstimatorGroup& group, const std::vector<const Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                   const std::vector<char>& initialized, std::vector<std::vector<okb_keyframe_cam>>* cams,
                                   std::vector<okb_keyframe_result>* results) {
     const size_t n = sessions.size();
@@ -329,9 +339,7 @@ class Frontend {
       jobs.push_back(j);
     }
     if (!jobs.empty()) {
-      okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
-      if (okb_keyframe_overlap_batch(ctx, (int)jobs.size(), jobs.data()) != OKB_OK)
-        throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+      throwIfFailed(group.ctx_, okb_keyframe_overlap_batch(group.ctx_, (int)jobs.size(), jobs.data()));
       for (size_t i = 0; i < n; ++i) if (!c[i].empty()) need[i] = r[i].need_keyframe != 0;
     }
     if (cams) *cams = c;
@@ -339,7 +347,7 @@ class Frontend {
     return need;
   }
 
-  std::vector<FrameResult> associateGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+  std::vector<FrameResult> associateGroup(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                           const std::vector<std::function<uint64_t()>>& newIds, const std::vector<std::vector<bool>>& overlap,
                                           std::vector<char>& asKeyframe, const RansacHooks& hooks, std::vector<char>& initialized) {
     const size_t n = sessions.size();
@@ -423,74 +431,44 @@ class Frontend {
     return out;
   }
 
-  std::vector<TrackResult> match2D2DGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+  std::vector<TrackResult> match2D2DGroup(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                           const std::vector<std::function<uint64_t()>>& newIds, bool keyframes,
                                           const std::function<void(size_t, size_t, uint64_t)>& afterKeyframe,
                                           const std::function<void(const std::vector<size_t>&)>& firstKeyframeDone = {}) {
     const size_t n = sessions.size();
     if (frameIds.size() != n || newIds.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one id source per session");
-    if (group) group->validate(sessions);
-    // per session its rounds (frame A, camera), in the reference's order; `last` closes a keyframe's rounds
-    struct Round { uint64_t frameA; size_t cam, kf; bool last; };
-    std::vector<std::vector<Round>> rounds(n);
+    std::vector<std::vector<Estimator::TrackRound>> rounds(n);
     size_t R = 0;
     for (size_t i = 0; i < n; ++i) {
-      const Estimator& e = *sessions[i];
-      if (e.numFrames() < 2) continue;                 // just starting (Frontend.cpp:381-384, 470-473)
-      const size_t C = e.cameras_.size();
-      if (keyframes) {
-        for (size_t age = 1, kf = 0; age < e.numFrames() && kf < 2; ++age) {
-          const uint64_t id = e.frameIdByAge(age);
-          if (!e.isKeyframe(id)) continue;
-          for (size_t im = 0; im < C; ++im) rounds[i].push_back(Round{id, im, kf, im + 1 == C});
-          ++kf;
-        }
-      } else {
-        const uint64_t last = e.frameIdByAge(1);
-        if (!e.isKeyframe(last))
-          for (size_t im = 0; im < C; ++im) rounds[i].push_back(Round{last, im, 0, false});
-      }
+      rounds[i] = sessions[i]->olderFrameRounds(keyframes, 2);
       R = std::max(R, rounds[i].size());
     }
     std::vector<TrackResult> out(n);
     for (size_t r = 0; r < R; ++r) {
-      std::vector<Estimator::Match2D2DPlan> plans(n);
-      std::vector<char> has(n, 0);
-      std::vector<okb_match2d2d_job> jobs;
-      for (size_t i = 0; i < n; ++i) {
-        if (r >= rounds[i].size()) continue;
-        const Round& rd = rounds[i][r];
-        has[i] = sessions[i]->plan2D2D(rd.frameA, rd.cam, frameIds[i], rd.cam, (float)briskMatchingThreshold_, plans[i]);
-        if (has[i]) jobs.push_back(plans[i].job);
-      }
-      if (!jobs.empty()) {
-        okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
-        if (okb_match2d2d_batch(ctx, (int)jobs.size(), jobs.data()) != OKB_OK)
-          throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
-      }
-      for (size_t i = 0; i < n; ++i) if (has[i]) out[i].numMatches += sessions[i]->finish2D2D(plans[i], newIds[i]);
-      if (firstKeyframeDone) {                         // the sessions whose first keyframe's rounds end here, before afterKeyframe
+      const std::vector<int> m = match2D2DRound(group, sessions, frameIds, rounds, r, newIds);
+      for (size_t i = 0; i < n; ++i) out[i].numMatches += m[i];
+      // the sessions whose round r is the last camera's of a keyframe: the end of keyframe r / C's rounds
+      std::vector<size_t> closing;
+      for (size_t i = 0; i < n; ++i)
+        if (keyframes && r < rounds[i].size() && rounds[i][r].camA + 1 == sessions[i]->cameras_.size()) closing.push_back(i);
+      if (firstKeyframeDone) {                         // those whose first keyframe's rounds end here, before afterKeyframe
         std::vector<size_t> done;
-        for (size_t i = 0; i < n; ++i)
-          if (r < rounds[i].size() && rounds[i][r].last && rounds[i][r].kf == 0) done.push_back(i);
+        for (size_t i : closing) if (r < sessions[i]->cameras_.size()) done.push_back(i);
         if (!done.empty()) firstKeyframeDone(done);
       }
       if (afterKeyframe)
-        for (size_t i = 0; i < n; ++i)
-          if (r < rounds[i].size() && rounds[i][r].last) afterKeyframe(i, rounds[i][r].kf, rounds[i][r].frameA);
+        for (size_t i : closing) afterKeyframe(i, r / sessions[i]->cameras_.size(), rounds[i][r].frameA);
     }
     for (size_t i = 0; i < n; ++i)
       for (size_t c = 0; c < sessions[i]->cameras_.size(); ++c) out[i].landmarkIds.push_back(sessions[i]->frameLandmarkIds(frameIds[i], c));
     return out;
   }
 
-  std::vector<TrackResult> stereoGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+  std::vector<TrackResult> stereoGroup(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                        const std::vector<std::function<uint64_t()>>& newIds, const std::vector<std::vector<bool>>& overlap) {
     const size_t n = sessions.size();
     if (frameIds.size() != n || newIds.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one id source per session");
-    if (group) group->validate(sessions);
     if (n == 0) return {};
-    okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
     const size_t C = sessions[0]->cameras_.size();
     if (overlap.size() < C) throw std::invalid_argument("okvis_b200: matchStereo: overlap must be numCameras x numCameras");
     for (size_t i = 0; i < n; ++i) {
@@ -501,35 +479,55 @@ class Frontend {
     for (size_t im0 = 0; im0 < C; ++im0)
       for (size_t im1 = im0 + 1; im1 < C; ++im1) {
         if (overlap[im0].size() < C || !overlap[im0][im1]) continue;
-        // the 2D-2D match (:532-546)
-        std::vector<Estimator::Match2D2DPlan> sp(n);
-        std::vector<char> hs(n, 0);
-        std::vector<okb_match2d2d_job> sj;
-        for (size_t i = 0; i < n; ++i) {
-          hs[i] = sessions[i]->plan2D2D(frameIds[i], im0, frameIds[i], im1, (float)briskMatchingThreshold_, sp[i]);
-          if (hs[i]) sj.push_back(sp[i].job);
-        }
-        if (!sj.empty() && okb_match2d2d_batch(ctx, (int)sj.size(), sj.data()) != OKB_OK)
-          throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
-        for (size_t i = 0; i < n; ++i) if (hs[i]) sessions[i]->finish2D2D(sp[i], newIds[i]);
-        // the 3D-2D and 2D-3D passes of the same pair (:547-553)
-        std::vector<Estimator::TrackPlan> tp(n);
-        std::vector<char> ht(n, 0);
-        std::vector<okb_track_job> tj;
-        for (size_t i = 0; i < n; ++i) {
-          const std::vector<Estimator::TrackRound> rounds{{frameIds[i], im0, im1}, {frameIds[i], im1, im0}};
-          ht[i] = sessions[i]->planTrackRounds(frameIds[i], rounds, (float)briskMatchingThreshold_, tp[i]);
-          if (ht[i]) tj.push_back(tp[i].job);
-        }
-        if (!tj.empty() && okb_track_3d2d_batch(ctx, (int)tj.size(), tj.data()) != OKB_OK)
-          throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
-        for (size_t i = 0; i < n; ++i) if (ht[i]) sessions[i]->finishTrack(tp[i], out[i].numMatches, out[i].numUncertainMatches);
+        // the pair's rounds: the 2D-2D match (:532-546) is the first, the 3D-2D and 2D-3D passes (:547-553) are both
+        std::vector<std::vector<Estimator::TrackRound>> rounds(n);
+        for (size_t i = 0; i < n; ++i) rounds[i] = {{frameIds[i], im0, im1}, {frameIds[i], im1, im0}};
+        match2D2DRound(group, sessions, frameIds, rounds, 0, newIds);
+        track3D2D(group, sessions, frameIds, rounds, out);
       }
     for (size_t i = 0; i < n; ++i) {
       sessions[i]->nameRemainingKeypoints(frameIds[i], newIds[i]);
       for (size_t c = 0; c < C; ++c) out[i].landmarkIds.push_back(sessions[i]->frameLandmarkIds(frameIds[i], c));
     }
     return out;
+  }
+
+  // One 2D-2D round for many sessions: session i matches its round rounds[i][r] (none when r is past its rounds) into
+  // its frame frameIds[i] -- plan2D2D per session, one okb_match2d2d_batch, finish2D2D per session in list order (new
+  // landmarks take newIds[i]()).  Returns each session's numMatches_ of the round.
+  std::vector<int> match2D2DRound(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                  const std::vector<std::vector<Estimator::TrackRound>>& rounds, size_t r,
+                                  const std::vector<std::function<uint64_t()>>& newIds) {
+    const size_t n = sessions.size();
+    std::vector<Estimator::Match2D2DPlan> plans(n);
+    std::vector<char> has(n, 0);
+    std::vector<okb_match2d2d_job> jobs;
+    for (size_t i = 0; i < n; ++i) {
+      if (r >= rounds[i].size()) continue;
+      const Estimator::TrackRound& rd = rounds[i][r];
+      has[i] = sessions[i]->plan2D2D(rd.frameA, rd.camA, frameIds[i], rd.camB, (float)briskMatchingThreshold_, plans[i]);
+      if (has[i]) jobs.push_back(plans[i].job);
+    }
+    if (!jobs.empty()) throwIfFailed(group.ctx_, okb_match2d2d_batch(group.ctx_, (int)jobs.size(), jobs.data()));
+    std::vector<int> numMatches(n, 0);
+    for (size_t i = 0; i < n; ++i) if (has[i]) numMatches[i] = sessions[i]->finish2D2D(plans[i], newIds[i]);
+    return numMatches;
+  }
+  // One 3D-2D call for many sessions: session i tracks its frame frameIds[i] in the rounds rounds[i] (planTrackRounds
+  // per session; one whose rounds all lack features sits out), one okb_track_3d2d_batch, finishTrack per session in
+  // list order, its counts added to out[i].
+  void track3D2D(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                 const std::vector<std::vector<Estimator::TrackRound>>& rounds, std::vector<TrackResult>& out) {
+    const size_t n = sessions.size();
+    std::vector<Estimator::TrackPlan> plans(n);
+    std::vector<char> has(n, 0);
+    std::vector<okb_track_job> jobs;
+    for (size_t i = 0; i < n; ++i) {
+      has[i] = sessions[i]->planTrackRounds(frameIds[i], rounds[i], (float)briskMatchingThreshold_, plans[i]);
+      if (has[i]) jobs.push_back(plans[i].job);
+    }
+    if (!jobs.empty()) throwIfFailed(group.ctx_, okb_track_3d2d_batch(group.ctx_, (int)jobs.size(), jobs.data()));
+    for (size_t i = 0; i < n; ++i) if (has[i]) sessions[i]->finishTrack(plans[i], out[i].numMatches, out[i].numUncertainMatches);
   }
 
   // R_CW = C_WC^T from the quaternion of T_WC
@@ -551,12 +549,11 @@ class Frontend {
     return p;
   }
 
-  std::vector<std::vector<std::vector<okb_keypoint>>> detectStoreGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions,
+  std::vector<std::vector<std::vector<okb_keypoint>>> detectStoreGroup(EstimatorGroup& group, const std::vector<Estimator*>& sessions,
                                                                        const std::vector<uint64_t>& frameIds,
                                                                        const std::vector<std::vector<CameraImage>>& images) {
     const size_t n = sessions.size();
     if (frameIds.size() != n || images.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one image list per session");
-    if (group) group->validate(sessions);
     const okb_detect_params prm = detectParams();
     for (size_t i = 0; i < n; ++i) sessions[i]->checkDetectStore(frameIds[i], images[i].size(), prm);   // before any device work
     std::vector<Estimator::DetectStorePlan> plans(n);
@@ -575,20 +572,18 @@ class Frontend {
     }
     std::vector<std::vector<std::vector<okb_keypoint>>> out(n);
     if (n == 0) return out;
-    okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
-    const int rc = okb_detect_describe_store_batch(ctx, (int)n, jobs.data(), &prm, prm.max_keypoints, 0);
-    if (rc != OKB_OK && rc != OKB_ERR_CAPACITY) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+    const int rc = okb_detect_describe_store_batch(group.ctx_, (int)n, jobs.data(), &prm, prm.max_keypoints, 0);
+    if (rc != OKB_ERR_CAPACITY) throwIfFailed(group.ctx_, rc);
     for (size_t i = 0; i < n; ++i) out[i] = sessions[i]->finishDetectStore(plans[i]);   // the store and the host agree, also on capacity
-    if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
+    throwIfFailed(group.ctx_, rc);
     isInitialized_ = true;
     return out;
   }
 
-  std::vector<int> ransacGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+  std::vector<int> ransacGroup(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                bool removeOutliers) {
     const size_t n = sessions.size();
     if (frameIds.size() != n) throw std::invalid_argument("okvis_b200: one current frame id per session");
-    if (group) group->validate(sessions);
     std::vector<int> out(n, 1);                        // nothing to match against, just starting (:579-582)
     std::vector<Estimator::RansacPlan> plans(n);
     std::vector<char> has(n, 0);
@@ -599,52 +594,21 @@ class Frontend {
       has[i] = 1;
       jobs.push_back(plans[i].job);
     }
-    if (!jobs.empty()) {
-      okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
-      if (okb_ransac_3d2d_batch(ctx, (int)jobs.size(), jobs.data()) != OKB_OK)
-        throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
-    }
+    if (!jobs.empty()) throwIfFailed(group.ctx_, okb_ransac_3d2d_batch(group.ctx_, (int)jobs.size(), jobs.data()));
     for (size_t i = 0; i < n; ++i) if (has[i]) out[i] = sessions[i]->finishRansac3d2d(plans[i], removeOutliers);
     return out;
   }
 
-  std::vector<TrackResult> trackGroup(EstimatorGroup* group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+  std::vector<TrackResult> trackGroup(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                       bool keyframes) {
     if (sessions.size() != frameIds.size()) throw std::invalid_argument("okvis_b200: one current frame id per session");
-    if (group) group->validate(sessions);
     const size_t n = sessions.size();
-    std::vector<Estimator::TrackPlan> plans(n);
-    std::vector<char> has(n, 0);
-    std::vector<okb_track_job> jobs;
-    for (size_t i = 0; i < n; ++i) {
-      Estimator& e = *sessions[i];
-      if (e.numFrames() < 2) continue;                 // just starting (Frontend.cpp:381-384, 470-473)
-      std::vector<uint64_t> frameA;
-      if (keyframes) {
-        for (size_t age = 1, kf = 0; age < e.numFrames() && kf < 3; ++age) {
-          const uint64_t id = e.frameIdByAge(age);
-          if (!e.isKeyframe(id)) continue;
-          frameA.push_back(id);
-          ++kf;
-        }
-      } else {
-        const uint64_t last = e.frameIdByAge(1);
-        if (!e.isKeyframe(last)) frameA.push_back(last);
-      }
-      has[i] = e.planTrack(frameIds[i], frameA, (float)briskMatchingThreshold_, plans[i]);
-    }
-    for (size_t i = 0; i < n; ++i) if (has[i]) jobs.push_back(plans[i].job);
-    if (!jobs.empty()) {
-      okb_ctx* ctx = group ? group->ctx_ : sessions[0]->ctx_;
-      const int rc = okb_track_3d2d_batch(ctx, (int)jobs.size(), jobs.data());
-      if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx));
-    }
+    std::vector<std::vector<Estimator::TrackRound>> rounds(n);
+    for (size_t i = 0; i < n; ++i) rounds[i] = sessions[i]->olderFrameRounds(keyframes, 3);
     std::vector<TrackResult> out(n);
-    for (size_t i = 0; i < n; ++i) {
-      Estimator& e = *sessions[i];
-      if (has[i]) e.finishTrack(plans[i], out[i].numMatches, out[i].numUncertainMatches);
-      for (size_t c = 0; c < e.cameras_.size(); ++c) out[i].landmarkIds.push_back(e.frameLandmarkIds(frameIds[i], c));
-    }
+    track3D2D(group, sessions, frameIds, rounds, out);
+    for (size_t i = 0; i < n; ++i)
+      for (size_t c = 0; c < sessions[i]->cameras_.size(); ++c) out[i].landmarkIds.push_back(sessions[i]->frameLandmarkIds(frameIds[i], c));
     return out;
   }
 
@@ -713,7 +677,7 @@ class DenseMatcher {
       colIdx.resize(cap); dist.resize(cap);
       const int rc = okb_hamming_candidates(ctx_, A, nA, B, nB, descriptorBytes, threshold, rowPtr.data(), colIdx.data(), dist.data(), (int)cap);
       if (rc == OKB_OK) { colIdx.resize(rowPtr[nA]); dist.resize(rowPtr[nA]); return; }
-      if (rc != OKB_ERR_CAPACITY) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx_));
+      if (rc != OKB_ERR_CAPACITY) throwIfFailed(ctx_, rc);
       cap = rowPtr[nA];
     }
     throw std::runtime_error("okvis_b200: candidate capacity");
@@ -735,7 +699,7 @@ class DenseMatcher {
                         : okb_hamming_match(ctx_, matchingAlgorithm.descriptorsA(), nA, matchingAlgorithm.descriptorsB(), nB,
                                             matchingAlgorithm.descriptorBytes(), skipA.data(), skipB.data(), thr, numBest_, 0, 0.f, topk.data(),
                                             pairs.data());
-    if (rc != OKB_OK) throw std::runtime_error(std::string("okvis_b200: ") + okb_last_error(ctx_));
+    throwIfFailed(ctx_, rc);
     // epilogue of matchBody (implementation/DenseMatcher.hpp:92-122), ascending B
     matchingAlgorithm.reserveMatches((size_t)nB);
     const distance_t ratio = matchingAlgorithm.distanceRatioThreshold();
