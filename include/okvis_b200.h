@@ -60,7 +60,8 @@ typedef enum {
   OKB_ERR_UNSUPPORTED = -3,   /* e.g. non-fixed extrinsics in the device solver */
   OKB_ERR_CAPACITY = -4,      /* window larger than the compiled-in limits */
   OKB_ERR_NO_DEVICE = -5,
-  OKB_ERR_NUMERIC = -6        /* solver failure (all windows report in summary) */
+  OKB_ERR_NUMERIC = -6,       /* solver failure (all windows report in summary) */
+  OKB_ERR_SHARD_TIMEOUT = -7  /* a peer rank of a landmark-sharded window did not arrive at an exchange (status 7) */
 } okb_status;
 
 /* --------------------------------------------------------------- basic PODs */
@@ -415,8 +416,29 @@ int okb_window_download_slots(okb_ctx* ctx, int n, const int32_t* slots, double*
  *   multi-process (one process per GPU): okb_shard_export on every rank, exchange the OKB_SHARD_HANDLE_BYTES-byte
  *     handles out of band (e.g. torch.distributed.all_gather), okb_shard_connect with all `world` handles in rank order.
  *   single process driving several contexts (same or different devices): okb_shard_connect_local.
- * max_frames bounds the keyframes of any sharded window (mailbox sizing). */
+ * max_frames bounds the keyframes of any sharded window (mailbox sizing).
+ *
+ * The frontend calls on the feature store (okb_detect_describe_store_batch, okb_track_3d2d_batch, okb_match2d2d_batch,
+ * okb_stereo_init_batch, okb_keyframe_overlap_batch, okb_ransac_3d2d_batch) run on a sharded window when the context
+ * reserved its global landmark slots with okb_shard_reserve_landmarks before okb_shard_export / okb_shard_connect_local
+ * (otherwise they return OKB_ERR_UNSUPPORTED).  The feature store is replicated: every rank reserves it and receives
+ * the same store edits (okb_window_reserve_features, okb_window_set_features, okb_window_set_feature_landmarks,
+ * okb_window_clear_features), whose landmark slots are GLOBAL slots below max_landmarks.  okb_window_set_landmark_-
+ * initialized is landmark state and goes to the owner (rank g mod world) at its local slot g div world, as
+ * okb_window_set_landmarks does.  Every rank makes the same call with the same arguments, concurrently (one host thread
+ * or process per rank: the calls return only after their device work); track, 2D-2D, stereo initialisation and RANSAC
+ * 3D-2D first all-gather the landmark state they read (point, observation count, initialised flag; 40 bytes per global
+ * slot, double-buffered) over the mailbox, and return OKB_ERR_SHARD_TIMEOUT (status 7) if a peer does not arrive
+ * within the solver's time-out.  Every rank returns the same results as an unsharded context holding the whole
+ * window; landmark slots in them are global, and edits derived from them are routed like any other.  A landmark
+ * removed on its owner is forgotten by every rank's store at the next exchange. */
 #define OKB_SHARD_HANDLE_BYTES 64
+/* Global landmark slots of the frontend's landmark replica (0: none, the default); before okb_shard_export /
+ * okb_shard_connect_local.  Adds 2 * 40 * max_landmarks bytes to each window's mailbox on every rank. */
+int okb_shard_reserve_landmarks(okb_ctx* ctx, int max_landmarks);
+/* Mailbox bytes of one window slot on every rank (no context needed): out[0] = offset of the landmark replica,
+ * out[1] = its bytes (2 * 40 * max_landmarks), out[2] = the slot's whole mailbox (256-byte aligned). */
+int okb_shard_mailbox_layout(int world, int max_frames, int max_landmarks, uint64_t out[3]);
 int okb_shard_export(okb_ctx* ctx, int rank, int world, int max_frames, void* handle_out /* OKB_SHARD_HANDLE_BYTES */);
 int okb_shard_connect(okb_ctx* ctx, const void* handles /* [world][OKB_SHARD_HANDLE_BYTES] */);
 int okb_shard_connect_local(okb_ctx* const* ctxs /* [world], rank order */, int world, int max_frames);
@@ -640,7 +662,12 @@ int okb_hamming_candidates(okb_ctx* ctx, const uint8_t* A, int nA, const uint8_t
  * okb_window_reserve and before the slot's first upload, which then sizes the window's command buffer for one frame's
  * features on top of a full upload (OKB_ERR_CAPACITY if the slot was uploaded without); the initialised flags cover
  * the landmark capacity the slot has then.  Calling it again with other sizes commits what is pending and replaces the
- * store by an empty one (waiting for the device). */
+ * store by an empty one (waiting for the device).
+ * Landmark-sharded windows (okb_shard_reserve_landmarks): the store is replicated -- every rank reserves it alike and
+ * receives the same okb_window_reserve_features / set_features / set_feature_landmarks / clear_features calls, whose
+ * landmark slots are GLOBAL slots (below max_landmarks, else OKB_ERR_INVALID_ARG) -- while the initialised flags are
+ * landmark state: each rank's cover its own landmarks at their local slots (okb_window_set_landmark_initialized goes
+ * to the owner only).  A removal on the owner reaches the other ranks' stores at the next landmark exchange. */
 int okb_window_reserve_features(okb_ctx* ctx, int win, int max_feature_frames, int max_cameras, int max_keypoints,
                                 int desc_bytes);
 /* Replaces the keypoints of (feat_slot, cam): n keypoints (x, y, size are used), their descriptors [n][desc_bytes],
@@ -696,7 +723,8 @@ typedef struct okb_track_job {
  * window, store reserved, feature slots present, ranges of cameras, poses, speed/bias, num_best <= 8, output
  * capacities, one descriptor length per call, a window listed twice, a round of frame B against itself in one
  * camera): the first failure returns OKB_ERR_INVALID_ARG
- * and names the job in okb_last_error.  A landmark-sharded context returns OKB_ERR_UNSUPPORTED.  Pending edits of the
+ * and names the job in okb_last_error.  A landmark-sharded context runs it as described with okb_shard_reserve_landmarks
+ * (without that reservation: OKB_ERR_UNSUPPORTED).  Pending edits of the
  * job windows are committed first, one commit per run of consecutive windows; the call then runs on the transfer stream after the solver work already launched on
  * those windows only, with one H2D copy of the job table and one D2H copy of the results, and returns when they are
  * back.  Later solver calls on those windows are ordered after it.  n_jobs == 0 is a no-op. */
@@ -733,7 +761,9 @@ typedef struct okb_stereo_job {
  * checked on the host before any device work (uploaded window, store reserved, the feature slot present for both
  * cameras, cam_a != cam_b in range, pose in range, num_best <= 8, out_cap, one descriptor length per call, a window
  * listed twice): the first failure returns OKB_ERR_INVALID_ARG and names the job in okb_last_error.  A landmark-sharded
- * context returns OKB_ERR_UNSUPPORTED.  Pending edits of the job windows are committed first; the call runs on the
+ * context runs it as described with okb_shard_reserve_landmarks (landmark exchange first; OKB_ERR_SHARD_TIMEOUT if a
+ * peer does not arrive; without that reservation OKB_ERR_UNSUPPORTED).  Pending edits of the job windows are committed
+ * first; the call runs on the
  * transfer stream after the solver work already launched on those windows, with one H2D copy of the job table and one
  * D2H copy of the results, and returns when they are back.  n_jobs == 0 is a no-op.  It runs as okb_match2d2d_batch
  * with frame A = frame B. */
@@ -768,7 +798,9 @@ typedef struct okb_match2d2d_job {
  * returning OKB_ERR_INVALID_ARG and naming the job: uploaded window, store reserved, both feature slots present for their
  * cameras; cameras, poses and sb_current in range; feat_slot_a == feat_slot_b exactly when pose_a == pose_b; no match of
  * one frame against itself in one camera; num_best <= 8; out_cap; one descriptor length per call; a window listed twice.
- * A landmark-sharded context returns OKB_ERR_UNSUPPORTED; n_jobs == 0 is a no-op.  The call changes nothing in the window,
+ * A landmark-sharded context runs it as described with okb_shard_reserve_landmarks (landmark exchange first;
+ * OKB_ERR_SHARD_TIMEOUT if a peer does not arrive; without that reservation OKB_ERR_UNSUPPORTED); n_jobs == 0 is a
+ * no-op.  The call changes nothing in the window,
  * its store or its flags; commits, stream order and copies are those of okb_stereo_init_batch (four launches, one H2D
  * copy of the job table, one D2H copy of the results). */
 int okb_match2d2d_batch(okb_ctx* ctx, int n_jobs, const okb_match2d2d_job* jobs);
@@ -803,8 +835,9 @@ typedef struct okb_keyframe_job {
  * in camera order (std::max(value, running): a NaN value wins, a NaN running maximum is replaced) and the decision.
  * Every job is checked on the host before any device work (uploaded window, store reserved, n_cams in 1..the store's
  * cameras, the feature slot present for each of them, cams and out present, a window listed twice): the first failure
- * returns OKB_ERR_INVALID_ARG and names the job in okb_last_error.  A landmark-sharded context returns
- * OKB_ERR_UNSUPPORTED.  Pending edits of the job windows are committed first (2D-2D bookkeeping and RANSAC removals
+ * returns OKB_ERR_INVALID_ARG and names the job in okb_last_error.  A landmark-sharded context runs it as described with
+ * okb_shard_reserve_landmarks (landmark exchange first; OKB_ERR_SHARD_TIMEOUT if a peer does not arrive; without that
+ * reservation OKB_ERR_UNSUPPORTED).  Pending edits of the job windows are committed first (2D-2D bookkeeping and RANSAC removals
  * arrive as store edits just before the decision); the call runs on the transfer stream after the solver work already
  * launched on those windows, with one H2D copy of the job table and one D2H copy of the results, returns when they are
  * back and changes nothing in the window or its store.  Results per job are bit-identical to calling it alone.
@@ -847,7 +880,9 @@ typedef struct okb_ransac_job {
  * reserved, n_cams in 1..the store's, the window's extrinsics and cameras (at most 16), the feature slot present for
  * each camera, max_iterations in 1..64, a finite positive threshold, out present, outlier capacity, a window listed
  * twice): the first failure returns OKB_ERR_INVALID_ARG and names the job in okb_last_error.  A landmark-sharded context
- * returns OKB_ERR_UNSUPPORTED.  Pending edits of the job windows are committed first (removals from earlier rounds);
+ * runs it as described with okb_shard_reserve_landmarks (landmark exchange first; OKB_ERR_SHARD_TIMEOUT if a peer does
+ * not arrive; without that reservation OKB_ERR_UNSUPPORTED).  Pending edits of the job windows are committed first
+ * (removals from earlier rounds);
  * the call runs on the transfer stream after the solver work already launched on those windows, with one H2D copy of
  * the job table and one D2H copy of the results, returns when they are back and changes nothing in the window or its
  * store: the caller applies the removals.  Results per job are bit-identical to calling it alone.  n_jobs == 0 is a
@@ -876,7 +911,8 @@ typedef struct okb_detect_store_job {
  * in 1..the store's cameras, params->desc_bytes = the store's descriptor length, the store's keypoints per image >=
  * min(max_keypoints, max_out), out_kp and n_out present, each image as okb_detect_describe_batch checks it, at most
  * 65535 images in all, a window listed twice): the first failure returns OKB_ERR_INVALID_ARG and names the job in
- * okb_last_error.  A landmark-sharded context returns OKB_ERR_UNSUPPORTED; n_jobs == 0 is a no-op.
+ * okb_last_error.  A landmark-sharded context runs it as described with okb_shard_reserve_landmarks (every rank
+ * detects redundantly into its replicated store; without that reservation OKB_ERR_UNSUPPORTED); n_jobs == 0 is a no-op.
  * Pending edits of the job windows are committed first, and the store writes are ordered after that commit and after
  * the solver work already launched on those windows: a clear of the slot queued before the call does not erase the new
  * features, one queued after it does.  The detection runs as okb_detect_describe_batch over all images of the call (its

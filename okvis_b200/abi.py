@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libokvis_b200.so")
 OKB_OK = 0
 OKB_ERR_INVALID_ARG, OKB_ERR_CUDA, OKB_ERR_UNSUPPORTED, OKB_ERR_CAPACITY, OKB_ERR_NO_DEVICE, OKB_ERR_NUMERIC = (
     -1, -2, -3, -4, -5, -6)
+OKB_ERR_SHARD_TIMEOUT = -7
 DIST_NONE, DIST_RADTAN, DIST_EQUIDISTANT, DIST_RADTAN8 = 0, 1, 2, 3
 BLOCK_POSE, BLOCK_SPEED_BIAS, BLOCK_EXTRINSICS = 0, 1, 2
 IMU_TERM_OUT = 931      # OKB_IMU_TERM_OUT: doubles per term of okb_debug_imu_terms (H30 | g30 | cost)

@@ -87,9 +87,11 @@ class Context:
                     quality_ms=out[4], quality_launches=int(out[5]))
 
     # ---------------------------------------------------------------- landmark-sharded window (multi-GPU)
-    def shard_export(self, rank, world, max_frames=32):
-        """okb_shard_export: allocates this rank's mailbox; returns the 64-byte IPC handle (numpy uint8)."""
+    def shard_export(self, rank, world, max_frames=32, max_landmarks=0):
+        """okb_shard_export: allocates this rank's mailbox; returns the 64-byte IPC handle (numpy uint8).  max_landmarks > 0
+        also reserves the landmark replica of the frontend calls for that many global landmark slots."""
         h = np.zeros(64, np.uint8)
+        self._check(lib().okb_shard_reserve_landmarks(self._h, int(max_landmarks)))
         self._check(lib().okb_shard_export(self._h, int(rank), int(world), int(max_frames), _p(h)))
         return h
 
@@ -98,11 +100,22 @@ class Context:
         self._check(lib().okb_shard_connect(self._h, _p(h)))
 
     @staticmethod
-    def shard_connect_local(ctxs, max_frames=32):
+    def shard_connect_local(ctxs, max_frames=32, max_landmarks=0):
+        for c in ctxs:
+            c._check(lib().okb_shard_reserve_landmarks(c._h, int(max_landmarks)))
         arr = (C.c_void_p * len(ctxs))(*[c._h for c in ctxs])
         rc = lib().okb_shard_connect_local(arr, len(ctxs), int(max_frames))
         if rc != 0:
             raise OkbError(rc, "; ".join(lib().okb_last_error(c._h).decode() for c in ctxs))
+
+    @staticmethod
+    def shard_mailbox_layout(world, max_frames, max_landmarks):
+        """okb_shard_mailbox_layout: (landmark replica offset, replica bytes, mailbox bytes) of one window slot."""
+        out = np.zeros(3, np.uint64)
+        rc = lib().okb_shard_mailbox_layout(int(world), int(max_frames), int(max_landmarks), _p(out))
+        if rc != 0:
+            raise OkbError(rc, "okb_shard_mailbox_layout: invalid arguments")
+        return tuple(int(x) for x in out)
 
     def shard_stats(self, win=0):
         out = np.zeros(4)
@@ -518,7 +531,8 @@ class Context:
             d.img = img.ctypes.data
             d.height, d.width = img.shape
             d.stride = img.strides[0]
-            C.memmove(C.addressof(d.cam), np.array([cam], abi.camera_dtype).ctypes.data, C.sizeof(abi.Camera))
+            ca = np.array([cam], abi.camera_dtype)      # held until the copy: callers may run on several threads
+            C.memmove(C.addressof(d.cam), ca.ctypes.data, C.sizeof(abi.Camera))
             for k, v in enumerate(np.asarray(R, dtype=np.float64).reshape(9)):
                 d.R_CW[k] = float(v)
         return descs, keep

@@ -140,6 +140,7 @@ struct okb_ctx {
   okb_frontend_state* frontend = nullptr;
   // landmark-sharded windows (okb_shard_*): this rank's mailbox and the peers' mailboxes as mapped on this device
   int shard_rank = 0, shard_world = 1, shard_box_cap = 0, shard_marg_cap = 0;
+  int shard_lm_cap = 0;                                       // global landmark slots of the frontend's replica
   size_t shard_win_bytes = 0;
   unsigned char* shard_local = nullptr;                       // cudaMalloc'ed, exported through cudaIpc
   unsigned char* shard_peer[okb::kMaxShard] = {};             // [rank]; own entry = shard_local

@@ -570,6 +570,7 @@ static int upload_pack(okb_ctx* c, int win, const okb_window_desc* D) {
   W.imu_params = D->imu_params;
   derive_dims(W);
   W.shard_rank = c->shard_rank; W.shard_world = c->shard_world; W.shard_box_cap = c->shard_box_cap; W.shard_marg_cap = c->shard_marg_cap;
+  W.shard_lm_cap = c->shard_lm_cap;
   if (c->shard_world > 1) {
     if (shard_box_doubles(K, W.dcp) > (size_t)c->shard_box_cap) { c->set_error("window exceeds the shard mailbox (max_frames of okb_shard_export)"); return OKB_ERR_CAPACITY; }
     for (int r = 0; r < c->shard_world; ++r) {
@@ -912,6 +913,17 @@ extern "C" int okb_window_reserve_features(okb_ctx* c, int win, int max_feature_
   return OKB_OK;
 }
 
+// A landmark-sharded store names global landmark slots: each must lie below the replica's global slot count.
+static int store_slots_invalid(okb_ctx* c, const int32_t* lm_slot, int n, const char* who) {
+  if (c->shard_world < 2 || !lm_slot) return OKB_OK;
+  for (int i = 0; i < n; ++i)
+    if (lm_slot[i] >= c->shard_lm_cap) {
+      c->set_error(std::string(who) + ": landmark slot beyond the sharded window's global landmark slots (okb_shard_reserve_landmarks)");
+      return OKB_ERR_INVALID_ARG;
+    }
+  return OKB_OK;
+}
+
 static int feat_begin(okb_ctx* c, int win, int feat_slot, int cam, size_t extra, WinStore** S, WinDev** W, const char* who) {
   int rc = delta_begin(c, win, extra, S, W);
   if (rc) return rc;
@@ -932,6 +944,7 @@ extern "C" int okb_window_set_features(okb_ctx* c, int win, int feat_slot, int c
   if (n > S->feat.N) { c->set_error("okb_window_set_features: more keypoints than reserved"); return OKB_ERR_CAPACITY; }
   for (int i = 0; lm_slot && i < n; ++i)
     if (lm_slot[i] < -1) { c->set_error("okb_window_set_features: landmark slot below -1"); return OKB_ERR_INVALID_ARG; }
+  if ((rc = store_slots_invalid(c, lm_slot, n, "okb_window_set_features"))) return rc;
   unsigned char* q = cmd_put(*S, CMD_SET_FEATURES, (uint32_t)n, (uint32_t)feat_slot, (uint32_t)cam, bk + bl + bo + bd);
   double* x = reinterpret_cast<double*>(q);
   for (int i = 0; i < n; ++i) { x[3 * i] = kp[i].x; x[3 * i + 1] = kp[i].y; x[3 * i + 2] = kp[i].size; }
@@ -956,6 +969,7 @@ extern "C" int okb_window_set_feature_landmarks(okb_ctx* c, int win, int feat_sl
       c->set_error("okb_window_set_feature_landmarks: keypoint index or landmark slot out of range");
       return OKB_ERR_INVALID_ARG;
     }
+  if ((rc = store_slots_invalid(c, lm_slot, n, "okb_window_set_feature_landmarks"))) return rc;
   unsigned char* q = cmd_put(*S, CMD_SET_FEATURE_LMS, (uint32_t)n, (uint32_t)feat_slot, (uint32_t)cam, 2 * b4 + b1);
   std::memcpy(q, kp_idx, 4 * (size_t)n);
   std::memcpy(q + b4, lm_slot, 4 * (size_t)n);
@@ -1323,7 +1337,7 @@ static int shard_alloc(okb_ctx* c, int rank, int world, int max_frames) {
   const int dcp = 4 * ((6 * max_frames + 1 + 3) / 4);
   c->shard_box_cap = (int)shard_box_doubles(max_frames, dcp);
   c->shard_marg_cap = (int)shard_marg_box_doubles(max_frames);
-  c->shard_win_bytes = shard_win_bytes(world, (size_t)c->shard_box_cap, (size_t)c->shard_marg_cap);
+  c->shard_win_bytes = shard_win_bytes(world, (size_t)c->shard_box_cap, (size_t)c->shard_marg_cap, (size_t)c->shard_lm_cap);
   const size_t total = c->shard_win_bytes * (size_t)c->max_windows;
   OKB_CUDA(c, cudaMalloc(&c->shard_local, total));
   OKB_CUDA(c, cudaMemset(c->shard_local, 0, total));
@@ -1331,6 +1345,22 @@ static int shard_alloc(okb_ctx* c, int rank, int world, int max_frames) {
   c->shard_rank = rank;
   c->shard_world = world;
   c->shard_peer[rank] = c->shard_local;
+  return OKB_OK;
+}
+
+extern "C" int okb_shard_mailbox_layout(int world, int max_frames, int max_landmarks, uint64_t out[3]) {
+  if (world < 2 || world > kMaxShard || max_frames < 1 || max_frames > kMaxFrames || max_landmarks < 0 || !out) return OKB_ERR_INVALID_ARG;
+  const size_t box = shard_box_doubles(max_frames, 4 * ((6 * max_frames + 1 + 3) / 4)), marg = shard_marg_box_doubles(max_frames);
+  out[0] = shard_lm_offset(world, box, marg);
+  out[1] = 2 * shard_lm_half_bytes((size_t)max_landmarks);
+  out[2] = shard_win_bytes(world, box, marg, (size_t)max_landmarks);
+  return OKB_OK;
+}
+
+extern "C" int okb_shard_reserve_landmarks(okb_ctx* c, int max_landmarks) {
+  if (!c || max_landmarks < 0) return OKB_ERR_INVALID_ARG;
+  if (c->shard_local) { c->set_error("okb_shard_reserve_landmarks: call it before okb_shard_export / okb_shard_connect_local"); return OKB_ERR_INVALID_ARG; }
+  c->shard_lm_cap = max_landmarks;
   return OKB_OK;
 }
 

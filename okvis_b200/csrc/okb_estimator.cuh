@@ -80,8 +80,28 @@ constexpr size_t kShardCounter = 256;    // u32                  last-CTA counte
 constexpr size_t kShardMargEpoch = 384;  // u64                  epoch of the last marginalisation exchange (local use)
 constexpr size_t kShardScalars = 512;    // f64 [2][kMaxShard][16]
 constexpr size_t kShardFlagsM = 2560;    // u64 [2][kMaxShard]   marginalisation boxes ready
+constexpr size_t kShardFlagsL = 2688;    // u64 [2][kMaxShard]   landmark replica pushed (frontend calls)
+constexpr size_t kShardLmEpoch = 2816;   // u64                  epoch of the last landmark exchange (local use)
+constexpr size_t kShardLmCounter = 2824; // u32                  last-CTA counter of k_shard_lm_push (local use)
+constexpr size_t kShardLmStatus = 2828;  // i32                  0, or 7: a peer did not arrive (local use)
 static_assert(kShardScalars + 2 * kMaxShard * 16 * sizeof(double) <= kShardFlagsM &&
-              kShardFlagsM + 2 * kMaxShard * sizeof(unsigned long long) <= kShardHeaderBytes, "shard mailbox header layout");
+              kShardFlagsM + 2 * kMaxShard * sizeof(unsigned long long) <= kShardFlagsL &&
+              kShardFlagsL + 2 * kMaxShard * sizeof(unsigned long long) <= kShardLmEpoch &&
+              kShardLmStatus + 4 <= kShardHeaderBytes, "shard mailbox header layout");
+constexpr unsigned long long kShardTimeoutNs = 4000000000ull;   // a peer that does not arrive within 4 s: FAILURE, no hang
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ void st_release_sys_u64(unsigned long long* p, unsigned long long v) {
+  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_acquire_sys_u64(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
 __host__ __device__ inline size_t shard_box_doubles(int K, int dcp) { return (size_t)dcp * dcp + (size_t)K * 32 + 8; }
 // Marginalisation box (k_marginalize<true>): header [fingerprint, error word, epoch, pad] | pose-pose sums [P][P] | pose
 // rows of b [P], P = 6 * (pose blocks of the job) <= 6 * max_frames.  A region of [2][world] such boxes follows the
@@ -91,8 +111,25 @@ __host__ __device__ inline size_t shard_marg_box_doubles(int max_frames) {
   const size_t p = 6 * (size_t)max_frames;
   return kMargBoxHeader + p * p + p;
 }
-__host__ __device__ inline size_t shard_win_bytes(int world, size_t box_cap, size_t marg_cap) {
+// Landmark replica of the frontend calls (okb_frontend.cu): the state the store kernels read of every global landmark
+// slot g < lm_cap, all-gathered from the owners (rank g mod world, local slot g div world) at the start of a call.  A
+// region of two halves follows the marginalisation boxes, double-buffered by the parity of the exchange epoch: a peer
+// already in its next call never writes the half a rank may still be reading.  A half holds the homogeneous points
+// [lm_cap][4] (zero: not in the graph, Estimator::isLandmarkAdded) and then ShardLmAux [lm_cap]: 40 bytes per slot,
+// the half rounded up to 256 bytes.
+struct ShardLmAux {
+  int32_t n_obs;      // observations of the landmark in the graph
+  uint8_t init;       // Estimator::isLandmarkInitialized
+  uint8_t removed;    // removed since the last exchange: every rank forgets the slot's store references
+  uint8_t _pad[2];
+};
+static_assert(sizeof(ShardLmAux) == 8, "landmark replica record");
+__host__ __device__ inline size_t shard_lm_offset(int world, size_t box_cap, size_t marg_cap) {
   return (kShardHeaderBytes + 2 * (size_t)world * (box_cap + marg_cap) * sizeof(double) + 255) & ~(size_t)255;
+}
+__host__ __device__ inline size_t shard_lm_half_bytes(size_t lm_cap) { return (40 * lm_cap + 255) & ~(size_t)255; }
+__host__ __device__ inline size_t shard_win_bytes(int world, size_t box_cap, size_t marg_cap, size_t lm_cap = 0) {
+  return (shard_lm_offset(world, box_cap, marg_cap) + 2 * shard_lm_half_bytes(lm_cap) + 255) & ~(size_t)255;
 }
 
 // Everything kernels need to know about one window.  All pointers are device pointers into the
@@ -212,6 +249,7 @@ struct WinDev {
   int shard_rank, shard_world;                 // world <= 1: not sharded
   int shard_box_cap;                           // doubles per box
   int shard_marg_cap;                          // doubles per marginalisation box (shard_marg_box_doubles)
+  int shard_lm_cap;                            // global landmark slots of the replica (ShardLmAux), 0: none
   unsigned char* shard_mail[kMaxShard];       // this window's mailbox in every rank's memory, as mapped on this device
   SolverState* st;
   FeatStore* feat;                             // feature store (okb_window_reserve_features), nullptr: none

@@ -1700,11 +1700,158 @@ struct TrackJobDev {
 };
 struct TrackRoundDev { int feat_a, cam_a, cam_b, _pad; };
 
+// Landmark replica of a sharded window (ShardLmAux, okb_estimator.cuh): one half of rank `rank`'s replica, points
+// [lm_cap][4] then ShardLmAux [lm_cap].
+struct ShardLmHalf { double* x; ShardLmAux* aux; };
+__device__ __forceinline__ ShardLmHalf shard_lm_half(const WinDev& W, int rank, int par) {
+  unsigned char* h = W.shard_mail[rank] + shard_lm_offset(W.shard_world, W.shard_box_cap, W.shard_marg_cap) +
+                     (size_t)par * shard_lm_half_bytes(W.shard_lm_cap);
+  return ShardLmHalf{reinterpret_cast<double*>(h), reinterpret_cast<ShardLmAux*>(h + 32 * (size_t)W.shard_lm_cap)};
+}
+__device__ __forceinline__ unsigned long long shard_lm_epoch(const WinDev& W) {
+  return *reinterpret_cast<const unsigned long long*>(W.shard_mail[W.shard_rank] + kShardLmEpoch);
+}
+// the half of this rank's replica the current call reads (the last exchange's)
+__device__ __forceinline__ ShardLmHalf shard_lm_replica(const WinDev& W) { return shard_lm_half(W, W.shard_rank, (int)(shard_lm_epoch(W) & 1ull)); }
+
+// Per-landmark state the store kernels read, through one indexed read selected by the window: its own graph, or on a
+// landmark-sharded window the replica all-gathered at the start of the call (k_shard_lm_* below), indexed by the global
+// slots the replicated store names.
+__device__ __forceinline__ bool lm_sharded(const WinDev& W) { return W.shard_world > 1; }
+// landmark slots the call may name: the graph's, or the replica's global slots
+__device__ __forceinline__ int lm_slots(const WinDev& W) { return lm_sharded(W) ? W.shard_lm_cap : W.st->g.L; }
+// homogeneous point of slot l < lm_slots(W) (32-byte aligned)
+__device__ __forceinline__ const double* lm_point(const WinDev& W, int l) {
+  return (lm_sharded(W) ? shard_lm_replica(W).x : W.m_lm) + 4 * (size_t)l;
+}
+// Estimator::isLandmarkInitialized of slot l
+__device__ __forceinline__ bool lm_initialised(const WinDev& W, const FeatStore& F, int l) {
+  return lm_sharded(W) ? shard_lm_replica(W).aux[l].init != 0 : (l < F.lm_cap && F.lm_init[l]);
+}
+// Estimator::setLandmarkInitialized(false) on slot l, initialised before: sharded, in the replica of every rank (each
+// clears it in its own) and in the owner's shard at its local slot
+__device__ __forceinline__ void lm_clear_initialised(const WinDev& W, const FeatStore& F, int l) {
+  if (!lm_sharded(W)) { F.lm_init[l] = 0; return; }
+  shard_lm_replica(W).aux[l].init = 0;
+  if (l % W.shard_world == W.shard_rank && l / W.shard_world < F.lm_cap) F.lm_init[l / W.shard_world] &= 2;
+}
+// observations per landmark slot into cnt[0, L) (cnt zeroed by the caller, all threads of the CTA take part)
+template <int NT>
+__device__ __forceinline__ void lm_count_obs(const WinDev& W, int* cnt, int L) {
+  if (lm_sharded(W)) {
+    const ShardLmAux* aux = shard_lm_replica(W).aux;
+    for (int i = threadIdx.x; i < L; i += NT) cnt[i] = aux[i].n_obs;
+    return;
+  }
+  const int n_obs = W.st->g.n_obs;
+  for (int i = threadIdx.x; i < n_obs; i += NT) {
+    const okb_observation& ob = W.m_obs[i];
+    if (ob.sqrt_info != 0.0 && (int)ob.lm_idx < L) atomicAdd(&cnt[ob.lm_idx], 1);
+  }
+}
+
+// ---- landmark exchange of a sharded window, at the start of a call that reads landmark state (track, 2D-2D, stereo
+// initialisation, RANSAC 3D-2D).  Every rank writes the records of the global slots it owns (g = rank + i * world,
+// local slot i) into its own replica half of the new epoch's parity and counts their observations there, then pushes
+// those records with plain stores into the same half of every peer's replica and releases its flag in every peer's
+// mailbox header (st.release.sys), as k_shard_push does for the solver.  k_shard_lm_wait acquires the `world` flags of
+// the epoch, or reports status 7 after kShardTimeoutNs; on success k_shard_lm_forget clears, on every rank alike, the
+// store references to slots the owners removed since the last exchange.
+__device__ __forceinline__ int shard_lm_owned(const WinDev& W) {
+  return W.shard_lm_cap > W.shard_rank ? (W.shard_lm_cap - W.shard_rank + W.shard_world - 1) / W.shard_world : 0;
+}
+
+__global__ void __launch_bounds__(256) k_shard_lm_own(const WinDev* __restrict__ Wp) {
+  const WinDev& W = *Wp;
+  const FeatStore& F = *W.feat;
+  const ShardLmHalf rep = shard_lm_half(W, W.shard_rank, (int)((shard_lm_epoch(W) + 1ull) & 1ull));
+  const int n = shard_lm_owned(W), L = W.st->g.L;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const size_t g = W.shard_rank + (size_t)i * W.shard_world;
+    *reinterpret_cast<double4*>(rep.x + 4 * g) = i < L ? *reinterpret_cast<const double4*>(W.m_lm + 4 * (size_t)i) : make_double4(0, 0, 0, 0);
+    const uint8_t v = i < F.lm_cap ? F.lm_init[i] : 0;
+    ShardLmAux a;
+    a.n_obs = 0; a.init = v & 1; a.removed = v >> 1; a._pad[0] = a._pad[1] = 0;
+    rep.aux[g] = a;
+    if (v & 2) F.lm_init[i] = v & 1;             // the mark is taken: every rank forgets the slot's references
+  }
+}
+
+__global__ void __launch_bounds__(256) k_shard_lm_count(const WinDev* __restrict__ Wp) {
+  const WinDev& W = *Wp;
+  ShardLmAux* aux = shard_lm_half(W, W.shard_rank, (int)((shard_lm_epoch(W) + 1ull) & 1ull)).aux;
+  const int n_obs = W.st->g.n_obs, L = min(W.st->g.L, shard_lm_owned(W));
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_obs; i += gridDim.x * blockDim.x) {
+    const okb_observation& ob = W.m_obs[i];
+    if (ob.sqrt_info != 0.0 && (int)ob.lm_idx < L) atomicAdd(&aux[W.shard_rank + (size_t)ob.lm_idx * W.shard_world].n_obs, 1);
+  }
+}
+
+__global__ void __launch_bounds__(256) k_shard_lm_push(const WinDev* __restrict__ Wp) {
+  const WinDev& W = *Wp;
+  const int world = W.shard_world, me = W.shard_rank;
+  const unsigned long long epoch = shard_lm_epoch(W) + 1ull;
+  const int par = (int)(epoch & 1ull), n = shard_lm_owned(W);
+  const ShardLmHalf own = shard_lm_half(W, me, par);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const size_t g = me + (size_t)i * world;
+    const double4 x = *reinterpret_cast<const double4*>(own.x + 4 * g);
+    const ShardLmAux a = own.aux[g];
+    for (int q = 0; q < world; ++q)
+      if (q != me) {
+        const ShardLmHalf dst = shard_lm_half(W, q, par);
+        *reinterpret_cast<double4*>(dst.x + 4 * g) = x;
+        dst.aux[g] = a;
+      }
+  }
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned int* counter = reinterpret_cast<unsigned int*>(W.shard_mail[me] + kShardLmCounter);
+    if (atomicAdd(counter, 1u) == gridDim.x - 1) {
+      *counter = 0u;
+      __threadfence_system();
+      for (int q = 0; q < world; ++q)
+        st_release_sys_u64(reinterpret_cast<unsigned long long*>(W.shard_mail[q] + kShardFlagsL) + par * kMaxShard + me, epoch);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(32) k_shard_lm_wait(const WinDev* __restrict__ Wp) {
+  const WinDev& W = *Wp;
+  unsigned char* box = W.shard_mail[W.shard_rank];
+  const unsigned long long epoch = shard_lm_epoch(W) + 1ull;
+  const int par = (int)(epoch & 1ull);
+  int late = 0;
+  if ((int)threadIdx.x < W.shard_world) {
+    const unsigned long long* fl = reinterpret_cast<const unsigned long long*>(box + kShardFlagsL) + par * kMaxShard + threadIdx.x;
+    const unsigned long long t0 = globaltimer_ns();
+    while (ld_acquire_sys_u64(fl) < epoch)
+      if (globaltimer_ns() - t0 > kShardTimeoutNs) { late = 1; break; }
+  }
+  late = __any_sync(0xffffffffu, late);
+  if (threadIdx.x == 0) {
+    *reinterpret_cast<int*>(box + kShardLmStatus) = late ? 7 : 0;
+    *reinterpret_cast<unsigned long long*>(box + kShardLmEpoch) = epoch;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_shard_lm_forget(const WinDev* __restrict__ Wp) {
+  const WinDev& W = *Wp;
+  const FeatStore& F = *W.feat;
+  const ShardLmAux* aux = shard_lm_replica(W).aux;
+  const int n_ent = F.F * F.C * F.N;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n_ent; e += gridDim.x * blockDim.x) {
+    const int l = F.lm[e];
+    if (l >= 0 && l < W.shard_lm_cap && aux[l].removed) { F.lm[e] = -1; F.observed[e] = 0; }
+  }
+}
+
 __device__ __forceinline__ bool track_live(const WinDev& W, int L, int l) {
   // a landmark slot is in the graph iff it is below L and its estimate is not the all-zero vector the graph leaves in
   // removed and unused slots (Estimator::isLandmarkAdded)
   if (l < 0 || l >= L) return false;
-  const double4 x = *reinterpret_cast<const double4*>(W.m_lm + 4 * (size_t)l);
+  const double4 x = *reinterpret_cast<const double4*>(lm_point(W, l));
   return x.x != 0.0 || x.y != 0.0 || x.z != 0.0 || x.w != 0.0;
 }
 
@@ -1720,17 +1867,13 @@ __global__ void __launch_bounds__(TK_T, 1) k_track_setup(const TrackJobDev* __re
   const WinDev& W = *J.W;
   const FeatStore& F = *W.feat;
   const int tid = threadIdx.x;
-  const int L = min(W.st->g.L, J.cnt_cap);
+  const int L = min(lm_slots(W), J.cnt_cap);
   if (round == 0) {
     // observation counts of the window (landmark.observations.size()); later rounds see them raised by the matches
     for (int i = tid; i < J.cnt_cap; i += TK_T) J.cnt[i] = 0;
     for (int i = tid; i < 2 * J.n_rounds + 2; i += TK_T) J.hdr[i] = 0;
     __syncthreads();
-    const int n_obs = W.st->g.n_obs;
-    for (int i = tid; i < n_obs; i += TK_T) {
-      const okb_observation& ob = W.m_obs[i];
-      if (ob.sqrt_info != 0.0 && (int)ob.lm_idx < L) atomicAdd(&J.cnt[ob.lm_idx], 1);
-    }
+    lm_count_obs<TK_T>(W, J.cnt, L);
     __syncthreads();
   }
   // skipB (:238-250): B keypoint k refers to a landmark of the graph that already holds this keypoint's observation
@@ -1762,9 +1905,9 @@ __global__ void __launch_bounds__(TK_T, 1) k_track_setup(const TrackJobDev* __re
       const int l = F.lm[base_a + k];
       bool skip = true;
       if (!track_live(W, L, l)) {                                       // 1. no landmark, or not in the graph
-      } else if (!(l < F.lm_cap && F.lm_init[l])) {                      // 2. not initialised
+      } else if (!lm_initialised(W, F, l)) {                             // 2. not initialised
       } else {
-        const double* X = W.m_lm + 4 * (size_t)l;
+        const double* X = lm_point(W, l);
         const double w = X[3];
         double pc[3];
         pc[0] = xf.R[0] * X[0] + xf.R[1] * X[1] + xf.R[2] * X[2] + xf.t[0] * w;
@@ -1801,7 +1944,7 @@ __global__ void __launch_bounds__(TK_T, 1) k_track_setup(const TrackJobDev* __re
       int n_u = J.hdr[h];
       for (int i = 0; i < total; ++i) {
         const int l = F.lm[base_a + s_cand[i]];
-        if (F.lm_init[l]) { F.lm_init[l] = 0; J.uninit[n_u++] = (uint32_t)l; }
+        if (lm_initialised(W, F, l)) { lm_clear_initialised(W, F, l); J.uninit[n_u++] = (uint32_t)l; }
       }
       J.hdr[h] = n_u;
     }
@@ -1880,7 +2023,8 @@ static std::string store_window_invalid(okb_ctx* c, int win, std::vector<char>& 
 }
 
 // The argument checks of a call `fn` on the feature store, before any device work: an empty call is a no-op (OKB_OK, and
-// the caller returns), more than max_jobs jobs and a landmark-sharded context are refused, and invalid(i, seen) checks
+// the caller returns), more than max_jobs jobs and a landmark-sharded context connected without a landmark replica are
+// refused, and invalid(i, seen) checks
 // job i against the store as the pending commands leave it ("" = valid; the first failure is reported as
 // "fn: jobs[i]: why").
 template <typename Job, typename Invalid>
@@ -1888,7 +2032,10 @@ static int store_call_checks(okb_ctx* c, const char* fn, int n_jobs, const Job* 
   if (!c || n_jobs < 0 || (n_jobs > 0 && !jobs)) return OKB_ERR_INVALID_ARG;
   if (n_jobs == 0) return OKB_OK;
   if (n_jobs > max_jobs) { c->set_error(std::string(fn) + ": more than " + std::to_string(max_jobs) + " jobs"); return OKB_ERR_INVALID_ARG; }
-  if (c->shard_world > 1) { c->set_error(std::string(fn) + ": landmark-sharded windows are not supported"); return OKB_ERR_UNSUPPORTED; }
+  if (c->shard_world > 1 && c->shard_lm_cap < 1) {
+    c->set_error(std::string(fn) + ": a landmark-sharded context needs its global landmark slots (okb_shard_reserve_landmarks)");
+    return OKB_ERR_UNSUPPORTED;
+  }
   std::vector<char> seen(c->max_windows, 0);
   for (int i = 0; i < n_jobs; ++i) {
     const std::string why = invalid(i, seen);
@@ -1904,6 +2051,50 @@ static int commit_job_windows(okb_ctx* c, const Job* jobs, int n_jobs) {
   std::vector<int32_t> wl(n_jobs);
   for (int i = 0; i < n_jobs; ++i) wl[i] = jobs[i].win;
   return okb_commit_windows(c, wl.data(), n_jobs);
+}
+
+// Landmark slots a call names on window `win`: the graph's, or on a landmark-sharded context the replica's global slots.
+static int lm_slots_host(const okb_ctx* c, int win) { return c->shard_world > 1 ? c->shard_lm_cap : std::max(c->host[win].L, 1); }
+
+// Landmark-sharded context: the landmark exchange (k_shard_lm_*) of every job window on `xs`, after the commit.  Every
+// rank must make the same call; a peer that does not arrive within the time-out fails the call with status 7 before
+// any of its own device work, and a window whose shard names global slots beyond the replica is refused.
+template <typename Job>
+static int shard_lm_exchange(okb_ctx* c, const char* fn, const Job* jobs, int n_jobs, cudaStream_t xs) {
+  if (c->shard_world < 2) return OKB_OK;
+  for (int i = 0; i < n_jobs; ++i)
+    if ((int64_t)(c->host[jobs[i].win].L - 1) * c->shard_world + c->shard_rank >= c->shard_lm_cap) {
+      c->set_error(std::string(fn) + ": the shard's landmarks exceed the global landmark slots (okb_shard_reserve_landmarks)");
+      return OKB_ERR_CAPACITY;
+    }
+  const int gx = std::max(1, std::min(c->sm_count, (c->shard_lm_cap / c->shard_world + 255) / 256));
+  for (int i = 0; i < n_jobs; ++i) {
+    const WinDev* W = c->d_wins + jobs[i].win;
+    k_shard_lm_own<<<gx, 256, 0, xs>>>(W);
+    k_shard_lm_count<<<gx, 256, 0, xs>>>(W);
+    k_shard_lm_push<<<gx, 256, 0, xs>>>(W);
+    k_shard_lm_wait<<<1, 32, 0, xs>>>(W);
+  }
+  fe(c)->launches += 4 * (int64_t)n_jobs;
+  OKB_CUDA(c, cudaGetLastError());
+  std::vector<int> status(n_jobs, 0);
+  for (int i = 0; i < n_jobs; ++i)
+    OKB_CUDA(c, cudaMemcpyAsync(&status[i], c->shard_local + (size_t)jobs[i].win * c->shard_win_bytes + kShardLmStatus, sizeof(int),
+                                cudaMemcpyDeviceToHost, xs));
+  OKB_CUDA(c, cudaStreamSynchronize(xs));
+  for (int i = 0; i < n_jobs; ++i)
+    if (status[i]) {
+      c->set_error(std::string(fn) + ": jobs[" + std::to_string(i) + "]: a peer rank did not arrive at the landmark exchange (status 7)");
+      return OKB_ERR_SHARD_TIMEOUT;
+    }
+  for (int i = 0; i < n_jobs; ++i) {
+    const FeatStore& F = c->wins[jobs[i].win].feat;
+    const int n = F.F * F.C * F.N;
+    k_shard_lm_forget<<<std::max(1, std::min(c->sm_count, (n + 255) / 256)), 256, 0, xs>>>(c->d_wins + jobs[i].win);
+  }
+  fe(c)->launches += n_jobs;
+  OKB_CUDA(c, cudaGetLastError());
+  return OKB_OK;
 }
 
 // Host checks of one job (first_win: the window of the call's first job, already checked); "" = valid.
@@ -1947,6 +2138,7 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
   CallBuffers& B = F->track;
   std::lock_guard<std::mutex> lk(B.mtx);
   if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
+  if ((rc = shard_lm_exchange(c, "okb_track_3d2d_batch", jobs, n_jobs, c->stream_xfer))) return rc;
   cudaStream_t xs = c->stream_xfer;
   // jobs by decreasing round count: the jobs of round r are the first m[r]
   std::vector<int> order(n_jobs);
@@ -1971,7 +2163,7 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
     const okb_track_job& j = jobs[i];
     const WinStore& S = c->wins[j.win];
     r0[i] = rl.size();
-    o_cnt[i] = sc.take(4 * (size_t)std::max(c->host[j.win].L, 1));
+    o_cnt[i] = sc.take(4 * (size_t)lm_slots_host(c, j.win));
     size_t sumA = 0, sumB = 0;
     for (int r = 0; r < j.n_rounds; ++r) {
       RoundLay x;
@@ -2003,7 +2195,7 @@ extern "C" int okb_track_3d2d_batch(okb_ctx* c, int n_jobs, const okb_track_job*
     J.W = c->d_wins + j.win;
     J.pose_b = j.pose_b; J.sb_b = j.sb_b; J.feat_b = j.feat_slot_b; J.n_rounds = j.n_rounds;
     J.threshold = j.threshold;
-    J.cnt_cap = std::max(c->host[j.win].L, 1);
+    J.cnt_cap = lm_slots_host(c, j.win);
     J.cnt = reinterpret_cast<int*>(B.d_scratch + o_cnt[i]);
     J.hdr = reinterpret_cast<int*>(d + o_hdr[i]);
     J.assoc = reinterpret_cast<uint2*>(d + o_assoc[i]);
@@ -2186,7 +2378,7 @@ __global__ void __launch_bounds__(TK_T) k_stereo_setup(const StereoJobDev* __res
   double* br = const_cast<double*>(side ? M.gate.bearing_b : M.gate.bearing_a) + 3 * (size_t)k;
   br[0] = pu[0]; br[1] = pu[1]; br[2] = 1.0;
   const int l = F.lm[e];
-  const bool skip = track_live(W, W.st->g.L, l) && l < F.lm_cap && F.lm_init[l];
+  const bool skip = track_live(W, lm_slots(W), l) && lm_initialised(W, F, l);
   const_cast<uint8_t*>(side ? M.skipB : M.skipA)[k] = skip ? 1 : 0;
 }
 
@@ -2295,7 +2487,7 @@ __global__ void __launch_bounds__(TK_T, 1) k_stereo_apply(const StereoJobDev* __
   const GateDev& g = M.gate;
   const WinDev& W = *J.W;
   const FeatStore& F = *W.feat;
-  const int L = W.st->g.L;
+  const int L = lm_slots(W);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const size_t base_a = ((size_t)J.feat_a * F.C + J.cam_a) * F.N;
   const size_t base_b = ((size_t)J.feat_b * F.C + J.cam_b) * F.N;
@@ -2419,6 +2611,7 @@ static int match2d2d_batch(okb_ctx* c, int n_jobs, const okb_match2d2d_job* jobs
   CallBuffers& B = F->stereo;
   std::lock_guard<std::mutex> lk(B.mtx);
   if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
+  if ((rc = shard_lm_exchange(c, fn, jobs, n_jobs, c->stream_xfer))) return rc;
   cudaStream_t xs = c->stream_xfer;
   // staging (pinned + device mirror): in  = [job table | match table]
   //                                   out = [per job: count | records]
@@ -3268,7 +3461,7 @@ __global__ void __launch_bounds__(RS_T) k_ransac_3d2d(const RansacJobDev* __rest
     return;
   }
   // observation counts (landmark.observations.size())
-  const int L = min(W.st->g.L, J.cnt_cap);
+  const int L = min(lm_slots(W), J.cnt_cap);
   for (int i = tid; i < J.cnt_cap; i += RS_T) J.cnt[i] = 0;
   if (tid < J.n_cams) {
     XfQ T;
@@ -3278,11 +3471,7 @@ __global__ void __launch_bounds__(RS_T) k_ransac_3d2d(const RansacJobDev* __rest
     for (int k = 0; k < 3; ++k) s_ext[tid][9 + k] = T.r[k];
   }
   __syncthreads();
-  const int n_obs = W.st->g.n_obs;
-  for (int i = tid; i < n_obs; i += RS_T) {
-    const okb_observation& ob = W.m_obs[i];
-    if (ob.sqrt_info != 0.0 && (int)ob.lm_idx < L) atomicAdd(&J.cnt[ob.lm_idx], 1);
-  }
+  lm_count_obs<RS_T>(W, J.cnt, L);
   __syncthreads();
   // the adapter's correspondences, cameras ascending, keypoints ascending
   int n = 0;
@@ -3296,13 +3485,13 @@ __global__ void __launch_bounds__(RS_T) k_ransac_3d2d(const RansacJobDev* __rest
       int take = 0, l = -1;
       if (k < nk) {
         l = F.lm[base + k];
-        if (track_live(W, L, l) && J.cnt[l] >= 2 && fabs(W.m_lm[4 * (size_t)l + 3]) >= 1.0e-8) take = 1;
+        if (track_live(W, L, l) && J.cnt[l] >= 2 && fabs(lm_point(W, l)[3]) >= 1.0e-8) take = 1;
       }
       int total;
       const int pos = block_scan<RS_T>(take, s_warp, &total);
       if (take) {
         double* cd = J.cd + (size_t)(n + pos) * RS_CD;
-        const double* hp = W.m_lm + 4 * (size_t)l;
+        const double* hp = lm_point(W, l);
         for (int r = 0; r < 3; ++r) cd[r] = hp[r] / hp[3];
         // PinholeCamera::backProject (its return value ignored), then bearing.normalize()
         double pu[2];
@@ -3464,6 +3653,7 @@ extern "C" int okb_ransac_3d2d_batch(okb_ctx* c, int n_jobs, const okb_ransac_jo
   CallBuffers& B = F->ransac;
   std::lock_guard<std::mutex> lk(B.mtx);
   if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
+  if ((rc = shard_lm_exchange(c, "okb_ransac_3d2d_batch", jobs, n_jobs, c->stream_xfer))) return rc;
   cudaStream_t xs = c->stream_xfer;
   // staging (pinned + device mirror): in  = [job table]
   //                                   out = [per job: result | hypothesis inliers | outlier records]
@@ -3480,7 +3670,7 @@ extern "C" int okb_ransac_3d2d_batch(okb_ctx* c, int n_jobs, const okb_ransac_jo
     o_res[i] = st.take(sizeof(okb_ransac_result));
     o_hyp[i] = st.take(4 * (size_t)j.max_iterations);
     o_out[i] = st.take(sizeof(okb_ransac_outlier) * (size_t)n_kp[i]);
-    o_cnt[i] = sc.take(4 * (size_t)std::max(c->host[j.win].L, 1));
+    o_cnt[i] = sc.take(4 * (size_t)lm_slots_host(c, j.win));
     o_cd[i] = sc.take(8 * RS_CD * (size_t)n_kp[i]);
     o_ci[i] = sc.take(12 * (size_t)n_kp[i]);
   }
@@ -3495,7 +3685,7 @@ extern "C" int okb_ransac_3d2d_batch(okb_ctx* c, int n_jobs, const okb_ransac_jo
     std::memset(&J, 0, sizeof J);
     J.W = c->d_wins + j.win;
     J.feat = j.feat_slot; J.n_cams = j.n_cams; J.n_hyp = j.max_iterations;
-    J.cnt_cap = std::max(c->host[j.win].L, 1);
+    J.cnt_cap = lm_slots_host(c, j.win);
     J.threshold = j.threshold;
     J.seed = (unsigned long long)j.seed;
     J.cnt = reinterpret_cast<int*>(B.d_scratch + o_cnt[i]);

@@ -268,7 +268,12 @@ __global__ void __launch_bounds__(1024) k_apply_commands(const WinDev* __restric
           okb_observation* ob = W.m_obs + i;
           if ((int)ob->lm_idx < L && W.m_mark[ob->lm_idx]) ob->sqrt_info = 0.0;
         }
-        if (W.feat) {
+        if (W.feat && W.shard_world > 1) {
+          // landmark-sharded: the store names global slots and is replicated; the removal reaches only the owner, so
+          // the slot is marked (bit 1) and every rank's store forgets it at the next landmark exchange (okb_frontend.cu)
+          for (int i = tid; i < n; i += NT)
+            if ((int)idx[i] < W.feat->lm_cap) W.feat->lm_init[idx[i]] = 2;
+        } else if (W.feat) {
           // the store forgets the removed slots (the reference's isLandmarkAdded(id) == false for a gone id), so a slot
           // reused later is never reached through a keypoint that referred to its previous occupant
           const FeatStore& F = *W.feat;
@@ -517,7 +522,7 @@ __global__ void __launch_bounds__(1024) k_apply_commands(const WinDev* __restric
         const uint8_t* fl = pay + (((size_t)4 * n + 7) & ~(size_t)7);
         for (int i = tid; i < n; i += NT) {
           if ((int)idx[i] >= W.feat->lm_cap) { graph_error(g, GERR_INDEX); continue; }
-          W.feat->lm_init[idx[i]] = fl[i] ? 1 : 0;
+          W.feat->lm_init[idx[i]] = (W.feat->lm_init[idx[i]] & 2) | (fl[i] ? 1 : 0);   // keeps a sharded removal mark
         }
         break;
       }

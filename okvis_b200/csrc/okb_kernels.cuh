@@ -18,12 +18,6 @@ constexpr int S_WARPS = S_THREADS / 32;
 constexpr int kImuOut = 932;     // doubles per IMU term produced by k_imu: H30 | g30 | cost | pad
 static_assert(OKB_IMU_TERM_OUT == 900 + 30 + 1 && OKB_IMU_TERM_OUT < kImuOut, "okb_debug_imu_terms copies H30 | g30 | cost");
 
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -112,8 +106,6 @@ struct SShared {
   int shard_fault, chain_ok;
   double x2[8];         // landmark-sharded windows: step scalars combined over the ranks
 };
-
-constexpr unsigned long long kShardTimeoutNs = 4000000000ull;   // a peer that does not arrive within 4 s: FAILURE, no hang
 
 // Landmark-sharded window, second exchange of a round (inside k_solve): the landmark parts of the dogleg scalars
 // [N2, GU, G2, VHV, ||x||^2, max|g|, #non-finite, elapsed+last (time-limit callback)] of every rank.  Each rank stores

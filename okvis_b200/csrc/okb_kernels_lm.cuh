@@ -663,14 +663,6 @@ __global__ void __launch_bounds__(256) k_reduce_partials(const WinDev* __restric
 // `world` ready flags.  The sum over ranks happens in k_solve's prologue (every rank adds the boxes in rank order
 // => bit-identical reduced systems, so the redundant reduced solves stay in lock step).
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void st_release_sys_u64(unsigned long long* p, unsigned long long v) {
-  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long ld_acquire_sys_u64(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ double* shard_box(const WinDev& W, int dst, int parity, int src) {
   return reinterpret_cast<double*>(W.shard_mail[dst] + kShardHeaderBytes) + ((size_t)parity * W.shard_world + src) * W.shard_box_cap;
 }

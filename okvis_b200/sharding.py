@@ -79,16 +79,18 @@ def shard_marg_job(rank, world, block_kind, block_idx, block_prev, block_margina
 
 
 # Resident edits of a sliding landmark-sharded window: landmark edits go to the slot's owner, the dense edits (frames,
-# states, priors, speed/bias removal) to every rank unchanged.  Any other op is refused: its arguments may hold
-# landmark slots that would be read as local ones.
-LANDMARK_EDITS = ("set_landmarks", "remove_landmarks", "add_observations", "remove_observations")
+# states, priors, speed/bias removal) to every rank unchanged.  The feature store is replicated and names global
+# landmark slots, so its edits also go to every rank unchanged; a landmark's initialised flag is landmark state and goes
+# to its owner.  Any other op is refused: its arguments may hold landmark slots that would be read as local ones.
+LANDMARK_EDITS = ("set_landmarks", "remove_landmarks", "add_observations", "remove_observations", "set_landmark_initialized")
 DENSE_EDITS = ("add_frame", "remove_frame", "set_states", "set_priors", "remove_speed_bias")
+STORE_EDITS = ("reserve_features", "set_features", "set_feature_landmarks", "clear_features")
 
 
 def route_edit(op, rank, world, *args):
     """Arguments of Context.<op>(win, *args) for rank `rank`, or None when the rank has nothing to do.  `args` are the
     unsharded window's (global landmark slots)."""
-    if op in DENSE_EDITS:
+    if op in DENSE_EDITS or op in STORE_EDITS:
         return args
     if op == "remove_observations":
         (keys,) = args
@@ -107,6 +109,10 @@ def route_edit(op, rank, world, *args):
         (idx,) = args
         _, local = owned_slots(idx, rank, world)
         return (local,) if len(local) else None
+    if op == "set_landmark_initialized":
+        idx, flags = args
+        pos, local = owned_slots(idx, rank, world)
+        return (local, np.asarray(flags).reshape(-1)[pos]) if len(pos) else None
     if op == "add_observations":
         (obs,) = args
         pos, local = owned_slots(obs["lm_idx"], rank, world)
@@ -129,11 +135,12 @@ def merge_shard_results(n_landmarks, parts):
     return out
 
 
-def connect_shards(ctx, dist, device, rank, world, max_frames):
+def connect_shards(ctx, dist, device, rank, world, max_frames, max_landmarks=0):
     """Multi-process mailbox set-up of a landmark-sharded context: export this rank's cudaIpc handle, all-gather the
-    handles with torch.distributed (64 bytes per rank; plumbing only), map the peers."""
+    handles with torch.distributed (64 bytes per rank; plumbing only), map the peers.  max_landmarks > 0: the global
+    landmark slots of the frontend's landmark replica."""
     import torch
-    handle = torch.from_numpy(ctx.shard_export(rank, world, max_frames)).to(device)
+    handle = torch.from_numpy(ctx.shard_export(rank, world, max_frames, max_landmarks)).to(device)
     gathered = [torch.zeros_like(handle) for _ in range(world)]
     dist.all_gather(gathered, handle)
     ctx.shard_connect(np.stack([g.cpu().numpy() for g in gathered]))

@@ -44,7 +44,7 @@ def slide_problem(n_landmarks=2000, extra=3, K=20, seed=0):
 class Slide:
     """members: [(rank, Context)] this process drives, all on window slot 0; world 1 = an unsharded window."""
 
-    def __init__(self, members, world, full, w0, first_seen):
+    def __init__(self, members, world, full, w0, first_seen, features=None):
         self.members, self.world, self.full, self.first_seen = members, world, full, first_seen
         self.K, self.L = len(w0.poses), len(w0.landmarks)
         self.w = w0                  # host mirror of the current window (global landmark slots; estimates not tracked)
@@ -54,6 +54,8 @@ class Slide:
             sw, idx = sharding.shard_window(w0, r, world)
             self.local[r] = idx
             c.reserve(0, self.K, len(sw.landmarks), int(np.isin(full.obs["lm_idx"], idx).sum()), len(full.imu_samples) + 4096, 160)
+            if features:                 # (feature slots, cameras, keypoints, descriptor bytes) of a replicated store
+                c.reserve_features(0, *features)
             c.upload(0, sw)
 
     def optimize(self, iters):
