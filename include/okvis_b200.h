@@ -38,6 +38,9 @@
  *                                pointPolygonTest over the current frame's keypoints, for many sessions in one launch
  *   okb_ransac_3d2d_batch     <- Frontend::runRansac3d2d (Frontend.cpp:575-642): FrameNoncentralAbsoluteAdapter's
  *                                correspondences, FrameAbsolutePoseSacProblem's score; own sampler and generalised P3P
+ *   okb_ransac_2d2d_batch     <- Frontend::runRansac2d2d (Frontend.cpp:645-810): FrameRelativeAdapter's correspondences,
+ *                                FrameRotationOnly / FrameRelativePoseSacProblem's scores, the decision, outliers and pose
+ *                                initialisation; own sampler, two-point rotation and five-point solvers
  *   okb_detect_describe       <- okvis::Frontend::detectAndDescribe    okvis_frontend/src/Frontend.cpp:92-114
  *                                (Frame::detect / Frame::describe      okvis_cv/include/okvis/implementation/Frame.hpp:109-156)
  *   okb_detect_describe_store_batch <- the same for every camera of many sessions' frames, written straight into the
@@ -419,7 +422,8 @@ int okb_window_download_slots(okb_ctx* ctx, int n, const int32_t* slots, double*
  * max_frames bounds the keyframes of any sharded window (mailbox sizing).
  *
  * The frontend calls on the feature store (okb_detect_describe_store_batch, okb_track_3d2d_batch, okb_match2d2d_batch,
- * okb_stereo_init_batch, okb_keyframe_overlap_batch, okb_ransac_3d2d_batch) run on a sharded window when the context
+ * okb_stereo_init_batch, okb_keyframe_overlap_batch, okb_ransac_3d2d_batch, okb_ransac_2d2d_batch) run on a sharded
+ * window when the context
  * reserved its global landmark slots with okb_shard_reserve_landmarks before okb_shard_export / okb_shard_connect_local
  * (otherwise they return OKB_ERR_UNSUPPORTED).  The feature store is replicated: every rank reserves it and receives
  * the same store edits (okb_window_reserve_features, okb_window_set_features, okb_window_set_feature_landmarks,
@@ -888,6 +892,88 @@ typedef struct okb_ransac_job {
  * store: the caller applies the removals.  Results per job are bit-identical to calling it alone.  n_jobs == 0 is a
  * no-op. */
 int okb_ransac_3d2d_batch(okb_ctx* ctx, int n_jobs, const okb_ransac_job* jobs);
+
+/* ---- 2D-2D outlier rejection and pose initialisation (Frontend::runRansac2d2d, Frontend.cpp:645-810) -----------------
+ * One job = one session's runRansac2d2d(currentFrameId, olderFrameId, initializePose, removeOutliers): frame B (the
+ * current frame) and frame A (the older frame), each named by its position in the window (T_WS) and its feature slot,
+ * cameras 0..n_cams-1.  Per camera im, ascending, as the reference's loop runs:
+ *   correspondences as FrameRelativeAdapter (FrameRelativeAdapter.cpp:139-244) collects them: B's keypoints ascending
+ *     whose store slot names a landmark of the graph, the first keypoint per landmark kept (std::map::insert); then A's
+ *     keypoints ascending whose store slot names one of those landmarks, matched to B's keypoint for it.  Bearings are
+ *     the normalised backProject (a failed backProject leaves a NaN bearing: counted, never an inlier, never in a usable
+ *     sample), sigmaAngle = sqrt(2) sigma^2 / fu^2 with sigma = 0.8 size / 12;
+ *   fewer than 10 correspondences: the camera is skipped (:670-671);
+ *   two RANSACs of max_iterations hypotheses each, drawn by the counter-based generator of okb_ransac_3d2d_batch keyed by
+ *     (seed, (2 im + problem) 64 + hypothesis, draw), no adaptive stop (DESIGN.md 6i):
+ *     rotation-only (problem 0): 2 correspondences, R from their bearing triads; score
+ *       0.5 |R f2 - f1|^2 / sigma1 + 0.5 |R^T f1 - f2|^2 / sigma2 (FrameRotationOnlySacProblem.hpp);
+ *     relative pose (problem 1): a five-point solver on 5 correspondences, the 6th choosing among the admissible
+ *       solutions; score FrameRelativePoseSacProblem.hpp's, the point triangulated in frame A as the midpoint of the
+ *       common perpendicular of the rays l1 f1 and t + l2 R f2;
+ *     inlier iff score < threshold; the most inliers win, ties to the lowest hypothesis;
+ *   the decision (:709-733): float ratios inliers / correspondences; rotation-only is chosen iff rot_ratio > rel_ratio ||
+ *     rot_ratio > 0.8 (rotationOnly = true); more than 10 inliers of the chosen model set that model's success flag;
+ *     the flags are not reset between cameras, and the camera is applied when either is set (:735-737), its
+ *     correspondences outside the chosen model's inliers becoming outlier records;
+ *   with initialize_pose, each applied camera sets T_WS0 = T_WSA T_SCA T_C1C2 T_SC0^-1 (:756-798), T_C1C2 = the
+ *     five-point winner when any camera's five-point model succeeded (its unit translation scaled by
+ *     max(0, t . r(T_SCA^-1 T_WSA^-1 T_WS0 T_SC0)), T_WS0 as the previous camera left it), else the rotation-only
+ *     winner with zero translation; a missing winner leaves T_C1C2 the identity;
+ *   ret = the summed inliers of the chosen models of all cameras that were not skipped, or -1 with rotationOnly = true
+ *     when no model succeeded (:802-808).
+ * One deliberate departure (:735-753): the reference reads and clears multiFrame->landmarkId(im, k) with k the
+ * correspondence number and then removes the observation (lmId, current, im, idxB), which clears an unrelated keypoint's
+ * id and removes an observation that usually does not exist.  The outlier record names the correspondence's own B
+ * keypoint (idxB) and its landmark slot instead, so that the caller reaches okb_ransac_3d2d_batch's end state: the
+ * observation removed, the host id 0 and the store slot -1.  A B keypoint that several A keypoints of one landmark
+ * matched comes in one record per correspondence; the caller applies the first (Estimator::finishRansac2d2d skips the
+ * records whose keypoint no longer carries the landmark). */
+typedef struct okb_ransac2d_outlier { int32_t cam, kp_a, kp_b, lm_slot; } okb_ransac2d_outlier;
+typedef struct okb_ransac2d_cam {
+  int32_t n_correspondences;            /* adapter.getNumberCorrespondences() */
+  int32_t rot_inliers, rel_inliers;     /* inliers of each RANSAC's winner (0: skipped or no model) */
+  int32_t rot_best, rel_best;           /* winning hypotheses, -1: skipped or no hypothesis had a model */
+  int32_t rotation_only;                /* 1: the rotation-only model was chosen */
+  int32_t applied;                      /* 1: outliers reported (and, with initialize_pose, the pose set) */
+  int32_t n_outliers;
+  double R_rot[9];                      /* rotation-only winner, row-major (identity when rot_best == -1) */
+  double R_rel[9], t_rel[3];            /* five-point winner T_C1C2 = [R t] (C1: frame A's camera, C2: frame B's), |t| = 1
+                                           (identity and zero when rel_best == -1) */
+} okb_ransac2d_cam;
+typedef struct okb_ransac2d_result {
+  int32_t ret;                          /* what runRansac2d2d returns */
+  int32_t rotation_only;                /* its rotationOnly */
+  int32_t pose_set;                     /* 1: T_WS holds frame B's initialised pose (the caller applies it with set_T_WS) */
+  int32_t n_outliers;
+  double T_WS[7];                       /* [t, q_xyzw], zero unless pose_set */
+} okb_ransac2d_result;
+typedef struct okb_ransac2d_job {
+  int32_t win;
+  int32_t pose_b, feat_slot_b;          /* frame B: the current frame (its position in the window, feature slot) */
+  int32_t pose_a, feat_slot_a;          /* frame A: the older frame */
+  int32_t n_cams;
+  int32_t initialize_pose;              /* initializePose && !isInitialized_ */
+  int32_t max_iterations;               /* hypotheses per RANSAC, 1..64 (the reference: 50) */
+  double threshold;                     /* threshold_ of both RANSACs (9) */
+  uint64_t seed;
+  int32_t* hyp_inliers;                 /* [n_cams][2][max_iterations] inliers of every hypothesis (problem 0: rotation-only,
+                                           1: five-point), or NULL */
+  okb_ransac2d_cam* cams;               /* [n_cams], or NULL */
+  okb_ransac2d_outlier* outliers;       /* [outlier_cap], cameras ascending, then correspondence order */
+  int32_t outlier_cap, _pad;            /* >= the keypoints of frame A in cameras 0..n_cams-1 */
+  okb_ransac2d_result* out;
+} okb_ransac2d_job;
+/* One CTA per job in one launch.  Every job is checked on the host before any device work (uploaded window, store
+ * reserved, both feature slots in range and present for each camera, both poses in range, n_cams in 1..the store's, the
+ * window's extrinsics and cameras (at most 16), max_iterations in 1..64, a finite positive threshold, out present,
+ * outlier capacity, a window listed twice): the first failure returns OKB_ERR_INVALID_ARG and names the job in
+ * okb_last_error.  A landmark-sharded context runs it as described with okb_shard_reserve_landmarks (landmark exchange
+ * first; OKB_ERR_SHARD_TIMEOUT if a peer does not arrive; without that reservation OKB_ERR_UNSUPPORTED).  Pending edits of
+ * the job windows are committed first; the call runs on the transfer stream after the solver work already launched on
+ * those windows, with one H2D copy of the job table and one D2H copy of the results, returns when they are back and
+ * changes nothing in the window or its store: the caller applies the removals and the pose.  Results per job are
+ * bit-identical to calling it alone.  n_jobs == 0 is a no-op. */
+int okb_ransac_2d2d_batch(okb_ctx* ctx, int n_jobs, const okb_ransac2d_job* jobs);
 
 /* ---- detection straight into the feature store (Frontend::detectAndDescribe, Frontend.cpp:92-114, for every camera of
  * a frame whose features the window's store is to hold) ---------------------------------------------------------------

@@ -909,6 +909,63 @@ class Estimator {
     return p.result.ret;
   }
 
+  // One okb_ransac_2d2d_batch job of Frontend::runRansac2d2d(currentFrameId, olderFrameId, ...) on every camera, with
+  // its parameters (threshold_ = 9, max_iterations_ = 50), initialize_pose = initializePose (the caller's
+  // initializePose && !isInitialized_) and `seed`.  Returns false when either frame has no features: every camera has
+  // then fewer than 10 correspondences and the reference returns -1 with rotationOnly (:802-808).
+  // finishRansac2d2d applies the device's outliers and pose.
+  struct Ransac2d2dPlan {
+    uint64_t frameId = 0;
+    std::vector<okb_ransac2d_outlier> outliers;
+    okb_ransac2d_result result{};
+    okb_ransac2d_job job{};
+  };
+  bool planRansac2d2d(uint64_t currentFrameId, uint64_t olderFrameId, bool initializePose, uint64_t seed, Ransac2d2dPlan& p) {
+    if (!states_.count(currentFrameId) || !states_.count(olderFrameId))
+      throw std::runtime_error("okvis_b200: runRansac2d2d: frame " + std::to_string(states_.count(currentFrameId) ? olderFrameId : currentFrameId) +
+                               " is not in the window");
+    auto fb = featSlot_.find(currentFrameId), fa = featSlot_.find(olderFrameId);
+    if (fa == featSlot_.end() || fb == featSlot_.end()) return false;
+    size_t n = 0;
+    for (const FrameFeatures& f : feats_.at(olderFrameId)) n += f.kp.size();
+    p.frameId = currentFrameId;
+    p.outliers.assign(std::max<size_t>(n, 1), okb_ransac2d_outlier{});
+    p.result = okb_ransac2d_result{};
+    p.job = okb_ransac2d_job{};
+    p.job.win = slot_;
+    p.job.pose_b = (int32_t)posePos(currentFrameId); p.job.feat_slot_b = fb->second;
+    p.job.pose_a = (int32_t)posePos(olderFrameId); p.job.feat_slot_a = fa->second;
+    p.job.n_cams = (int32_t)cameras_.size(); p.job.initialize_pose = initializePose ? 1 : 0;
+    p.job.max_iterations = 50; p.job.threshold = 9.0; p.job.seed = seed;
+    p.job.outliers = p.outliers.data(); p.job.outlier_cap = (int32_t)n; p.job.out = &p.result;
+    return true;
+  }
+  // Frontend.cpp:735-753 and :756-798 for the device's results.  Each outlier record names the correspondence's B
+  // keypoint (okvis_b200.h's one departure): removeObservation (when removeOutliers), then the keypoint's id set to 0,
+  // the order of finishRansac3d2d.  A B keypoint that several A keypoints of one landmark matched comes in more than one
+  // record; the first applies it, the others find the id already 0 and are skipped.  Throws unless each applied record's
+  // store slot is the slot of the keypoint's host id.  With pose_set, set_T_WS(frameId, T_WS) before returning, so the
+  // next round sees the pose.  Returns what runRansac2d2d returns and sets rotationOnly.
+  int finishRansac2d2d(const Ransac2d2dPlan& p, bool removeOutliers, bool& rotationOnly) {
+    for (int i = 0; i < p.result.n_outliers; ++i) {
+      const okb_ransac2d_outlier& o = p.outliers[i];
+      const uint64_t id = feats_.at(p.frameId)[o.cam].lm[o.kp_b];
+      if (id == 0) continue;
+      auto s = lmSlot_.find(id);
+      if (s == lmSlot_.end() || s->second != (uint32_t)o.lm_slot)
+        throw std::runtime_error("okvis_b200: runRansac2d2d: the store and the frame's landmark ids disagree");
+      if (removeOutliers) removeObservation(id, p.frameId, (size_t)o.cam, (size_t)o.kp_b);
+      setFrameLandmarkId(p.frameId, (size_t)o.cam, (size_t)o.kp_b, 0);
+    }
+    if (p.result.pose_set) {
+      Pose7 T;
+      for (int k = 0; k < 7; ++k) T[k] = p.result.T_WS[k];
+      set_T_WS(p.frameId, T);
+    }
+    rotationOnly = p.result.rotation_only != 0;
+    return p.result.ret;
+  }
+
   // One okb_detect_describe_store_batch job of this session's frame: images[c] for camera c, detected with `prm` into the
   // frame's feature slot.  checkDetectStore throws what planDetectStore would, without touching anything;
   // planDetectStore takes (or reuses) the frame's feature slot as setFrameFeatures does; finishDetectStore records the

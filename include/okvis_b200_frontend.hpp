@@ -24,8 +24,11 @@
 // (:575-642) rejects 3D-2D outliers on the device (okb_ransac_3d2d_batch: the adapter's correspondences, the project's
 // own sampler and generalised P3P, the reference's score and decision) and applies them through
 // Estimator::removeObservation and Estimator::setFrameLandmarkId; with RansacHooks::device3d2d set,
-// dataAssociationAndInitialization runs it at both of the reference's call points.  runRansac2d2d (on OpenGV) stays
-// with the adaptor, in RansacHooks.  Frontend::detectAndDescribe(estimator, frameId, images) detects every camera of a
+// dataAssociationAndInitialization runs it at both of the reference's call points.  Frontend::runRansac2d2d (:645-810)
+// rejects 2D-2D outliers and initialises the pose on the device (okb_ransac_2d2d_batch: the adapter's correspondences,
+// the project's own sampler, two-point rotation and five-point solvers, the reference's scores, decision and pose
+// chain), applies the outliers the same way and the pose with Estimator::set_T_WS; with RansacHooks::device2d2d set,
+// dataAssociationAndInitialization runs it at both of its call points.  Without those flags the hooks keep OpenGV.  Frontend::detectAndDescribe(estimator, frameId, images) detects every camera of a
 // frame straight into the frame's feature slot of the estimator's store (okb_detect_describe_store_batch: one device
 // call, the descriptors stay on the device), in place of the single-image detectAndDescribe + setFrameFeatures; its
 // EstimatorGroup form makes one call for many sessions.  Each call has one body: a group form validates its list once,
@@ -48,13 +51,19 @@ namespace okvis_b200 {
 
 // Frontend::RansacHooks (declared here so that its defaults hold in Frontend's default arguments): the three places
 // where the reference runs RANSAC, each receiving the session index (0 for the single form) and that
-// session's initialisation flag.  The adaptor keeps OpenGV there and reports outliers through
+// session's initialisation flag.  Without device3d2d / device2d2d the adaptor keeps OpenGV there and reports outliers through
 // Estimator::removeObservation and Estimator::setFrameLandmarkId(..., 0).  An empty hook means no RANSAC.
 struct FrontendRansacHooks {
   // true: runRansac3d2d on the device at both of its call points, before the hooks there are called -- after the
   // first keyframe's 2D-2D rounds for initialised sessions (:434-436) and after matchToLastFrame's 3D-2D rounds
   // (:496-497) -- one device call for all sessions that reach the point; afterKeyframe is then left with runRansac2d2d
+  // (nothing, with device2d2d)
   bool device3d2d = false;
+  // true: runRansac2d2d on the device at both of its call points, before the hooks there are called -- after each
+  // keyframe's 2D-2D rounds for sessions that are not initialised, with initializePose (:438-446), and after
+  // matchToLastFrame's 2D-2D rounds, without (:512-515) -- one device call per point and keyframe index for all sessions
+  // that reach it; rotationOnly_tmp then comes from the device and afterKeyframe's return value is not used
+  bool device2d2d = false;
   // after each keyframe's 2D-2D rounds of matchToKeyframes (:432-447): runRansac3d2d when kfcounter == 0 and
   // initialised, runRansac2d2d while not initialised; returns rotationOnly_tmp (empty hook: false)
   std::function<bool(size_t session, bool initialized, size_t kfcounter, uint64_t olderFrameId)> afterKeyframe;
@@ -282,6 +291,33 @@ class Frontend {
     return ransacGroup(group, sessions, currentFrameIds, removeOutliers);
   }
 
+  // ---- 2D-2D outlier rejection and pose initialisation (device: okb_ransac_2d2d_batch)
+  // Frontend::runRansac2d2d (Frontend.cpp:645-810) between the current frame and an older one: one device job
+  // (threshold 9, 50 hypotheses per problem, seed = currentFrameId, initialize_pose = initializePose && !isInitialized_
+  // of this Frontend), then Estimator::finishRansac2d2d: every outlier's B keypoint removed (removeObservation when
+  // removeOutliers, then setFrameLandmarkId(..., 0)) and, when the device initialised the pose, set_T_WS.  Returns what
+  // the reference returns and sets rotationOnly.
+  int runRansac2d2d(Estimator& estimator, uint64_t currentFrameId, uint64_t olderFrameId, bool initializePose, bool removeOutliers,
+                    bool& rotationOnly) {
+    std::vector<char> ro;
+    const int r = ransac2dGroup(*estimator.group_, {&estimator}, {currentFrameId}, {olderFrameId},
+                                {(char)(initializePose && !isInitialized_ ? 1 : 0)}, removeOutliers, ro)[0];
+    rotationOnly = ro[0] != 0;
+    return r;
+  }
+  // The same for sessions of one EstimatorGroup, with each session's own initialisation flag: one okb_ransac_2d2d_batch
+  // for all listed sessions; results[i], rotationOnly[i], the removals and the pose equal the single call's on
+  // sessions[i] with isInitialized_ = initialized[i].
+  std::vector<int> runRansac2d2d(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& currentFrameIds,
+                                 const std::vector<uint64_t>& olderFrameIds, bool initializePose, const std::vector<char>& initialized,
+                                 bool removeOutliers, std::vector<char>& rotationOnly) {
+    group.validate(sessions);
+    if (initialized.size() != sessions.size()) throw std::invalid_argument("okvis_b200: one initialisation flag per session");
+    std::vector<char> init(sessions.size());
+    for (size_t i = 0; i < sessions.size(); ++i) init[i] = initializePose && !initialized[i] ? 1 : 0;
+    return ransac2dGroup(group, sessions, currentFrameIds, olderFrameIds, init, removeOutliers, rotationOnly);
+  }
+
   // ---- one frame of Frontend::dataAssociationAndInitialization (Frontend.cpp:117-271)
   using RansacHooks = FrontendRansacHooks;
   struct FrameResult {
@@ -367,11 +403,27 @@ class Frontend {
       for (size_t i : at) { s.push_back(sessions[i]); f.push_back(frameIds[i]); ni.push_back(newIds[i]); }
       // matchToKeyframes (:373-460)
       const std::vector<TrackResult> kf3 = trackGroup(group, s, f, true);
-      std::vector<char> rotationOnly(at.size(), 1), first(at.size(), 1);
+      std::vector<char> rotationOnly(at.size(), 1), first(at.size(), 1), deviceRotationOnly(at.size(), 0);
       auto afterKeyframe = [&](size_t k, size_t kf, uint64_t older) {
-        const bool tmp = hooks.afterKeyframe ? hooks.afterKeyframe(at[k], initialized[at[k]] != 0, kf, older) : false;
+        const bool hook = hooks.afterKeyframe ? hooks.afterKeyframe(at[k], initialized[at[k]] != 0, kf, older) : false;
+        const bool tmp = hooks.device2d2d ? deviceRotationOnly[k] != 0 : hook;
         if (first[k]) { rotationOnly[k] = tmp ? 1 : 0; first[k] = 0; }
       };
+      std::function<void(const std::vector<size_t>&, const std::vector<uint64_t>&)> keyframeRansac2d;
+      if (hooks.device2d2d)
+        keyframeRansac2d = [&](const std::vector<size_t>& ks, const std::vector<uint64_t>& older) {   // !isInitialized_ (:438-442)
+          std::vector<Estimator*> rs;
+          std::vector<uint64_t> rf, ro;
+          std::vector<size_t> rk;
+          for (size_t j = 0; j < ks.size(); ++j) {
+            deviceRotationOnly[ks[j]] = 0;                                 // rotationOnly_tmp = false (:437)
+            if (!initialized[at[ks[j]]]) { rs.push_back(s[ks[j]]); rf.push_back(f[ks[j]]); ro.push_back(older[j]); rk.push_back(ks[j]); }
+          }
+          if (rs.empty()) return;
+          std::vector<char> rot;
+          ransac2dGroup(group, rs, rf, ro, std::vector<char>(rs.size(), 1), true, rot);
+          for (size_t j = 0; j < rk.size(); ++j) deviceRotationOnly[rk[j]] = rot[j];
+        };
       std::function<void(const std::vector<size_t>&)> firstKeyframeRansac;
       if (hooks.device3d2d)
         firstKeyframeRansac = [&](const std::vector<size_t>& ks) {      // kfcounter == 0 && isInitialized_ (:434-436)
@@ -380,7 +432,7 @@ class Frontend {
           for (size_t k : ks) if (initialized[at[k]]) { rs.push_back(s[k]); rf.push_back(f[k]); }
           if (!rs.empty()) ransacGroup(group, rs, rf, true);
         };
-      const std::vector<TrackResult> kf2 = match2D2DGroup(group, s, f, ni, true, afterKeyframe, firstKeyframeRansac);
+      const std::vector<TrackResult> kf2 = match2D2DGroup(group, s, f, ni, true, afterKeyframe, firstKeyframeRansac, keyframeRansac2d);
       for (size_t k = 0; k < at.size(); ++k) {
         out[at[k]].num3dMatches = kf3[k].numMatches + kf2[k].numMatches;
         if (!initialized[at[k]] && !rotationOnly[k]) initialized[at[k]] = 1;     // (:184-189)
@@ -411,6 +463,14 @@ class Frontend {
       if (hooks.afterLastFrame3D2D)
         for (size_t k = 0; k < at.size(); ++k) if (last[k]) hooks.afterLastFrame3D2D(at[k], initialized[at[k]] != 0);
       match2D2DGroup(group, s, f, ni, false, {});
+      if (hooks.device2d2d) {                                              // !isInitialized_ (:512-515)
+        std::vector<Estimator*> rs;
+        std::vector<uint64_t> rf, ro;
+        for (size_t k = 0; k < at.size(); ++k)
+          if (last[k] && !initialized[at[k]]) { rs.push_back(s[k]); rf.push_back(f[k]); ro.push_back(s[k]->frameIdByAge(1)); }
+        std::vector<char> rot;
+        if (!rs.empty()) ransac2dGroup(group, rs, rf, ro, std::vector<char>(rs.size(), 0), true, rot);
+      }
       if (hooks.afterLastFrame2D2D)
         for (size_t k = 0; k < at.size(); ++k) if (last[k]) hooks.afterLastFrame2D2D(at[k], initialized[at[k]] != 0);
     }
@@ -434,7 +494,8 @@ class Frontend {
   std::vector<TrackResult> match2D2DGroup(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
                                           const std::vector<std::function<uint64_t()>>& newIds, bool keyframes,
                                           const std::function<void(size_t, size_t, uint64_t)>& afterKeyframe,
-                                          const std::function<void(const std::vector<size_t>&)>& firstKeyframeDone = {}) {
+                                          const std::function<void(const std::vector<size_t>&)>& firstKeyframeDone = {},
+                                          const std::function<void(const std::vector<size_t>&, const std::vector<uint64_t>&)>& keyframeDone = {}) {
     const size_t n = sessions.size();
     if (frameIds.size() != n || newIds.size() != n) throw std::invalid_argument("okvis_b200: one frame id and one id source per session");
     std::vector<std::vector<Estimator::TrackRound>> rounds(n);
@@ -455,6 +516,11 @@ class Frontend {
         std::vector<size_t> done;
         for (size_t i : closing) if (r < sessions[i]->cameras_.size()) done.push_back(i);
         if (!done.empty()) firstKeyframeDone(done);
+      }
+      if (keyframeDone && !closing.empty()) {          // every session whose keyframe's rounds end here, with that keyframe
+        std::vector<uint64_t> older;
+        for (size_t i : closing) older.push_back(rounds[i][r].frameA);
+        keyframeDone(closing, older);
       }
       if (afterKeyframe)
         for (size_t i : closing) afterKeyframe(i, r / sessions[i]->cameras_.size(), rounds[i][r].frameA);
@@ -596,6 +662,31 @@ class Frontend {
     }
     if (!jobs.empty()) throwIfFailed(group.ctx_, okb_ransac_3d2d_batch(group.ctx_, (int)jobs.size(), jobs.data()));
     for (size_t i = 0; i < n; ++i) if (has[i]) out[i] = sessions[i]->finishRansac3d2d(plans[i], removeOutliers);
+    return out;
+  }
+
+  std::vector<int> ransac2dGroup(EstimatorGroup& group, const std::vector<Estimator*>& sessions, const std::vector<uint64_t>& frameIds,
+                                 const std::vector<uint64_t>& olderIds, const std::vector<char>& initializePose, bool removeOutliers,
+                                 std::vector<char>& rotationOnly) {
+    const size_t n = sessions.size();
+    if (frameIds.size() != n || olderIds.size() != n || initializePose.size() != n)
+      throw std::invalid_argument("okvis_b200: one current frame id, older frame id and pose flag per session");
+    std::vector<int> out(n, -1);                      // no features: no camera reaches 10 correspondences (:802-808)
+    rotationOnly.assign(n, 1);
+    std::vector<Estimator::Ransac2d2dPlan> plans(n);
+    std::vector<char> has(n, 0);
+    std::vector<okb_ransac2d_job> jobs;
+    for (size_t i = 0; i < n; ++i) {
+      has[i] = sessions[i]->planRansac2d2d(frameIds[i], olderIds[i], initializePose[i] != 0, frameIds[i], plans[i]) ? 1 : 0;
+      if (has[i]) jobs.push_back(plans[i].job);
+    }
+    if (!jobs.empty()) throwIfFailed(group.ctx_, okb_ransac_2d2d_batch(group.ctx_, (int)jobs.size(), jobs.data()));
+    for (size_t i = 0; i < n; ++i)
+      if (has[i]) {
+        bool ro = true;
+        out[i] = sessions[i]->finishRansac2d2d(plans[i], removeOutliers, ro);
+        rotationOnly[i] = ro ? 1 : 0;
+      }
     return out;
   }
 

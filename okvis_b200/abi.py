@@ -165,6 +165,25 @@ class RansacJob(C.Structure):
                 ("outliers", C.c_void_p), ("outlier_cap", C.c_int32), ("_pad", C.c_int32), ("out", C.POINTER(RansacResult))]
 
 
+class Ransac2dCam(C.Structure):
+    _fields_ = [("n_correspondences", C.c_int32), ("rot_inliers", C.c_int32), ("rel_inliers", C.c_int32),
+                ("rot_best", C.c_int32), ("rel_best", C.c_int32), ("rotation_only", C.c_int32), ("applied", C.c_int32),
+                ("n_outliers", C.c_int32), ("R_rot", C.c_double * 9), ("R_rel", C.c_double * 9), ("t_rel", C.c_double * 3)]
+
+
+class Ransac2dResult(C.Structure):
+    _fields_ = [("ret", C.c_int32), ("rotation_only", C.c_int32), ("pose_set", C.c_int32), ("n_outliers", C.c_int32),
+                ("T_WS", C.c_double * 7)]
+
+
+class Ransac2dJob(C.Structure):
+    _fields_ = [("win", C.c_int32), ("pose_b", C.c_int32), ("feat_slot_b", C.c_int32), ("pose_a", C.c_int32),
+                ("feat_slot_a", C.c_int32), ("n_cams", C.c_int32), ("initialize_pose", C.c_int32),
+                ("max_iterations", C.c_int32), ("threshold", C.c_double), ("seed", C.c_uint64),
+                ("hyp_inliers", C.POINTER(C.c_int32)), ("cams", C.POINTER(Ransac2dCam)), ("outliers", C.c_void_p),
+                ("outlier_cap", C.c_int32), ("_pad", C.c_int32), ("out", C.POINTER(Ransac2dResult))]
+
+
 class DetectStoreJob(C.Structure):
     _fields_ = [("win", C.c_int32), ("feat_slot", C.c_int32), ("n_cams", C.c_int32), ("_pad", C.c_int32),
                 ("images", C.POINTER(ImageDesc)), ("out_kp", C.c_void_p), ("out_desc", C.c_void_p), ("n_out", C.POINTER(C.c_int32))]
@@ -226,6 +245,7 @@ pair_dtype = np.dtype([("index_a", "<i4"), ("distance", "<f4")], align=True)
 stereo_match_dtype = np.dtype([("kp_a", "<i4"), ("kp_b", "<i4"), ("lm_slot_a", "<i4"), ("lm_slot_b", "<i4"),
                                ("can_be_initialized", "<i4"), ("_pad", "<i4"), ("hp_W", "<f8", (4,))], align=True)
 ransac_outlier_dtype = np.dtype([("cam", "<i4"), ("kp", "<i4"), ("lm_slot", "<i4")], align=True)
+ransac2d_outlier_dtype = np.dtype([("cam", "<i4"), ("kp_a", "<i4"), ("kp_b", "<i4"), ("lm_slot", "<i4")], align=True)
 track_assoc_dtype = np.dtype([("round", "<i4"), ("cam_b", "<i4"), ("kp_b", "<i4"), ("lm_slot", "<i4"), ("uncertain", "<i4"),
                               ("_pad", "<i4")], align=True)
 

@@ -765,6 +765,48 @@ class Context:
             res.append(r)
         return res
 
+    def ransac_2d2d_batch(self, jobs):
+        """okb_ransac_2d2d_batch.  jobs: dicts with win, pose_b, feat_slot_b, pose_a, feat_slot_a, n_cams, seed and
+        optionally initialize_pose (False), max_iterations (50) and threshold (9.0).  Returns one dict per job:
+        okb_ransac2d_result's fields (T_WS as an array of 7), cams (one dict of okb_ransac2d_cam's fields per camera, the
+        models as arrays: R_rot and R_rel 3x3, t_rel), hyp_inliers ([n_cams][2][max_iterations], problem 0: rotation-only,
+        1: five-point) and outliers (ransac2d_outlier_dtype, cameras ascending, then correspondence order)."""
+        arr = (abi.Ransac2dJob * max(len(jobs), 1))()
+        outs = []
+        for i, j in enumerate(jobs):
+            n_hyp, n_cams = int(j.get("max_iterations", 50)), int(j["n_cams"])
+            cap = int(j.get("outlier_cap", max(n_cams, 0) * getattr(self, "_feat", {}).get(int(j["win"]), 0)))
+            o = dict(res=abi.Ransac2dResult(), cams=(abi.Ransac2dCam * max(n_cams, 1))(),
+                     hyp=np.zeros(max(n_cams * 2 * n_hyp, 1), np.int32), outl=np.zeros(max(cap, 1), abi.ransac2d_outlier_dtype))
+            t = arr[i]
+            (t.win, t.pose_b, t.feat_slot_b, t.pose_a, t.feat_slot_a) = (
+                int(j[k]) for k in ("win", "pose_b", "feat_slot_b", "pose_a", "feat_slot_a"))
+            t.n_cams, t.initialize_pose, t.max_iterations = n_cams, int(bool(j.get("initialize_pose", False))), n_hyp
+            t.threshold, t.seed = float(j.get("threshold", 9.0)), int(j["seed"]) & 0xFFFFFFFFFFFFFFFF
+            t.hyp_inliers = o["hyp"].ctypes.data_as(C.POINTER(C.c_int32))
+            t.cams = C.cast(o["cams"], C.POINTER(abi.Ransac2dCam))
+            t.outliers, t.outlier_cap = o["outl"].ctypes.data, cap
+            t.out = C.pointer(o["res"]) if j.get("out", True) is not None else None
+            outs.append((o, n_hyp, n_cams))
+        self._check(lib().okb_ransac_2d2d_batch(self._h, len(jobs), arr))
+        res = []
+        for o, n_hyp, n_cams in outs:
+            r = {k: getattr(o["res"], k) for k, _ in abi.Ransac2dResult._fields_ if k != "T_WS"}
+            r["T_WS"] = np.array(o["res"].T_WS[:])
+            cams = []
+            for c in range(n_cams):
+                oc = o["cams"][c]
+                d = {k: getattr(oc, k) for k, _ in abi.Ransac2dCam._fields_ if k not in ("R_rot", "R_rel", "t_rel")}
+                d["R_rot"] = np.array(oc.R_rot[:]).reshape(3, 3)
+                d["R_rel"] = np.array(oc.R_rel[:]).reshape(3, 3)
+                d["t_rel"] = np.array(oc.t_rel[:])
+                cams.append(d)
+            r["cams"] = cams
+            r["hyp_inliers"] = o["hyp"][:n_cams * 2 * n_hyp].reshape(n_cams, 2, n_hyp).copy()
+            r["outliers"] = o["outl"][:r["n_outliers"]].copy()
+            res.append(r)
+        return res
+
     def hamming_match_batch(self, jobs, desc_bytes):
         """okb_hamming_match_batch over `jobs`: make_match_job results, or dicts of its keyword arguments.  Returns one
         dict(topk, pairs) per job, like hamming_match / hamming_match_gated."""

@@ -172,12 +172,13 @@ struct okb_frontend_state {
   CallBuffers stereo;              // okb_match2d2d_batch / okb_stereo_init_batch
   CallBuffers kf;                  // okb_keyframe_overlap_batch (scratch: images too large for shared memory)
   CallBuffers ransac;              // okb_ransac_3d2d_batch
+  CallBuffers ransac2d;            // okb_ransac_2d2d_batch
 };
 
 void okb_frontend_release(okb_ctx* c) {
   if (!c->frontend) return;
   okb_frontend_state* F = c->frontend;
-  for (CallBuffers* b : {&F->match_io, &F->batch_match, &F->track, &F->stereo, &F->kf, &F->ransac}) b->release();
+  for (CallBuffers* b : {&F->match_io, &F->batch_match, &F->track, &F->stereo, &F->kf, &F->ransac, &F->ransac2d}) b->release();
   F->batch_det.release();
   if (F->batch_stream) cudaStreamDestroy(F->batch_stream);
   if (F->store_ready) cudaEventDestroy(F->store_ready);
@@ -3209,17 +3210,18 @@ __device__ __forceinline__ unsigned long long rs_draw(unsigned long long seed, i
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
   return z ^ (z >> 31);
 }
-// 4 distinct indices in [0, n) (multiply-shift of the draw's high word); a duplicate is redrawn with the next counter,
+// K distinct indices in [0, n) (multiply-shift of the draw's high word); a duplicate is redrawn with the next counter,
 // at most 64 draws (false: no sample)
+template <int K>
 __device__ bool rs_sample(unsigned long long seed, int h, int n, int* idx) {
   int m = 0;
-  for (int c = 0; c < 64 && m < 4; ++c) {
+  for (int c = 0; c < 64 && m < K; ++c) {
     const int v = (int)(((rs_draw(seed, h, c) >> 32) * (unsigned long long)n) >> 32);
     bool dup = false;
     for (int i = 0; i < m; ++i) dup = dup || idx[i] == v;
     if (!dup) idx[m++] = v;
   }
-  return m == 4;
+  return m == K;
 }
 
 __device__ __forceinline__ double rs_dot(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
@@ -3246,34 +3248,36 @@ __device__ void rs_bmul(const double (*A)[5], const double (*B)[5], double (*Cm)
     }
 }
 
-// The roots of p (degree <= 8) in (0, B], B = Cauchy's bound of p made monic after dropping leading coefficients below
-// 1e-14 of the largest, ascending.  Level m = 1..n takes the (n-m)-th derivative: between consecutive roots of the level
-// below (and 0, B) it is monotone, and each sign change is bisected RS_BISECT times.
-__device__ int rs_positive_roots(const double* p, double* roots) {
+// The roots of p (degree <= D) in (0, B] (SIGNED: in (-B, B]), B = Cauchy's bound of p made monic after dropping
+// leading coefficients below 1e-14 of the largest, ascending.  Level m = 1..n takes the (n-m)-th derivative: between
+// consecutive roots of the level below (and the interval's ends) it is monotone, and each sign change is bisected
+// RS_BISECT times.
+template <int D, bool SIGNED>
+__device__ int rs_real_roots(const double* p, double* roots) {
   double mx = 0.0;
-  for (int i = 0; i <= 8; ++i) {
+  for (int i = 0; i <= D; ++i) {
     if (!isfinite(p[i])) return 0;
     mx = fmax(mx, fabs(p[i]));
   }
-  int n = 8;
+  int n = D;
   while (n > 0 && !(fabs(p[n]) > 1e-14 * mx)) --n;
   if (n == 0) return 0;
-  double q[9];
+  double q[D + 1];
   for (int i = 0; i <= n; ++i) q[i] = p[i] / p[n];
   double bound = 0.0;
   for (int i = 0; i < n; ++i) bound = fmax(bound, fabs(q[i]));
   bound += 1.0;
   int nr = 0;
   for (int m = 1; m <= n; ++m) {
-    double c[9];
+    double c[D + 1];
     for (int i = 0; i <= m; ++i) {
       double f = q[i + n - m];
       for (int t = i + 1; t <= i + n - m; ++t) f *= (double)t;
       c[i] = f;
     }
-    double nxt[8];
+    double nxt[D];
     int k = 0;
-    double lo = 0.0, flo = rs_horner(c, m, 0.0);
+    double lo = SIGNED ? -bound : 0.0, flo = rs_horner(c, m, lo);
     for (int e = 0; e <= nr; ++e) {
       const double hi = e < nr ? roots[e] : bound;
       const double fhi = rs_horner(c, m, hi);
@@ -3292,6 +3296,15 @@ __device__ int rs_positive_roots(const double* p, double* roots) {
     nr = k;
   }
   return nr;
+}
+
+// The triad of an edge u1 and a normal nn: rows e1 = u1 / |u1|, e2 = n x e1, n = nn / |nn|
+__device__ __forceinline__ void rs_triad(const double* u1, const double* nn, double (*Fr)[3]) {
+  const double i1 = 1.0 / sqrt(rs_dot(u1, u1)), in = 1.0 / sqrt(rs_dot(nn, nn));
+  for (int k = 0; k < 3; ++k) { Fr[0][k] = u1[k] * i1; Fr[2][k] = nn[k] * in; }
+  Fr[1][0] = Fr[2][1] * Fr[0][2] - Fr[2][2] * Fr[0][1];
+  Fr[1][1] = Fr[2][2] * Fr[0][0] - Fr[2][0] * Fr[0][2];
+  Fr[1][2] = Fr[2][0] * Fr[0][1] - Fr[2][1] * Fr[0][0];
 }
 
 // Generalised P3P: rays c_i + l_i f_i (body frame, |f_i| = 1) through world points X_i, i = 0..2.  Depths solve
@@ -3360,7 +3373,7 @@ __device__ void rs_gp3p(const double (*c)[3], const double (*f)[3], const double
   rs_umul(al, 3, be, 4, u);   rs_umul(u, 7, a, 1, t);  for (int i = 0; i < 9; ++i) oct[i] -= t[i];
   rs_umul(be, 4, be, 4, u);   for (int i = 0; i < 9; ++i) oct[i] += u[i];
   double roots[8];
-  const int nr = rs_positive_roots(oct, roots);
+  const int nr = rs_real_roots<8, false>(oct, roots);
   for (int r = 0; r < nr; ++r) {
     double x = roots[r];
     const double alx = rs_horner(al, 3, x), bex = rs_horner(be, 4, x);
@@ -3403,15 +3416,10 @@ __device__ void rs_gp3p(const double (*c)[3], const double (*f)[3], const double
     double Fp[3][3], Fx[3][3];                        // rows: e1, e2, n
     for (int side = 0; side < 2; ++side) {
       const double (*P)[3] = side ? X : p;
-      double (*Fr)[3] = side ? Fx : Fp;
       double u1[3], u2[3], nn[3];
       for (int k = 0; k < 3; ++k) { u1[k] = P[1][k] - P[0][k]; u2[k] = P[2][k] - P[0][k]; }
       nn[0] = u1[1] * u2[2] - u1[2] * u2[1]; nn[1] = u1[2] * u2[0] - u1[0] * u2[2]; nn[2] = u1[0] * u2[1] - u1[1] * u2[0];
-      const double i1 = 1.0 / sqrt(rs_dot(u1, u1)), in = 1.0 / sqrt(rs_dot(nn, nn));
-      for (int k = 0; k < 3; ++k) { Fr[0][k] = u1[k] * i1; Fr[2][k] = nn[k] * in; }
-      Fr[1][0] = Fr[2][1] * Fr[0][2] - Fr[2][2] * Fr[0][1];
-      Fr[1][1] = Fr[2][2] * Fr[0][0] - Fr[2][0] * Fr[0][2];
-      Fr[1][2] = Fr[2][0] * Fr[0][1] - Fr[2][1] * Fr[0][0];
+      rs_triad(u1, nn, side ? Fx : Fp);
     }
     double R[9], tt[3];
     for (int r0 = 0; r0 < 3; ++r0)
@@ -3421,6 +3429,26 @@ __device__ void rs_gp3p(const double (*c)[3], const double (*f)[3], const double
     for (int k = 0; k < 3; ++k) { pc[k] = (p[0][k] + p[1][k] + p[2][k]) / 3.0; xc[k] = (X[0][k] + X[1][k] + X[2][k]) / 3.0; }
     for (int k = 0; k < 3; ++k) tt[k] = xc[k] - (R[3 * k] * pc[0] + R[3 * k + 1] * pc[1] + R[3 * k + 2] * pc[2]);
     emit(R, tt);
+  }
+}
+
+// Eigen's Quaternion(Matrix3d) of M (row-major), q = [x, y, z, w]
+__device__ __forceinline__ void rs_quat(const double* M, double* q) {
+  const double tr = M[0] + M[4] + M[8];
+  if (tr > 0.0) {
+    double s = sqrt(tr + 1.0);
+    q[3] = 0.5 * s; s = 0.5 / s;
+    q[0] = (M[7] - M[5]) * s; q[1] = (M[2] - M[6]) * s; q[2] = (M[3] - M[1]) * s;
+  } else {
+    int i = 0;
+    if (M[4] > M[0]) i = 1;
+    if (M[8] > M[4 * i]) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    double s = sqrt(M[4 * i] - M[4 * j] - M[4 * k] + 1.0);
+    q[i] = 0.5 * s; s = 0.5 / s;
+    q[3] = (M[3 * k + j] - M[3 * j + k]) * s;
+    q[j] = (M[3 * j + i] + M[3 * i + j]) * s;
+    q[k] = (M[3 * k + i] + M[3 * i + k]) * s;
   }
 }
 
@@ -3521,7 +3549,7 @@ __global__ void __launch_bounds__(RS_T) k_ransac_3d2d(const RansacJobDev* __rest
   if (tid < J.n_hyp) {
     int idx[4];
     int ok = 0;
-    if (rs_sample(J.seed, tid, n, idx)) {
+    if (rs_sample<4>(J.seed, tid, n, idx)) {
       const double* q[4];
       bool finite = true;
       for (int i = 0; i < 4; ++i) {
@@ -3579,23 +3607,7 @@ __global__ void __launch_bounds__(RS_T) k_ransac_3d2d(const RansacJobDev* __rest
   if (best >= 0) {
     const double* M = s_model[best];
     double q[4];
-    // Eigen's Quaternion(Matrix3d)
-    const double tr = M[0] + M[4] + M[8];
-    if (tr > 0.0) {
-      double s = sqrt(tr + 1.0);
-      q[3] = 0.5 * s; s = 0.5 / s;
-      q[0] = (M[7] - M[5]) * s; q[1] = (M[2] - M[6]) * s; q[2] = (M[3] - M[1]) * s;
-    } else {
-      int i = 0;
-      if (M[4] > M[0]) i = 1;
-      if (M[8] > M[4 * i]) i = 2;
-      const int j = (i + 1) % 3, k = (j + 1) % 3;
-      double s = sqrt(M[4 * i] - M[4 * j] - M[4 * k] + 1.0);
-      q[i] = 0.5 * s; s = 0.5 / s;
-      q[3] = (M[3 * k + j] - M[3 * j + k]) * s;
-      q[j] = (M[3 * j + i] + M[3 * i + j]) * s;
-      q[k] = (M[3 * k + i] + M[3 * i + k]) * s;
-    }
+    rs_quat(M, q);
     for (int r = 0; r < 3; ++r) res.T_WS[r] = M[9 + r];
     for (int r = 0; r < 4; ++r) res.T_WS[3 + r] = q[r];
   }
@@ -3707,6 +3719,701 @@ extern "C" int okb_ransac_3d2d_batch(okb_ctx* c, int n_jobs, const okb_ransac_jo
     *j.out = *reinterpret_cast<const okb_ransac_result*>(h + o_res[i]);
     if (j.hyp_inliers) std::memcpy(j.hyp_inliers, h + o_hyp[i], 4 * (size_t)j.max_iterations);
     if (j.out->n_outliers) std::memcpy(j.outliers, h + o_out[i], sizeof(okb_ransac_outlier) * (size_t)j.out->n_outliers);
+  }
+  return OKB_OK;
+}
+
+// =================================================================================================
+// 2D-2D outlier rejection and pose initialisation (okb_ransac_2d2d_batch): Frontend::runRansac2d2d
+// (okvis_frontend/src/Frontend.cpp:645-810) on the window's feature store, one CTA per job in one launch (DESIGN.md 6i;
+// tests/ransac2d2d_reference.py restates it):
+//   1. per camera, FrameRelativeAdapter's correspondences (FrameRelativeAdapter.cpp:139-244): B's first keypoint per
+//      landmark of the graph by an atomicMin over the landmark slots, then A's keypoints compacted in order by a block
+//      scan;
+//   2. one thread per (camera, problem, hypothesis): the two-point rotation or the five-point relative pose, the 6th
+//      correspondence choosing among the five-point solutions;
+//   3. a warp per (camera, problem, hypothesis) counts its inliers; thread 0 takes the winners, the reference's decision
+//      and the pose initialisation camera by camera;
+//   4. the outlier records of the applied cameras in correspondence order (block scan).
+// The call writes nothing but its scratch and its results.
+// =================================================================================================
+namespace {
+constexpr int R2_CD = 8;           // doubles per correspondence: bearing A (3), bearing B (3), sigmaAngle A, sigmaAngle B
+constexpr int R2_TASKS = RS_MAX_CAMS * 2 * RS_MAX_HYP;
+constexpr double R2_CONS_TOL = 1e-10;  // an essential matrix is kept when its constraints hold to this, relative to |E|^3
+
+struct Ransac2JobDev {
+  const WinDev* W;
+  int feat_a, feat_b, pose_a, pose_b, n_cams, n_hyp, init_pose, L;
+  double threshold;
+  unsigned long long seed;
+  int* first;                      // [L] B's first keypoint per landmark slot (scratch)
+  double* cd;                      // [sum of A's keypoints][R2_CD] correspondences (scratch)
+  int* ci;                         // [sum of A's keypoints][3] kp_a, kp_b, landmark slot (scratch)
+  double* model;                   // [n_cams][2][n_hyp][12] R (row-major), t (scratch)
+  okb_ransac2d_result* res;
+  okb_ransac2d_cam* cams;          // [n_cams]
+  int* hyp;                        // [n_cams][2][n_hyp]
+  okb_ransac2d_outlier* outl;
+};
+
+// Monomial tables of the five-point constraints.  Linear: x, y, z, 1.  Quadratic: x^2, y^2, z^2, xy, xz, yz, x, y, z, 1.
+// Cubic (Nister's order): x^3, y^3, x^2y, xy^2, x^2z, x^2, y^2z, y^2, xyz, xy | xz^2, xz, x, yz^2, yz, y, z^3, z^2, z, 1.
+__constant__ int8_t c_r2_ll[4][4] = {{0, 3, 4, 6}, {3, 1, 5, 7}, {4, 5, 2, 8}, {6, 7, 8, 9}};
+__constant__ int8_t c_r2_ql[10][4] = {{0, 2, 4, 5}, {3, 1, 6, 7}, {10, 13, 16, 17}, {2, 3, 8, 9}, {4, 8, 10, 11},
+                                      {8, 6, 13, 14}, {5, 9, 11, 12}, {9, 7, 14, 15}, {11, 14, 17, 18}, {12, 15, 18, 19}};
+__constant__ int8_t c_r2_exp[20][3] = {{3, 0, 0}, {0, 3, 0}, {2, 1, 0}, {1, 2, 0}, {2, 0, 1}, {2, 0, 0}, {0, 2, 1},
+                                       {0, 2, 0}, {1, 1, 1}, {1, 1, 0}, {1, 0, 2}, {1, 0, 1}, {1, 0, 0}, {0, 1, 2},
+                                       {0, 1, 1}, {0, 1, 0}, {0, 0, 3}, {0, 0, 2}, {0, 0, 1}, {0, 0, 0}};
+
+__device__ __forceinline__ void r2_cross(const double* a, const double* b, double* c) {
+  c[0] = a[1] * b[2] - a[2] * b[1]; c[1] = a[2] * b[0] - a[0] * b[2]; c[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// triangulate2 as specified (DESIGN.md 6i): the midpoint of the common perpendicular of l1 f1 and t + l2 R f2, the 2x2
+// normal equations solved in closed form; l = (l1, l2)
+__device__ __forceinline__ void r2_triangulate(const double* R, const double* t, const double* f1, const double* f2, double* p, double* l) {
+  double g[3];
+  for (int r = 0; r < 3; ++r) g[r] = R[3 * r] * f2[0] + R[3 * r + 1] * f2[1] + R[3 * r + 2] * f2[2];
+  const double a = rs_dot(f1, f1), b = rs_dot(f1, g), c = rs_dot(g, g), d1 = rs_dot(f1, t), d2 = rs_dot(g, t);
+  const double det = a * c - b * b;
+  l[0] = (c * d1 - b * d2) / det;
+  l[1] = (b * d1 - a * d2) / det;
+  for (int k = 0; k < 3; ++k) p[k] = 0.5 * (l[0] * f1[k] + (t[k] + l[1] * g[k]));
+}
+
+// FrameRotationOnlySacProblem::getSelectedDistancesToModel for one correspondence.  Not inlined: the inlier count and
+// the outlier scan call one compiled body, so a score within rounding of the threshold decides both alike.
+__device__ __noinline__ double r2_score_rot(const double* R, const double* cd) {
+  double e1[3], e2[3];
+  for (int r = 0; r < 3; ++r) {
+    e1[r] = R[3 * r] * cd[3] + R[3 * r + 1] * cd[4] + R[3 * r + 2] * cd[5] - cd[r];
+    e2[r] = R[r] * cd[0] + R[3 + r] * cd[1] + R[6 + r] * cd[2] - cd[3 + r];
+  }
+  return rs_dot(e1, e1) * 0.5 / cd[6] + rs_dot(e2, e2) * 0.5 / cd[7];
+}
+
+// FrameRelativePoseSacProblem::getSelectedDistancesToModel for one correspondence (not inlined, as r2_score_rot)
+__device__ __noinline__ double r2_score_rel(const double* R, const double* t, const double* cd) {
+  double p[3], l[2], q[3];
+  r2_triangulate(R, t, cd, cd + 3, p, l);
+  for (int r = 0; r < 3; ++r) {
+    const double ti = -(R[r] * t[0] + R[3 + r] * t[1] + R[6 + r] * t[2]);
+    q[r] = R[r] * p[0] + R[3 + r] * p[1] + R[6 + r] * p[2] + ti;
+  }
+  const double n1 = sqrt(rs_dot(p, p)), n2 = sqrt(rs_dot(q, q));
+  const double e1[3] = {p[0] / n1 - cd[0], p[1] / n1 - cd[1], p[2] / n1 - cd[2]};
+  const double e2[3] = {q[0] / n2 - cd[3], q[1] / n2 - cd[4], q[2] / n2 - cd[5]};
+  return rs_dot(e1, e1) * 0.5 / cd[6] + rs_dot(e2, e2) * 0.5 / cd[7];
+}
+
+// Two-point rotation: R maps B's triad of (f_a + f_b, f_a x f_b) onto A's (R f2 = f1 for both points when noise-free)
+__device__ bool r2_rotation(const double* a0, const double* b0, const double* a1, const double* b1, double* R) {
+  double FA[3][3], FB[3][3];
+  for (int side = 0; side < 2; ++side) {
+    const double* u = side ? b0 : a0;
+    const double* v = side ? b1 : a1;
+    const double s[3] = {u[0] + v[0], u[1] + v[1], u[2] + v[2]};
+    double nn[3];
+    r2_cross(u, v, nn);
+    rs_triad(s, nn, side ? FB : FA);
+  }
+  double sum = 0.0;
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) {
+      R[3 * r + c] = FA[0][r] * FB[0][c] + FA[1][r] * FB[1][c] + FA[2][r] * FB[2][c];
+      sum += R[3 * r + c];
+    }
+  return isfinite(sum);
+}
+
+__device__ __forceinline__ double r2_det3(const double (*A)[3]) {
+  return A[0][0] * (A[1][1] * A[2][2] - A[1][2] * A[2][1]) - A[0][1] * (A[1][0] * A[2][2] - A[1][2] * A[2][0]) +
+         A[0][2] * (A[1][0] * A[2][1] - A[1][1] * A[2][0]);
+}
+
+// RS_POLISH Gauss-Newton steps of (x, y, z) on the 10 cubic constraints G0 (before elimination), the 3x3 normal
+// equations solved by Cramer's rule; stops at a singular or non-finite system
+__device__ void r2_polish(const double (*G0)[20], double& x, double& y, double& z) {
+  if (!isfinite(x + y + z)) return;
+  for (int it = 0; it < RS_POLISH; ++it) {
+    const double px[4] = {1.0, x, x * x, x * x * x}, py[4] = {1.0, y, y * y, y * y * y}, pz[4] = {1.0, z, z * z, z * z * z};
+    double g[10], Jm[10][3];
+    for (int i = 0; i < 10; ++i) { g[i] = 0.0; Jm[i][0] = Jm[i][1] = Jm[i][2] = 0.0; }
+    for (int m = 0; m < 20; ++m) {
+      const int a = c_r2_exp[m][0], b = c_r2_exp[m][1], c = c_r2_exp[m][2];
+      const double mon = px[a] * py[b] * pz[c];
+      const double dx = a * px[max(a - 1, 0)] * py[b] * pz[c];
+      const double dy = b * px[a] * py[max(b - 1, 0)] * pz[c];
+      const double dw = c * px[a] * py[b] * pz[max(c - 1, 0)];
+      for (int i = 0; i < 10; ++i) {
+        g[i] += G0[i][m] * mon;
+        Jm[i][0] += G0[i][m] * dx; Jm[i][1] += G0[i][m] * dy; Jm[i][2] += G0[i][m] * dw;
+      }
+    }
+    double A[3][3], bb[3];
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) {
+        double s = 0.0;
+        for (int k = 0; k < 10; ++k) s += Jm[k][r] * Jm[k][c];
+        A[r][c] = s;
+      }
+      double s = 0.0;
+      for (int k = 0; k < 10; ++k) s += Jm[k][r] * g[k];
+      bb[r] = s;
+    }
+    const double det = r2_det3(A);
+    if (!(det != 0.0) || !isfinite(det)) return;
+    double d[3];
+    for (int v = 0; v < 3; ++v) {
+      double Av[3][3];
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) Av[r][c] = c == v ? bb[r] : A[r][c];
+      d[v] = r2_det3(Av) / det;
+    }
+    x -= d[0]; y -= d[1]; z -= d[2];
+  }
+}
+
+// Five-point relative pose (Nister's formulation, DESIGN.md 6i) on correspondences (f1[i], f2[i]), i = 0..4, with
+// f1^T E f2 = 0, E = [t]x R: the null space of the 5x9 epipolar system by Householder QR, E = x X + y Y + z Z + W, the
+// 10 cubic constraints Gauss-Jordan eliminated (partial pivoting), the degree-10 polynomial in z, its real roots, (x, y)
+// from the first two rows of the 3x3 polynomial system, RS_POLISH Gauss-Newton steps of (x, y, z) on the 10 cubic
+// constraints, E kept when det E and 2 E E^T E - tr(E E^T) E vanish to R2_CONS_TOL |E|^3, and per root the 4 (R, t)
+// candidates of E.  emit(R, t) per
+// candidate whose 5 points triangulate in front of both cameras (l1 > 0, l2 > 0), roots ascending, candidates in the
+// order (R1, t), (R1, -t), (R2, t), (R2, -t).
+template <typename Emit>
+__device__ void r2_fivept(const double (*f1)[3], const double (*f2)[3], Emit&& emit) {
+  double M[9][5];                                   // the epipolar system, transposed
+  for (int i = 0; i < 5; ++i)
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) M[3 * r + c][i] = f1[i][r] * f2[i][c];
+  double V[5][9], beta[5];
+  for (int j = 0; j < 5; ++j) {
+    double nx = 0.0;
+    for (int i = j; i < 9; ++i) nx += M[i][j] * M[i][j];
+    nx = sqrt(nx);
+    const double alpha = M[j][j] < 0.0 ? nx : -nx;
+    for (int i = 0; i < 9; ++i) V[j][i] = i < j ? 0.0 : M[i][j];
+    V[j][j] -= alpha;
+    double b = 0.0;
+    for (int i = j; i < 9; ++i) b += V[j][i] * V[j][i];
+    beta[j] = b;
+    if (!(b > 0.0)) continue;
+    for (int k = j; k < 5; ++k) {
+      double s = 0.0;
+      for (int i = j; i < 9; ++i) s += V[j][i] * M[i][k];
+      s = 2.0 * s / b;
+      for (int i = j; i < 9; ++i) M[i][k] -= s * V[j][i];
+    }
+  }
+  double N[4][9];                                   // X, Y, Z, W = Q e_5 .. Q e_8
+  for (int b4 = 0; b4 < 4; ++b4) {
+    for (int i = 0; i < 9; ++i) N[b4][i] = i == 5 + b4 ? 1.0 : 0.0;
+    for (int j = 4; j >= 0; --j) {
+      if (!(beta[j] > 0.0)) continue;
+      double s = 0.0;
+      for (int i = j; i < 9; ++i) s += V[j][i] * N[b4][i];
+      s = 2.0 * s / beta[j];
+      for (int i = j; i < 9; ++i) N[b4][i] -= s * V[j][i];
+    }
+  }
+  double G[10][20];                                 // row 0: det E; rows 1..9: 2 E E^T E - tr(E E^T) E, row-major
+  {
+    double EE[3][3][10];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) {
+        for (int q = 0; q < 10; ++q) EE[r][c][q] = 0.0;
+        for (int k = 0; k < 3; ++k)
+          for (int i = 0; i < 4; ++i)
+            for (int j = 0; j < 4; ++j) EE[r][c][c_r2_ll[i][j]] += N[i][3 * r + k] * N[j][3 * c + k];
+      }
+    double tr[10];
+    for (int q = 0; q < 10; ++q) tr[q] = EE[0][0][q] + EE[1][1][q] + EE[2][2][q];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) {
+        double S[20], T[20];
+        for (int m = 0; m < 20; ++m) S[m] = T[m] = 0.0;
+        for (int k = 0; k < 3; ++k)
+          for (int q = 0; q < 10; ++q)
+            for (int i = 0; i < 4; ++i) S[c_r2_ql[q][i]] += EE[r][k][q] * N[i][3 * k + c];
+        for (int q = 0; q < 10; ++q)
+          for (int i = 0; i < 4; ++i) T[c_r2_ql[q][i]] += tr[q] * N[i][3 * r + c];
+        for (int m = 0; m < 20; ++m) G[1 + 3 * r + c][m] = 2.0 * S[m] - T[m];
+      }
+    // det E = E00 (E11 E22 - E12 E21) - E01 (E10 E22 - E12 E20) + E02 (E10 E21 - E11 E20)
+    for (int m = 0; m < 20; ++m) G[0][m] = 0.0;
+    const int cof[3][4] = {{4, 8, 5, 7}, {3, 8, 5, 6}, {3, 7, 4, 6}};
+    const double sg[3] = {1.0, -1.0, 1.0};
+    for (int e = 0; e < 3; ++e) {
+      double mq[10];
+      for (int q = 0; q < 10; ++q) mq[q] = 0.0;
+      for (int i = 0; i < 4; ++i)
+        for (int j = 0; j < 4; ++j)
+          mq[c_r2_ll[i][j]] += N[i][cof[e][0]] * N[j][cof[e][1]] - N[i][cof[e][2]] * N[j][cof[e][3]];
+      for (int q = 0; q < 10; ++q)
+        for (int i = 0; i < 4; ++i) G[0][c_r2_ql[q][i]] += sg[e] * (N[i][e] * mq[q]);
+    }
+  }
+  double G0[10][20];
+  for (int i = 0; i < 10; ++i)
+    for (int m = 0; m < 20; ++m) G0[i][m] = G[i][m];
+  for (int j = 0; j < 10; ++j) {                    // Gauss-Jordan, partial pivoting (first largest)
+    int p = j;
+    for (int i = j + 1; i < 10; ++i)
+      if (fabs(G[i][j]) > fabs(G[p][j])) p = i;
+    if (!(G[p][j] != 0.0) || !isfinite(G[p][j])) return;
+    if (p != j)
+      for (int m = j; m < 20; ++m) { const double tmp = G[j][m]; G[j][m] = G[p][m]; G[p][m] = tmp; }
+    const double piv = G[j][j];
+    for (int m = j; m < 20; ++m) G[j][m] /= piv;
+    for (int i = 0; i < 10; ++i) {
+      if (i == j) continue;
+      const double f = G[i][j];
+      for (int m = j; m < 20; ++m) G[i][m] -= f * G[j][m];
+    }
+  }
+  // k = <e> - z <f>, l = <g> - z <h>, m = <i> - z <j>: rows (4, 5), (6, 7), (8, 9); P[row][0: x, 1: y, 2: 1][power of z]
+  double P[3][3][5];
+  for (int r = 0; r < 3; ++r) {
+    const double* a = G[4 + 2 * r];
+    const double* b = G[5 + 2 * r];
+    P[r][0][0] = a[12]; P[r][0][1] = a[11] - b[12]; P[r][0][2] = a[10] - b[11]; P[r][0][3] = -b[10]; P[r][0][4] = 0.0;
+    P[r][1][0] = a[15]; P[r][1][1] = a[14] - b[15]; P[r][1][2] = a[13] - b[14]; P[r][1][3] = -b[13]; P[r][1][4] = 0.0;
+    P[r][2][0] = a[19]; P[r][2][1] = a[18] - b[19]; P[r][2][2] = a[17] - b[18]; P[r][2][3] = a[16] - b[17]; P[r][2][4] = -b[16];
+  }
+  double dz[11];
+  {
+    double t1[8], t2[8], t3[7], u[11];
+    rs_umul(P[1][1], 3, P[2][2], 4, t1); rs_umul(P[1][2], 4, P[2][1], 3, u);  for (int i = 0; i < 8; ++i) t1[i] -= u[i];
+    rs_umul(P[1][0], 3, P[2][2], 4, t2); rs_umul(P[1][2], 4, P[2][0], 3, u);  for (int i = 0; i < 8; ++i) t2[i] -= u[i];
+    rs_umul(P[1][0], 3, P[2][1], 3, t3); rs_umul(P[1][1], 3, P[2][0], 3, u);  for (int i = 0; i < 7; ++i) t3[i] -= u[i];
+    rs_umul(P[0][0], 3, t1, 7, dz);
+    rs_umul(P[0][1], 3, t2, 7, u);  for (int i = 0; i < 11; ++i) dz[i] -= u[i];
+    rs_umul(P[0][2], 4, t3, 6, u);  for (int i = 0; i < 11; ++i) dz[i] += u[i];
+  }
+  double roots[10];
+  const int nr = rs_real_roots<10, true>(dz, roots);
+  for (int ir = 0; ir < nr; ++ir) {
+    double row[2][3];
+    for (int r = 0; r < 2; ++r)
+      for (int v = 0; v < 3; ++v) row[r][v] = rs_horner(P[r][v], 4, roots[ir]);
+    double u[3];
+    r2_cross(row[0], row[1], u);
+    if (!(u[2] != 0.0) || !isfinite(u[0] + u[1] + u[2])) continue;
+    double x = u[0] / u[2], y = u[1] / u[2], z = roots[ir];
+    r2_polish(G0, x, y, z);
+    double E[9], ss = 0.0;
+    for (int e = 0; e < 9; ++e) {
+      E[e] = x * N[0][e] + y * N[1][e] + z * N[2][e] + N[3][e];
+      ss += E[e] * E[e];
+    }
+    if (!(ss > 0.0) || !isfinite(ss)) continue;
+    const double sc = sqrt(2.0) / sqrt(ss);
+    for (int e = 0; e < 9; ++e) E[e] *= sc;
+    {                                               // det E = 0, 2 E E^T E - tr(E E^T) E = 0 to R2_CONS_TOL |E|^3
+      double EEt[9], worst = 0.0;
+      for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) EEt[3 * i + j] = E[3 * i] * E[3 * j] + E[3 * i + 1] * E[3 * j + 1] + E[3 * i + 2] * E[3 * j + 2];
+      const double tr = EEt[0] + EEt[4] + EEt[8];
+      for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j)
+          worst = fmax(worst, fabs(2.0 * (EEt[3 * i] * E[j] + EEt[3 * i + 1] * E[3 + j] + EEt[3 * i + 2] * E[6 + j]) - tr * E[3 * i + j]));
+      const double Em[3][3] = {{E[0], E[1], E[2]}, {E[3], E[4], E[5]}, {E[6], E[7], E[8]}};
+      worst = fmax(worst, fabs(r2_det3(Em)));
+      if (!(worst <= R2_CONS_TOL * 2.0 * sqrt(2.0))) continue;
+    }
+    // t: the left null vector of E, the largest cross product of two of its columns
+    double col[3][3], t[3], tn = -1.0;
+    for (int c = 0; c < 3; ++c)
+      for (int r = 0; r < 3; ++r) col[c][r] = E[3 * r + c];
+    const int pr[3][2] = {{0, 1}, {0, 2}, {1, 2}};
+    for (int e = 0; e < 3; ++e) {
+      double w[3];
+      r2_cross(col[pr[e][0]], col[pr[e][1]], w);
+      const double wn = sqrt(rs_dot(w, w));
+      if (wn > tn) { tn = wn; for (int k = 0; k < 3; ++k) t[k] = w[k]; }
+    }
+    if (!(tn > 0.0)) continue;
+    for (int k = 0; k < 3; ++k) t[k] /= tn;
+    // E = +-[t]x R: R1 = cof(E) - [t]x E, R2 = cof(E) + [t]x E
+    double Rs[2][9];
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) {
+        const int i1 = (i + 1) % 3, i2 = (i + 2) % 3, j1 = (j + 1) % 3, j2 = (j + 2) % 3;
+        const double cf = E[3 * i1 + j1] * E[3 * i2 + j2] - E[3 * i1 + j2] * E[3 * i2 + j1];
+        const double tx = t[i1] * E[3 * i2 + j] - t[i2] * E[3 * i1 + j];
+        Rs[0][3 * i + j] = cf - tx;
+        Rs[1][3 * i + j] = cf + tx;
+      }
+    for (int cand = 0; cand < 4; ++cand) {
+      const double* R = Rs[cand >> 1];
+      const double sgn = (cand & 1) ? -1.0 : 1.0;
+      const double tc[3] = {sgn * t[0], sgn * t[1], sgn * t[2]};
+      bool ok = true;
+      for (int i = 0; i < 5 && ok; ++i) {
+        double p[3], l[2];
+        r2_triangulate(R, tc, f1[i], f2[i], p, l);
+        ok = l[0] > 0.0 && l[1] > 0.0;
+      }
+      if (ok) emit(R, tc);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(RS_T) k_ransac_2d2d(const Ransac2JobDev* __restrict__ jobs) {
+  __shared__ int s_warp[RS_T / 32];
+  __shared__ int s_off[RS_MAX_CAMS + 1];            // correspondences of camera c: [s_off[c], s_off[c + 1])
+  __shared__ int s_cnt[R2_TASKS];
+  __shared__ unsigned char s_ok[R2_TASKS];
+  __shared__ int s_pick[RS_MAX_CAMS];               // the applied camera's chosen task, -1: not applied
+  const Ransac2JobDev& J = jobs[blockIdx.x];
+  const WinDev& W = *J.W;
+  const FeatStore& F = *W.feat;
+  const int tid = threadIdx.x, H = J.n_hyp;
+  for (int i = tid; i < J.L; i += RS_T) J.first[i] = INT_MAX;
+  __syncthreads();
+  // the adapter's correspondences, per camera
+  int n = 0;
+  for (int cam = 0; cam < J.n_cams; ++cam) {
+    if (tid == 0) s_off[cam] = n;
+    const int nA = F.n[(size_t)J.feat_a * F.C + cam], nB = F.n[(size_t)J.feat_b * F.C + cam];
+    const size_t bA = ((size_t)J.feat_a * F.C + cam) * F.N, bB = ((size_t)J.feat_b * F.C + cam) * F.N;
+    for (int k = tid; k < nB; k += RS_T) {
+      const int l = F.lm[bB + k];
+      if (track_live(W, J.L, l)) atomicMin(&J.first[l], k);
+    }
+    __syncthreads();
+    CamIntr ci;
+    cam_load(W.cams[cam], ci);
+    for (int k0 = 0; k0 < nA; k0 += RS_T) {
+      const int k = k0 + tid;
+      int take = 0, l = -1, kb = -1;
+      if (k < nA) {
+        l = F.lm[bA + k];
+        if (l >= 0 && l < J.L) kb = J.first[l];
+        take = kb != INT_MAX && kb >= 0 ? 1 : 0;
+      }
+      int total;
+      const int pos = block_scan<RS_T>(take, s_warp, &total);
+      if (take) {
+        double* cd = J.cd + (size_t)(n + pos) * R2_CD;
+        for (int side = 0; side < 2; ++side) {
+          const size_t e = side ? bB + kb : bA + k;
+          // PinholeCamera::backProject (its return value ignored), then bearing.normalize()
+          double pu[2];
+          undistort_gn(ci, (F.kp[2 * e] - ci.cu) * (1.0 / ci.fu), (F.kp[2 * e + 1] - ci.cv) * (1.0 / ci.fv), pu);
+          double br[3] = {pu[0], pu[1], 1.0};
+          const double n2 = rs_dot(br, br);
+          if (n2 > 0.0) { const double in = sqrt(n2); br[0] /= in; br[1] /= in; br[2] /= in; }
+          for (int r = 0; r < 3; ++r) cd[3 * side + r] = br[r];
+          const double sd = 0.8 * F.size[e] / 12.0;
+          cd[6 + side] = sqrt(2.0) * sd * sd / (ci.fu * ci.fu);
+        }
+        int* cr = J.ci + 3 * (size_t)(n + pos);
+        cr[0] = k; cr[1] = kb; cr[2] = l;
+      }
+      n += total;
+    }
+    __syncthreads();
+    for (int k = tid; k < nB; k += RS_T) {
+      const int l = F.lm[bB + k];
+      if (l >= 0 && l < J.L) J.first[l] = INT_MAX;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) s_off[J.n_cams] = n;
+  __syncthreads();                                  // the correspondences are in global scratch
+  // hypotheses, a thread each: task = (2 cam + problem) H + h
+  const int n_tasks = J.n_cams * 2 * H;
+  for (int task = tid; task < n_tasks; task += RS_T) {
+    const int cam = task / (2 * H), prob = (task / H) & 1, h = task % H;
+    const int o = s_off[cam], nc = s_off[cam + 1] - o;
+    const int key = (2 * cam + prob) * RS_MAX_HYP + h;
+    double* Mo = J.model + (size_t)task * 12;
+    int ok = 0;
+    if (nc >= 10) {
+      int idx[6];
+      const int k = prob ? 6 : 2;
+      if (prob ? rs_sample<6>(J.seed, key, nc, idx) : rs_sample<2>(J.seed, key, nc, idx)) {
+        bool finite = true;
+        for (int i = 0; i < k; ++i) {
+          const double* q = J.cd + (size_t)(o + idx[i]) * R2_CD;
+          finite = finite && isfinite(q[0] + q[1] + q[2] + q[3] + q[4] + q[5]);
+        }
+        if (finite && !prob) {
+          const double* q0 = J.cd + (size_t)(o + idx[0]) * R2_CD;
+          const double* q1 = J.cd + (size_t)(o + idx[1]) * R2_CD;
+          double R[9];
+          if (r2_rotation(q0, q0 + 3, q1, q1 + 3, R)) {
+            for (int e = 0; e < 9; ++e) Mo[e] = R[e];
+            for (int e = 9; e < 12; ++e) Mo[e] = 0.0;
+            ok = 1;
+          }
+        } else if (finite) {
+          double a[5][3], b[5][3];
+          for (int i = 0; i < 5; ++i) {
+            const double* q = J.cd + (size_t)(o + idx[i]) * R2_CD;
+            for (int r = 0; r < 3; ++r) { a[i][r] = q[r]; b[i][r] = q[3 + r]; }
+          }
+          const double* q6 = J.cd + (size_t)(o + idx[5]) * R2_CD;
+          double best = INFINITY;
+          r2_fivept(a, b, [&](const double* R, const double* t) {
+            const double sc = r2_score_rel(R, t, q6);
+            if (sc < best) {
+              best = sc;
+              for (int e = 0; e < 9; ++e) Mo[e] = R[e];
+              for (int e = 0; e < 3; ++e) Mo[9 + e] = t[e];
+            }
+          });
+          ok = best < INFINITY ? 1 : 0;
+        }
+      }
+    }
+    s_ok[task] = (unsigned char)ok;
+  }
+  __syncthreads();
+  // inliers of every hypothesis, a warp each
+  const int lane = tid & 31, warp = tid >> 5;
+  for (int task = warp; task < n_tasks; task += RS_T / 32) {
+    const int cam = task / (2 * H), prob = (task / H) & 1;
+    const int o = s_off[cam], nc = s_off[cam + 1] - o;
+    int cnt = 0;
+    if (s_ok[task]) {
+      const double* Mo = J.model + (size_t)task * 12;
+      for (int k = lane; k < nc; k += 32) {
+        const double* cd = J.cd + (size_t)(o + k) * R2_CD;
+        cnt += (prob ? r2_score_rel(Mo, Mo + 9, cd) : r2_score_rot(Mo, cd)) < J.threshold ? 1 : 0;
+      }
+    }
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    if (lane == 0) s_cnt[task] = cnt;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    for (int task = 0; task < n_tasks; ++task) J.hyp[task] = s_cnt[task];
+    okb_ransac2d_result res;
+    memset(&res, 0, sizeof res);
+    bool rot_success = false, rel_success = false;
+    int total = 0;
+    XfQ T_WSA, T_SCA, T_WS0, T_SC0;
+    const double* Pa = W.pose + 7 * (size_t)J.pose_a;
+    const double* Pb = W.pose + 7 * (size_t)J.pose_b;
+    xfq_make(Pa, Pa + 3, T_WSA);
+    xfq_make(Pb, Pb + 3, T_WS0);
+    for (int cam = 0; cam < J.n_cams; ++cam) {
+      okb_ransac2d_cam cr;
+      memset(&cr, 0, sizeof cr);
+      cr.n_correspondences = s_off[cam + 1] - s_off[cam];
+      cr.rot_best = cr.rel_best = -1;
+      for (int k = 0; k < 9; k += 4) cr.R_rot[k] = cr.R_rel[k] = 1.0;
+      s_pick[cam] = -1;
+      if (cr.n_correspondences >= 10) {             // Frontend.cpp:670-671
+        int best[2] = {-1, -1}, bc[2] = {-1, -1};
+        for (int prob = 0; prob < 2; ++prob)
+          for (int h = 0; h < H; ++h) {
+            const int task = (2 * cam + prob) * H + h;
+            if (s_ok[task] && s_cnt[task] > bc[prob]) { best[prob] = h; bc[prob] = s_cnt[task]; }
+          }
+        cr.rot_best = best[0]; cr.rel_best = best[1];
+        cr.rot_inliers = best[0] >= 0 ? bc[0] : 0;
+        cr.rel_inliers = best[1] >= 0 ? bc[1] : 0;
+        if (best[0] >= 0) {
+          const double* Mo = J.model + (size_t)((2 * cam) * H + best[0]) * 12;
+          for (int k = 0; k < 9; ++k) cr.R_rot[k] = Mo[k];
+        }
+        if (best[1] >= 0) {
+          const double* Mo = J.model + (size_t)((2 * cam + 1) * H + best[1]) * 12;
+          for (int k = 0; k < 9; ++k) cr.R_rel[k] = Mo[k];
+          for (int k = 0; k < 3; ++k) cr.t_rel[k] = Mo[9 + k];
+        }
+        // Frontend.cpp:709-733
+        const float rot_ratio = float(cr.rot_inliers) / float(cr.n_correspondences);
+        const float rel_ratio = float(cr.rel_inliers) / float(cr.n_correspondences);
+        if (rot_ratio > rel_ratio || rot_ratio > 0.8f) {
+          if (cr.rot_inliers > 10) rot_success = true;
+          res.rotation_only = 1;
+          cr.rotation_only = 1;
+          total += cr.rot_inliers;
+        } else {
+          if (cr.rel_inliers > 10) rel_success = true;
+          total += cr.rel_inliers;
+        }
+        if (rot_success || rel_success) {
+          cr.applied = 1;
+          const int prob = cr.rotation_only ? 0 : 1;
+          const int b = prob ? best[1] : best[0];
+          s_pick[cam] = b >= 0 ? (2 * cam + prob) * H + b : -2;      // -2: no model, every correspondence an outlier
+          if (J.init_pose) {                        // Frontend.cpp:756-798
+            const double* E = W.ext + 7 * (size_t)cam;
+            xfq_make(E, E + 3, T_SCA);
+            xfq_make(E, E + 3, T_SC0);
+            double Rm[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, tm[3] = {0, 0, 0};
+            if (rel_success) {
+              if (cr.rel_best >= 0) {
+                for (int k = 0; k < 9; ++k) Rm[k] = cr.R_rel[k];
+                XfQ a, b2, c2, d, prior;
+                xfq_inv(T_SCA, a);
+                xfq_inv(T_WSA, b2);
+                xfq_mul(a, b2, c2);
+                xfq_mul(c2, T_WS0, d);
+                xfq_mul(d, T_SC0, prior);
+                const double s = fmax(0.0, cr.t_rel[0] * prior.r[0] + cr.t_rel[1] * prior.r[1] + cr.t_rel[2] * prior.r[2]);
+                for (int k = 0; k < 3; ++k) tm[k] = cr.t_rel[k] * s;
+              }
+            } else if (cr.rot_best >= 0) {
+              for (int k = 0; k < 9; ++k) Rm[k] = cr.R_rot[k];
+            }
+            double qm[4];
+            rs_quat(Rm, qm);
+            XfQ T12, a, b2, c2, inv0;
+            xfq_make(tm, qm, T12);
+            xfq_mul(T_WSA, T_SCA, a);
+            xfq_mul(a, T12, b2);
+            xfq_inv(T_SC0, inv0);
+            xfq_mul(b2, inv0, c2);
+            T_WS0 = c2;
+            res.pose_set = 1;
+          }
+        }
+      }
+      J.cams[cam] = cr;
+    }
+    if (rot_success || rel_success) res.ret = total;
+    else { res.ret = -1; res.rotation_only = 1; }                   // Frontend.cpp:802-808
+    if (res.pose_set) {
+      for (int k = 0; k < 3; ++k) res.T_WS[k] = T_WS0.r[k];
+      for (int k = 0; k < 4; ++k) res.T_WS[3 + k] = T_WS0.q[k];
+    }
+    *J.res = res;
+  }
+  __syncthreads();
+  // the outlier records of the applied cameras (Frontend.cpp:735-753, with the B keypoint of the correspondence)
+  int n_out = 0;
+  for (int cam = 0; cam < J.n_cams; ++cam) {
+    const int pick = s_pick[cam];
+    if (pick == -1) continue;
+    const int o = s_off[cam], nc = s_off[cam + 1] - o;
+    const bool rel = pick >= 0 && ((pick / H) & 1);
+    const double* Mo = J.model + (size_t)max(pick, 0) * 12;
+    int cam_out = 0;
+    for (int k0 = 0; k0 < nc; k0 += RS_T) {
+      const int k = k0 + tid;
+      int bad = 0;
+      if (k < nc) {
+        const double* cd = J.cd + (size_t)(o + k) * R2_CD;
+        bad = pick >= 0 && (rel ? r2_score_rel(Mo, Mo + 9, cd) : r2_score_rot(Mo, cd)) < J.threshold ? 0 : 1;
+      }
+      int total;
+      const int pos = block_scan<RS_T>(bad, s_warp, &total);
+      if (bad) {
+        const int* cr = J.ci + 3 * (size_t)(o + k);
+        J.outl[n_out + pos] = okb_ransac2d_outlier{cam, cr[0], cr[1], cr[2]};
+      }
+      n_out += total;
+      cam_out += total;
+    }
+    if (tid == 0) J.cams[cam].n_outliers = cam_out;
+  }
+  if (tid == 0) J.res->n_outliers = n_out;
+}
+}  // namespace
+
+// Host checks of one job; "" = valid.  *n_kp_a: frame A's keypoints in the job's cameras.
+static std::string ransac2d_job_invalid(okb_ctx* c, const okb_ransac2d_job& j, std::vector<char>& seen, size_t* n_kp_a) {
+  const std::string why = store_window_invalid(c, j.win, seen);
+  if (!why.empty()) return why;
+  const WinStore& S = c->wins[j.win];
+  const WinDev& W = c->host[j.win];
+  const FeatStore& F = S.feat;
+  if (j.feat_slot_a < 0 || j.feat_slot_a >= F.F || j.feat_slot_b < 0 || j.feat_slot_b >= F.F) return "feat_slot_a / feat_slot_b out of range";
+  if (j.pose_a < 0 || j.pose_a >= W.K || j.pose_b < 0 || j.pose_b >= W.K) return "pose_a / pose_b out of range";
+  if (j.n_cams < 1 || j.n_cams > F.C || j.n_cams > W.NE || j.n_cams > W.NC || j.n_cams > RS_MAX_CAMS)
+    return "n_cams out of range (1..the store's cameras, the window's extrinsics and cameras, 16)";
+  size_t n_kp = 0;
+  for (int cam = 0; cam < j.n_cams; ++cam) {
+    const int na = S.feat_n_pending[(size_t)j.feat_slot_a * F.C + cam], nb = S.feat_n_pending[(size_t)j.feat_slot_b * F.C + cam];
+    if (na < 0 || nb < 0) return "feature slot has no keypoints for camera " + std::to_string(cam);
+    n_kp += na;
+  }
+  if (j.max_iterations < 1 || j.max_iterations > RS_MAX_HYP) return "max_iterations out of range (1..64)";
+  if (!(j.threshold > 0.0) || !std::isfinite(j.threshold)) return "threshold not finite and positive";
+  if (!j.out) return "out missing";
+  if ((size_t)std::max(j.outlier_cap, 0) < n_kp || (n_kp && !j.outliers)) return "outlier capacity below frame A's keypoints";
+  *n_kp_a = n_kp;
+  return "";
+}
+
+extern "C" int okb_ransac_2d2d_batch(okb_ctx* c, int n_jobs, const okb_ransac2d_job* jobs) {
+  const char* fn = "okb_ransac_2d2d_batch";
+  std::vector<size_t> n_kp(std::max(n_jobs, 0), 0);
+  int rc = store_call_checks(c, fn, n_jobs, jobs, INT_MAX,
+                             [&](int i, std::vector<char>& seen) { return ransac2d_job_invalid(c, jobs[i], seen, &n_kp[i]); });
+  if (rc || n_jobs == 0) return rc;
+  cudaSetDevice(c->device);
+  okb_frontend_state* F = fe(c);
+  CallBuffers& B = F->ransac2d;
+  std::lock_guard<std::mutex> lk(B.mtx);
+  if ((rc = commit_job_windows(c, jobs, n_jobs))) return rc;
+  if ((rc = shard_lm_exchange(c, fn, jobs, n_jobs, c->stream_xfer))) return rc;
+  cudaStream_t xs = c->stream_xfer;
+  // staging (pinned + device mirror): in  = [job table]
+  //                                   out = [per job: result | cameras | hypothesis inliers | outlier records]
+  // scratch (device only), per job: first keypoint per landmark slot | correspondences | their indices | models
+  Carve st, sc;
+  st.take(sizeof(Ransac2JobDev) * (size_t)n_jobs, 256);
+  const size_t in_bytes = st.off;
+  std::vector<size_t> o_res(n_jobs), o_cam(n_jobs), o_hyp(n_jobs), o_out(n_jobs), o_first(n_jobs), o_cd(n_jobs), o_ci(n_jobs), o_mod(n_jobs);
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_ransac2d_job& j = jobs[i];
+    const size_t tasks = (size_t)j.n_cams * 2 * j.max_iterations;
+    o_res[i] = st.take(sizeof(okb_ransac2d_result));
+    o_cam[i] = st.take(sizeof(okb_ransac2d_cam) * (size_t)j.n_cams);
+    o_hyp[i] = st.take(4 * tasks);
+    o_out[i] = st.take(sizeof(okb_ransac2d_outlier) * n_kp[i]);
+    o_first[i] = sc.take(4 * (size_t)lm_slots_host(c, j.win));
+    o_cd[i] = sc.take(8 * R2_CD * n_kp[i]);
+    o_ci[i] = sc.take(12 * n_kp[i]);
+    o_mod[i] = sc.take(8 * 12 * tasks);
+  }
+  const size_t out_end = st.off;
+  if ((rc = B.reserve(c, out_end, sc.off))) return rc;
+  uint8_t* h = B.h_stage;
+  uint8_t* d = B.d_stage;
+  Ransac2JobDev* tj = reinterpret_cast<Ransac2JobDev*>(h);
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_ransac2d_job& j = jobs[i];
+    Ransac2JobDev J;
+    std::memset(&J, 0, sizeof J);
+    J.W = c->d_wins + j.win;
+    J.feat_a = j.feat_slot_a; J.feat_b = j.feat_slot_b; J.pose_a = j.pose_a; J.pose_b = j.pose_b;
+    J.n_cams = j.n_cams; J.n_hyp = j.max_iterations; J.init_pose = j.initialize_pose ? 1 : 0;
+    J.L = lm_slots_host(c, j.win);
+    J.threshold = j.threshold;
+    J.seed = (unsigned long long)j.seed;
+    J.first = reinterpret_cast<int*>(B.d_scratch + o_first[i]);
+    J.cd = reinterpret_cast<double*>(B.d_scratch + o_cd[i]);
+    J.ci = reinterpret_cast<int*>(B.d_scratch + o_ci[i]);
+    J.model = reinterpret_cast<double*>(B.d_scratch + o_mod[i]);
+    J.res = reinterpret_cast<okb_ransac2d_result*>(d + o_res[i]);
+    J.cams = reinterpret_cast<okb_ransac2d_cam*>(d + o_cam[i]);
+    J.hyp = reinterpret_cast<int*>(d + o_hyp[i]);
+    J.outl = reinterpret_cast<okb_ransac2d_outlier*>(d + o_out[i]);
+    tj[i] = J;
+  }
+  OKB_CUDA(c, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, xs));
+  k_ransac_2d2d<<<n_jobs, RS_T, 0, xs>>>(reinterpret_cast<const Ransac2JobDev*>(d));
+  F->launches += 1;
+  OKB_CUDA(c, cudaGetLastError());
+  OKB_CUDA(c, cudaMemcpyAsync(h + in_bytes, d + in_bytes, out_end - in_bytes, cudaMemcpyDeviceToHost, xs));
+  OKB_CUDA(c, cudaStreamSynchronize(xs));
+  for (int i = 0; i < n_jobs; ++i) {
+    const okb_ransac2d_job& j = jobs[i];
+    *j.out = *reinterpret_cast<const okb_ransac2d_result*>(h + o_res[i]);
+    if (j.cams) std::memcpy(j.cams, h + o_cam[i], sizeof(okb_ransac2d_cam) * (size_t)j.n_cams);
+    if (j.hyp_inliers) std::memcpy(j.hyp_inliers, h + o_hyp[i], 4 * (size_t)j.n_cams * 2 * j.max_iterations);
+    if (j.out->n_outliers) std::memcpy(j.outliers, h + o_out[i], sizeof(okb_ransac2d_outlier) * (size_t)j.out->n_outliers);
   }
   return OKB_OK;
 }
